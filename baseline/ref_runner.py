@@ -1,8 +1,8 @@
 """CPU arm of bench.py: times the UNMODIFIED reference (zengxianyu/sketchedit) on the host cores.
 
 Runs in its own process because the reference's top-level packages are called ``models`` / ``util`` like this
-repo's mirrors: here ``baseline/_ref`` (a verbatim, git-ignored copy of the reference's ``models/`` and ``util/``
-python files made by ``__graft_entry__.build()`` from /root/reference; it ships to the GPU box with the snapshot)
+repo's mirrors: here ``oracle/_ref`` (a verbatim, git-ignored copy of the reference's ``models/`` and ``util/``
+python files staged by ``__graft_entry__.build()``, oracle/stage_reference.py)
 comes first on sys.path. The model is the reference's own ``EditLine2Model`` built the way
 ``oracle/make_golden.py`` builds it (``isSkip`` escape hatch, reference models/editline2_model.py:195, then a strict
 ``load_state_dict`` of the seeded synthetic checkpoints) and the timed call is the reference's public entry point
@@ -22,7 +22,7 @@ import time
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = os.path.join(HERE, "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 def main():
@@ -35,7 +35,7 @@ def main():
     ap.add_argument("--face", action="store_true")
     args = ap.parse_args()
     if not os.path.isfile(os.path.join(REF, "models", "editline2_model.py")):
-        print(json.dumps({"ok": False, "why": "baseline/_ref is empty (run __graft_entry__.build() where /root/reference exists)"}))
+        print(json.dumps({"ok": False, "why": "oracle/_ref is empty (run __graft_entry__.build() where the reference is checked out)"}))
         return
     sys.path.insert(0, REF)
     sys.path.append(ROOT)            # only for sketchedit_b200.synth (seeded checkpoints / inputs); `models` resolves to _ref
@@ -97,7 +97,10 @@ def main():
         for _ in range(3):
             comp, _ = fwd(fimg, fsk)
         out["face_b1_s"] = (time.perf_counter() - t0) / 3
-        out["face_b1_max_abs_vs_golden"] = float((comp - torch.from_numpy(z["composed"])).abs().max())
+        ref = torch.from_numpy(z["composed"])
+        if "composed@idx" in z.files:   # the golden stores a fixed sample of positions (oracle/make_golden.py shrink)
+            comp = comp.reshape(-1)[torch.from_numpy(z["composed@idx"].astype(np.int64))]
+        out["face_b1_max_abs_vs_golden"] = float((comp - ref).abs().max())
     print(json.dumps(out))
 
 

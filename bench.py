@@ -1,23 +1,26 @@
-"""Benchmark of the SketchEdit generator forward pass (BASELINE.json metric: images/sec, 256x256
+"""Benchmark of the SketchEdit generator forward pass (metric: images/sec, 256x256
 CelebA-HQ-shaped inputs, synthetic seeded weights of the real architecture).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dtype bf16|fp32] [--batch B] [--size S]
+                    [--dump-outputs DIR]
 
 One "step" = one forward of `model(data, mode='inference')` (netM + threshold + netG incl. contextual
-attention + blend) over one batch. Default workload = BASELINE.json configs[2]: 256x256, batch 128 per GPU, bf16
-tensor-core path (== the per-GPU shard of configs[4], 1024 images over 8 GPUs; weak scaling). `--dtype fp32
---batch 32` runs configs[1] (fp32 parity path); `--size 512 --batch 16` runs configs[3] (Places-size inputs,
+attention + blend) over one batch. Default workload: 256x256, batch 128 per GPU, bf16
+tensor-core path (weak scaling over GPUs). `--dtype fp32
+--batch 32` runs the fp32 parity path; `--size 512 --batch 16` runs Places-size inputs (with
 contextual attention over L = 3969 patches).
 
 Prints ONE JSON line (rank 0):
   value     whole-job throughput, inputs resident in HBM, NO instrumentation inside the timed region
   e2e       same metric through the reference-facing module API with pinned host tensors in and host tensors out
             (N > 1: including the NCCL all-gather of the outputs)
-  roofline  from ONE separate instrumented pass (CUDA events around every launch, se_timing_enable): all tcgen05
+  roofline  from ONE separate instrumented pass (CUDA events around every launch, se_timing_enable): all tensor-core
             launches together, the dominant kernel class, and the per-class table with each class's own bound
   latency   batch-1 forward latency at 256x256 and 512x512 (N = 1, default workload only)
-`--impl reference` times the UNMODIFIED reference (baseline/_ref, staged by __graft_entry__.build()) on the host cores
+`--impl reference` times the UNMODIFIED reference (oracle/_ref, staged by __graft_entry__.build()) on the host cores
 through baseline/ref_runner.py; if it was never staged, the CPU oracle port (kind "port").
+`--dump-outputs DIR` writes what the timed path returned in its last timed step (composed image, mask) as DIR/<name>.npy,
+float32, for a fixed seeded sample of the batch's images (at most 64 MB in all), so two builds can be compared output for output.
 """
 import argparse
 import ctypes
@@ -108,12 +111,13 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s; not reached, a card may be power-limited
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet"
 
 
 # ------------------------------------------------------------------------------------------------ CPU arm
 def cpu_reference(size, n_img, steps, warm, face=False, threads=0):
-    """The UNMODIFIED reference on the host cores (baseline/_ref through baseline/ref_runner.py, own process: its
+    """The UNMODIFIED reference on the host cores (oracle/_ref through baseline/ref_runner.py, own process: its
     packages are called `models` / `util` like this repo's). Returns the runner's dict or None if it was never staged."""
     cmd = [sys.executable, os.path.join(ROOT, "baseline", "ref_runner.py"), "--size", str(size), "--batch", str(n_img), "--steps", str(steps),
            "--warmup", str(warm), "--threads", str(threads)] + (["--face"] if face else [])
@@ -126,7 +130,7 @@ def cpu_reference(size, n_img, steps, warm, face=False, threads=0):
 
 
 def cpu_port(size, n_img, steps, warm):
-    """Fallback: the CPU oracle port of the reference path (oracle/), when baseline/_ref is absent."""
+    """Fallback: the CPU oracle port of the reference path (oracle/), when oracle/_ref is absent."""
     from oracle import sketchedit_oracle as O
     from sketchedit_b200 import synth
     WM, WG = synth.synth_state_dict("M"), synth.synth_state_dict("G")
@@ -156,8 +160,8 @@ def cpu_arm(size, n_img, steps, warm, face=False):
 
 
 def cpu_baseline_entry(d):
-    what = ("the UNMODIFIED reference EditLine2Model (baseline/_ref), model(data, mode='inference')" if d["kind"] == "reference"
-            else "torch CPU fp32 oracle port of the reference forward (baseline/_ref not staged)")
+    what = ("the UNMODIFIED reference EditLine2Model (oracle/_ref), model(data, mode='inference')" if d["kind"] == "reference"
+            else "torch CPU fp32 oracle port of the reference forward (oracle/_ref not staged)")
     e = {"value": d["images_per_s"], "unit": UNIT, "cores": d["threads"], "kind": d["kind"],
          "sample": "%s: batch %d of the workload at %dx%d, fp32, %d intra-op threads (fastest of a calibration over 8..%d host cores)" % (
              what, d["batch"], d["size"], d["size"], d["threads"], d["cores"])}
@@ -213,9 +217,9 @@ def roofline_from_classes(classes, steps, peaks, src, step_ms):
         t_sum += ms
         rows.append({"class": c["name"], "launches_per_step": c["launches"] / steps, "us_per_step": ms * 1e3, "bound": bound,
                      "tflops_alg": fa / ms / 1e9, "tflops_exec": fe / ms / 1e9, "gbs_alg": by / ms / 1e6, "frac": ideal / ms,
-                     "tcgen05": bool(c["tensor"])})
+                     "tensor": bool(c["tensor"])})
     rows.sort(key=lambda r: -r["us_per_step"])
-    tc = [r for r in rows if r["tcgen05"]]
+    tc = [r for r in rows if r["tensor"]]
     tc_ms = sum(r["us_per_step"] for r in tc) / 1e3
     tc_fa = sum(r["tflops_alg"] * r["us_per_step"] for r in tc) / 1e3      # TFLOP/s * ms = GFLOP... keep consistent below
     tc_fe = sum(r["tflops_exec"] * r["us_per_step"] for r in tc) / 1e3
@@ -223,7 +227,7 @@ def roofline_from_classes(classes, steps, peaks, src, step_ms):
     ach_exec = tc_fe / tc_ms if tc_ms else 0.0
     dom = tc[0] if tc else None
     roof = {
-        "bound": "tensor", "kernel": "all tcgen05 launches (conv_c8_kernel classes: gated convs; cam_s / cam_pv or gemm_split: attention GEMMs)",
+        "bound": "tensor", "kernel": "all wgmma launches (conv_c8_kernel classes: gated convs; cam_s / cam_pv or gemm_split: attention GEMMs)",
         "achieved": ach_alg, "achieved_executed": ach_exec, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach_alg / peak_tf,
         "frac_executed": ach_exec / peak_tf,
         "flops_convention": "achieved = ALGORITHMIC 2*MAC of the reference ops the forward executes (SURVEY.md 8d; mode='inference' skips the dead netM "
@@ -233,24 +237,12 @@ def roofline_from_classes(classes, steps, peaks, src, step_ms):
         "per_layer_roofline_frac": t_ideal_sum / t_sum if t_sum else None,
         "per_layer_note": "sum over ALL launches of max(alg FLOPs / sustained bf16 peak, alg bytes / measured HBM GB/s) divided by the summed measured "
                           "launch time (north_star's 'per-layer tensor-core/HBM roofline')",
-        "traffic": None,
         "dominant": dom and {k: dom[k] for k in ("class", "launches_per_step", "us_per_step", "tflops_alg", "frac")},
         "per_class": [[r["class"], round(r["launches_per_step"], 2), round(r["us_per_step"], 1), r["bound"],
                        round(r["tflops_alg"], 1) if r["bound"] == "tensor" else round(r["gbs_alg"], 1), round(r["frac"], 3)] for r in rows],
         "per_class_columns": ["class", "launches/step", "us/step", "bound", "TFLOP/s (tensor) or GB/s (hbm), algorithmic", "frac of its bound"],
     }
     return roof, rows
-
-
-def load_traffic(workload_key):
-    """DRAM bytes per launch of the dominant kernel from the committed ncu capture of this workload (profiles/), or None."""
-    p = os.path.join(ROOT, "profiles", "dram_traffic.json")
-    if not os.path.exists(p):
-        return None, None
-    with open(p) as f:
-        d = json.load(f)
-    e = d.get(workload_key)
-    return (e["bytes_per_launch"], e["note"]) if e else (None, None)
 
 
 def write_class_table(path, rows, header):
@@ -262,6 +254,22 @@ def write_class_table(path, rows, header):
 
 
 # ------------------------------------------------------------------------------------------------ GPU arm
+DUMP_BYTES = 64_000_000 - 4096   # 64 MB in all, .npy headers included
+DUMP_SEED = 0
+
+
+def dump_outputs(out_dir, outs):
+    """outs: name -> [B, ...] device tensors of one step. Writes out_dir/<name>.npy (float32) for the same fixed, seeded
+    sample of images for every output (all of them when they fit DUMP_BYTES), in batch order."""
+    import numpy as np
+    B = next(iter(outs.values())).shape[0]
+    per_image = sum(t[0].numel() * 4 for t in outs.values())
+    k = max(1, min(B, DUMP_BYTES // per_image))
+    idx = torch.randperm(B, generator=torch.Generator().manual_seed(DUMP_SEED))[:k].sort().values
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in outs.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach()[idx.to(t.device)].float().cpu().numpy())
+
 def run_b200(args):
     import torch.distributed as dist
     from argparse import Namespace
@@ -278,6 +286,7 @@ def run_b200(args):
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     assert world == args.gpus, "launch with torchrun --nproc-per-node %d (WORLD_SIZE=%d)" % (args.gpus, world)
+    assert not args.dump_outputs or world == 1, "--dump-outputs runs on one GPU (--gpus 1)"
     B, H, W = args.batch, args.size, args.size
     prec = args.dtype
 
@@ -303,8 +312,8 @@ def run_b200(args):
             slot = gather.next_slot()            # step i runs on NCCL's stream while step i+1 computes
             eng.inference_packed(img_d, sk_d, precision=prec, out=slot)
             gather.launch()
-        else:
-            eng.inference(img_d, sk_d, precision=prec)
+            return None
+        return eng.inference(img_d, sk_d, precision=prec)
 
     def barrier():
         if gather is not None:
@@ -325,8 +334,9 @@ def run_b200(args):
     barrier()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
+    last = None
     for _ in range(args.steps):
-        step_device()
+        last = step_device()
     if gather is not None:
         gather.wait()               # the last step's collective belongs to the region
     e1.record()
@@ -337,6 +347,8 @@ def run_b200(args):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms = float(t.item())
     value = world * B * args.steps / (ms / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"composed": last[0], "mask": last[1]})
 
     # ---------------- e2e: reference-facing module API, pinned host tensors in, host tensors out
     comp_h = torch.empty(B, 3, H, W).pin_memory()
@@ -401,10 +413,6 @@ def run_b200(args):
         lib.se_timing_enable(0)
         peaks, src = measured_peaks()
         roof, rows = roofline_from_classes(classes, n_inst, peaks, src, ms / args.steps)
-        wkey = "%s_b%d_%d" % (prec, B, args.size)
-        roof["traffic"], tnote = load_traffic(wkey)
-        if tnote:
-            roof["traffic_note"] = tnote
         if args.classes_out:
             write_class_table(args.classes_out, rows, "# per-kernel-class roofline, %s (one instrumented pass of %d steps, CUDA events per launch)" % (
                 workload_name(prec, B, world, args.size), n_inst))
@@ -436,7 +444,7 @@ def run_b200(args):
             "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": prec, "data": "synthetic",
             "config": {"workload": workload_name(prec, B, world, args.size), "global_batch": world * B, "H": H, "W": W,
-                       "l2": "inputs + per-step activations (%.1f GB workspace) far exceed the 126 MB L2; no explicit flush" % (eng.workspace_bytes() / 1e9),
+                       "l2": "inputs + per-step activations (%.1f GB workspace) far exceed the 50 MB L2; no explicit flush" % (eng.workspace_bytes() / 1e9),
                        "parallelism": "dp%d (batch shards; one NCCL all-gather of the packed outputs per step, overlapped with the next step)" % world if world > 1 else "single GPU",
                        "algorithmic_gflop_per_image_reference": alg,
                        "algorithmic_gflop_per_image_executed_layers": alg - dead_flops_per_image(H, W) / 1e9,
@@ -476,6 +484,8 @@ def main():
     ap.add_argument("--size", type=int, default=256, help="H = W of the synthetic inputs (256: CelebA-HQ configs, 512: Places config)")
     ap.add_argument("--classes-out", default=None, help="write the per-kernel-class roofline table (markdown) here")
     ap.add_argument("--no-latency", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's outputs as DIR/<name>.npy (float32, <= 64 MB, fixed seeded image sample)")
     args = ap.parse_args()
     if args.batch is None:
         args.batch = 16 if args.size >= 512 else (128 if args.dtype == "bf16" else 32)

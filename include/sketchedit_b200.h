@@ -1,5 +1,5 @@
 /*
- * sketchedit_b200 -- C ABI of the B200-native SketchEdit generator forward pass.
+ * sketchedit_b200 -- C ABI of the H100-native SketchEdit generator forward pass.
  *
  * The reference (zengxianyu/sketchedit) has no FFI / plugin layer: its boundary for this path is the
  * Python nn.Module surface. These entry points are what a binding for that surface calls; each one
@@ -8,7 +8,7 @@
  * torch types cross the boundary. Every function returns 0 on success; on failure it returns non-zero
  * and se_last_error() describes why. `stream` is a cudaStream_t (pass torch's current stream).
  *
- * Kernels are sm_100a only; there is no CPU fallback.
+ * Kernels are sm_90a only; there is no CPU fallback.
  */
 #ifndef SKETCHEDIT_B200_H
 #define SKETCHEDIT_B200_H
@@ -21,11 +21,11 @@ typedef struct se_model se_model;
 
 /* arithmetic / storage mode of a forward call */
 enum {
-  SE_PREC_BF16_TC = 0,     /* bf16 activations + weights, tcgen05 tensor-core kernels, fp32 accumulation */
+  SE_PREC_BF16_TC = 0,     /* bf16 activations + weights, wgmma tensor-core kernels, fp32 accumulation */
   SE_PREC_FP32_EXACT = 1,  /* fp32 activations + weights, CUDA-core fp32 FMA kernels (fp32 parity config) */
-  SE_PREC_BF16_DIRECT = 2, /* bf16 activations, CUDA-core kernels (cross-check of the tcgen05 path) */
+  SE_PREC_BF16_DIRECT = 2, /* bf16 activations, CUDA-core kernels (cross-check of the tensor-core path) */
   SE_PREC_FP32_TC = 3      /* fp32-parity arithmetic ON the tensor cores: activations and weights as fp16 hi + fp16 lo pairs (22
-                              significant bits), three tcgen05 products per tap (hi*hi + hi*lo + lo*hi), fp32 accumulation and exact-math
+                              significant bits), three wgmma products per tap (hi*hi + hi*lo + lo*hi), fp32 accumulation and exact-math
                               epilogue. The fp32 parity config (1e-3) runs here; SE_PREC_FP32_EXACT stays as its cross-check. */
 };
 

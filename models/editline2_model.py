@@ -3,7 +3,7 @@
 ``forward(data, mode)`` with mode 'inference' returns ``(composed_image, mask)`` exactly like the
 reference: netM predicts the edit mask from (image, sketch), the mask is binarised at 0.5, netG inpaints,
 and the result is blended with the SOFT mask. All of it is one C-ABI call (``se_forward_inference``) on the
-B200 kernels; tensors in ``data`` may live on the CPU (they are copied to the GPU like the reference's
+CUDA kernels; tensors in ``data`` may live on the CPU (they are copied to the GPU like the reference's
 ``preprocess_input`` does) and the outputs are CUDA tensors. Training modes are out of scope."""
 import torch
 
@@ -16,7 +16,7 @@ class EditLine2Model(torch.nn.Module):
     def modify_commandline_options(parser, is_train):
         networks.modify_commandline_options(parser, is_train)
         parser.add_argument("--precision", default="bf16", choices=("bf16", "fp32", "fp32_direct"),
-                            help="B200 arithmetic: bf16 tensor-core path, fp32-parity arithmetic on the tensor cores (split-half fp16), "
+                            help="GPU arithmetic: bf16 tensor-core path, fp32-parity arithmetic on the tensor cores (split-half fp16), "
                                  "or its fp32 CUDA-core cross-check")
         return parser
 
@@ -24,7 +24,7 @@ class EditLine2Model(torch.nn.Module):
         super().__init__()
         self.opt = opt
         if getattr(opt, "isTrain", False):
-            raise NotImplementedError("only the inference path is implemented on B200")
+            raise NotImplementedError("only the inference path is implemented on the GPU")
         self.precision = getattr(opt, "precision", "bf16")
         self.netM, self.netG, self.netD = self.initialize_networks(opt)
         self._engine = None

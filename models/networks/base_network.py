@@ -1,11 +1,11 @@
 """BaseNetwork (reference models/networks/base_network.py:5-57) plus the glue that binds a
-generator module to its packed B200 engine."""
+generator module to its packed CUDA engine."""
 import torch.nn as nn
 from torch.nn import init
 
 
 class BaseNetwork(nn.Module):
-    NET_ID = None   # 'M' or 'G' for the generators on the B200 path
+    NET_ID = None   # 'M' or 'G' for the generators on the CUDA path
 
     def __init__(self):
         super().__init__()
@@ -50,7 +50,7 @@ class BaseNetwork(nn.Module):
                     init.constant_(m.bias.data, 0.0)
         self.apply(visit)
 
-    # ------------------------------------------------------------------ B200 engine binding
+    # ------------------------------------------------------------------ CUDA engine binding
     def _weights_key(self):
         return tuple((p.data_ptr(), p._version) for p in self.parameters())
 

@@ -1,5 +1,5 @@
 """Contextual attention modules with the reference's two-module surface
-(reference models/networks/splitcam.py:17-174). On the B200 path similarity, masking, softmax and the
+(reference models/networks/splitcam.py:17-174). On the GPU path similarity, masking, softmax and the
 fold-sum paste run as ONE fused C-ABI call (``se_contextual_attention_forward``); P1 returns the
 attention weights like the reference and hands the pasted features to P2 through the tensor it returns.
 Only the configuration netG instantiates is implemented (editline_g.py:35-42)."""
@@ -13,7 +13,7 @@ class ReduceContextAttentionP1(nn.Module):
         super().__init__()
         cfg = (bkg_patch_size, stride, ufstride, softmax_scale, nn_hard, pd, is_fuse, th, norm_type, is_th)
         if cfg != (4, 2, 2, 10., False, 0, False, 0.1, 1, True):
-            raise NotImplementedError("B200 contextual attention implements netG's configuration only "
+            raise NotImplementedError("the CUDA contextual attention implements netG's configuration only "
                                       "(patch 4, stride 2, pd 0, scale 10, is_th th=0.1, norm_type 1); got %r" % (cfg,))
         self.precision = "bf16"
 
@@ -35,7 +35,7 @@ class ReduceContextAttentionP2(nn.Module):
     def __init__(self, bkg_patch_size=16, stride=8, ufstride=8, pd=4, mk=True):
         super().__init__()
         if (bkg_patch_size, stride, ufstride, pd, mk) != (4, 2, 2, 0, False):
-            raise NotImplementedError("B200 contextual attention implements netG's paste configuration only")
+            raise NotImplementedError("the CUDA contextual attention implements netG's paste configuration only")
 
     def forward(self, cos_similar, b, mask, dict_aux):
         if dict_aux:

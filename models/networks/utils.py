@@ -1,7 +1,7 @@
 """Gated convolution modules with the reference's constructor signatures and parameter layout
 (reference models/networks/utils.py:9-51). They own the fp32 OIHW ``weight`` / ``bias`` parameters
-(state_dict source of truth); ``forward`` runs the layer on the B200 kernels through the C ABI
-(``se_gated_conv_forward``) -- the tcgen05 implicit-GEMM with the fused bias/ELU x sigmoid epilogue in
+(state_dict source of truth); ``forward`` runs the layer on the CUDA kernels through the C ABI
+(``se_gated_conv_forward``) -- the wgmma implicit-GEMM with the fused bias/ELU x sigmoid epilogue in
 bf16 mode, the fp32 CUDA-core kernel in fp32 mode. No torch compute op is on this path."""
 import torch
 import torch.nn as nn
@@ -17,7 +17,7 @@ class gen_conv(nn.Conv2d):
 
     def _bound(self):
         if self._se_owner is None:
-            raise RuntimeError("this gen_conv is not attached to a MDGenerator / DeepFillC2Generator; the B200 path "
+            raise RuntimeError("this gen_conv is not attached to a MDGenerator / DeepFillC2Generator; the CUDA path "
                                "packs weights per network (there is no stand-alone or CPU fallback)")
         return self._se_owner
 
@@ -27,7 +27,7 @@ class gen_conv(nn.Conv2d):
 
 
 class gen_deconv(gen_conv):
-    """nearest x2 upsample followed by a 3x3 gated conv (reference utils.py:35-51); on the B200 path the
+    """nearest x2 upsample followed by a 3x3 gated conv (reference utils.py:35-51); on the CUDA path the
     upsample is folded into four sub-pixel 2x2 convolutions and never materialised."""
 
     def __init__(self, cin, cout):

@@ -29,7 +29,7 @@ class BaseOptions:
     def initialize(self, parser):
         parser.add_argument("--name", type=str, default="label2coco", help="experiment name = checkpoint sub-directory")
         parser.add_argument("--joint_train_inp", action="store_true", help="zero the sketch channel of the style encoder")
-        parser.add_argument("--gpu_ids", type=str, default="0", help="e.g. 0 or 0,1; the B200 path needs at least one GPU")
+        parser.add_argument("--gpu_ids", type=str, default="0", help="e.g. 0 or 0,1; the GPU path needs at least one GPU")
         parser.add_argument("--checkpoints_dir", type=str, default="./checkpoints")
         parser.add_argument("--model", type=str, default="pix2pix")
         parser.add_argument("--phase", type=str, default="train")

@@ -1,7 +1,6 @@
 """Generate tests/golden/*.npz by running the UNMODIFIED reference  --  TEST INFRASTRUCTURE ONLY.
 
-Run in the build container only (it needs /root/reference, which does not exist on the
-GPU box):
+Run where the unmodified reference is checked out (path in SKETCHEDIT_REFERENCE):
 
     python oracle/make_golden.py
 
@@ -59,6 +58,35 @@ def u8_case(img_u8, edge_u8, keep=()):
     return dict(inputs=(image, sketch), flags={}, u8=(img_u8, edge_u8), keep=keep)
 
 
+MAX_FILE_BYTES = 1_000_000
+SAMPLE_SEED = 2024
+
+
+def shrink(out, n_keep):
+    """Replace every float array with more than `n_keep` elements by a fixed, seeded sample of n_keep of its elements in flat
+    order; the sorted flat positions go to `<key>@idx` (int32). Tests compare on those positions. The inputs and the mask are
+    always kept whole: the binarised-mask checks are exact, over every pixel."""
+    rng = np.random.default_rng(SAMPLE_SEED)
+    for k in sorted(out):
+        v = out[k]
+        if k in ("image", "sketch", "mask") or v.dtype != np.float32 or v.size <= n_keep:
+            continue
+        idx = np.sort(rng.choice(v.size, n_keep, replace=False)).astype(np.int32)
+        out[k] = v.reshape(-1)[idx]
+        out[k + "@idx"] = idx
+    return out
+
+
+def save(path, out):
+    """np.savez_compressed, sampling the large arrays (shrink) until the file is at most MAX_FILE_BYTES."""
+    n_keep = None
+    while True:
+        np.savez_compressed(path, **(shrink(dict(out), n_keep) if n_keep else out))
+        if os.path.getsize(path) <= MAX_FILE_BYTES:
+            return
+        n_keep = max(v.size for k, v in out.items() if k != "mask") // 2 if n_keep is None else n_keep // 2
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=os.path.join(ROOT, "tests", "golden"))
@@ -78,9 +106,9 @@ def main():
                                             flags=dict(no_mask_cc=True, no_mask_coarse=True,
                                                        joint_train_inp=False)),
     }
-    # config 1 of BASELINE.json: a real 256x256 face + sketch from the reference's dataset
+    # a real 256x256 face + sketch from the reference's dataset
     cases["face_602_256x256"] = u8_case(*load_pair("602_images_celeb_00033.png"), keep=("fine", "tap:netM.conv_mask_17"))
-    # config 4 of BASELINE.json (Places-size contextual attention): the reference's non-square general-scene input,
+    # Places-size contextual attention: the reference's non-square general-scene input,
     # 408 wide x 512 high -> attention over L = 63 * 50 = 3150 patches. Only the end-to-end tensors are kept (file size).
     cases["places_11_512x408"] = u8_case(*load_pair("11.png", "general_release"))
     if args.only:
@@ -128,7 +156,7 @@ def main():
             out["image"], out["sketch"] = image.numpy(), sketch.numpy()
         out["flags"] = np.array(repr(sorted(case["flags"].items())))
         path = os.path.join(args.out, name + ".npz")
-        np.savez_compressed(path, **out)
+        save(path, out)
         print("wrote %s  (%.1f KB)  mask-on %.3f" % (path, os.path.getsize(path) / 1024,
                                                       float((mask > 0.5).float().mean())))
 

@@ -18,7 +18,7 @@ weights passed as a ``{name: tensor}`` dict in the reference's state_dict format
 
 Pinning: the reference ships no tests or golden vectors for this path (SURVEY.md section 4)
 and no checkpoints, so the oracle is pinned against OUTPUTS OF THE REFERENCE ITSELF:
-``oracle/make_golden.py`` imports the unmodified reference from /root/reference in the build
+``oracle/make_golden.py`` imports the unmodified reference from the reference checkout (SKETCHEDIT_REFERENCE) where it is
 container, runs it on seeded synthetic checkpoints (``oracle/synth.py``) and commits the
 results under ``tests/golden/``; ``tests/test_oracle_golden.py`` checks this file against
 them (fp32, max-abs <= 2e-5).

@@ -59,7 +59,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise SketchEditB200Error(
-            "%s not found. Build it with `python -m sketchedit_b200.build` (nvcc, sm_100a). "
+            "%s not found. Build it with `python -m sketchedit_b200.build` (nvcc, sm_90a). "
             "There is no CPU or PyTorch fallback for this path." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():

@@ -1,4 +1,4 @@
-"""Build libsketchedit_b200.so in-tree with nvcc for sm_100a (no JIT cache, no torch extension).
+"""Build libsketchedit_b200.so in-tree with nvcc for sm_90a (H100; no JIT cache, no torch extension).
 
     python -m sketchedit_b200.build [--force]
 
@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsketchedit_b200.so")
 SOURCES = ["se_engine.cu", "se_conv_c8.cu", "se_cam.cu", "se_conv_direct.cu", "se_misc.cu", "se_split.cu", "se_gemm_split.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
 
@@ -55,7 +55,7 @@ def build(force=False, verbose=True):
         if verbose and out.strip():
             print(out)
     out_lib = os.environ.get("SE_LIB_OUT", LIB)   # A/B builds go next to the product library, selected with SE_B200_LIB at load time
-    cmd = [nvcc, "-shared", "-o", out_lib] + objs + ["-lcudart"]
+    cmd = [nvcc, "-shared", NVCC_FLAGS[0], NVCC_FLAGS[1], "-o", out_lib] + objs + ["-lcudart"]
     if verbose:
         print(" ".join(cmd), flush=True)
     subprocess.check_call(cmd)

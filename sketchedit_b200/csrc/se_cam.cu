@@ -1,6 +1,6 @@
 // Contextual attention (reference models/networks/splitcam.py:37-108,132-174 with netG's configuration, editline_g.py:35-42:
 // 4x4 patches at stride 2, keys normalised per (image, channel) plane, logits x10, masked keys -> logit 0, soft attention,
-// paste = fold-SUM of the weighted raw patches) on the tcgen05 tensor cores of sm_100a, in three steps:
+// paste = fold-SUM of the weighted raw patches) with wgmma on the tensor cores of sm_90a, in three steps:
 //
 //   prep   rnorm[c] = 1 / sqrt(sum_plane f^2 + 1e-8);  fn = f * rnorm  (same layout as f);  per-key logit scale
 //   S      P[n, l]  = softmax_l(10 * m_l * <Q_n, K_l>)        cam_s_kernel   (QK^T twice: statistics sweep + output sweep)
@@ -9,18 +9,17 @@
 // Nothing is packed or unfolded: the feature map arrives SPACE-TO-DEPTH channel-blocked, [B][4 parities x 12 blocks][h/2][w/2][8]
 // bf16 (written that way by pmconv6's epilogue). A 4x4 / stride-2 patch tap (u, v) of patch n is then pixel n + (u>>1, v>>1) of
 // parity plane (u&1, v&1): a stride-1 window, so ONE TMA box (17 x 9 positions of the planes) holds all 16 taps of a tile of
-// 16 x 8 patches, and eight horizontally adjacent patches x eight channels are one no-swizzle UMMA core matrix (the trick of
+// 16 x 8 patches, and eight horizontally adjacent patches x eight channels are one no-swizzle wgmma core matrix (the trick of
 // se_conv_c8.cu). Queries (A), keys (B, K-major) and values (B, MN-major) are all such boxes; tap / channel selection is
 // descriptor start-address arithmetic.
 //
-// Both GEMM kernels run as CTA PAIRS (cta_group::2, M = 256 = two tiles): every CTA loads the operands of its own tile and HALF
-// of the shared B operand. 640 threads: warp 0 TMA producer, warp 1 MMA issuer (leader CTA), warp 2 TMEM allocator, warps 4-19
-// epilogue (warp % 4 = TMEM lane quadrant, (warp - 4) / 4 = column group).
+// Both GEMM kernels run 288 threads: two consumer warpgroups (wgmma, accumulators in registers, epilogue on the fragments) and a
+// TMA producer warp.
 //
 // Probabilities are the only attention-sized tensor that touches HBM: bf16 P[B][key block][hs][ws][8] ("channel-blocked with
-// keys as channels"), written once by the S kernel and read once (per output tile pair) by the PV kernel. The logits never
-// leave TMEM: the S kernel sweeps the key tiles twice per query tile - sweep 0 keeps the running row maximum and sum (fp32,
-// one TMEM lane = one query row = one thread: no cross-thread reduction), sweep 1 recomputes the logits and writes
+// keys as channels"), written once by the S kernel and read once (per output tile) by the PV kernel. The logits never
+// leave the registers: the S kernel sweeps the key tiles twice per query tile - sweep 0 keeps the running row maximum and sum
+// (fp32, per lane, combined over the row's quad of lanes at the end), sweep 1 recomputes the logits and writes
 // exp(t - max) / sum. Key order inside P is the S kernel's tile order, which is also the order the PV kernel walks the keys.
 #include "se_cam.h"
 
@@ -33,26 +32,29 @@
 namespace se {
 
 constexpr int CAM_CB = 12;                 // channel blocks of the 96-channel map
-constexpr int CAM_TH = 16, CAM_TW = 8;     // query / output tile: 128 positions = UMMA M per CTA
+constexpr int CAM_TH = 16, CAM_TW = 8;     // query tile: 128 positions = two wgmma M = 64 halves
 constexpr int CAM_HR = CAM_TH + 1, CAM_WR = CAM_TW + 1;   // its window in a parity plane (taps reach +1 row / column)
 constexpr int CAM_PLANE = CAM_HR * CAM_WR * 16;           // bytes of one channel block of a 17 x 9 window = LBO of the K-major operands
 constexpr int CAM_ROW = CAM_WR * 16;                      // bytes of one window row = SBO
 constexpr int CAM_Q_TX = 4 * CAM_CB * CAM_PLANE;          // query window, all four parities: 117,504 B
 constexpr int CAM_Q_BYTES = (CAM_Q_TX + 1023) / 1024 * 1024;
-constexpr int CAM_K_TX = CAM_CB * CAM_PLANE;              // key window of one parity (this CTA's 16 x 8 half of a 32 x 8 key tile)
+constexpr int CAM_K_TX = CAM_CB * CAM_PLANE;              // key window of one parity (one 16 x 8 half of a 32 x 8 key tile)
 constexpr int CAM_K_STAGE = (CAM_K_TX + 1023) / 1024 * 1024;
 constexpr int CAM_S_STAGES = 3;
-constexpr int CAM_KEYS = 256;              // keys per S tile (N of the pair MMA)
-// PV: a stage = 64 keys: P window (8 key blocks x 17 x 9) + value windows of two parities (12 blocks x 9 x 9)
-constexpr int CAM_PW_TX = 8 * CAM_PLANE;                  // 19,584 B
+constexpr int CAM_KEYS = 256;              // keys per key tile (two 128-key accumulator tiles)
+// PV: output tile = 8 x 8 positions (wgmma M = 64); a stage = 64 keys: P window (8 key blocks x 9 x 9) + value windows of
+// all four parities (12 blocks x 9 x 9 each)
+constexpr int CAM_PV_TH = 8;
+constexpr int CAM_PPLANE = 9 * 9 * 16;                    // one key block of the 9 x 9 P window = LBO of the K-major A operand
+constexpr int CAM_PW_TX = 8 * CAM_PPLANE;                 // 10,368 B
 constexpr int CAM_VPLANE = 9 * 9 * 16;                    // one channel block of a 9 x 9 value window = SBO of the MN-major operand
 constexpr int CAM_V_TX = CAM_CB * CAM_VPLANE;             // 15,552 B
-constexpr int CAM_V0_OFF = CAM_PW_TX;                     // 128 B aligned
-constexpr int CAM_V1_OFF = (CAM_V0_OFF + CAM_V_TX + 127) / 128 * 128;
-constexpr int CAM_PV_STAGE = (CAM_V1_OFF + CAM_V_TX + 1023) / 1024 * 1024;
-constexpr int CAM_PV_STAGES = 4;
-
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+constexpr int CAM_V_PITCH = (CAM_V_TX + 127) / 128 * 128;
+__host__ __device__ constexpr int CAM_V_OFF(int par) { return CAM_PW_TX + par * CAM_V_PITCH; }   // 128 B aligned
+constexpr int CAM_PV_STAGE = (CAM_V_OFF(4) + 1023) / 1024 * 1024;
+constexpr int CAM_PV_STAGES = 3;
+constexpr int CAM_CONSUMER_WARPS = 8;
+constexpr int CAM_THREADS = 32 * CAM_CONSUMER_WARPS + 32;
 
 // ------------------------------------------------------------------------------------------ prep kernels
 // one block per (channel block, image): sum of squares over the four parity planes in a fixed order (deterministic: the
@@ -140,17 +142,20 @@ __global__ void cam_attn_export_kernel(const __nv_bfloat16* __restrict__ P, floa
 }
 
 // ------------------------------------------------------------------------------------------ S kernel
+// One CTA per query tile (16 x 8 queries, persistent over the tiles of the batch): warps 0-7 = two consumer warpgroups
+// (queries 0-63 / 64-127 of the tile: wgmma M = 64, N = 128 keys = one 16 x 8 half of a 32 x 8 key tile), warp 8 = TMA
+// producer. A query row's logits live in one quad of lanes (accumulator fragment), so the softmax statistics need
+// only two shuffles per row.
 struct CamSParams {
   int hs, ws;
-  int tq_x, tq_n, pairs_per_img, n_pairs;
+  int tq_x, tq_n, n_tiles;
   int tk_x, KT, KB;
   const float* colscale;
   __nv_bfloat16* P;
 };
 
-__global__ void __launch_bounds__(TC_NUM_THREADS, 1)
+__global__ void __launch_bounds__(CAM_THREADS, 1)
 cam_s_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const CamSParams p) {
-  const uint32_t rank = cluster_ctarank();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
@@ -160,343 +165,286 @@ cam_s_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
   uint64_t* q_empty = bars + 1;
   uint64_t* k_full = bars + 2;
   uint64_t* k_empty = k_full + CAM_S_STAGES;
-  uint64_t* tmem_full = k_empty + CAM_S_STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* stat_m = reinterpret_cast<float*>(tmem_ptr_smem + 4);   // [4 column groups][128 rows]
-  float* stat_s = stat_m + 4 * 128;
 
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmQ)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmK)) : "memory");
-  }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
-    mbar_init(q_empty, 1);
-    for (int i = 0; i < CAM_S_STAGES; ++i) { mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 2 * 4 * TC_EPI_GROUPS); }   // one arrive per epilogue warp of both CTAs
+    mbar_init(q_empty, CAM_CONSUMER_WARPS);
+    for (int i = 0; i < CAM_S_STAGES; ++i) { mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], CAM_CONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(TC_TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_ptr_smem, 0);
+  __syncthreads();
+  const int n_kt = 4 * p.KT;   // accumulator tiles per query tile: two sweeps over the key tiles, two 128-key halves each
 
-  const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-  const int n_kt = 2 * p.KT;   // accumulator tiles per query tile pair: two sweeps over the key tiles
-
-  if (warp == 0) {
-    // ==================================================================== producer (both CTAs: own query window, own half of the keys)
+  if (warp == CAM_CONSUMER_WARPS) {
+    // ==================================================================== producer
+    if (lane == 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmQ)) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmK)) : "memory");
+    }
     int stage = 0;
     uint32_t phase = 0, qphase = 0;
-    for (int pr = cluster_id; pr < p.n_pairs; pr += n_clusters) {
-      const int img = pr / p.pairs_per_img, t = (pr - img * p.pairs_per_img) * 2 + (int)rank;
-      const bool real = t < p.tq_n;
-      const int qy0 = real ? (t / p.tq_x) * CAM_TH : (1 << 20), qx0 = real ? (t % p.tq_x) * CAM_TW : 0;   // a missing tile loads zeros
+    for (int qt = blockIdx.x; qt < p.n_tiles; qt += gridDim.x) {
+      const int img = qt / p.tq_n, t = qt - img * p.tq_n;
+      const int qy0 = (t / p.tq_x) * CAM_TH, qx0 = (t % p.tq_x) * CAM_TW;
       mbar_wait(q_empty, qphase ^ 1, 10);
       if (elect_one()) {
-        if (rank == 0) mbar_expect_tx(q_full, 2u * CAM_Q_TX);
-        tma_load_4d_pair(sQ, &tmQ, mapa_rank(smem_u32(q_full), 0), qx0 * 8, qy0, 0, img);
+        mbar_expect_tx(q_full, CAM_Q_TX);
+        tma_load_4d(sQ, &tmQ, q_full, qx0 * 8, qy0, 0, img);
       }
       __syncwarp();
       qphase ^= 1;
       for (int it = 0; it < n_kt; ++it) {
-        const int j = it >= p.KT ? it - p.KT : it;
-        const int ky0 = (j / p.tk_x) * 32 + 16 * (int)rank, kx0 = (j % p.tk_x) * 8;
+        const int jj = it % (2 * p.KT), j = jj >> 1, hh = jj & 1;
+        const int ky0 = (j / p.tk_x) * 32 + 16 * hh, kx0 = (j % p.tk_x) * 8;
         for (int par = 0; par < 4; ++par) {
           mbar_wait(&k_empty[stage], phase ^ 1, 11);
           if (elect_one()) {
-            if (rank == 0) mbar_expect_tx(&k_full[stage], 2u * CAM_K_TX);
-            tma_load_4d_pair(sK + stage * CAM_K_STAGE, &tmK, mapa_rank(smem_u32(&k_full[stage]), 0), kx0 * 8, ky0, par * CAM_CB, img);
+            mbar_expect_tx(&k_full[stage], CAM_K_TX);
+            tma_load_4d(sK + stage * CAM_K_STAGE, &tmK, &k_full[stage], kx0 * 8, ky0, par * CAM_CB, img);
           }
           __syncwarp();
           if (++stage == CAM_S_STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1 && rank == 0) {
-    // ==================================================================== MMA issuer (leader, for both CTAs): M = 256, N = 256
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(CAM_KEYS >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t d_lo = ((uint32_t)(CAM_PLANE >> 4) & 0x3FFF) << 16;        // LBO: next channel block (K direction)
-    const uint32_t d_hi = ((uint32_t)(CAM_ROW >> 4) & 0x3FFF) | (1u << 14);    // SBO: next 8 rows (next window row); descriptor version 1
-    int stage = 0, acc_it = 0;
+  } else {
+    // ==================================================================== consumers: logits, softmax statistics, probabilities
+    const int wg = warp >> 2, wq = warp & 3;
+    const uint32_t base = smem_u32(smem);
+    const uint32_t a_m = (uint32_t)wg * 8u * CAM_ROW;   // queries 64..127 = tile rows 8..15
+    auto release = [&](uint64_t* bar) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar);
+    };
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+    int stage = 0;
     uint32_t phase = 0, qphase = 0;
-    for (int pr = cluster_id; pr < p.n_pairs; pr += n_clusters) {
+    for (int qt = blockIdx.x; qt < p.n_tiles; qt += gridDim.x) {
+      const int img = qt / p.tq_n, t = qt - img * p.tq_n;
+      int qy[2], qx[2];
+      bool valid[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        qy[h] = (t / p.tq_x) * CAM_TH + 8 * wg + 2 * wq + h;
+        qx[h] = (t % p.tq_x) * CAM_TW + (lane >> 2);
+        valid[h] = qy[h] < p.hs && qx[h] < p.ws;
+      }
+      float m_run[2] = {-INFINITY, -INFINITY}, s_run[2] = {0.0f, 0.0f}, inv[2] = {0.0f, 0.0f};
       mbar_wait(q_full, qphase, 12);
       qphase ^= 1;
-      for (int it = 0; it < n_kt; ++it, ++acc_it) {
-        const int as = acc_it & 1;
-        mbar_wait_cluster(&tmem_empty[as], ((acc_it >> 1) & 1) ^ 1, 13);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * 256;
+      for (int it = 0; it < n_kt; ++it) {
+        const bool second = it >= 2 * p.KT;
+        const int jj = it % (2 * p.KT), j = jj >> 1, hh = jj & 1;
+        if (it == 2 * p.KT) {
+          // combine the four lanes' partial statistics of each row
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float M = m_run[h];
+            M = fmaxf(M, __shfl_xor_sync(0xffffffffu, M, 1));
+            M = fmaxf(M, __shfl_xor_sync(0xffffffffu, M, 2));
+            float S = m_run[h] > -INFINITY ? s_run[h] * ex2_approx(m_run[h] - M) : 0.0f;
+            S += __shfl_xor_sync(0xffffffffu, S, 1);
+            S += __shfl_xor_sync(0xffffffffu, S, 2);
+            m_run[h] = M;
+            inv[h] = 1.0f / S;
+          }
+        }
+        int prev = -1;
         for (int par = 0; par < 4; ++par) {
           mbar_wait(&k_full[stage], phase, 14);
-          tc_fence_after();
-          const uint32_t lead = elect_one() ? 1u : 0u;
-          const uint32_t aQ = (smem_base + (uint32_t)(par * CAM_CB) * CAM_PLANE) >> 4;
-          const uint32_t aK = (smem_base + CAM_Q_BYTES + (uint32_t)stage * CAM_K_STAGE) >> 4;
-          uint32_t acc = par ? 1u : 0u;
+          const uint32_t aQ = base + (uint32_t)(par * CAM_CB) * CAM_PLANE + a_m;
+          const uint32_t aK = base + CAM_Q_BYTES + (uint32_t)stage * CAM_K_STAGE;
+          wg_fence();
+          wg_fence_acc(acc);
 #pragma unroll
           for (int tap = 0; tap < 4; ++tap) {
-            const uint32_t toff = (uint32_t)((tap >> 1) * CAM_WR + (tap & 1));   // (a, b) = tap offsets inside the window, 16 B units
+            const uint32_t toff = (uint32_t)((tap >> 1) * CAM_WR + (tap & 1)) * 16u;   // (a, b) = tap offsets inside the window
 #pragma unroll
             for (int k2 = 0; k2 < 6; ++k2) {
-              const uint32_t koff = (uint32_t)(2 * k2) * (CAM_PLANE >> 4) + toff;
-              umma2_bf16_if32(lead, tmem_d, d_lo | (aQ + koff), d_hi, d_lo | (aK + koff), d_hi, idesc, acc);
-              acc = 1u;
+              const uint32_t koff = (uint32_t)(2 * k2) * CAM_PLANE + toff;
+              Wgmma<128, false, 0>::mma(acc, wg_desc(aQ + koff, CAM_PLANE, CAM_ROW, WG_SW_NONE), wg_desc(aK + koff, CAM_PLANE, CAM_ROW, WG_SW_NONE),
+                                        (par | tap | k2) ? 1u : 0u);
             }
           }
-          umma2_commit_if(lead, &k_empty[stage]);
-          if (par == 3) umma2_commit_if(lead, &tmem_full[as]);
-          __syncwarp();
+          wg_commit();
+          if (prev >= 0) {
+            wg_wait<1>();
+            release(&k_empty[prev]);
+          }
+          prev = stage;
           if (++stage == CAM_S_STAGES) { stage = 0; phase ^= 1; }
         }
-      }
-      umma2_commit_if(elect_one() ? 1u : 0u, q_empty);   // the query windows of both CTAs are free once every MMA above has retired
-      __syncwarp();
-    }
-  } else if (warp >= 4) {
-    // ==================================================================== epilogue: softmax statistics, then probabilities
-    const int q = warp & 3, grp = (warp - 4) >> 2;
-    const int row = q * 32 + lane;
-    const int ry = row / CAM_TW, rx = row % CAM_TW;
-    int acc_it = 0;
-    for (int pr = cluster_id; pr < p.n_pairs; pr += n_clusters) {
-      const int img = pr / p.pairs_per_img, t = (pr - img * p.pairs_per_img) * 2 + (int)rank;
-      const int qy = (t / p.tq_x) * CAM_TH + ry, qx = (t % p.tq_x) * CAM_TW + rx;
-      const bool valid = t < p.tq_n && qy < p.hs && qx < p.ws;
-      float m_run = -INFINITY, s_run = 0.0f, inv = 0.0f;
-      for (int it = 0; it < n_kt; ++it, ++acc_it) {
-        const bool second = it >= p.KT;
-        const int j = second ? it - p.KT : it;
-        if (it == p.KT) {
-          // combine the four column groups' partial statistics of this row
-          stat_m[grp * 128 + row] = m_run;
-          stat_s[grp * 128 + row] = s_run;
-          named_bar_sync(1, TC_EPI_THREADS);
-          float M = stat_m[row];
+        wg_wait<0>();
+        wg_fence_acc(acc);
+        release(&k_empty[prev]);
+        if (it == n_kt - 1) release(q_empty);   // the query window is free once every MMA of this tile has retired
+        // logits in log2 units; padding keys (scale < 0) are excluded, masked keys (scale 0) keep logit 0
+        const float* cs = p.colscale + ((size_t)img * p.KT + j) * CAM_KEYS + hh * 128;
 #pragma unroll
-          for (int g = 1; g < TC_EPI_GROUPS; ++g) M = fmaxf(M, stat_m[g * 128 + row]);
-          float S = 0.0f;
+        for (int b = 0; b < 16; ++b) {
+          const float2 c2 = __ldg(reinterpret_cast<const float2*>(cs + frag_col(lane, b)));
 #pragma unroll
-          for (int g = 0; g < TC_EPI_GROUPS; ++g) {
-            const float mg = stat_m[g * 128 + row];
-            if (mg > -INFINITY) S += stat_s[g * 128 + row] * ex2_approx(mg - M);
+          for (int h = 0; h < 2; ++h) {
+            float& v0 = acc[4 * b + 2 * h];
+            float& v1 = acc[4 * b + 2 * h + 1];
+            v0 = c2.x < 0.0f ? -INFINITY : v0 * c2.x;
+            v1 = c2.y < 0.0f ? -INFINITY : v1 * c2.y;
           }
-          m_run = M;
-          inv = 1.0f / S;
-          named_bar_sync(1, TC_EPI_THREADS);   // everyone has read the partials before the next tile pair overwrites them
         }
-        const int as = acc_it & 1;
-        mbar_wait(&tmem_full[as], (acc_it >> 1) & 1, 15);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + as * 256 + grp * 64;
-        const float4* cs4 = reinterpret_cast<const float4*>(p.colscale + ((size_t)img * p.KT + j) * CAM_KEYS + grp * 64);
-        uint4* prow = reinterpret_cast<uint4*>(p.P) + (((size_t)img * p.KB + (size_t)j * 32 + grp * 8) * p.hs + qy) * p.ws + qx;
-        const size_t pstep = (size_t)p.hs * p.ws;   // next key block
-#pragma unroll 1
-        for (int c16 = 0; c16 < 4; ++c16) {
-          float v[16];
-          tmem_ld16(taddr + c16 * 16, v);
-          float cs[16];
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float4 c4 = __ldg(cs4 + c16 * 4 + i);
-            cs[4 * i] = c4.x; cs[4 * i + 1] = c4.y; cs[4 * i + 2] = c4.z; cs[4 * i + 3] = c4.w;
-          }
-          tmem_ld_wait();
-          // logits in log2 units; padding keys (scale < 0) are excluded, masked keys (scale 0) keep logit 0
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = cs[i] < 0.0f ? -INFINITY : v[i] * cs[i];
+        for (int h = 0; h < 2; ++h) {
           if (!second) {
-            float mx = v[0];
+            float mx = -INFINITY;
 #pragma unroll
-            for (int i = 1; i < 16; ++i) mx = fmaxf(mx, v[i]);
+            for (int b = 0; b < 16; ++b) mx = fmaxf(mx, fmaxf(acc[4 * b + 2 * h], acc[4 * b + 2 * h + 1]));
             if (mx > -INFINITY) {
-              const float mn = fmaxf(m_run, mx);
+              const float mn = fmaxf(m_run[h], mx);
               float s = 0.0f;
 #pragma unroll
-              for (int i = 0; i < 16; ++i) s += ex2_approx(v[i] - mn);
-              s_run = s_run * ex2_approx(m_run - mn) + s;   // m_run = -inf: s_run is 0 and ex2(-inf) = 0
-              m_run = mn;
+              for (int b = 0; b < 16; ++b) s += ex2_approx(acc[4 * b + 2 * h] - mn) + ex2_approx(acc[4 * b + 2 * h + 1] - mn);
+              s_run[h] = s_run[h] * ex2_approx(m_run[h] - mn) + s;   // m_run = -inf: s_run is 0 and ex2(-inf) = 0
+              m_run[h] = mn;
             }
-          } else if (valid) {
-            float e[16];
+          } else if (valid[h]) {
+            // key column c of this half = key (row hh * 16 + c / 8, column c % 8) of tile j: P block j * 32 + hh * 16 + c / 8
+            uint32_t* prow = reinterpret_cast<uint32_t*>(p.P) +
+                             ((((size_t)img * p.KB + (size_t)j * 32 + hh * 16) * p.hs + qy[h]) * p.ws + qx[h]) * 4 + (lane & 3);
+            const size_t pstep = (size_t)p.hs * p.ws * 4;   // next key block
 #pragma unroll
-            for (int i = 0; i < 16; ++i) e[i] = ex2_approx(v[i] - m_run) * inv;
-            prow[(size_t)(2 * c16) * pstep] = make_uint4(pack_bf16x2(e[0], e[1]), pack_bf16x2(e[2], e[3]), pack_bf16x2(e[4], e[5]), pack_bf16x2(e[6], e[7]));
-            prow[(size_t)(2 * c16 + 1) * pstep] =
-                make_uint4(pack_bf16x2(e[8], e[9]), pack_bf16x2(e[10], e[11]), pack_bf16x2(e[12], e[13]), pack_bf16x2(e[14], e[15]));
+            for (int b = 0; b < 16; ++b)
+              prow[b * pstep] = pack_bf16x2(ex2_approx(acc[4 * b + 2 * h] - m_run[h]) * inv[h], ex2_approx(acc[4 * b + 2 * h + 1] - m_run[h]) * inv[h]);
           }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(mapa_rank(smem_u32(&tmem_empty[as]), 0));
       }
     }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TC_TMEM_COLS) : "memory");
   }
 }
 
 // ------------------------------------------------------------------------------------------ PV kernel
+// One CTA per output tile (8 x 8 positions of the sub-pixel class grid, persistent): both consumer warpgroups take all 64
+// positions (wgmma M = 64, A = probabilities); warpgroup g produces sub-pixel classes 2g and 2g + 1 (N = 96 channels each,
+// B = values of that parity, MN-major). Warp 8 = TMA producer.
 struct CamPVParams {
   int h, w, Hs, Ws;
-  int to_x, to_n, pairs_per_img, n_pairs;
+  int to_x, to_n, n_tiles;
   int tk_x, n_chunks;   // 64-key chunks = KB / 8
   __nv_bfloat16* out;   // [B][12][h][w][8]
 };
 
-__global__ void __launch_bounds__(TC_NUM_THREADS, 1)
+__global__ void __launch_bounds__(CAM_THREADS, 1)
 cam_pv_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmV, const CamPVParams p) {
-  const uint32_t rank = cluster_ctarank();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + CAM_PV_STAGES * CAM_PV_STAGE);
   uint64_t* full = bars;
   uint64_t* empty = bars + CAM_PV_STAGES;
-  uint64_t* tmem_full = empty + CAM_PV_STAGES;
-  uint64_t* tmem_empty = tmem_full + 1;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty + 1);
 
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmP)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmV)) : "memory");
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < CAM_PV_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(tmem_full, 1);
-    mbar_init(tmem_empty, 2 * 4 * TC_EPI_GROUPS);
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < CAM_PV_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], CAM_CONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(TC_TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_ptr_smem, 0);
-  const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
+  __syncthreads();
 
-  if (warp == 0) {
+  if (warp == CAM_CONSUMER_WARPS) {
     // ==================================================================== producer
+    if (lane == 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmP)) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmV)) : "memory");
+    }
     int stage = 0;
     uint32_t phase = 0;
-    for (int pr = cluster_id; pr < p.n_pairs; pr += n_clusters) {
-      const int img = pr / p.pairs_per_img, t = (pr - img * p.pairs_per_img) * 2 + (int)rank;
-      const bool real = t < p.to_n;
-      const int yy0 = real ? (t / p.to_x) * CAM_TH : (1 << 20), xx0 = real ? (t % p.to_x) * CAM_TW : 0;
+    for (int ot = blockIdx.x; ot < p.n_tiles; ot += gridDim.x) {
+      const int img = ot / p.to_n, t = ot - img * p.to_n;
+      const int yy0 = (t / p.to_x) * CAM_PV_TH, xx0 = (t % p.to_x) * CAM_TW;
       for (int c = 0; c < p.n_chunks; ++c) {
         const int j = c >> 2;
         const int kyc = (j / p.tk_x) * 32 + (c & 3) * 8, kx0 = (j % p.tk_x) * 8;
         mbar_wait(&empty[stage], phase ^ 1, 20);
         if (elect_one()) {
           uint8_t* st = smem + stage * CAM_PV_STAGE;
-          const uint32_t bar = mapa_rank(smem_u32(&full[stage]), 0);
-          if (rank == 0) mbar_expect_tx(&full[stage], 2u * (CAM_PW_TX + 2 * CAM_V_TX));
+          mbar_expect_tx(&full[stage], CAM_PW_TX + 4 * CAM_V_TX);
           // probabilities of the queries (yy - a, xx - b), a, b in {0, 1}: window starts one row / column before the tile
-          tma_load_4d_pair(st, &tmP, bar, (xx0 - 1) * 8, yy0 - 1, c * 8, img);
-          // values: this CTA supplies the B rows (= output channels) of parity `rank` (columns [0,192) MMA) and `rank + 2`
-          tma_load_4d_pair(st + CAM_V0_OFF, &tmV, bar, kx0 * 8, kyc, (int)rank * CAM_CB, img);
-          tma_load_4d_pair(st + CAM_V1_OFF, &tmV, bar, kx0 * 8, kyc, ((int)rank + 2) * CAM_CB, img);
+          tma_load_4d(st, &tmP, &full[stage], (xx0 - 1) * 8, yy0 - 1, c * 8, img);
+          for (int par = 0; par < 4; ++par) tma_load_4d(st + CAM_V_OFF(par), &tmV, &full[stage], kx0 * 8, kyc, par * CAM_CB, img);
         }
         __syncwarp();
         if (++stage == CAM_PV_STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1 && rank == 0) {
-    // ==================================================================== MMA issuer: M = 256, N = 192 (two parities), B MN-major
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 16) | ((uint32_t)(192 >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t a_lo = ((uint32_t)(CAM_PLANE >> 4) & 0x3FFF) << 16;          // A = P, K-major: LBO = next key block
-    const uint32_t a_hi = ((uint32_t)(CAM_ROW >> 4) & 0x3FFF) | (1u << 14);      //                 SBO = next output row (8 positions)
-    const uint32_t b_lo = ((uint32_t)((9 * 16) >> 4) & 0x3FFF) << 16;           // B = V, MN-major: LBO = next 8 keys (next window row)
-    const uint32_t b_hi = ((uint32_t)(CAM_VPLANE >> 4) & 0x3FFF) | (1u << 14);   //                  SBO = next channel block
-    int stage = 0, tile_it = 0;
+  } else {
+    // ==================================================================== consumers
+    const int wg = warp >> 2, wq = warp & 3;
+    const uint32_t base = smem_u32(smem);
+    auto release = [&](uint64_t* bar) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar);
+    };
+    float acc0[48], acc1[48];
+#pragma unroll
+    for (int i = 0; i < 48; ++i) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
+    int stage = 0;
     uint32_t phase = 0;
-    for (int pr = cluster_id; pr < p.n_pairs; pr += n_clusters, ++tile_it) {
-      mbar_wait_cluster(tmem_empty, (tile_it & 1) ^ 1, 21);
-      tc_fence_after();
+    for (int ot = blockIdx.x; ot < p.n_tiles; ot += gridDim.x) {
+      const int img = ot / p.to_n, t = ot - img * p.to_n;
+      int prev = -1;
       for (int c = 0; c < p.n_chunks; ++c) {
         mbar_wait(&full[stage], phase, 22);
-        tc_fence_after();
-        const uint32_t lead = elect_one() ? 1u : 0u;
-        const uint32_t st = smem_base + (uint32_t)stage * CAM_PV_STAGE;
-        const uint32_t aP = st >> 4, aV0 = (st + CAM_V0_OFF) >> 4, aV1 = (st + CAM_V1_OFF) >> 4;
-        uint32_t acc = c ? 1u : 0u;
+        const uint32_t st = base + (uint32_t)stage * CAM_PV_STAGE;
+        const uint32_t aV0 = st + CAM_V_OFF(2 * wg), aV1 = st + CAM_V_OFF(2 * wg + 1);
+        wg_fence();
+        wg_fence_acc(acc0);
+        wg_fence_acc(acc1);
 #pragma unroll
         for (int tap = 0; tap < 4; ++tap) {
           const int a = tap >> 1, b = tap & 1;
-          const uint32_t poff = (uint32_t)((1 - a) * CAM_WR + (1 - b));   // query (yy - a, xx - b) inside the 17 x 9 window
-          const uint32_t voff = (uint32_t)(a * 9 + b);                    // value pixel (ky + a, kx + b) inside the 9 x 9 window
+          const uint32_t poff = (uint32_t)((1 - a) * CAM_WR + (1 - b)) * 16u;   // query (yy - a, xx - b) inside the 9 x 9 window
+          const uint32_t voff = (uint32_t)(a * 9 + b) * 16u;                    // value pixel (ky + a, kx + b) inside the 9 x 9 window
 #pragma unroll
           for (int k2 = 0; k2 < 4; ++k2) {
-            const uint32_t pa = aP + (uint32_t)(2 * k2) * (CAM_PLANE >> 4) + poff;
-            const uint32_t vb = (uint32_t)(2 * k2) * 9 + voff;
-            umma2_bf16_if32(lead, tmem_base, a_lo | pa, a_hi, b_lo | (aV0 + vb), b_hi, idesc, acc);
-            umma2_bf16_if32(lead, tmem_base + 192, a_lo | pa, a_hi, b_lo | (aV1 + vb), b_hi, idesc, acc);
-            acc = 1u;
+            const uint64_t da = wg_desc(st + (uint32_t)(2 * k2) * CAM_PPLANE + poff, CAM_PPLANE, CAM_ROW, WG_SW_NONE);
+            const uint32_t vb = (uint32_t)(2 * k2) * 9u * 16u + voff;
+            const uint32_t accum = (c | tap | k2) ? 1u : 0u;
+            Wgmma<96, false, 1>::mma(acc0, da, wg_desc(aV0 + vb, 9 * 16, CAM_VPLANE, WG_SW_NONE), accum);
+            Wgmma<96, false, 1>::mma(acc1, da, wg_desc(aV1 + vb, 9 * 16, CAM_VPLANE, WG_SW_NONE), accum);
           }
         }
-        umma2_commit_if(lead, &empty[stage]);
-        if (c == p.n_chunks - 1) umma2_commit_if(lead, tmem_full);
-        __syncwarp();
+        wg_commit();
+        if (prev >= 0) {
+          wg_wait<1>();
+          release(&empty[prev]);
+        }
+        prev = stage;
         if (++stage == CAM_PV_STAGES) { stage = 0; phase ^= 1; }
       }
-    }
-  } else if (warp >= 4) {
-    // ==================================================================== epilogue: column group g = sub-pixel class (py, px)
-    const int q = warp & 3, g = (warp - 4) >> 2;
-    const int row = q * 32 + lane;
-    const int ry = row / CAM_TW, rx = row % CAM_TW;
-    int tile_it = 0;
-    for (int pr = cluster_id; pr < p.n_pairs; pr += n_clusters, ++tile_it) {
-      const int img = pr / p.pairs_per_img, t = (pr - img * p.pairs_per_img) * 2 + (int)rank;
-      const int yy = (t / p.to_x) * CAM_TH + ry, xx = (t % p.to_x) * CAM_TW + rx;
-      const bool valid = t < p.to_n && yy < p.Hs && xx < p.Ws;
-      mbar_wait(tmem_full, tile_it & 1, 23);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + g * 96;
-      const int oy = 2 * yy + (g >> 1), ox = 2 * xx + (g & 1);
-      uint4* o = reinterpret_cast<uint4*>(p.out) + (((size_t)img * CAM_CB) * p.h + oy) * p.w + ox;
-      const size_t ostep = (size_t)p.h * p.w;
-#pragma unroll 1
-      for (int c16 = 0; c16 < 6; ++c16) {
-        float v[16];
-        tmem_ld16(taddr + c16 * 16, v);
-        tmem_ld_wait();
-        if (valid) {
-          o[(size_t)(2 * c16) * ostep] = make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
-          o[(size_t)(2 * c16 + 1) * ostep] =
-              make_uint4(pack_bf16x2(v[8], v[9]), pack_bf16x2(v[10], v[11]), pack_bf16x2(v[12], v[13]), pack_bf16x2(v[14], v[15]));
+      wg_wait<0>();
+      wg_fence_acc(acc0);
+      wg_fence_acc(acc1);
+      if (prev >= 0) release(&empty[prev]);
+      // epilogue: class g = (py, px) = parity of the values, output pixel (2 yy + py, 2 xx + px)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int yy = (t / p.to_x) * CAM_PV_TH + 2 * wq + h, xx = (t % p.to_x) * CAM_TW + (lane >> 2);
+        if (yy >= p.Hs || xx >= p.Ws) continue;
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          const int g = 2 * wg + q;
+          const int oy = 2 * yy + (g >> 1), ox = 2 * xx + (g & 1);
+          uint32_t* o = reinterpret_cast<uint32_t*>(p.out) + ((((size_t)img * CAM_CB) * p.h + oy) * p.w + ox) * 4 + (lane & 3);
+          const size_t ostep = (size_t)p.h * p.w * 4;   // next channel block
+#pragma unroll
+          for (int b = 0; b < 12; ++b) {
+            const float v0 = q ? acc1[4 * b + 2 * h] : acc0[4 * b + 2 * h], v1 = q ? acc1[4 * b + 2 * h + 1] : acc0[4 * b + 2 * h + 1];
+            o[b * ostep] = pack_bf16x2(v0, v1);
+          }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(mapa_rank(smem_u32(tmem_empty), 0));
     }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TC_TMEM_COLS) : "memory");
   }
 }
 
@@ -541,7 +489,7 @@ int cam_plan(int B, int h, int w, CamPlan* out) {
   p.KT = p.tk_x * ((p.hs + 31) / 32);
   p.KB = p.KT * 32;
   p.to_x = (p.Ws + CAM_TW - 1) / CAM_TW;
-  p.to_n = p.to_x * ((p.Hs + CAM_TH - 1) / CAM_TH);
+  p.to_n = p.to_x * ((p.Hs + CAM_PV_TH - 1) / CAM_PV_TH);
   p.fn_bytes = (size_t)B * 48 * p.Hs * p.Ws * 16;
   p.cs_bytes = (size_t)B * p.KT * CAM_KEYS * 4;
   p.p_bytes = (size_t)B * p.KB * p.hs * p.ws * 16;
@@ -550,18 +498,13 @@ int cam_plan(int B, int h, int w, CamPlan* out) {
 }
 
 static int g_cam_sms = 0, g_cam_optin = 0;
-static const int kCamSSmem = 1024 + CAM_Q_BYTES + CAM_S_STAGES * CAM_K_STAGE + 64 * 8 + 16 + 2 * 4 * 128 * 4 + 64;
-static const int kCamPVSmem = 1024 + CAM_PV_STAGES * CAM_PV_STAGE + 64 * 8 + 16 + 64;
+static const int kCamSSmem = 1024 + CAM_Q_BYTES + CAM_S_STAGES * CAM_K_STAGE + 64 * 8;
+static const int kCamPVSmem = 1024 + CAM_PV_STAGES * CAM_PV_STAGE + 64 * 8;
 
-static int cam_launch_pairs(const void* kernel, int n_pairs, int smem, cudaStream_t stream, void** args) {
-  cudaLaunchConfig_t cfg = {};
-  int grid = 2 * n_pairs < (g_cam_sms & ~1) ? 2 * n_pairs : (g_cam_sms & ~1);
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(TC_NUM_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cudaLaunchAttribute attr;
-  attr.id = cudaLaunchAttributeClusterDimension;
-  attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-  cfg.attrs = &attr; cfg.numAttrs = 1;
-  SE_CUDA_OK(cudaLaunchKernelExC(&cfg, kernel, args));
+// persistent launch: one CTA per SM at most, each walks tiles blockIdx.x, + gridDim.x, ...
+static int cam_launch(const void* kernel, int n_tiles, int smem, cudaStream_t stream, void** args) {
+  const int grid = n_tiles < g_cam_sms ? n_tiles : g_cam_sms;
+  SE_CUDA_OK(cudaLaunchKernel(kernel, dim3(grid), dim3(CAM_THREADS), args, (size_t)smem, stream));
   return 0;
 }
 
@@ -594,11 +537,11 @@ int cam_forward_tc(const void* f_s2d, const float* mask_s, void* out_c8, const C
     if (rc) return rc;
     CamSParams sp;
     sp.hs = pl.hs; sp.ws = pl.ws;
-    sp.tq_x = pl.tq_x; sp.tq_n = pl.tq_n; sp.pairs_per_img = (pl.tq_n + 1) / 2; sp.n_pairs = B * sp.pairs_per_img;
+    sp.tq_x = pl.tq_x; sp.tq_n = pl.tq_n; sp.n_tiles = B * pl.tq_n;
     sp.tk_x = pl.tk_x; sp.KT = pl.KT; sp.KB = pl.KB;
     sp.colscale = colscale; sp.P = (__nv_bfloat16*)P;
     void* args[3] = {&tmQ, &tmK, &sp};
-    rc = cam_launch_pairs((const void*)cam_s_kernel, sp.n_pairs, kCamSSmem, stream, args);
+    rc = cam_launch((const void*)cam_s_kernel, sp.n_tiles, kCamSSmem, stream, args);
     if (rc) return rc;
   }
   if (attn) {
@@ -608,17 +551,17 @@ int cam_forward_tc(const void* f_s2d, const float* mask_s, void* out_c8, const C
   }
   {
     CUtensorMap tmP, tmV;
-    int rc = cam_map(&tmP, P, pl.ws, pl.hs, pl.KB, B, CAM_WR, CAM_HR, 8);
+    int rc = cam_map(&tmP, P, pl.ws, pl.hs, pl.KB, B, CAM_WR, CAM_PV_TH + 1, 8);
     if (rc) return rc;
     rc = cam_map(&tmV, f_s2d, pl.Ws, pl.Hs, 48, B, 9, 9, CAM_CB);
     if (rc) return rc;
     CamPVParams pp;
     pp.h = pl.h; pp.w = pl.w; pp.Hs = pl.Hs; pp.Ws = pl.Ws;
-    pp.to_x = pl.to_x; pp.to_n = pl.to_n; pp.pairs_per_img = (pl.to_n + 1) / 2; pp.n_pairs = B * pp.pairs_per_img;
+    pp.to_x = pl.to_x; pp.to_n = pl.to_n; pp.n_tiles = B * pl.to_n;
     pp.tk_x = pl.tk_x; pp.n_chunks = pl.KB / 8;
     pp.out = (__nv_bfloat16*)out_c8;
     void* args[3] = {&tmP, &tmV, &pp};
-    rc = cam_launch_pairs((const void*)cam_pv_kernel, pp.n_pairs, kCamPVSmem, stream, args);
+    rc = cam_launch((const void*)cam_pv_kernel, pp.n_tiles, kCamPVSmem, stream, args);
     if (rc) return rc;
   }
   SE_CUDA_OK(cudaGetLastError());

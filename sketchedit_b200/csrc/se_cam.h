@@ -12,7 +12,7 @@ struct CamPlan {
   int tq_x, tq_n;   // query tiles (16 x 8 patches) per row / per image
   int tk_x, KT;     // key tiles (32 x 8 patches = 256 keys) per row / per image
   int KB;           // 8-key blocks of P per image = KT * 32
-  int to_x, to_n;   // output tiles (16 x 8 positions of the class grid) per row / per image
+  int to_x, to_n;   // output tiles (8 x 8 positions of the class grid) per row / per image
   size_t fn_bytes, cs_bytes, p_bytes;
 };
 int cam_plan(int B, int h, int w, CamPlan* out);

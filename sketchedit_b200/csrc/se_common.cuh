@@ -1,4 +1,4 @@
-// Shared device/host helpers for the sketchedit_b200 CUDA library (sm_100a only).
+// Shared device/host helpers for the sketchedit_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -39,7 +39,7 @@ const char* last_error();
 // tile geometry shared by every convolution kernel: one CTA tile = 8 x 16 output positions
 constexpr int TILE_H = 8;
 constexpr int TILE_W = 16;
-constexpr int TILE_M = TILE_H * TILE_W;  // 128 = UMMA M = TMEM lanes
+constexpr int TILE_M = TILE_H * TILE_W;  // 128 = two wgmma M = 64 halves
 constexpr int MAX_TAPS = 64;              // 9 taps x 3 operand-split products (+ space-to-depth / deconv variants)
 constexpr int KCHUNK = 32;               // bf16 elements per K chunk = 64 B = SWIZZLE_64B span
 
@@ -52,7 +52,7 @@ enum Epilogue : int {
 enum DType : int { DT_BF16 = 0, DT_F32 = 1, DT_F16X2 = 2 };
 // DT_F16X2: "split half" storage of an fp32 tensor for the fp32-on-tensor-cores mode: value = hi + lo with hi = fp16(v),
 // lo = fp16(v - hi) (22 significant bits). A channel-blocked tensor keeps the hi blocks first and the lo blocks `CB` blocks
-// further on ([N][2*CB][H][W][8]; space-to-depth: per parity group). A convolution then is three tcgen05 products per tap,
+// further on ([N][2*CB][H][W][8]; space-to-depth: per parity group). A convolution then is three wgmma products per tap,
 // x_hi*w_hi + x_hi*w_lo + x_lo*w_hi (the dropped lo*lo term is 2^-22 relative), accumulated in fp32.
 
 // One generalised convolution launch. Positions p=(py,px) on an Ho x Wo grid; input pixel for tap t

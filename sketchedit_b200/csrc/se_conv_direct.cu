@@ -1,8 +1,8 @@
-// CUDA-core direct convolution with the same op descriptor as the tcgen05 kernel.
+// CUDA-core direct convolution with the same op descriptor as the wgmma kernel.
 //
 // Role: (1) the fp32-exact path (activations and weights in fp32, fp32 FMA accumulation) used for
 // the fp32 parity configuration, (2) the low-channel head layers (12 -> 3 / 12 -> 1) whose K does
-// not fill a tensor-core tile, (3) an on-device cross-check of the tcgen05 kernel in tests.
+// not fill a tensor-core tile, (3) an on-device cross-check of the wgmma kernel in tests.
 // Weights: fp32 [img][tap][Ci][CoutP] with CoutP = Cout rounded up to 4.
 #include "se_common.cuh"
 #include "se_conv_direct.h"

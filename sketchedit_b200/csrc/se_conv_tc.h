@@ -1,4 +1,4 @@
-// Weight stage images of the tcgen05 convolution (se_conv_c8.cu): the swizzled shared-memory layout shared by the packer
+// Weight stage images of the wgmma convolution (se_conv_c8.cu): the swizzled shared-memory layout shared by the packer
 // (se_engine.cu) and the kernel.
 #pragma once
 #include "se_common.cuh"
@@ -28,7 +28,7 @@ inline int tc_stage_b_bytes(const TcWeights& w) { return w.NT * (w.r64 * 128 + w
 inline long long tc_weight_bytes_per_image(const TcWeights& w) { return (long long)w.n_tiles * tc_ksteps(w) * tc_stage_b_bytes(w); }
 
 // byte offset of (row r, byte kb within the row) inside a K-major operand tile with RB-byte rows whose base is
-// 1024 B aligned: the 128B / 64B TMA+UMMA swizzle (cute Swizzle<3,4,3> / Swizzle<2,4,3>).
+// 1024 B aligned: the 128B / 64B TMA + wgmma swizzle (cute Swizzle<3,4,3> / Swizzle<2,4,3>).
 __host__ __device__ inline uint32_t tc_swizzle_offset(int r, int kb, int RB) {
   uint32_t off = (uint32_t)r * RB + kb;
   return off ^ (((off >> 7) & (RB == 128 ? 7u : 3u)) << 4);
@@ -41,6 +41,5 @@ __host__ __device__ inline uint32_t tc_b_image_offset(int NT, int r64, bool is64
 }
 
 void fill_epi(const ConvParams& c, int NT, EpiParams* e);
-bool epi_addressable(const ConvParams& c);   // output fits the fast epilogue's 32-bit (16 B unit) addressing
 
 }  // namespace se

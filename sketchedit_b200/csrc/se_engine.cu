@@ -312,43 +312,27 @@ static int pack_class(se_model* m, Layer& L, const std::vector<EffTap>& taps, Cl
     // the exact (swizzled) shared-memory image of every pipeline stage, see se_conv_tc.h. Gate channels (n >= Cout/2) are stored
     // pre-multiplied by 0.5 (exact): the accumulator then holds 0.5*g and the epilogue's sigmoid(g + b) = 0.5*tanh(0.5*g + 0.5*b) + 0.5
     // needs one add (with a constant operand) before the MUFU
-    auto build_images = [&](TcWeights& tc, C8Layer* c8, const std::function<uint16_t(int, int, int)>& wv) -> int {
+    auto build_images = [&](TcWeights& tc, const std::function<uint16_t(int, int, int)>& wv) -> int {
       const int ksteps = tc_ksteps(tc), sb = tc_stage_b_bytes(tc);
       std::vector<uint16_t> img((size_t)ksteps * sb / 2, 0);
-      for (int pass = 0; pass < 2; ++pass) {
-        const bool pair = pass == 1;
-        if (pair && !(c8 && c8_pair_capable(*c8))) break;
-        // pass 1: second copy in CTA-pair format (se_conv_c8.cu, PAIR = 1): each CTA of a pair streams only its half of the rows
-        std::fill(img.begin(), img.end(), (uint16_t)0);
-        for (int ks = 0; ks < ksteps; ++ks) {
-          uint16_t* base = img.data() + (size_t)ks * sb / 2;
-          for (int j = 0; j < tc.r64 && tc.n64; ++j) {
-            const int u = ks * tc.r64 + j, t = u / tc.n64, chunk = u % tc.n64;
-            for (int n = 0; n < Cout; ++n)
-              for (int k = 0; k < 64; ++k) {
-                const uint32_t off = pair ? c8_pair_image_offset(tc, true, j, gated_column(Cout, n), k) : tc_b_image_offset(tc.NT, tc.r64, true, j, gated_column(Cout, n), k);
-                base[off / 2] = wv(t, chunk * 64 + k, n);
-              }
-          }
-          for (int j = 0; j < tc.r32 && tc.n32; ++j) {
-            const int t = ks * tc.r32 + j;
-            for (int n = 0; n < Cout; ++n)
-              for (int k = 0; k < 32; ++k) {
-                const uint32_t off = pair ? c8_pair_image_offset(tc, false, j, gated_column(Cout, n), k)
-                                          : tc_b_image_offset(tc.NT, tc.n64 ? tc.r64 : 0, false, j, gated_column(Cout, n), k);
-                base[off / 2] = wv(t, tc.n64 * 64 + k, n);
-              }
-          }
+      for (int ks = 0; ks < ksteps; ++ks) {
+        uint16_t* base = img.data() + (size_t)ks * sb / 2;
+        for (int j = 0; j < tc.r64 && tc.n64; ++j) {
+          const int u = ks * tc.r64 + j, t = u / tc.n64, chunk = u % tc.n64;
+          for (int n = 0; n < Cout; ++n)
+            for (int k = 0; k < 64; ++k) base[tc_b_image_offset(tc.NT, tc.r64, true, j, gated_column(Cout, n), k) / 2] = wv(t, chunk * 64 + k, n);
         }
-        void* d = nullptr;
-        int rc = upload(m, img.data(), img.size() * 2, &d);
-        if (rc) return rc;
-        if (pair) c8->w_pair = d; else tc.data = d;
+        for (int j = 0; j < tc.r32 && tc.n32; ++j) {
+          const int t = ks * tc.r32 + j;
+          for (int n = 0; n < Cout; ++n)
+            for (int k = 0; k < 32; ++k)
+              base[tc_b_image_offset(tc.NT, tc.n64 ? tc.r64 : 0, false, j, gated_column(Cout, n), k) / 2] = wv(t, tc.n64 * 64 + k, n);
+        }
       }
-      return 0;
+      return upload(m, img.data(), img.size() * 2, (void**)&tc.data);
     };
     auto wval = [&](int t, int ci, int n) -> float { return ci < Ci ? weff[((size_t)t * Ci + ci) * Cout + n] * (n >= Cout / 2 ? 0.5f : 1.0f) : 0.0f; };
-    int rc = build_images(*tcp, cw.use_c8 ? &cw.c8 : nullptr, [&](int t, int ci, int n) -> uint16_t { return f32_to_bf16_rn(wval(t, ci, n)); });
+    int rc = build_images(*tcp, [&](int t, int ci, int n) -> uint16_t { return f32_to_bf16_rn(wval(t, ci, n)); });
     if (rc) return rc;
     if (cw.use_c8) {
       // ---- split-half twin: virtual tap 3t + p, p = 0: (x_hi, w_hi), 1: (x_hi, w_lo), 2: (x_lo, w_hi)
@@ -373,7 +357,7 @@ static int pack_class(se_model* m, Layer& L, const std::vector<EffTap>& taps, Cl
       if (wmax > 0.0f && std::isfinite(wmax)) kw = std::min(24, std::max(0, 13 - (int)std::floor(std::log2(wmax))));
       cw.s_wscale = std::ldexp(1.0f, kw);
       auto half_bits = [](float v) -> uint16_t { return __half_as_ushort(__float2half_rn(v)); };
-      rc = build_images(cw.c8s.w, &cw.c8s, [&](int vt, int ci, int n) -> uint16_t {
+      rc = build_images(cw.c8s.w, [&](int vt, int ci, int n) -> uint16_t {
         const float w = wval(vt / 3, ci, n) * cw.s_wscale;
         const float hi = __half2float(__float2half_rn(w));
         return (vt % 3) == 1 ? half_bits(w - hi) : half_bits(w);
@@ -552,7 +536,7 @@ struct Ctx {
     if (!g_timing || dry) return;
     tag_.name = name; tag_.tensor = tensor; tag_.flops_alg = flops_alg; tag_.flops_exec = flops_exec; tag_.bytes_alg = bytes_alg; tag_.set = true;
   }
-  bool tc() const { return prec == SE_PREC_BF16_TC || prec == SE_PREC_FP32_TC; }   // tcgen05 kernels over channel-blocked activations
+  bool tc() const { return prec == SE_PREC_BF16_TC || prec == SE_PREC_FP32_TC; }   // wgmma kernels over channel-blocked activations
   bool split() const { return prec == SE_PREC_FP32_TC; }                            // ... in split-half storage (DT_F16X2)
   int sp() const { return split() ? 2 : 1; }                                        // channel-block multiplier of that storage
   int act_dt() const { return prec == SE_PREC_FP32_EXACT ? DT_F32 : (split() ? DT_F16X2 : DT_BF16); }
@@ -920,7 +904,7 @@ static int run_cam(Ctx& c, const View& f, const float* mask_s, void* out, int ou
   return 0;
 }
 
-// Attention of the fp32-on-tensor-cores mode: f fp32 NHWC [B][h][w][96] -> out fp32 NHWC, split-half fp16 tcgen05 GEMMs (se_gemm_split.cu)
+// Attention of the fp32-on-tensor-cores mode: f fp32 NHWC [B][h][w][96] -> out fp32 NHWC, split-half fp16 wgmma GEMMs (se_gemm_split.cu)
 static int run_cam_split(Ctx& c, const float* f, int h, int w, int C, const float* mask_s, float* out) {
   CamSplitPlan pl;
   {

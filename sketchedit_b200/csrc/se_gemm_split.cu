@@ -1,5 +1,5 @@
 // Contextual attention of the fp32-on-tensor-cores mode (SE_PREC_FP32_TC): the two attention GEMMs as split-half fp16
-// tcgen05 GEMMs (three products per K step: hi*hi + hi*lo + lo*hi, fp32 accumulation in TMEM: ~22 significant bits), with the
+// wgmma GEMMs (three products per K step: hi*hi + hi*lo + lo*hi, fp32 accumulation in registers: ~22 significant bits), with the
 // same semantics as the CUDA-core path in se_engine.cu run_cam (reference models/networks/splitcam.py:37-108,132-174 with
 // netG's configuration, editline_g.py:35-42: 4x4 patches at stride 2, keys normalised per (image, channel) plane, logits x10,
 // masked keys -> logit 0, softmax over the keys, paste = fold-SUM of the weighted raw patches):
@@ -12,7 +12,7 @@
 //
 // Operand layout ("K-blocked", the channel-blocked layout of se_conv_c8.cu with GEMM rows as pixels): fp16
 // [image][hi | lo][K / 8][rows][8]. A TMA box {8, rows, 4 K-blocks} lands in shared memory as the canonical no-swizzle
-// K-major UMMA layout (core matrix = 8 rows x 16 B contiguous; SBO = 128 B, LBO = rows x 16 B); read along its rows instead
+// K-major wgmma layout (core matrix = 8 rows x 16 B contiguous; SBO = 128 B, LBO = rows x 16 B); read along its rows instead
 // ({8, 32 rows, 32 blocks}) the same buffer is an MN-major operand (LBO = 128 B = next 8 K, SBO = 512 B = next 8 N).
 // Values are stored times a power of two per operand (fp16 exponent range, see se_common.cuh kSplitActScale); the epilogue
 // undoes it exactly.
@@ -30,7 +30,7 @@ constexpr int GS_A_BYTES = GS_BM * GS_BK * 2;                 // 8 KB  (one half
 constexpr int GS_B_BYTES = GS_BN * GS_BK * 2;                 // 16 KB
 constexpr int GS_STAGE = 2 * GS_A_BYTES + 2 * GS_B_BYTES;     // 48 KB: A_hi | A_lo | B_hi | B_lo
 constexpr int GS_STAGES = 4;
-constexpr int GS_THREADS = 192;                               // warp 0 TMA producer, warp 1 MMA issuer + TMEM owner, warps 2-5 epilogue
+constexpr int GS_THREADS = 288;                               // warps 0-7: two consumer warpgroups (rows 0-63 / 64-127), warp 8: TMA producer
 constexpr int GS_SMEM = 1024 + GS_STAGES * GS_STAGE;
 
 constexpr float kScaleQ = kSplitActScale;       // raw feature patches (queries / values)
@@ -100,27 +100,18 @@ __global__ void __launch_bounds__(GS_THREADS, 1)
 gemm_split_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmSplitParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* const smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ uint64_t full_bar[GS_STAGES], empty_bar[GS_STAGES], acc_bar;
-  __shared__ uint32_t tmem_ptr;
+  __shared__ uint64_t full_bar[GS_STAGES], empty_bar[GS_STAGES];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nt = blockIdx.x, mt = blockIdx.y, img = blockIdx.z;
   const int ksteps = p.K / GS_BK;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < GS_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(&acc_bar, 1);
+    for (int i = 0; i < GS_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }   // one arrival per consumer warp
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_ptr)), "r"(256) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ==================================================================== TMA producer
     if (elect_one()) {
       for (int ks = 0; ks < ksteps; ++ks) {
@@ -140,68 +131,62 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    // ==================================================================== MMA issuer: M = 128, N = 256, fp16 x fp16 -> fp32
-    const uint32_t idesc = (1u << 4) | (kBMN ? (1u << 16) : 0u) | ((uint32_t)(GS_BN >> 3) << 17) | ((uint32_t)(GS_BM >> 4) << 24);
-    // A, K-major no-swizzle: LBO = next K block (128 rows x 16 B), SBO = next 8 rows
-    const uint32_t a_lo = ((uint32_t)((GS_BM * 16) >> 4) & 0x3FFF) << 16, a_hi = ((128u >> 4) & 0x3FFF) | (1u << 14);
+  } else {
+    // ==================================================================== consumers: M = 64 rows each, N = 256, fp16 x fp16 -> fp32
+    const int wg = warp >> 2, wq = warp & 3;
+    // A, K-major no-swizzle: LBO = next K block (128 rows x 16 B), SBO = next 8 rows; this warpgroup's rows start 64 rows in
     // B, K-major: LBO = 256 rows x 16 B, SBO = 128 B.  MN-major: LBO = next 8 K rows (128 B), SBO = next N block (32 rows x 16 B)
-    const uint32_t b_lo = (kBMN ? ((128u >> 4) & 0x3FFF) : ((uint32_t)((GS_BN * 16) >> 4) & 0x3FFF)) << 16;
-    const uint32_t b_hi = (kBMN ? ((uint32_t)((GS_BK * 16) >> 4) & 0x3FFF) : ((128u >> 4) & 0x3FFF)) | (1u << 14);
-    const uint32_t a_k16 = (2u * GS_BM * 16) >> 4;                         // two K blocks further
-    const uint32_t b_k16 = kBMN ? (256u >> 4) : ((2u * GS_BN * 16) >> 4);
-    const uint32_t lead = elect_one() ? 1u : 0u;
+    const uint32_t a_lbo = GS_BM * 16, a_sbo = 128, a_m = (uint32_t)wg * 64u * 16u;
+    const uint32_t b_lbo = kBMN ? 128u : (uint32_t)GS_BN * 16u, b_sbo = kBMN ? (uint32_t)GS_BK * 16u : 128u;
+    const uint32_t a_k16 = 2u * GS_BM * 16;                         // two K blocks further
+    const uint32_t b_k16 = kBMN ? 256u : 2u * GS_BN * 16;
     const uint32_t base = smem_u32(smem);
+    float acc[GS_BN / 2];
+#pragma unroll
+    for (int i = 0; i < GS_BN / 2; ++i) acc[i] = 0.0f;
+    int prev = -1;
     for (int ks = 0; ks < ksteps; ++ks) {
       const int s = ks % GS_STAGES;
       const uint32_t ph = (uint32_t)(ks / GS_STAGES) & 1u;
       mbar_wait(&full_bar[s], ph, 2);
-      tc_fence_after();
       const uint32_t st = base + (uint32_t)s * GS_STAGE;
-      const uint32_t aH = st >> 4, aL = (st + GS_A_BYTES) >> 4, bH = (st + 2 * GS_A_BYTES) >> 4, bL = (st + 2 * GS_A_BYTES + GS_B_BYTES) >> 4;
+      const uint32_t aH = st + a_m, aL = st + GS_A_BYTES + a_m, bH = st + 2 * GS_A_BYTES, bL = st + 2 * GS_A_BYTES + GS_B_BYTES;
+      wg_fence();
+      wg_fence_acc(acc);
 #pragma unroll
       for (int k = 0; k < GS_BK / 16; ++k) {
-        umma_bf16_if32(lead, tmem, a_lo | (aH + k * a_k16), a_hi, b_lo | (bH + k * b_k16), b_hi, idesc, (ks | k) ? 1u : 0u);
-        umma_bf16_if32(lead, tmem, a_lo | (aH + k * a_k16), a_hi, b_lo | (bL + k * b_k16), b_hi, idesc, 1u);
-        umma_bf16_if32(lead, tmem, a_lo | (aL + k * a_k16), a_hi, b_lo | (bH + k * b_k16), b_hi, idesc, 1u);
+        const uint64_t dAH = wg_desc(aH + k * a_k16, a_lbo, a_sbo, WG_SW_NONE), dAL = wg_desc(aL + k * a_k16, a_lbo, a_sbo, WG_SW_NONE);
+        const uint64_t dBH = wg_desc(bH + k * b_k16, b_lbo, b_sbo, WG_SW_NONE), dBL = wg_desc(bL + k * b_k16, b_lbo, b_sbo, WG_SW_NONE);
+        Wgmma<GS_BN, true, kBMN ? 1 : 0>::mma(acc, dAH, dBH, (ks | k) ? 1u : 0u);
+        Wgmma<GS_BN, true, kBMN ? 1 : 0>::mma(acc, dAH, dBL, 1u);
+        Wgmma<GS_BN, true, kBMN ? 1 : 0>::mma(acc, dAL, dBH, 1u);
       }
-      umma_commit_if(lead, &empty_bar[s]);
-      __syncwarp();
+      wg_commit();
+      if (prev >= 0) {
+        wg_wait<1>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      prev = s;
     }
-    umma_commit_if(lead, &acc_bar);
-    __syncwarp();
-  } else {
-    // ==================================================================== epilogue: TMEM lane = row of the tile
-    const int q = warp & 3;                       // a warp may only read its own TMEM lane quadrant (warp id mod 4)
-    const int row = q * 32 + lane;
-    mbar_wait(&acc_bar, 0, 3);
-    tc_fence_after();
-    float* crow = p.C + (size_t)img * p.c_img_stride + (size_t)(mt * GS_BM + row) * p.ldc + nt * GS_BN;
+    wg_wait<0>();
+    wg_fence_acc(acc);
+    // epilogue straight from the fragment: row 64 wg + 16 wq + lane / 4 (+ 8), columns 8 j + 2 (lane % 4) (+ 1)
     const float* cs = p.colscale ? p.colscale + (size_t)img * p.ncs : nullptr;
-    const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16);
-    for (int c0 = 0; c0 < GS_BN; c0 += 32) {
-      float v0[16], v1[16];
-      tmem_ld16(taddr + c0, v0);
-      tmem_ld16(taddr + c0 + 16, v1);
-      tmem_ld_wait();
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int n0 = nt * GS_BN + c0 + j, n1 = n0 + 16;
-        v0[j] *= p.scale * (cs ? (n0 < p.ncs ? __ldg(cs + n0) : 0.0f) : 1.0f);
-        v1[j] *= p.scale * (cs ? (n1 < p.ncs ? __ldg(cs + n1) : 0.0f) : 1.0f);
-      }
+    for (int h = 0; h < 2; ++h) {
+      float* crow = p.C + (size_t)img * p.c_img_stride + (size_t)(mt * GS_BM + 64 * wg + frag_row(wq, lane, h)) * p.ldc + nt * GS_BN;
 #pragma unroll
-      for (int j = 0; j < 16; j += 4) {
-        *reinterpret_cast<float4*>(crow + c0 + j) = make_float4(v0[j], v0[j + 1], v0[j + 2], v0[j + 3]);
-        *reinterpret_cast<float4*>(crow + c0 + 16 + j) = make_float4(v1[j], v1[j + 1], v1[j + 2], v1[j + 3]);
+      for (int j = 0; j < GS_BN / 8; ++j) {
+        const int c = frag_col(lane, j), n0 = nt * GS_BN + c;
+        float v0 = acc[4 * j + 2 * h] * p.scale, v1 = acc[4 * j + 2 * h + 1] * p.scale;
+        if (cs) {
+          v0 *= n0 < p.ncs ? __ldg(cs + n0) : 0.0f;
+          v1 *= n0 + 1 < p.ncs ? __ldg(cs + n0 + 1) : 0.0f;
+        }
+        *reinterpret_cast<float2*>(crow + c) = make_float2(v0, v1);
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(256) : "memory");
   }
 }
 

@@ -1,4 +1,4 @@
-// Contextual attention of the fp32-on-tensor-cores mode: split-half fp16 tcgen05 GEMMs over explicit patch matrices (se_gemm_split.cu).
+// Contextual attention of the fp32-on-tensor-cores mode: split-half fp16 wgmma GEMMs over explicit patch matrices (se_gemm_split.cu).
 #pragma once
 #include "se_common.cuh"
 

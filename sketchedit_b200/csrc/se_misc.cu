@@ -161,19 +161,13 @@ __global__ void head_kernel(const T* __restrict__ x, const float* __restrict__ w
 // bf16 channel-blocked input (the tensor-core path): same arithmetic, organised for the FP32 pipe.
 //   * weights come in as a by-value kernel parameter: they sit in the constant bank and feed the FMAs directly
 //     (the generic kernel spends one shared-memory load per FMA)
-//   * channels are processed in pairs with the packed fma.rn.f32x2 (two FMAs per issue slot): a bf16x2 word expands
-//     to the (even, odd) channel pair, the weights are stored as matching pairs, and each output keeps an (even, odd)
-//     pair of partial sums that is added at the end
+//   * channels are processed in pairs: a bf16x2 word expands to the (even, odd) channel pair, the weights are stored as
+//     matching pairs, and each output keeps an (even, odd) pair of partial sums that is added at the end
 template <int COUT>
 struct HeadWeights {
   float2 w[9][6][COUT];   // [tap][channel pair][out] = (w[tap][2p][o], w[tap][2p+1][o])
   float b[COUT];
 };
-__device__ __forceinline__ unsigned long long ffma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
 template <int COUT>
 __global__ void __launch_bounds__(128) head_c8_kernel(const __nv_bfloat16* __restrict__ x, const __grid_constant__ HeadWeights<COUT> hw, int B, int H,
                                                       int W, int mode, const float* __restrict__ img, const float* __restrict__ mask_bin,
@@ -185,9 +179,9 @@ __global__ void __launch_bounds__(128) head_c8_kernel(const __nv_bfloat16* __res
   if (i >= B * HW) return;
   const long long b = i / HW, pix = i % HW;
   const int yy = (int)(pix / W), xx = (int)(pix % W);
-  unsigned long long acc[COUT];
+  float2 acc[COUT];
 #pragma unroll
-  for (int o = 0; o < COUT; ++o) acc[o] = 0ull;
+  for (int o = 0; o < COUT; ++o) acc[o] = make_float2(0.0f, 0.0f);
   const uint4* plane0 = reinterpret_cast<const uint4*>(x) + (b * 2) * HW;   // [b][2 blocks][H][W] x 16 B
 #pragma unroll
   for (int t = 0; t < 9; ++t) {
@@ -199,18 +193,18 @@ __global__ void __launch_bounds__(128) head_c8_kernel(const __nv_bfloat16* __res
 #pragma unroll
     for (int p = 0; p < 6; ++p) {
       // bf16x2 -> (even channel, odd channel) as an fp32 pair
-      const unsigned long long xp = ((unsigned long long)(wds[p] & 0xffff0000u) << 32) | (unsigned long long)(wds[p] << 16);
+      const float xe = __uint_as_float(wds[p] << 16), xo = __uint_as_float(wds[p] & 0xffff0000u);
 #pragma unroll
       for (int o = 0; o < COUT; ++o) {
         const float2 wv = hw.w[t][p][o];
-        const unsigned long long wp = ((unsigned long long)__float_as_uint(wv.y) << 32) | __float_as_uint(wv.x);
-        acc[o] = ffma2(xp, wp, acc[o]);
+        acc[o].x = fmaf(xe, wv.x, acc[o].x);
+        acc[o].y = fmaf(xo, wv.y, acc[o].y);
       }
     }
   }
   float r[COUT];
 #pragma unroll
-  for (int o = 0; o < COUT; ++o) r[o] = hw.b[o] + (__uint_as_float((uint32_t)acc[o]) + __uint_as_float((uint32_t)(acc[o] >> 32)));
+  for (int o = 0; o < COUT; ++o) r[o] = hw.b[o] + (acc[o].x + acc[o].y);
   if (mode == HEAD_MASK) {
     const float sg = 1.0f / (1.0f + expf(-r[0]));
     out_nchw[b * obs + pix] = sg;

@@ -89,7 +89,7 @@ class Engine:
 
     def finalize(self):
         if not torch.cuda.is_available():
-            raise _lib.SketchEditB200Error("sketchedit_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise _lib.SketchEditB200Error("sketchedit_b200 needs a CUDA device (sm_90a, H100); there is no CPU fallback")
         _lib.check(self.lib.se_model_finalize(self.h))
         self.finalized = True
         self.device = torch.device("cuda", torch.cuda.current_device())   # weights + workspace live here

@@ -1,6 +1,6 @@
 """Batch inference entry point -- same command line as the reference's test.py (reference test.py:12-37,
 test_celeb.sh, test_places.sh): build the dataloader and the model from the flags, run
-``model(data, mode='inference')`` per batch on the B200 kernels, convert to uint8 (truncating, like
+``model(data, mode='inference')`` per batch on the CUDA kernels, convert to uint8 (truncating, like
 ``astype(np.uint8)``), RGB->BGR, and write PNGs to --output_dir (masks to --output_mask_dir)."""
 import os
 

@@ -1,7 +1,7 @@
 """GPU parity of netM / netG / the whole inference path against the CPU oracle and the committed
 reference-generated golden vectors.
 
-Tolerances are BASELINE.json's: 1e-3 max-abs (fp32 path), 1e-2 (bf16 tensor-core path), both against
+Tolerances (DESIGN.md section 3): 1e-3 max-abs (fp32 path), 1e-2 (bf16 tensor-core path), both against
 the fp32 oracle. The mask threshold (reference editline2_model.py:347) is discontinuous, so netG and the
 end-to-end output are compared with the oracle evaluated on OUR binarised mask; the number of
 threshold flips against the oracle's own mask is bounded separately (SURVEY.md section 7.3-2).
@@ -15,7 +15,7 @@ import torch
 
 from oracle import sketchedit_oracle as O
 from sketchedit_b200 import synth
-from tests.util_parity import engine, maxdiff, weights
+from tests.util_parity import engine, golden, maxdiff, weights
 
 pytestmark = pytest.mark.gpu
 TOL = {"fp32": 1e-3, "fp32_direct": 1e-3, "bf16": 1e-2}   # "fp32": split-half tensor-core arithmetic, "fp32_direct": CUDA cores
@@ -80,21 +80,21 @@ def test_fp32_path_matches_reference_golden(name, golden_dir, prec):
     flags = dict(eval(str(z["flags"])))
     eng = engine(**flags)
     composed, mask, ex = eng.inference(image.cuda(), sketch.cuda(), precision=prec, want=("fine", "mask_bin"))
-    ref_bin = (torch.from_numpy(z["mask"]) > 0.5).float()
-    assert int((ex["mask_bin"].cpu() != ref_bin).sum()) == 0
-    assert maxdiff(mask.cpu(), torch.from_numpy(z["mask"])) <= 1e-3
+    ours_bin, ref_mask = golden(z, "mask", ex["mask_bin"])
+    assert int((ours_bin != (ref_mask > 0.5).float()).sum()) == 0
+    assert maxdiff(*golden(z, "mask", mask)) <= 1e-3
     if "fine" in z:
-        assert maxdiff(ex["fine"].cpu(), torch.from_numpy(z["fine"])) <= 1e-3
-    assert maxdiff(composed.cpu(), torch.from_numpy(z["composed"])) <= 1e-3
+        assert maxdiff(*golden(z, "fine", ex["fine"])) <= 1e-3
+    assert maxdiff(*golden(z, "composed", composed)) <= 1e-3
 
 
 def test_bf16_face_config(golden_dir):
-    """BASELINE.json config: 256x256 face + sketch, bf16 tensor-core path, 1e-2 vs the fp32 reference."""
+    """256x256 face + sketch, bf16 tensor-core path, 1e-2 vs the fp32 reference."""
     WM, WG = weights()
     z = np.load(os.path.join(golden_dir, "face_602_256x256.npz"))
     image, sketch = _golden_inputs(z)
     composed, mask, ex = engine().inference(image.cuda(), sketch.cuda(), precision="bf16", want=("mask_bin",))
-    assert maxdiff(mask.cpu(), torch.from_numpy(z["mask"])) <= 1e-2
+    assert maxdiff(*golden(z, "mask", mask)) <= 1e-2
     ours_bin = ex["mask_bin"].cpu()
     ref = O.inference(WM, WG, image, sketch, mask_bin_override=ours_bin)
     assert maxdiff(composed.cpu(), ref["composed"]) <= 1e-2

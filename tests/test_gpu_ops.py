@@ -1,9 +1,9 @@
 """GPU parity of the operators behind gen_conv / gen_deconv / contextual attention, through the C ABI.
 
-fp32 mode  : "fp32" = fp32-parity arithmetic on the tensor cores (split-half fp16 operands, three tcgen05 products per tap),
+fp32 mode  : "fp32" = fp32-parity arithmetic on the tensor cores (split-half fp16 operands, three wgmma products per tap),
              "fp32_direct" = the fp32 CUDA-core kernels (its cross-check); both vs the fp32 oracle, tolerance 1e-4 (abs,
              activations are O(1)).
-bf16 mode  : tcgen05 kernels vs the oracle evaluated on the SAME bf16-rounded inputs and weights, so the
+bf16 mode  : wgmma kernels vs the oracle evaluated on the SAME bf16-rounded inputs and weights, so the
              only differences are fp32 accumulation order and the final bf16 rounding of the output:
              tolerance 2^-8 relative to max|y| (one bf16 ulp at the top of the range) + 1e-3.
 """
@@ -88,7 +88,7 @@ def test_contextual_attention_fp32(h, w, B):
 
 @pytest.mark.parametrize("h,w,B", CAM_CASES)
 def test_contextual_attention_fp32_split_gemm(h, w, B):
-    """precision='fp32' without the attention-map output: the split-half fp16 tcgen05 GEMM attention (se_gemm_split.cu), which the
+    """precision='fp32' without the attention-map output: the split-half fp16 wgmma GEMM attention (se_gemm_split.cu), which the
     fp32-on-tensor-cores forward uses; same tolerance as the CUDA-core fp32 attention above."""
     feat = F.relu(rand_act((B, 96, h, w), seed=h * w))
     mask = torch.zeros(B, 1, 4 * h, 4 * w)

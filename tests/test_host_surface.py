@@ -99,7 +99,7 @@ def test_testimage_dataset_reads_the_reference_list_format(tmp_path):
 
 
 def test_bench_roofline_math_from_class_table():
-    """bench.py's roofline block is recomputable from its per-class rows: frac = sum(algorithmic FLOPs of the tcgen05 classes) / sum(their
+    """bench.py's roofline block is recomputable from its per-class rows: frac = sum(algorithmic FLOPs of the tensor-core classes) / sum(their
     time) / peak; a class is 'hbm' bound when its bytes / HBM peak exceed its FLOPs / tensor peak; per-layer frac = sum(ideal) / sum(time)."""
     import bench
     peaks = {"hbm_gbs": 6000.0, "bf16_tflops": 1700.0, "bf16_tflops_sustained": 1500.0}

@@ -1,5 +1,5 @@
 """Pin the CPU oracle against outputs of the UNMODIFIED reference (tests/golden/*.npz,
-made by oracle/make_golden.py from /root/reference in the build container)."""
+made by oracle/make_golden.py from the reference checkout; large arrays stored as a fixed sample)."""
 import glob
 import os
 
@@ -9,6 +9,7 @@ import torch
 
 from oracle import sketchedit_oracle as O
 from sketchedit_b200 import synth
+from tests.util_parity import golden
 
 TOL = 2e-5   # fp32 vs fp32, different op order (attention form vs grouped conv)
 
@@ -37,17 +38,18 @@ def test_oracle_matches_reference(name, weights, golden_dir):
     taps = {}
     r = O.inference(WM, WG, image, sketch, taps=taps, **flags)
     # the binarised mask must agree exactly (otherwise nothing downstream is comparable)
-    ref_bin = torch.from_numpy(z["mask"]) > 0.5
-    assert int((ref_bin != (r["mask_bin"] > 0.5)).sum()) == 0
+    ours_bin, ref_mask = golden(z, "mask", r["mask_bin"])
+    assert int(((ref_mask > 0.5) != (ours_bin > 0.5)).sum()) == 0
     for key in ("composed", "mask", "coarse", "fine"):
         if key in z:
-            d = float((r[key] - torch.from_numpy(z[key])).abs().max())
+            ours, ref = golden(z, key, r[key])
+            d = float((ours - ref).abs().max())
             assert d <= TOL, (name, key, d)
     for key in z.files:
-        if key.startswith("tap:"):
-            ours = taps[key[4:]]
-            d = float((ours - torch.from_numpy(z[key])).abs().max())
-            scale = max(1.0, float(torch.from_numpy(z[key]).abs().max()))
+        if key.startswith("tap:") and not key.endswith("@idx"):
+            ours, ref = golden(z, key, taps[key[4:]])
+            d = float((ours - ref).abs().max())
+            scale = max(1.0, float(ref.abs().max()))
             assert d <= TOL * scale * 4, (name, key, d)
 
 

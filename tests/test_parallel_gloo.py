@@ -1,6 +1,6 @@
 """world_size-2 gloo test of the multi-GPU host logic: contiguous batch shards + the single all-gather of the
 packed outputs reproduce the single-process result (per-sample independence of the path, SURVEY.md section 8e).
-The per-shard compute is the CPU oracle (the B200 kernels cannot run here); ordering / packing / gather are the
+The per-shard compute is the CPU oracle (the CUDA kernels cannot run here); ordering / packing / gather are the
 code bench.py uses on the GPU box."""
 import os
 import socket

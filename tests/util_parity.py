@@ -9,6 +9,16 @@ from sketchedit_b200.arch import layer_map
 _W = {}
 
 
+def golden(z, key, ours):
+    """(ours, reference) for golden array `key`: large arrays are stored as a fixed sample of their flat positions
+    (`<key>@idx`, oracle/make_golden.py shrink), and `ours` is then restricted to the same positions."""
+    ref = torch.from_numpy(z[key])
+    ours = torch.as_tensor(ours).detach().cpu()
+    if key + "@idx" in z.files:
+        return ours.reshape(-1)[torch.from_numpy(z[key + "@idx"].astype(np.int64))], ref
+    return ours, ref
+
+
 def weights():
     if not _W:
         _W["M"] = synth.synth_state_dict("M")

@@ -1,6 +1,6 @@
 """Error of every precision mode against the CPU oracle on the same inputs and weights (GPU side; test infrastructure):
 
-    python tools/precision_report.py [B H W]   ->  markdown table on stdout (profiles/r02_precision_modes.md)
+    python tools/precision_report.py [B H W]   ->  markdown table on stdout
 
 max / mean |difference| of the soft mask, the fine stage and the composed image, threshold flips of the binarised mask, and
 the share of uint8 output values (test.py's PNG conversion) that differ from the oracle's.
