@@ -100,6 +100,13 @@ int se_gated_conv_forward(se_model* m, char net, const char* layer, const float*
 int se_contextual_attention_forward(const float* feat, const float* mask_s, int B, int C, int h, int w, int precision,
                                     float* out, float* attn, void* stream);
 
+/* ---- attention workspace: the contextual attention's probabilities (and, in the fp32 modes, its logits) are L x L per
+ * image (L = patches of the 1/4-resolution map). They are computed in bands of query rows through one band-sized buffer:
+ * the tallest band whose buffers fit `bytes` (process-wide; every forward and se_contextual_attention_forward). Results do
+ * not depend on the band split. 0 restores the default of 16 GiB; a negative value is an error. A call whose smallest band
+ * does not fit fails and names the bytes it needs. Calls that return the attention map (attn != NULL) use one band. */
+int se_set_attention_workspace_limit(long long bytes);
+
 /* ---- test.py:25-27 output conversion on device: uint8 HWC BGR image + uint8 mask (truncating) */
 int se_outputs_to_uint8(const float* composed, const float* mask, int B, int H, int W, unsigned char* bgr_hwc,
                         unsigned char* mask_u8, void* stream);

@@ -38,6 +38,7 @@ SIGNATURES = {
                                        _c_void_p]),
     "se_contextual_attention_forward": (_c_int, [_c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_int, _c_int, _c_void_p,
                                                  _c_void_p, _c_void_p]),
+    "se_set_attention_workspace_limit": (_c_int, [ctypes.c_longlong]),
     "se_outputs_to_uint8": (_c_int, [_c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_void_p, _c_void_p, _c_void_p]),
     "se_last_launch_count": (_c_int, []),
     "se_workspace_bytes": (ctypes.c_longlong, [_c_void_p]),

@@ -21,6 +21,12 @@
 // leave the registers: the S kernel sweeps the key tiles twice per query tile - sweep 0 keeps the running row maximum and sum
 // (fp32, per lane, combined over the row's quad of lanes at the end), sweep 1 recomputes the logits and writes
 // exp(t - max) / sum. Key order inside P is the S kernel's tile order, which is also the order the PV kernel walks the keys.
+//
+// Bands: P is L x L per image, so large maps run in bands of query rows [q0, q1) (q0 a multiple of 16: the S tiles keep their
+// alignment) through one band-sized P buffer. Output class row y reads query rows y - 1 and y, so band [q0, q1) writes class
+// rows [q0, q1) (the last band also row hs) and needs query row q0 - 1 as well: it is carried over from the previous band
+// (buffer row 0) by one strided copy instead of being recomputed. Every row's S and PV arithmetic is the same as in a single
+// band, so the output does not depend on the band split.
 #include "se_cam.h"
 
 #include <stdlib.h>
@@ -148,6 +154,7 @@ __global__ void cam_attn_export_kernel(const __nv_bfloat16* __restrict__ P, floa
 // only two shuffles per row.
 struct CamSParams {
   int hs, ws;
+  int q0, q1, qa, prows;   // band query rows [q0, q1); P buffer row r holds query row qa + r, prows rows per key block
   int tq_x, tq_n, n_tiles;
   int tk_x, KT, KB;
   const float* colscale;
@@ -187,7 +194,7 @@ cam_s_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
     uint32_t phase = 0, qphase = 0;
     for (int qt = blockIdx.x; qt < p.n_tiles; qt += gridDim.x) {
       const int img = qt / p.tq_n, t = qt - img * p.tq_n;
-      const int qy0 = (t / p.tq_x) * CAM_TH, qx0 = (t % p.tq_x) * CAM_TW;
+      const int qy0 = p.q0 + (t / p.tq_x) * CAM_TH, qx0 = (t % p.tq_x) * CAM_TW;
       mbar_wait(q_empty, qphase ^ 1, 10);
       if (elect_one()) {
         mbar_expect_tx(q_full, CAM_Q_TX);
@@ -229,9 +236,9 @@ cam_s_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
       bool valid[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        qy[h] = (t / p.tq_x) * CAM_TH + 8 * wg + 2 * wq + h;
+        qy[h] = p.q0 + (t / p.tq_x) * CAM_TH + 8 * wg + 2 * wq + h;
         qx[h] = (t % p.tq_x) * CAM_TW + (lane >> 2);
-        valid[h] = qy[h] < p.hs && qx[h] < p.ws;
+        valid[h] = qy[h] < p.q1 && qx[h] < p.ws;
       }
       float m_run[2] = {-INFINITY, -INFINITY}, s_run[2] = {0.0f, 0.0f}, inv[2] = {0.0f, 0.0f};
       mbar_wait(q_full, qphase, 12);
@@ -312,8 +319,8 @@ cam_s_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
           } else if (valid[h]) {
             // key column c of this half = key (row hh * 16 + c / 8, column c % 8) of tile j: P block j * 32 + hh * 16 + c / 8
             uint32_t* prow = reinterpret_cast<uint32_t*>(p.P) +
-                             ((((size_t)img * p.KB + (size_t)j * 32 + hh * 16) * p.hs + qy[h]) * p.ws + qx[h]) * 4 + (lane & 3);
-            const size_t pstep = (size_t)p.hs * p.ws * 4;   // next key block
+                             ((((size_t)img * p.KB + (size_t)j * 32 + hh * 16) * p.prows + (qy[h] - p.qa)) * p.ws + qx[h]) * 4 + (lane & 3);
+            const size_t pstep = (size_t)p.prows * p.ws * 4;   // next key block
 #pragma unroll
             for (int b = 0; b < 16; ++b)
               prow[b * pstep] = pack_bf16x2(ex2_approx(acc[4 * b + 2 * h] - m_run[h]) * inv[h], ex2_approx(acc[4 * b + 2 * h + 1] - m_run[h]) * inv[h]);
@@ -330,6 +337,7 @@ cam_s_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
 // B = values of that parity, MN-major). Warp 8 = TMA producer.
 struct CamPVParams {
   int h, w, Hs, Ws;
+  int y0, y1, qa;       // band: class rows [y0, y1); row 0 of the P tensor map is query row qa
   int to_x, to_n, n_tiles;
   int tk_x, n_chunks;   // 64-key chunks = KB / 8
   __nv_bfloat16* out;   // [B][12][h][w][8]
@@ -361,7 +369,7 @@ cam_pv_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_constant__ C
     uint32_t phase = 0;
     for (int ot = blockIdx.x; ot < p.n_tiles; ot += gridDim.x) {
       const int img = ot / p.to_n, t = ot - img * p.to_n;
-      const int yy0 = (t / p.to_x) * CAM_PV_TH, xx0 = (t % p.to_x) * CAM_TW;
+      const int yy0 = p.y0 + (t / p.to_x) * CAM_PV_TH, xx0 = (t % p.to_x) * CAM_TW;
       for (int c = 0; c < p.n_chunks; ++c) {
         const int j = c >> 2;
         const int kyc = (j / p.tk_x) * 32 + (c & 3) * 8, kx0 = (j % p.tk_x) * 8;
@@ -370,7 +378,7 @@ cam_pv_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_constant__ C
           uint8_t* st = smem + stage * CAM_PV_STAGE;
           mbar_expect_tx(&full[stage], CAM_PW_TX + 4 * CAM_V_TX);
           // probabilities of the queries (yy - a, xx - b), a, b in {0, 1}: window starts one row / column before the tile
-          tma_load_4d(st, &tmP, &full[stage], (xx0 - 1) * 8, yy0 - 1, c * 8, img);
+          tma_load_4d(st, &tmP, &full[stage], (xx0 - 1) * 8, yy0 - 1 - p.qa, c * 8, img);
           for (int par = 0; par < 4; ++par) tma_load_4d(st + CAM_V_OFF(par), &tmV, &full[stage], kx0 * 8, kyc, par * CAM_CB, img);
         }
         __syncwarp();
@@ -429,8 +437,8 @@ cam_pv_kernel(const __grid_constant__ CUtensorMap tmP, const __grid_constant__ C
       // epilogue: class g = (py, px) = parity of the values, output pixel (2 yy + py, 2 xx + px)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int yy = (t / p.to_x) * CAM_PV_TH + 2 * wq + h, xx = (t % p.to_x) * CAM_TW + (lane >> 2);
-        if (yy >= p.Hs || xx >= p.Ws) continue;
+        const int yy = p.y0 + (t / p.to_x) * CAM_PV_TH + 2 * wq + h, xx = (t % p.to_x) * CAM_TW + (lane >> 2);
+        if (yy >= p.y1 || xx >= p.Ws) continue;
 #pragma unroll
         for (int q = 0; q < 2; ++q) {
           const int g = 2 * wg + q;
@@ -463,12 +471,13 @@ static EncodeTiledFn cam_encode_fn() {
   return fn;
 }
 
-// channel-blocked 4-D view (8*W, H, blocks, N) of a bf16 tensor [N][blocks][H][W][8]; box = (cols x 8, rows, nblk, 1)
-static int cam_map(CUtensorMap* tm, const void* base, int W, int H, int blocks, int N, int cols, int rows, int nblk) {
+// channel-blocked 4-D view (8*W, H, blocks, N) of a bf16 tensor [N][blocks][Hp][W][8] (H <= Hp rows of each plane are in
+// the view); box = (cols x 8, rows, nblk, 1)
+static int cam_map(CUtensorMap* tm, const void* base, int W, int H, int Hp, int blocks, int N, int cols, int rows, int nblk) {
   EncodeTiledFn enc = cam_encode_fn();
   SE_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
   cuuint64_t dims[4] = {(cuuint64_t)W * 8, (cuuint64_t)H, (cuuint64_t)blocks, (cuuint64_t)N};
-  cuuint64_t strides[3] = {(cuuint64_t)W * 16, (cuuint64_t)H * W * 16, (cuuint64_t)blocks * H * W * 16};
+  cuuint64_t strides[3] = {(cuuint64_t)W * 16, (cuuint64_t)Hp * W * 16, (cuuint64_t)blocks * Hp * W * 16};
   cuuint32_t box[4] = {(cuuint32_t)(cols * 8), (cuuint32_t)rows, (cuuint32_t)nblk, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -477,22 +486,33 @@ static int cam_map(CUtensorMap* tm, const void* base, int W, int H, int blocks, 
   return 0;
 }
 
-int cam_plan(int B, int h, int w, CamPlan* out) {
+int cam_plan(int B, int h, int w, long long limit, bool single_band, CamPlan* out) {
   SE_REQUIRE(h % 2 == 0 && w % 2 == 0 && h >= 4 && w >= 4, "attention map must be even-sized and >= 4");
   CamPlan p;
   p.B = B; p.h = h; p.w = w;
   p.Hs = h / 2; p.Ws = w / 2;
   p.hs = p.Hs - 1; p.ws = p.Ws - 1;
   p.tq_x = (p.ws + CAM_TW - 1) / CAM_TW;
-  p.tq_n = p.tq_x * ((p.hs + CAM_TH - 1) / CAM_TH);
   p.tk_x = (p.ws + 7) / 8;
   p.KT = p.tk_x * ((p.hs + 31) / 32);
   p.KB = p.KT * 32;
   p.to_x = (p.Ws + CAM_TW - 1) / CAM_TW;
-  p.to_n = p.to_x * ((p.Hs + CAM_PV_TH - 1) / CAM_PV_TH);
   p.fn_bytes = (size_t)B * 48 * p.Hs * p.Ws * 16;
   p.cs_bytes = (size_t)B * p.KT * CAM_KEYS * 4;
-  p.p_bytes = (size_t)B * p.KB * p.hs * p.ws * 16;
+  // the tallest band whose P fits the limit; several bands take 16-row multiples plus the carried row
+  const size_t row_bytes = (size_t)B * p.KB * p.ws * 16;   // one query row of P, every key block and image
+  p.band = p.prows = p.hs;
+  if (!single_band && row_bytes * p.hs > (size_t)limit) {
+    const long long fit = (long long)((size_t)limit / row_bytes) - 1;
+    const int band = (int)(fit < p.hs ? fit : p.hs) / CAM_TH * CAM_TH;
+    const size_t min_bytes = row_bytes * (p.hs < CAM_TH + 1 ? p.hs : CAM_TH + 1);
+    SE_REQUIRE(band >= CAM_TH, "attention workspace limit of " + std::to_string(limit) + " bytes is below the " + std::to_string(min_bytes) +
+                                   " bytes one band of " + std::to_string(CAM_TH) + " query rows needs at this size and batch");
+    p.band = band;
+    p.prows = band + 1;
+  }
+  p.n_bands = (p.hs + p.band - 1) / p.band;
+  p.p_bytes = row_bytes * p.prows;
   *out = p;
   return 0;
 }
@@ -529,40 +549,58 @@ int cam_forward_tc(const void* f_s2d, const float* mask_s, void* out_c8, const C
     cam_colscale_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(mask_s, colscale, B, pl.h, pl.w, pl.hs, pl.ws, pl.tk_x, pl.KT);
   }
   SE_CUDA_OK(cudaGetLastError());
-  {
-    CUtensorMap tmQ, tmK;
-    int rc = cam_map(&tmQ, f_s2d, pl.Ws, pl.Hs, 48, B, CAM_WR, CAM_HR, 48);
-    if (rc) return rc;
-    rc = cam_map(&tmK, fn, pl.Ws, pl.Hs, 48, B, CAM_WR, CAM_HR, CAM_CB);
-    if (rc) return rc;
-    CamSParams sp;
-    sp.hs = pl.hs; sp.ws = pl.ws;
-    sp.tq_x = pl.tq_x; sp.tq_n = pl.tq_n; sp.n_tiles = B * pl.tq_n;
-    sp.tk_x = pl.tk_x; sp.KT = pl.KT; sp.KB = pl.KB;
-    sp.colscale = colscale; sp.P = (__nv_bfloat16*)P;
-    void* args[3] = {&tmQ, &tmK, &sp};
-    rc = cam_launch((const void*)cam_s_kernel, sp.n_tiles, kCamSSmem, stream, args);
-    if (rc) return rc;
-  }
-  if (attn) {
-    const long long n = (long long)B * pl.hs * pl.ws * pl.hs * pl.ws;
-    cam_attn_export_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>((const __nv_bfloat16*)P, attn, B, pl.hs, pl.ws, pl.tk_x, pl.KB);
-    SE_CUDA_OK(cudaGetLastError());
-  }
-  {
-    CUtensorMap tmP, tmV;
-    int rc = cam_map(&tmP, P, pl.ws, pl.hs, pl.KB, B, CAM_WR, CAM_PV_TH + 1, 8);
-    if (rc) return rc;
-    rc = cam_map(&tmV, f_s2d, pl.Ws, pl.Hs, 48, B, 9, 9, CAM_CB);
-    if (rc) return rc;
-    CamPVParams pp;
-    pp.h = pl.h; pp.w = pl.w; pp.Hs = pl.Hs; pp.Ws = pl.Ws;
-    pp.to_x = pl.to_x; pp.to_n = pl.to_n; pp.n_tiles = B * pl.to_n;
-    pp.tk_x = pl.tk_x; pp.n_chunks = pl.KB / 8;
-    pp.out = (__nv_bfloat16*)out_c8;
-    void* args[3] = {&tmP, &tmV, &pp};
-    rc = cam_launch((const void*)cam_pv_kernel, pp.n_tiles, kCamPVSmem, stream, args);
-    if (rc) return rc;
+  SE_REQUIRE(!attn || pl.n_bands == 1, "the attention-map output needs a single band");
+  CUtensorMap tmQ, tmK, tmV;
+  int rc = cam_map(&tmQ, f_s2d, pl.Ws, pl.Hs, pl.Hs, 48, B, CAM_WR, CAM_HR, 48);
+  if (rc) return rc;
+  rc = cam_map(&tmK, fn, pl.Ws, pl.Hs, pl.Hs, 48, B, CAM_WR, CAM_HR, CAM_CB);
+  if (rc) return rc;
+  rc = cam_map(&tmV, f_s2d, pl.Ws, pl.Hs, pl.Hs, 48, B, 9, 9, CAM_CB);
+  if (rc) return rc;
+  const size_t prow_bytes = (size_t)pl.ws * 16;   // one query row of one key block of P
+  for (int q0 = 0, prev_qa = 0; q0 < pl.hs; q0 += pl.band) {
+    const int q1 = q0 + pl.band < pl.hs ? q0 + pl.band : pl.hs;
+    const int qa = q0 ? q0 - 1 : 0;   // query row held in buffer row 0
+    if (q0) {
+      // carry query row q0 - 1 (the previous band's last row) into buffer row 0 of every key block and image
+      char* Pb = (char*)P;
+      SE_CUDA_OK(cudaMemcpy2DAsync(Pb, (size_t)pl.prows * prow_bytes, Pb + (size_t)(q0 - 1 - prev_qa) * prow_bytes, (size_t)pl.prows * prow_bytes,
+                                   prow_bytes, (size_t)B * pl.KB, cudaMemcpyDeviceToDevice, stream));
+    }
+    prev_qa = qa;
+    {
+      CamSParams sp;
+      sp.hs = pl.hs; sp.ws = pl.ws;
+      sp.q0 = q0; sp.q1 = q1; sp.qa = qa; sp.prows = pl.prows;
+      sp.tq_x = pl.tq_x; sp.tq_n = pl.tq_x * ((q1 - q0 + CAM_TH - 1) / CAM_TH); sp.n_tiles = B * sp.tq_n;
+      sp.tk_x = pl.tk_x; sp.KT = pl.KT; sp.KB = pl.KB;
+      sp.colscale = colscale; sp.P = (__nv_bfloat16*)P;
+      void* args[3] = {&tmQ, &tmK, &sp};
+      rc = cam_launch((const void*)cam_s_kernel, sp.n_tiles, kCamSSmem, stream, args);
+      if (rc) return rc;
+    }
+    if (attn) {
+      const long long n = (long long)B * pl.hs * pl.ws * pl.hs * pl.ws;
+      cam_attn_export_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>((const __nv_bfloat16*)P, attn, B, pl.hs, pl.ws, pl.tk_x, pl.KB);
+      SE_CUDA_OK(cudaGetLastError());
+    }
+    {
+      // class rows [q0, q1) (the last band also row hs) read query rows [q0 - 1, q1): rows outside [qa, q1) are out of the
+      // map's bounds and load as zeros, as query rows -1 and hs must
+      const int y1 = q1 == pl.hs ? pl.Hs : q1;
+      CUtensorMap tmP;
+      rc = cam_map(&tmP, P, pl.ws, q1 - qa, pl.prows, pl.KB, B, CAM_WR, CAM_PV_TH + 1, 8);
+      if (rc) return rc;
+      CamPVParams pp;
+      pp.h = pl.h; pp.w = pl.w; pp.Hs = pl.Hs; pp.Ws = pl.Ws;
+      pp.y0 = q0; pp.y1 = y1; pp.qa = qa;
+      pp.to_x = pl.to_x; pp.to_n = pl.to_x * ((y1 - q0 + CAM_PV_TH - 1) / CAM_PV_TH); pp.n_tiles = B * pp.to_n;
+      pp.tk_x = pl.tk_x; pp.n_chunks = pl.KB / 8;
+      pp.out = (__nv_bfloat16*)out_c8;
+      void* args[3] = {&tmP, &tmV, &pp};
+      rc = cam_launch((const void*)cam_pv_kernel, pp.n_tiles, kCamPVSmem, stream, args);
+      if (rc) return rc;
+    }
   }
   SE_CUDA_OK(cudaGetLastError());
   return 0;

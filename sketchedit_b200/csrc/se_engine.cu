@@ -8,6 +8,7 @@
 #include <cuda_fp16.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <functional>
 #include <map>
@@ -31,6 +32,10 @@ void set_error(const std::string& msg) { g_err = msg; }
 const char* last_error() { return g_err.c_str(); }
 
 static thread_local int g_launches = 0;
+
+// bytes the contextual attention's quadratic temporaries (probabilities, logits) may take; se_set_attention_workspace_limit
+constexpr long long kDefaultAttnLimit = 16LL << 30;
+static std::atomic<long long> g_attn_limit{kDefaultAttnLimit};
 
 // ------------------------------------------------------------------------------------------ launch timing
 // se_timing_enable(1): every launch of a forward is bracketed by CUDA events on its stream and accounted to a kernel
@@ -529,6 +534,7 @@ struct Ctx {
   bool dry;
   Arena arena;
   int B;
+  long long attn_limit;   // se_set_attention_workspace_limit, read once per call (the dry and the real pass plan alike)
   int rc = 0;
   LaunchTag tag_;
   // label + algorithmic work of the NEXT launch (consumed by CK); see "launch timing" above
@@ -797,17 +803,17 @@ static int run_head(Ctx& c, char net, const std::string& name, const View& in, i
 static int run_cam_tc(Ctx& c, const View& f, const float* mask_s, void* out, float* attn_out) {
   SE_REQUIRE(f.c8 == 2 && f.C == 96, "tensor-core attention reads a 96-channel space-to-depth channel-blocked map");
   CamPlan pl;
-  int rc = cam_plan(c.B, f.H, f.W, &pl);
+  int rc = cam_plan(c.B, f.H, f.W, c.attn_limit, attn_out != nullptr, &pl);
   if (rc) return rc;
   Buf fn = c.get(pl.fn_bytes), cs = c.get(pl.cs_bytes), P = c.get(pl.p_bytes);
   if (g_timing && !c.dry) {
     const double L = (double)pl.hs * pl.ws;
     const double fl = 4.0 * c.B * L * L * 96 * 16;   // QK^T + PV (SURVEY.md 8d); the statistics sweep repeats QK^T: executed = 1.5x
     c.tag("cam_s_kernel + cam_pv_kernel (+ norm, colscale)|contextual attention", 1, fl, 1.5 * fl,
-          (double)c.B * f.H * f.W * 96 * 2 * 2 + 2.0 * (double)pl.p_bytes);
+          (double)c.B * f.H * f.W * 96 * 2 * 2 + 2.0 * (double)c.B * pl.KB * pl.hs * pl.ws * 16);   // P of all bands
   }
   CK(cam_forward_tc(f.p, mask_s, out, pl, fn.p, (float*)cs.p, P.p, attn_out, c.stream));
-  if (!c.dry) g_launches += 3;   // four kernels behind one call
+  if (!c.dry) g_launches += 1 + 2 * pl.n_bands;   // norm, colscale and an S + PV pair per band behind one call
   c.put(P); c.put(cs); c.put(fn);
   return 0;
 }
@@ -836,71 +842,94 @@ static int run_cam(Ctx& c, const View& f, const float* mask_s, void* out, int ou
   c.tag("cam_pack_k|attention key operand", 0, 0, 0, (double)B * h * w * C * c.esz() + (double)kbytes);
   CK(cam_pack_k(f.p, dt, (const float*)rnorm.p, kbuf.p, B, h, w, C, ws, L, Lpad, c.stream));
 
-  // ---- logits S[b, n, l] (fp32, row pitch Lpad), scaled by 10 * m_l in the GEMM epilogue
-  Buf sbuf = c.get((size_t)B * L * Lpad * 4);
-  {
-    ConvParams cp;
-    memset(&cp, 0, sizeof(cp));
-    cp.x = f.p; cp.in_dt = dt; cp.N = B; cp.Hi = h; cp.Wi = w; cp.Ci = C; cp.ldx = f.ld;
-    cp.Ho = hs; cp.Wo = ws; cp.stride = 2; cp.ntaps = 16;
-    for (int t = 0; t < 16; ++t) { cp.dy[t] = (int8_t)(t / 4); cp.dx[t] = (int8_t)(t % 4); }
-    cp.bias = nullptr; cp.Cout = L;
-    cp.y = sbuf.p; cp.out_dt = DT_F32; cp.Hout = hs; cp.Wout = ws; cp.ldo = Lpad; cp.choff = 0;
-    cp.osy = 1; cp.ooy = 0; cp.osx = 1; cp.oox = 0;
-    cp.epi = EPI_LINEAR; cp.scale = 10.0f; cp.colscale = (const float*)colm.p;
-    ClassW cw;
-    cw.ntaps = 16;
-    cw.CoutP = Lpad;
-    cw.w_direct = (float*)kbuf.p;
-    cp.w_img_stride = (long long)16 * C * Lpad;
-    c.tag("conv_direct_kernel|attention S=QK^T", 0, 2.0 * B * L * (double)L * C * 16,
-          2.0 * B * L * (double)L * C * 16, (double)B * h * w * C * c.esz() + (double)kbytes + (double)B * L * Lpad * 4);
-    CK(launch_conv(c, cp, cw));
+  // ---- bands of output class rows [y0, y1): S and P hold the query rows [qa, q1) those rows read (y0 - 1 .. y1 - 1, clipped
+  // to the patch grid; the boundary query row is computed by both bands that read it). R = class rows per band: the tallest
+  // whose S + P fit the attention workspace limit, every row when the attention map is wanted.
+  const int Hs = h / 2;
+  const size_t qrow_bytes = (size_t)B * ws * Lpad * (4 + c.esz());   // one query row of S (fp32) and P
+  int R = Hs;
+  if (!attn_out && qrow_bytes * hs > (size_t)c.attn_limit) {
+    R = (int)((size_t)c.attn_limit / qrow_bytes) - 1;
+    SE_REQUIRE(R >= 1, "attention workspace limit of " + std::to_string(c.attn_limit) + " bytes is below the " +
+                           std::to_string(qrow_bytes * (hs < 2 ? hs : 2)) + " bytes one band of 1 output row needs at this size and batch");
   }
-  c.put(kbuf);
-  c.put(rnorm);
-
-  // ---- softmax over keys -> P[b, n, 0..Lpad)
-  Buf pbuf = c.get((size_t)B * L * Lpad * c.esz());
-  c.tag("softmax_rows|attention", 0, 0, 0, (double)B * L * Lpad * (4 + c.esz()));
-  CK(softmax_rows((const float*)sbuf.p, Lpad, pbuf.p, dt, Lpad, (long long)B * L, L, c.stream));
-  if (attn_out) {
-    // cam_1 returns [B, L(keys), hs, ws]: transpose of P
-    // (small, test-only path: done with the generic layout kernel, P viewed as NHWC with C = L keys)
-    if (dt == DT_F32) CK(nhwc_to_nchw(pbuf.p, dt, attn_out, B, L, L, Lpad, 0, c.stream));
-    else CK(nhwc_to_nchw(pbuf.p, dt, attn_out, B, L, L, Lpad, 0, c.stream));
-  }
-  c.put(sbuf);
-  c.put(colm);
-
-  // ---- values + fold-sum
   const size_t per_pc_bytes = (size_t)B * 4 * Lpad * C * 4;   // values per sub-pixel class: fp32 [b][tap][key][c]
-  Buf vbuf = c.get(4 * per_pc_bytes);
-  c.tag("cam_pack_v|attention value operand", 0, 0, 0, (double)B * h * w * C * c.esz() + 4.0 * per_pc_bytes);
-  CK(cam_pack_v(f.p, dt, vbuf.p, B, h, w, C, ws, L, Lpad, c.stream));
-  for (int pc = 0; pc < 4; ++pc) {
-    ConvParams cp;
-    memset(&cp, 0, sizeof(cp));
-    cp.x = pbuf.p; cp.in_dt = dt; cp.N = B; cp.Hi = hs; cp.Wi = ws; cp.Ci = Lpad; cp.ldx = Lpad;
-    cp.Ho = h / 2; cp.Wo = w / 2; cp.stride = 1; cp.ntaps = 4;
-    for (int t = 0; t < 4; ++t) { cp.dy[t] = (int8_t)(-(t / 2)); cp.dx[t] = (int8_t)(-(t % 2)); }
-    cp.bias = nullptr; cp.Cout = C;
-    cp.y = out; cp.out_dt = dt; cp.Hout = h; cp.Wout = w; cp.ldo = out_c8 ? (C + 7) / 8 : out_ld; cp.choff = 0;
-    cp.out_c8 = out_c8;
-    cp.osy = 2; cp.ooy = pc / 2; cp.osx = 2; cp.oox = pc % 2;
-    cp.epi = EPI_LINEAR; cp.scale = 1.0f; cp.colscale = nullptr;
-    ClassW cw;
-    cw.ntaps = 4;
-    cw.CoutP = C;
-    cw.w_direct = reinterpret_cast<float*>((char*)vbuf.p + pc * per_pc_bytes);
-    cp.w_img_stride = (long long)4 * Lpad * C;
-    c.tag("conv_direct_kernel|attention out=fold(PV) class", 0,
-          2.0 * B * (h / 2) * (w / 2) * (double)C * L * 4, 2.0 * B * (h / 2) * (w / 2) * (double)C * L * 4,
-          ((double)B * L * Lpad + (double)B * 4 * Lpad * C + (double)B * (h / 2) * (w / 2) * C) * c.esz());
-    CK(launch_conv(c, cp, cw));
+  Buf vbuf;
+  for (int y0 = 0; y0 < Hs; y0 += R) {
+    const int y1 = y0 + R < Hs ? y0 + R : Hs;
+    const int qa = y0 ? y0 - 1 : 0, q1 = y1 < hs ? y1 : hs, nq = q1 - qa;
+    const bool last = y1 == Hs;
+    // ---- logits S[b, n, l] of query rows [qa, q1) (fp32, row pitch Lpad), scaled by 10 * m_l in the GEMM epilogue
+    Buf sbuf = c.get((size_t)B * nq * ws * Lpad * 4);
+    {
+      ConvParams cp;
+      memset(&cp, 0, sizeof(cp));
+      cp.x = (const char*)f.p + (size_t)2 * qa * w * f.ld * c.esz(); cp.in_dt = dt; cp.N = B; cp.Hi = h - 2 * qa; cp.Wi = w; cp.Ci = C; cp.ldx = f.ld;
+      cp.x_img_pitch = (long long)h * w * f.ld;
+      cp.Ho = nq; cp.Wo = ws; cp.stride = 2; cp.ntaps = 16;
+      for (int t = 0; t < 16; ++t) { cp.dy[t] = (int8_t)(t / 4); cp.dx[t] = (int8_t)(t % 4); }
+      cp.bias = nullptr; cp.Cout = L;
+      cp.y = sbuf.p; cp.out_dt = DT_F32; cp.Hout = nq; cp.Wout = ws; cp.ldo = Lpad; cp.choff = 0;
+      cp.osy = 1; cp.ooy = 0; cp.osx = 1; cp.oox = 0;
+      cp.epi = EPI_LINEAR; cp.scale = 10.0f; cp.colscale = (const float*)colm.p;
+      ClassW cw;
+      cw.ntaps = 16;
+      cw.CoutP = Lpad;
+      cw.w_direct = (float*)kbuf.p;
+      cp.w_img_stride = (long long)16 * C * Lpad;
+      const double nL = (double)nq * ws;
+      c.tag("conv_direct_kernel|attention S=QK^T", 0, 2.0 * B * nL * (double)L * C * 16,
+            2.0 * B * nL * (double)L * C * 16, (double)B * h * w * C * c.esz() + (double)kbytes + (double)B * nL * Lpad * 4);
+      CK(launch_conv(c, cp, cw));
+    }
+    if (last) {
+      c.put(kbuf);
+      c.put(rnorm);
+    }
+
+    // ---- softmax over keys -> P[b, n, 0..Lpad)
+    Buf pbuf = c.get((size_t)B * nq * ws * Lpad * c.esz());
+    c.tag("softmax_rows|attention", 0, 0, 0, (double)B * nq * ws * Lpad * (4 + c.esz()));
+    CK(softmax_rows((const float*)sbuf.p, Lpad, pbuf.p, dt, Lpad, (long long)B * nq * ws, L, c.stream));
+    if (attn_out) {
+      // cam_1 returns [B, L(keys), hs, ws]: transpose of P (one band)
+      // (small, test-only path: done with the generic layout kernel, P viewed as NHWC with C = L keys)
+      CK(nhwc_to_nchw(pbuf.p, dt, attn_out, B, L, L, Lpad, 0, c.stream));
+    }
+    c.put(sbuf);
+    if (last) c.put(colm);
+
+    // ---- values + fold-sum of class rows [y0, y1): query row y - a is P row y - a - qa
+    if (!vbuf.p) {
+      vbuf = c.get(4 * per_pc_bytes);
+      c.tag("cam_pack_v|attention value operand", 0, 0, 0, (double)B * h * w * C * c.esz() + 4.0 * per_pc_bytes);
+      CK(cam_pack_v(f.p, dt, vbuf.p, B, h, w, C, ws, L, Lpad, c.stream));
+    }
+    for (int pc = 0; pc < 4; ++pc) {
+      ConvParams cp;
+      memset(&cp, 0, sizeof(cp));
+      cp.x = pbuf.p; cp.in_dt = dt; cp.N = B; cp.Hi = nq; cp.Wi = ws; cp.Ci = Lpad; cp.ldx = Lpad;
+      cp.Ho = y1 - y0; cp.Wo = w / 2; cp.stride = 1; cp.ntaps = 4;
+      for (int t = 0; t < 4; ++t) { cp.dy[t] = (int8_t)(y0 - qa - t / 2); cp.dx[t] = (int8_t)(-(t % 2)); }
+      cp.bias = nullptr; cp.Cout = C;
+      cp.y = out; cp.out_dt = dt; cp.Hout = h; cp.Wout = w; cp.ldo = out_c8 ? (C + 7) / 8 : out_ld; cp.choff = 0;
+      cp.out_c8 = out_c8;
+      cp.osy = 2; cp.ooy = 2 * y0 + pc / 2; cp.osx = 2; cp.oox = pc % 2;
+      cp.epi = EPI_LINEAR; cp.scale = 1.0f; cp.colscale = nullptr;
+      ClassW cw;
+      cw.ntaps = 4;
+      cw.CoutP = C;
+      cw.w_direct = reinterpret_cast<float*>((char*)vbuf.p + pc * per_pc_bytes);
+      cp.w_img_stride = (long long)4 * Lpad * C;
+      const double ny = y1 - y0;
+      c.tag("conv_direct_kernel|attention out=fold(PV) class", 0,
+            2.0 * B * ny * (w / 2) * (double)C * L * 4, 2.0 * B * ny * (w / 2) * (double)C * L * 4,
+            ((double)B * nq * ws * Lpad + (double)B * 4 * Lpad * C + (double)B * ny * (w / 2) * C) * c.esz());
+      CK(launch_conv(c, cp, cw));
+    }
+    if (last) c.put(vbuf);
+    c.put(pbuf);
   }
-  c.put(vbuf);
-  c.put(pbuf);
   return 0;
 }
 
@@ -908,7 +937,7 @@ static int run_cam(Ctx& c, const View& f, const float* mask_s, void* out, int ou
 static int run_cam_split(Ctx& c, const float* f, int h, int w, int C, const float* mask_s, float* out) {
   CamSplitPlan pl;
   {
-    int rc = cam_split_plan(c.B, h, w, C, &pl);
+    int rc = cam_split_plan(c.B, h, w, C, c.attn_limit, &pl);
     if (rc) return rc;
   }
   Buf rnorm = c.get((size_t)c.B * C * 4), colm = c.get((size_t)c.B * pl.L * 4);
@@ -919,9 +948,9 @@ static int run_cam_split(Ctx& c, const float* f, int h, int w, int C, const floa
   CK(cam_colmask(mask_s, (float*)colm.p, c.B, h, w, pl.hs, pl.ws, 0.1f, c.stream));
   const double fl = 2.0 * c.B * (double)pl.L * pl.L * pl.KQ * 2.0;   // S and PV, algorithmic (one product each)
   c.tag("gemm_split_kernel x2 (split-half fp16 x3) + pack / softmax / fold|contextual attention", 1, fl, 3.0 * 2.0 * c.B * (double)pl.Mp * pl.Mp * pl.KQ * 2.0,
-        (double)c.B * h * w * C * 4 * 2 + 2.0 * pl.q_bytes * 2 + 2.0 * pl.s_bytes + 2.0 * pl.p_bytes + 2.0 * pl.o_bytes);
+        (double)c.B * h * w * C * 4 * 2 + 2.0 * pl.q_bytes * 2 + 2.0 * c.B * (double)pl.Mp * pl.Mp * 8 /* S + P of all bands */ + 2.0 * pl.o_bytes);
   CK(cam_forward_split(f, (const float*)rnorm.p, (const float*)colm.p, out, pl, q.p, kn.p, (float*)sb.p, pb.p, (float*)ob.p, c.stream));
-  if (!c.dry) g_launches += 4;   // pack, S GEMM, softmax, PV GEMM, fold behind one call
+  if (!c.dry) g_launches += 1 + 3 * pl.n_bands;   // pack, S GEMM + softmax + PV GEMM per band, fold behind one call
   c.put(ob); c.put(pb); c.put(sb); c.put(kn); c.put(q); c.put(colm); c.put(rnorm);
   return 0;
 }
@@ -1194,10 +1223,12 @@ static int with_arena(se_model* m, int prec, int B, cudaStream_t stream, F fn, s
     if (gs != stream) { SE_CUDA_OK(cudaEventRecord(m->bridge_out, gs)); SE_CUDA_OK(cudaStreamWaitEvent(stream, m->bridge_out, 0)); }
     return 0;
   };
+  const long long attn_limit = g_attn_limit.load();
   if (graphable) {
     for (int k = 0; k < 8; ++k) key.push_back((uintptr_t)m->opt[k]);
     key.push_back((uintptr_t)prec);
     key.push_back((uintptr_t)B);
+    key.push_back((uintptr_t)attn_limit);   // decides the attention's band plan
     for (auto& g : m->graphs)
       if (g.exec && g.arena == m->arena && g.key == key) {
         int rb = bridge_in();
@@ -1211,7 +1242,7 @@ static int with_arena(se_model* m, int prec, int B, cudaStream_t stream, F fn, s
       }
   }
   Ctx c;
-  c.m = m; c.stream = stream; c.prec = prec; c.B = B;
+  c.m = m; c.stream = stream; c.prec = prec; c.B = B; c.attn_limit = attn_limit;
   c.dry = true;
   c.arena.reset(nullptr);
   int rc = fn(c);
@@ -1622,6 +1653,12 @@ int se_outputs_to_uint8(const float* composed, const float* mask, int B, int H, 
                         void* stream) {
   SE_REQUIRE(composed && bgr_hwc && (mask || !mask_u8), "null tensor");
   return to_uint8(composed, mask, bgr_hwc, mask_u8, B, H, W, (cudaStream_t)stream);
+}
+
+int se_set_attention_workspace_limit(long long bytes) {
+  SE_REQUIRE(bytes >= 0, "attention workspace limit must be >= 0 bytes (0 = the default)");
+  g_attn_limit = bytes ? bytes : kDefaultAttnLimit;
+  return 0;
 }
 
 int se_last_launch_count(void) { return se::g_launches; }

@@ -16,6 +16,10 @@
 // ({8, 32 rows, 32 blocks}) the same buffer is an MN-major operand (LBO = 128 B = next 8 K, SBO = 512 B = next 8 N).
 // Values are stored times a power of two per operand (fp16 exponent range, see se_common.cuh kSplitActScale); the epilogue
 // undoes it exactly.
+//
+// Bands: S and P are Mp x Mp per image, so large maps run S GEMM -> softmax -> PV GEMM per band of query rows [n0, n0 + band)
+// (M rows of both GEMMs) through band-sized S and P buffers; O stays whole and is folded once. Each row's arithmetic does not
+// depend on the band split.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>
@@ -39,6 +43,7 @@ constexpr float kScaleP = 16384.0f;             // probabilities: p <= 1
 
 struct GemmSplitParams {
   int K;                       // multiple of GS_BK
+  int a_row0;                  // first A row (M tile 0 starts here)
   float* C;                    // fp32 [image][Mp][ldc]
   long long c_img_stride;
   int ldc;
@@ -120,8 +125,8 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         mbar_wait(&empty_bar[s], ph ^ 1u, 1);
         mbar_expect_tx(&full_bar[s], GS_STAGE);
         uint8_t* st = smem + (size_t)s * GS_STAGE;
-        tma_load_4d(st, &tmA, &full_bar[s], 0, mt * GS_BM, ks * (GS_BK / 8), img * 2);
-        tma_load_4d(st + GS_A_BYTES, &tmA, &full_bar[s], 0, mt * GS_BM, ks * (GS_BK / 8), img * 2 + 1);
+        tma_load_4d(st, &tmA, &full_bar[s], 0, p.a_row0 + mt * GS_BM, ks * (GS_BK / 8), img * 2);
+        tma_load_4d(st + GS_A_BYTES, &tmA, &full_bar[s], 0, p.a_row0 + mt * GS_BM, ks * (GS_BK / 8), img * 2 + 1);
         if (kBMN) {   // rows of the buffer are the K dimension here: box {8, 32 K rows, 32 N blocks}
           tma_load_4d(st + 2 * GS_A_BYTES, &tmB, &full_bar[s], 0, ks * GS_BK, nt * (GS_BN / 8), img * 2);
           tma_load_4d(st + 2 * GS_A_BYTES + GS_B_BYTES, &tmB, &full_bar[s], 0, ks * GS_BK, nt * (GS_BN / 8), img * 2 + 1);
@@ -191,21 +196,14 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 }
 
 // ------------------------------------------------------------------------------------------ softmax -> P (split-half, K-blocked)
-// S: fp32 [B][Mp][Np]; P: fp16 [B][2][Np / 8][Mp][8] (times kScaleP). Block = 8 rows (one warp each); rows >= L and keys >= L are 0.
-__global__ void __launch_bounds__(256) cam_split_softmax_kernel(const float* __restrict__ S, uint4* __restrict__ P, int L, int Mp, int Np) {
-  extern __shared__ float srow[];               // 8 x (Np + 4)
+// S: fp32 [B][rows][Np] (query rows n_base + r); P: fp16 [B][2][Np / 8][rows][8] (times kScaleP). Rows of any length, read
+// from global memory. Block = 8 rows (one warp each computes its row's statistics); query rows >= L and keys >= L are 0.
+__global__ void __launch_bounds__(256) cam_split_softmax_kernel(const float* __restrict__ S, uint4* __restrict__ P, int L, int rows, int n_base, int Np) {
   __shared__ float s_inv[8], s_max[8];
-  const int b = blockIdx.y, n0 = blockIdx.x * 8, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int pitch = Np + 4;
-  const float* src = S + ((size_t)b * Mp + n0) * Np;
-  for (int i = threadIdx.x; i < 8 * (Np / 4); i += 256) {
-    const int r = i / (Np / 4), c4 = i % (Np / 4);
-    const float4 v = reinterpret_cast<const float4*>(src + (size_t)r * Np)[c4];
-    *reinterpret_cast<float4*>(&srow[r * pitch + c4 * 4]) = v;
-  }
-  __syncthreads();
+  const int b = blockIdx.y, r0 = blockIdx.x * 8, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const float* src = S + ((size_t)b * rows + r0) * Np;
   {
-    const float* row = &srow[warp * pitch];
+    const float* row = src + (size_t)warp * Np;
     float mx = -INFINITY;
     for (int l = lane; l < L; l += 32) mx = fmaxf(mx, row[l]);
 #pragma unroll
@@ -220,10 +218,12 @@ __global__ void __launch_bounds__(256) cam_split_softmax_kernel(const float* __r
   const size_t LB = (size_t)Np / 8;
   for (int i = threadIdx.x; i < (int)LB * 8; i += 256) {
     const int lb = i >> 3, r = i & 7;
-    const int n = n0 + r;
+    const int n = n_base + r0 + r;
     uint32_t hi[4] = {0, 0, 0, 0}, lo[4] = {0, 0, 0, 0};
     if (n < L) {
-      const float* row = &srow[r * pitch + lb * 8];
+      const float4* row4 = reinterpret_cast<const float4*>(src + (size_t)r * Np + lb * 8);   // Np % 256 == 0: 32 B aligned
+      const float4 a0 = row4[0], a1 = row4[1];
+      const float row[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
       const float mx = s_max[r], inv = s_inv[r];
 #pragma unroll
       for (int k = 0; k < 8; k += 2) {
@@ -236,8 +236,8 @@ __global__ void __launch_bounds__(256) cam_split_softmax_kernel(const float* __r
         lo[k >> 1] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
       }
     }
-    P[((size_t)(b * 2) * LB + lb) * Mp + n] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-    P[((size_t)(b * 2 + 1) * LB + lb) * Mp + n] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+    P[((size_t)(b * 2) * LB + lb) * rows + r0 + r] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    P[((size_t)(b * 2 + 1) * LB + lb) * rows + r0 + r] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
   }
 }
 
@@ -293,7 +293,7 @@ static int gs_map(CUtensorMap* tm, const void* base, int rows, int blocks, int i
   return 0;
 }
 
-int cam_split_plan(int B, int h, int w, int C, CamSplitPlan* out) {
+int cam_split_plan(int B, int h, int w, int C, long long limit, CamSplitPlan* out) {
   SE_REQUIRE(h % 2 == 0 && w % 2 == 0 && h >= 4 && w >= 4 && C % 8 == 0, "attention map must be even-sized, >= 4, channels a multiple of 8");
   CamSplitPlan p;
   p.B = B; p.h = h; p.w = w; p.C = C;
@@ -302,8 +302,18 @@ int cam_split_plan(int B, int h, int w, int C, CamSplitPlan* out) {
   p.KQ = 16 * C;
   SE_REQUIRE(p.KQ % GS_BN == 0, "16 * channels must be a multiple of 256");   // N of the PV GEMM
   p.q_bytes = (size_t)B * 2 * (p.KQ / 8) * p.Mp * 16;
-  p.s_bytes = (size_t)B * p.Mp * p.Mp * 4;
-  p.p_bytes = (size_t)B * 2 * (p.Mp / 8) * p.Mp * 16;
+  // the tallest band (a multiple of the 128-row M tile) whose S and P fit the limit
+  const size_t row_bytes = (size_t)B * p.Mp * (4 + 4);   // one query row: S fp32 + P as fp16 hi and lo
+  p.band = p.Mp;
+  if (row_bytes * p.Mp > (size_t)limit) {
+    p.band = (int)((size_t)limit / row_bytes / GS_BM * GS_BM);
+    SE_REQUIRE(p.band >= GS_BM, "attention workspace limit of " + std::to_string(limit) + " bytes is below the " +
+                                     std::to_string(row_bytes * GS_BM) + " bytes one band of " + std::to_string(GS_BM) +
+                                     " query rows needs at this size and batch");
+  }
+  p.n_bands = (p.Mp + p.band - 1) / p.band;
+  p.s_bytes = (size_t)B * p.band * p.Mp * 4;
+  p.p_bytes = (size_t)B * 2 * (p.Mp / 8) * p.band * 16;
   p.o_bytes = (size_t)B * p.Mp * p.KQ * 4;
   *out = p;
   return 0;
@@ -335,39 +345,34 @@ int cam_forward_split(const float* f, const float* rnorm, const float* colmask, 
     cam_split_pack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(f, rnorm, (uint4*)Q, (uint4*)Kn, pl.h, pl.w, CB, pl.ws, L, Mp, total);
     SE_CUDA_OK(cudaGetLastError());
   }
-  {   // S = 10 * m_l * Q K^T
-    CUtensorMap tmA, tmB;
-    int rc = gs_map(&tmA, Q, Mp, pl.KQ / 8, 2 * B, GS_BM, GS_BK / 8);
-    if (rc) return rc;
-    rc = gs_map(&tmB, Kn, Mp, pl.KQ / 8, 2 * B, GS_BN, GS_BK / 8);
-    if (rc) return rc;
-    GemmSplitParams p;
-    p.K = pl.KQ; p.C = S; p.c_img_stride = (long long)Mp * Mp; p.ldc = Mp;
-    p.scale = 10.0f / (kScaleQ * kScaleK); p.colscale = colmask; p.ncs = L;
-    rc = gs_launch(false, tmA, tmB, p, Mp / GS_BN, Mp / GS_BM, B, stream);
-    if (rc) return rc;
-  }
-  {
-    const int smem = 8 * (Mp + 4) * 4;
-    static int smem_set = 0;
-    if (smem > smem_set) {
-      SE_CUDA_OK(cudaFuncSetAttribute(cam_split_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-      smem_set = smem;
+  CUtensorMap tmQ, tmK, tmV;
+  int rc = gs_map(&tmQ, Q, Mp, pl.KQ / 8, 2 * B, GS_BM, GS_BK / 8);
+  if (rc) return rc;
+  rc = gs_map(&tmK, Kn, Mp, pl.KQ / 8, 2 * B, GS_BN, GS_BK / 8);
+  if (rc) return rc;
+  rc = gs_map(&tmV, Q, Mp, pl.KQ / 8, 2 * B, GS_BK, GS_BN / 8);
+  if (rc) return rc;
+  for (int n0 = 0; n0 < Mp; n0 += pl.band) {
+    const int rows = n0 + pl.band < Mp ? pl.band : Mp - n0;   // a multiple of GS_BM (Mp is one of GS_BN)
+    {   // S[n0 + r] = 10 * m_l * Q K^T
+      GemmSplitParams p;
+      p.K = pl.KQ; p.a_row0 = n0; p.C = S; p.c_img_stride = (long long)rows * Mp; p.ldc = Mp;
+      p.scale = 10.0f / (kScaleQ * kScaleK); p.colscale = colmask; p.ncs = L;
+      rc = gs_launch(false, tmQ, tmK, p, Mp / GS_BN, rows / GS_BM, B, stream);
+      if (rc) return rc;
     }
-    cam_split_softmax_kernel<<<dim3(Mp / 8, B), 256, smem, stream>>>(S, (uint4*)P, L, Mp, Mp);
+    cam_split_softmax_kernel<<<dim3(rows / 8, B), 256, 0, stream>>>(S, (uint4*)P, L, rows, n0, Mp);
     SE_CUDA_OK(cudaGetLastError());
-  }
-  {   // O = P Q  (B operand = the query patches again, read MN-major)
-    CUtensorMap tmA, tmB;
-    int rc = gs_map(&tmA, P, Mp, Mp / 8, 2 * B, GS_BM, GS_BK / 8);
-    if (rc) return rc;
-    rc = gs_map(&tmB, Q, Mp, pl.KQ / 8, 2 * B, GS_BK, GS_BN / 8);
-    if (rc) return rc;
-    GemmSplitParams p;
-    p.K = Mp; p.C = O; p.c_img_stride = (long long)Mp * pl.KQ; p.ldc = pl.KQ;
-    p.scale = 1.0f / (kScaleP * kScaleQ); p.colscale = nullptr; p.ncs = 0;
-    rc = gs_launch(true, tmA, tmB, p, pl.KQ / GS_BN, Mp / GS_BM, B, stream);
-    if (rc) return rc;
+    {   // O[n0 + r] = P Q  (B operand = the query patches again, read MN-major)
+      CUtensorMap tmP;
+      rc = gs_map(&tmP, P, rows, Mp / 8, 2 * B, GS_BM, GS_BK / 8);
+      if (rc) return rc;
+      GemmSplitParams p;
+      p.K = Mp; p.a_row0 = 0; p.C = O + (size_t)n0 * pl.KQ; p.c_img_stride = (long long)Mp * pl.KQ; p.ldc = pl.KQ;
+      p.scale = 1.0f / (kScaleP * kScaleQ); p.colscale = nullptr; p.ncs = 0;
+      rc = gs_launch(true, tmP, tmV, p, pl.KQ / GS_BN, rows / GS_BM, B, stream);
+      if (rc) return rc;
+    }
   }
   {
     const long long total = (long long)B * pl.h * pl.w * (C / 4);

@@ -9,10 +9,13 @@ struct CamSplitPlan {
   int hs, ws, L;     // patch grid (4x4 patches, stride 2) and its size
   int Mp;            // L rounded up to 256: rows of every patch matrix, pitch of S
   int KQ;            // 16 * C: K of the S GEMM, N of the PV GEMM
+  int band;          // query rows (M rows of both GEMMs) per band: Mp (one band) or a multiple of 128
+  int n_bands;
   size_t q_bytes;    // query (= value) patches and normalised key patches, each
-  size_t s_bytes, p_bytes, o_bytes;
+  size_t s_bytes, p_bytes, o_bytes;   // S and P: one band
 };
-int cam_split_plan(int B, int h, int w, int C, CamSplitPlan* out);
+// limit: bytes S and P may take together (the quadratic buffers)
+int cam_split_plan(int B, int h, int w, int C, long long limit, CamSplitPlan* out);
 
 // f: fp32 NHWC [B][h][w][C]; rnorm: fp32 [B][C] (1 / plane norm); colmask: fp32 [B][L] (0 / 1 per key); out: fp32 NHWC [B][h][w][C].
 // Q, Kn (q_bytes each), S (s_bytes), P (p_bytes), O (o_bytes): workspace, 128 B aligned.

@@ -226,6 +226,12 @@ def contextual_attention(feat, mask_s, precision="bf16", want_attn=False):
     return (out, attn) if want_attn else out
 
 
+def set_attention_workspace_limit(nbytes):
+    """Bytes the contextual attention's L x L temporaries may take (process-wide; 0 = the default of 16 GiB). Larger
+    inputs run the attention in bands of query rows that fit; the results do not depend on the band split."""
+    _lib.check(_lib.load().se_set_attention_workspace_limit(int(nbytes)))
+
+
 def outputs_to_uint8(composed, mask):
     """test.py:25-27 on device -> (uint8 [B,H,W,3] BGR, uint8 [B,H,W])."""
     lib = _lib.load()
