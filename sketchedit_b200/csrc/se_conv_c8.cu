@@ -365,8 +365,7 @@ static int c8_dispatch(const C8Params& p, const CUtensorMap& tmA, int grid, int 
 static const int kGroupSmemMax = 222 * 1024;   // fused classes may use (almost) the whole opt-in window: weights of all classes + 2 halos
 
 int c8_configure_group(C8Group* G, int ncls, int ntaps, const int8_t (*dy)[8], const int8_t (*dx)[8], const int* ooy, const int* oox, int Ci, int Cout) {
-  static const bool off = getenv("SE_C8_NOGROUP") != nullptr;   // A/B switch for experiments
-  if (off || ncls < 2 || ncls > C8_MAX_CLS || ntaps > 8) return 1;
+  if (ncls < 2 || ncls > C8_MAX_CLS || ntaps > 8) return 1;
   int mn_y = 0, mx_y = 0, mn_x = 0, mx_x = 0;
   for (int c = 0; c < ncls; ++c)
     for (int t = 0; t < ntaps; ++t) {

@@ -90,27 +90,10 @@ static int timing_end(size_t slot, cudaStream_t st) {
 
 // ------------------------------------------------------------------------------------------ architecture
 struct Spec {
-  const char* name;
   int cin, cout, k, stride, rate;
   bool deconv;
   int act;   // 0 elu, 1 relu, -1 none
 };
-
-static std::vector<Spec> encoder(const std::string& pfx, int cin0, std::vector<std::string>& names) {
-  const int c = 48;
-  struct R { const char* n; int ci, co, k, s, r; };
-  const R rows[10] = {{"conv1", cin0, c, 5, 1, 1},          {"conv2_downsample", c / 2, 2 * c, 3, 2, 1},
-                      {"conv3", c, 2 * c, 3, 1, 1},         {"conv4_downsample", c, 4 * c, 3, 2, 1},
-                      {"conv5", 2 * c, 4 * c, 3, 1, 1},     {"conv6", 2 * c, 4 * c, 3, 1, 1},
-                      {"conv7_atrous", 2 * c, 4 * c, 3, 1, 2},  {"conv8_atrous", 2 * c, 4 * c, 3, 1, 4},
-                      {"conv9_atrous", 2 * c, 4 * c, 3, 1, 8},  {"conv10_atrous", 2 * c, 4 * c, 3, 1, 16}};
-  std::vector<Spec> v;
-  for (auto& r : rows) {
-    names.push_back(pfx + r.n);
-    v.push_back(Spec{nullptr, r.ci, r.co, r.k, r.s, r.r, false, 0});
-  }
-  return v;
-}
 
 struct ArchTable {
   std::vector<std::string> names;
@@ -118,12 +101,20 @@ struct ArchTable {
   void add(const std::string& n, int ci, int co, int k = 3, int s = 1, int r = 1, bool deconv = false, int act = 0) {
     if (co == 3) act = -1;   // reference utils.py:27
     names.push_back(n);
-    specs.push_back(Spec{nullptr, ci, co, k, s, r, deconv, act});
+    specs.push_back(Spec{ci, co, k, s, r, deconv, act});
   }
   void add_encoder(const std::string& pfx, int cin0) {
-    std::vector<std::string> nn;
-    auto v = encoder(pfx, cin0, nn);
-    for (size_t i = 0; i < v.size(); ++i) { names.push_back(nn[i]); specs.push_back(v[i]); }
+    const int c = 48;
+    add(pfx + "conv1", cin0, c, 5);
+    add(pfx + "conv2_downsample", c / 2, 2 * c, 3, 2);
+    add(pfx + "conv3", c, 2 * c);
+    add(pfx + "conv4_downsample", c, 4 * c, 3, 2);
+    add(pfx + "conv5", 2 * c, 4 * c);
+    add(pfx + "conv6", 2 * c, 4 * c);
+    add(pfx + "conv7_atrous", 2 * c, 4 * c, 3, 1, 2);
+    add(pfx + "conv8_atrous", 2 * c, 4 * c, 3, 1, 4);
+    add(pfx + "conv9_atrous", 2 * c, 4 * c, 3, 1, 8);
+    add(pfx + "conv10_atrous", 2 * c, 4 * c, 3, 1, 16);
   }
   void add_decoder(const std::string& pfx, int cin11, int cout17) {
     const int c = 48;
@@ -172,27 +163,30 @@ static ArchTable make_arch(char net) {
 }
 
 // ------------------------------------------------------------------------------------------ packed layers
+// the taps of one launch form: tap t reads the input at offset (dy, dx) from its position, starting at channel block cb
+struct Taps {
+  int n = 0;
+  int8_t dy[MAX_TAPS] = {}, dx[MAX_TAPS] = {}, cb[MAX_TAPS] = {};
+};
+
 struct ClassW {
-  int ntaps = 0;
-  int8_t dy[MAX_TAPS], dx[MAX_TAPS];
+  Taps direct;                 // CUDA-core form (se_conv_direct.cu) over NHWC input
   float* w_direct = nullptr;   // device fp32 [tap][Ci][CoutP]
   int CoutP = 0;
-  bool has_tc = false;
-  C8Layer c8;                  // se_conv_c8.cu: channel-blocked input (every stride-1 layer on the bf16 path)
-  bool use_c8 = false;
-  // stride-2 3x3 layers on the tensor-core path read a SPACE-TO-DEPTH channel-blocked input (written that way by
-  // the producing layer's epilogue): tap (ky,kx) of output (y,x) reads input row 2y+ky-1 = row y+c8dy of parity
-  // (ky-1)&1, i.e. a stride-1 read at offset (c8dy, c8dx) starting at channel block c8cb = parity * Ci/8
-  bool s2d = false;
-  int8_t c8dy[MAX_TAPS], c8dx[MAX_TAPS], c8cb[MAX_TAPS];
   int osy = 1, ooy = 0, osx = 1, oox = 0;
+  // channel-blocked wgmma forms (se_conv_c8.cu): every gated layer has them, the heads (CUDA-core only) do not
+  bool tc = false;
+  // stride-2 3x3 layers on the tensor-core path read a SPACE-TO-DEPTH channel-blocked input (written that way by
+  // the producing layer's epilogue): tap (ky,kx) of output (y,x) reads input row 2y+ky-1 = row y+dy of parity
+  // (ky-1)&1, i.e. a stride-1 read at offset (dy, dx) starting at channel block cb = parity * Ci/8
+  bool s2d = false;
+  Taps bf16;                   // bf16 form: the direct taps, in space-to-depth form on s2d layers
+  C8Layer c8;
   // split-half twin (SE_PREC_FP32_TC, DT_F16X2): every tap becomes three virtual taps (x_hi, w_hi), (x_hi, w_lo), (x_lo, w_hi); a
-  // virtual tap reads the hi or lo channel blocks of the input (s_cb) and its weight image holds fp16(w) or fp16(w - fp16(w))
+  // virtual tap reads the hi or lo channel blocks of the input (cb) and its weight image holds fp16(w) or fp16(w - fp16(w))
+  Taps split;
   C8Layer c8s;
-  bool has_split = false;
-  int s_ntaps = 0;
   float s_wscale = 1.0f;   // power of two the split-half weight images are multiplied by
-  int8_t s_dy[MAX_TAPS], s_dx[MAX_TAPS], s_cb[MAX_TAPS];
 };
 
 struct Layer {
@@ -272,45 +266,43 @@ struct EffTap { int dy, dx; std::vector<SrcTap> src; };
 static int pack_class(se_model* m, Layer& L, const std::vector<EffTap>& taps, ClassW& cw) {
   const Spec& s = L.spec;
   const int Ci = L.Ci, Cout = s.cout, k = s.k;
-  cw.ntaps = (int)taps.size();
-  SE_REQUIRE(cw.ntaps <= MAX_TAPS, "too many taps");
+  const int ntaps = (int)taps.size();
+  SE_REQUIRE(ntaps <= MAX_TAPS, "too many taps");
+  cw.direct.n = ntaps;
   cw.CoutP = (Cout + 3) / 4 * 4;
-  std::vector<float> weff((size_t)cw.ntaps * Ci * Cout, 0.0f);
-  for (int t = 0; t < cw.ntaps; ++t) {
-    cw.dy[t] = (int8_t)taps[t].dy;
-    cw.dx[t] = (int8_t)taps[t].dx;
+  std::vector<float> weff((size_t)ntaps * Ci * Cout, 0.0f);
+  for (int t = 0; t < ntaps; ++t) {
+    cw.direct.dy[t] = (int8_t)taps[t].dy;
+    cw.direct.dx[t] = (int8_t)taps[t].dx;
     for (auto& sk : taps[t].src)
       for (int ci = 0; ci < s.cin; ++ci)
         for (int co = 0; co < Cout; ++co)
           weff[((size_t)t * Ci + sk.ci_off + ci) * Cout + co] += L.w_host[(((size_t)co * s.cin + ci) * k + sk.ky) * k + sk.kx];
   }
   {
-    std::vector<float> wd((size_t)cw.ntaps * Ci * cw.CoutP, 0.0f);
-    for (int t = 0; t < cw.ntaps; ++t)
+    std::vector<float> wd((size_t)ntaps * Ci * cw.CoutP, 0.0f);
+    for (int t = 0; t < ntaps; ++t)
       for (int ci = 0; ci < Ci; ++ci)
         for (int co = 0; co < Cout; ++co) wd[((size_t)t * Ci + ci) * cw.CoutP + co] = weff[((size_t)t * Ci + ci) * Cout + co];
     int rc = upload(m, wd.data(), wd.size() * 4, (void**)&cw.w_direct);
     if (rc) return rc;
   }
-  cw.has_tc = (Ci % 8 == 0) && !L.is_head;
-  if (cw.has_tc) {
-    cw.s2d = (s.stride == 2 && s.k == 3 && s.rate == 1 && !s.deconv && !L.is_stem && Ci % 8 == 0);
-    cw.use_c8 = (s.stride == 1) || cw.s2d;
-    memset(cw.c8cb, 0, sizeof(cw.c8cb));
-    memcpy(cw.c8dy, cw.dy, sizeof(cw.c8dy));
-    memcpy(cw.c8dx, cw.dx, sizeof(cw.c8dx));
+  cw.tc = !L.is_head;
+  if (cw.tc) {
+    cw.s2d = (s.stride == 2 && s.k == 3 && s.rate == 1 && !s.deconv && !L.is_stem);
+    SE_REQUIRE(Ci % 8 == 0 && (s.stride == 1 || cw.s2d), "layer " + L.name + " has no tensor-core form");   // every gated layer of the two generators has one
+    cw.bf16 = cw.direct;
     if (cw.s2d) {
-      for (int t = 0; t < cw.ntaps; ++t) {
-        const int oy = cw.dy[t], ox = cw.dx[t];          // -1, 0, +1 (input row 2y + oy)
-        const int py = oy & 1, px = ox & 1;              // parity of that row / column
-        cw.c8dy[t] = (int8_t)((oy - py) / 2);            // -1 for oy = -1, else 0
-        cw.c8dx[t] = (int8_t)((ox - px) / 2);
-        cw.c8cb[t] = (int8_t)((py * 2 + px) * (Ci / 8));
+      for (int t = 0; t < ntaps; ++t) {
+        const int oy = cw.direct.dy[t], ox = cw.direct.dx[t];   // -1, 0, +1 (input row 2y + oy)
+        const int py = oy & 1, px = ox & 1;                     // parity of that row / column
+        cw.bf16.dy[t] = (int8_t)((oy - py) / 2);                // -1 for oy = -1, else 0
+        cw.bf16.dx[t] = (int8_t)((ox - px) / 2);
+        cw.bf16.cb[t] = (int8_t)((py * 2 + px) * (Ci / 8));
       }
     }
-    SE_REQUIRE(cw.use_c8, "layer " + L.name + " has no tensor-core form");   // every gated layer of the two generators has one
     {
-      int rc = c8_configure(&cw.c8, cw.ntaps, cw.c8dy, cw.c8dx, Ci, Cout, L.is_stem, cw.c8cb);
+      int rc = c8_configure(&cw.c8, ntaps, cw.bf16.dy, cw.bf16.dx, Ci, Cout, L.is_stem, cw.bf16.cb);
       if (rc) return rc;
     }
     TcWeights* tcp = &cw.c8.w;
@@ -339,37 +331,34 @@ static int pack_class(se_model* m, Layer& L, const std::vector<EffTap>& taps, Cl
     auto wval = [&](int t, int ci, int n) -> float { return ci < Ci ? weff[((size_t)t * Ci + ci) * Cout + n] * (n >= Cout / 2 ? 0.5f : 1.0f) : 0.0f; };
     int rc = build_images(*tcp, [&](int t, int ci, int n) -> uint16_t { return f32_to_bf16_rn(wval(t, ci, n)); });
     if (rc) return rc;
-    if (cw.use_c8) {
-      // ---- split-half twin: virtual tap 3t + p, p = 0: (x_hi, w_hi), 1: (x_hi, w_lo), 2: (x_lo, w_hi)
-      const int CB = L.is_stem ? 1 : Ci / 8;   // channel blocks of one half of the input (the packed stem input is one block)
-      cw.s_ntaps = 3 * cw.ntaps;
-      SE_REQUIRE(cw.s_ntaps <= MAX_TAPS, "too many virtual taps");
-      for (int t = 0; t < cw.ntaps; ++t)
-        for (int pp = 0; pp < 3; ++pp) {
-          cw.s_dy[3 * t + pp] = cw.c8dy[t];
-          cw.s_dx[3 * t + pp] = cw.c8dx[t];
-          cw.s_cb[3 * t + pp] = (int8_t)(2 * cw.c8cb[t] + (pp == 2 ? CB : 0));   // a parity group holds 2 * CB blocks
-        }
-      rc = c8_configure(&cw.c8s, cw.s_ntaps, cw.s_dy, cw.s_dx, Ci, Cout, L.is_stem, cw.s_cb);
-      if (rc) return rc;
-      // weights times a power of two (exact) that brings the largest one to [8192, 16384): the lo halves of all but negligible
-      // weights are then normal fp16 numbers (22 bits for the pair); the epilogue undoes it (se_common.cuh: kSplitActScale)
-      float wmax = 0.0f;
-      for (int t = 0; t < cw.ntaps; ++t)
-        for (int ci = 0; ci < Ci; ++ci)
-          for (int n = 0; n < Cout; ++n) wmax = std::max(wmax, std::fabs(wval(t, ci, n)));
-      int kw = 0;
-      if (wmax > 0.0f && std::isfinite(wmax)) kw = std::min(24, std::max(0, 13 - (int)std::floor(std::log2(wmax))));
-      cw.s_wscale = std::ldexp(1.0f, kw);
-      auto half_bits = [](float v) -> uint16_t { return __half_as_ushort(__float2half_rn(v)); };
-      rc = build_images(cw.c8s.w, [&](int vt, int ci, int n) -> uint16_t {
-        const float w = wval(vt / 3, ci, n) * cw.s_wscale;
-        const float hi = __half2float(__float2half_rn(w));
-        return (vt % 3) == 1 ? half_bits(w - hi) : half_bits(w);
-      });
-      if (rc) return rc;
-      cw.has_split = true;
-    }
+    // ---- split-half twin: virtual tap 3t + p, p = 0: (x_hi, w_hi), 1: (x_hi, w_lo), 2: (x_lo, w_hi)
+    const int CB = L.is_stem ? 1 : Ci / 8;   // channel blocks of one half of the input (the packed stem input is one block)
+    cw.split.n = 3 * ntaps;
+    SE_REQUIRE(cw.split.n <= MAX_TAPS, "too many virtual taps");
+    for (int t = 0; t < ntaps; ++t)
+      for (int pp = 0; pp < 3; ++pp) {
+        cw.split.dy[3 * t + pp] = cw.bf16.dy[t];
+        cw.split.dx[3 * t + pp] = cw.bf16.dx[t];
+        cw.split.cb[3 * t + pp] = (int8_t)(2 * cw.bf16.cb[t] + (pp == 2 ? CB : 0));   // a parity group holds 2 * CB blocks
+      }
+    rc = c8_configure(&cw.c8s, cw.split.n, cw.split.dy, cw.split.dx, Ci, Cout, L.is_stem, cw.split.cb);
+    if (rc) return rc;
+    // weights times a power of two (exact) that brings the largest one to [8192, 16384): the lo halves of all but negligible
+    // weights are then normal fp16 numbers (22 bits for the pair); the epilogue undoes it (se_common.cuh: kSplitActScale)
+    float wmax = 0.0f;
+    for (int t = 0; t < ntaps; ++t)
+      for (int ci = 0; ci < Ci; ++ci)
+        for (int n = 0; n < Cout; ++n) wmax = std::max(wmax, std::fabs(wval(t, ci, n)));
+    int kw = 0;
+    if (wmax > 0.0f && std::isfinite(wmax)) kw = std::min(24, std::max(0, 13 - (int)std::floor(std::log2(wmax))));
+    cw.s_wscale = std::ldexp(1.0f, kw);
+    auto half_bits = [](float v) -> uint16_t { return __half_as_ushort(__float2half_rn(v)); };
+    rc = build_images(cw.c8s.w, [&](int vt, int ci, int n) -> uint16_t {
+      const float w = wval(vt / 3, ci, n) * cw.s_wscale;
+      const float hi = __half2float(__float2half_rn(w));
+      return (vt % 3) == 1 ? half_bits(w - hi) : half_bits(w);
+    });
+    if (rc) return rc;
   }
   return 0;
 }
@@ -440,7 +429,7 @@ static int pack_layer(se_model* m, Layer& L) {
   }
   // fuse the classes into as few launches as shared memory allows: all four (48->48), else one launch per output-row
   // parity (96->96: classes {0,1} and {2,3}); the per-class launches stay available as the fallback
-  if (L.cls[0].has_tc && L.cls[0].use_c8 && L.cls[0].c8.resident && L.cls[0].c8.mode == C8_HALO) {
+  if (L.cls[0].tc && L.cls[0].c8.resident && L.cls[0].c8.mode == C8_HALO) {
     for (int per : {4, 2}) {
       std::vector<C8Group> gs;
       bool ok = true;
@@ -449,11 +438,11 @@ static int pack_layer(se_model* m, Layer& L) {
         int ooy[C8_MAX_CLS], oox[C8_MAX_CLS];
         for (int k = 0; k < per; ++k) {
           const ClassW& cw = L.cls[g0 + k];
-          for (int t = 0; t < cw.ntaps; ++t) { dy[k][t] = cw.dy[t]; dx[k][t] = cw.dx[t]; }
+          for (int t = 0; t < cw.bf16.n; ++t) { dy[k][t] = cw.bf16.dy[t]; dx[k][t] = cw.bf16.dx[t]; }
           ooy[k] = cw.ooy; oox[k] = cw.oox;
         }
         C8Group G;
-        if (c8_configure_group(&G, per, L.cls[0].ntaps, dy, dx, ooy, oox, L.Ci, s.cout)) { ok = false; break; }
+        if (c8_configure_group(&G, per, L.cls[0].bf16.n, dy, dx, ooy, oox, L.Ci, s.cout)) { ok = false; break; }
         const C8Layer& c0 = L.cls[g0].c8;
         ok = (G.geo.w.r64 == c0.w.r64 && G.geo.w.r32 == c0.w.r32 && G.geo.w.NT == c0.w.NT && G.cls_bytes == (int)tc_weight_bytes_per_image(c0.w));
         if (!ok) break;
@@ -527,6 +516,21 @@ struct Arena {
 
 struct Buf { void* p = nullptr; size_t bytes = 0; };
 
+// activation view. c8 == 0: NHWC, channels [0,C) at pixel pitch ld. c8 == 1: [B][ld blocks][H][W][8], the view's
+// channels start at block cb_off. c8 == 2: channel-blocked space-to-depth, [B][ld blocks][H/2][W/2][8] with the four
+// (row, column) parity groups of ld / 4 blocks one after the other (H, W: the full-resolution size)
+struct View { void* p; int H, W, C, ld; int c8 = 0; int cb_off = 0; };
+static inline View nhwc(void* p, int H, int W, int C, int ld) { return View{p, H, W, C, ld, 0, 0}; }
+static inline View c8view(void* p, int H, int W, int C, int cbtot, int cb_off = 0) { return View{p, H, W, C, cbtot, 1, cb_off}; }
+static inline View s2dview(void* p, int H, int W, int C, int cbtot, int cb_off = 0) { return View{p, H, W, C, cbtot, 2, cb_off}; }
+
+// an activation: its view plus the workspace buffer it owns (own.p == nullptr: a view into a buffer owned elsewhere)
+struct Act {
+  View v;
+  Buf own;
+  Act borrow() const { return Act{v, Buf()}; }
+};
+
 struct Ctx {
   se_model* m;
   cudaStream_t stream;
@@ -535,7 +539,6 @@ struct Ctx {
   Arena arena;
   int B;
   long long attn_limit;   // se_set_attention_workspace_limit, read once per call (the dry and the real pass plan alike)
-  int rc = 0;
   LaunchTag tag_;
   // label + algorithmic work of the NEXT launch (consumed by CK); see "launch timing" above
   void tag(const std::string& name, int tensor, double flops_alg, double flops_exec, double bytes_alg) {
@@ -549,6 +552,14 @@ struct Ctx {
   size_t esz() const { return (prec == SE_PREC_FP32_EXACT || split()) ? 4 : 2; }
   Buf get(size_t bytes) { Buf b; b.bytes = bytes; b.p = arena.alloc(bytes); return b; }
   void put(Buf& b) { if (b.p) arena.release(b.p, b.bytes); b.p = nullptr; }
+  void put(Act& a) { put(a.own); }
+  size_t act_bytes(int H, int W, int C, int c8) const { return c8 ? (size_t)B * ((C + 7) / 8) * H * W * 16 * sp() : (size_t)B * H * W * C * esz(); }
+  // a dense activation of layout c8 at p
+  View dense(void* p, int H, int W, int C, int c8) const {
+    if (c8 == 2) return s2dview(p, H, W, C, 4 * (C / 8) * sp());   // split-half: twice the blocks per parity group
+    if (c8 == 1) return c8view(p, H, W, C, (C + 7) / 8 * sp());
+    return nhwc(p, H, W, C, C);
+  }
 };
 
 #define CK(expr)                                                    \
@@ -556,21 +567,14 @@ struct Ctx {
     if (!c.dry) {                                                   \
       size_t _slot = 0;                                             \
       const bool _timed = g_timing;                                 \
-      if (_timed) { int _rt = timing_begin(c.tag_, c.stream, &_slot); if (_rt) { c.rc = _rt; return _rt; } } \
+      if (_timed) { int _rt = timing_begin(c.tag_, c.stream, &_slot); if (_rt) return _rt; } \
       c.tag_.set = false;                                           \
       int _rc = (expr);                                             \
-      if (_rc) { c.rc = _rc; return _rc; }                          \
-      if (_timed) { int _rt = timing_end(_slot, c.stream); if (_rt) { c.rc = _rt; return _rt; } } \
+      if (_rc) return _rc;                                          \
+      if (_timed) { int _rt = timing_end(_slot, c.stream); if (_rt) return _rt; } \
       ++g_launches;                                                 \
     }                                                               \
   } while (0)
-
-// activation view. c8 == 0: NHWC, channels [0,C) at pixel pitch ld. c8 == 1: [B][ld blocks][H][W][8], the view's
-// channels start at block cb_off.
-struct View { void* p; int H, W, C, ld; int c8 = 0; int cb_off = 0; };
-static inline View nhwc(void* p, int H, int W, int C, int ld) { View v; v.p = p; v.H = H; v.W = W; v.C = C; v.ld = ld; return v; }
-static inline View c8view(void* p, int H, int W, int C, int cbtot, int cb_off) { View v; v.p = p; v.H = H; v.W = W; v.C = C; v.ld = cbtot; v.c8 = 1; v.cb_off = cb_off; return v; }
-static inline size_t act_bytes(const struct Ctx& c, int H, int W, int C, int c8);
 
 static Layer* find_layer(se_model* m, char net, const std::string& name) {
   auto it = m->layers.find(std::string(1, net) + "." + name);
@@ -586,24 +590,12 @@ static Layer* find_ready(se_model* m, char net, const std::string& name) {
   return L;
 }
 
-static int launch_conv(Ctx& c, const ConvParams& cp, const ClassW& cw) {
-  if (c.split() && cw.has_split) return c8_launch(cp, cw.c8s, c.stream);
-  if (c.prec == SE_PREC_BF16_TC && cw.has_tc) return c8_launch(cp, cw.c8, c.stream);
-  ConvParams d = cp;
-  d.w = cw.w_direct;
-  return direct_launch(d, cw.CoutP, c.prec == SE_PREC_FP32_EXACT, c.stream);
-}
-
-// one gated conv / deconv layer: in (Hi x Wi x Ci) -> out view (channels written at [choff, choff+cout_g))
-// layout a layer wants for its input on the bf16 tensor-core path (stride-2 layers read NHWC, the rest C8)
-// 0 NHWC, 1 channel-blocked (C8), 2 channel-blocked space-to-depth (stride-2 layers)
+// layout a layer wants for its input: 0 NHWC (CUDA-core path, heads), 1 channel-blocked (C8), 2 channel-blocked
+// space-to-depth (stride-2 layers on the tensor-core path)
 static int wants_c8(const Ctx& c, const Layer& L) {
   if (!c.tc() || L.is_head) return 0;
   if (L.spec.stride == 1) return 1;
   return (!L.cls.empty() && L.cls[0].s2d) ? 2 : 0;
-}
-static inline size_t act_bytes(const Ctx& c, int H, int W, int C, int c8) {
-  return c8 ? (size_t)c.B * ((C + 7) / 8) * H * W * 16 * c.sp() : (size_t)c.B * H * W * C * c.esz();
 }
 // the packed 8-channel network input (zero-padded rows of stem_wp(W) pixels): NHWC with C = ld = 8 for the CUDA-core
 // kernels, the same bytes seen as one channel block of width stem_wp(W) for the tensor-core path
@@ -612,6 +604,7 @@ static View stem_view(const Ctx& c, void* p, int H, int W) {
   return nhwc(p, H, W, 8, 8);
 }
 
+// one gated conv / deconv layer: in (Hi x Wi x Ci) -> out (channels written at [choff, choff+cout_g), layout out_c8)
 static int run_layer(Ctx& c, Layer& L, const View& in, void* out, int ldo, int choff, int out_c8 = 0) {
   SE_REQUIRE(in.c8 == wants_c8(c, L), "activation layout mismatch at layer " + L.name);
   const Spec& s = L.spec;
@@ -639,11 +632,14 @@ static int run_layer(Ctx& c, Layer& L, const View& in, void* out, int ldo, int c
     }
     cp.out_c8 = out_c8;
     cp.Ho = Ho; cp.Wo = Wo; cp.stride = s.deconv ? 1 : s.stride;
-    cp.ntaps = cw.ntaps;
-    memcpy(cp.dy, cw.dy, sizeof(cp.dy));
-    memcpy(cp.dx, cw.dx, sizeof(cp.dx));
+    // the taps of the form this mode launches (the tensor-core forms are already in space-to-depth form where that applies)
+    const Taps& tp = split ? cw.split : c.tc() ? cw.bf16 : cw.direct;
+    cp.ntaps = tp.n;
+    memcpy(cp.dy, tp.dy, sizeof(cp.dy));
+    memcpy(cp.dx, tp.dx, sizeof(cp.dx));
+    memcpy(cp.tap_cb, tp.cb, sizeof(cp.tap_cb));
     if (split) {
-      SE_REQUIRE(cw.has_split && in.c8 && out_c8, "split-half mode runs on channel-blocked activations (layer " + L.name + ")");
+      SE_REQUIRE(in.c8 && out_c8, "split-half mode runs on channel-blocked activations (layer " + L.name + ")");
       cp.f16x2 = 1;
       // hi blocks first, lo blocks after them: per image (channel-blocked) or per parity group (space-to-depth)
       cp.out_split_stride = out_c8 == 2 ? (long long)(ldo / 8) * (Ho * cw.osy / 2) * (Wo * cw.osx / 2) : (long long)(ldo / 2) * (Ho * cw.osy) * (Wo * cw.osx);
@@ -651,15 +647,6 @@ static int run_layer(Ctx& c, Layer& L, const View& in, void* out, int ldo, int c
     if (in.c8 == 2) {   // space-to-depth input: a stride-1 problem on the half-resolution grid with per-tap parity blocks
       SE_REQUIRE(cw.s2d && in.H % 2 == 0 && in.W % 2 == 0, "space-to-depth input at layer " + L.name);
       cp.Hi = in.H / 2; cp.Wi = in.W / 2; cp.stride = 1;
-      memcpy(cp.dy, cw.c8dy, sizeof(cp.dy));
-      memcpy(cp.dx, cw.c8dx, sizeof(cp.dx));
-      memcpy(cp.tap_cb, cw.c8cb, sizeof(cp.tap_cb));
-    }
-    if (split) {        // the virtual taps of the split-half twin (already in space-to-depth form where that applies)
-      cp.ntaps = cw.s_ntaps;
-      memcpy(cp.dy, cw.s_dy, sizeof(cp.dy));
-      memcpy(cp.dx, cw.s_dx, sizeof(cp.dx));
-      memcpy(cp.tap_cb, cw.s_cb, sizeof(cp.tap_cb));
     }
     cp.w = nullptr; cp.w_img_stride = 0;
     cp.bias = L.bias; cp.bias_host = L.b_host.data(); cp.Cout = s.cout;
@@ -685,23 +672,17 @@ static int run_layer(Ctx& c, Layer& L, const View& in, void* out, int ldo, int c
       const double f_alg = 2.0 * pos * s.cout * cin_alg * (s.deconv ? 9.0 : (double)s.k * s.k);
       const double f_exec = 2.0 * pos * s.cout * cin_alg * (s.deconv ? 4.0 : (double)s.k * s.k) * (split ? 3.0 : 1.0);   // split-half: 3 products per tap
       const double bytes = ((double)c.B * in.H * in.W * (L.fused_pair ? 8.0 : (double)s.cin) / ncls + pos * (s.cout / 2) + (double)s.cout * s.cin * s.k * s.k / ncls) * c.esz();
-      const bool tcp = c.tc() && cw.has_tc;
       char buf[160];
-      snprintf(buf, sizeof(buf), "%s|%s %d->%d k%d s%d d%d @%dx%d", tcp ? (split ? "conv_c8_kernel (split-half fp16 x3)" : "conv_c8_kernel") : "conv_direct_kernel",
+      snprintf(buf, sizeof(buf), "%s|%s %d->%d k%d s%d d%d @%dx%d", c.tc() ? (split ? "conv_c8_kernel (split-half fp16 x3)" : "conv_c8_kernel") : "conv_direct_kernel",
                s.deconv ? (grp ? (grp->ncls == 4 ? "deconv (4 classes fused)" : "deconv (2 classes fused)") : "deconv-class") : (L.fused_pair ? "stem pair" : "conv"), s.cin, s.cout, s.k, s.stride, s.rate, Ho * cw.osy, Wo * cw.osx);
-      c.tag(buf, tcp ? 1 : 0, f_alg, f_exec, bytes);
+      c.tag(buf, c.tc() ? 1 : 0, f_alg, f_exec, bytes);
     }
-    if (grp) CK(c8_launch(cp, cw.c8, c.stream, grp));
-    else CK(launch_conv(c, cp, cw));
-  }
-  static const bool dbg = getenv("SE_DEBUG_NAN") != nullptr;
-  if (dbg && !c.dry && c.act_dt() == DT_BF16 && !split) {
-    const int cg = s.cout / 2, Hout = Ho * L.cls[0].osy, Wout = Wo * L.cls[0].osx;
-    const long long n_out = out_c8 ? (long long)c.B * ldo * Hout * Wout * 8 : (long long)c.B * Hout * Wout * ldo;
-    const long long n_in = in.c8 ? (long long)c.B * in.ld * in.H * (L.is_stem ? stem_wp(in.W) : in.W) * 8 / (in.c8 == 2 ? 4 : 1) : (long long)c.B * in.H * in.W * in.ld;
-    fprintf(stderr, "[nan] %-28s in %dx%d c8=%d ld=%d nonfinite_in=%lld | out %dx%d c8=%d ld=%d choff=%d cg=%d nonfinite_out(buffer)=%lld use_c8=%d mode=%d res=%d\n", L.name.c_str(), in.H, in.W,
-            in.c8, in.ld, count_nonfinite_bf16(in.p, n_in, c.stream), Hout, Wout, out_c8, ldo, choff, cg, count_nonfinite_bf16(out, n_out, c.stream), (int)L.cls[0].use_c8,
-            L.cls[0].c8.mode, (int)L.cls[0].c8.resident);
+    if (split) CK(c8_launch(cp, cw.c8s, c.stream));
+    else if (c.tc()) CK(c8_launch(cp, cw.c8, c.stream, grp));
+    else {
+      cp.w = cw.w_direct;
+      CK(direct_launch(cp, cw.CoutP, c.prec == SE_PREC_FP32_EXACT, c.stream));
+    }
   }
   return 0;
 }
@@ -711,54 +692,51 @@ static void out_dims(const Spec& s, int H, int W, int* Ho, int* Wo) {
   else { *Ho = (H + s.stride - 1) / s.stride; *Wo = (W + s.stride - 1) / s.stride; }
 }
 
+// where the last layer of a chain writes: into p (ld pixel pitch / channel blocks, channel offset choff) when given, else
+// into a fresh workspace buffer. c8: layout of the result, -1 = the mode's own (channel-blocked on the tensor-core path)
+struct Dst { void* p = nullptr; int ld = 0, choff = 0, c8 = -1; };
+
 // run a chain of gated layers; intermediate buffers come from the arena. Each intermediate is written in the layout
-// its consumer wants. The last layer writes to (final_out, final_ld, final_choff, final_c8) when given, else to a
-// fresh buffer (layout final_c8) returned in *res.
-static int run_chain(Ctx& c, char net, const std::vector<std::string>& names, View in, bool free_in, Buf in_buf, View* res, Buf* res_buf,
-                     void* final_out = nullptr, int final_ld = 0, int final_choff = 0, int final_c8 = -1) {
-  View cur = in;
-  Buf cur_buf = in_buf;
-  bool cur_owned = free_in;
-  if (final_c8 < 0) final_c8 = c.tc() ? 1 : 0;
+// its consumer wants. The chain releases `in` when it owns its buffer; *out (may be null when dst.p is given) receives
+// the result.
+static int run_chain(Ctx& c, char net, const std::vector<std::string>& names, Act in, Act* out, Dst dst = Dst()) {
+  Act cur = in;
+  if (dst.c8 < 0) dst.c8 = c.tc() ? 1 : 0;
   for (size_t i = 0; i < names.size(); ++i) {
     Layer* L = find_ready(c.m, net, names[i]);
     SE_REQUIRE(L != nullptr, "unknown or unloaded layer " + names[i] + ": " + last_error());
     int Ho, Wo;
-    out_dims(L->spec, cur.H, cur.W, &Ho, &Wo);
+    out_dims(L->spec, cur.v.H, cur.v.W, &Ho, &Wo);
     const int cg = L->spec.cout / 2;
     const bool last = (i + 1 == names.size());
-    View nxt;
-    Buf nb;
-    if (last && final_out) {
-      nxt = final_c8 ? c8view(final_out, Ho, Wo, cg, final_ld, final_choff / 8) : nhwc(final_out, Ho, Wo, cg, final_ld);
-      int rc = run_layer(c, *L, cur, final_out, final_ld, final_choff, final_c8);
+    Act nxt;
+    if (last && dst.p) {
+      nxt.v = dst.c8 ? c8view(dst.p, Ho, Wo, cg, dst.ld, dst.choff / 8) : nhwc(dst.p, Ho, Wo, cg, dst.ld);
+      int rc = run_layer(c, *L, cur.v, dst.p, dst.ld, dst.choff, dst.c8);
       if (rc) return rc;
     } else {
-      int oc8 = final_c8;
+      int oc8 = dst.c8;
       if (!last) {
         Layer* nx = find_ready(c.m, net, names[i + 1]);
         SE_REQUIRE(nx != nullptr, "unknown or unloaded layer " + names[i + 1]);
         oc8 = wants_c8(c, *nx);
       }
-      nb = c.get(act_bytes(c, Ho, Wo, cg, oc8));
-      nxt = oc8 ? c8view(nb.p, Ho, Wo, cg, (cg + 7) / 8 * c.sp(), 0) : nhwc(nb.p, Ho, Wo, cg, cg);
-      if (oc8 == 2) { nxt.c8 = 2; nxt.ld = 4 * (cg / 8) * c.sp(); }   // [N][4*cg/8][Ho/2][Wo/2][8] (split-half: twice the blocks per parity)
-      int rc = run_layer(c, *L, cur, nb.p, oc8 ? nxt.ld : cg, 0, oc8);
+      nxt.own = c.get(c.act_bytes(Ho, Wo, cg, oc8));
+      nxt.v = c.dense(nxt.own.p, Ho, Wo, cg, oc8);
+      int rc = run_layer(c, *L, cur.v, nxt.own.p, nxt.v.ld, 0, oc8);
       if (rc) return rc;
     }
-    if (cur_owned) c.put(cur_buf);
+    c.put(cur);
     cur = nxt;
-    cur_buf = nb;
-    cur_owned = !(last && final_out);
   }
-  if (res) *res = cur;
-  if (res_buf) *res_buf = cur_buf;
+  if (out) *out = cur;
   return 0;
 }
 
-static std::vector<std::string> with_prefix(const std::string& pfx, std::initializer_list<const char*> l) {
+// pfx + each name of l from the skip-th on
+static std::vector<std::string> with_prefix(const std::string& pfx, std::initializer_list<const char*> l, int skip = 0) {
   std::vector<std::string> v;
-  for (auto s : l) v.push_back(pfx + s);
+  for (auto s = l.begin() + skip; s != l.end(); ++s) v.push_back(pfx + *s);
   return v;
 }
 
@@ -785,12 +763,13 @@ static int run_head(Ctx& c, char net, const std::string& name, const View& in, i
                   c.m->opt[SE_OPT_NO_MASK_COARSE], stem_wp(in.W), STEM_PADL, out_bs, msoft_bs, out_u8, c.stream));
     return 0;
   }
-  if (in.c8 == 1 && c.act_dt() == DT_BF16) {
+  if (in.c8) {
+    SE_REQUIRE(in.c8 == 1 && c.act_dt() == DT_BF16, "a channel-blocked head input is bf16");
     CK(head_c8(in.p, L->w_head_host.data(), L->b_host.data(), L->spec.cout, c.B, in.H, in.W, mode, img, mask_bin, mask_soft, out_nchw, out2,
                out_pack8, c.m->opt[SE_OPT_NO_MASK_COARSE], stem_wp(in.W), STEM_PADL, out_bs, msoft_bs, out_u8, c.stream));
     return 0;
   }
-  CK(head(in.p, c.act_dt(), in.c8, L->w_head, L->bias, L->spec.cout, c.B, in.H, in.W, mode, img, mask_bin, mask_soft, out_nchw, out2,
+  CK(head(in.p, c.act_dt(), L->w_head, L->bias, L->spec.cout, c.B, in.H, in.W, mode, img, mask_bin, mask_soft, out_nchw, out2,
           out_pack8, c.m->opt[SE_OPT_NO_MASK_COARSE], stem_wp(in.W), STEM_PADL, out_bs, msoft_bs, out_u8, c.stream));
   return 0;
 }
@@ -872,15 +851,11 @@ static int run_cam(Ctx& c, const View& f, const float* mask_s, void* out, int ou
       cp.y = sbuf.p; cp.out_dt = DT_F32; cp.Hout = nq; cp.Wout = ws; cp.ldo = Lpad; cp.choff = 0;
       cp.osy = 1; cp.ooy = 0; cp.osx = 1; cp.oox = 0;
       cp.epi = EPI_LINEAR; cp.scale = 10.0f; cp.colscale = (const float*)colm.p;
-      ClassW cw;
-      cw.ntaps = 16;
-      cw.CoutP = Lpad;
-      cw.w_direct = (float*)kbuf.p;
-      cp.w_img_stride = (long long)16 * C * Lpad;
+      cp.w = kbuf.p; cp.w_img_stride = (long long)16 * C * Lpad;
       const double nL = (double)nq * ws;
       c.tag("conv_direct_kernel|attention S=QK^T", 0, 2.0 * B * nL * (double)L * C * 16,
             2.0 * B * nL * (double)L * C * 16, (double)B * h * w * C * c.esz() + (double)kbytes + (double)B * nL * Lpad * 4);
-      CK(launch_conv(c, cp, cw));
+      CK(direct_launch(cp, Lpad, c.prec == SE_PREC_FP32_EXACT, c.stream));
     }
     if (last) {
       c.put(kbuf);
@@ -916,16 +891,12 @@ static int run_cam(Ctx& c, const View& f, const float* mask_s, void* out, int ou
       cp.out_c8 = out_c8;
       cp.osy = 2; cp.ooy = 2 * y0 + pc / 2; cp.osx = 2; cp.oox = pc % 2;
       cp.epi = EPI_LINEAR; cp.scale = 1.0f; cp.colscale = nullptr;
-      ClassW cw;
-      cw.ntaps = 4;
-      cw.CoutP = C;
-      cw.w_direct = reinterpret_cast<float*>((char*)vbuf.p + pc * per_pc_bytes);
-      cp.w_img_stride = (long long)4 * Lpad * C;
+      cp.w = (char*)vbuf.p + pc * per_pc_bytes; cp.w_img_stride = (long long)4 * Lpad * C;
       const double ny = y1 - y0;
       c.tag("conv_direct_kernel|attention out=fold(PV) class", 0,
             2.0 * B * ny * (w / 2) * (double)C * L * 4, 2.0 * B * ny * (w / 2) * (double)C * L * 4,
             ((double)B * nq * ws * Lpad + (double)B * 4 * Lpad * C + (double)B * ny * (w / 2) * C) * c.esz());
-      CK(launch_conv(c, cp, cw));
+      CK(direct_launch(cp, C, c.prec == SE_PREC_FP32_EXACT, c.stream));
     }
     if (last) c.put(vbuf);
     c.put(pbuf);
@@ -956,61 +927,81 @@ static int run_cam_split(Ctx& c, const float* f, int h, int w, int C, const floa
 }
 
 // ------------------------------------------------------------------------------------------ networks
-static const std::initializer_list<const char*> kTrunk9 = {"conv1", "conv2_downsample", "conv3", "conv4_downsample", "conv5",
-                                                           "conv6", "conv7_atrous", "conv8_atrous", "conv9_atrous"};
+static const std::initializer_list<const char*> kEncoder = {"conv1", "conv2_downsample", "conv3", "conv4_downsample", "conv5", "conv6",
+                                                            "conv7_atrous", "conv8_atrous", "conv9_atrous", "conv10_atrous"};
+static const std::initializer_list<const char*> kDecoder = {"11", "12", "13_upsample_conv", "14", "15_upsample_conv", "16"};
 
 // input packing / pooling glue in the activation storage of the current mode
-static int do_pack8(Ctx& c, const float* img, const float* sk, const float* mask, void* out, int H, int W, int img_mode, float sscale, int write_mask,
+// the packed 8-channel network input (stem_view) in a fresh workspace buffer
+static int do_pack8(Ctx& c, Act* out, const float* img, const float* sk, const float* mask, int H, int W, int img_mode, float sscale, int write_mask,
                     int img2_mode = -1) {
-  if (c.split()) return pack8_split(img, sk, mask, out, c.B, H, W, stem_wp(W), STEM_PADL, img_mode, sscale, write_mask, c.stream);
-  return pack8(img, sk, mask, out, c.act_dt(), c.B, H, W, stem_wp(W), STEM_PADL, img_mode, sscale, write_mask, c.stream, img2_mode);
+  Buf in8 = c.get((size_t)c.B * H * stem_wp(W) * 8 * c.esz());
+  c.tag("pack8_kernel|mask-mul + concat + cast", 0, 0, 0, (double)c.B * H * W * 20 + (double)c.B * H * stem_wp(W) * 8 * c.esz());
+  if (c.split()) CK(pack8_split(img, sk, mask, in8.p, c.B, H, W, stem_wp(W), STEM_PADL, img_mode, sscale, write_mask, c.stream));
+  else CK(pack8(img, sk, mask, in8.p, c.act_dt(), c.B, H, W, stem_wp(W), STEM_PADL, img_mode, sscale, write_mask, c.stream, img2_mode));
+  *out = Act{stem_view(c, in8.p, H, W), in8};
+  return 0;
 }
-static int do_pool_broadcast(Ctx& c, const View& v, int HW, int mode, float* pooled, void* cat, int cat_ld, int tc) {
-  if (c.split()) {
-    int rc = plane_reduce_split(v.p, c.B, HW, 96, v.ld / 2, mode, pooled, c.stream);
-    if (rc) return rc;
-    return broadcast_split(pooled, cat, c.B, HW, 96, cat_ld / 2, 96, c.stream);
-  }
-  int rc = plane_reduce(v.p, c.act_dt(), c.B, HW, 96, v.ld, v.c8, mode, pooled, c.stream);
-  if (rc) return rc;
-  return broadcast_channels(pooled, cat, c.act_dt(), c.B, HW, 96, cat_ld, 96, tc, c.stream);
+// global pooling of the 96-channel map v, broadcast into channels 96..191 of the concat buffer cat
+static int do_pool_broadcast(Ctx& c, const View& v, int mode, void* cat, int cat_ld) {
+  const int HW = v.H * v.W;
+  Buf pooled = c.get((size_t)c.B * 96 * 4);
+  c.tag("plane_reduce + broadcast_channels|global style pooling -> concat blocks", 0, 0, 0, 2.0 * c.B * v.H * v.W * 96 * (c.esz() > 2 ? 4 : 2));
+  auto launch = [&](float* pl) -> int {   // one timed launch pair
+    if (c.split()) {
+      int rc = plane_reduce_split(v.p, c.B, HW, 96, v.ld / 2, mode, pl, c.stream);
+      return rc ? rc : broadcast_split(pl, cat, c.B, HW, 96, cat_ld / 2, 96, c.stream);
+    }
+    int rc = plane_reduce(v.p, c.act_dt(), c.B, HW, 96, v.ld, v.c8, mode, pl, c.stream);
+    return rc ? rc : broadcast_channels(pl, cat, c.act_dt(), c.B, HW, 96, cat_ld, 96, c.tc() ? 1 : 0, c.stream);
+  };
+  CK(launch((float*)pooled.p));
+  c.put(pooled);
+  return 0;
 }
 
 // MDGenerator.forward: x [B,3,H,W], guide [B,1,H,W] -> mask1 (soft, NCHW), optional x_stage1; also the
 // binarised mask plane (mask1 > 0.5) when mask_bin != nullptr.
 static int run_netM(Ctx& c, const float* x, const float* guide, int H, int W, float* mask1, float* x_stage1, float* mask_bin, long long mask1_bs = 0,
                     unsigned char* mask_u8 = nullptr) {
-  const int dt = c.act_dt();
-  Buf in8 = c.get((size_t)c.B * H * stem_wp(W) * 8 * c.esz());
-  c.tag("pack8_kernel|mask-mul + concat + cast", 0, 0, 0, (double)c.B * H * W * 20 + (double)c.B * H * stem_wp(W) * 8 * c.esz());
-  CK(do_pack8(c, x, guide, nullptr, in8.p, H, W, PACK_IMG_ONE, 1.0f, 0));
-  View x9;
-  Buf b9;
-  int rc = run_chain(c, 'M', with_prefix("", kTrunk9), stem_view(c, in8.p, H, W), true, in8, &x9, &b9);
+  Act in8, x9;
+  int rc = do_pack8(c, &in8, x, guide, nullptr, H, W, PACK_IMG_ONE, 1.0f, 0);
+  if (rc) return rc;
+  std::vector<std::string> trunk = with_prefix("", kEncoder);
+  trunk.pop_back();   // conv10_atrous opens the mask branch
+  rc = run_chain(c, 'M', trunk, in8, &x9);
   if (rc) return rc;
   if (x_stage1) {
-    // image decoder consumes the conv9 output (editline2_g.py:76-77)
-    View v16;
-    Buf b16;
-    rc = run_chain(c, 'M', with_prefix("conv", {"11", "12", "13_upsample_conv", "14", "15_upsample_conv", "16"}), x9, false, Buf(), &v16, &b16);
+    // image decoder reads the conv9 output too (editline2_g.py:76-77)
+    Act v16;
+    rc = run_chain(c, 'M', with_prefix("conv", kDecoder), x9.borrow(), &v16);
     if (rc) return rc;
-    rc = run_head(c, 'M', "conv17", v16, HEAD_TANH, nullptr, nullptr, nullptr, x_stage1, nullptr, nullptr);
+    rc = run_head(c, 'M', "conv17", v16.v, HEAD_TANH, nullptr, nullptr, nullptr, x_stage1, nullptr, nullptr);
     if (rc) return rc;
-    c.put(b16);
+    c.put(v16);
   }
-  View v;
-  Buf b;
+  Act v;
   rc = run_chain(c, 'M', with_prefix("", {"conv10_atrous", "conv_mask_11", "conv_mask_12", "conv_mask_13_upsample_conv", "conv_mask_14",
                                           "conv_mask_15_upsample_conv", "conv_mask_16"}),
-                 x9, true, b9, &v, &b);
+                 x9, &v);
   if (rc) return rc;
   Buf scratch;
   float* mb = mask_bin;
   if (!mb) { scratch = c.get((size_t)c.B * H * W * 4); mb = (float*)scratch.p; }
-  rc = run_head(c, 'M', "conv_mask_17", v, HEAD_MASK, nullptr, nullptr, nullptr, mask1, mb, nullptr, mask1_bs, 0, mask_u8);
+  rc = run_head(c, 'M', "conv_mask_17", v.v, HEAD_MASK, nullptr, nullptr, nullptr, mask1, mb, nullptr, mask1_bs, 0, mask_u8);
   if (rc) return rc;
   c.put(scratch);
-  c.put(b);
+  c.put(v);
+  return 0;
+}
+
+// the fused stem pair `pair` (make_stem_pair) over the packed input `in`, which it releases: *st = the two stems' space-to-depth
+// outputs side by side (24 blocks per image, 12 per stem)
+static int run_stem_pair(Ctx& c, Layer& pair, Act in, Buf* st) {
+  *st = c.get((size_t)c.B * 24 * (in.v.H / 2) * (in.v.W / 2) * 16);
+  int rc = run_layer(c, pair, in.v, st->p, 24, 0, 2);
+  if (rc) return rc;
+  c.put(in);
   return 0;
 }
 
@@ -1020,162 +1011,102 @@ static int run_netG(Ctx& c, const float* x, const float* x2, const float* mask, 
                     float* x_stage1, float* x_stage2, float* composed, const float* mask_soft, const float* blend_img,
                     long long composed_bs = 0, long long msoft_bs = 0, unsigned char* composed_u8 = nullptr) {
   // guide == nullptr: the reference's guide=None -> an all-ones sketch channel (editline_g.py:127-130), built by pack8
-  const int dt = c.act_dt();
   const int* opt = c.m->opt;
   const int h = H / 4, w = W / 4;
   const size_t e = c.esz();
-
-  // ---- stage 1: coarse encoder + style ("warp-in") encoder -> 192-channel concat -> coarse decoder
   const int tc = c.tc() ? 1 : 0;
   const int cat_ld = tc ? 24 * c.sp() : 192;           // 192-channel concat buffers: 24 channel blocks (x2 split-half) or pixel pitch 192
-  auto cat_view = [&](void* p) { return tc ? c8view(p, h, w, 192, cat_ld, 0) : nhwc(p, h, w, 192, 192); };
-  Buf cat1 = c.get((size_t)c.B * h * w * 192 * e);
+  const int style_img = opt[SE_OPT_NO_MASK_CC] ? PACK_IMG_ONE : PACK_IMG_M;   // image channels of the style encoder's input
   // stem pairs (tensor-core path, make_stem_pair): conv1 + wconv1 share one packed input when both encoders see the same image
-  // and mask (always true on the inference path: netG(inputs, inputs, mask_bin, mask_bin, line))
+  // and mask (always true on the inference path: netG(inputs, inputs, mask_bin, mask_bin, line)); xconv1 + pmconv1 always do.
+  // Each encoder then reads its half of the pair's output and its chain starts at its second layer.
   Layer* pair1 = (c.prec == SE_PREC_BF16_TC && x == x2 && mask == mask2) ? find_layer(c.m, 'G', "conv1+wconv1") : nullptr;
   Layer* pair2 = c.prec == SE_PREC_BF16_TC ? find_layer(c.m, 'G', "xconv1+pmconv1") : nullptr;
-  const size_t pair_bytes = (size_t)c.B * 24 * (H / 2) * (W / 2) * 16;   // two space-to-depth tensors of 24 channels
-  auto pair_view = [&](void* p, int which) { View v = c8view(p, H, W, 24, 24, 12 * which); v.c8 = 2; return v; };
-  std::vector<std::string> trunk_rest(kTrunk9.begin() + 1, kTrunk9.end());   // conv2_downsample .. conv9_atrous
+  auto pair_half = [&](const Buf& st, int which) { return s2dview(st.p, H, W, 24, 24, 12 * which); };
+
+  // ---- stage 1: coarse encoder + style ("warp-in") encoder -> 192-channel concat -> coarse decoder
+  Buf cat1 = c.get((size_t)c.B * h * w * 192 * e);
+  Buf st1;
+  int rc = 0;
   if (pair1) {
-    Buf in8 = c.get((size_t)c.B * H * stem_wp(W) * 8 * e);
-    c.tag("pack8_kernel|mask-mul + concat + cast", 0, 0, 0, (double)c.B * H * W * 20 + (double)c.B * H * stem_wp(W) * 8 * c.esz());
-    CK(do_pack8(c, x, guide, mask, in8.p, H, W, PACK_IMG_ONE_MINUS_M, 1.0f, 1, opt[SE_OPT_NO_MASK_CC] ? PACK_IMG_ONE : PACK_IMG_M));
-    Buf st = c.get(pair_bytes);
-    int rc = run_layer(c, *pair1, stem_view(c, in8.p, H, W), st.p, 24, 0, 2);
+    Act in8;
+    rc = do_pack8(c, &in8, x, guide, mask, H, W, PACK_IMG_ONE_MINUS_M, 1.0f, 1, style_img);
     if (rc) return rc;
-    c.put(in8);
-    std::vector<std::string> na, nb;
-    for (auto& n : trunk_rest) { na.push_back(n); nb.push_back("w" + n); }
-    na.push_back("conv10_atrous"); nb.push_back("wconv10_atrous");
-    rc = run_chain(c, 'G', na, pair_view(st.p, 0), false, Buf(), nullptr, nullptr, cat1.p, cat_ld, 0);
+    rc = run_stem_pair(c, *pair1, in8, &st1);
     if (rc) return rc;
-    View v;
-    Buf b;
-    rc = run_chain(c, 'G', nb, pair_view(st.p, 1), false, Buf(), &v, &b);
-    if (rc) return rc;
-    c.put(st);
-    Buf pooled = c.get((size_t)c.B * 96 * 4);
-    c.tag("plane_reduce + broadcast_channels|global style pooling -> concat blocks", 0, 0, 0, 2.0 * c.B * h * w * 96 * (c.esz() > 2 ? 4 : 2));
-    CK(do_pool_broadcast(c, v, h * w, opt[SE_OPT_POOL_AVG] ? RED_AVG : RED_MAX, (float*)pooled.p, cat1.p, cat_ld, tc));
-    c.put(pooled);
-    c.put(b);
-  } else {
-  {
-      Buf in8 = c.get((size_t)c.B * H * stem_wp(W) * 8 * e);
-      c.tag("pack8_kernel|mask-mul + concat + cast", 0, 0, 0, (double)c.B * H * W * 20 + (double)c.B * H * stem_wp(W) * 8 * c.esz());
-      CK(do_pack8(c, x, guide, mask, in8.p, H, W, PACK_IMG_ONE_MINUS_M, 1.0f, 1));
-      std::vector<std::string> names = with_prefix("", kTrunk9);
-      names.push_back("conv10_atrous");
-      int rc = run_chain(c, 'G', names, stem_view(c, in8.p, H, W), true, in8, nullptr, nullptr, cat1.p, cat_ld, 0);
-      if (rc) return rc;
-    }
-    {
-      Buf in8 = c.get((size_t)c.B * H * stem_wp(W) * 8 * e);
-      c.tag("pack8_kernel|mask-mul + concat + cast", 0, 0, 0, (double)c.B * H * W * 20 + (double)c.B * H * stem_wp(W) * 8 * c.esz());
-      CK(do_pack8(c, x2, guide, mask2, in8.p, H, W, opt[SE_OPT_NO_MASK_CC] ? PACK_IMG_ONE : PACK_IMG_M, opt[SE_OPT_JOINT_TRAIN_INP] ? 0.0f : 1.0f, 1));
-      std::vector<std::string> names = with_prefix("w", kTrunk9);
-      names.push_back("wconv10_atrous");
-      View v;
-      Buf b;
-      int rc = run_chain(c, 'G', names, stem_view(c, in8.p, H, W), true, in8, &v, &b);
-      if (rc) return rc;
-      Buf pooled = c.get((size_t)c.B * 96 * 4);
-      c.tag("plane_reduce + broadcast_channels|global style pooling -> concat blocks", 0, 0, 0, 2.0 * c.B * h * w * 96 * (c.esz() > 2 ? 4 : 2));
-      CK(do_pool_broadcast(c, v, h * w, opt[SE_OPT_POOL_AVG] ? RED_AVG : RED_MAX, (float*)pooled.p, cat1.p, cat_ld, tc));
-      c.put(pooled);
-      c.put(b);
-    }
   }
-  Buf xnow = c.get((size_t)c.B * H * stem_wp(W) * 8 * e);
-  {
-    View v16;
-    Buf b16;
-    int rc = run_chain(c, 'G', with_prefix("conv", {"11", "12", "13_upsample_conv", "14", "15_upsample_conv", "16"}),
-                       cat_view(cat1.p), true, cat1, &v16, &b16);
-    if (rc) return rc;
-    c.tag("memset|pad pixels of the packed stage-2 input", 0, 0, 0, (double)xnow.bytes);
-    CK(fill_zero(xnow.p, xnow.bytes, c.stream));   // zero pad pixels of the packed stage-2 input
-    rc = run_head(c, 'G', "conv17", v16, HEAD_COARSE, x, mask, nullptr, x_stage1, nullptr, xnow.p);
-    if (rc) return rc;
-    c.put(b16);
-  }
+  Act in;
+  if (!pair1) rc = do_pack8(c, &in, x, guide, mask, H, W, PACK_IMG_ONE_MINUS_M, 1.0f, 1);
+  if (rc) return rc;
+  rc = run_chain(c, 'G', with_prefix("", kEncoder, pair1 ? 1 : 0), pair1 ? Act{pair_half(st1, 0)} : in, nullptr, Dst{cat1.p, cat_ld, 0});
+  if (rc) return rc;
+  if (!pair1) rc = do_pack8(c, &in, x2, guide, mask2, H, W, style_img, opt[SE_OPT_JOINT_TRAIN_INP] ? 0.0f : 1.0f, 1);
+  if (rc) return rc;
+  Act style;
+  rc = run_chain(c, 'G', with_prefix("w", kEncoder, pair1 ? 1 : 0), pair1 ? Act{pair_half(st1, 1)} : in, &style);
+  if (rc) return rc;
+  c.put(st1);
+  rc = do_pool_broadcast(c, style.v, opt[SE_OPT_POOL_AVG] ? RED_AVG : RED_MAX, cat1.p, cat_ld);
+  if (rc) return rc;
+  c.put(style);
+  Buf xnow = c.get((size_t)c.B * H * stem_wp(W) * 8 * e);   // stage-2 input: the blended coarse result, packed like the network input
+  Act dec;
+  rc = run_chain(c, 'G', with_prefix("conv", kDecoder), Act{c.dense(cat1.p, h, w, 192, tc), cat1}, &dec);
+  if (rc) return rc;
+  c.tag("memset|pad pixels of the packed stage-2 input", 0, 0, 0, (double)xnow.bytes);
+  CK(fill_zero(xnow.p, xnow.bytes, c.stream));   // zero pad pixels of the packed stage-2 input
+  rc = run_head(c, 'G', "conv17", dec.v, HEAD_COARSE, x, mask, nullptr, x_stage1, nullptr, xnow.p);
+  if (rc) return rc;
+  c.put(dec);
+
   // ---- stage 2: hallucination branch + patch-match branch -> concat -> joint decoder
   Buf cat2 = c.get((size_t)c.B * h * w * 192 * e);
+  Act in2{stem_view(c, xnow.p, H, W), xnow};
   Buf st2;
   if (pair2) {
-    st2 = c.get(pair_bytes);
-    int rc = run_layer(c, *pair2, stem_view(c, xnow.p, H, W), st2.p, 24, 0, 2);
-    if (rc) return rc;
-    c.put(xnow);
-    std::vector<std::string> nx;
-    for (auto& n : trunk_rest) nx.push_back("x" + n);
-    nx.push_back("xconv10_atrous");
-    rc = run_chain(c, 'G', nx, pair_view(st2.p, 0), false, Buf(), nullptr, nullptr, cat2.p, cat_ld, 0);
-    if (rc) return rc;
-  } else {
-    std::vector<std::string> names = with_prefix("x", kTrunk9);
-    names.push_back("xconv10_atrous");
-    int rc = run_chain(c, 'G', names, stem_view(c, xnow.p, H, W), false, Buf(), nullptr, nullptr, cat2.p, cat_ld, 0);
+    rc = run_stem_pair(c, *pair2, in2, &st2);
     if (rc) return rc;
   }
-  {
-    View pm;
-    Buf pmb;
-    // pmconv6 writes the layout the attention reads: space-to-depth channel-blocked on the tensor-core path, NHWC otherwise
-    const int pm_c8 = opt[SE_OPT_USE_CAM] ? (c.split() ? 1 : (tc ? 2 : 0)) : -1;
-    int rc = pair2 ? run_chain(c, 'G', with_prefix("pm", {"conv2_downsample", "conv3", "conv4_downsample", "conv5", "conv6"}), pair_view(st2.p, 1), true, st2,
-                               &pm, &pmb, nullptr, 0, 0, pm_c8)
-                   : run_chain(c, 'G', with_prefix("pm", {"conv1", "conv2_downsample", "conv3", "conv4_downsample", "conv5", "conv6"}),
-                               stem_view(c, xnow.p, H, W), true, xnow, &pm, &pmb, nullptr, 0, 0, pm_c8);
-    if (rc) return rc;
-    if (opt[SE_OPT_USE_CAM]) {
-      Buf ms = c.get((size_t)c.B * h * w * 4);
-      c.tag("avgpool4_kernel", 0, 0, 0, (double)c.B * H * W * 4);
-      CK(avgpool4(mask, (float*)ms.p, c.B, H, W, c.stream));
-      Buf camo = c.get((size_t)c.B * h * w * 96 * e);
-      if (c.split()) {
-        // split-half mode: fp32 NHWC in / out of the attention (split-half fp16 GEMMs over explicit patch matrices, se_gemm_split.cu)
-        Buf f32 = c.get((size_t)c.B * h * w * 96 * 4), o32 = c.get((size_t)c.B * h * w * 96 * 4);
-        CK(split_to_f32(pm.p, (float*)f32.p, c.B, 96, h * w, pm.ld / 2, 0, 1, c.stream));
-        static const bool cuda_core_cam = getenv("SE_SPLIT_CAM_DIRECT") != nullptr;   // A/B: the fp32 CUDA-core attention instead
-        if (cuda_core_cam) {
-          const int saved = c.prec;
-          c.prec = SE_PREC_FP32_EXACT;
-          rc = run_cam(c, nhwc(f32.p, h, w, 96, 96), (const float*)ms.p, o32.p, 96, nullptr, 0);
-          c.prec = saved;
-        } else {
-          rc = run_cam_split(c, (const float*)f32.p, h, w, 96, (const float*)ms.p, (float*)o32.p);
-        }
-        if (rc) return rc;
-        CK(nhwc_f32_to_split((const float*)o32.p, camo.p, c.B, 96, h * w, 12, 0, c.stream));
-        c.put(o32); c.put(f32);
-      } else {
-        rc = tc ? run_cam_tc(c, pm, (const float*)ms.p, camo.p, nullptr) : run_cam(c, pm, (const float*)ms.p, camo.p, 96, nullptr, 0);
-        if (rc) return rc;
-      }
-      c.put(ms);
-      c.put(pmb);
-      pm = tc ? c8view(camo.p, h, w, 96, 12 * c.sp(), 0) : nhwc(camo.p, h, w, 96, 96);
-      pmb = camo;
-    }
-    rc = run_chain(c, 'G', with_prefix("pm", {"conv9", "conv10"}), pm, true, pmb, nullptr, nullptr, cat2.p, cat_ld, 96);
-    if (rc) return rc;
-  }
-  {
-    View v16;
-    Buf b16;
-    int rc = run_chain(c, 'G', with_prefix("allconv", {"11", "12", "13_upsample_conv", "14", "15_upsample_conv", "16"}),
-                       cat_view(cat2.p), true, cat2, &v16, &b16);
-    if (rc) return rc;
-    if (composed || composed_u8) {
-      rc = run_head(c, 'G', "allconv17", v16, HEAD_FINE, blend_img, nullptr, mask_soft, composed, x_stage2, nullptr, composed_bs, msoft_bs, composed_u8);
+  rc = run_chain(c, 'G', with_prefix("x", kEncoder, pair2 ? 1 : 0), pair2 ? Act{pair_half(st2, 0)} : in2.borrow(), nullptr, Dst{cat2.p, cat_ld, 0});
+  if (rc) return rc;
+  // pmconv6 writes the layout the attention reads: space-to-depth channel-blocked on the tensor-core path, NHWC otherwise
+  const int pm_c8 = opt[SE_OPT_USE_CAM] ? (c.split() ? 1 : (tc ? 2 : 0)) : -1;
+  Act pm;
+  rc = run_chain(c, 'G', with_prefix("pm", {"conv1", "conv2_downsample", "conv3", "conv4_downsample", "conv5", "conv6"}, pair2 ? 1 : 0),
+                 pair2 ? Act{pair_half(st2, 1), st2} : in2, &pm, Dst{nullptr, 0, 0, pm_c8});
+  if (rc) return rc;
+  if (opt[SE_OPT_USE_CAM]) {
+    Buf ms = c.get((size_t)c.B * h * w * 4);
+    c.tag("avgpool4_kernel", 0, 0, 0, (double)c.B * H * W * 4);
+    CK(avgpool4(mask, (float*)ms.p, c.B, H, W, c.stream));
+    Buf camo = c.get((size_t)c.B * h * w * 96 * e);
+    if (c.split()) {
+      // split-half mode: fp32 NHWC in / out of the attention (split-half fp16 GEMMs over explicit patch matrices, se_gemm_split.cu)
+      Buf f32 = c.get((size_t)c.B * h * w * 96 * 4), o32 = c.get((size_t)c.B * h * w * 96 * 4);
+      CK(split_to_f32(pm.v.p, (float*)f32.p, c.B, 96, h * w, pm.v.ld / 2, 0, 1, c.stream));
+      rc = run_cam_split(c, (const float*)f32.p, h, w, 96, (const float*)ms.p, (float*)o32.p);
+      if (rc) return rc;
+      CK(nhwc_f32_to_split((const float*)o32.p, camo.p, c.B, 96, h * w, 12, 0, c.stream));
+      c.put(o32); c.put(f32);
     } else {
-      rc = run_head(c, 'G', "allconv17", v16, HEAD_TANH, nullptr, nullptr, nullptr, x_stage2, nullptr, nullptr);
+      rc = tc ? run_cam_tc(c, pm.v, (const float*)ms.p, camo.p, nullptr) : run_cam(c, pm.v, (const float*)ms.p, camo.p, 96, nullptr, 0);
+      if (rc) return rc;
     }
-    if (rc) return rc;
-    c.put(b16);
+    c.put(ms);
+    c.put(pm);
+    pm = Act{c.dense(camo.p, h, w, 96, tc), camo};
   }
+  rc = run_chain(c, 'G', with_prefix("pm", {"conv9", "conv10"}), pm, nullptr, Dst{cat2.p, cat_ld, 96});
+  if (rc) return rc;
+  rc = run_chain(c, 'G', with_prefix("allconv", kDecoder), Act{c.dense(cat2.p, h, w, 192, tc), cat2}, &dec);
+  if (rc) return rc;
+  if (composed || composed_u8) {
+    rc = run_head(c, 'G', "allconv17", dec.v, HEAD_FINE, blend_img, nullptr, mask_soft, composed, x_stage2, nullptr, composed_bs, msoft_bs, composed_u8);
+  } else {
+    rc = run_head(c, 'G', "allconv17", dec.v, HEAD_TANH, nullptr, nullptr, nullptr, x_stage2, nullptr, nullptr);
+  }
+  if (rc) return rc;
+  c.put(dec);
   return 0;
 }
 
@@ -1204,7 +1135,7 @@ static int with_arena(se_model* m, int prec, int B, cudaStream_t stream, F fn, s
     m->used = true;
   }
   // ---- replay a captured forward
-  const bool graphable = g_graphs_on && !g_timing && !key.empty() && getenv("SE_TC_DEBUG") == nullptr && getenv("SE_DEBUG_NAN") == nullptr;
+  const bool graphable = g_graphs_on && !g_timing && !key.empty();
   const bool legacy = (stream == nullptr || stream == cudaStreamLegacy);
   cudaStream_t gs = stream;   // stream the graph is captured on / launched into
   if (graphable && legacy) {
@@ -1320,7 +1251,7 @@ static int make_stem_pair(se_model* m, const char* key, const char* a, const cha
   if (!A || !B || !A->set || !B->set) return 0;
   Layer F;
   F.name = key;
-  F.spec = Spec{nullptr, 8, 96, 5, 1, 1, false, 0};
+  F.spec = Spec{8, 96, 5, 1, 1, false, 0};
   F.set = true;
   F.fused_pair = true;
   F.pair_cin_sum = A->spec.cin + B->spec.cin;
@@ -1427,14 +1358,11 @@ int se_model_finalize(se_model* m) {
     SE_REQUIRE(nset == 0 || nset == ntot, "layer not set: net" + first_missing);
   }
   {
-    static const bool no_pairs = getenv("SE_NO_STEM_PAIRS") != nullptr;   // A/B switch for experiments
     const int id5[5] = {0, 1, 2, 3, 4}, w5[5] = {5, 6, 7, 3, 4}, id3[3] = {0, 1, 2};
-    if (!no_pairs) {
-      int rc = make_stem_pair(m, "conv1+wconv1", "conv1", "wconv1", id5, w5, m->opt[SE_OPT_JOINT_TRAIN_INP] ? 0.0f : 1.0f);
-      if (rc) return rc;
-      rc = make_stem_pair(m, "xconv1+pmconv1", "xconv1", "pmconv1", id3, id3, 1.0f);
-      if (rc) return rc;
-    }
+    int rc = make_stem_pair(m, "conv1+wconv1", "conv1", "wconv1", id5, w5, m->opt[SE_OPT_JOINT_TRAIN_INP] ? 0.0f : 1.0f);
+    if (rc) return rc;
+    rc = make_stem_pair(m, "xconv1+pmconv1", "xconv1", "pmconv1", id3, id3, 1.0f);
+    if (rc) return rc;
   }
   for (auto& kv : m->layers) {
     if (!kv.second.set || kv.second.fused_pair) continue;
@@ -1542,7 +1470,7 @@ int se_gated_conv_forward(se_model* m, char net, const char* layer, const float*
     const int dt = c.act_dt();
     const int Ci = L->is_head ? 12 : L->Ci;
     const int in_c8 = wants_c8(c, *L);
-    Buf in = c.get(L->is_stem ? (size_t)B * H * stem_wp(W) * 8 * c.esz() : act_bytes(c, H, W, Ci, in_c8));
+    Buf in = c.get(L->is_stem ? (size_t)B * H * stem_wp(W) * 8 * c.esz() : c.act_bytes(H, W, Ci, in_c8));
     if (c.split()) {
       // split-half storage: hi / lo fp16 halves of the fp32 input in the layout the layer reads
       if (L->is_stem || s.cin % 8) CK(fill_zero(in.p, in.bytes, c.stream));
@@ -1567,9 +1495,9 @@ int se_gated_conv_forward(se_model* m, char net, const char* layer, const float*
       memset(&cp, 0, sizeof(cp));
       ClassW& cw = L->cls[0];
       cp.x = in.p; cp.in_dt = dt; cp.N = B; cp.Hi = H; cp.Wi = W; cp.Ci = Ci; cp.ldx = Ci;
-      cp.Ho = Ho; cp.Wo = Wo; cp.stride = 1; cp.ntaps = cw.ntaps;
-      memcpy(cp.dy, cw.dy, sizeof(cp.dy));
-      memcpy(cp.dx, cw.dx, sizeof(cp.dx));
+      cp.Ho = Ho; cp.Wo = Wo; cp.stride = 1; cp.ntaps = cw.direct.n;
+      memcpy(cp.dy, cw.direct.dy, sizeof(cp.dy));
+      memcpy(cp.dx, cw.direct.dx, sizeof(cp.dx));
       cp.w = cw.w_direct; cp.bias = L->bias; cp.Cout = s.cout;
       cp.y = o.p; cp.out_dt = DT_F32; cp.Hout = Ho; cp.Wout = Wo; cp.ldo = s.cout; cp.choff = 0;
       cp.osy = cp.osx = 1; cp.epi = EPI_LINEAR; cp.scale = 1.0f;
@@ -1578,11 +1506,10 @@ int se_gated_conv_forward(se_model* m, char net, const char* layer, const float*
       c.put(o);
     } else {
       const int cg = s.cout / 2;
-      View vin = L->is_stem ? stem_view(c, in.p, H, W) : (in_c8 ? c8view(in.p, H, W, Ci, (Ci + 7) / 8 * c.sp(), 0) : nhwc(in.p, H, W, Ci, Ci));
-      if (in_c8 == 2) { vin.c8 = 2; vin.ld = 4 * (Ci / 8) * c.sp(); }
+      const View vin = L->is_stem ? stem_view(c, in.p, H, W) : c.dense(in.p, H, W, Ci, in_c8);
       if (c.split()) {
         const int cbo = (cg + 7) / 8;
-        Buf o = c.get(act_bytes(c, Ho, Wo, cg, 1));
+        Buf o = c.get(c.act_bytes(Ho, Wo, cg, 1));
         if (cg % 8) CK(fill_zero(o.p, o.bytes, c.stream));
         int r = run_layer(c, *L, vin, o.p, 2 * cbo, 0, 1);
         if (r) return r;
@@ -1610,7 +1537,7 @@ int se_contextual_attention_forward(const float* feat, const float* mask_s, int 
   if (!holder) { holder = new se_model(); holder->finalized = true; }
   // fp32-on-tensor-cores mode: split-half GEMM attention (needs 16 * C to be a multiple of 256 and no attention-map output);
   // everything else of the fp32 modes runs on the fp32 CUDA-core kernels
-  const bool split_cam = precision == SE_PREC_FP32_TC && C % 16 == 0 && attn == nullptr && h % 2 == 0 && w % 2 == 0 && getenv("SE_SPLIT_CAM_DIRECT") == nullptr;
+  const bool split_cam = precision == SE_PREC_FP32_TC && C % 16 == 0 && attn == nullptr && h % 2 == 0 && w % 2 == 0;
   if (precision == SE_PREC_FP32_TC) precision = SE_PREC_FP32_EXACT;
   cudaStream_t st = (cudaStream_t)stream;
   return with_arena(holder, precision, B, st, [&](Ctx& c) -> int {
@@ -1630,9 +1557,7 @@ int se_contextual_attention_forward(const float* feat, const float* mask_s, int 
     if (precision == SE_PREC_BF16_TC && C == 96 && h % 2 == 0 && w % 2 == 0) {
       // the layouts netG uses on the tensor-core path: space-to-depth channel-blocked in, channel-blocked out
       CK(nchw_to_c8_s2d(feat, in.p, B, C, h, w, c.stream));
-      View fv = c8view(in.p, h, w, C, 4 * (C / 8), 0);
-      fv.c8 = 2;
-      int r = run_cam_tc(c, fv, mask_s, o.p, attn);
+      int r = run_cam_tc(c, c.dense(in.p, h, w, C, 2), mask_s, o.p, attn);
       if (r) return r;
       CK(c8_to_nchw(o.p, out, B, C, h * w, c.stream));
       c.put(o);

@@ -84,7 +84,7 @@ template <typename T, int COUT>
 __global__ void head_kernel(const T* __restrict__ x, const float* __restrict__ w /*[9][12][COUT]*/, const float* __restrict__ bias,
                             int B, int H, int W, int mode, const float* __restrict__ img, const float* __restrict__ mask_bin,
                             const float* __restrict__ mask_soft, float* __restrict__ out_nchw, float* __restrict__ out2,
-                            T* __restrict__ out_pack8, int no_mask_coarse, int Wp, int padl, int in_c8, long long obs, long long msbs,
+                            T* __restrict__ out_pack8, int no_mask_coarse, int Wp, int padl, long long obs, long long msbs,
                             unsigned char* __restrict__ out_u8) {
   // obs: elements between images of out_nchw (COUT*HW when dense; 4*HW when it is a view into a packed [B,4,H,W] output);
   // msbs: likewise for mask_soft
@@ -104,20 +104,10 @@ __global__ void head_kernel(const T* __restrict__ x, const float* __restrict__ w
   for (int t = 0; t < 9; ++t) {
     const int iy = yy + t / 3 - 1, ix = xx + t % 3 - 1;
     if (iy < 0 || iy >= H || ix < 0 || ix >= W) continue;
-    // NHWC: 12 contiguous channels; C8: two channel blocks [b][2][H][W][8] (channels 12..15 are padding)
-    const T* xp = in_c8 ? x + (((b * 2) * H + iy) * W + ix) * 8 : x + ((b * H + iy) * W + ix) * 12;
-    const long long blk = in_c8 ? (long long)H * W * 8 - 8 : 0;
-    __align__(16) T xl[16];
-    if (in_c8 && sizeof(T) == 2) {   // two 16 B loads instead of twelve 2 B loads
-      *reinterpret_cast<uint4*>(xl) = *reinterpret_cast<const uint4*>(xp);
-      *reinterpret_cast<uint4*>(xl + 8) = *reinterpret_cast<const uint4*>(xp + blk + 8);
-    } else {
-#pragma unroll
-      for (int c = 0; c < 12; ++c) xl[c] = xp[c + (c >= 8 ? blk : 0)];
-    }
+    const T* xp = x + ((b * H + iy) * W + ix) * 12;   // NHWC: 12 contiguous channels
 #pragma unroll
     for (int c = 0; c < 12; ++c) {
-      const float xv = to_f<T>(xl[c]);
+      const float xv = to_f<T>(xp[c]);
 #pragma unroll
       for (int o = 0; o < COUT; ++o) acc[o] = fmaf(xv, ws[(t * 12 + c) * COUT + o], acc[o]);
     }
@@ -267,7 +257,7 @@ int head_c8(const void* x, const float* w_host, const float* b_host, int cout, i
   return head_c8_launch<3>(x, w_host, b_host, B, H, W, mode, img, mask_bin, mask_soft, out_nchw, out2, out_pack8, no_mask_coarse, Wp, padl, obs, msbs, out_u8, s);
 }
 
-int head(const void* x, int dt, int in_c8, const float* w, const float* bias, int cout, int B, int H, int W, int mode, const float* img,
+int head(const void* x, int dt, const float* w, const float* bias, int cout, int B, int H, int W, int mode, const float* img,
          const float* mask_bin, const float* mask_soft, float* out_nchw, float* out2, void* out_pack8, int no_mask_coarse,
          int Wp, int padl, long long obs, long long msbs, unsigned char* out_u8, cudaStream_t s) {
   const long long n = (long long)B * H * W;
@@ -276,9 +266,9 @@ int head(const void* x, int dt, int in_c8, const float* w, const float* bias, in
   if (!msbs) msbs = (long long)H * W;
   SE_DISPATCH_T(dt, {
     if (cout == 1)
-      head_kernel<T, 1><<<cdiv(n, 128), 128, 0, s>>>((const T*)x, w, bias, B, H, W, mode, img, mask_bin, mask_soft, out_nchw, out2, (T*)out_pack8, no_mask_coarse, Wp, padl, in_c8, obs, msbs, out_u8);
+      head_kernel<T, 1><<<cdiv(n, 128), 128, 0, s>>>((const T*)x, w, bias, B, H, W, mode, img, mask_bin, mask_soft, out_nchw, out2, (T*)out_pack8, no_mask_coarse, Wp, padl, obs, msbs, out_u8);
     else
-      head_kernel<T, 3><<<cdiv(n, 128), 128, 0, s>>>((const T*)x, w, bias, B, H, W, mode, img, mask_bin, mask_soft, out_nchw, out2, (T*)out_pack8, no_mask_coarse, Wp, padl, in_c8, obs, msbs, out_u8);
+      head_kernel<T, 3><<<cdiv(n, 128), 128, 0, s>>>((const T*)x, w, bias, B, H, W, mode, img, mask_bin, mask_soft, out_nchw, out2, (T*)out_pack8, no_mask_coarse, Wp, padl, obs, msbs, out_u8);
   });
   SE_CUDA_OK(cudaGetLastError());
   return 0;
@@ -289,17 +279,16 @@ int head(const void* x, int dt, int in_c8, const float* w, const float* bias, in
 //   RED_MAX / RED_AVG      global pooling            (editline_g.py:160-165)
 //   RED_RNORM              1/sqrt(sum x^2 + 1e-8)    (splitcam.py:40)
 template <typename T>
-__global__ void plane_reduce_kernel(const T* __restrict__ x, int ldx, int c8, int C, int HW, int mode, float* __restrict__ out) {
+__global__ void plane_reduce_kernel(const T* __restrict__ x, int ldx, int C, int HW, int mode, float* __restrict__ out) {
   __shared__ float red[8][33];
   const int b = blockIdx.y;
   const int c = blockIdx.x * 32 + threadIdx.x;
   float acc = (mode == RED_MAX) ? -INFINITY : 0.0f;
   if (c < C) {
-    // NHWC: pixel pitch ldx; C8: [b][ldx blocks][HW][8]
-    const T* xp = c8 ? x + ((size_t)b * ldx + (c >> 3)) * HW * 8 + (c & 7) : x + (size_t)b * HW * ldx + c;
-    const size_t pitch = c8 ? 8 : ldx;
+    const T* xp = x + (size_t)b * HW * ldx + c;   // pixel pitch ldx
+#pragma unroll 4   // left to itself nvcc unrolls further and needs 32 registers instead of 22-24
     for (int p = threadIdx.y; p < HW; p += 8) {
-      const float v = to_f<T>(xp[(size_t)p * pitch]);
+      const float v = to_f<T>(xp[(size_t)p * ldx]);
       if (mode == RED_MAX) acc = fmaxf(acc, v);
       else if (mode == RED_AVG) acc += v;
       else acc = fmaf(v, v, acc);
@@ -387,6 +376,7 @@ __global__ void rnorm_finalize_kernel(float* __restrict__ v, int n) {
 }
 
 int plane_reduce(const void* x, int dt, int B, int HW, int C, int ldx, int c8, int mode, float* out, cudaStream_t s) {
+  SE_REQUIRE(!c8 || dt == DT_BF16, "channel-blocked plane reductions read bf16");
   if (!c8 && dt == DT_BF16 && mode == RED_RNORM && HW >= 1024) {
     const int slices = 16;
     SE_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)B * C * 4, s));
@@ -396,14 +386,14 @@ int plane_reduce(const void* x, int dt, int B, int HW, int C, int ldx, int c8, i
     SE_CUDA_OK(cudaGetLastError());
     return 0;
   }
-  if (c8 && dt == DT_BF16) {
+  if (c8) {
     dim3 grid((C + 7) / 8, B);
     plane_reduce_c8_kernel<<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, ldx, C, HW, mode, out);
     SE_CUDA_OK(cudaGetLastError());
     return 0;
   }
   dim3 grid(cdiv(C, 32), B), block(32, 8);
-  SE_DISPATCH_T(dt, (plane_reduce_kernel<T><<<grid, block, 0, s>>>((const T*)x, ldx, c8, C, HW, mode, out)));
+  SE_DISPATCH_T(dt, (plane_reduce_kernel<T><<<grid, block, 0, s>>>((const T*)x, ldx, C, HW, mode, out)));
   SE_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -411,18 +401,9 @@ int plane_reduce(const void* x, int dt, int B, int HW, int C, int ldx, int c8, i
 // nearest 1x1 -> h x w broadcast of the pooled vector into channels [choff, choff+C) of an NHWC map
 // (editline_g.py:166-167: interpolate + cat).
 template <typename T>
-__global__ void broadcast_kernel(const float* __restrict__ v, T* __restrict__ y, int C, int HW, int ldo, int choff, int c8, long long total) {
+__global__ void broadcast_kernel(const float* __restrict__ v, T* __restrict__ y, int C, int HW, int ldo, int choff, long long total) {
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= total) return;
-  if (c8) {   // [b][ldo blocks][HW][8]: i enumerates (b, c/8, p, c%8) so that consecutive threads write consecutive bytes
-    const int c7 = (int)(i & 7);
-    long long r = i >> 3;
-    const long long p = r % HW; r /= HW;
-    const int cb = (int)(r % (C >> 3));
-    const long long b = r / (C >> 3);
-    y[((b * ldo + (choff >> 3) + cb) * HW + p) * 8 + c7] = from_f<T>(v[b * C + cb * 8 + c7]);
-    return;
-  }
   const int c = (int)(i % C);
   const long long pix = i / C;
   const long long b = pix / HW;
@@ -442,15 +423,15 @@ __global__ void broadcast_c8_kernel(const float* __restrict__ v, __nv_bfloat16* 
 }
 
 int broadcast_channels(const float* v, void* y, int dt, int B, int HW, int C, int ldo, int choff, int c8, cudaStream_t s) {
-  if (c8 && dt == DT_BF16 && C % 8 == 0 && choff % 8 == 0) {
+  if (c8) {
+    SE_REQUIRE(dt == DT_BF16 && C % 8 == 0 && choff % 8 == 0, "C8 broadcast writes whole bf16 channel blocks");
     const long long n = (long long)B * (C >> 3) * HW;
     broadcast_c8_kernel<<<cdiv(n, 256), 256, 0, s>>>(v, (__nv_bfloat16*)y, C, HW, ldo, choff, n);
     SE_CUDA_OK(cudaGetLastError());
     return 0;
   }
   const long long total = (long long)B * HW * C;
-  SE_REQUIRE(!c8 || (C % 8 == 0 && choff % 8 == 0), "C8 broadcast needs whole channel blocks");
-  SE_DISPATCH_T(dt, (broadcast_kernel<T><<<cdiv(total, 256), 256, 0, s>>>(v, (T*)y, C, HW, ldo, choff, c8, total)));
+  SE_DISPATCH_T(dt, (broadcast_kernel<T><<<cdiv(total, 256), 256, 0, s>>>(v, (T*)y, C, HW, ldo, choff, total)));
   SE_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -808,27 +789,6 @@ int to_uint8(const float* comp, const float* mask, unsigned char* bgr, unsigned 
   to_uint8_kernel<<<cdiv(B * HW, 256), 256, 0, s>>>(comp, mask, bgr, mk, B, HW);
   SE_CUDA_OK(cudaGetLastError());
   return 0;
-}
-
-// debug: number of non-finite bf16 values in a buffer
-__global__ void count_nonfinite_kernel(const __nv_bfloat16* __restrict__ x, long long n, unsigned long long* out) {
-  long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  unsigned long long c = 0;
-  for (; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const float v = __bfloat162float(x[i]);
-    if (!(fabsf(v) <= 3.0e38f)) ++c;
-  }
-  if (c) atomicAdd(out, c);
-}
-long long count_nonfinite_bf16(const void* x, long long n, cudaStream_t s) {
-  static unsigned long long* d = nullptr;
-  if (!d) cudaMalloc(&d, 8);
-  cudaMemsetAsync(d, 0, 8, s);
-  count_nonfinite_kernel<<<256, 256, 0, s>>>((const __nv_bfloat16*)x, n, d);
-  unsigned long long h = 0;
-  cudaMemcpyAsync(&h, d, 8, cudaMemcpyDeviceToHost, s);
-  cudaStreamSynchronize(s);
-  return (long long)h;
 }
 
 // zero-fill helper for padded channel tails

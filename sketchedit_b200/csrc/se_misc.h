@@ -10,7 +10,7 @@ enum { RED_MAX = 0, RED_AVG = 1, RED_RNORM = 2 };
 
 int pack8(const float* img, const float* sketch, const float* mask, void* out, int dt, int B, int H, int W, int Wp, int padl,
           int img_mode, float sketch_scale, int write_mask, cudaStream_t s, int img2_mode = -1);   // img2_mode >= 0: channels 5..7 = img * f(mask)
-int head(const void* x, int dt, int in_c8, const float* w, const float* bias, int cout, int B, int H, int W, int mode, const float* img,
+int head(const void* x, int dt, const float* w, const float* bias, int cout, int B, int H, int W, int mode, const float* img,
          const float* mask_bin, const float* mask_soft, float* out_nchw, float* out2, void* out_pack8, int no_mask_coarse,
          int Wp, int padl, long long out_bstride, long long msoft_bstride, unsigned char* out_u8,
          cudaStream_t s);   // strides: elements between images, 0 = dense; out_u8: HEAD_MASK -> mask bytes [B,H,W], HEAD_FINE -> BGR HWC bytes
@@ -43,7 +43,6 @@ int broadcast_split(const float* v, void* y, int B, int HW, int C, int ld, int c
 int nchw_to_split(const float* x, void* y, int B, int C, int H, int W, int layout, int Wp, int padl, cudaStream_t s);
 int split_to_f32(const void* x, float* y, int B, int C, int HW, int ld, int choff, int nhwc, cudaStream_t s);
 int nhwc_f32_to_split(const float* x, void* y, int B, int C, int HW, int ld, int choff, cudaStream_t s);
-long long count_nonfinite_bf16(const void* x, long long n, cudaStream_t s);
 int fill_zero(void* p, size_t bytes, cudaStream_t s);
 
 }  // namespace se
