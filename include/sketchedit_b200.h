@@ -111,6 +111,29 @@ int se_set_attention_workspace_limit(long long bytes);
 int se_outputs_to_uint8(const float* composed, const float* mask, int B, int H, int W, unsigned char* bgr_hwc,
                         unsigned char* mask_u8, void* stream);
 
+/* ---- Pillow-exact resize of uint8 HWC images: PIL.Image.resize(size) with its default filter (BICUBIC, no box, no
+ * reducing_gap), bit for bit, for a batch of n <= 32 images of their own sizes (the resize-to-a-multiple-of-8 before the
+ * forward and back after it of the reference demo, demo.py:39-73). Image i is read from src + src_off[i] (bytes) with size
+ * src_hw[2i] x src_hw[2i+1] x channels and written to dst + dst_off[i] at dst_hw[2i] x dst_hw[2i+1] x channels; channels is 1
+ * or 3, sizes are in [1, 65535]. Only the destination slices are written. swap_rb (channels 3) reverses the channel order of
+ * the output (BGR <-> RGB). An axis whose length does not change is not resampled; an image of unchanged size is copied.
+ * scratch holds the intermediate of images resized along both axes. Query form: scratch == NULL stores the bytes it needs in
+ * *scratch_bytes and enqueues nothing; otherwise *scratch_bytes is the size of scratch. The coefficient tables are built on
+ * the host and cached on the device per (in, out) pair: the first call with a new length pair uploads its table (a
+ * synchronous copy); later calls only enqueue the kernels on `stream`. */
+int se_resize_u8(const unsigned char* src, const long long* src_off, const int* src_hw, unsigned char* dst, const long long* dst_off,
+                 const int* dst_hw, int n, int channels, int swap_rb, void* scratch, long long* scratch_bytes, void* stream);
+/* Bytes of coefficient tables se_resize_u8 keeps per device (process-wide; 0 restores the default of 256 MiB; negative is an
+ * error). When a call's new tables would pass the limit, the device's cache is emptied (after a device synchronise) before the
+ * call looks up any table; one call's own tables may exceed it. */
+int se_resize_set_table_cache_limit(long long bytes);
+/* bytes of coefficient tables currently cached for the current device */
+long long se_resize_table_cache_bytes(void);
+/* Host only (no device needed): the coefficient table se_resize_u8 uses for one axis of length in -> out. Returns ksize;
+ * bounds [out][2] = (first input sample, number of taps), coeffs [out][ksize] = weights with 22 fractional bits, zero beyond
+ * the taps. cap = ints coeffs holds (>= out * ksize). bounds == coeffs == NULL: returns ksize only. Returns -1 on error. */
+int se_resize_coeffs(int in, int out, int* bounds, int* coeffs, long long cap);
+
 /* ---- introspection for bench.py */
 /* number of kernels this library launched during the most recent forward-type call on this thread */
 int se_last_launch_count(void);

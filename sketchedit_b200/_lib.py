@@ -40,6 +40,11 @@ SIGNATURES = {
                                                  _c_void_p, _c_void_p]),
     "se_set_attention_workspace_limit": (_c_int, [ctypes.c_longlong]),
     "se_outputs_to_uint8": (_c_int, [_c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_void_p, _c_void_p, _c_void_p]),
+    "se_resize_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_void_p,
+                              ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
+    "se_resize_coeffs": (_c_int, [_c_int, _c_int, _c_void_p, _c_void_p, ctypes.c_longlong]),
+    "se_resize_set_table_cache_limit": (_c_int, [ctypes.c_longlong]),
+    "se_resize_table_cache_bytes": (ctypes.c_longlong, []),
     "se_last_launch_count": (_c_int, []),
     "se_workspace_bytes": (ctypes.c_longlong, [_c_void_p]),
     "se_timing_enable": (_c_int, [_c_int]),

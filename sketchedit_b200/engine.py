@@ -232,6 +232,97 @@ def set_attention_workspace_limit(nbytes):
     _lib.check(_lib.load().se_set_attention_workspace_limit(int(nbytes)))
 
 
+RESIZE_MAX_BATCH = 32    # images per se_resize_u8 call; resize_u8_packed splits longer lists into calls of this size
+
+
+def resize_u8_packed(src, src_offsets, src_sizes, dst_sizes, channels, swap_rb=False, out=None, dst_offsets=None):
+    """PIL.Image.resize(size) (BICUBIC, its default) of a batch of uint8 HWC images, bit for bit, on the device.
+
+    Image i is the ``src_sizes[i] = (h, w)`` x ``channels`` bytes at byte ``src_offsets[i]`` of the contiguous CUDA uint8 tensor
+    ``src``; it is resized to ``dst_sizes[i]`` and written at ``dst_offsets[i]`` of ``out``. Without ``out`` the results are
+    packed into a new tensor at 16-byte aligned offsets. ``swap_rb`` reverses the channel order of the output (channels 3).
+    Returns ``(out, dst_offsets)``. Only enqueues work on the current stream, except that the first resize between a pair of
+    lengths uploads its coefficient table."""
+    n = len(src_sizes)
+    if len(src_offsets) != n or len(dst_sizes) != n:
+        raise _lib.SketchEditB200Error("src_offsets, src_sizes and dst_sizes must have the same length")
+    for t, nm in ((src, "src"), (out, "out")):
+        if t is not None and not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
+            raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % nm)
+    src_sizes = [(int(h), int(w)) for h, w in src_sizes]
+    dst_sizes = [(int(h), int(w)) for h, w in dst_sizes]
+    nbytes = lambda hw: hw[0] * hw[1] * channels
+    if out is None:
+        if dst_offsets is not None:
+            raise _lib.SketchEditB200Error("dst_offsets needs out")
+        dst_offsets, total = [], 0
+        for hw in dst_sizes:
+            dst_offsets.append(total)
+            total += (nbytes(hw) + 15) // 16 * 16
+        out = torch.empty(total, device=src.device, dtype=torch.uint8)
+    elif dst_offsets is None or len(dst_offsets) != n:
+        raise _lib.SketchEditB200Error("out needs one dst_offsets entry per image")
+    if out.device != src.device:
+        raise _lib.SketchEditB200Error("src on %s but out on %s" % (src.device, out.device))
+    dst_offsets = [int(o) for o in dst_offsets]
+    for buf, offs, sizes, nm in ((src, src_offsets, src_sizes, "src"), (out, dst_offsets, dst_sizes, "out")):
+        for o, hw in zip(offs, sizes):
+            if o < 0 or o + nbytes(hw) > buf.numel():
+                raise _lib.SketchEditB200Error("%s slice [%d, %d) outside the %d-byte buffer" % (nm, o, o + nbytes(hw), buf.numel()))
+    lib = _lib.load()
+    with torch.cuda.device(src.device):
+        chunks = []
+        for c0 in range(0, n, RESIZE_MAX_BATCH):
+            sl = slice(c0, c0 + RESIZE_MAX_BATCH)
+            k = len(src_sizes[sl])
+            arr = (ctypes.c_longlong * k, ctypes.c_int * (2 * k))
+            args = (arr[0](*[int(o) for o in src_offsets[sl]]), arr[1](*[v for hw in src_sizes[sl] for v in hw]),
+                    arr[0](*dst_offsets[sl]), arr[1](*[v for hw in dst_sizes[sl] for v in hw]), k)
+            need = ctypes.c_longlong(0)
+            _lib.check(lib.se_resize_u8(None, args[0], args[1], None, args[2], args[3], k, channels, int(bool(swap_rb)), None,
+                                        ctypes.byref(need), None))
+            chunks.append((args, need.value))
+        scratch = torch.empty(max([1] + [b for _, b in chunks]), device=src.device, dtype=torch.uint8)
+        for (a, _) in chunks:
+            size = ctypes.c_longlong(scratch.numel())
+            _lib.check(lib.se_resize_u8(_ptr(src), a[0], a[1], _ptr(out), a[2], a[3], a[4], channels, int(bool(swap_rb)), _ptr(scratch),
+                                        ctypes.byref(size), _stream()))
+    return out, dst_offsets
+
+
+def set_resize_table_cache_limit(nbytes):
+    """Bytes of coefficient tables the resize keeps per device (process-wide; 0 = the default of 256 MiB). Past the limit the
+    device's tables are dropped, after a device synchronise, before the next call that needs a new one."""
+    _lib.check(_lib.load().se_resize_set_table_cache_limit(int(nbytes)))
+
+
+def resize_table_cache_bytes():
+    """Bytes of coefficient tables cached for the current device."""
+    return int(_lib.load().se_resize_table_cache_bytes())
+
+
+def resize_u8(images, sizes, swap_rb=False):
+    """List form of ``resize_u8_packed``: ``images`` are CUDA uint8 tensors [h,w,3] or [h,w] (one channel count for the
+    list), ``sizes`` the target ``(h, w)`` of each. Returns the resized images, views of one packed tensor. The inputs are
+    first packed into one buffer; callers that already hold packed data use ``resize_u8_packed`` and skip that copy."""
+    if len(images) != len(sizes):
+        raise _lib.SketchEditB200Error("one target size per image")
+    if not images:
+        return []
+    chans = {1 if t.dim() == 2 else t.shape[-1] for t in images}
+    C = chans.pop()
+    if chans or C not in (1, 3) or any(t.dim() not in (2, 3) for t in images):
+        raise _lib.SketchEditB200Error("images must all be [h,w] or all be [h,w,3]")
+    offs, total = [], 0
+    for t in images:
+        offs.append(total)
+        total += t.numel()
+    src = torch.cat([t.reshape(-1) for t in images]) if len(images) > 1 else images[0].reshape(-1).contiguous()
+    out, dst_offs = resize_u8_packed(src, offs, [tuple(t.shape[:2]) for t in images], sizes, C, swap_rb=swap_rb)
+    shape = (lambda h, w: (h, w)) if images[0].dim() == 2 else (lambda h, w: (h, w, C))
+    return [out[o:o + h * w * C].view(*shape(int(h), int(w))) for o, (h, w) in zip(dst_offs, sizes)]
+
+
 def outputs_to_uint8(composed, mask):
     """test.py:25-27 on device -> (uint8 [B,H,W,3] BGR, uint8 [B,H,W])."""
     lib = _lib.load()

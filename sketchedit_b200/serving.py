@@ -4,7 +4,8 @@ The reference's demo handles one request per Flask thread (``app.run(threaded=Tr
 batch-1 forward. Here concurrent requests are BATCHED: ``RequestBatcher`` collects the requests that arrive within a short
 window, groups them by input size and runs each group as one forward (``Engine.inference_u8``: the codecs of
 demo.py:52-53,64-66 run on the device); ``DemoProcessor.process_image`` is the reference's ``process_image`` around it
-(floor the size to a multiple of 8, PIL resize in, forward, PIL resize back).
+(floor the size to a multiple of 8, PIL resize in, forward, PIL resize back). By default the two resizes run on the device
+too (``engine.resize_u8_packed``, bit-identical to Pillow), so a batch is one upload and one download of raw bytes.
 
     proc = DemoProcessor(models.create_model(opt), max_batch=16, max_wait_ms=2.0)
     result_pil = proc.process_image(image_pil, mask_pil)       # callable from any number of threads
@@ -115,23 +116,86 @@ def floor8(n):
     return n // 8 * 8
 
 
+def _aligned_offsets(nbytes, align=16):
+    offs, total = [], 0
+    for n in nbytes:
+        offs.append(total)
+        total += (n + align - 1) // align * align
+    return offs, total
+
+
 class DemoProcessor:
     """``process_image`` of the reference demo (demo.py:39-73) on the batched uint8 forward.
 
     Differences from the reference function, none of them numerical: it returns the PIL result instead of writing
     ``static/results/<name>``, and concurrent calls share forwards. ``precision``: 'bf16' | 'fp32' | 'fp32_direct'.
+
+    ``resize``: where the three Pillow resizes of the demo run (photo and sketch mask down to the floored size, result back).
+    'device' (default): on the GPU with ``engine.resize_u8_packed``, bit-identical to Pillow; a batch is one upload of the raw
+    photos and masks from pinned memory and one download of the results. 'host': with Pillow on the requesting thread.
+    The device flow's two pinned staging buffers are reused and grow to the largest batch seen (raw photos plus masks in, raw
+    photos out: about 680 MB at 16 requests of 12 MP); ``close()`` releases them.
     """
 
-    def __init__(self, model, precision=None, max_batch=16, max_wait_ms=2.0):
+    def __init__(self, model, precision=None, max_batch=16, max_wait_ms=2.0, resize="device"):
         import torch
+        if resize not in ("device", "host"):
+            raise ValueError("resize must be 'device' or 'host'")
         self._torch = torch
         self.model = model
         self.precision = precision or getattr(model, "precision", "bf16")
+        self.resize = resize
         self.engine = model.engine()
-        self.batcher = RequestBatcher(self._run_batch, max_batch=max_batch, max_wait_ms=max_wait_ms)
+        self._pinned = {}              # name -> reused pinned host staging buffer (grown on demand)
+        self.batcher = RequestBatcher(self._run_batch if resize == "host" else self._run_batch_device, max_batch=max_batch,
+                                      max_wait_ms=max_wait_ms)
 
     def close(self):
         self.batcher.close()
+        self._pinned.clear()
+
+    def _staging(self, name, nbytes):
+        buf = self._pinned.get(name)
+        if buf is None or buf.numel() < nbytes:
+            buf = self._pinned[name] = self._torch.empty(max(nbytes, 1), dtype=self._torch.uint8, pin_memory=True)
+        return buf
+
+    def _run_batch_device(self, key, payloads):
+        """payloads: (raw RGB photo [h,w,3], raw 'L' mask [hm,wm]) at their own sizes; key: the floored network size."""
+        torch = self._torch
+        from .engine import resize_u8_packed
+        H, W = key
+        B = len(payloads)
+        dev = self.engine.device
+        photos, masks = [p[0] for p in payloads], [p[1] for p in payloads]
+        offs, total = _aligned_offsets([a.nbytes for a in photos + masks])
+        out_offs, out_total = _aligned_offsets([a.nbytes for a in photos])
+        stage = self._staging("in", total)          # free: every batch, failed ones included, ends with a stream synchronise
+        host = stage.numpy()
+        for a, o in zip(photos + masks, offs):
+            host[o:o + a.nbytes] = a.reshape(-1)
+        down = self._staging("out", out_total)
+        with torch.cuda.device(dev):
+            try:
+                src = stage[:total].to(dev, non_blocking=True)
+                img = torch.empty(B, H, W, 3, device=dev, dtype=torch.uint8)
+                msk = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
+                resize_u8_packed(src, offs[:B], [a.shape[:2] for a in photos], [(H, W)] * B, 3, out=img,
+                                 dst_offsets=[i * H * W * 3 for i in range(B)])
+                # the resized mask goes to the forward as it is: its input codec applies > 0 (demo.py:52)
+                resize_u8_packed(src, offs[B:], [a.shape[:2] for a in masks], [(H, W)] * B, 1, out=msk,
+                                 dst_offsets=[i * H * W for i in range(B)])
+                with torch.no_grad():
+                    bgr, _ = self.engine.inference_u8(img, msk, precision=self.precision)
+                # back to each photo's own size; the forward writes BGR, the demo keeps RGB
+                res, _ = resize_u8_packed(bgr, [i * H * W * 3 for i in range(B)], [(H, W)] * B, [a.shape[:2] for a in photos], 3,
+                                          swap_rb=True, out=torch.empty(max(out_total, 1), device=dev, dtype=torch.uint8),
+                                          dst_offsets=out_offs)
+                down[:out_total].copy_(res[:out_total], non_blocking=True)
+            finally:
+                torch.cuda.current_stream().synchronize()
+        host = down.numpy()
+        return [host[o:o + a.nbytes].reshape(a.shape).copy() for a, o in zip(photos, out_offs)]
 
     def _run_batch(self, key, payloads):
         torch = self._torch
@@ -143,14 +207,19 @@ class DemoProcessor:
         return [np.ascontiguousarray(rgb[i]) for i in range(len(payloads))]
 
     def process_image(self, img, mask):
-        """img: PIL image; mask: PIL 'L' image of the same size (non-zero = sketch stroke). Returns the edited PIL image at the
-        input's size. Sizes are floored to a multiple of 8 for the network exactly like demo.py:43."""
+        """img: PIL image; mask: PIL 'L' image, usually of the same size (non-zero = sketch stroke). Returns the edited PIL
+        image at the input's size. Sizes are floored to a multiple of 8 for the network exactly like demo.py:43."""
         from PIL import Image
         img = img.convert("RGB")
         w_raw, h_raw = img.size
         h_t, w_t = floor8(h_raw), floor8(w_raw)
         if h_t < 16 or w_t < 16:
             raise ValueError("image smaller than 16x16 (two stride-2 convolutions, 4x4 mask pool, stride-2 patch grid)")
+        if self.resize == "device":
+            if mask.mode != "L":
+                raise ValueError("resize='device' takes an 'L' mask (got mode %r); resize='host' resizes it with Pillow" % mask.mode)
+            out = self.batcher.submit((h_t, w_t), (np.asarray(img), np.asarray(mask)))
+            return Image.fromarray(out)
         img_t = np.ascontiguousarray(np.array(img.resize((w_t, h_t))), dtype=np.uint8)
         mask_t = np.array(mask.resize((w_t, h_t)))
         mask_t = np.ascontiguousarray((mask_t > 0).astype(np.uint8) * 255)
