@@ -93,25 +93,25 @@ struct ConvParams {
   const float* colscale;        // EPI_LINEAR: [N][Cout] or nullptr
 };
 
-// Output side of one launch (shared by both kernels). Layouts: NHWC (pixel pitch ldo elements, channel offset
-// choff) or C8 = [N][CBtot][H][W][8] (ldo = CBtot channel blocks, choff multiple of 8).
+// Output side of one gated conv_c8 launch. Layouts: NHWC (pixel pitch ldo elements, channel offset choff) or
+// C8 = [N][CBtot][H][W][8] (ldo = CBtot channel blocks, choff multiple of 8).
 struct EpiParams {
   void* y;
-  int out_dt, out_c8;   // out_c8: 0 NHWC, 1 channel-blocked, 2 channel-blocked space-to-depth (see epilogue)
+  int out_c8;   // 0 NHWC, 1 channel-blocked, 2 channel-blocked space-to-depth (see epilogue)
   int Hout, Wout, ldo, choff;
   int osy, ooy, osx, oox;
-  int epi;
-  float scale;
-  const float* colscale;
+  int epi;       // EPI_GATE_ELU or EPI_GATE_RELU
+  float scale;   // split-half: accumulator -> pre-activation
   int Cout, NT;
   // two gated layers fused along N (stem pairs that read the same packed input): output blocks >= blk_split belong to the second
   // layer's tensor, blk_jump (16 B units) further on; par_stride = channel blocks between the parity groups of a
   // space-to-depth output (ldo / 4 unless two such tensors share the buffer). blk_split = 1 << 20: off.
   int blk_split, blk_jump, par_stride;
-  int nsplit, split_stride;   // nsplit = 2: split-half output (DT_F16X2): the lo part of every block is stored split_stride (16 B units) further on
-  int has_bias;   // 0: the launch has no bias vector (attention GEMMs): no per-column constants are staged in shared memory
-  int goff;   // gated epilogues: accumulator column of gate channel 0 (= Cout/2 rounded up to 8; the weight image
-              // places feature c at column c and its gate at goff + c, columns in between are zero weights)
+  int blk_stride;     // elements between channel block b and b + 1 of one output pixel
+  int paired;         // every column pair of the fragment is one aligned 4 B store (see conv_epilogue)
+  int split_stride;   // split-half output (DT_F16X2): the lo part of every block is stored split_stride (16 B units) further on
+  int goff;   // accumulator column of gate channel 0 (= Cout/2 rounded up to 8; the weight image places feature c at column c
+              // and its gate at goff + c, columns in between are zero weights)
 };
 // Split-half tensors (DT_F16X2) store value * kSplitActScale: fp16's narrow exponent would otherwise push the lo half of every
 // activation below ~0.25 into the subnormals (quantum 2^-24: ~1e-6 relative at 0.03). Times 64 the pair keeps ~22 bits down to

@@ -147,6 +147,8 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
     const uint32_t n_u64 = p.ntaps * p.n64;
     const int ncls = p.ncls;
     const uint32_t tpi = (uint32_t)(p.tiles_x * p.tiles_y);
+    const uint32_t cst_s = smem_u32(bias_s);
+    const bool elu = p.e.epi == EPI_GATE_ELU, paired = p.e.paired != 0;
     if (p.resident) mbar_wait(wres_bar, 0, 6);
     auto release = [&](uint64_t* bar) {
       __syncwarp();
@@ -217,32 +219,41 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
       if (halo && cls == ncls - 1) release(&a_empty[ab]);
       // output pixel of fragment row half h (sub-pixel classes: osy = osx = 2 and a per-class offset)
       const int ooy = ncls > 1 ? p.cls_ooy[cls] : p.e.ooy, oox = ncls > 1 ? p.cls_oox[cls] : p.e.oox;
-      auto pix = [&](int h, int& oy, int& ox) -> bool {
+      size_t base[2];
+      bool ok[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
         const int ry = 8 * wg + 2 * wq + h, rx = lane >> 2;   // tile row / column of fragment row 64 wg + frag_row(wq, lane, h)
         const int py = ty * C8_TH + ry, px = tx * C8_TW + rx;
-        oy = py * p.e.osy + ooy;
-        ox = px * p.e.osx + oox;
-        return py < p.Ho && px < p.Wo;
-      };
-      conv_epilogue<NT>(p.e, bias_s, cst_n, acc, img, lane, pix);
+        ok[h] = py < p.Ho && px < p.Wo;
+        base[h] = epi_pixel_offset(p.e, img, py * p.e.osy + ooy, px * p.e.osx + oox, 2 * (lane & 3));
+      }
+      if (elu) {
+        if (kF16 || paired) conv_epilogue<NT, kF16, true, true>(p.e, cst_s, acc, base, ok, lane);
+        else conv_epilogue<NT, false, true, false>(p.e, cst_s, acc, base, ok, lane);
+      } else {
+        if (kF16 || paired) conv_epilogue<NT, kF16, false, true>(p.e, cst_s, acc, base, ok, lane);
+        else conv_epilogue<NT, false, false, false>(p.e, cst_s, acc, base, ok, lane);
+      }
     }
   }
 }
 
 // ------------------------------------------------------------------------------------------ host
 void fill_epi(const ConvParams& c, int NT, EpiParams* e) {
-  e->y = c.y; e->out_dt = c.out_dt; e->out_c8 = c.out_c8;
+  e->y = c.y; e->out_c8 = c.out_c8;
   e->Hout = c.Hout; e->Wout = c.Wout; e->ldo = c.ldo; e->choff = c.choff;
   e->osy = c.osy; e->ooy = c.ooy; e->osx = c.osx; e->oox = c.oox;
-  e->epi = c.epi; e->scale = c.scale; e->colscale = c.colscale;
+  e->epi = c.epi; e->scale = c.scale;
   e->Cout = c.Cout; e->NT = NT;
-  e->has_bias = c.bias != nullptr ? 1 : 0;
   e->blk_split = c.out_blk_split > 0 ? c.out_blk_split : (1 << 20);
   e->blk_jump = c.out_blk_split > 0 ? c.out_blk_jump : 0;
   e->par_stride = c.out_par_stride > 0 ? c.out_par_stride : (c.ldo >> 2);
-  e->nsplit = c.f16x2 ? 2 : 1;
+  const long long plane = c.out_c8 == 2 ? (long long)(c.Hout / 2) * (c.Wout / 2) : (long long)c.Hout * c.Wout;
+  e->blk_stride = (int)(c.out_c8 ? plane * 8 : 8);
+  e->goff = gated_goff(c.Cout);
+  e->paired = (c.out_c8 != 0 || (((c.ldo | c.choff) & 1) == 0 && c.Cout / 2 == e->goff)) ? 1 : 0;
   e->split_stride = (int)c.out_split_stride;
-  e->goff = (c.epi == EPI_LINEAR) ? 0 : gated_goff(c.Cout);
 }
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -418,7 +429,8 @@ int c8_launch(const ConvParams& c, const C8Layer& L_in, cudaStream_t stream, con
   for (int t = 0; t < c.ntaps && !grp; ++t) SE_REQUIRE(c.tap_cb[t] == L.tap_cb[t], "per-tap channel blocks differ from the packed layer");
   SE_REQUIRE(c.Wi * 8 <= (1 << 30) && L.WR * 8 <= 256 && L.HR <= 256 && L.cb_in <= 256, "TMA box limits");
   SE_REQUIRE(c8_nt_supported(w.NT), "no conv_c8 instantiation for N = " + std::to_string(w.NT));
-  SE_REQUIRE(c.epi == EPI_LINEAR || w.NT == 2 * gated_goff(c.Cout), "gated layers keep the gate columns in the upper half of the tile");
+  SE_REQUIRE(c.epi == EPI_GATE_ELU || c.epi == EPI_GATE_RELU, "conv_c8 runs gated epilogues only");
+  SE_REQUIRE(w.NT == 2 * gated_goff(c.Cout), "gated layers keep the gate columns in the upper half of the tile");
   C8Params p;
   memset(&p, 0, sizeof(p));
   p.f16 = c.f16x2 ? 1 : 0;
@@ -463,11 +475,15 @@ int c8_launch(const ConvParams& c, const C8Layer& L_in, cudaStream_t stream, con
         p.aoff[k * C8_CLS_UNITS + u] = (uint32_t)((cb0 * L.HR + oy) * L.WR + ox) * 16u;
       }
   }
-  SE_REQUIRE(c.epi == EPI_LINEAR || (c.Cout % 2 == 0 && (c.out_dt == DT_BF16 || c.out_dt == DT_F16X2)), "gated epilogue needs even Cout, 16-bit out");
-  SE_REQUIRE(!c.out_c8 || ((c.out_dt == DT_BF16 || c.out_dt == DT_F16X2) && c.choff % 8 == 0), "C8 output must be 16-bit with a channel offset multiple of 8");
-  SE_REQUIRE(!c.f16x2 || (c.out_c8 != 0 && c.epi != EPI_LINEAR), "split-half output is channel-blocked and gated");
-  SE_REQUIRE(c.out_c8 != 2 || (c.epi != EPI_LINEAR && c.Hout % 2 == 0 && c.Wout % 2 == 0 && c.ldo % 4 == 0 && (c.Cout / 2) % 8 == 0),
-             "space-to-depth output: gated layer, even size, whole channel blocks");
+  SE_REQUIRE(c.Cout % 2 == 0 && (c.out_dt == DT_BF16 || c.out_dt == DT_F16X2), "gated epilogue needs even Cout, 16-bit out");
+  SE_REQUIRE(!c.out_c8 || c.choff % 8 == 0, "C8 output needs a channel offset multiple of 8");
+  SE_REQUIRE(!c.f16x2 || c.out_c8 != 0, "split-half output is channel-blocked");
+  SE_REQUIRE(c.out_c8 != 2 || (c.Hout % 2 == 0 && c.Wout % 2 == 0 && c.ldo % 4 == 0 && (c.Cout / 2) % 8 == 0),
+             "space-to-depth output: even size, whole channel blocks");
+  {
+    const long long plane = c.out_c8 == 2 ? (long long)(c.Hout / 2) * (c.Wout / 2) : (long long)c.Hout * c.Wout;
+    SE_REQUIRE((long long)(w.NT / 16) * (c.out_c8 ? 8 * plane : 8) + 8LL * p.e.blk_jump < (1LL << 31), "output block offsets must fit in 31 bits");
+  }
 
   const int total_tiles = p.N * p.tiles_x * p.tiles_y;
   const int smem_budget = grp ? kGroupSmemMax - 4096 : kSmemBudget;

@@ -117,8 +117,7 @@ __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
 __device__ __forceinline__ void epi_fill_constants(float* cst, int n, const float* bias, const EpiParams& e, int tid, int nthreads) {
   const int half = e.Cout >> 1;
   for (int i = tid; i < n; i += nthreads) {
-    int ch = i;   // output channel held by column i (-1: padding column)
-    if (e.epi != EPI_LINEAR) ch = i < half ? i : (i >= e.goff && i < e.goff + half ? half + i - e.goff : -1);
+    const int ch = i < half ? i : (i >= e.goff && i < e.goff + half ? half + i - e.goff : -1);   // -1: padding column
     const float b = (bias != nullptr && ch >= 0 && ch < e.Cout) ? bias[ch] : 0.0f;
     cst[i] = b;
     cst[n + i] = b * 1.4426950408889634f;
@@ -162,102 +161,86 @@ __device__ __forceinline__ float gate_one_exact(float f, float ghalf, float b, f
   return a * rcp_approx(1.0f + ex2_approx(-gx * 1.4426950408889634f));
 }
 
-// Element offset of output channel c of pixel (img, oy, ox) in the launch's output tensor.
-//   out_c8 == 0: NHWC, pixel pitch ldo, channel offset choff
-//   out_c8 == 1: channel-blocked [N][ldo blocks][Hout][Wout][8]
+// Element offset of channel (c & 7) of block 0 of pixel (img, oy, ox) in the launch's output tensor; block b of the pixel
+// is e.blk_stride elements further on (plus e.blk_jump * 8 from block blk_split on).
+//   out_c8 == 0: NHWC, pixel pitch ldo, channel offset choff                          (blk_stride = 8)
+//   out_c8 == 1: channel-blocked [N][ldo blocks][Hout][Wout][8]                      (blk_stride = Hout * Wout * 8)
 //   out_c8 == 2: channel-blocked space-to-depth for a stride-2 consumer: [N][4 * ldo/4 blocks][Hout/2][Wout/2][8], parity
-//                (oy&1, ox&1) selects the block group (par_stride blocks apart)
+//                (oy&1, ox&1) selects the block group (par_stride blocks apart)     (blk_stride = Hout/2 * Wout/2 * 8)
 // Fused layer pairs: channel blocks >= blk_split belong to the second layer's tensor, blk_jump 16 B units further on.
-__device__ __forceinline__ size_t epi_offset(const EpiParams& e, int img, int oy, int ox, int c) {
+__device__ __forceinline__ size_t epi_pixel_offset(const EpiParams& e, int img, int oy, int ox, int c) {
   if (e.out_c8 == 0) return (((size_t)img * e.Hout + oy) * e.Wout + ox) * e.ldo + e.choff + c;
-  const int b = c >> 3;
   size_t unit;
   if (e.out_c8 == 2) {
     const size_t Hs = e.Hout >> 1, Ws = e.Wout >> 1, par = ((oy & 1) << 1) | (ox & 1);
-    unit = (((size_t)img * e.ldo + par * e.par_stride + (e.choff >> 3) + b) * Hs + (oy >> 1)) * Ws + (ox >> 1);
+    unit = (((size_t)img * e.ldo + par * e.par_stride + (e.choff >> 3)) * Hs + (oy >> 1)) * Ws + (ox >> 1);
   } else {
-    unit = (((size_t)img * e.ldo + (e.choff >> 3) + b) * e.Hout + oy) * e.Wout + ox;
+    unit = (((size_t)img * e.ldo + (e.choff >> 3)) * e.Hout + oy) * e.Wout + ox;
   }
-  if (b >= e.blk_split) unit += (size_t)e.blk_jump;
   return unit * 8 + (c & 7);
 }
 
-// store channels c (v0) and c + 1 (v1, only if two) of one pixel
-__device__ __forceinline__ void epi_store2(const EpiParams& e, int img, int oy, int ox, int c, float v0, float v1, bool two) {
-  const size_t o = epi_offset(e, img, oy, ox, c);
-  if (e.nsplit > 1) {   // split-half output: hi = fp16(64 v), lo = fp16(64 v - hi), the lo block split_stride 16 B units further on
-    __half* y = reinterpret_cast<__half*>(e.y);
-    v0 = fminf(fmaxf(v0 * kSplitActScale, -kSplitActMax), kSplitActMax);
-    v1 = fminf(fmaxf(v1 * kSplitActScale, -kSplitActMax), kSplitActMax);
-    const __half h0 = __float2half_rn(v0), h1 = __float2half_rn(v1);
-    const size_t lo = o + (size_t)e.split_stride * 8;
-    // split-half outputs are channel-blocked and gated with whole blocks: c is even, c + 1 is in the same block
-    *reinterpret_cast<uint32_t*>(y + o) = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-    *reinterpret_cast<uint32_t*>(y + lo) = pack_f16x2(v0 - __half2float(h0), v1 - __half2float(h1));
-    return;
-  }
-  const bool paired = two && (e.out_c8 != 0 || ((e.ldo | e.choff) & 1) == 0);
-  if (e.out_dt == DT_F32) {
-    float* y = reinterpret_cast<float*>(e.y) + o;
-    if (paired) *reinterpret_cast<float2*>(y) = make_float2(v0, v1);
-    else { y[0] = v0; if (two) y[1] = v1; }
-  } else {
-    __nv_bfloat16* y = reinterpret_cast<__nv_bfloat16*>(e.y) + o;
-    if (paired) *reinterpret_cast<uint32_t*>(y) = pack_bf16x2(v0, v1);
-    else { y[0] = __float2bfloat16(v0); if (two) y[1] = __float2bfloat16(v1); }
-  }
+__device__ __forceinline__ float2 lds_f2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
+  return v;
 }
 
-// Fused epilogue of one 64 x NT accumulator fragment (one warpgroup's half of a 128-position tile):
-//   gated : out[c] = act(acc[c] + b[c]) * sigmoid(acc[goff + c] + b[Cout/2 + c])   (goff = NT / 2 for every gated layer)
-//   linear: out[c] = (acc[c] + b[c]) * scale * colscale[img][c]
-// pix(h) gives this thread's output pixel (and whether it exists) for fragment row half h. Channel-blocked outputs also get
-// the padding channels of their last block written (as 0: padding columns hold zero weights and zero bias), because the
-// next layer's tensor-core MMAs read whole blocks.
-template <int NT, typename PixFn>
-__device__ __forceinline__ void conv_epilogue(const EpiParams& e, const float* cst, int cst_n, const float (&acc)[NT / 2], int img, int lane, PixFn pix) {
-  const bool split = e.nsplit > 1;
-  const bool elu = e.epi == EPI_GATE_ELU;
+// Fused gated epilogue of one 64 x NT accumulator fragment (one warpgroup's half of a 128-position tile):
+//   out[c] = act(acc[c] + b[c]) * sigmoid(acc[goff + c] + b[Cout/2 + c])   (goff = NT / 2, act = ELU or ReLU: kElu)
+// kF16: split-half output (exact-class math, hi and lo stores). kPaired: every column pair of the fragment is one aligned
+// 4 B store (channel-blocked outputs, or NHWC with even pitch / offset and Cout / 2 = goff); otherwise NHWC stores are per
+// channel and stop at Cout / 2. Channel-blocked outputs also get the padding channels of their last block written (as 0:
+// padding columns hold zero weights and zero bias), because the next layer's tensor-core MMAs read whole blocks.
+// Everything that depends on the launch only (mode, layout, block strides) is resolved outside the unrolled loop: row half h of
+// the fragment writes pixel offset base[h] (if ok[h]), block j at base[h] + j * blk_stride. `cst` = shared-memory address
+// of the constants (epi_fill_constants, n = NT + 32).
+template <int NT, bool kF16, bool kElu, bool kPaired>
+__device__ __forceinline__ void conv_epilogue(const EpiParams& e, uint32_t cst, const float (&acc)[NT / 2], const size_t (&base)[2],
+                                              const bool (&ok)[2], int lane) {
+  static_assert(!kF16 || kPaired, "split-half outputs are channel-blocked");
+  constexpr int n = NT + 32, goff = NT / 2, G = NT / 16;   // G: fragment block of the gate column goff + c
+  const int c0 = 2 * (lane & 3);
+  const uint32_t cq = cst + 4u * (uint32_t)c0;
+  const int lim = e.Cout >> 1;   // NHWC (not paired): channels written
+  const uint32_t jump = (uint32_t)e.blk_jump * 8u;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    int oy, ox;
-    if (!pix(h, oy, ox)) continue;
-    if (e.epi == EPI_LINEAR) {
-      const float* cs = e.colscale ? e.colscale + (size_t)img * e.Cout : nullptr;
-      const int lim = e.out_c8 ? (e.Cout + 7) / 8 * 8 : e.Cout;
+    if (!ok[h]) continue;
+    if constexpr (kF16) {
+      __half* y = reinterpret_cast<__half*>(e.y) + base[h];
+      __half* ylo = y + (size_t)e.split_stride * 8;   // the lo part of a block, split_stride 16 B units further on
 #pragma unroll
-      for (int j = 0; j < NT / 8; ++j) {
-        const int c = frag_col(lane, j);
-        if (c >= lim) continue;
-        float v0 = 0.0f, v1 = 0.0f;
-        if (c < e.Cout) {
-          v0 = (acc[4 * j + 2 * h] + (e.has_bias ? cst[c] : 0.0f)) * e.scale * (cs ? __ldg(cs + c) : 1.0f);
-        }
-        if (c + 1 < e.Cout) {
-          v1 = (acc[4 * j + 2 * h + 1] + (e.has_bias ? cst[c + 1] : 0.0f)) * e.scale * (cs ? __ldg(cs + c + 1) : 1.0f);
-        }
-        epi_store2(e, img, oy, ox, c, v0, v1, c + 1 < lim);
+      for (int j = 0; j < G; ++j) {
+        const float2 b = lds_f2(cq + 32u * j), hb = lds_f2(cq + 4u * (2 * n + goff) + 32u * j);
+        float v0 = gate_one_exact<kElu>(acc[4 * j + 2 * h], acc[4 * (j + G) + 2 * h], b.x, hb.x, e.scale);
+        float v1 = gate_one_exact<kElu>(acc[4 * j + 2 * h + 1], acc[4 * (j + G) + 2 * h + 1], b.y, hb.y, e.scale);
+        // split-half output: hi = fp16(64 v), lo = fp16(64 v - hi)
+        v0 = fminf(fmaxf(v0 * kSplitActScale, -kSplitActMax), kSplitActMax);
+        v1 = fminf(fmaxf(v1 * kSplitActScale, -kSplitActMax), kSplitActMax);
+        const __half h0 = __float2half_rn(v0), h1 = __float2half_rn(v1);
+        const uint32_t off = (uint32_t)j * (uint32_t)e.blk_stride + (j >= e.blk_split ? jump : 0u);
+        *reinterpret_cast<uint32_t*>(y + off) = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
+        *reinterpret_cast<uint32_t*>(ylo + off) = pack_f16x2(v0 - __half2float(h0), v1 - __half2float(h1));
       }
-      continue;
-    }
-    const int lim = e.out_c8 ? e.goff : (e.Cout >> 1);
+    } else {
+      __nv_bfloat16* y = reinterpret_cast<__nv_bfloat16*>(e.y) + base[h];
 #pragma unroll
-    for (int j = 0; j < NT / 16; ++j) {
-      const int c = frag_col(lane, j);
-      if (c >= lim) continue;
-      constexpr int G = NT / 16;   // fragment block of the gate column goff + c (goff = NT / 2)
-      float o[2];
-#pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        const float f = acc[4 * j + 2 * h + k], g = acc[4 * (j + G) + 2 * h + k];
-        const float b = cst[c + k], hb = cst[2 * cst_n + e.goff + c + k];
-        if (split) o[k] = elu ? gate_one_exact<true>(f, g, b, hb, e.scale) : gate_one_exact<false>(f, g, b, hb, e.scale);
-        else {
-          const float bl = cst[cst_n + c + k];
-          o[k] = elu ? gate_one<true>(f, g, b, bl, hb) : gate_one<false>(f, g, b, bl, hb);
+      for (int j = 0; j < G; ++j) {
+        const float2 b = lds_f2(cq + 32u * j), hb = lds_f2(cq + 4u * (2 * n + goff) + 32u * j);
+        float2 bl = make_float2(0.0f, 0.0f);
+        if constexpr (kElu) bl = lds_f2(cq + 4u * n + 32u * j);
+        const float v0 = gate_one<kElu>(acc[4 * j + 2 * h], acc[4 * (j + G) + 2 * h], b.x, bl.x, hb.x);
+        const float v1 = gate_one<kElu>(acc[4 * j + 2 * h + 1], acc[4 * (j + G) + 2 * h + 1], b.y, bl.y, hb.y);
+        const uint32_t off = (uint32_t)j * (uint32_t)e.blk_stride + (j >= e.blk_split ? jump : 0u);
+        if constexpr (kPaired) {
+          *reinterpret_cast<uint32_t*>(y + off) = pack_bf16x2(v0, v1);
+        } else {
+          const int c = 8 * j + c0;
+          if (c < lim) y[off] = __float2bfloat16(v0);
+          if (c + 1 < lim) y[off + 1] = __float2bfloat16(v1);
         }
       }
-      epi_store2(e, img, oy, ox, c, o[0], o[1], c + 1 < lim);
     }
   }
 }
