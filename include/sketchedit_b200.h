@@ -26,7 +26,10 @@ enum {
   SE_PREC_BF16_DIRECT = 2, /* bf16 activations, CUDA-core kernels (cross-check of the tensor-core path) */
   SE_PREC_FP32_TC = 3      /* fp32-parity arithmetic ON the tensor cores: activations and weights as fp16 hi + fp16 lo pairs (22
                               significant bits), three wgmma products per tap (hi*hi + hi*lo + lo*hi), fp32 accumulation and exact-math
-                              epilogue. The fp32 parity config (1e-3) runs here; SE_PREC_FP32_EXACT stays as its cross-check. */
+                              epilogue. The fp32 parity config (1e-3) runs here; SE_PREC_FP32_EXACT stays as its cross-check.
+                              Range: pairs store 64 v, saturated at +-65000, so inputs and activations with |v| > 65000 / 64
+                              (about 1015.6) are silently clamped; below 2^-9 the lo half is an fp16 subnormal (absolute
+                              quantum 2^-30). */
 };
 
 /* model options == the reference's command-line flags read on the hot path

@@ -132,8 +132,18 @@ def cam_flops_per_image(H, W, c=2 * CNUM, patch=4, stride=2):
 
 def _out_hw(name, H, W):
     import re
-    m = re.search(r"(\d+)", name)
-    idx = int(m.group(1))
+    return _out_hw_at_index(int(re.search(r"(\d+)", name).group(1)), H, W)
+
+
+def in_hw(name, H, W):
+    """input size of layer `name` in an H x W forward: the output size of the layer before it."""
+    import re
+    idx = int(re.search(r"(\d+)", name).group(1))
+    return (H, W) if idx == 1 else _out_hw_at_index(idx - 1, H, W)
+
+
+def _out_hw_at_index(idx, H, W):
+    """output size of the layers numbered idx (conv<idx>, xconv<idx>, conv_mask_<idx>, ...) in an H x W forward."""
     if idx == 1:
         return H, W
     if idx in (2, 3):

@@ -9,9 +9,16 @@ import torch
 import torch.nn.functional as F
 
 
-def contextual_attention_at(feat, mask_s, pixels, patch=4, stride=2, th=0.1, scale=10.0, key_rows=32):
+def contextual_attention_at(feat, mask_s, pixels, patch=4, stride=2, th=0.1, scale=10.0, key_rows=32, err=None):
     """feat [B, C, h, w], mask_s [B, 1, h, w] (as contextual_attention); pixels: iterable of (b, y, x).
-    Returns fp64 [len(pixels), C]: out[b, :, y, x] of contextual_attention(feat, mask_s)."""
+    Returns fp64 [len(pixels), C]: out[b, :, y, x] of contextual_attention(feat, mask_s).
+
+    With err = dict(logit_rel, logit_abs, rel, abs) it also returns an error bound of an implementation whose logits are
+    good to delta_n = logit_rel * max_l |scale m_l q_n| . |k_l| + logit_abs (query n; masked keys have the exact logit 0) and
+    whose softmax-weighted sums are good to rel * sum_l P_l |V_l| + abs: a softmax whose logits move by at most delta moves
+    each P_l by at most P_l (exp(2 delta) - 1), so query n's output element d is off by at most
+    (exp(2 delta_n) - 1 + rel) * sum_l P_l |V_ld| + abs. Returns (out, dict(bound [npix, C] summed over the <= 4 queries a
+    pixel reads))."""
     f = feat.detach().to("cpu", torch.float64)
     ms = mask_s.detach().to("cpu", torch.float64)
     B, C, h, w = f.shape
@@ -20,6 +27,7 @@ def contextual_attention_at(feat, mask_s, pixels, patch=4, stride=2, th=0.1, sca
     valid = (F.avg_pool2d(1.0 - ms, patch, stride)[:, 0] > th).to(torch.float64)           # [B, hs, ws]
     pixels = [tuple(int(v) for v in p) for p in pixels]
     out = torch.zeros(len(pixels), C, dtype=torch.float64)
+    bound = torch.zeros(len(pixels), C, dtype=torch.float64)
     for b in sorted({p[0] for p in pixels}):
         # queries read by the pixels of this image: pixel (y, x) += O[n][(c, u, v)] for 2 ny + u = y, 2 nx + v = x
         uses = []
@@ -39,6 +47,8 @@ def contextual_attention_at(feat, mask_s, pixels, patch=4, stride=2, th=0.1, sca
         m_run = torch.full((len(queries), 1), -float("inf"), dtype=torch.float64)
         s_run = torch.zeros(len(queries), 1, dtype=torch.float64)
         acc = torch.zeros(len(queries), Q.shape[1], dtype=torch.float64)
+        acc_abs = torch.zeros_like(acc)
+        qk_max = torch.zeros(len(queries), dtype=torch.float64)
         for k0 in range(0, hs, key_rows):
             k1 = min(k0 + key_rows, hs)
             rows = f[b:b + 1, :, stride * k0:stride * (k1 - 1) + patch]
@@ -51,9 +61,20 @@ def contextual_attention_at(feat, mask_s, pixels, patch=4, stride=2, th=0.1, sca
             s_run = s_run * corr + e.sum(1, keepdim=True)
             acc = acc * corr + e @ V.T
             m_run = m_new
+            if err is not None:
+                acc_abs = acc_abs * corr + e @ V.abs().T
+                qk_max = torch.maximum(qk_max, ((Q.abs() @ K.abs()) * valid[b, k0:k1].reshape(1, -1) * scale).max(1).values)
         O = acc / s_run                                                                   # [queries, (c, u, v)]
+        if err is not None:
+            PV = acc_abs / s_run
+            d_n = err["logit_rel"] * qk_max + err["logit_abs"]
+            Bq = (torch.expm1(2 * d_n)[:, None] + err["rel"]) * PV + err["abs"]
         for i, q, u, v in uses:
             out[i] += O[qi[q]].view(C, patch, patch)[:, u, v]
+            if err is not None:
+                bound[i] += Bq[qi[q]].view(C, patch, patch)[:, u, v]
+    if err is not None:
+        return out, dict(bound=bound)
     return out
 
 
