@@ -19,6 +19,9 @@
 
 #include <stdlib.h>
 
+#include <map>
+#include <mutex>
+
 #include "se_tc_device.cuh"
 
 namespace se {
@@ -65,10 +68,14 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  // 2-CTA cluster (streamed weights): both CTAs run the same number of tiles in lockstep and share every B stage, rank r
+  // multicasting part r of it; a stage slot is free when the consumers of BOTH CTAs have released it
+  const bool clustered = p.cluster > 1;
+  const uint32_t rank = clustered ? cluster_ctarank() : 0u;
   if (threadIdx.x == 0) {
     for (int i = 0; i < C8_MAX_STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], C8_CONSUMER_WARPS);   // one arrival per consumer warp
+      mbar_init(&empty_bar[i], C8_CONSUMER_WARPS * p.cluster);   // one arrival per consumer warp of each CTA
     }
     for (int i = 0; i < C8_MAX_ABUFS; ++i) {
       mbar_init(&a_full[i], 1);
@@ -79,10 +86,16 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
   }
   const int cst_n = NT + 32;
   epi_fill_constants(bias_s, cst_n, p.bias, p.e, threadIdx.x, C8_THREADS);
-  __syncthreads();
+  // a cluster's barriers are initialised before any multicast or remote arrive reaches them
+  if (clustered) cluster_sync();
+  else __syncthreads();
 
   const int total_tiles = p.N * p.tiles_x * p.tiles_y;
   const int ksteps = p.ksteps;
+  // CTA b runs tiles b, b + gridDim.x, ... (gridDim.x = 2 x clusters: rank r of cluster q runs tiles 2 (q + k G) + r) for as
+  // long as its cluster's rank-0 tile exists; when that one is the last tile, rank 1 is a PHANTOM for the pair: it loads no
+  // A, issues its B parts and releases the stages unread, so that its partner's stages complete
+  const int first_tile = (int)blockIdx.x - (int)rank;
 
   if (warp == C8_CONSUMER_WARPS) {
     // ==================================================================== producer
@@ -96,11 +109,14 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
       }
     }
     __syncwarp();
+    // B stage part of this CTA: all of it, or (cluster) part `rank` of a split at whole 1024 B swizzle atoms
+    const int b_split = (b_bytes >> 11) << 10;
+    const int b_off = rank ? b_split : 0, b_len = clustered ? (rank ? b_bytes - b_split : b_split) : b_bytes;
     int stage = 0, iter = 0;
     uint32_t phase = 0;
     // tile coordinates advance incrementally by gridDim.x tiles (mixed radix step), no per-tile integer division
     int tx = blockIdx.x % p.tiles_x, ty = (blockIdx.x / p.tiles_x) % p.tiles_y, img = blockIdx.x / (p.tiles_x * p.tiles_y);
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
+    for (int tile = blockIdx.x; tile - (int)rank < total_tiles; tile += gridDim.x, ++iter) {
       if (tile != (int)blockIdx.x) {
         tx += p.step_x;
         if (tx >= p.tiles_x) { tx -= p.tiles_x; ++ty; }
@@ -109,7 +125,8 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
         img += p.step_img;
       }
       const int x0 = tx * C8_TW, y0 = ty * C8_TH;
-      if (halo) {
+      const bool load_a = tile < total_tiles;   // false: phantom
+      if (halo && load_a) {
         int ab;
         uint32_t aphase;
         ring_of(iter, p.a_bufs, p.a_shift, ab, aphase);
@@ -125,9 +142,14 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
           mbar_wait(&empty_bar[stage], phase ^ 1, 1);
           uint8_t* st = sStages + (size_t)stage * stage_bytes;
           if (elect_one()) {
-            mbar_expect_tx(&full_bar[stage], (uint32_t)((halo ? 0 : p.a_tx_bytes) + stage_b));
-            if (!p.resident) bulk_load_1d(st + stage_a, p.w + (size_t)ks * b_bytes, (uint32_t)b_bytes, &full_bar[stage]);
-            if (!halo) {   // PERTAP: a stage is one tap, or one 64-channel chunk of a tap (cpt > 1)
+            // (cluster: the whole B stage lands here, the partner's part possibly before this expect_tx)
+            mbar_expect_tx(&full_bar[stage], (uint32_t)((halo || !load_a ? 0 : p.a_tx_bytes) + stage_b));
+            if (!p.resident) {
+              const uint8_t* src = p.w + (size_t)ks * b_bytes + b_off;
+              if (clustered) bulk_load_1d_multicast(st + stage_a + b_off, src, (uint32_t)b_len, &full_bar[stage], 0x3);
+              else bulk_load_1d(st + stage_a, src, (uint32_t)b_len, &full_bar[stage]);
+            }
+            if (!halo && load_a) {   // PERTAP: a stage is one tap, or one 64-channel chunk of a tap (cpt > 1)
               const int t = ks / p.cpt, ch = ks - t * p.cpt;
               tma_load_4d(st, &tmA, &full_bar[stage], (x0 + p.dx[t]) * 8, y0 + p.dy[t], p.x_cb_off + p.tap_cb[t] + 8 * ch, img);
             }
@@ -154,15 +176,31 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
       __syncwarp();
       if (lane == 0) mbar_arrive(bar);
     };
+    // a weight stage is released on this CTA's barrier and (cluster) on the partner's
+    auto release_stage = [&](int s) {
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&empty_bar[s]);
+        if (clustered) mbar_arrive_cluster(&empty_bar[s], rank ^ 1u);
+      }
+    };
     float acc[NT / 2];
 #pragma unroll
     for (int i = 0; i < NT / 2; ++i) acc[i] = 0.0f;
     int stage = 0;
     uint32_t phase = 0;
-    const int my_tiles = ((int)blockIdx.x < total_tiles) ? (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
+    const int my_tiles = (first_tile < total_tiles) ? (total_tiles - first_tile + (int)gridDim.x - 1) / (int)gridDim.x : 0;
     for (int v = 0; v < my_tiles * ncls; ++v) {
       const int riter = ncls == 1 ? v : v / ncls, cls = v - riter * ncls;
       const int tile = (int)blockIdx.x + riter * (int)gridDim.x;
+      if (tile >= total_tiles) {   // phantom (clusters stream their weights: ncls == 1)
+        for (int ks = 0; ks < ksteps; ++ks) {
+          mbar_wait(&full_bar[stage], phase, 3);
+          release_stage(stage);
+          if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
+        }
+        continue;
+      }
       const uint32_t img_u = (uint32_t)tile / tpi, rem = (uint32_t)tile - img_u * tpi;
       const uint32_t ty_u = rem / (uint32_t)p.tiles_x;
       const int img = (int)img_u, ty = (int)ty_u, tx = (int)(rem - ty_u * (uint32_t)p.tiles_x);
@@ -207,7 +245,7 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
           // keep one k-step in flight: the previous k-step's stage is free once its group has completed
           if (prev >= 0) {
             wg_wait<1>();
-            release(&empty_bar[prev]);
+            release_stage(prev);
           }
           prev = stage;
           if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
@@ -215,7 +253,7 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
       }
       wg_wait<0>();
       wg_fence_acc(acc);
-      if (prev >= 0) release(&empty_bar[prev]);
+      if (prev >= 0) release_stage(prev);
       if (halo && cls == ncls - 1) release(&a_empty[ab]);
       // output pixel of fragment row half h (sub-pixel classes: osy = osx = 2 and a per-class offset)
       const int ooy = ncls > 1 ? p.cls_ooy[cls] : p.e.ooy, oox = ncls > 1 ? p.cls_oox[cls] : p.e.oox;
@@ -237,6 +275,8 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
       }
     }
   }
+  // no CTA of a cluster exits while its partner may still multicast into its shared memory or arrive on its barriers
+  if (clustered) cluster_sync();
 }
 
 // ------------------------------------------------------------------------------------------ host
@@ -361,16 +401,47 @@ static int c8_set_smem_attr(int bytes) {
 #undef X
   return 0;
 }
-static int c8_dispatch(const C8Params& p, const CUtensorMap& tmA, int grid, int smem_bytes, cudaStream_t stream) {
-#define X(n)                                                                                      \
-  if (p.NT == n) {                                                                                \
-    if (p.f16) conv_c8_kernel<n, true><<<grid, C8_THREADS, smem_bytes, stream>>>(tmA, p);         \
-    else conv_c8_kernel<n, false><<<grid, C8_THREADS, smem_bytes, stream>>>(tmA, p);              \
-    return 0;                                                                                     \
-  }
+typedef void (*C8Kernel)(CUtensorMap, C8Params);
+static C8Kernel c8_kernel(const C8Params& p) {
+#define X(n) \
+  if (p.NT == n) return p.f16 ? conv_c8_kernel<n, true> : conv_c8_kernel<n, false>;
   C8_NT_LIST(X)
 #undef X
-  SE_REQUIRE(false, "no instantiation for N = " + std::to_string(p.NT));
+  return nullptr;
+}
+static void c8_launch_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, int grid, int smem_bytes, int cluster, cudaStream_t stream) {
+  *cfg = cudaLaunchConfig_t();
+  cfg->gridDim = dim3(grid);
+  cfg->blockDim = dim3(C8_THREADS);
+  cfg->dynamicSmemBytes = smem_bytes;
+  cfg->stream = stream;
+  if (cluster > 1) {
+    attr->id = cudaLaunchAttributeClusterDimension;
+    attr->val.clusterDim.x = cluster;
+    attr->val.clusterDim.y = 1;
+    attr->val.clusterDim.z = 1;
+    cfg->attrs = attr;
+    cfg->numAttrs = 1;
+  }
+}
+// clusters of 2 CTAs that can be resident at once, per (instantiation, shared memory size); asked once, outside graph capture
+// (the engine runs a launch sequence eagerly before it captures it)
+static int c8_max_clusters(C8Kernel k, int smem_bytes, int* out) {
+  static std::mutex mu;
+  static std::map<std::pair<C8Kernel, int>, int> cache;
+  std::lock_guard<std::mutex> lock(mu);
+  auto it = cache.find({k, smem_bytes});
+  if (it == cache.end()) {
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr;
+    c8_launch_config(&cfg, &attr, 2 * g_sms, smem_bytes, 2, 0);
+    int n = 0;
+    SE_CUDA_OK(cudaOccupancyMaxActiveClusters(&n, k, &cfg));
+    SE_REQUIRE(n > 0, "no 2-CTA cluster of conv_c8_kernel fits on the device");
+    it = cache.emplace(std::make_pair(k, smem_bytes), n).first;
+  }
+  *out = it->second;
+  return 0;
 }
 
 static const int kGroupSmemMax = 222 * 1024;   // fused classes may use (almost) the whole opt-in window: weights of all classes + 2 halos
@@ -532,12 +603,24 @@ int c8_launch(const ConvParams& c, const C8Layer& L_in, cudaStream_t stream, con
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     SE_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(C8) failed, CUresult=" + std::to_string((int)r));
   }
-  const int grid = total_tiles < g_sms ? total_tiles : g_sms;
+  const C8Kernel kernel = c8_kernel(p);
+  SE_REQUIRE(kernel != nullptr, "no instantiation for N = " + std::to_string(p.NT));
+  // streamed weights: 2-CTA clusters read each weight stage from L2 once per pair of neighbouring tiles (TMA multicast)
+  p.cluster = L.resident ? 1 : 2;
+  int grid = total_tiles < g_sms ? total_tiles : g_sms;
+  if (p.cluster > 1) {
+    int max_clusters = 0;
+    { int rc_occ = c8_max_clusters(kernel, smem_bytes, &max_clusters); if (rc_occ) return rc_occ; }
+    const int pairs = (total_tiles + 1) / 2;
+    grid = 2 * (pairs < max_clusters ? pairs : max_clusters);
+  }
   p.step_x = grid % p.tiles_x;
   p.step_y = (grid / p.tiles_x) % p.tiles_y;
   p.step_img = grid / (p.tiles_x * p.tiles_y);
-  { int rc_launch = c8_dispatch(p, tmA, grid, smem_bytes, stream); if (rc_launch) return rc_launch; }
-  SE_CUDA_OK(cudaGetLastError());
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr;
+  c8_launch_config(&cfg, &attr, grid, smem_bytes, p.cluster, stream);
+  SE_CUDA_OK(cudaLaunchKernelEx(&cfg, kernel, tmA, p));
   return 0;
 }
 

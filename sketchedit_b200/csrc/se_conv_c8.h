@@ -60,6 +60,7 @@ struct C8Params {
   int cpt;                        // PERTAP mode: k-steps per tap (C8Layer::chunks_per_tap)
   int ncls, cls_bytes;            // fused deconv classes (C8Group): classes per tile, bytes between their weight images
   int cls_ooy[C8_MAX_CLS], cls_oox[C8_MAX_CLS];
+  int cluster;                    // CTAs per cluster: 2 = streamed weights, each B stage multicast to both CTAs; 1 otherwise
 };
 
 int c8_configure(C8Layer* L, int ntaps, const int8_t* dy, const int8_t* dx, int Ci, int Cout, bool stem, const int8_t* tap_cb = nullptr);

@@ -58,6 +58,31 @@ __device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_
                ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+// the same copy multicast to every CTA of the cluster in cta_mask: lands at dst's offset in each, completes on each CTA's own
+// mbarrier at bar's offset
+__device__ __forceinline__ void bulk_load_1d_multicast(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint16_t cta_mask) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
+               ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask)
+               : "memory");
+}
+
+// ------------------------------------------------------------------------------------------ thread-block clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster: orders shared-memory writes and mbarrier inits before it, across the cluster
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at bar's offset in the shared memory of cluster CTA `cta`. Release at CTA scope: a consumer
+// releases a stage its retired wgmma no longer reads, and that needs no fence. (.release.cluster puts a GPU-scope
+// MEMBAR before the arrive, which waits for every global store the thread has in flight, e.g. the previous epilogue's.)
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile("{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\tmbarrier.arrive.release.cta.shared::cluster.b64 _, [ra];\n\t}"
+               ::"r"(smem_u32(bar)), "r"(cta) : "memory");
+}
 
 // one lane of a fully converged warp
 __device__ __forceinline__ bool elect_one() {
