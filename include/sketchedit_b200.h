@@ -149,6 +149,33 @@ long long se_workspace_bytes(se_model* m);
 int se_timing_enable(int on);
 int se_timing_report(char* buf, int cap);
 
+/* ---- activation taps (debugging and tests; off by default, no cost when off). While on, every forward of the model runs
+ * eagerly (no CUDA graph is captured or replayed) and records one tap per stage input: a device copy of the raw bytes the
+ * consumer reads, in memory the model owns outside the workspace arena. Tap points: the input of every gated conv / deconv /
+ * stem pair ("in:<net>.<layer>", e.g. "in:G.conv11", "in:G.conv1+wconv1"), of every head ("in:G.conv17"), of the global
+ * style pooling ("in:G.pool"), and the attention's feature map and pooled mask ("in:G.cam", "in:G.cam.mask_s"); in
+ * SE_PREC_FP32_TC also the fp32 map the attention reads and the fp32 result it writes ("in:G.cam.f32", "out:G.cam.f32"),
+ * either side of the split-half conversions. Taps are dropped at the next forward of the model, at se_taps_enable and at se_model_destroy. */
+enum {
+  SE_TAP_LAYOUT = 0,   /* 0 NHWC, 1 channel-blocked [B][ld][H][W][8], 2 space-to-depth channel-blocked [B][ld][H/2][W/2][8],
+                          3 packed 8-channel stem rows [B][H][Wp][8] (image at x + padl) */
+  SE_TAP_DTYPE = 1,    /* 0 fp32, 1 bf16, 2 split-half fp16 pairs (64 v = hi + lo; the lo blocks follow the hi blocks:
+                          ld / 2 blocks further on, per parity group (CB blocks further on) in space-to-depth, one [H][Wp][8]
+                          plane further on in packed rows) */
+  SE_TAP_B = 2, SE_TAP_C = 3, SE_TAP_H = 4, SE_TAP_W = 5,   /* H, W: the full-resolution size also for space-to-depth */
+  SE_TAP_LD = 6,       /* NHWC: pixel pitch in elements; channel-blocked: channel blocks per image (both halves) */
+  SE_TAP_CB_OFF = 7,   /* first channel block of the view (channel-blocked, space-to-depth) */
+  SE_TAP_WP = 8, SE_TAP_PADL = 9,   /* packed rows: row length in pixels, zero pixels left of the image */
+  SE_TAP_DESC_LEN = 10
+};
+int se_taps_enable(se_model* m, int on);
+/* taps recorded by the model's last forward (-1: no model) */
+int se_taps_count(se_model* m);
+/* tap i: its name (NUL-terminated, truncated to name_cap bytes), desc[SE_TAP_DESC_LEN] and size in bytes (each may be NULL) */
+int se_tap_info(se_model* m, int i, char* name, int name_cap, int* desc, long long* bytes);
+/* enqueues a copy of tap i's bytes to the device pointer dst on stream */
+int se_tap_copy(se_model* m, int i, void* dst, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -49,6 +49,10 @@ SIGNATURES = {
     "se_workspace_bytes": (ctypes.c_longlong, [_c_void_p]),
     "se_timing_enable": (_c_int, [_c_int]),
     "se_timing_report": (_c_int, [_c_char_p, _c_int]),
+    "se_taps_enable": (_c_int, [_c_void_p, _c_int]),
+    "se_taps_count": (_c_int, [_c_void_p]),
+    "se_tap_info": (_c_int, [_c_void_p, _c_int, _c_char_p, _c_int, ctypes.POINTER(_c_int), ctypes.POINTER(ctypes.c_longlong)]),
+    "se_tap_copy": (_c_int, [_c_void_p, _c_int, _c_void_p, _c_void_p]),
 }
 
 _lib = None

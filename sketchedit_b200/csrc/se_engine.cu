@@ -191,6 +191,7 @@ struct ClassW {
 
 struct Layer {
   Spec spec;
+  char net = 0;                // 'M' or 'G'
   std::string name;
   int Ci = 0;                  // stored input channels (stems are packed to 8)
   bool is_head = false;
@@ -233,6 +234,10 @@ struct se_model {
   cudaStream_t last_stream = nullptr;
   bool used = false;
   cudaEvent_t order_ev = nullptr;
+  // activation taps (se_taps_enable): device copies of the stage inputs of the last forward, recorded by se::tap
+  struct Tap { std::string name; int desc[SE_TAP_DESC_LEN] = {}; void* p = nullptr; size_t bytes = 0; };
+  bool taps_on = false;
+  std::vector<Tap> taps;
 };
 
 namespace se {
@@ -604,9 +609,49 @@ static View stem_view(const Ctx& c, void* p, int H, int W) {
   return nhwc(p, H, W, 8, 8);
 }
 
+// ------------------------------------------------------------------------------------------ activation taps
+static void drop_taps(se_model* m) {
+  if (m->taps.empty()) return;
+  cudaDeviceSynchronize();   // a se_tap_copy may still read them
+  for (auto& t : m->taps) cudaFree(t.p);
+  m->taps.clear();
+}
+
+// records the bytes of view v as tap `name` (se_taps_enable): layout 0..2 = v.c8, 3 = packed stem rows; dtype -1 = the
+// mode's activation storage. Enqueued on the forward's stream before the consumer's launch, so the buffer is still live.
+static int tap(Ctx& c, const std::string& name, const View& v, int layout, int dtype = -1) {
+  if (c.dry || !c.m->taps_on) return 0;
+  se_model::Tap t;
+  t.name = name;
+  if (dtype < 0) dtype = c.act_dt() == DT_F32 ? 0 : (c.split() ? 2 : 1);
+  int* d = t.desc;
+  d[SE_TAP_LAYOUT] = layout; d[SE_TAP_DTYPE] = dtype; d[SE_TAP_B] = c.B; d[SE_TAP_C] = v.C; d[SE_TAP_H] = v.H; d[SE_TAP_W] = v.W;
+  d[SE_TAP_LD] = v.ld; d[SE_TAP_CB_OFF] = v.cb_off;
+  size_t elems;
+  if (layout == 3) {
+    d[SE_TAP_WP] = stem_wp(v.W); d[SE_TAP_PADL] = STEM_PADL;
+    elems = (size_t)c.B * v.H * stem_wp(v.W) * 8 * (dtype == 2 ? 2 : 1);
+  } else if (layout == 0) {
+    elems = (size_t)c.B * v.H * v.W * v.ld;
+  } else {
+    elems = (size_t)c.B * v.ld * (layout == 2 ? (size_t)(v.H / 2) * (v.W / 2) : (size_t)v.H * v.W) * 8;
+  }
+  t.bytes = elems * (dtype == 0 ? 4 : 2);
+  SE_CUDA_OK(cudaMalloc(&t.p, t.bytes));
+  c.m->taps.push_back(t);
+  SE_CUDA_OK(cudaMemcpyAsync(t.p, v.p, t.bytes, cudaMemcpyDeviceToDevice, c.stream));
+  return 0;
+}
+#define TAP(...)                  \
+  do {                            \
+    int _rt = tap(c, __VA_ARGS__); \
+    if (_rt) return _rt;          \
+  } while (0)
+
 // one gated conv / deconv layer: in (Hi x Wi x Ci) -> out (channels written at [choff, choff+cout_g), layout out_c8)
 static int run_layer(Ctx& c, Layer& L, const View& in, void* out, int ldo, int choff, int out_c8 = 0) {
   SE_REQUIRE(in.c8 == wants_c8(c, L), "activation layout mismatch at layer " + L.name);
+  TAP("in:" + std::string(1, L.net) + "." + L.name, in, L.is_stem ? 3 : in.c8);
   const Spec& s = L.spec;
   const int Ho = s.deconv ? in.H : (in.H + s.stride - 1) / s.stride;   // position grid
   const int Wo = s.deconv ? in.W : (in.W + s.stride - 1) / s.stride;
@@ -747,6 +792,7 @@ static int run_head(Ctx& c, char net, const std::string& name, const View& in, i
                     unsigned char* out_u8 = nullptr) {
   Layer* L = find_ready(c.m, net, name);
   SE_REQUIRE(L != nullptr && L->is_head, "head layer " + name + ": " + last_error());
+  TAP("in:" + std::string(1, net) + "." + name, in, in.c8);
   {
     // 12-channel map in (two channel blocks on the C8 path), image / mask planes in, cout (+ blend / pack) planes out
     const double px = (double)c.B * in.H * in.W;
@@ -945,6 +991,7 @@ static int do_pack8(Ctx& c, Act* out, const float* img, const float* sk, const f
 // global pooling of the 96-channel map v, broadcast into channels 96..191 of the concat buffer cat
 static int do_pool_broadcast(Ctx& c, const View& v, int mode, void* cat, int cat_ld) {
   const int HW = v.H * v.W;
+  TAP("in:G.pool", v, v.c8);
   Buf pooled = c.get((size_t)c.B * 96 * 4);
   c.tag("plane_reduce + broadcast_channels|global style pooling -> concat blocks", 0, 0, 0, 2.0 * c.B * v.H * v.W * 96 * (c.esz() > 2 ? 4 : 2));
   auto launch = [&](float* pl) -> int {   // one timed launch pair
@@ -1079,13 +1126,17 @@ static int run_netG(Ctx& c, const float* x, const float* x2, const float* mask, 
     Buf ms = c.get((size_t)c.B * h * w * 4);
     c.tag("avgpool4_kernel", 0, 0, 0, (double)c.B * H * W * 4);
     CK(avgpool4(mask, (float*)ms.p, c.B, H, W, c.stream));
+    TAP("in:G.cam", pm.v, pm.v.c8);
+    TAP("in:G.cam.mask_s", nhwc(ms.p, h, w, 1, 1), 0, 0);
     Buf camo = c.get((size_t)c.B * h * w * 96 * e);
     if (c.split()) {
       // split-half mode: fp32 NHWC in / out of the attention (split-half fp16 GEMMs over explicit patch matrices, se_gemm_split.cu)
       Buf f32 = c.get((size_t)c.B * h * w * 96 * 4), o32 = c.get((size_t)c.B * h * w * 96 * 4);
       CK(split_to_f32(pm.v.p, (float*)f32.p, c.B, 96, h * w, pm.v.ld / 2, 0, 1, c.stream));
+      TAP("in:G.cam.f32", nhwc(f32.p, h, w, 96, 96), 0, 0);
       rc = run_cam_split(c, (const float*)f32.p, h, w, 96, (const float*)ms.p, (float*)o32.p);
       if (rc) return rc;
+      TAP("out:G.cam.f32", nhwc(o32.p, h, w, 96, 96), 0, 0);
       CK(nhwc_f32_to_split((const float*)o32.p, camo.p, c.B, 96, h * w, 12, 0, c.stream));
       c.put(o32); c.put(f32);
     } else {
@@ -1134,8 +1185,9 @@ static int with_arena(se_model* m, int prec, int B, cudaStream_t stream, F fn, s
     m->last_stream = stream;
     m->used = true;
   }
-  // ---- replay a captured forward
-  const bool graphable = g_graphs_on && !g_timing && !key.empty();
+  drop_taps(m);
+  // ---- replay a captured forward (a forward with taps on runs eagerly)
+  const bool graphable = g_graphs_on && !g_timing && !m->taps_on && !key.empty();
   const bool legacy = (stream == nullptr || stream == cudaStreamLegacy);
   cudaStream_t gs = stream;   // stream the graph is captured on / launched into
   if (graphable && legacy) {
@@ -1250,6 +1302,7 @@ static int make_stem_pair(se_model* m, const char* key, const char* a, const cha
   Layer* B = find_layer(m, 'G', b);
   if (!A || !B || !A->set || !B->set) return 0;
   Layer F;
+  F.net = 'G';
   F.name = key;
   F.spec = Spec{8, 96, 5, 1, 1, false, 0};
   F.set = true;
@@ -1297,6 +1350,7 @@ int se_model_create(se_model** out) {
     for (size_t i = 0; i < t.specs.size(); ++i) {
       Layer L;
       L.spec = t.specs[i];
+      L.net = net;
       L.name = t.names[i];
       m->layers[std::string(1, net) + "." + t.names[i]] = L;
     }
@@ -1307,6 +1361,7 @@ int se_model_create(se_model** out) {
 
 void se_model_destroy(se_model* m) {
   if (!m) return;
+  drop_taps(m);
   for (void* p : m->owned) cudaFree(p);
   if (m->arena) cudaFree(m->arena);
   if (m->order_ev) cudaEventDestroy(m->order_ev);
@@ -1583,6 +1638,43 @@ int se_outputs_to_uint8(const float* composed, const float* mask, int B, int H, 
 int se_set_attention_workspace_limit(long long bytes) {
   SE_REQUIRE(bytes >= 0, "attention workspace limit must be >= 0 bytes (0 = the default)");
   g_attn_limit = bytes ? bytes : kDefaultAttnLimit;
+  return 0;
+}
+
+int se_taps_enable(se_model* m, int on) {
+  SE_REQUIRE(m, "model");
+  std::lock_guard<std::mutex> lk(m->mu);
+  m->taps_on = on != 0;
+  drop_taps(m);
+  return 0;
+}
+
+int se_taps_count(se_model* m) {
+  if (!m) return -1;
+  std::lock_guard<std::mutex> lk(m->mu);
+  return (int)m->taps.size();
+}
+
+int se_tap_info(se_model* m, int i, char* name, int name_cap, int* desc, long long* bytes) {
+  SE_REQUIRE(m, "model");
+  std::lock_guard<std::mutex> lk(m->mu);
+  SE_REQUIRE(i >= 0 && i < (int)m->taps.size(), "tap index " + std::to_string(i) + " of " + std::to_string(m->taps.size()));
+  const se_model::Tap& t = m->taps[i];
+  if (name && name_cap > 0) {
+    const size_t n = std::min(t.name.size(), (size_t)name_cap - 1);
+    memcpy(name, t.name.data(), n);
+    name[n] = 0;
+  }
+  if (desc) memcpy(desc, t.desc, sizeof(t.desc));
+  if (bytes) *bytes = (long long)t.bytes;
+  return 0;
+}
+
+int se_tap_copy(se_model* m, int i, void* dst, void* stream) {
+  SE_REQUIRE(m && dst, "null argument");
+  std::lock_guard<std::mutex> lk(m->mu);
+  SE_REQUIRE(i >= 0 && i < (int)m->taps.size(), "tap index " + std::to_string(i) + " of " + std::to_string(m->taps.size()));
+  SE_CUDA_OK(cudaMemcpyAsync(dst, m->taps[i].p, m->taps[i].bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return 0;
 }
 

@@ -14,6 +14,10 @@ from . import _lib
 from .arch import NET_LAYERS, layer_map, out_channels_after_gate
 
 
+# fields of a tap descriptor, in the order of SE_TAP_LAYOUT .. SE_TAP_PADL (include/sketchedit_b200.h)
+TAP_DESC = ("layout", "dtype", "B", "C", "H", "W", "ld", "cb_off", "Wp", "padl")
+
+
 def _ptr(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
 
@@ -203,6 +207,24 @@ class Engine:
         _lib.check(self.lib.se_gated_conv_forward(self.h, net.encode(), name.encode(), _ptr(x), B, H, W, _lib.PREC[precision],
                                                   _ptr(y), _stream()))
         return y
+
+    def set_taps(self, on):
+        """Record the stored input of every stage of each following forward (include/sketchedit_b200.h, se_taps_enable);
+        those forwards run eagerly."""
+        _lib.check(self.lib.se_taps_enable(self.h, int(bool(on))))
+
+    def taps(self):
+        """{name: (desc, uint8 CUDA tensor of the raw bytes)} of the last forward; desc is a dict with the keys of TAP_DESC."""
+        out = {}
+        name = ctypes.create_string_buffer(256)
+        desc = (ctypes.c_int * len(TAP_DESC))()
+        nbytes = ctypes.c_longlong(0)
+        for i in range(int(self.lib.se_taps_count(self.h))):
+            _lib.check(self.lib.se_tap_info(self.h, i, name, len(name), desc, ctypes.byref(nbytes)))
+            raw = torch.empty(nbytes.value, device=self.device, dtype=torch.uint8)
+            _lib.check(self.lib.se_tap_copy(self.h, i, _ptr(raw), _stream()))
+            out[name.value.decode()] = (dict(zip(TAP_DESC, list(desc))), raw)
+        return out
 
     def launches(self):
         return int(self.lib.se_last_launch_count())

@@ -53,6 +53,22 @@ def test_shape_validation_without_gpu(lib_path):
     lib.se_model_destroy(h)
 
 
+def test_taps_without_gpu(lib_path):
+    """the activation-tap calls are host-side: a model that never ran a forward has no taps, with taps on or off, and an
+    index past the end is an error."""
+    lib = _lib.load()
+    h = ctypes.c_void_p()
+    assert lib.se_model_create(ctypes.byref(h)) == 0
+    assert lib.se_taps_count(h) == 0
+    assert lib.se_taps_enable(h, 1) == 0
+    assert lib.se_taps_count(h) == 0
+    assert lib.se_tap_info(h, 0, None, 0, None, None) != 0
+    assert b"tap index" in lib.se_last_error()
+    assert lib.se_taps_enable(h, 0) == 0
+    lib.se_model_destroy(h)
+    assert lib.se_taps_count(None) == -1
+
+
 def test_no_cpu_fallback(lib_path):
     """Without a CUDA device finalize must fail loudly, never fall back."""
     import torch
