@@ -19,11 +19,11 @@ extern "C" {
 
 typedef struct se_model se_model;
 
-/* arithmetic / storage mode of a forward call */
+/* arithmetic / storage mode of a forward call. Value 2 (bf16 activations on the CUDA-core kernels) is retired: every entry
+ * point rejects it. */
 enum {
   SE_PREC_BF16_TC = 0,     /* bf16 activations + weights, wgmma tensor-core kernels, fp32 accumulation */
   SE_PREC_FP32_EXACT = 1,  /* fp32 activations + weights, CUDA-core fp32 FMA kernels (fp32 parity config) */
-  SE_PREC_BF16_DIRECT = 2, /* bf16 activations, CUDA-core kernels (cross-check of the tensor-core path) */
   SE_PREC_FP32_TC = 3      /* fp32-parity arithmetic ON the tensor cores: activations and weights as fp16 hi + fp16 lo pairs (22
                               significant bits), three wgmma products per tap (hi*hi + hi*lo + lo*hi), fp32 accumulation and exact-math
                               epilogue. The fp32 parity config (1e-3) runs here; SE_PREC_FP32_EXACT stays as its cross-check.

@@ -87,5 +87,5 @@ def check(rc):
 
 
 # "fp32": fp32-parity arithmetic on the tensor cores (split-half fp16, SE_PREC_FP32_TC); "fp32_direct": the fp32 CUDA-core kernels
-PREC = {"bf16": 0, "fp32": 3, "fp32_direct": 1, "bf16_direct": 2}
+PREC = {"bf16": 0, "fp32": 3, "fp32_direct": 1}
 OPT = {"use_cam": 0, "pool_avg": 1, "no_mask_cc": 2, "no_mask_coarse": 3, "joint_train_inp": 4}

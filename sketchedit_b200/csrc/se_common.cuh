@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -118,26 +119,25 @@ struct EpiParams {
 // |v| = 2^-9 and stays finite up to |v| = 1000 (saturating beyond). Weights are scaled per class by a power of two of their own
 // (ClassW::s_wscale); the epilogue multiplies the accumulator by 1 / (kSplitActScale * s_wscale) inside the bias FMA.
 constexpr float kSplitActScale = 64.0f, kSplitActInv = 1.0f / 64.0f, kSplitActMax = 65000.0f;
+
+#ifdef __CUDACC__
+// the split-half encoding of v times `scale` (kSplitActScale for activations) and its inverse (inv = 1 / scale)
+__device__ __forceinline__ void split_half(float v, float scale, __half& hi, __half& lo) {
+  const float s = fminf(fmaxf(v * scale, -kSplitActMax), kSplitActMax);
+  hi = __float2half_rn(s);
+  lo = __float2half_rn(s - __half2float(hi));
+}
+__device__ __forceinline__ float join_half(__half hi, __half lo, float inv) { return (__half2float(hi) + __half2float(lo)) * inv; }
+#endif
 // column of output channel n in the B (weight) image / accumulator of a gated layer
 inline int gated_goff(int Cout) { return ((Cout / 2) + 7) / 8 * 8; }
 inline int gated_column(int Cout, int n) { const int half = Cout / 2; return n < half ? n : gated_goff(Cout) + (n - half); }
 
 // ------------------------------------------------------------------------------------------
 #ifdef __CUDACC__
-__device__ __forceinline__ float bf16_bits_to_f32(uint16_t b) { return __uint_as_float(((uint32_t)b) << 16); }
-
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
-}
-
-__device__ __forceinline__ float fast_sigmoid(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
-
-__device__ __forceinline__ float elu1(float x) { return x > 0.0f ? x : (__expf(x) - 1.0f); }
-
-__device__ __forceinline__ float gate_act(float f, float g, int epi) {
-  float a = (epi == EPI_GATE_ELU) ? elu1(f) : fmaxf(f, 0.0f);
-  return a * fast_sigmoid(g);
 }
 #endif
 

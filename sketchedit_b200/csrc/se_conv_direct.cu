@@ -1,8 +1,8 @@
 // CUDA-core direct convolution with the same op descriptor as the wgmma kernel.
 //
-// Role: (1) the fp32-exact path (activations and weights in fp32, fp32 FMA accumulation) used for
-// the fp32 parity configuration, (2) the low-channel head layers (12 -> 3 / 12 -> 1) whose K does
-// not fill a tensor-core tile, (3) an on-device cross-check of the wgmma kernel in tests.
+// Roles: (1) every convolution of the fp32_direct mode, the cross-check of the tensor-core modes (activations and weights in
+// fp32, fp32 FMA accumulation, expf / expm1f), including its attention GEMMs, (2) the heads (12 -> 3 / 12 -> 1) of the
+// per-operator API in every mode.
 // Weights: fp32 [img][tap][Ci][CoutP] with CoutP = Cout rounded up to 4.
 #include "se_common.cuh"
 #include "se_conv_direct.h"
@@ -13,14 +13,6 @@ constexpr int DC_THREADS = TILE_M;   // one thread per output position of the 8 
 constexpr int DC_CK = 32;            // input channels staged per step
 constexpr int DC_CO = 32;            // accumulators per thread (16 feature + 16 gate, or 32 linear)
 
-template <typename TIn>
-__device__ __forceinline__ float ld_in(const TIn* p);
-template <>
-__device__ __forceinline__ float ld_in<float>(const float* p) { return *p; }
-template <>
-__device__ __forceinline__ float ld_in<__nv_bfloat16>(const __nv_bfloat16* p) { return __bfloat162float(*p); }
-
-template <typename TIn, bool kExactMath>
 __global__ void __launch_bounds__(DC_THREADS)
 conv_direct_kernel(const ConvParams p, const int CoutP) {
   __shared__ float ws[DC_CK][DC_CO];
@@ -54,7 +46,7 @@ conv_direct_kernel(const ConvParams p, const int CoutP) {
 #pragma unroll
   for (int i = 0; i < DC_CO; ++i) acc[i] = 0.0f;
 
-  const TIn* xin = reinterpret_cast<const TIn*>(p.x);
+  const float* xin = reinterpret_cast<const float*>(p.x);
   const float* wbase = reinterpret_cast<const float*>(p.w) + (size_t)img * p.w_img_stride;
 
   for (int t = 0; t < p.ntaps; ++t) {
@@ -62,7 +54,7 @@ conv_direct_kernel(const ConvParams p, const int CoutP) {
     const bool inb = valid && iy >= 0 && iy < p.Hi && ix >= 0 && ix < p.Wi;
     const long long row_pitch = p.x_row_pitch ? p.x_row_pitch : (long long)p.Wi * p.ldx;
     const long long img_pitch = p.x_img_pitch ? p.x_img_pitch : (long long)p.Hi * row_pitch;
-    const TIn* xp = xin + (size_t)img * img_pitch + (size_t)(inb ? iy : 0) * row_pitch + (size_t)(inb ? ix : 0) * p.ldx;
+    const float* xp = xin + (size_t)img * img_pitch + (size_t)(inb ? iy : 0) * row_pitch + (size_t)(inb ? ix : 0) * p.ldx;
     for (int c0 = 0; c0 < p.Ci; c0 += DC_CK) {
       const int cc = min(DC_CK, p.Ci - c0);
       __syncthreads();
@@ -74,7 +66,7 @@ conv_direct_kernel(const ConvParams p, const int CoutP) {
       __syncthreads();
       if (inb) {
         for (int ci = 0; ci < cc; ++ci) {
-          const float xv = ld_in<TIn>(xp + c0 + ci);
+          const float xv = xp[c0 + ci];
           const float4* wr = reinterpret_cast<const float4*>(&ws[ci][0]);
 #pragma unroll
           for (int s4 = 0; s4 < DC_CO / 4; ++s4) {
@@ -99,16 +91,8 @@ conv_direct_kernel(const ConvParams p, const int CoutP) {
       if (f < half) {
         const float fv = acc[s] + (p.bias ? p.bias[f] : 0.0f);
         const float gv = acc[s + DC_CO / 2] + (p.bias ? p.bias[half + f] : 0.0f);
-        float r;
-        if (kExactMath) {
-          const float a = (p.epi == EPI_GATE_ELU) ? (fv > 0.0f ? fv : expm1f(fv)) : fmaxf(fv, 0.0f);
-          r = a * (1.0f / (1.0f + expf(-gv)));
-        } else {
-          r = gate_act(fv, gv, p.epi);
-        }
-        const size_t o = opix * p.ldo + p.choff + f;
-        if (p.out_dt == DT_F32) reinterpret_cast<float*>(p.y)[o] = r;
-        else reinterpret_cast<__nv_bfloat16*>(p.y)[o] = __float2bfloat16(r);
+        const float a = (p.epi == EPI_GATE_ELU) ? (fv > 0.0f ? fv : expm1f(fv)) : fmaxf(fv, 0.0f);
+        reinterpret_cast<float*>(p.y)[opix * p.ldo + p.choff + f] = a * (1.0f / (1.0f + expf(-gv)));
       }
     }
   } else {
@@ -118,15 +102,14 @@ conv_direct_kernel(const ConvParams p, const int CoutP) {
       if (c < p.Cout) {
         float r = acc[s] + (p.bias ? p.bias[c] : 0.0f);
         r *= p.scale * (p.colscale ? p.colscale[(size_t)img * p.Cout + c] : 1.0f);
-        const size_t o = opix * p.ldo + p.choff + c;
-        if (p.out_dt == DT_F32) reinterpret_cast<float*>(p.y)[o] = r;
-        else reinterpret_cast<__nv_bfloat16*>(p.y)[o] = __float2bfloat16(r);
+        reinterpret_cast<float*>(p.y)[opix * p.ldo + p.choff + c] = r;
       }
     }
   }
 }
 
-int direct_launch(const ConvParams& c, int CoutP, bool exact_math, cudaStream_t stream) {
+int direct_launch(const ConvParams& c, int CoutP, cudaStream_t stream) {
+  SE_REQUIRE(c.in_dt == DT_F32 && c.out_dt == DT_F32, "the direct kernel reads and writes fp32");
   SE_REQUIRE(c.ntaps <= MAX_TAPS, "too many taps");
   SE_REQUIRE(CoutP >= c.Cout, "CoutP");
   const bool gated = c.epi != EPI_LINEAR;
@@ -135,13 +118,7 @@ int direct_launch(const ConvParams& c, int CoutP, bool exact_math, cudaStream_t 
   const int units = gated ? c.Cout / 2 : c.Cout;
   const int per = gated ? DC_CO / 2 : DC_CO;
   dim3 grid(tiles, (units + per - 1) / per, c.N);
-  if (c.in_dt == DT_F32) {
-    if (exact_math) conv_direct_kernel<float, true><<<grid, DC_THREADS, 0, stream>>>(c, CoutP);
-    else conv_direct_kernel<float, false><<<grid, DC_THREADS, 0, stream>>>(c, CoutP);
-  } else {
-    if (exact_math) conv_direct_kernel<__nv_bfloat16, true><<<grid, DC_THREADS, 0, stream>>>(c, CoutP);
-    else conv_direct_kernel<__nv_bfloat16, false><<<grid, DC_THREADS, 0, stream>>>(c, CoutP);
-  }
+  conv_direct_kernel<<<grid, DC_THREADS, 0, stream>>>(c, CoutP);
   SE_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -3,6 +3,6 @@
 #include "se_common.cuh"
 
 namespace se {
-// weights: fp32 [img][tap][Ci][CoutP]; exact_math selects expf/expm1f instead of the fast intrinsics.
-int direct_launch(const ConvParams& c, int CoutP, bool exact_math, cudaStream_t stream);
+// fp32 in and out; weights: fp32 [img][tap][Ci][CoutP]
+int direct_launch(const ConvParams& c, int CoutP, cudaStream_t stream);
 }  // namespace se

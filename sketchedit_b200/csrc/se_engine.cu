@@ -203,8 +203,7 @@ struct Layer {
   int pair_cin_sum = 0;        // fused_pair: real input channels of the two source layers together (algorithmic FLOPs)
   bool fused_pair = false;     // two 5x5 stems over the same packed input fused along N (tensor-core path; see make_stem_pair)
   float* bias = nullptr;       // device [cout]
-  float* w_head = nullptr;     // device [9][12][cout] (heads)
-  std::vector<float> w_head_host;   // same, host copy (kernel-parameter weights of the channel-blocked head kernel)
+  std::vector<float> w_head_host;   // heads: host [9][12][cout], the head kernel's by-value weights are built from it
 };
 
 }  // namespace se
@@ -380,8 +379,6 @@ static int pack_layer(se_model* m, Layer& L) {
     for (int t = 0; t < 9; ++t)
       for (int c = 0; c < 12; ++c)
         for (int o = 0; o < s.cout; ++o) wh[((size_t)t * 12 + c) * s.cout + o] = L.w_host[(((size_t)o * 12 + c) * 3 + t / 3) * 3 + t % 3];
-    rc = upload(m, wh.data(), wh.size() * 4, (void**)&L.w_head);
-    if (rc) return rc;
     L.w_head_host = wh;
   }
   if (L.is_stem) {
@@ -550,11 +547,12 @@ struct Ctx {
     if (!g_timing || dry) return;
     tag_.name = name; tag_.tensor = tensor; tag_.flops_alg = flops_alg; tag_.flops_exec = flops_exec; tag_.bytes_alg = bytes_alg; tag_.set = true;
   }
-  bool tc() const { return prec == SE_PREC_BF16_TC || prec == SE_PREC_FP32_TC; }   // wgmma kernels over channel-blocked activations
-  bool split() const { return prec == SE_PREC_FP32_TC; }                            // ... in split-half storage (DT_F16X2)
-  int sp() const { return split() ? 2 : 1; }                                        // channel-block multiplier of that storage
-  int act_dt() const { return prec == SE_PREC_FP32_EXACT ? DT_F32 : (split() ? DT_F16X2 : DT_BF16); }
-  size_t esz() const { return (prec == SE_PREC_FP32_EXACT || split()) ? 4 : 2; }
+  // the mode's activation storage: bf16 and split-half channel-blocked for the wgmma kernels, fp32 NHWC for the CUDA-core kernels
+  bool tc() const { return prec != SE_PREC_FP32_EXACT; }
+  bool split() const { return prec == SE_PREC_FP32_TC; }
+  int sp() const { return split() ? 2 : 1; }                                        // channel-block multiplier of the storage
+  int act_dt() const { return split() ? DT_F16X2 : tc() ? DT_BF16 : DT_F32; }
+  size_t esz() const { return prec == SE_PREC_BF16_TC ? 2 : 4; }
   Buf get(size_t bytes) { Buf b; b.bytes = bytes; b.p = arena.alloc(bytes); return b; }
   void put(Buf& b) { if (b.p) arena.release(b.p, b.bytes); b.p = nullptr; }
   void put(Act& a) { put(a.own); }
@@ -726,7 +724,7 @@ static int run_layer(Ctx& c, Layer& L, const View& in, void* out, int ldo, int c
     else if (c.tc()) CK(c8_launch(cp, cw.c8, c.stream, grp));
     else {
       cp.w = cw.w_direct;
-      CK(direct_launch(cp, cw.CoutP, c.prec == SE_PREC_FP32_EXACT, c.stream));
+      CK(direct_launch(cp, cw.CoutP, c.stream));
     }
   }
   return 0;
@@ -799,24 +797,13 @@ static int run_head(Ctx& c, char net, const std::string& name, const View& in, i
     const double bytes = px * ((in.c8 ? 16 : 12) * c.esz() + (img ? 12 : 0) + (mask_bin ? 4 : 0) + (mask_soft ? 4 : 0) + (out_nchw ? 4 * L->spec.cout : 0) +
                                (out2 ? 4 * (mode == HEAD_MASK ? 1 : L->spec.cout) : 0) + (out_pack8 ? 8 * c.esz() : 0));
     const double fl = 2.0 * px * 9 * 12 * L->spec.cout;
-    c.tag(std::string(in.c8 == 1 && c.act_dt() == DT_BF16 ? "head_c8_kernel" : "head_kernel") + "|12->" + std::to_string(L->spec.cout) + " k3 + " +
+    c.tag(std::string("head_kernel|12->") + std::to_string(L->spec.cout) + " k3 + " +
               (mode == HEAD_MASK ? "sigmoid+threshold" : mode == HEAD_TANH ? "tanh" : mode == HEAD_COARSE ? "tanh+blend+pack8" : "tanh+soft blend"),
           0, fl, fl, bytes);
   }
-  if (c.split()) {
-    SE_REQUIRE(in.c8 == 1 && in.ld == 4, "split-half head input: two channel blocks, hi + lo");
-    CK(head_split(in.p, L->w_head, L->bias, L->spec.cout, c.B, in.H, in.W, mode, img, mask_bin, mask_soft, out_nchw, out2, out_pack8,
-                  c.m->opt[SE_OPT_NO_MASK_COARSE], stem_wp(in.W), STEM_PADL, out_bs, msoft_bs, out_u8, c.stream));
-    return 0;
-  }
-  if (in.c8) {
-    SE_REQUIRE(in.c8 == 1 && c.act_dt() == DT_BF16, "a channel-blocked head input is bf16");
-    CK(head_c8(in.p, L->w_head_host.data(), L->b_host.data(), L->spec.cout, c.B, in.H, in.W, mode, img, mask_bin, mask_soft, out_nchw, out2,
-               out_pack8, c.m->opt[SE_OPT_NO_MASK_COARSE], stem_wp(in.W), STEM_PADL, out_bs, msoft_bs, out_u8, c.stream));
-    return 0;
-  }
-  CK(head(in.p, c.act_dt(), L->w_head, L->bias, L->spec.cout, c.B, in.H, in.W, mode, img, mask_bin, mask_soft, out_nchw, out2,
-          out_pack8, c.m->opt[SE_OPT_NO_MASK_COARSE], stem_wp(in.W), STEM_PADL, out_bs, msoft_bs, out_u8, c.stream));
+  SE_REQUIRE(in.c8 == (c.tc() ? 1 : 0) && in.ld == (c.tc() ? 2 * c.sp() : 12), "head input: dense 12 channels in the mode's storage");
+  CK(head(in.p, c.act_dt(), L->w_head_host.data(), L->b_host.data(), L->spec.cout, c.B, in.H, in.W, mode, img, mask_bin, mask_soft, out_nchw,
+          out2, out_pack8, c.m->opt[SE_OPT_NO_MASK_COARSE], stem_wp(in.W), STEM_PADL, out_bs, msoft_bs, out_u8, c.stream));
   return 0;
 }
 
@@ -844,19 +831,17 @@ static int run_cam_tc(Ctx& c, const View& f, const float* mask_s, void* out, flo
 }
 
 static int run_cam(Ctx& c, const View& f, const float* mask_s, void* out, int out_ld, float* attn_out /*fp32 [B,L,N] or null*/, int out_c8 = 0) {
-  SE_REQUIRE(f.c8 == 0, "attention reads an NHWC feature map");
+  SE_REQUIRE(f.c8 == 0 && c.act_dt() == DT_F32, "the CUDA-core attention reads an fp32 NHWC feature map");
   const int B = c.B, h = f.H, w = f.W, C = f.C;
   SE_REQUIRE(h % 2 == 0 && w % 2 == 0 && h >= 4 && w >= 4, "attention map must be even-sized and >= 4");
   const int hs = (h - 4) / 2 + 1, ws = (w - 4) / 2 + 1, L = hs * ws;
   const int Lpad = (L + 127) / 128 * 128;
-  // CUDA-core path (fp32 modes, the bf16 cross-check, and channel counts other than netG's 96): the tensor-core attention is
-  // run_cam_tc / se_cam.cu
-  const int dt = c.act_dt();
-
+  // CUDA-core path (fp32 modes; bf16 with channel counts other than netG's 96): the tensor-core attention is run_cam_tc / se_cam.cu
+  const float* fp = (const float*)f.p;
   Buf rnorm = c.get((size_t)B * C * 4);
   Buf colm = c.get((size_t)B * L * 4);
-  c.tag("plane_sumsq/rnorm|attention key norm", 0, 0, 0, (double)B * h * w * C * c.esz());
-  CK(plane_reduce(f.p, dt, B, h * w, C, f.ld, 0, RED_RNORM, (float*)rnorm.p, c.stream));
+  c.tag("plane_reduce|attention key norm", 0, 0, 0, (double)B * h * w * C * 4);
+  CK(plane_reduce(fp, DT_F32, B, h * w, C, f.ld, RED_RNORM, (float*)rnorm.p, c.stream));
   c.tag("cam_colmask_kernel", 0, 0, 0, (double)B * h * w * 4);
   CK(cam_colmask(mask_s, (float*)colm.p, B, h, w, hs, ws, 0.1f, c.stream));
 
@@ -864,14 +849,14 @@ static int run_cam(Ctx& c, const View& f, const float* mask_s, void* out, int ou
   const size_t kbytes = (size_t)B * 16 * C * Lpad * 4;   // keys as per-image conv kernels: fp32 [b][tap][c][Lpad]
   Buf kbuf = c.get(kbytes);
   SE_REQUIRE(f.ld == C, "attention input must be dense NHWC");
-  c.tag("cam_pack_k|attention key operand", 0, 0, 0, (double)B * h * w * C * c.esz() + (double)kbytes);
-  CK(cam_pack_k(f.p, dt, (const float*)rnorm.p, kbuf.p, B, h, w, C, ws, L, Lpad, c.stream));
+  c.tag("cam_pack_k|attention key operand", 0, 0, 0, (double)B * h * w * C * 4 + (double)kbytes);
+  CK(cam_pack_k(fp, (const float*)rnorm.p, (float*)kbuf.p, B, h, w, C, ws, L, Lpad, c.stream));
 
   // ---- bands of output class rows [y0, y1): S and P hold the query rows [qa, q1) those rows read (y0 - 1 .. y1 - 1, clipped
   // to the patch grid; the boundary query row is computed by both bands that read it). R = class rows per band: the tallest
   // whose S + P fit the attention workspace limit, every row when the attention map is wanted.
   const int Hs = h / 2;
-  const size_t qrow_bytes = (size_t)B * ws * Lpad * (4 + c.esz());   // one query row of S (fp32) and P
+  const size_t qrow_bytes = (size_t)B * ws * Lpad * 8;   // one query row of S and P (fp32)
   int R = Hs;
   if (!attn_out && qrow_bytes * hs > (size_t)c.attn_limit) {
     R = (int)((size_t)c.attn_limit / qrow_bytes) - 1;
@@ -889,7 +874,7 @@ static int run_cam(Ctx& c, const View& f, const float* mask_s, void* out, int ou
     {
       ConvParams cp;
       memset(&cp, 0, sizeof(cp));
-      cp.x = (const char*)f.p + (size_t)2 * qa * w * f.ld * c.esz(); cp.in_dt = dt; cp.N = B; cp.Hi = h - 2 * qa; cp.Wi = w; cp.Ci = C; cp.ldx = f.ld;
+      cp.x = fp + (size_t)2 * qa * w * f.ld; cp.in_dt = DT_F32; cp.N = B; cp.Hi = h - 2 * qa; cp.Wi = w; cp.Ci = C; cp.ldx = f.ld;
       cp.x_img_pitch = (long long)h * w * f.ld;
       cp.Ho = nq; cp.Wo = ws; cp.stride = 2; cp.ntaps = 16;
       for (int t = 0; t < 16; ++t) { cp.dy[t] = (int8_t)(t / 4); cp.dx[t] = (int8_t)(t % 4); }
@@ -900,8 +885,8 @@ static int run_cam(Ctx& c, const View& f, const float* mask_s, void* out, int ou
       cp.w = kbuf.p; cp.w_img_stride = (long long)16 * C * Lpad;
       const double nL = (double)nq * ws;
       c.tag("conv_direct_kernel|attention S=QK^T", 0, 2.0 * B * nL * (double)L * C * 16,
-            2.0 * B * nL * (double)L * C * 16, (double)B * h * w * C * c.esz() + (double)kbytes + (double)B * nL * Lpad * 4);
-      CK(direct_launch(cp, Lpad, c.prec == SE_PREC_FP32_EXACT, c.stream));
+            2.0 * B * nL * (double)L * C * 16, (double)B * h * w * C * 4 + (double)kbytes + (double)B * nL * Lpad * 4);
+      CK(direct_launch(cp, Lpad, c.stream));
     }
     if (last) {
       c.put(kbuf);
@@ -909,13 +894,13 @@ static int run_cam(Ctx& c, const View& f, const float* mask_s, void* out, int ou
     }
 
     // ---- softmax over keys -> P[b, n, 0..Lpad)
-    Buf pbuf = c.get((size_t)B * nq * ws * Lpad * c.esz());
-    c.tag("softmax_rows|attention", 0, 0, 0, (double)B * nq * ws * Lpad * (4 + c.esz()));
-    CK(softmax_rows((const float*)sbuf.p, Lpad, pbuf.p, dt, Lpad, (long long)B * nq * ws, L, c.stream));
+    Buf pbuf = c.get((size_t)B * nq * ws * Lpad * 4);
+    c.tag("softmax_rows|attention", 0, 0, 0, (double)B * nq * ws * Lpad * 8);
+    CK(softmax_rows((const float*)sbuf.p, Lpad, (float*)pbuf.p, Lpad, (long long)B * nq * ws, L, c.stream));
     if (attn_out) {
       // cam_1 returns [B, L(keys), hs, ws]: transpose of P (one band)
-      // (small, test-only path: done with the generic layout kernel, P viewed as NHWC with C = L keys)
-      CK(nhwc_to_nchw(pbuf.p, dt, attn_out, B, L, L, Lpad, 0, c.stream));
+      // (small, test-only path: done with the layout conversion, P viewed as an NHWC map of L x 1 pixels with C = L keys)
+      CK(act_to_f32(pbuf.p, DT_F32, Layout{LAYOUT_NHWC, L, 1, Lpad}, attn_out, 0, B, L, c.stream));
     }
     c.put(sbuf);
     if (last) c.put(colm);
@@ -923,17 +908,17 @@ static int run_cam(Ctx& c, const View& f, const float* mask_s, void* out, int ou
     // ---- values + fold-sum of class rows [y0, y1): query row y - a is P row y - a - qa
     if (!vbuf.p) {
       vbuf = c.get(4 * per_pc_bytes);
-      c.tag("cam_pack_v|attention value operand", 0, 0, 0, (double)B * h * w * C * c.esz() + 4.0 * per_pc_bytes);
-      CK(cam_pack_v(f.p, dt, vbuf.p, B, h, w, C, ws, L, Lpad, c.stream));
+      c.tag("cam_pack_v|attention value operand", 0, 0, 0, (double)B * h * w * C * 4 + 4.0 * per_pc_bytes);
+      CK(cam_pack_v(fp, (float*)vbuf.p, B, h, w, C, ws, L, Lpad, c.stream));
     }
     for (int pc = 0; pc < 4; ++pc) {
       ConvParams cp;
       memset(&cp, 0, sizeof(cp));
-      cp.x = pbuf.p; cp.in_dt = dt; cp.N = B; cp.Hi = nq; cp.Wi = ws; cp.Ci = Lpad; cp.ldx = Lpad;
+      cp.x = pbuf.p; cp.in_dt = DT_F32; cp.N = B; cp.Hi = nq; cp.Wi = ws; cp.Ci = Lpad; cp.ldx = Lpad;
       cp.Ho = y1 - y0; cp.Wo = w / 2; cp.stride = 1; cp.ntaps = 4;
       for (int t = 0; t < 4; ++t) { cp.dy[t] = (int8_t)(y0 - qa - t / 2); cp.dx[t] = (int8_t)(-(t % 2)); }
       cp.bias = nullptr; cp.Cout = C;
-      cp.y = out; cp.out_dt = dt; cp.Hout = h; cp.Wout = w; cp.ldo = out_c8 ? (C + 7) / 8 : out_ld; cp.choff = 0;
+      cp.y = out; cp.out_dt = DT_F32; cp.Hout = h; cp.Wout = w; cp.ldo = out_c8 ? (C + 7) / 8 : out_ld; cp.choff = 0;
       cp.out_c8 = out_c8;
       cp.osy = 2; cp.ooy = 2 * y0 + pc / 2; cp.osx = 2; cp.oox = pc % 2;
       cp.epi = EPI_LINEAR; cp.scale = 1.0f; cp.colscale = nullptr;
@@ -941,8 +926,8 @@ static int run_cam(Ctx& c, const View& f, const float* mask_s, void* out, int ou
       const double ny = y1 - y0;
       c.tag("conv_direct_kernel|attention out=fold(PV) class", 0,
             2.0 * B * ny * (w / 2) * (double)C * L * 4, 2.0 * B * ny * (w / 2) * (double)C * L * 4,
-            ((double)B * nq * ws * Lpad + (double)B * 4 * Lpad * C + (double)B * ny * (w / 2) * C) * c.esz());
-      CK(direct_launch(cp, C, c.prec == SE_PREC_FP32_EXACT, c.stream));
+            ((double)B * nq * ws * Lpad + (double)B * 4 * Lpad * C + (double)B * ny * (w / 2) * C) * 4);
+      CK(direct_launch(cp, C, c.stream));
     }
     if (last) c.put(vbuf);
     c.put(pbuf);
@@ -959,8 +944,8 @@ static int run_cam_split(Ctx& c, const float* f, int h, int w, int C, const floa
   }
   Buf rnorm = c.get((size_t)c.B * C * 4), colm = c.get((size_t)c.B * pl.L * 4);
   Buf q = c.get(pl.q_bytes), kn = c.get(pl.q_bytes), sb = c.get(pl.s_bytes), pb = c.get(pl.p_bytes), ob = c.get(pl.o_bytes);
-  c.tag("plane_sumsq/rnorm|attention key norm", 0, 0, 0, (double)c.B * h * w * C * 4);
-  CK(plane_reduce(f, DT_F32, c.B, h * w, C, C, 0, RED_RNORM, (float*)rnorm.p, c.stream));
+  c.tag("plane_reduce|attention key norm", 0, 0, 0, (double)c.B * h * w * C * 4);
+  CK(plane_reduce(f, DT_F32, c.B, h * w, C, C, RED_RNORM, (float*)rnorm.p, c.stream));
   c.tag("cam_colmask_kernel", 0, 0, 0, (double)c.B * h * w * 4);
   CK(cam_colmask(mask_s, (float*)colm.p, c.B, h, w, pl.hs, pl.ws, 0.1f, c.stream));
   const double fl = 2.0 * c.B * (double)pl.L * pl.L * pl.KQ * 2.0;   // S and PV, algorithmic (one product each)
@@ -983,8 +968,7 @@ static int do_pack8(Ctx& c, Act* out, const float* img, const float* sk, const f
                     int img2_mode = -1) {
   Buf in8 = c.get((size_t)c.B * H * stem_wp(W) * 8 * c.esz());
   c.tag("pack8_kernel|mask-mul + concat + cast", 0, 0, 0, (double)c.B * H * W * 20 + (double)c.B * H * stem_wp(W) * 8 * c.esz());
-  if (c.split()) CK(pack8_split(img, sk, mask, in8.p, c.B, H, W, stem_wp(W), STEM_PADL, img_mode, sscale, write_mask, c.stream));
-  else CK(pack8(img, sk, mask, in8.p, c.act_dt(), c.B, H, W, stem_wp(W), STEM_PADL, img_mode, sscale, write_mask, c.stream, img2_mode));
+  CK(pack8(img, sk, mask, in8.p, c.act_dt(), c.B, H, W, stem_wp(W), STEM_PADL, img_mode, sscale, write_mask, c.stream, img2_mode));
   *out = Act{stem_view(c, in8.p, H, W), in8};
   return 0;
 }
@@ -995,12 +979,8 @@ static int do_pool_broadcast(Ctx& c, const View& v, int mode, void* cat, int cat
   Buf pooled = c.get((size_t)c.B * 96 * 4);
   c.tag("plane_reduce + broadcast_channels|global style pooling -> concat blocks", 0, 0, 0, 2.0 * c.B * v.H * v.W * 96 * (c.esz() > 2 ? 4 : 2));
   auto launch = [&](float* pl) -> int {   // one timed launch pair
-    if (c.split()) {
-      int rc = plane_reduce_split(v.p, c.B, HW, 96, v.ld / 2, mode, pl, c.stream);
-      return rc ? rc : broadcast_split(pl, cat, c.B, HW, 96, cat_ld / 2, 96, c.stream);
-    }
-    int rc = plane_reduce(v.p, c.act_dt(), c.B, HW, 96, v.ld, v.c8, mode, pl, c.stream);
-    return rc ? rc : broadcast_channels(pl, cat, c.act_dt(), c.B, HW, 96, cat_ld, 96, c.tc() ? 1 : 0, c.stream);
+    int rc = plane_reduce(v.p, c.act_dt(), c.B, HW, 96, v.ld, mode, pl, c.stream);
+    return rc ? rc : broadcast_channels(pl, cat, c.act_dt(), c.B, HW, 96, cat_ld, 96, c.stream);
   };
   CK(launch((float*)pooled.p));
   c.put(pooled);
@@ -1132,12 +1112,13 @@ static int run_netG(Ctx& c, const float* x, const float* x2, const float* mask, 
     if (c.split()) {
       // split-half mode: fp32 NHWC in / out of the attention (split-half fp16 GEMMs over explicit patch matrices, se_gemm_split.cu)
       Buf f32 = c.get((size_t)c.B * h * w * 96 * 4), o32 = c.get((size_t)c.B * h * w * 96 * 4);
-      CK(split_to_f32(pm.v.p, (float*)f32.p, c.B, 96, h * w, pm.v.ld / 2, 0, 1, c.stream));
+      const Layout pml{LAYOUT_C8, h, w, pm.v.ld};
+      CK(act_to_f32(pm.v.p, DT_F16X2, pml, (float*)f32.p, 1, c.B, 96, c.stream));
       TAP("in:G.cam.f32", nhwc(f32.p, h, w, 96, 96), 0, 0);
       rc = run_cam_split(c, (const float*)f32.p, h, w, 96, (const float*)ms.p, (float*)o32.p);
       if (rc) return rc;
       TAP("out:G.cam.f32", nhwc(o32.p, h, w, 96, 96), 0, 0);
-      CK(nhwc_f32_to_split((const float*)o32.p, camo.p, c.B, 96, h * w, 12, 0, c.stream));
+      CK(f32_to_act((const float*)o32.p, 1, camo.p, DT_F16X2, pml, c.B, 96, c.stream));
       c.put(o32); c.put(f32);
     } else {
       rc = tc ? run_cam_tc(c, pm.v, (const float*)ms.p, camo.p, nullptr) : run_cam(c, pm.v, (const float*)ms.p, camo.p, 96, nullptr, 0);
@@ -1169,7 +1150,8 @@ constexpr size_t kMaxGraphs = 16;
 template <typename F>
 static int with_arena(se_model* m, int prec, int B, cudaStream_t stream, F fn, std::vector<uintptr_t> key = {}) {
   SE_REQUIRE(m && m->finalized, "model not finalized");
-  SE_REQUIRE(prec >= 0 && prec <= 3, "precision");
+  SE_REQUIRE(prec == SE_PREC_BF16_TC || prec == SE_PREC_FP32_TC || prec == SE_PREC_FP32_EXACT,
+             "precision " + std::to_string(prec) + ": the modes are SE_PREC_BF16_TC (0), SE_PREC_FP32_TC (3) and SE_PREC_FP32_EXACT (1)");
   std::lock_guard<std::mutex> model_lock(m->mu);
   {
     int dev = -1;
@@ -1518,66 +1500,55 @@ int se_gated_conv_forward(se_model* m, char net, const char* layer, const float*
   Layer* L = find_ready(m, net, layer);
   SE_REQUIRE(L != nullptr, std::string("no such (loaded) layer: ") + layer);
   cudaStream_t st = (cudaStream_t)stream;
-  // heads are raw fp32 CUDA-core convolutions in every mode; the fp32-on-tensor-cores mode runs them like the fp32 path
-  if (precision == SE_PREC_FP32_TC && L->is_head) precision = SE_PREC_FP32_EXACT;
   return with_arena(m, precision, B, st, [&](Ctx& c) -> int {
     const Spec& s = L->spec;
-    const int dt = c.act_dt();
-    const int Ci = L->is_head ? 12 : L->Ci;
-    const int in_c8 = wants_c8(c, *L);
-    Buf in = c.get(L->is_stem ? (size_t)B * H * stem_wp(W) * 8 * c.esz() : c.act_bytes(H, W, Ci, in_c8));
-    if (c.split()) {
-      // split-half storage: hi / lo fp16 halves of the fp32 input in the layout the layer reads
-      if (L->is_stem || s.cin % 8) CK(fill_zero(in.p, in.bytes, c.stream));
-      CK(nchw_to_split(x, in.p, B, s.cin, H, W, L->is_stem ? 3 : in_c8, stem_wp(W), STEM_PADL, c.stream));
-    } else if (L->is_stem) {
-      CK(fill_zero(in.p, in.bytes, c.stream));
-      CK(nchw_to_stem8(x, in.p, dt, B, s.cin, H, W, stem_wp(W), STEM_PADL, c.stream));
-    } else if (in_c8 == 2) {
-      CK(nchw_to_c8_s2d(x, in.p, B, s.cin, H, W, c.stream));
-    } else if (in_c8) {
-      if (s.cin % 8) CK(fill_zero(in.p, in.bytes, c.stream));
-      CK(nchw_to_c8(x, in.p, B, s.cin, H * W, c.stream));
-    } else {
-      CK(nchw_to_nhwc(x, in.p, dt, B, s.cin, H * W, Ci, 0, c.stream));
-    }
     int Ho, Wo;
     out_dims(s, H, W, &Ho, &Wo);
     if (L->is_head) {
-      // raw conv (activation=None / cout==3, utils.py:27): run through the direct kernel, fp32 out
-      Buf o = c.get((size_t)B * Ho * Wo * s.cout * 4);
+      // raw conv (activation=None / cout==3, utils.py:27) on the fp32 direct kernel in every mode, fp32 NHWC in and out; bf16
+      // rounds its input to bf16 first (through a bf16 copy), like the heads of its forward read it
+      const Layout lin{LAYOUT_NHWC, H, W, 12}, lout{LAYOUT_NHWC, Ho, Wo, s.cout};
+      Buf in = c.get((size_t)B * H * W * 12 * 4), o = c.get((size_t)B * Ho * Wo * s.cout * 4);
+      if (c.prec == SE_PREC_BF16_TC) {
+        Buf r = c.get((size_t)B * H * W * 12 * 2);
+        CK(f32_to_act(x, 0, r.p, DT_BF16, lin, B, 12, c.stream));
+        CK(act_to_f32(r.p, DT_BF16, lin, (float*)in.p, 1, B, 12, c.stream));
+        c.put(r);
+      } else {
+        CK(f32_to_act(x, 0, in.p, DT_F32, lin, B, 12, c.stream));
+      }
       ConvParams cp;
       memset(&cp, 0, sizeof(cp));
       ClassW& cw = L->cls[0];
-      cp.x = in.p; cp.in_dt = dt; cp.N = B; cp.Hi = H; cp.Wi = W; cp.Ci = Ci; cp.ldx = Ci;
+      cp.x = in.p; cp.in_dt = DT_F32; cp.N = B; cp.Hi = H; cp.Wi = W; cp.Ci = 12; cp.ldx = 12;
       cp.Ho = Ho; cp.Wo = Wo; cp.stride = 1; cp.ntaps = cw.direct.n;
       memcpy(cp.dy, cw.direct.dy, sizeof(cp.dy));
       memcpy(cp.dx, cw.direct.dx, sizeof(cp.dx));
       cp.w = cw.w_direct; cp.bias = L->bias; cp.Cout = s.cout;
       cp.y = o.p; cp.out_dt = DT_F32; cp.Hout = Ho; cp.Wout = Wo; cp.ldo = s.cout; cp.choff = 0;
       cp.osy = cp.osx = 1; cp.epi = EPI_LINEAR; cp.scale = 1.0f;
-      CK(direct_launch(cp, cw.CoutP, precision == SE_PREC_FP32_EXACT, c.stream));
-      CK(nhwc_to_nchw(o.p, DT_F32, y, B, s.cout, Ho * Wo, s.cout, 0, c.stream));
+      CK(direct_launch(cp, cw.CoutP, c.stream));
+      CK(act_to_f32(o.p, DT_F32, lout, y, 0, B, s.cout, c.stream));
       c.put(o);
-    } else {
-      const int cg = s.cout / 2;
-      const View vin = L->is_stem ? stem_view(c, in.p, H, W) : c.dense(in.p, H, W, Ci, in_c8);
-      if (c.split()) {
-        const int cbo = (cg + 7) / 8;
-        Buf o = c.get(c.act_bytes(Ho, Wo, cg, 1));
-        if (cg % 8) CK(fill_zero(o.p, o.bytes, c.stream));
-        int r = run_layer(c, *L, vin, o.p, 2 * cbo, 0, 1);
-        if (r) return r;
-        CK(split_to_f32(o.p, y, B, cg, Ho * Wo, cbo, 0, 0, c.stream));
-        c.put(o);
-      } else {
-        Buf o = c.get((size_t)B * Ho * Wo * cg * c.esz());
-        int r = run_layer(c, *L, vin, o.p, cg, 0, 0);
-        if (r) return r;
-        CK(nhwc_to_nchw(o.p, dt, y, B, cg, Ho * Wo, cg, 0, c.stream));
-        c.put(o);
-      }
+      c.put(in);
+      return 0;
     }
+    // input in the layout the layer reads, in the mode's storage (channel-blocked padding channels and the pad pixels of the
+    // packed stem rows zeroed first); output channel-blocked in split-half, NHWC otherwise
+    const int in_c8 = wants_c8(c, *L);
+    Buf in = c.get(L->is_stem ? (size_t)B * H * stem_wp(W) * 8 * c.esz() : c.act_bytes(H, W, L->Ci, in_c8));
+    const View vin = L->is_stem ? stem_view(c, in.p, H, W) : c.dense(in.p, H, W, L->Ci, in_c8);
+    if (L->is_stem || (in_c8 && s.cin % 8)) CK(fill_zero(in.p, in.bytes, c.stream));
+    const Layout lin{L->is_stem ? LAYOUT_ROWS : in_c8, H, W, vin.ld, stem_wp(W), STEM_PADL};
+    CK(f32_to_act(x, 0, in.p, c.act_dt(), lin, B, s.cin, c.stream));
+    const int cg = s.cout / 2, out_c8 = c.split() ? 1 : 0;
+    Buf o = c.get(c.act_bytes(Ho, Wo, cg, out_c8));
+    const View vo = c.dense(o.p, Ho, Wo, cg, out_c8);
+    if (out_c8 && cg % 8) CK(fill_zero(o.p, o.bytes, c.stream));
+    int r = run_layer(c, *L, vin, o.p, vo.ld, 0, out_c8);
+    if (r) return r;
+    CK(act_to_f32(o.p, c.act_dt(), Layout{out_c8, Ho, Wo, vo.ld}, y, 0, B, cg, c.stream));
+    c.put(o);
     c.put(in);
     return 0;
   });
@@ -1591,38 +1562,28 @@ int se_contextual_attention_forward(const float* feat, const float* mask_s, int 
   std::lock_guard<std::mutex> lk(mu);
   if (!holder) { holder = new se_model(); holder->finalized = true; }
   // fp32-on-tensor-cores mode: split-half GEMM attention (needs 16 * C to be a multiple of 256 and no attention-map output);
-  // everything else of the fp32 modes runs on the fp32 CUDA-core kernels
-  const bool split_cam = precision == SE_PREC_FP32_TC && C % 16 == 0 && attn == nullptr && h % 2 == 0 && w % 2 == 0;
-  if (precision == SE_PREC_FP32_TC) precision = SE_PREC_FP32_EXACT;
+  // bf16: the tensor-core attention over netG's 96 channels. Everything else runs on the fp32 CUDA-core kernels.
+  const bool even = h % 2 == 0 && w % 2 == 0;
+  const bool split_cam = precision == SE_PREC_FP32_TC && C % 16 == 0 && attn == nullptr && even;
+  const bool tc_cam = precision == SE_PREC_BF16_TC && C == 96 && even;
+  if (precision == SE_PREC_FP32_TC || (precision == SE_PREC_BF16_TC && !tc_cam)) precision = SE_PREC_FP32_EXACT;
   cudaStream_t st = (cudaStream_t)stream;
   return with_arena(holder, precision, B, st, [&](Ctx& c) -> int {
-    const int dt = c.act_dt();
-    if (split_cam) {
-      Buf in = c.get((size_t)B * h * w * C * 4), o = c.get((size_t)B * h * w * C * 4);
-      CK(nchw_to_nhwc(feat, in.p, DT_F32, B, C, h * w, C, 0, c.stream));
-      int r = run_cam_split(c, (const float*)in.p, h, w, C, mask_s, (float*)o.p);
-      if (r) return r;
-      CK(nhwc_to_nchw(o.p, DT_F32, out, B, C, h * w, C, 0, c.stream));
-      c.put(o);
-      c.put(in);
-      return 0;
-    }
-    Buf in = c.get((size_t)B * h * w * C * c.esz());
-    Buf o = c.get((size_t)B * h * w * C * c.esz());
-    if (precision == SE_PREC_BF16_TC && C == 96 && h % 2 == 0 && w % 2 == 0) {
+    const Layout nhwc_l{LAYOUT_NHWC, h, w, C};
+    Buf in = c.get((size_t)B * h * w * C * c.esz()), o = c.get((size_t)B * h * w * C * c.esz());
+    if (tc_cam) {
       // the layouts netG uses on the tensor-core path: space-to-depth channel-blocked in, channel-blocked out
-      CK(nchw_to_c8_s2d(feat, in.p, B, C, h, w, c.stream));
+      CK(f32_to_act(feat, 0, in.p, DT_BF16, Layout{LAYOUT_S2D, h, w, 4 * (C / 8)}, B, C, c.stream));
       int r = run_cam_tc(c, c.dense(in.p, h, w, C, 2), mask_s, o.p, attn);
       if (r) return r;
-      CK(c8_to_nchw(o.p, out, B, C, h * w, c.stream));
-      c.put(o);
-      c.put(in);
-      return 0;
+      CK(act_to_f32(o.p, DT_BF16, Layout{LAYOUT_C8, h, w, C / 8}, out, 0, B, C, c.stream));
+    } else {
+      CK(f32_to_act(feat, 0, in.p, DT_F32, nhwc_l, B, C, c.stream));
+      int r = split_cam ? run_cam_split(c, (const float*)in.p, h, w, C, mask_s, (float*)o.p)
+                        : run_cam(c, nhwc(in.p, h, w, C, C), mask_s, o.p, C, attn);
+      if (r) return r;
+      CK(act_to_f32(o.p, DT_F32, nhwc_l, out, 0, B, C, c.stream));
     }
-    CK(nchw_to_nhwc(feat, in.p, dt, B, C, h * w, C, 0, c.stream));
-    int r = run_cam(c, nhwc(in.p, h, w, C, C), mask_s, o.p, C, attn);
-    if (r) return r;
-    CK(nhwc_to_nchw(o.p, dt, out, B, C, h * w, C, 0, c.stream));
     c.put(o);
     c.put(in);
     return 0;

@@ -52,12 +52,6 @@ struct GemmSplitParams {
   int ncs;
 };
 
-__device__ __forceinline__ void split_f16(float v, float scale, __half& hi, __half& lo) {
-  const float s = fminf(fmaxf(v * scale, -kSplitActMax), kSplitActMax);
-  hi = __float2half_rn(s);
-  lo = __float2half_rn(s - __half2float(hi));
-}
-
 // ------------------------------------------------------------------------------------------ pack: Q and K patch matrices
 // f: fp32 NHWC [B][h][w][C] (C = 8 * CB). Q, Kn: fp16 [B][2][16 * CB][Mp][8]. One thread = one (patch n, tap, channel block).
 __global__ void cam_split_pack_kernel(const float* __restrict__ f, const float* __restrict__ rnorm, uint4* __restrict__ Q, uint4* __restrict__ Kn,
@@ -80,12 +74,12 @@ __global__ void cam_split_pack_kernel(const float* __restrict__ f, const float* 
 #pragma unroll
     for (int k = 0; k < 8; k += 2) {
       __half h0, l0, h1, l1;
-      split_f16(x[k], kScaleQ, h0, l0);
-      split_f16(x[k + 1], kScaleQ, h1, l1);
+      split_half(x[k], kScaleQ, h0, l0);
+      split_half(x[k + 1], kScaleQ, h1, l1);
       qh[k >> 1] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
       ql[k >> 1] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
-      split_f16(x[k] * rr[k], kScaleK, h0, l0);
-      split_f16(x[k + 1] * rr[k + 1], kScaleK, h1, l1);
+      split_half(x[k] * rr[k], kScaleK, h0, l0);
+      split_half(x[k + 1] * rr[k + 1], kScaleK, h1, l1);
       kh[k >> 1] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
       kl[k >> 1] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
     }
@@ -230,8 +224,8 @@ __global__ void __launch_bounds__(256) cam_split_softmax_kernel(const float* __r
         const float p0 = (lb * 8 + k < L) ? expf(row[k] - mx) * inv : 0.0f;
         const float p1 = (lb * 8 + k + 1 < L) ? expf(row[k + 1] - mx) * inv : 0.0f;
         __half h0, l0, h1, l1;
-        split_f16(p0, kScaleP, h0, l0);
-        split_f16(p1, kScaleP, h1, l1);
+        split_half(p0, kScaleP, h0, l0);
+        split_half(p1, kScaleP, h1, l1);
         hi[k >> 1] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
         lo[k >> 1] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
       }

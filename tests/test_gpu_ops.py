@@ -121,3 +121,6 @@ def test_bad_arguments_fail_loudly():
         eng.gated_conv("M", "conv5", torch.zeros(1, 96, 8, 8), precision="bf16")        # CPU tensor
     with pytest.raises(SketchEditB200Error):
         eng.inference(torch.zeros(1, 3, 20, 20).cuda(), torch.zeros(1, 1, 20, 20).cuda())   # not a multiple of 8
+    x, y = torch.zeros(1, 96, 8, 8).cuda(), torch.zeros(1, 96, 8, 8).cuda()
+    rc = eng.lib.se_gated_conv_forward(eng.h, b"M", b"conv5", x.data_ptr(), 1, 8, 8, 2, y.data_ptr(), None)   # retired precision 2
+    assert rc != 0 and b"precision 2" in eng.lib.se_last_error()

@@ -26,7 +26,7 @@ PM = ["pmconv1", "pmconv2_downsample", "pmconv3", "pmconv4_downsample", "pmconv5
 # --------------------------------------------------------------------------------------------- storage of each mode
 def store(v, prec):
     """v (fp32) as the activation storage of `prec` holds it: bf16 round to nearest even, the split-half pair of
-    se_split.cu split8 (64 v clamped to +-65000, hi = fp16, lo = fp16 of the rest), or fp32."""
+    se_common.cuh split_half (64 v clamped to +-65000, hi = fp16, lo = fp16 of the rest), or fp32."""
     v = v.float()
     if prec == "bf16":
         return UB.bf16(v)
@@ -106,7 +106,7 @@ def stem_inputs(io, flags):
 
 
 def packed_expect(io, flags, name):
-    """the fp32 8 channels pack8 writes for packed tap `name` (se_misc.cu pack8_kernel / se_split.cu pack8_split_kernel)."""
+    """the fp32 8 channels pack8 writes for packed tap `name` (se_misc.cu pack8_kernel)."""
     x, x2, m, m2, g = io["x"], io["x2"], io["mask"], io["mask2"], io["guide"]
     ones = torch.ones_like(m) if g is None else g
     z1, z3 = torch.zeros_like(m), torch.zeros_like(x)
@@ -254,8 +254,8 @@ def check_attention(T, io, prec, max_pixels=2048):
         out["attention"] = UB.max_ratio(y, Y, bound)
         return out
     if prec == "fp32":
-        # the split-half mode runs the attention in fp32 between two conversions (se_split.cu split_to_f32 and
-        # nhwc_f32_to_split): the fp32 map equals the stored one, and the stored result is the re-split of the fp32 one
+        # the split-half mode runs the attention in fp32 between two conversions (se_misc.cu act_to_f32 and
+        # f32_to_act): the fp32 map equals the stored one, and the stored result is the re-split of the fp32 one
         out["attention_glue"] = max(exact_ratio(T["in:G.cam.f32"], feat), exact_ratio(y.float(), store(T["out:G.cam.f32"], prec)))
         y = T["out:G.cam.f32"].double()
     err = UB.attention_err(prec, C, h, w)

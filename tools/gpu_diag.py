@@ -48,7 +48,7 @@ def layer_case(net, name, H, W, prec):
 def run_group(g):
     print("=== group", g, flush=True)
     if g in GROUPS:
-        precs = ["fp32"] if g == "fp32" else (["bf16_direct", "bf16"] if g != "heads" else ["fp32", "bf16"])
+        precs = ["fp32"] if g == "fp32" else (["bf16"] if g != "heads" else ["fp32", "bf16"])
         for prec in precs:
             for case in GROUPS[g]:
                 try:
@@ -63,7 +63,7 @@ def run_group(g):
             mask[:, :, h:3 * h, w:2 * w + 8] = 1.0
             mask_s = F.avg_pool2d(mask, 4, 4)
             ref, A = O.contextual_attention(feat, mask_s)
-            for prec in ("fp32", "bf16_direct", "bf16"):
+            for prec in ("fp32", "bf16"):
                 try:
                     out, attn = contextual_attention(feat.cuda(), mask_s.cuda(), precision=prec, want_attn=True)
                     torch.cuda.synchronize()
@@ -80,7 +80,7 @@ def run_group(g):
         mask[0, :, 16:40, 8:50] = 1
         mask[1, :, 30:60, 20:44] = 1
         r1, r2 = O.netG_forward(WG, img, img, mask, mask, sk)
-        for prec in ("fp32", "bf16_direct", "bf16"):
+        for prec in ("fp32", "bf16"):
             try:
                 m, s = engine().netM(img.cuda(), sk.cuda(), precision=prec)
                 print("netM %-11s mask diff %.3e  img diff %.3e  launches %d" % (prec, maxdiff(m.cpu(), rm), maxdiff(s.cpu(), rs), engine().launches()), flush=True)
