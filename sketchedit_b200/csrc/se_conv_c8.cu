@@ -38,19 +38,22 @@ __device__ __forceinline__ void ring_of(int i, int n, int shift, int& slot, uint
 }
 
 // NT: GEMM N (accumulator columns) of the layer; kF16: operands are fp16 (split-half mode) instead of bf16.
+// k-step shape: R64 64-wide K units of M64 K16 MMAs each, then R32 32-wide units of two. A k-step is one fully unrolled
+// wgmma chain between one fence and one commit: with a run-time shape ptxas keeps the accumulators live across a loop and
+// inserts a warpgroup.arrive before every wgmma, so each one closed its own group.
 // p.ncls > 1: fused sub-pixel classes of a x2 deconv (C8Group): the consumers run over VIRTUAL tiles v = tile * ncls + class;
 // the producer loads one (union) halo per real tile, a class selects its resident weight image (cls_bytes apart), its
 // A-offset row aoff[class * C8_CLS_UNITS + unit] and its output sub-pixel offset; the halo buffer is released after the
 // tile's last class.
-template <int NT, bool kF16>
+template <int NT, bool kF16, int R64, int M64, int R32>
 __global__ void __launch_bounds__(C8_THREADS, 1)
 conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   // carve: [halo A buffers][resident weights][stages: (tap A box) + (B image)] [barriers][bias]
   const bool halo = (p.mode == C8_HALO);
-  const int b64_bytes = NT * 128, b32_bytes = NT * 64;
-  const int b_bytes = p.r64 * b64_bytes + p.r32 * b32_bytes;
+  constexpr int b64_bytes = NT * 128, b32_bytes = NT * 64;
+  constexpr int b_bytes = R64 * b64_bytes + R32 * b32_bytes;
   const int stage_a = halo ? 0 : p.a_bytes;
   const int stage_b = p.resident ? 0 : b_bytes;
   const int stage_bytes = stage_a + stage_b;
@@ -190,7 +193,20 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
     int stage = 0;
     uint32_t phase = 0;
     const int my_tiles = (first_tile < total_tiles) ? (total_tiles - first_tile + (int)gridDim.x - 1) / (int)gridDim.x : 0;
-    for (int v = 0; v < my_tiles * ncls; ++v) {
+    const int nv = my_tiles * ncls;
+    // Ping-pong (resident weights, one k-step per tile: plain layers, stems, stem pairs, fused classes): the two warpgroups'
+    // MMA phases alternate on named barriers 1 and 2 (the 256 consumer threads). Warpgroup 1 issues its MMAs of virtual
+    // tile v after warpgroup 0 has issued its own of v, warpgroup 0 those of v + 1 after warpgroup 1 has issued its own of v.
+    // The tensor cores run them in issue order, so each warpgroup's epilogue overlaps the other's MMAs: a tile takes
+    // max(2m, m + E) instead of 2m + E (m: one half tile's MMAs, E: its epilogue).
+    //  * resident plans have >= 2 halo buffers (c8_configure, checked in c8_launch): the producer loads tile v + 1 while
+    //    warpgroup 1 still reads tile v;
+    //  * every bar.arrive meets its bar.sync: warpgroup 0 arrives on 1 for every v, where warpgroup 1 syncs; warpgroup 1
+    //    arrives on 2 for every v but the last, warpgroup 0 syncs on it for every v but the first. No barrier is left
+    //    half-arrived at exit, whatever the tile count (0 and 1 included).
+    // Streamed launches keep both warpgroups in lockstep: their stage ring cannot cover one that lags a whole MMA phase.
+    const bool pingpong = p.resident && ksteps == 1;
+    for (int v = 0; v < nv; ++v) {
       const int riter = ncls == 1 ? v : v / ncls, cls = v - riter * ncls;
       const int tile = (int)blockIdx.x + riter * (int)gridDim.x;
       if (tile >= total_tiles) {   // phantom (clusters stream their weights: ncls == 1)
@@ -210,6 +226,7 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
         ring_of(riter, p.a_bufs, p.a_shift, ab, aph);
         mbar_wait(&a_full[ab], aph, 7);
       }
+      if (pingpong && (wg == 1 || v > 0)) named_bar_sync(wg == 0 ? 2 : 1, 256);
       int prev = -1;
       for (int ks = 0; ks < ksteps; ++ks) {
         if (staged) mbar_wait(&full_bar[stage], phase, 3);
@@ -217,28 +234,27 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
         const uint32_t sB = p.resident ? smem_base + off_wres + (uint32_t)cls * (uint32_t)p.cls_bytes + (uint32_t)ks * b_bytes : st + stage_a;
         const uint32_t sA = (halo ? smem_base + (uint32_t)ab * p.a_bytes : st) + a_m;
         const int ub = cls * C8_CLS_UNITS;
-        const int u0 = ub + ks * p.r64, v0 = ub + (int)n_u64 + ks * p.r32;
+        const int u0 = ub + ks * R64, v0 = ub + (int)n_u64 + ks * R32;
+        const uint32_t acc0 = ks ? 1u : 0u;   // the tile's first MMA overwrites the accumulators
         wg_fence();
         wg_fence_acc(acc);
-        uint32_t accum = ks ? 1u : 0u;
-        for (int j = 0; j < p.r64; ++j) {
+#pragma unroll
+        for (int j = 0; j < R64; ++j) {
           const uint32_t a0 = sA + p.aoff[u0 + j];
           const uint32_t b0 = sB + (uint32_t)(j * b64_bytes);
-          for (int k = 0; k < p.mmas64; ++k) {
-            Wgmma<NT, kF16, 0>::mma(acc, wg_desc(a0 + k * p.kstep_bytes, p.lbo_bytes, p.sbo_bytes, WG_SW_NONE),
-                                    wg_desc(b0 + 32u * k, 16u, 1024u, WG_SW128), accum);
-            accum = 1u;
-          }
-        }
-        for (int j = 0; j < p.r32; ++j) {
-          const uint32_t a0 = sA + p.aoff[v0 + j];
-          const uint32_t b0 = sB + (uint32_t)(p.r64 * b64_bytes + j * b32_bytes);
 #pragma unroll
-          for (int k = 0; k < 2; ++k) {
+          for (int k = 0; k < M64; ++k)
             Wgmma<NT, kF16, 0>::mma(acc, wg_desc(a0 + k * p.kstep_bytes, p.lbo_bytes, p.sbo_bytes, WG_SW_NONE),
-                                    wg_desc(b0 + 32u * k, 16u, 512u, WG_SW64), accum);
-            accum = 1u;
-          }
+                                    wg_desc(b0 + 32u * k, 16u, 1024u, WG_SW128), j + k ? 1u : acc0);
+        }
+#pragma unroll
+        for (int j = 0; j < R32; ++j) {
+          const uint32_t a0 = sA + p.aoff[v0 + j];
+          const uint32_t b0 = sB + (uint32_t)(R64 * b64_bytes + j * b32_bytes);
+#pragma unroll
+          for (int k = 0; k < 2; ++k)
+            Wgmma<NT, kF16, 0>::mma(acc, wg_desc(a0 + k * p.kstep_bytes, p.lbo_bytes, p.sbo_bytes, WG_SW_NONE),
+                                    wg_desc(b0 + 32u * k, 16u, 512u, WG_SW64), R64 + j + k ? 1u : acc0);
         }
         wg_commit();
         if (staged) {
@@ -251,6 +267,7 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
           if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
         }
       }
+      if (pingpong && (wg == 0 || v + 1 < nv)) named_bar_arrive(wg == 0 ? 1 : 2, 256);
       wg_wait<0>();
       wg_fence_acc(acc);
       if (prev >= 0) release_stage(prev);
@@ -385,29 +402,60 @@ int c8_configure(C8Layer* L, int ntaps, const int8_t* dy, const int8_t* dx, int 
   return 0;
 }
 
-// accumulator widths with an instantiation (every gated layer of the two generators: N = 2 * round8(Cout / 2))
-#define C8_NT_LIST(X) X(32) X(48) X(64) X(96) X(128) X(192)
-static bool c8_nt_supported(int NT) {
-#define X(n) if (NT == n) return true;
-  C8_NT_LIST(X)
-#undef X
-  return false;
+// The instantiations: every (N, split-half, k-step shape) that c8_configure / c8_configure_group plan for a layer, fused
+// class group or stem pair of the two generators, in both precisions (split-half layers count three product taps per tap).
+// This one table selects the kernel of a launch, gets the shared-memory opt-in and keys the cluster-occupancy cache;
+// se_model_finalize checks every packed layer against it (c8_instantiated).
+typedef void (*C8Kernel)(CUtensorMap, C8Params);
+struct C8Inst { int nt; bool f16; int r64, m64, r32; C8Kernel fn; };
+#define C8_INST(nt, f16, r64, m64, r32) {nt, f16, r64, m64, r32, conv_c8_kernel<nt, f16, r64, m64, r32>}
+static const C8Inst kC8Insts[] = {
+    // bf16 (resident weights: the whole tile is one k-step)
+    C8_INST(32, false, 0, 0, 9),    // 24->24
+    C8_INST(48, false, 0, 0, 9),    // 24->48 stride 2
+    C8_INST(48, false, 4, 3, 0),    // deconv 48->48 class
+    C8_INST(48, false, 5, 3, 0),    // 5x5 stem
+    C8_INST(96, false, 0, 0, 9),    // 24->96 stride 1 and 2
+    C8_INST(96, false, 4, 4, 4),    // deconv 96->96 class
+    C8_INST(96, false, 5, 3, 0),    // stem pair
+    C8_INST(96, false, 9, 3, 0),    // 48->96
+    // bf16, streamed weights
+    C8_INST(96, false, 3, 3, 0),    // 48->96 stride 2
+    C8_INST(192, false, 1, 3, 0),   // 48->192 (stride 1 and 2)
+    C8_INST(192, false, 1, 4, 0),   // 192->192
+    C8_INST(192, false, 1, 4, 1),   // 96->192 (all rates)
+    // split-half
+    C8_INST(32, true, 0, 0, 27),    // 24->24 (resident)
+    C8_INST(48, true, 0, 0, 3),     // 24->48 stride 2
+    C8_INST(48, true, 12, 3, 0),    // deconv 48->48 class (resident)
+    C8_INST(48, true, 15, 3, 0),    // 5x5 stem (resident)
+    C8_INST(96, true, 0, 0, 3),     // 24->96 stride 1 and 2
+    C8_INST(96, true, 1, 3, 0),     // 48->96 stride 2 (one box per tap)
+    C8_INST(96, true, 1, 4, 1),     // deconv 96->96 class
+    C8_INST(96, true, 3, 3, 0),     // 48->96, stem pair
+    C8_INST(192, true, 1, 3, 0),    // 48->192 (stride 1 and 2)
+    C8_INST(192, true, 1, 4, 0),    // 192->192 (one 64-channel chunk per stage)
+    C8_INST(192, true, 1, 4, 1),    // 96->192 (all rates)
+};
+#undef C8_INST
+static C8Kernel c8_kernel(const C8Layer& L, bool f16) {
+  const TcWeights& w = L.w;
+  const int r64 = w.n64 ? w.r64 : 0, r32 = w.n32 ? w.r32 : 0, m64 = r64 ? L.mmas64 : 0;
+  for (const C8Inst& k : kC8Insts)
+    if (k.nt == w.NT && k.f16 == f16 && k.r64 == r64 && k.m64 == m64 && k.r32 == r32) return k.fn;
+  return nullptr;
 }
 static int c8_set_smem_attr(int bytes) {
-#define X(n)                                                                                                  \
-  SE_CUDA_OK(cudaFuncSetAttribute(conv_c8_kernel<n, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)); \
-  SE_CUDA_OK(cudaFuncSetAttribute(conv_c8_kernel<n, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-  C8_NT_LIST(X)
-#undef X
+  for (const C8Inst& k : kC8Insts) SE_CUDA_OK(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
   return 0;
 }
-typedef void (*C8Kernel)(CUtensorMap, C8Params);
-static C8Kernel c8_kernel(const C8Params& p) {
-#define X(n) \
-  if (p.NT == n) return p.f16 ? conv_c8_kernel<n, true> : conv_c8_kernel<n, false>;
-  C8_NT_LIST(X)
-#undef X
-  return nullptr;
+int c8_instantiated(const C8Layer& L, bool f16, const std::string& name) {
+  const TcWeights& w = L.w;
+  SE_REQUIRE(c8_kernel(L, f16) != nullptr,
+             "layer " + name + (f16 ? " (split-half)" : "") + ": no conv_c8_kernel instantiation for N = " + std::to_string(w.NT) +
+                 ", k-step of " + std::to_string(w.n64 ? w.r64 : 0) + " x " + std::to_string(L.mmas64) + " + " +
+                 std::to_string(w.n32 ? w.r32 : 0) + " x 2 MMAs (se_conv_c8.cu: kC8Insts)");
+  return 0;
 }
 static void c8_launch_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, int grid, int smem_bytes, int cluster, cudaStream_t stream) {
   *cfg = cudaLaunchConfig_t();
@@ -468,7 +516,7 @@ int c8_configure_group(C8Group* G, int ncls, int ntaps, const int8_t (*dy)[8], c
   w.r64 = ntaps * w.n64;      // resident weights + halo: one k-step issues every MMA of a (tile, class)
   w.r32 = ntaps * w.n32;
   L.mmas64 = Ci == 48 ? 3 : 4;
-  if (w.r64 + w.r32 > C8_CLS_UNITS || !c8_nt_supported(w.NT)) return 1;
+  if (w.r64 + w.r32 > C8_CLS_UNITS) return 1;
   L.mode = C8_HALO;
   L.resident = true;
   L.stem = false;
@@ -499,7 +547,6 @@ int c8_launch(const ConvParams& c, const C8Layer& L_in, cudaStream_t stream, con
   SE_REQUIRE(c.ntaps == w.ntaps && c.ntaps <= MAX_TAPS, "tap count mismatch");
   for (int t = 0; t < c.ntaps && !grp; ++t) SE_REQUIRE(c.tap_cb[t] == L.tap_cb[t], "per-tap channel blocks differ from the packed layer");
   SE_REQUIRE(c.Wi * 8 <= (1 << 30) && L.WR * 8 <= 256 && L.HR <= 256 && L.cb_in <= 256, "TMA box limits");
-  SE_REQUIRE(c8_nt_supported(w.NT), "no conv_c8 instantiation for N = " + std::to_string(w.NT));
   SE_REQUIRE(c.epi == EPI_GATE_ELU || c.epi == EPI_GATE_RELU, "conv_c8 runs gated epilogues only");
   SE_REQUIRE(w.NT == 2 * gated_goff(c.Cout), "gated layers keep the gate columns in the upper half of the tile");
   C8Params p;
@@ -512,7 +559,7 @@ int c8_launch(const ConvParams& c, const C8Layer& L_in, cudaStream_t stream, con
   p.ntaps = c.ntaps;
   memcpy(p.dy, c.dy, sizeof(p.dy));
   memcpy(p.dx, c.dx, sizeof(p.dx));
-  p.n64 = w.n64; p.n32 = w.n32; p.r64 = w.n64 ? w.r64 : 0; p.r32 = w.n32 ? w.r32 : 0; p.NT = w.NT;
+  p.n64 = w.n64; p.n32 = w.n32; p.NT = w.NT;
   p.ksteps = tc_ksteps(w);
   p.w = reinterpret_cast<const uint8_t*>(grp ? grp->w_all : w.data);
   p.mode = L.mode; p.HR = L.HR; p.WR = L.WR; p.pad_y0 = L.pad_y0; p.pad_x0 = L.pad_x0;
@@ -523,8 +570,8 @@ int c8_launch(const ConvParams& c, const C8Layer& L_in, cudaStream_t stream, con
   p.ncls = grp ? grp->ncls : 1;
   p.cls_bytes = grp ? grp->cls_bytes : 0;
   for (int k = 0; k < C8_MAX_CLS; ++k) { p.cls_ooy[k] = grp && k < grp->ncls ? grp->ooy[k] : 0; p.cls_oox[k] = grp && k < grp->ncls ? grp->oox[k] : 0; }
-  if (L.stem) { p.lbo_bytes = 16; p.kstep_bytes = 32; p.mmas64 = 3; }
-  else { p.lbo_bytes = L.HR * L.WR * 16; p.kstep_bytes = 2 * p.lbo_bytes; p.mmas64 = L.mmas64; }
+  if (L.stem) { p.lbo_bytes = 16; p.kstep_bytes = 32; }
+  else { p.lbo_bytes = L.HR * L.WR * 16; p.kstep_bytes = 2 * p.lbo_bytes; }
   p.sbo_bytes = L.WR * 16;
   p.bias = c.bias;
   fill_epi(c, w.NT, &p.e);
@@ -574,6 +621,7 @@ int c8_launch(const ConvParams& c, const C8Layer& L_in, cudaStream_t stream, con
   for (int sh = 0; sh < 4; ++sh) if ((1 << sh) == p.a_bufs) p.a_shift = sh;
   SE_REQUIRE(p.a_bufs <= C8_MAX_ABUFS, "halo ring plan");
   SE_REQUIRE(!grp || (p.a_bufs >= 2 && p.ksteps == 1), "fused classes need two halo buffers and a single k-step");
+  SE_REQUIRE(!(L.resident && p.ksteps == 1) || p.a_bufs >= 2, "ping-pong warpgroups need two halo buffers");
   int stages = stage_bytes ? (smem_budget - fixed) / stage_bytes : 1;
   if (stages > C8_MAX_STAGES) stages = C8_MAX_STAGES;
   SE_REQUIRE(stages >= (stage_bytes ? 2 : 1), "shared memory plan does not fit");
@@ -603,8 +651,8 @@ int c8_launch(const ConvParams& c, const C8Layer& L_in, cudaStream_t stream, con
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     SE_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(C8) failed, CUresult=" + std::to_string((int)r));
   }
-  const C8Kernel kernel = c8_kernel(p);
-  SE_REQUIRE(kernel != nullptr, "no instantiation for N = " + std::to_string(p.NT));
+  const C8Kernel kernel = c8_kernel(L, p.f16 != 0);
+  SE_REQUIRE(kernel != nullptr, "no conv_c8_kernel instantiation for the layer's plan (N = " + std::to_string(p.NT) + ")");
   // streamed weights: 2-CTA clusters read each weight stage from L2 once per pair of neighbouring tiles (TMA multicast)
   p.cluster = L.resident ? 1 : 2;
   int grid = total_tiles < g_sms ? total_tiles : g_sms;

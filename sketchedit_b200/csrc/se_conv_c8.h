@@ -46,11 +46,11 @@ struct C8Params {
   int step_x, step_y, step_img;   // gridDim.x decomposed in (tiles_x, tiles_y, images): incremental tile decode
   int ntaps;
   int8_t dy[MAX_TAPS], dx[MAX_TAPS];
-  int n64, n32, r64, r32, NT, ksteps;
+  int n64, n32, NT, ksteps;   // (the k-step shape r64 / mmas64 / r32 is the instantiation's)
   const uint8_t* w;
   int mode, HR, WR, pad_y0, pad_x0, cb_in, x_cb_off;
   int a_bytes, a_tx_bytes, a_bufs, a_shift;   // halo ring: a_bufs buffers; a_shift = log2(a_bufs) or -1 (ring of 3 / 6: index by division)
-  int lbo_bytes, sbo_bytes, kstep_bytes, mmas64;
+  int lbo_bytes, sbo_bytes, kstep_bytes;
   uint32_t aoff[C8_MAX_UNITS];   // byte offset of each K unit's A operand inside the shared-memory region
   int num_stages, resident, wres_bytes;
   const float* bias;
@@ -65,6 +65,8 @@ struct C8Params {
 
 int c8_configure(C8Layer* L, int ntaps, const int8_t* dy, const int8_t* dx, int Ci, int Cout, bool stem, const int8_t* tap_cb = nullptr);
 int c8_launch(const ConvParams& c, const C8Layer& L, cudaStream_t stream, const C8Group* grp = nullptr);
+// error (naming the layer) when no conv_c8_kernel instantiation runs L's plan; f16: the split-half form
+int c8_instantiated(const C8Layer& L, bool f16, const std::string& name);
 // geometry of a fused-class launch; returns non-zero (no error text) when the classes do not fit in shared memory
 int c8_configure_group(C8Group* G, int ncls, int ntaps, const int8_t (*dy)[8], const int8_t (*dx)[8], const int* ooy, const int* oox, int Ci, int Cout);
 

@@ -308,6 +308,8 @@ static int pack_class(se_model* m, Layer& L, const std::vector<EffTap>& taps, Cl
     {
       int rc = c8_configure(&cw.c8, ntaps, cw.bf16.dy, cw.bf16.dx, Ci, Cout, L.is_stem, cw.bf16.cb);
       if (rc) return rc;
+      rc = c8_instantiated(cw.c8, false, L.name);
+      if (rc) return rc;
     }
     TcWeights* tcp = &cw.c8.w;
     // the exact (swizzled) shared-memory image of every pipeline stage, see se_conv_tc.h. Gate channels (n >= Cout/2) are stored
@@ -346,6 +348,8 @@ static int pack_class(se_model* m, Layer& L, const std::vector<EffTap>& taps, Cl
         cw.split.cb[3 * t + pp] = (int8_t)(2 * cw.bf16.cb[t] + (pp == 2 ? CB : 0));   // a parity group holds 2 * CB blocks
       }
     rc = c8_configure(&cw.c8s, cw.split.n, cw.split.dy, cw.split.dx, Ci, Cout, L.is_stem, cw.split.cb);
+    if (rc) return rc;
+    rc = c8_instantiated(cw.c8s, true, L.name);
     if (rc) return rc;
     // weights times a power of two (exact) that brings the largest one to [8192, 16384): the lo halves of all but negligible
     // weights are then normal fp16 numbers (22 bits for the pair); the epilogue undoes it (se_common.cuh: kSplitActScale)
@@ -448,6 +452,8 @@ static int pack_layer(se_model* m, Layer& L) {
         const C8Layer& c0 = L.cls[g0].c8;
         ok = (G.geo.w.r64 == c0.w.r64 && G.geo.w.r32 == c0.w.r32 && G.geo.w.NT == c0.w.NT && G.cls_bytes == (int)tc_weight_bytes_per_image(c0.w));
         if (!ok) break;
+        rc = c8_instantiated(G.geo, false, L.name + " (fused classes)");
+        if (rc) return rc;
         void* d = nullptr;
         SE_CUDA_OK(cudaMalloc(&d, (size_t)per * G.cls_bytes));
         m->owned.push_back(d);
