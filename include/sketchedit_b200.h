@@ -81,6 +81,28 @@ int se_forward_inference_packed(se_model* m, const float* image, const float* sk
 int se_forward_inference_u8(se_model* m, const unsigned char* image_u8, const unsigned char* sketch_u8, int B, int H, int W,
                             int precision, unsigned char* bgr_u8, unsigned char* mask_u8, void* stream);
 
+/* ---- the same forward on a caller-supplied edit mask instead of netM's prediction (mask revising): generate_fake
+ *      (editline2_model.py:338-370) with netM's soft mask replaced by edit_mask [B,1,H,W] (any fp32 values, used as given:
+ *      not clamped, not checked):
+ *        mask_inpaint = (edit_mask > 0.5)        strict >, like :347
+ *        coarse, fine = netG(image, image, mask_inpaint, mask_inpaint, sketch)
+ *        composed     = fine * edit_mask + image * (1 - edit_mask)        soft blend with the SUPPLIED mask, like :132
+ *      netM's mask branch never runs; its trunk and image decoder run only when mask_image is requested (mode='visualize').
+ *      Passing the soft mask se_forward_inference returned reproduces every output of that call bit for bit.
+ *      Optional (may be NULL): coarse, fine, mask_image [B,3,H,W], mask_bin_out [B,1,H,W] (= mask_inpaint). NULL inputs or
+ *      composed, and the retired precision 2, are errors. */
+int se_forward_with_mask(se_model* m, const float* image, const float* sketch, const float* edit_mask, int B, int H, int W,
+                         int precision, float* composed, float* coarse, float* fine, float* mask_image, float* mask_bin_out,
+                         void* stream);
+/* uint8 form, with se_forward_inference_u8's codecs: edit_mask_u8 [B,H,W] decodes to v/255 (ToTensor), so mask_inpaint is 1
+ * exactly for v >= 128, and the blend uses v/255. The mask_u8 se_forward_inference_u8 writes ((int)(m * 255), truncating)
+ * decodes back to the same byte, but it is not netM's exact mask: fed back, the blend moves by up to 1/255 and pixels with
+ * 0.5 < m < 128/255 leave mask_inpaint. There is no mask output (the mask used is the caller's own bytes). NULL pointers and
+ * the retired precision 2 are errors. */
+int se_forward_with_mask_u8(se_model* m, const unsigned char* image_u8, const unsigned char* sketch_u8,
+                            const unsigned char* edit_mask_u8, int B, int H, int W, int precision, unsigned char* bgr_u8,
+                            void* stream);
+
 /* ---- netM: replaces MDGenerator.forward(x, guide) -> (mask1, x_stage1)  (editline2_g.py:59-94) */
 int se_netM_forward(se_model* m, const float* x, const float* guide, int B, int H, int W, int precision, float* mask1,
                     float* x_stage1 /* may be NULL */, void* stream);

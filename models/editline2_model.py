@@ -4,7 +4,10 @@
 reference: netM predicts the edit mask from (image, sketch), the mask is binarised at 0.5, netG inpaints,
 and the result is blended with the SOFT mask. All of it is one C-ABI call (``se_forward_inference``) on the
 CUDA kernels; tensors in ``data`` may live on the CPU (they are copied to the GPU like the reference's
-``preprocess_input`` does) and the outputs are CUDA tensors. Training modes are out of scope."""
+``preprocess_input`` does) and the outputs are CUDA tensors. Training modes are out of scope.
+
+An optional ``data['edit_mask']`` [B,1,H,W] replaces netM's prediction (mask revising): 'inference' then returns
+``(composed, edit_mask)`` and 'visualize' the same five keys with ``mask`` = (edit_mask > 0.5)."""
 import torch
 
 import models.networks as networks
@@ -64,6 +67,8 @@ class EditLine2Model(torch.nn.Module):
 
     def forward(self, data, mode, is_real_im=True):
         image, line = self.preprocess_input(data)
+        if data.get("edit_mask") is not None:
+            return self._forward_with_mask(image, line, data["edit_mask"], mode)
         if mode == "inference":
             composed, mask, _ = self.engine().inference(image, line, precision=self.precision)
             return composed, mask
@@ -72,6 +77,20 @@ class EditLine2Model(torch.nn.Module):
             # with the SOFT mask exactly like mode='inference'
             composed, _, ex = self.engine().inference(image, line, precision=self.precision,
                                                       want=("coarse", "fine", "mask_image", "mask_bin"))
+            return {"mask": ex["mask_bin"], "maskim": ex["mask_image"], "coarse": ex["coarse"], "fine": ex["fine"],
+                    "composed": composed}
+        raise ValueError("|mode| is invalid or training-only: %r" % (mode,))
+
+    def _forward_with_mask(self, image, line, edit_mask, mode):
+        """``data['edit_mask']`` [B,1,H,W] replaces netM's predicted mask (``data['mask']`` is the sketch, as in the
+        reference): netG inpaints edit_mask > 0.5 and the result is blended with edit_mask itself."""
+        edit_mask = edit_mask.to(image.device, torch.float32, non_blocking=True)
+        if mode == "inference":
+            composed, _ = self.engine().inference_with_mask(image, line, edit_mask, precision=self.precision)
+            return composed, edit_mask
+        if mode == "visualize":
+            composed, ex = self.engine().inference_with_mask(image, line, edit_mask, precision=self.precision,
+                                                             want=("coarse", "fine", "mask_image", "mask_bin"))
             return {"mask": ex["mask_bin"], "maskim": ex["mask_image"], "coarse": ex["coarse"], "fine": ex["fine"],
                     "composed": composed}
         raise ValueError("|mode| is invalid or training-only: %r" % (mode,))
@@ -87,7 +106,10 @@ class EditLine2Model(torch.nn.Module):
         uint8=True: the reference's host-side codecs run on the device (``Engine.inference_u8``): a batch supplies
         ``data['image_u8']`` [B,H,W,3] RGB uint8 and ``data['mask_u8']`` [B,H,W] uint8 (what the dataset holds before
         ToTensor/Normalize, reference data/testimage_dataset.py:89-103) and the results are ``(bgr_u8 [B,H,W,3], mask_u8
-        [B,H,W])`` exactly as test.py:25-35 writes them: 4x fewer bytes over PCIe in each direction.
+        [B,H,W])`` exactly as test.py:25-35 writes them: 4x fewer bytes over PCIe in each direction. A batch that also
+        carries ``data['edit_mask_u8']`` [B,H,W] uint8 runs on that mask instead of netM's prediction
+        (``Engine.inference_with_mask_u8``) and its mask result is a copy of the supplied bytes; batches with and without
+        one may be mixed. Float mode rejects batches that carry an edit mask.
 
         with_data=True: yield ``(out0, out1, data)`` (test.py needs the batch's output paths).
 
@@ -136,6 +158,9 @@ class EditLine2Model(torch.nn.Module):
         in_keys = ("image_u8", "mask_u8") if uint8 else ("image", "mask")
         for i, data in enumerate(loader):
             img_h, line_h = data[in_keys[0]], data[in_keys[1]]
+            edit_h = data.get("edit_mask_u8") if uint8 else None
+            if not uint8 and (data.get("edit_mask") is not None or data.get("edit_mask_u8") is not None):
+                raise ValueError("inference_stream runs batches with an edit mask in uint8 mode only (uint8=True, data['edit_mask_u8'])")
             B, H, W = (img_h.shape[0], img_h.shape[1], img_h.shape[2]) if uint8 else (img_h.shape[0], img_h.shape[2], img_h.shape[3])
             slot = slots[i % depth]
             if slot is None or slot["shape"] != (B, H, W):
@@ -150,10 +175,16 @@ class EditLine2Model(torch.nn.Module):
                     bufs = {"img": f32(3), "line": f32(1), "out": None if gather is not None else (f32(4),)}
                 slot = dict(bufs, shape=(B, H, W), ev_in=torch.cuda.Event(), ev_comp=torch.cuda.Event(), ev_out=torch.cuda.Event())
                 slots[i % depth] = slot
+            if edit_h is not None and "edit" not in slot:
+                slot["edit"] = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
             s_in.wait_event(slot["ev_comp"])           # the previous user of these input buffers has been computed
+            if edit_h is not None:
+                s_in.wait_event(slot["ev_out"])        # ... and the edit mask, which is also an output, has left the device
             with torch.cuda.stream(s_in):
                 slot["img"].copy_(img_h, non_blocking=True)
                 slot["line"].copy_(line_h, non_blocking=True)
+                if edit_h is not None:
+                    slot["edit"].copy_(edit_h, non_blocking=True)
                 slot["ev_in"].record(s_in)
             cur.wait_event(slot["ev_in"])
             cur.wait_event(slot["ev_out"])             # ... and its outputs have left the device buffers
@@ -168,13 +199,16 @@ class EditLine2Model(torch.nn.Module):
                     gather.wait(k)                     # s_out waits for the all-gather of this batch
                     src = (gather.bufs[k][gather.rank * B:(gather.rank + 1) * B],)
             else:
-                if uint8:
+                src = slot["out"]
+                if edit_h is not None:
+                    eng.inference_with_mask_u8(slot["img"], slot["line"], slot["edit"], precision=self.precision, out=slot["out"][0])
+                    src = (slot["out"][0], slot["edit"])   # the mask result is the mask the batch ran on
+                elif uint8:
                     eng.inference_u8(slot["img"], slot["line"], precision=self.precision, out=slot["out"])
                 else:
                     eng.inference_packed(slot["img"], slot["line"], precision=self.precision, out=slot["out"][0])
                 slot["ev_comp"].record(cur)
                 s_out.wait_event(slot["ev_comp"])
-                src = slot["out"]
             with torch.cuda.stream(s_out):
                 host = host_out(B, H, W)
                 for h_t, d_t in zip(host, src):

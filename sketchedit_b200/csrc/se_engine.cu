@@ -994,9 +994,11 @@ static int do_pool_broadcast(Ctx& c, const View& v, int mode, void* cat, int cat
 }
 
 // MDGenerator.forward: x [B,3,H,W], guide [B,1,H,W] -> mask1 (soft, NCHW), optional x_stage1; also the
-// binarised mask plane (mask1 > 0.5) when mask_bin != nullptr.
+// binarised mask plane (mask1 > 0.5) when mask_bin != nullptr. mask1 == nullptr (a forward on a caller-supplied edit mask):
+// only the trunk (conv1-conv9) and the image decoder run, for x_stage1.
 static int run_netM(Ctx& c, const float* x, const float* guide, int H, int W, float* mask1, float* x_stage1, float* mask_bin, long long mask1_bs = 0,
                     unsigned char* mask_u8 = nullptr) {
+  SE_REQUIRE(mask1 || x_stage1, "netM with neither output");
   Act in8, x9;
   int rc = do_pack8(c, &in8, x, guide, nullptr, H, W, PACK_IMG_ONE, 1.0f, 0);
   if (rc) return rc;
@@ -1012,6 +1014,10 @@ static int run_netM(Ctx& c, const float* x, const float* guide, int H, int W, fl
     rc = run_head(c, 'M', "conv17", v16.v, HEAD_TANH, nullptr, nullptr, nullptr, x_stage1, nullptr, nullptr);
     if (rc) return rc;
     c.put(v16);
+  }
+  if (!mask1) {
+    c.put(x9);
+    return 0;
   }
   Act v;
   rc = run_chain(c, 'M', with_prefix("", {"conv10_atrous", "conv_mask_11", "conv_mask_12", "conv_mask_13_upsample_conv", "conv_mask_14",
@@ -1475,6 +1481,51 @@ int se_forward_inference_u8(se_model* m, const unsigned char* image_u8, const un
     if (r) return r;
     r = run_netG(c, (const float*)img.p, (const float*)img.p, (const float*)mb.p, (const float*)mb.p, (const float*)sk.p, H, W, nullptr, nullptr, nullptr,
                  (const float*)soft.p, (const float*)img.p, 0, 0, bgr_u8);
+    if (r) return r;
+    c.put(mb); c.put(soft); c.put(sk); c.put(img);
+    return 0;
+  }, key);
+}
+
+// generate_fake (editline2_model.py:338-370) with netM's soft mask replaced by the caller's edit mask: netG inpaints
+// (edit_mask > 0.5) and the result is blended with edit_mask itself. netM runs only for mask_image (its trunk and image decoder).
+int se_forward_with_mask(se_model* m, const float* image, const float* sketch, const float* edit_mask, int B, int H, int W, int precision,
+                         float* composed, float* coarse, float* fine, float* mask_image, float* mask_bin_out, void* stream) {
+  SE_REQUIRE(image && sketch && edit_mask && composed, "null tensor");
+  int rc = check_hw(H, W);
+  if (rc) return rc;
+  std::vector<uintptr_t> key = {5, (uintptr_t)H, (uintptr_t)W, (uintptr_t)image, (uintptr_t)sketch, (uintptr_t)edit_mask, (uintptr_t)composed,
+                                (uintptr_t)coarse, (uintptr_t)fine, (uintptr_t)mask_image, (uintptr_t)mask_bin_out};
+  return with_arena(m, precision, B, (cudaStream_t)stream, [&](Ctx& c) -> int {
+    Buf mb;
+    float* mbin = mask_bin_out;
+    if (!mbin) { mb = c.get((size_t)B * H * W * 4); mbin = (float*)mb.p; }
+    c.tag("binarise_kernel|edit mask > 0.5", 0, 0, 0, (double)B * H * W * 8);
+    CK(binarise(edit_mask, mbin, (long long)B * H * W, c.stream));
+    if (mask_image) {
+      int r = run_netM(c, image, sketch, H, W, nullptr, mask_image, nullptr);
+      if (r) return r;
+    }
+    int r = run_netG(c, image, image, mbin, mbin, sketch, H, W, coarse, fine, composed, edit_mask, image);
+    if (r) return r;
+    c.put(mb);
+    return 0;
+  }, key);
+}
+
+// se_forward_inference_u8's codecs around se_forward_with_mask: the edit mask arrives as bytes v and means v/255
+int se_forward_with_mask_u8(se_model* m, const unsigned char* image_u8, const unsigned char* sketch_u8, const unsigned char* edit_mask_u8, int B,
+                            int H, int W, int precision, unsigned char* bgr_u8, void* stream) {
+  SE_REQUIRE(image_u8 && sketch_u8 && edit_mask_u8 && bgr_u8, "null tensor");
+  int rc = check_hw(H, W);
+  if (rc) return rc;
+  std::vector<uintptr_t> key = {6, (uintptr_t)H, (uintptr_t)W, (uintptr_t)image_u8, (uintptr_t)sketch_u8, (uintptr_t)edit_mask_u8, (uintptr_t)bgr_u8};
+  return with_arena(m, precision, B, (cudaStream_t)stream, [&](Ctx& c) -> int {
+    Buf img = c.get((size_t)B * 3 * H * W * 4), sk = c.get((size_t)B * H * W * 4), soft = c.get((size_t)B * H * W * 4), mb = c.get((size_t)B * H * W * 4);
+    c.tag("u8_to_inputs_kernel|input codec + edit mask", 0, 0, 0, (double)B * H * W * (5 + 24));
+    CK(u8_to_inputs(image_u8, sketch_u8, (float*)img.p, (float*)sk.p, B, H, W, c.stream, edit_mask_u8, (float*)soft.p, (float*)mb.p));
+    int r = run_netG(c, (const float*)img.p, (const float*)img.p, (const float*)mb.p, (const float*)mb.p, (const float*)sk.p, H, W, nullptr, nullptr, nullptr,
+                     (const float*)soft.p, (const float*)img.p, 0, 0, bgr_u8);
     if (r) return r;
     c.put(mb); c.put(soft); c.put(sk); c.put(img);
     return 0;

@@ -605,19 +605,41 @@ int act_to_f32(const void* x, int dt, const Layout& v, float* y, int nhwc, int B
 }
 
 // reference data/testimage_dataset.py:89-103 on device: image uint8 HWC RGB -> fp32 NCHW (ToTensor: /255; Normalize(0.5, 0.5)),
-// sketch uint8 (already resized to the image) -> {0, 1} fp32 (ToTensor then > 0)
+// sketch uint8 (already resized to the image) -> {0, 1} fp32 (ToTensor then > 0). A caller-supplied edit mask (mask_u8, optional)
+// -> its soft plane v/255 (ToTensor; the inverse of the (int)(m * 255) output codec: trunc((v/255)*255) == v for every byte) and
+// its binarised plane (soft > 0.5, the comparison of head_kernel's HEAD_MASK branch: 1 exactly for v >= 128)
 __global__ void u8_to_inputs_kernel(const unsigned char* __restrict__ img_u8, const unsigned char* __restrict__ sk_u8, float* __restrict__ img,
-                                    float* __restrict__ sk, int B, long long HW) {
+                                    float* __restrict__ sk, int B, long long HW, const unsigned char* __restrict__ mask_u8,
+                                    float* __restrict__ mask_soft, float* __restrict__ mask_bin) {
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= B * HW) return;
   const long long b = i / HW, pix = i % HW;
 #pragma unroll
   for (int c = 0; c < 3; ++c) img[(b * 3 + c) * HW + pix] = (__fdiv_rn((float)img_u8[i * 3 + c], 255.0f) - 0.5f) / 0.5f;
   sk[i] = sk_u8[i] > 0 ? 1.0f : 0.0f;
+  if (mask_u8) {
+    const float m = __fdiv_rn((float)mask_u8[i], 255.0f);
+    mask_soft[i] = m;
+    mask_bin[i] = m > 0.5f ? 1.0f : 0.0f;
+  }
 }
-int u8_to_inputs(const unsigned char* img_u8, const unsigned char* sk_u8, float* img, float* sk, int B, int H, int W, cudaStream_t s) {
+int u8_to_inputs(const unsigned char* img_u8, const unsigned char* sk_u8, float* img, float* sk, int B, int H, int W, cudaStream_t s,
+                 const unsigned char* mask_u8, float* mask_soft, float* mask_bin) {
+  SE_REQUIRE(!mask_u8 || (mask_soft && mask_bin), "an edit mask needs its soft and binarised planes");
   const long long HW = (long long)H * W;
-  u8_to_inputs_kernel<<<cdiv(B * HW, 256), 256, 0, s>>>(img_u8, sk_u8, img, sk, B, HW);
+  u8_to_inputs_kernel<<<cdiv(B * HW, 256), 256, 0, s>>>(img_u8, sk_u8, img, sk, B, HW, mask_u8, mask_soft, mask_bin);
+  SE_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// a caller-supplied fp32 edit mask -> the binarised plane netG inpaints: m > 0.5 (editline2_model.py:347), the comparison of
+// head_kernel's HEAD_MASK branch, so netM's own soft mask binarises to the bytes the plain forward uses
+__global__ void binarise_kernel(const float* __restrict__ m, float* __restrict__ out, long long n) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i < n) out[i] = m[i] > 0.5f ? 1.0f : 0.0f;
+}
+int binarise(const float* m, float* out, long long n, cudaStream_t s) {
+  binarise_kernel<<<cdiv(n, 256), 256, 0, s>>>(m, out, n);
   SE_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -38,7 +38,11 @@ int softmax_rows(const float* S, int lds, float* P, int ldp, long long rows, int
 // fp32 [B][C][v.H][v.W] (nhwc: [B][v.H][v.W][C]) -> channels [0, C) of the activation y in layout v, and back
 int f32_to_act(const float* x, int nhwc, void* y, int dt, const Layout& v, int B, int C, cudaStream_t s);
 int act_to_f32(const void* x, int dt, const Layout& v, float* y, int nhwc, int B, int C, cudaStream_t s);
-int u8_to_inputs(const unsigned char* img_u8, const unsigned char* sk_u8, float* img, float* sk, int B, int H, int W, cudaStream_t s);
+// mask_u8 (optional, [B,H,W]): also writes its soft plane v/255 and its binarised plane (v/255 > 0.5) as fp32 [B,H,W]
+int u8_to_inputs(const unsigned char* img_u8, const unsigned char* sk_u8, float* img, float* sk, int B, int H, int W, cudaStream_t s,
+                 const unsigned char* mask_u8 = nullptr, float* mask_soft = nullptr, float* mask_bin = nullptr);
+// out[i] = m[i] > 0.5 ? 1 : 0 over n floats
+int binarise(const float* m, float* out, long long n, cudaStream_t s);
 int to_uint8(const float* comp, const float* mask, unsigned char* bgr, unsigned char* mk, int B, int H, int W, cudaStream_t s);
 int fill_zero(void* p, size_t bytes, cudaStream_t s);
 

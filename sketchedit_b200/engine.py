@@ -171,6 +171,46 @@ class Engine:
                                                     _stream()))
         return bgr, mk
 
+    def inference_with_mask(self, image, sketch, edit_mask, precision="bf16", want=()):
+        """The forward on a caller-supplied edit mask [B,1,H,W] instead of netM's prediction: netG inpaints
+        (edit_mask > 0.5) and composed = fine * edit_mask + image * (1 - edit_mask); values are used as given. Returns
+        (composed, extra) with any of want = ('coarse', 'fine', 'mask_image', 'mask_bin') in the dict. netM runs only
+        for 'mask_image'. Given the soft mask ``inference`` returned, every output equals that call's bit for bit."""
+        image = _chk_in(image, name="image")
+        sketch = _chk_in(sketch, name="sketch")
+        edit_mask = _chk_in(edit_mask, name="edit_mask")
+        B, _, H, W = image.shape
+        if tuple(edit_mask.shape) != (B, 1, H, W):
+            raise _lib.SketchEditB200Error("edit_mask must have shape %r (got %r)" % ((B, 1, H, W), tuple(edit_mask.shape)))
+        composed = _f32(B, 3, H, W, like=image)
+        extra = {k: _f32(B, 1 if k == "mask_bin" else 3, H, W, like=image) for k in want}
+        self._on_device(image, sketch, edit_mask)
+        _lib.check(self.lib.se_forward_with_mask(
+            self.h, _ptr(image), _ptr(sketch), _ptr(edit_mask), B, H, W, _lib.PREC[precision], _ptr(composed),
+            _ptr(extra.get("coarse")), _ptr(extra.get("fine")), _ptr(extra.get("mask_image")), _ptr(extra.get("mask_bin")),
+            _stream()))
+        return composed, extra
+
+    def inference_with_mask_u8(self, image_u8, sketch_u8, edit_mask_u8, precision="bf16", out=None):
+        """``inference_u8`` on a caller-supplied edit mask: edit_mask_u8 [B,H,W] uint8 means v/255 (inpainted where
+        v >= 128). Returns bgr_u8 [B,H,W,3]; ``out`` is a caller-owned contiguous CUDA uint8 tensor of that shape."""
+        for t, nm in ((image_u8, "image_u8"), (sketch_u8, "sketch_u8"), (edit_mask_u8, "edit_mask_u8")):
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
+                raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % nm)
+        B, H, W, C = image_u8.shape
+        if C != 3 or tuple(sketch_u8.shape) != (B, H, W) or tuple(edit_mask_u8.shape) != (B, H, W):
+            raise _lib.SketchEditB200Error("image_u8 must be [B,H,W,3], sketch_u8 and edit_mask_u8 [B,H,W]")
+        if out is None:
+            bgr = torch.empty(B, H, W, 3, device=image_u8.device, dtype=torch.uint8)
+        else:
+            bgr = out
+            if not (bgr.is_cuda and bgr.dtype == torch.uint8 and bgr.is_contiguous() and tuple(bgr.shape) == (B, H, W, 3)):
+                raise _lib.SketchEditB200Error("out must be a contiguous CUDA uint8 [B,H,W,3] tensor")
+        self._on_device(image_u8, sketch_u8, edit_mask_u8, bgr)
+        _lib.check(self.lib.se_forward_with_mask_u8(self.h, _ptr(image_u8), _ptr(sketch_u8), _ptr(edit_mask_u8), B, H, W,
+                                                    _lib.PREC[precision], _ptr(bgr), _stream()))
+        return bgr
+
     def netM(self, x, guide, precision="bf16", want_image=True):
         x, guide = _chk_in(x), _chk_in(guide)
         B, _, H, W = x.shape

@@ -9,6 +9,8 @@ too (``engine.resize_u8_packed``, bit-identical to Pillow), so a batch is one up
 
     proc = DemoProcessor(models.create_model(opt), max_batch=16, max_wait_ms=2.0)
     result_pil = proc.process_image(image_pil, mask_pil)       # callable from any number of threads
+    result_pil, mask = proc.process_image(image_pil, mask_pil, return_mask=True)       # ... and the predicted edit mask
+    result_pil = proc.process_image(image_pil, mask_pil, edit_mask=corrected_mask)      # run on a revised edit mask
     proc.close()
 
 Everything except the forward itself (``run_batch``) is plain host logic and is unit-tested on the CPU with a fake forward.
@@ -161,18 +163,22 @@ class DemoProcessor:
         return buf
 
     def _run_batch_device(self, key, payloads):
-        """payloads: (raw RGB photo [h,w,3], raw 'L' mask [hm,wm]) at their own sizes; key: the floored network size."""
+        """payloads: (raw RGB photo [h,w,3], raw 'L' mask [hm,wm], raw 'L' edit mask [he,we] or None, return_mask) at their own
+        sizes; key: the floored network size, plus True when the batch runs on edit masks."""
         torch = self._torch
         from .engine import resize_u8_packed
-        H, W = key
+        H, W = key[:2]
+        edit = len(key) > 2
         B = len(payloads)
         dev = self.engine.device
         photos, masks = [p[0] for p in payloads], [p[1] for p in payloads]
-        offs, total = _aligned_offsets([a.nbytes for a in photos + masks])
-        out_offs, out_total = _aligned_offsets([a.nbytes for a in photos])
+        edits = [p[2] for p in payloads] if edit else []
+        back = [i for i, p in enumerate(payloads) if p[3] and not edit]   # predicted masks to resize back and download
+        offs, total = _aligned_offsets([a.nbytes for a in photos + masks + edits])
+        out_offs, out_total = _aligned_offsets([a.nbytes for a in photos] + [photos[i].shape[0] * photos[i].shape[1] for i in back])
         stage = self._staging("in", total)          # free: every batch, failed ones included, ends with a stream synchronise
         host = stage.numpy()
-        for a, o in zip(photos + masks, offs):
+        for a, o in zip(photos + masks + edits, offs):
             host[o:o + a.nbytes] = a.reshape(-1)
         down = self._staging("out", out_total)
         with torch.cuda.device(dev):
@@ -183,45 +189,80 @@ class DemoProcessor:
                 resize_u8_packed(src, offs[:B], [a.shape[:2] for a in photos], [(H, W)] * B, 3, out=img,
                                  dst_offsets=[i * H * W * 3 for i in range(B)])
                 # the resized mask goes to the forward as it is: its input codec applies > 0 (demo.py:52)
-                resize_u8_packed(src, offs[B:], [a.shape[:2] for a in masks], [(H, W)] * B, 1, out=msk,
+                resize_u8_packed(src, offs[B:2 * B], [a.shape[:2] for a in masks], [(H, W)] * B, 1, out=msk,
                                  dst_offsets=[i * H * W for i in range(B)])
                 with torch.no_grad():
-                    bgr, _ = self.engine.inference_u8(img, msk, precision=self.precision)
+                    if edit:
+                        edt = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
+                        resize_u8_packed(src, offs[2 * B:], [a.shape[:2] for a in edits], [(H, W)] * B, 1, out=edt,
+                                         dst_offsets=[i * H * W for i in range(B)])
+                        bgr = self.engine.inference_with_mask_u8(img, msk, edt, precision=self.precision)
+                    else:
+                        bgr, mk = self.engine.inference_u8(img, msk, precision=self.precision)
                 # back to each photo's own size; the forward writes BGR, the demo keeps RGB
-                res, _ = resize_u8_packed(bgr, [i * H * W * 3 for i in range(B)], [(H, W)] * B, [a.shape[:2] for a in photos], 3,
-                                          swap_rb=True, out=torch.empty(max(out_total, 1), device=dev, dtype=torch.uint8),
-                                          dst_offsets=out_offs)
+                res = torch.empty(max(out_total, 1), device=dev, dtype=torch.uint8)
+                resize_u8_packed(bgr, [i * H * W * 3 for i in range(B)], [(H, W)] * B, [a.shape[:2] for a in photos], 3,
+                                 swap_rb=True, out=res, dst_offsets=out_offs[:B])
+                if back:
+                    resize_u8_packed(mk, [i * H * W for i in back], [(H, W)] * len(back), [photos[i].shape[:2] for i in back], 1,
+                                     out=res, dst_offsets=out_offs[B:])
                 down[:out_total].copy_(res[:out_total], non_blocking=True)
             finally:
                 torch.cuda.current_stream().synchronize()
         host = down.numpy()
-        return [host[o:o + a.nbytes].reshape(a.shape).copy() for a, o in zip(photos, out_offs)]
+        results = [host[o:o + a.nbytes].reshape(a.shape).copy() for a, o in zip(photos, out_offs)]
+        masks_back = dict(zip(back, [host[o:o + photos[i].shape[0] * photos[i].shape[1]].reshape(photos[i].shape[:2]).copy()
+                                     for i, o in zip(back, out_offs[B:])]))
+        return [(r, masks_back.get(i)) for i, r in enumerate(results)]
 
     def _run_batch(self, key, payloads):
+        """payloads: (photo [H,W,3], mask [H,W], edit mask [H,W] or None, return_mask) at the floored size ``key[:2]``."""
         torch = self._torch
         img = torch.from_numpy(np.stack([p[0] for p in payloads])).cuda(non_blocking=True)     # [B,H,W,3] RGB uint8
         msk = torch.from_numpy(np.stack([p[1] for p in payloads])).cuda(non_blocking=True)     # [B,H,W] uint8 (> 0 = stroke)
+        mk = None
         with torch.no_grad():
-            bgr, _ = self.engine.inference_u8(img, msk, precision=self.precision)
+            if len(key) > 2:
+                edt = torch.from_numpy(np.stack([p[2] for p in payloads])).cuda(non_blocking=True)
+                bgr = self.engine.inference_with_mask_u8(img, msk, edt, precision=self.precision)
+            else:
+                bgr, mk = self.engine.inference_u8(img, msk, precision=self.precision)
         rgb = bgr.cpu().numpy()[..., ::-1]                                                     # demo.py keeps RGB (test.py swaps to BGR)
-        return [np.ascontiguousarray(rgb[i]) for i in range(len(payloads))]
+        mk = mk.cpu().numpy() if mk is not None else None
+        return [(np.ascontiguousarray(rgb[i]), mk[i] if mk is not None and p[3] else None) for i, p in enumerate(payloads)]
 
-    def process_image(self, img, mask):
+    def process_image(self, img, mask, edit_mask=None, return_mask=False):
         """img: PIL image; mask: PIL 'L' image, usually of the same size (non-zero = sketch stroke). Returns the edited PIL
-        image at the input's size. Sizes are floored to a multiple of 8 for the network exactly like demo.py:43."""
+        image at the input's size. Sizes are floored to a multiple of 8 for the network exactly like demo.py:43.
+
+        edit_mask: PIL 'L' image of any size that replaces the predicted edit mask (mask revising): resized to the floored
+        size like the sketch mask, v/255 blends the result and v >= 128 is inpainted. return_mask=True returns
+        ``(result, mask)``: the predicted mask as an 'L' image at the photo's size (resized back like the result), or
+        ``edit_mask`` itself when one was given."""
         from PIL import Image
         img = img.convert("RGB")
         w_raw, h_raw = img.size
         h_t, w_t = floor8(h_raw), floor8(w_raw)
         if h_t < 16 or w_t < 16:
             raise ValueError("image smaller than 16x16 (two stride-2 convolutions, 4x4 mask pool, stride-2 patch grid)")
+        # requests on edit masks run their own forward: a batch never mixes them with predicted-mask requests
+        key = (h_t, w_t) if edit_mask is None else (h_t, w_t, True)
         if self.resize == "device":
-            if mask.mode != "L":
-                raise ValueError("resize='device' takes an 'L' mask (got mode %r); resize='host' resizes it with Pillow" % mask.mode)
-            out = self.batcher.submit((h_t, w_t), (np.asarray(img), np.asarray(mask)))
-            return Image.fromarray(out)
-        img_t = np.ascontiguousarray(np.array(img.resize((w_t, h_t))), dtype=np.uint8)
-        mask_t = np.array(mask.resize((w_t, h_t)))
-        mask_t = np.ascontiguousarray((mask_t > 0).astype(np.uint8) * 255)
-        out = self.batcher.submit((h_t, w_t), (img_t, mask_t))
-        return Image.fromarray(out).resize((w_raw, h_raw))
+            for m, nm in ((mask, "mask"), (edit_mask, "edit_mask")):
+                if m is not None and m.mode != "L":
+                    raise ValueError("resize='device' takes an 'L' %s (got mode %r); resize='host' resizes it with Pillow" % (nm, m.mode))
+            edit_raw = np.asarray(edit_mask) if edit_mask is not None else None
+            out, mk = self.batcher.submit(key, (np.asarray(img), np.asarray(mask), edit_raw, return_mask))
+            res = Image.fromarray(out)
+            mk = Image.fromarray(mk) if mk is not None else None
+        else:
+            img_t = np.ascontiguousarray(np.array(img.resize((w_t, h_t))), dtype=np.uint8)
+            mask_t = np.array(mask.resize((w_t, h_t)))
+            mask_t = np.ascontiguousarray((mask_t > 0).astype(np.uint8) * 255)
+            edit_t = np.ascontiguousarray(np.array(edit_mask.convert("L").resize((w_t, h_t))), dtype=np.uint8) if edit_mask is not None else None
+            out, mk = self.batcher.submit(key, (img_t, mask_t, edit_t, return_mask))
+            res = Image.fromarray(out).resize((w_raw, h_raw))
+            mk = Image.fromarray(mk).resize((w_raw, h_raw)) if mk is not None else None
+        if not return_mask:
+            return res
+        return res, (edit_mask if edit_mask is not None else mk)

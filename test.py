@@ -1,7 +1,10 @@
 """Batch inference entry point -- same command line as the reference's test.py (reference test.py:12-37,
 test_celeb.sh, test_places.sh): build the dataloader and the model from the flags, run
 ``model(data, mode='inference')`` per batch on the CUDA kernels, convert to uint8 (truncating, like
-``astype(np.uint8)``), RGB->BGR, and write PNGs to --output_dir (masks to --output_mask_dir)."""
+``astype(np.uint8)``), RGB->BGR, and write PNGs to --output_dir (masks to --output_mask_dir).
+
+``--edit_mask_dir D`` runs every entry on the mask ``D/<output name>`` instead of netM's prediction: write the masks with
+--output_mask_dir, correct the wrong ones by hand, and rerun with --edit_mask_dir pointing at them."""
 import os
 
 import cv2
