@@ -67,33 +67,22 @@ class EditLine2Model(torch.nn.Module):
 
     def forward(self, data, mode, is_real_im=True):
         image, line = self.preprocess_input(data)
-        if data.get("edit_mask") is not None:
-            return self._forward_with_mask(image, line, data["edit_mask"], mode)
+        if mode not in ("inference", "visualize"):
+            raise ValueError("|mode| is invalid or training-only: %r" % (mode,))
+        want = ("coarse", "fine", "mask_image", "mask_bin") if mode == "visualize" else ()
+        if data.get("edit_mask") is None:
+            composed, mask, ex = self.engine().inference(image, line, precision=self.precision, want=want)
+        else:
+            # data['mask'] is the sketch, as in the reference: netG inpaints edit_mask > 0.5 and the result is blended with
+            # edit_mask itself
+            mask = data["edit_mask"].to(image.device, torch.float32, non_blocking=True)
+            composed, ex = self.engine().inference_with_mask(image, line, mask, precision=self.precision, want=want)
         if mode == "inference":
-            composed, mask, _ = self.engine().inference(image, line, precision=self.precision)
             return composed, mask
-        if mode == "visualize":
-            # reference :134-145 -- 'mask' is the BINARISED mask netG inpaints (mask_inpaint), 'composed' is blended
-            # with the SOFT mask exactly like mode='inference'
-            composed, _, ex = self.engine().inference(image, line, precision=self.precision,
-                                                      want=("coarse", "fine", "mask_image", "mask_bin"))
-            return {"mask": ex["mask_bin"], "maskim": ex["mask_image"], "coarse": ex["coarse"], "fine": ex["fine"],
-                    "composed": composed}
-        raise ValueError("|mode| is invalid or training-only: %r" % (mode,))
-
-    def _forward_with_mask(self, image, line, edit_mask, mode):
-        """``data['edit_mask']`` [B,1,H,W] replaces netM's predicted mask (``data['mask']`` is the sketch, as in the
-        reference): netG inpaints edit_mask > 0.5 and the result is blended with edit_mask itself."""
-        edit_mask = edit_mask.to(image.device, torch.float32, non_blocking=True)
-        if mode == "inference":
-            composed, _ = self.engine().inference_with_mask(image, line, edit_mask, precision=self.precision)
-            return composed, edit_mask
-        if mode == "visualize":
-            composed, ex = self.engine().inference_with_mask(image, line, edit_mask, precision=self.precision,
-                                                             want=("coarse", "fine", "mask_image", "mask_bin"))
-            return {"mask": ex["mask_bin"], "maskim": ex["mask_image"], "coarse": ex["coarse"], "fine": ex["fine"],
-                    "composed": composed}
-        raise ValueError("|mode| is invalid or training-only: %r" % (mode,))
+        # reference :134-145 -- 'mask' is the BINARISED mask netG inpaints (mask_inpaint), 'composed' is blended
+        # with the SOFT mask exactly like mode='inference'
+        return {"mask": ex["mask_bin"], "maskim": ex["mask_image"], "coarse": ex["coarse"], "fine": ex["fine"],
+                "composed": composed}
 
     def inference_stream(self, loader, depth=2, pinned_ring=True, gather=None, uint8=False, with_data=False):
         """Pipelined form of ``for data in loader: model(data, mode='inference')`` for throughput serving.

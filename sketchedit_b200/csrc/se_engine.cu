@@ -10,10 +10,12 @@
 #include <algorithm>
 #include <atomic>
 #include <cmath>
+#include <cstring>
 #include <functional>
 #include <map>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/sketchedit_b200.h"
@@ -789,27 +791,25 @@ static std::vector<std::string> with_prefix(const std::string& pfx, std::initial
   return v;
 }
 
-// out_bs / msoft_bs: elements between images of out_nchw / mask_soft (0 = dense); non-zero when they are views into a packed
-// [B,4,H,W] output (se_forward_inference_packed)
-static int run_head(Ctx& c, char net, const std::string& name, const View& in, int mode, const float* img, const float* mask_bin,
-                    const float* mask_soft, float* out_nchw, float* out2, void* out_pack8, long long out_bs = 0, long long msoft_bs = 0,
-                    unsigned char* out_u8 = nullptr) {
+// io: the tensors of the head (HeadIO); its input map, sizes and mode are filled in here
+static int run_head(Ctx& c, char net, const std::string& name, const View& in, int mode, HeadIO io) {
   Layer* L = find_ready(c.m, net, name);
   SE_REQUIRE(L != nullptr && L->is_head, "head layer " + name + ": " + last_error());
   TAP("in:" + std::string(1, net) + "." + name, in, in.c8);
   {
     // 12-channel map in (two channel blocks on the C8 path), image / mask planes in, cout (+ blend / pack) planes out
     const double px = (double)c.B * in.H * in.W;
-    const double bytes = px * ((in.c8 ? 16 : 12) * c.esz() + (img ? 12 : 0) + (mask_bin ? 4 : 0) + (mask_soft ? 4 : 0) + (out_nchw ? 4 * L->spec.cout : 0) +
-                               (out2 ? 4 * (mode == HEAD_MASK ? 1 : L->spec.cout) : 0) + (out_pack8 ? 8 * c.esz() : 0));
+    const int outs = !!io.mask + !!io.mask_bin + !!io.stage + !!io.composed;
+    const double bytes = px * ((in.c8 ? 16 : 12) * c.esz() + (io.img ? 12 : 0) + (io.blend ? 4 : 0) + outs * 4 * L->spec.cout + (io.packed ? 8 * c.esz() : 0));
     const double fl = 2.0 * px * 9 * 12 * L->spec.cout;
     c.tag(std::string("head_kernel|12->") + std::to_string(L->spec.cout) + " k3 + " +
               (mode == HEAD_MASK ? "sigmoid+threshold" : mode == HEAD_TANH ? "tanh" : mode == HEAD_COARSE ? "tanh+blend+pack8" : "tanh+soft blend"),
           0, fl, fl, bytes);
   }
   SE_REQUIRE(in.c8 == (c.tc() ? 1 : 0) && in.ld == (c.tc() ? 2 * c.sp() : 12), "head input: dense 12 channels in the mode's storage");
-  CK(head(in.p, c.act_dt(), L->w_head_host.data(), L->b_host.data(), L->spec.cout, c.B, in.H, in.W, mode, img, mask_bin, mask_soft, out_nchw,
-          out2, out_pack8, c.m->opt[SE_OPT_NO_MASK_COARSE], stem_wp(in.W), STEM_PADL, out_bs, msoft_bs, out_u8, c.stream));
+  io.x = in.p; io.B = c.B; io.H = in.H; io.W = in.W; io.mode = mode;
+  io.Wp = stem_wp(in.W); io.padl = STEM_PADL; io.no_mask_coarse = c.m->opt[SE_OPT_NO_MASK_COARSE];
+  CK(head(io, c.act_dt(), L->w_head_host.data(), L->b_host.data(), L->spec.cout, c.stream));
   return 0;
 }
 
@@ -993,29 +993,39 @@ static int do_pool_broadcast(Ctx& c, const View& v, int mode, void* cat, int cat
   return 0;
 }
 
-// MDGenerator.forward: x [B,3,H,W], guide [B,1,H,W] -> mask1 (soft, NCHW), optional x_stage1; also the
-// binarised mask plane (mask1 > 0.5) when mask_bin != nullptr. mask1 == nullptr (a forward on a caller-supplied edit mask):
-// only the trunk (conv1-conv9) and the image decoder run, for x_stage1.
-static int run_netM(Ctx& c, const float* x, const float* guide, int H, int W, float* mask1, float* x_stage1, float* mask_bin, long long mask1_bs = 0,
-                    unsigned char* mask_u8 = nullptr) {
-  SE_REQUIRE(mask1 || x_stage1, "netM with neither output");
+// MDGenerator.forward: x [B,3,H,W], guide [B,1,H,W] -> the soft mask (mask_bs elements between images, 0 = dense) with its
+// binarised plane (> 0.5) and bytes where set, and x_stage1. Without a mask only the trunk (conv1-conv9) and the image decoder
+// run. All fields are 8 bytes wide: they form the graph key.
+struct NetMIO {
+  const float *x, *guide;
+  float* mask = nullptr;
+  long long mask_bs = 0;
+  float* mask_bin = nullptr;
+  unsigned char* mask_u8 = nullptr;
+  float* x_stage1 = nullptr;
+};
+
+static int run_netM(Ctx& c, int H, int W, const NetMIO& io) {
+  SE_REQUIRE(io.mask || io.x_stage1, "netM with neither output");
   Act in8, x9;
-  int rc = do_pack8(c, &in8, x, guide, nullptr, H, W, PACK_IMG_ONE, 1.0f, 0);
+  int rc = do_pack8(c, &in8, io.x, io.guide, nullptr, H, W, PACK_IMG_ONE, 1.0f, 0);
   if (rc) return rc;
   std::vector<std::string> trunk = with_prefix("", kEncoder);
   trunk.pop_back();   // conv10_atrous opens the mask branch
   rc = run_chain(c, 'M', trunk, in8, &x9);
   if (rc) return rc;
-  if (x_stage1) {
+  if (io.x_stage1) {
     // image decoder reads the conv9 output too (editline2_g.py:76-77)
     Act v16;
     rc = run_chain(c, 'M', with_prefix("conv", kDecoder), x9.borrow(), &v16);
     if (rc) return rc;
-    rc = run_head(c, 'M', "conv17", v16.v, HEAD_TANH, nullptr, nullptr, nullptr, x_stage1, nullptr, nullptr);
+    HeadIO h{};
+    h.stage = io.x_stage1;
+    rc = run_head(c, 'M', "conv17", v16.v, HEAD_TANH, h);
     if (rc) return rc;
     c.put(v16);
   }
-  if (!mask1) {
+  if (!io.mask) {
     c.put(x9);
     return 0;
   }
@@ -1025,9 +1035,10 @@ static int run_netM(Ctx& c, const float* x, const float* guide, int H, int W, fl
                  x9, &v);
   if (rc) return rc;
   Buf scratch;
-  float* mb = mask_bin;
-  if (!mb) { scratch = c.get((size_t)c.B * H * W * 4); mb = (float*)scratch.p; }
-  rc = run_head(c, 'M', "conv_mask_17", v.v, HEAD_MASK, nullptr, nullptr, nullptr, mask1, mb, nullptr, mask1_bs, 0, mask_u8);
+  HeadIO h{};
+  h.mask = io.mask; h.mask_bs = io.mask_bs; h.mask_bin = io.mask_bin; h.mask_u8 = io.mask_u8;
+  if (!h.mask_bin) { scratch = c.get((size_t)c.B * H * W * 4); h.mask_bin = (float*)scratch.p; }
+  rc = run_head(c, 'M', "conv_mask_17", v.v, HEAD_MASK, h);
   if (rc) return rc;
   c.put(scratch);
   c.put(v);
@@ -1044,12 +1055,19 @@ static int run_stem_pair(Ctx& c, Layer& pair, Act in, Buf* st) {
   return 0;
 }
 
-// DeepFillC2Generator.forward. x, x2 [B,3,H,W]; mask, mask2 planes [B,H,W]; guide [B,H,W] or null (ones).
-// Outputs: x_stage1 (optional), x_stage2 (optional NCHW), composed (optional: fine*soft + img*(1-soft)).
-static int run_netG(Ctx& c, const float* x, const float* x2, const float* mask, const float* mask2, const float* guide, int H, int W,
-                    float* x_stage1, float* x_stage2, float* composed, const float* mask_soft, const float* blend_img,
-                    long long composed_bs = 0, long long msoft_bs = 0, unsigned char* composed_u8 = nullptr) {
-  // guide == nullptr: the reference's guide=None -> an all-ones sketch channel (editline_g.py:127-130), built by pack8
+// DeepFillC2Generator.forward. x, x2 [B,3,H,W]; mask, mask2 planes [B,H,W]; guide [B,H,W] or null (ones, editline_g.py:127-130).
+// Outputs where set: x_stage1, x_stage2, composed = x_stage2 * mask_soft + x * (1 - mask_soft) (editline2_model.py:132) and its
+// BGR bytes. *_bs: elements between images, 0 = dense. All fields are 8 bytes wide: they form the graph key.
+struct NetGIO {
+  const float *x, *x2, *mask, *mask2, *guide;
+  float *x_stage1 = nullptr, *x_stage2 = nullptr, *composed = nullptr;
+  long long composed_bs = 0;
+  unsigned char* composed_u8 = nullptr;
+  const float* mask_soft = nullptr;
+  long long msoft_bs = 0;
+};
+
+static int run_netG(Ctx& c, int H, int W, const NetGIO& io) {
   const int* opt = c.m->opt;
   const int h = H / 4, w = W / 4;
   const size_t e = c.esz();
@@ -1059,7 +1077,7 @@ static int run_netG(Ctx& c, const float* x, const float* x2, const float* mask, 
   // stem pairs (tensor-core path, make_stem_pair): conv1 + wconv1 share one packed input when both encoders see the same image
   // and mask (always true on the inference path: netG(inputs, inputs, mask_bin, mask_bin, line)); xconv1 + pmconv1 always do.
   // Each encoder then reads its half of the pair's output and its chain starts at its second layer.
-  Layer* pair1 = (c.prec == SE_PREC_BF16_TC && x == x2 && mask == mask2) ? find_layer(c.m, 'G', "conv1+wconv1") : nullptr;
+  Layer* pair1 = (c.prec == SE_PREC_BF16_TC && io.x == io.x2 && io.mask == io.mask2) ? find_layer(c.m, 'G', "conv1+wconv1") : nullptr;
   Layer* pair2 = c.prec == SE_PREC_BF16_TC ? find_layer(c.m, 'G', "xconv1+pmconv1") : nullptr;
   auto pair_half = [&](const Buf& st, int which) { return s2dview(st.p, H, W, 24, 24, 12 * which); };
 
@@ -1069,17 +1087,17 @@ static int run_netG(Ctx& c, const float* x, const float* x2, const float* mask, 
   int rc = 0;
   if (pair1) {
     Act in8;
-    rc = do_pack8(c, &in8, x, guide, mask, H, W, PACK_IMG_ONE_MINUS_M, 1.0f, 1, style_img);
+    rc = do_pack8(c, &in8, io.x, io.guide, io.mask, H, W, PACK_IMG_ONE_MINUS_M, 1.0f, 1, style_img);
     if (rc) return rc;
     rc = run_stem_pair(c, *pair1, in8, &st1);
     if (rc) return rc;
   }
   Act in;
-  if (!pair1) rc = do_pack8(c, &in, x, guide, mask, H, W, PACK_IMG_ONE_MINUS_M, 1.0f, 1);
+  if (!pair1) rc = do_pack8(c, &in, io.x, io.guide, io.mask, H, W, PACK_IMG_ONE_MINUS_M, 1.0f, 1);
   if (rc) return rc;
   rc = run_chain(c, 'G', with_prefix("", kEncoder, pair1 ? 1 : 0), pair1 ? Act{pair_half(st1, 0)} : in, nullptr, Dst{cat1.p, cat_ld, 0});
   if (rc) return rc;
-  if (!pair1) rc = do_pack8(c, &in, x2, guide, mask2, H, W, style_img, opt[SE_OPT_JOINT_TRAIN_INP] ? 0.0f : 1.0f, 1);
+  if (!pair1) rc = do_pack8(c, &in, io.x2, io.guide, io.mask2, H, W, style_img, opt[SE_OPT_JOINT_TRAIN_INP] ? 0.0f : 1.0f, 1);
   if (rc) return rc;
   Act style;
   rc = run_chain(c, 'G', with_prefix("w", kEncoder, pair1 ? 1 : 0), pair1 ? Act{pair_half(st1, 1)} : in, &style);
@@ -1094,7 +1112,9 @@ static int run_netG(Ctx& c, const float* x, const float* x2, const float* mask, 
   if (rc) return rc;
   c.tag("memset|pad pixels of the packed stage-2 input", 0, 0, 0, (double)xnow.bytes);
   CK(fill_zero(xnow.p, xnow.bytes, c.stream));   // zero pad pixels of the packed stage-2 input
-  rc = run_head(c, 'G', "conv17", dec.v, HEAD_COARSE, x, mask, nullptr, x_stage1, nullptr, xnow.p);
+  HeadIO coarse{};
+  coarse.img = io.x; coarse.blend = io.mask; coarse.stage = io.x_stage1; coarse.packed = xnow.p;
+  rc = run_head(c, 'G', "conv17", dec.v, HEAD_COARSE, coarse);
   if (rc) return rc;
   c.put(dec);
 
@@ -1117,7 +1137,7 @@ static int run_netG(Ctx& c, const float* x, const float* x2, const float* mask, 
   if (opt[SE_OPT_USE_CAM]) {
     Buf ms = c.get((size_t)c.B * h * w * 4);
     c.tag("avgpool4_kernel", 0, 0, 0, (double)c.B * H * W * 4);
-    CK(avgpool4(mask, (float*)ms.p, c.B, H, W, c.stream));
+    CK(avgpool4(io.mask, (float*)ms.p, c.B, H, W, c.stream));
     TAP("in:G.cam", pm.v, pm.v.c8);
     TAP("in:G.cam.mask_s", nhwc(ms.p, h, w, 1, 1), 0, 0);
     Buf camo = c.get((size_t)c.B * h * w * 96 * e);
@@ -1144,13 +1164,76 @@ static int run_netG(Ctx& c, const float* x, const float* x2, const float* mask, 
   if (rc) return rc;
   rc = run_chain(c, 'G', with_prefix("allconv", kDecoder), Act{c.dense(cat2.p, h, w, 192, tc), cat2}, &dec);
   if (rc) return rc;
-  if (composed || composed_u8) {
-    rc = run_head(c, 'G', "allconv17", dec.v, HEAD_FINE, blend_img, nullptr, mask_soft, composed, x_stage2, nullptr, composed_bs, msoft_bs, composed_u8);
-  } else {
-    rc = run_head(c, 'G', "allconv17", dec.v, HEAD_TANH, nullptr, nullptr, nullptr, x_stage2, nullptr, nullptr);
+  HeadIO fine{};
+  fine.stage = io.x_stage2;
+  const bool blend = io.composed || io.composed_u8;
+  if (blend) {
+    fine.img = io.x; fine.blend = io.mask_soft; fine.blend_bs = io.msoft_bs;
+    fine.composed = io.composed; fine.composed_bs = io.composed_bs; fine.bgr_u8 = io.composed_u8;
   }
+  rc = run_head(c, 'G', "allconv17", dec.v, blend ? HEAD_FINE : HEAD_TANH, fine);
   if (rc) return rc;
   c.put(dec);
+  return 0;
+}
+
+// One generate_fake call (editline2_model.py:338-370): image and sketch or their bytes; netM or the caller's edit mask (fp32, or
+// bytes v meaning v/255); outputs where set, *_bs elements between images (0 = dense); mask_bin_in replaces netM's binarised
+// mask, mask_bin_out receives the one netG inpaints. All fields are 8 bytes wide: they form the graph key.
+struct Request {
+  const float *image = nullptr, *sketch = nullptr;
+  const unsigned char *image_u8 = nullptr, *sketch_u8 = nullptr;
+  const float* edit_mask = nullptr;
+  const unsigned char* edit_mask_u8 = nullptr;
+  float *composed = nullptr, *mask = nullptr;
+  long long composed_bs = 0, mask_bs = 0;
+  unsigned char *bgr_u8 = nullptr, *mask_u8 = nullptr;
+  float *coarse = nullptr, *fine = nullptr, *mask_image = nullptr;
+  const float* mask_bin_in = nullptr;
+  float* mask_bin_out = nullptr;
+};
+
+// input codec, mask source, netM (only its trunk and image decoder, for mask_image, on a caller's mask), then
+// netG(inputs, inputs, mask_bin, mask_bin, line) (editline2_model.py:368) blended with the soft mask
+static int run_generate(Ctx& c, int H, int W, const Request& r) {
+  const size_t plane = (size_t)c.B * H * W * 4;
+  const bool from_netM = !r.edit_mask && !r.edit_mask_u8;
+  const float *image = r.image, *sketch = r.sketch;
+  Buf img, sk, soft, mb;
+  if (r.image_u8) {
+    // input codec (reference data/testimage_dataset.py:89-103); the output codec is fused into the two heads (test.py:25-35):
+    // the float image and masks live only in the workspace
+    img = c.get(3 * plane); sk = c.get(plane); soft = c.get(plane); mb = c.get(plane);
+    image = (const float*)img.p, sketch = (const float*)sk.p;
+    c.tag(r.edit_mask_u8 ? "u8_to_inputs_kernel|input codec + edit mask" : "u8_to_inputs_kernel|input codec", 0, 0, 0,
+          (double)c.B * H * W * (r.edit_mask_u8 ? 5 + 24 : 4 + 16));
+    CK(u8_to_inputs(r.image_u8, r.sketch_u8, r.edit_mask_u8, (float*)img.p, (float*)sk.p, (float*)soft.p, (float*)mb.p, c.B, H, W, c.stream));
+  } else if (from_netM || !r.mask_bin_out) {
+    mb = c.get(plane);
+  }
+  float* msoft = r.image_u8 ? (float*)soft.p : r.mask;   // netM's soft mask, or the decoded edit mask
+  const float* mbin = r.edit_mask && r.mask_bin_out ? r.mask_bin_out : (const float*)mb.p;   // the mask netG inpaints
+  if (r.edit_mask) {
+    c.tag("binarise_kernel|edit mask > 0.5", 0, 0, 0, (double)c.B * H * W * 8);
+    CK(binarise(r.edit_mask, (float*)mbin, (long long)c.B * H * W, c.stream));
+  }
+  if (from_netM || r.mask_image) {
+    NetMIO nm{image, sketch};
+    nm.x_stage1 = r.mask_image;
+    if (from_netM) { nm.mask = msoft; nm.mask_bs = r.mask_bs; nm.mask_bin = (float*)mb.p; nm.mask_u8 = r.mask_u8; }
+    int rc = run_netM(c, H, W, nm);
+    if (rc) return rc;
+  }
+  if (from_netM && r.mask_bin_in) mbin = r.mask_bin_in;
+  if (from_netM && r.mask_bin_out && !c.dry) SE_CUDA_OK(cudaMemcpyAsync(r.mask_bin_out, mbin, plane, cudaMemcpyDeviceToDevice, c.stream));
+  NetGIO g{image, image, mbin, mbin, sketch};
+  g.x_stage1 = r.coarse; g.x_stage2 = r.fine;
+  g.composed = r.composed; g.composed_bs = r.composed_bs; g.composed_u8 = r.bgr_u8;
+  g.mask_soft = r.edit_mask ? r.edit_mask : msoft;
+  g.msoft_bs = r.edit_mask ? 0 : r.mask_bs;
+  int rc = run_netG(c, H, W, g);
+  if (rc) return rc;
+  c.put(mb); c.put(soft); c.put(sk); c.put(img);
   return 0;
 }
 
@@ -1328,6 +1411,21 @@ static int check_hw(int H, int W) {
   return 0;
 }
 
+// run(c, H, W, a) under a graph keyed on the kind, size and every byte of the argument struct a, so that a replay never writes
+// through a pointer the call did not pass (with_arena appends the options, precision, B and the attention limit)
+template <class Args>
+static int keyed_forward(se_model* m, int prec, int B, int H, int W, void* stream, uintptr_t kind, const Args& a,
+                         int (*run)(Ctx&, int, int, const Args&)) {
+  static_assert(std::has_unique_object_representations_v<Args> && sizeof(Args) % sizeof(uintptr_t) == 0,
+                "argument structs hold 8-byte fields only, so that every field is part of the key");
+  int rc = check_hw(H, W);
+  if (rc) return rc;
+  std::vector<uintptr_t> key(3 + sizeof(Args) / sizeof(uintptr_t));
+  key[0] = kind; key[1] = (uintptr_t)H; key[2] = (uintptr_t)W;
+  memcpy(&key[3], &a, sizeof(Args));
+  return with_arena(m, prec, B, (cudaStream_t)stream, [&](Ctx& c) { return run(c, H, W, a); }, key);
+}
+
 }  // namespace se
 
 // ============================================================================================ C ABI
@@ -1424,131 +1522,64 @@ int se_model_finalize(se_model* m) {
   return 0;
 }
 
-static int forward_inference(se_model* m, const float* image, const float* sketch, int B, int H, int W, int precision, float* composed,
-                             float* mask, long long composed_bs, long long mask_bs, float* coarse, float* fine, float* mask_image,
-                             const float* mask_bin_in, float* mask_bin_out, cudaStream_t st) {
-  SE_REQUIRE(image && sketch && composed && mask, "null tensor");
-  int rc = check_hw(H, W);
-  if (rc) return rc;
-  std::vector<uintptr_t> key = {1, (uintptr_t)H, (uintptr_t)W, (uintptr_t)image, (uintptr_t)sketch, (uintptr_t)composed, (uintptr_t)mask, (uintptr_t)composed_bs,
-                                (uintptr_t)mask_bs, (uintptr_t)coarse, (uintptr_t)fine, (uintptr_t)mask_image, (uintptr_t)mask_bin_in, (uintptr_t)mask_bin_out};
-  return with_arena(m, precision, B, st, [&](Ctx& c) -> int {
-    Buf mb = c.get((size_t)B * H * W * 4);
-    int r = run_netM(c, image, sketch, H, W, mask, mask_image, (float*)mb.p, mask_bs);
-    if (r) return r;
-    const float* mbin = (const float*)mb.p;
-    if (mask_bin_in) mbin = mask_bin_in;
-    if (mask_bin_out && !c.dry) {
-      SE_CUDA_OK(cudaMemcpyAsync(mask_bin_out, mbin, (size_t)B * H * W * 4, cudaMemcpyDeviceToDevice, c.stream));
-    }
-    // generate_fake: netG(inputs, inputs, mask_bin, mask_bin, line)   (editline2_model.py:368)
-    r = run_netG(c, image, image, mbin, mbin, sketch, H, W, coarse, fine, composed, mask, image, composed_bs, mask_bs);
-    if (r) return r;
-    c.put(mb);
-    return 0;
-  }, key);
-}
-
 int se_forward_inference(se_model* m, const float* image, const float* sketch, int B, int H, int W, int precision, float* composed,
                          float* mask, float* coarse, float* fine, float* mask_image, const float* mask_bin_in, float* mask_bin_out,
                          void* stream) {
-  return forward_inference(m, image, sketch, B, H, W, precision, composed, mask, 0, 0, coarse, fine, mask_image, mask_bin_in, mask_bin_out,
-                           (cudaStream_t)stream);
+  SE_REQUIRE(image && sketch && composed && mask, "null tensor");
+  Request r;
+  r.image = image; r.sketch = sketch; r.composed = composed; r.mask = mask;
+  r.coarse = coarse; r.fine = fine; r.mask_image = mask_image; r.mask_bin_in = mask_bin_in; r.mask_bin_out = mask_bin_out;
+  return keyed_forward(m, precision, B, H, W, stream, 1, r, run_generate);
 }
 
 int se_forward_inference_packed(se_model* m, const float* image, const float* sketch, int B, int H, int W, int precision, float* packed,
                                 void* stream) {
-  SE_REQUIRE(packed != nullptr, "null tensor");
-  const long long bs = 4LL * H * W;   // [B,4,H,W]: composed in channels 0-2, the soft mask in channel 3
-  return forward_inference(m, image, sketch, B, H, W, precision, packed, packed + 3LL * H * W, bs, bs, nullptr, nullptr, nullptr, nullptr, nullptr,
-                           (cudaStream_t)stream);
+  SE_REQUIRE(image && sketch && packed, "null tensor");
+  Request r;
+  r.image = image; r.sketch = sketch;
+  r.composed = packed; r.mask = packed + 3LL * H * W;   // [B,4,H,W]: composed in channels 0-2, the soft mask in channel 3
+  r.composed_bs = r.mask_bs = 4LL * H * W;
+  return keyed_forward(m, precision, B, H, W, stream, 1, r, run_generate);
 }
 
 int se_forward_inference_u8(se_model* m, const unsigned char* image_u8, const unsigned char* sketch_u8, int B, int H, int W, int precision,
                             unsigned char* bgr_u8, unsigned char* mask_u8, void* stream) {
   SE_REQUIRE(image_u8 && sketch_u8 && bgr_u8 && mask_u8, "null tensor");
-  int rc = check_hw(H, W);
-  if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  std::vector<uintptr_t> key = {4, (uintptr_t)H, (uintptr_t)W, (uintptr_t)image_u8, (uintptr_t)sketch_u8, (uintptr_t)bgr_u8, (uintptr_t)mask_u8};
-  return with_arena(m, precision, B, st, [&](Ctx& c) -> int {
-    // input codec (reference data/testimage_dataset.py:89-103) -> the usual forward -> output codec fused into the two heads
-    // (test.py:25-35): the float image / masks live only in the workspace
-    Buf img = c.get((size_t)B * 3 * H * W * 4), sk = c.get((size_t)B * H * W * 4), soft = c.get((size_t)B * H * W * 4), mb = c.get((size_t)B * H * W * 4);
-    c.tag("u8_to_inputs_kernel|input codec", 0, 0, 0, (double)B * H * W * (4 + 16));
-    CK(u8_to_inputs(image_u8, sketch_u8, (float*)img.p, (float*)sk.p, B, H, W, c.stream));
-    int r = run_netM(c, (const float*)img.p, (const float*)sk.p, H, W, (float*)soft.p, nullptr, (float*)mb.p, 0, mask_u8);
-    if (r) return r;
-    r = run_netG(c, (const float*)img.p, (const float*)img.p, (const float*)mb.p, (const float*)mb.p, (const float*)sk.p, H, W, nullptr, nullptr, nullptr,
-                 (const float*)soft.p, (const float*)img.p, 0, 0, bgr_u8);
-    if (r) return r;
-    c.put(mb); c.put(soft); c.put(sk); c.put(img);
-    return 0;
-  }, key);
+  Request r;
+  r.image_u8 = image_u8; r.sketch_u8 = sketch_u8; r.bgr_u8 = bgr_u8; r.mask_u8 = mask_u8;
+  return keyed_forward(m, precision, B, H, W, stream, 1, r, run_generate);
 }
 
-// generate_fake (editline2_model.py:338-370) with netM's soft mask replaced by the caller's edit mask: netG inpaints
-// (edit_mask > 0.5) and the result is blended with edit_mask itself. netM runs only for mask_image (its trunk and image decoder).
 int se_forward_with_mask(se_model* m, const float* image, const float* sketch, const float* edit_mask, int B, int H, int W, int precision,
                          float* composed, float* coarse, float* fine, float* mask_image, float* mask_bin_out, void* stream) {
   SE_REQUIRE(image && sketch && edit_mask && composed, "null tensor");
-  int rc = check_hw(H, W);
-  if (rc) return rc;
-  std::vector<uintptr_t> key = {5, (uintptr_t)H, (uintptr_t)W, (uintptr_t)image, (uintptr_t)sketch, (uintptr_t)edit_mask, (uintptr_t)composed,
-                                (uintptr_t)coarse, (uintptr_t)fine, (uintptr_t)mask_image, (uintptr_t)mask_bin_out};
-  return with_arena(m, precision, B, (cudaStream_t)stream, [&](Ctx& c) -> int {
-    Buf mb;
-    float* mbin = mask_bin_out;
-    if (!mbin) { mb = c.get((size_t)B * H * W * 4); mbin = (float*)mb.p; }
-    c.tag("binarise_kernel|edit mask > 0.5", 0, 0, 0, (double)B * H * W * 8);
-    CK(binarise(edit_mask, mbin, (long long)B * H * W, c.stream));
-    if (mask_image) {
-      int r = run_netM(c, image, sketch, H, W, nullptr, mask_image, nullptr);
-      if (r) return r;
-    }
-    int r = run_netG(c, image, image, mbin, mbin, sketch, H, W, coarse, fine, composed, edit_mask, image);
-    if (r) return r;
-    c.put(mb);
-    return 0;
-  }, key);
+  Request r;
+  r.image = image; r.sketch = sketch; r.edit_mask = edit_mask; r.composed = composed;
+  r.coarse = coarse; r.fine = fine; r.mask_image = mask_image; r.mask_bin_out = mask_bin_out;
+  return keyed_forward(m, precision, B, H, W, stream, 1, r, run_generate);
 }
 
-// se_forward_inference_u8's codecs around se_forward_with_mask: the edit mask arrives as bytes v and means v/255
 int se_forward_with_mask_u8(se_model* m, const unsigned char* image_u8, const unsigned char* sketch_u8, const unsigned char* edit_mask_u8, int B,
                             int H, int W, int precision, unsigned char* bgr_u8, void* stream) {
   SE_REQUIRE(image_u8 && sketch_u8 && edit_mask_u8 && bgr_u8, "null tensor");
-  int rc = check_hw(H, W);
-  if (rc) return rc;
-  std::vector<uintptr_t> key = {6, (uintptr_t)H, (uintptr_t)W, (uintptr_t)image_u8, (uintptr_t)sketch_u8, (uintptr_t)edit_mask_u8, (uintptr_t)bgr_u8};
-  return with_arena(m, precision, B, (cudaStream_t)stream, [&](Ctx& c) -> int {
-    Buf img = c.get((size_t)B * 3 * H * W * 4), sk = c.get((size_t)B * H * W * 4), soft = c.get((size_t)B * H * W * 4), mb = c.get((size_t)B * H * W * 4);
-    c.tag("u8_to_inputs_kernel|input codec + edit mask", 0, 0, 0, (double)B * H * W * (5 + 24));
-    CK(u8_to_inputs(image_u8, sketch_u8, (float*)img.p, (float*)sk.p, B, H, W, c.stream, edit_mask_u8, (float*)soft.p, (float*)mb.p));
-    int r = run_netG(c, (const float*)img.p, (const float*)img.p, (const float*)mb.p, (const float*)mb.p, (const float*)sk.p, H, W, nullptr, nullptr, nullptr,
-                     (const float*)soft.p, (const float*)img.p, 0, 0, bgr_u8);
-    if (r) return r;
-    c.put(mb); c.put(soft); c.put(sk); c.put(img);
-    return 0;
-  }, key);
+  Request r;
+  r.image_u8 = image_u8; r.sketch_u8 = sketch_u8; r.edit_mask_u8 = edit_mask_u8; r.bgr_u8 = bgr_u8;
+  return keyed_forward(m, precision, B, H, W, stream, 1, r, run_generate);
 }
 
 int se_netM_forward(se_model* m, const float* x, const float* guide, int B, int H, int W, int precision, float* mask1, float* x_stage1,
                     void* stream) {
   SE_REQUIRE(x && guide && mask1, "null tensor");
-  int rc = check_hw(H, W);
-  if (rc) return rc;
-  return with_arena(m, precision, B, (cudaStream_t)stream, [&](Ctx& c) -> int { return run_netM(c, x, guide, H, W, mask1, x_stage1, nullptr); },
-                    {2, (uintptr_t)H, (uintptr_t)W, (uintptr_t)x, (uintptr_t)guide, (uintptr_t)mask1, (uintptr_t)x_stage1});
+  NetMIO io{x, guide, mask1};
+  io.x_stage1 = x_stage1;
+  return keyed_forward(m, precision, B, H, W, stream, 2, io, run_netM);
 }
 
 int se_netG_forward(se_model* m, const float* x, const float* x2, const float* mask, const float* mask2, const float* guide, int B, int H,
                     int W, int precision, float* x_stage1, float* x_stage2, void* stream) {
   SE_REQUIRE(x && x2 && mask && mask2 && x_stage2, "null tensor");   // guide may be NULL: guide=None of the reference
-  int rc = check_hw(H, W);
-  if (rc) return rc;
-  return with_arena(m, precision, B, (cudaStream_t)stream,
-                    [&](Ctx& c) -> int { return run_netG(c, x, x2, mask, mask2, guide, H, W, x_stage1, x_stage2, nullptr, nullptr, nullptr); },
-                    {3, (uintptr_t)H, (uintptr_t)W, (uintptr_t)x, (uintptr_t)x2, (uintptr_t)mask, (uintptr_t)mask2, (uintptr_t)guide, (uintptr_t)x_stage1, (uintptr_t)x_stage2});
+  const NetGIO io{x, x2, mask, mask2, guide, x_stage1, x_stage2};
+  return keyed_forward(m, precision, B, H, W, stream, 3, io, run_netG);
 }
 
 int se_gated_conv_forward(se_model* m, char net, const char* layer, const float* x, int B, int H, int W, int precision, float* y,

@@ -176,19 +176,15 @@ struct HeadWeights {
   float b[COUT];
 };
 template <class St, int COUT>
-__global__ void __launch_bounds__(128) head_kernel(const void* __restrict__ x, const __grid_constant__ HeadWeights<COUT> hw, int B, int H,
-                                                   int W, int mode, const float* __restrict__ img, const float* __restrict__ mask_bin,
-                                                   const float* __restrict__ mask_soft, float* __restrict__ out_nchw,
-                                                   float* __restrict__ out2, void* __restrict__ out_pack8, int no_mask_coarse, int Wp,
-                                                   int padl, long long obs, long long msbs, unsigned char* __restrict__ out_u8) {
-  // obs: elements between images of out_nchw (COUT*HW when dense; 4*HW when it is a view into a packed [B,4,H,W] output);
-  // msbs: likewise for mask_soft
+__global__ void __launch_bounds__(128) head_kernel(const __grid_constant__ HeadWeights<COUT> hw, const __grid_constant__ HeadIO io) {
+  // the *_bs strides are set (head_launch); mask_bs and composed_bs are 4*HW when the output is a view into a packed [B,4,H,W] output
   // bf16 sums each output as an (even, odd) pair of partial sums over the channel pairs of its bf16x2 words, the bias added last;
   // the fp32 storages keep one FMA chain from the bias in channel order (the order tests/util_stages.py bounds)
   constexpr bool kPairs = std::is_same<St, Bf16>::value;
+  const int H = io.H, W = io.W;
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   const long long HW = (long long)H * W;
-  if (i >= B * HW) return;
+  if (i >= io.B * HW) return;
   const long long b = i / HW, pix = i % HW;
   const int yy = (int)(pix / W), xx = (int)(pix % W);
   float2 acc[COUT];
@@ -202,11 +198,11 @@ __global__ void __launch_bounds__(128) head_kernel(const void* __restrict__ x, c
     float v[2][8];   // channels 0..7, 8..11 (12..15: padding of the second block)
     if constexpr (St::kBlocked) {
       const size_t o = ((size_t)b * 2 * St::kHalves * HW + q) * 8, blk = (size_t)HW * 8;
-      St::load8(x, o, 2 * blk, v[0]);
-      St::load8(x, o + blk, 2 * blk, v[1]);
+      St::load8(io.x, o, 2 * blk, v[0]);
+      St::load8(io.x, o + blk, 2 * blk, v[1]);
     } else {
-      St::load8(x, (size_t)(b * HW + q) * 12, 0, v[0]);
-      St::template load8<4>(x, (size_t)(b * HW + q) * 12 + 8, 0, v[1]);
+      St::load8(io.x, (size_t)(b * HW + q) * 12, 0, v[0]);
+      St::template load8<4>(io.x, (size_t)(b * HW + q) * 12 + 8, 0, v[1]);
     }
 #pragma unroll
     for (int p = 0; p < 6; ++p) {
@@ -226,70 +222,60 @@ __global__ void __launch_bounds__(128) head_kernel(const void* __restrict__ x, c
   float r[COUT];
 #pragma unroll
   for (int o = 0; o < COUT; ++o) r[o] = kPairs ? hw.b[o] + (acc[o].x + acc[o].y) : acc[o].x;
-  if (mode == HEAD_MASK) {
+  if (io.mode == HEAD_MASK) {
     const float sg = 1.0f / (1.0f + expf(-r[0]));
-    out_nchw[b * obs + pix] = sg;
-    out2[i] = sg > 0.5f ? 1.0f : 0.0f;
-    if (out_u8) out_u8[i] = (unsigned char)(int)(sg * 255.0f);   // test.py:25: (mask * 255).astype(uint8)
+    io.mask[b * io.mask_bs + pix] = sg;
+    io.mask_bin[i] = sg > 0.5f ? 1.0f : 0.0f;
+    if (io.mask_u8) io.mask_u8[i] = (unsigned char)(int)(sg * 255.0f);   // test.py:25: (mask * 255).astype(uint8)
     return;
   }
   float t3[COUT];
 #pragma unroll
   for (int o = 0; o < COUT; ++o) t3[o] = tanhf(r[o]);
-  if (mode == HEAD_TANH) {
+  if (io.mode == HEAD_TANH) {
 #pragma unroll
-    for (int o = 0; o < COUT; ++o) out_nchw[b * obs + o * HW + pix] = t3[o];
-  } else if (mode == HEAD_COARSE) {
-    const float m = mask_bin[i];
+    for (int o = 0; o < COUT; ++o) io.stage[(b * COUT + o) * HW + pix] = t3[o];
+  } else if (io.mode == HEAD_COARSE) {
+    const float m = io.blend[i];
     float pk[8];
 #pragma unroll
     for (int o = 0; o < 8; ++o) pk[o] = 0.0f;
 #pragma unroll
     for (int o = 0; o < COUT; ++o) {
-      if (out_nchw) out_nchw[b * obs + o * HW + pix] = t3[o];
-      const float xin = img[(b * 3 + o) * HW + pix] * (1.0f - m);
-      pk[o] = no_mask_coarse ? t3[o] : (t3[o] * m + xin * (1.0f - m));
+      if (io.stage) io.stage[(b * COUT + o) * HW + pix] = t3[o];
+      const float xin = io.img[(b * 3 + o) * HW + pix] * (1.0f - m);
+      pk[o] = io.no_mask_coarse ? t3[o] : (t3[o] * m + xin * (1.0f - m));
     }
-    const size_t o = (((size_t)b * St::kHalves * H + yy) * Wp + xx + padl) * 8;   // packed rows, as pack8 writes them
-    St::store8(out_pack8, o, (size_t)H * Wp * 8, pk);
+    const size_t o = (((size_t)b * St::kHalves * H + yy) * io.Wp + xx + io.padl) * 8;   // packed rows, as pack8 writes them
+    St::store8(io.packed, o, (size_t)H * io.Wp * 8, pk);
   } else {  // HEAD_FINE
-    const float m = mask_soft[b * msbs + pix];
+    const float m = io.blend[b * io.blend_bs + pix];
 #pragma unroll
     for (int o = 0; o < COUT; ++o) {
-      if (out2) out2[(b * COUT + o) * HW + pix] = t3[o];
-      const float cv = t3[o] * m + img[(b * 3 + o) * HW + pix] * (1.0f - m);
-      if (out_nchw) out_nchw[b * obs + o * HW + pix] = cv;
-      if (out_u8) out_u8[i * 3 + (2 - o)] = (unsigned char)(int)((cv + 1.0f) / 2.0f * 255.0f);   // test.py:26-35: truncate, HWC, RGB -> BGR
+      if (io.stage) io.stage[(b * COUT + o) * HW + pix] = t3[o];
+      const float cv = t3[o] * m + io.img[(b * 3 + o) * HW + pix] * (1.0f - m);
+      if (io.composed) io.composed[b * io.composed_bs + o * HW + pix] = cv;
+      if (io.bgr_u8) io.bgr_u8[i * 3 + (2 - o)] = (unsigned char)(int)((cv + 1.0f) / 2.0f * 255.0f);   // test.py:26-35: truncate, HWC, RGB -> BGR
     }
   }
 }
 
 template <int COUT>
-static int head_launch(const void* x, int dt, const float* w_host, const float* b_host, int B, int H, int W, int mode, const float* img,
-                       const float* mask_bin, const float* mask_soft, float* out_nchw, float* out2, void* out_pack8, int no_mask_coarse,
-                       int Wp, int padl, long long obs, long long msbs, unsigned char* out_u8, cudaStream_t s) {
+static int head_launch(HeadIO io, int dt, const float* w_host, const float* b_host, cudaStream_t s) {
   HeadWeights<COUT> hw;
   for (int t = 0; t < 9; ++t)
     for (int p = 0; p < 6; ++p)
       for (int o = 0; o < COUT; ++o) hw.w[t][p][o] = make_float2(w_host[(t * 12 + 2 * p) * COUT + o], w_host[(t * 12 + 2 * p + 1) * COUT + o]);
   for (int o = 0; o < COUT; ++o) hw.b[o] = b_host[o];
-  const long long n = (long long)B * H * W;
-  if (!obs) obs = (long long)COUT * H * W;
-  if (!msbs) msbs = (long long)H * W;
-  return with_storage(dt, [&](auto st) {
-    head_kernel<decltype(st), COUT><<<cdiv(n, 128), 128, 0, s>>>(x, hw, B, H, W, mode, img, mask_bin, mask_soft, out_nchw, out2, out_pack8,
-                                                                 no_mask_coarse, Wp, padl, obs, msbs, out_u8);
-  });
+  const long long HW = (long long)io.H * io.W;
+  if (!io.blend_bs) io.blend_bs = HW;
+  if (!io.mask_bs) io.mask_bs = HW;
+  if (!io.composed_bs) io.composed_bs = 3 * HW;
+  return with_storage(dt, [&](auto st) { head_kernel<decltype(st), COUT><<<cdiv(io.B * HW, 128), 128, 0, s>>>(hw, io); });
 }
-int head(const void* x, int dt, const float* w_host, const float* b_host, int cout, int B, int H, int W, int mode, const float* img,
-         const float* mask_bin, const float* mask_soft, float* out_nchw, float* out2, void* out_pack8, int no_mask_coarse, int Wp, int padl,
-         long long obs, long long msbs, unsigned char* out_u8, cudaStream_t s) {
+int head(HeadIO io, int dt, const float* w_host, const float* b_host, int cout, cudaStream_t s) {
   SE_REQUIRE(cout == 1 || cout == 3, "head cout");
-  if (cout == 1)
-    return head_launch<1>(x, dt, w_host, b_host, B, H, W, mode, img, mask_bin, mask_soft, out_nchw, out2, out_pack8, no_mask_coarse, Wp, padl,
-                          obs, msbs, out_u8, s);
-  return head_launch<3>(x, dt, w_host, b_host, B, H, W, mode, img, mask_bin, mask_soft, out_nchw, out2, out_pack8, no_mask_coarse, Wp, padl, obs,
-                        msbs, out_u8, s);
+  return cout == 1 ? head_launch<1>(io, dt, w_host, b_host, s) : head_launch<3>(io, dt, w_host, b_host, s);
 }
 
 // ------------------------------------------------------------------------------------------ plane reductions
@@ -623,8 +609,8 @@ __global__ void u8_to_inputs_kernel(const unsigned char* __restrict__ img_u8, co
     mask_bin[i] = m > 0.5f ? 1.0f : 0.0f;
   }
 }
-int u8_to_inputs(const unsigned char* img_u8, const unsigned char* sk_u8, float* img, float* sk, int B, int H, int W, cudaStream_t s,
-                 const unsigned char* mask_u8, float* mask_soft, float* mask_bin) {
+int u8_to_inputs(const unsigned char* img_u8, const unsigned char* sk_u8, const unsigned char* mask_u8, float* img, float* sk, float* mask_soft,
+                 float* mask_bin, int B, int H, int W, cudaStream_t s) {
   SE_REQUIRE(!mask_u8 || (mask_soft && mask_bin), "an edit mask needs its soft and binarised planes");
   const long long HW = (long long)H * W;
   u8_to_inputs_kernel<<<cdiv(B * HW, 256), 256, 0, s>>>(img_u8, sk_u8, img, sk, B, HW, mask_u8, mask_soft, mask_bin);

@@ -20,12 +20,26 @@ struct Layout { int kind, H, W, ld, Wp, padl; };
 
 int pack8(const float* img, const float* sketch, const float* mask, void* out, int dt, int B, int H, int W, int Wp, int padl,
           int img_mode, float sketch_scale, int write_mask, cudaStream_t s, int img2_mode = -1);   // img2_mode >= 0: channels 5..7 = img * f(mask)
-// x: fp32 NHWC [B][H][W][12] or two channel blocks; w_host / b_host: host copies of the [9][12][cout] weights and the bias (the
-// kernel parameters are built from them). out_pack8: packed rows as pack8 writes them. Strides: elements between images of
-// out_nchw / msoft, 0 = dense. out_u8: HEAD_MASK -> mask bytes [B,H,W], HEAD_FINE -> BGR HWC bytes
-int head(const void* x, int dt, const float* w_host, const float* b_host, int cout, int B, int H, int W, int mode, const float* img,
-         const float* mask_bin, const float* mask_soft, float* out_nchw, float* out2, void* out_pack8, int no_mask_coarse, int Wp, int padl,
-         long long out_bstride, long long msoft_bstride, unsigned char* out_u8, cudaStream_t s);
+// One head launch, passed by value. Outputs are written where set; *_bs: elements between images, 0 = dense. x: fp32 NHWC
+// [B][H][W][12] or two channel blocks. blend: the mask blended with, [B,H,W] (HEAD_COARSE: the binarised one, dense; HEAD_FINE:
+// the soft one). stage: the tanh result [B,cout,H,W]. packed: HEAD_COARSE's blend in packed rows as pack8 writes them.
+struct HeadIO {
+  const void* x;
+  int B, H, W, mode;
+  const float *img, *blend;
+  long long blend_bs;
+  float* mask;                       // HEAD_MASK: sigmoid, with its binarised plane and bytes
+  long long mask_bs;
+  float* mask_bin;
+  unsigned char* mask_u8;
+  float *stage, *composed;           // HEAD_FINE: composed, with its BGR HWC bytes
+  long long composed_bs;
+  unsigned char* bgr_u8;
+  void* packed;
+  int Wp, padl, no_mask_coarse;
+};
+// w_host / b_host: host copies of the [9][12][cout] weights and the bias (the kernel parameters are built from them)
+int head(HeadIO io, int dt, const float* w_host, const float* b_host, int cout, cudaStream_t s);
 // fp32: NHWC with pixel pitch ld; bf16 / split-half: channel-blocked with ld blocks per image (max / avg only)
 int plane_reduce(const void* x, int dt, int B, int HW, int C, int ld, int mode, float* out, cudaStream_t s);
 // v [B][C] into channels [choff, choff + C) of every pixel: fp32 NHWC (pitch ld), else channel-blocked (ld blocks per image)
@@ -38,9 +52,9 @@ int softmax_rows(const float* S, int lds, float* P, int ldp, long long rows, int
 // fp32 [B][C][v.H][v.W] (nhwc: [B][v.H][v.W][C]) -> channels [0, C) of the activation y in layout v, and back
 int f32_to_act(const float* x, int nhwc, void* y, int dt, const Layout& v, int B, int C, cudaStream_t s);
 int act_to_f32(const void* x, int dt, const Layout& v, float* y, int nhwc, int B, int C, cudaStream_t s);
-// mask_u8 (optional, [B,H,W]): also writes its soft plane v/255 and its binarised plane (v/255 > 0.5) as fp32 [B,H,W]
-int u8_to_inputs(const unsigned char* img_u8, const unsigned char* sk_u8, float* img, float* sk, int B, int H, int W, cudaStream_t s,
-                 const unsigned char* mask_u8 = nullptr, float* mask_soft = nullptr, float* mask_bin = nullptr);
+// mask_u8: an edit mask's bytes [B,H,W] or null; decoded into its soft plane v/255 and binarised plane (v/255 > 0.5), fp32 [B,H,W]
+int u8_to_inputs(const unsigned char* img_u8, const unsigned char* sk_u8, const unsigned char* mask_u8, float* img, float* sk, float* mask_soft,
+                 float* mask_bin, int B, int H, int W, cudaStream_t s);
 // out[i] = m[i] > 0.5 ? 1 : 0 over n floats
 int binarise(const float* m, float* out, long long n, cudaStream_t s);
 int to_uint8(const float* comp, const float* mask, unsigned char* bgr, unsigned char* mk, int B, int H, int W, cudaStream_t s);

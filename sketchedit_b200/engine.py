@@ -32,11 +32,11 @@ def _chk_in(t, shape_tail=None, name="tensor"):
     return t.contiguous()
 
 
-def _chk_out(t, shape, name):
-    """Caller-owned output: the kernels write through its pointer, so a silent .contiguous() copy is not an option."""
-    if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
-        raise _lib.SketchEditB200Error("%s must be a contiguous CUDA float32 tensor" % name)
-    if tuple(t.shape) != tuple(shape):
+def _chk_out(t, shape, name, dtype=torch.float32):
+    """Caller-owned output or uint8 input (shape None: any): the kernels use its pointer, so .contiguous() is not an option."""
+    if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == dtype and t.is_contiguous()):
+        raise _lib.SketchEditB200Error("%s must be a contiguous CUDA %s tensor" % (name, str(dtype)[len("torch."):]))
+    if shape is not None and tuple(t.shape) != tuple(shape):
         raise _lib.SketchEditB200Error("%s must have shape %r (got %r)" % (name, tuple(shape), tuple(t.shape)))
     return t
 
@@ -115,21 +115,38 @@ class Engine:
         return e
 
     # -------------------------------------------------------------------------------- forward
+    def _forward_tensors(self, dtype, ins, outs, out=None, want=()):
+        """Checked (name, tensor) inputs, image first (fp32: made contiguous, an edit mask [B,1,H,W]; uint8: [B,H,W,3] then
+        [B,H,W]), the results of ``outs`` channels (the caller's ``out``, one tensor for one result, or new) and the ``want``
+        extras: (B, H, W, inputs, results, extras)."""
+        names = [n for n, _ in ins]
+        if dtype == torch.uint8:
+            ins = [_chk_out(t, None, n, torch.uint8) for n, t in ins]
+            B, H, W, C = ins[0].shape
+            if C != 3 or any(tuple(t.shape) != (B, H, W) for t in ins[1:]):
+                raise _lib.SketchEditB200Error(", ".join(["image_u8 must be [B,H,W,3]"] + names[1:-1]) + " and %s [B,H,W]" % names[-1])
+            shape = lambda c: (B, H, W, 3) if c == 3 else (B, H, W)
+        else:
+            ins = [_chk_in(t, name=n) for n, t in ins]
+            B, _, H, W = ins[0].shape
+            shape = lambda c: (B, c, H, W)
+            for n, t in zip(names[2:], ins[2:]):
+                _chk_out(t, shape(1), n)
+        one = len(outs) == 1
+        res = [torch.empty(shape(c), device=ins[0].device, dtype=dtype) if out is None else
+               _chk_out(out if one else out[i], shape(c), "out" if one else "out[%d]" % i, dtype) for i, c in enumerate(outs)]
+        extra = {k: _f32(B, 1 if k == "mask_bin" else 3, H, W, like=ins[0]) for k in want}
+        self._on_device(*ins, *res)
+        return B, H, W, ins, res, extra
+
     def inference(self, image, sketch, precision="bf16", want=(), mask_bin=None, out=None):
         """EditLine2Model.forward(mode='inference'): returns (composed, mask) and, in a dict, any of
         want = ('coarse', 'fine', 'mask_image', 'mask_bin'). ``out=(composed, mask)`` writes into caller-owned
         fp32 CUDA tensors of shape [B,3,H,W] / [B,1,H,W] instead of allocating (pipelined callers)."""
-        image = _chk_in(image, name="image")
-        sketch = _chk_in(sketch, name="sketch")
-        B, _, H, W = image.shape
-        new = lambda c: _f32(B, c, H, W, like=image)
-        if out is not None:
-            composed, mask = _chk_out(out[0], (B, 3, H, W), "out[0]"), _chk_out(out[1], (B, 1, H, W), "out[1]")
-        else:
-            composed, mask = new(3), new(1)
-        extra = {k: new(1 if k == "mask_bin" else 3) for k in want}
+        B, H, W, (image, sketch), (composed, mask), extra = self._forward_tensors(
+            torch.float32, (("image", image), ("sketch", sketch)), (3, 1), out, want)
         mb_in = _chk_in(mask_bin, name="mask_bin") if mask_bin is not None else None
-        self._on_device(image, sketch, composed, mask, mb_in)
+        self._on_device(mb_in)
         _lib.check(self.lib.se_forward_inference(
             self.h, _ptr(image), _ptr(sketch), B, H, W, _lib.PREC[precision], _ptr(composed), _ptr(mask),
             _ptr(extra.get("coarse")), _ptr(extra.get("fine")), _ptr(extra.get("mask_image")), _ptr(mb_in),
@@ -139,11 +156,7 @@ class Engine:
     def inference_packed(self, image, sketch, precision="bf16", out=None):
         """Same forward, ONE packed output [B,4,H,W] (channels 0-2 composed, channel 3 the soft mask) = the layout of the
         data-parallel output all-gather: ``out`` may be this rank's slice of the gather buffer (parallel.OutputGather)."""
-        image = _chk_in(image, name="image")
-        sketch = _chk_in(sketch, name="sketch")
-        B, _, H, W = image.shape
-        packed = _f32(B, 4, H, W, like=image) if out is None else _chk_out(out, (B, 4, H, W), "out")
-        self._on_device(image, sketch, packed)
+        B, H, W, (image, sketch), (packed,), _ = self._forward_tensors(torch.float32, (("image", image), ("sketch", sketch)), (4,), out)
         _lib.check(self.lib.se_forward_inference_packed(self.h, _ptr(image), _ptr(sketch), B, H, W, _lib.PREC[precision], _ptr(packed),
                                                         _stream()))
         return packed
@@ -152,21 +165,8 @@ class Engine:
         """Forward with the reference's host-side codecs on the device: image_u8 [B,H,W,3] RGB uint8 and sketch_u8 [B,H,W]
         uint8 (reference data/testimage_dataset.py:89-103 up to ToTensor) -> (bgr_u8 [B,H,W,3], mask_u8 [B,H,W]) exactly as
         test.py:25-35 writes them. ``out=(bgr, mask)`` writes into caller-owned uint8 CUDA tensors."""
-        for t, nm in ((image_u8, "image_u8"), (sketch_u8, "sketch_u8")):
-            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
-                raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % nm)
-        B, H, W, C = image_u8.shape
-        if C != 3 or tuple(sketch_u8.shape) != (B, H, W):
-            raise _lib.SketchEditB200Error("image_u8 must be [B,H,W,3] and sketch_u8 [B,H,W]")
-        if out is None:
-            bgr = torch.empty(B, H, W, 3, device=image_u8.device, dtype=torch.uint8)
-            mk = torch.empty(B, H, W, device=image_u8.device, dtype=torch.uint8)
-        else:
-            bgr, mk = out
-            for t, shp in ((bgr, (B, H, W, 3)), (mk, (B, H, W))):
-                if not (t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous() and tuple(t.shape) == shp):
-                    raise _lib.SketchEditB200Error("out tensors must be contiguous CUDA uint8 [B,H,W,3] and [B,H,W]")
-        self._on_device(image_u8, sketch_u8, bgr, mk)
+        B, H, W, (image_u8, sketch_u8), (bgr, mk), _ = self._forward_tensors(
+            torch.uint8, (("image_u8", image_u8), ("sketch_u8", sketch_u8)), (3, 1), out)
         _lib.check(self.lib.se_forward_inference_u8(self.h, _ptr(image_u8), _ptr(sketch_u8), B, H, W, _lib.PREC[precision], _ptr(bgr), _ptr(mk),
                                                     _stream()))
         return bgr, mk
@@ -176,15 +176,8 @@ class Engine:
         (edit_mask > 0.5) and composed = fine * edit_mask + image * (1 - edit_mask); values are used as given. Returns
         (composed, extra) with any of want = ('coarse', 'fine', 'mask_image', 'mask_bin') in the dict. netM runs only
         for 'mask_image'. Given the soft mask ``inference`` returned, every output equals that call's bit for bit."""
-        image = _chk_in(image, name="image")
-        sketch = _chk_in(sketch, name="sketch")
-        edit_mask = _chk_in(edit_mask, name="edit_mask")
-        B, _, H, W = image.shape
-        if tuple(edit_mask.shape) != (B, 1, H, W):
-            raise _lib.SketchEditB200Error("edit_mask must have shape %r (got %r)" % ((B, 1, H, W), tuple(edit_mask.shape)))
-        composed = _f32(B, 3, H, W, like=image)
-        extra = {k: _f32(B, 1 if k == "mask_bin" else 3, H, W, like=image) for k in want}
-        self._on_device(image, sketch, edit_mask)
+        B, H, W, (image, sketch, edit_mask), (composed,), extra = self._forward_tensors(
+            torch.float32, (("image", image), ("sketch", sketch), ("edit_mask", edit_mask)), (3,), None, want)
         _lib.check(self.lib.se_forward_with_mask(
             self.h, _ptr(image), _ptr(sketch), _ptr(edit_mask), B, H, W, _lib.PREC[precision], _ptr(composed),
             _ptr(extra.get("coarse")), _ptr(extra.get("fine")), _ptr(extra.get("mask_image")), _ptr(extra.get("mask_bin")),
@@ -194,32 +187,18 @@ class Engine:
     def inference_with_mask_u8(self, image_u8, sketch_u8, edit_mask_u8, precision="bf16", out=None):
         """``inference_u8`` on a caller-supplied edit mask: edit_mask_u8 [B,H,W] uint8 means v/255 (inpainted where
         v >= 128). Returns bgr_u8 [B,H,W,3]; ``out`` is a caller-owned contiguous CUDA uint8 tensor of that shape."""
-        for t, nm in ((image_u8, "image_u8"), (sketch_u8, "sketch_u8"), (edit_mask_u8, "edit_mask_u8")):
-            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
-                raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % nm)
-        B, H, W, C = image_u8.shape
-        if C != 3 or tuple(sketch_u8.shape) != (B, H, W) or tuple(edit_mask_u8.shape) != (B, H, W):
-            raise _lib.SketchEditB200Error("image_u8 must be [B,H,W,3], sketch_u8 and edit_mask_u8 [B,H,W]")
-        if out is None:
-            bgr = torch.empty(B, H, W, 3, device=image_u8.device, dtype=torch.uint8)
-        else:
-            bgr = out
-            if not (bgr.is_cuda and bgr.dtype == torch.uint8 and bgr.is_contiguous() and tuple(bgr.shape) == (B, H, W, 3)):
-                raise _lib.SketchEditB200Error("out must be a contiguous CUDA uint8 [B,H,W,3] tensor")
-        self._on_device(image_u8, sketch_u8, edit_mask_u8, bgr)
+        B, H, W, (image_u8, sketch_u8, edit_mask_u8), (bgr,), _ = self._forward_tensors(
+            torch.uint8, (("image_u8", image_u8), ("sketch_u8", sketch_u8), ("edit_mask_u8", edit_mask_u8)), (3,), out)
         _lib.check(self.lib.se_forward_with_mask_u8(self.h, _ptr(image_u8), _ptr(sketch_u8), _ptr(edit_mask_u8), B, H, W,
                                                     _lib.PREC[precision], _ptr(bgr), _stream()))
         return bgr
 
     def netM(self, x, guide, precision="bf16", want_image=True):
-        x, guide = _chk_in(x), _chk_in(guide)
-        B, _, H, W = x.shape
-        self._on_device(x, guide)
-        mask1 = _f32(B, 1, H, W, like=x)
-        st1 = _f32(B, 3, H, W, like=x) if want_image else None
-        _lib.check(self.lib.se_netM_forward(self.h, _ptr(x), _ptr(guide), B, H, W, _lib.PREC[precision], _ptr(mask1), _ptr(st1),
-                                            _stream()))
-        return mask1, st1
+        B, H, W, (x, guide), (mask1,), ex = self._forward_tensors(torch.float32, (("tensor", x), ("tensor", guide)), (1,), None,
+                                                                  ("x_stage1",) if want_image else ())
+        _lib.check(self.lib.se_netM_forward(self.h, _ptr(x), _ptr(guide), B, H, W, _lib.PREC[precision], _ptr(mask1),
+                                            _ptr(ex.get("x_stage1")), _stream()))
+        return mask1, ex.get("x_stage1")
 
     def netG(self, x, x2, mask, mask2, guide, precision="bf16"):
         x, x2, mask, mask2 = _chk_in(x), _chk_in(x2), _chk_in(mask), _chk_in(mask2)
