@@ -148,6 +148,21 @@ int se_outputs_to_uint8(const float* composed, const float* mask, int B, int H, 
  * synchronous copy); later calls only enqueue the kernels on `stream`. */
 int se_resize_u8(const unsigned char* src, const long long* src_off, const int* src_hw, unsigned char* dst, const long long* dst_off,
                  const int* dst_hw, int n, int channels, int swap_rb, void* scratch, long long* scratch_bytes, void* stream);
+/* Resize back and paste, bit for bit as Pillow does it, for a batch of n <= 32 images of their own sizes (a region edit: the
+ * forward's result on a crop of the photo, pasted back into the crop):
+ *     res = Image.fromarray(rgb_i).resize((w, h));  m = Image.fromarray(mask_i).resize((w, h));  base_i.paste(res, (0, 0), m)
+ * Image i's result is the src_hw[2i] x src_hw[2i+1] x 3 bytes at rgb + rgb_off[i] and its mask the src_hw[2i] x src_hw[2i+1]
+ * bytes at mask + mask_off[i]; both are resized to h x w = dst_hw[2i] x dst_hw[2i+1] (each rounded to uint8, as se_resize_u8
+ * writes them) and blended per channel over the h x w x 3 bytes at base + base_off[i]:
+ * dst = DIV255(base * (255 - m) + res * m) with DIV255(a) = (((a + 128) >> 8) + a + 128) >> 8, Pillow's paste blend. The
+ * h x w x 3 output goes to dst + dst_off[i]; dst may be base (in place), but neither may overlap rgb or mask. swap_rb reverses
+ * the result's channel order first (the forward writes BGR). Sizes, the scratch query (scratch == NULL stores the bytes needed
+ * in *scratch_bytes; scratch holds the intermediates of images whose width changes) and the coefficient-table cache are those
+ * of se_resize_u8. */
+int se_resize_paste_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask, const long long* mask_off,
+                       const int* src_hw, const unsigned char* base, const long long* base_off, unsigned char* dst,
+                       const long long* dst_off, const int* dst_hw, int n, int swap_rb, void* scratch, long long* scratch_bytes,
+                       void* stream);
 /* Bytes of coefficient tables se_resize_u8 keeps per device (process-wide; 0 restores the default of 256 MiB; negative is an
  * error). When a call's new tables would pass the limit, the device's cache is emptied (after a device synchronise) before the
  * call looks up any table; one call's own tables may exceed it. */

@@ -331,6 +331,68 @@ def resize_u8_packed(src, src_offsets, src_sizes, dst_sizes, channels, swap_rb=F
     return out, dst_offsets
 
 
+def resize_paste_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, base, base_offsets, dst_sizes, swap_rb=False, out=None,
+                           dst_offsets=None):
+    """Resize back and paste (``se_resize_paste_u8``), bit for bit as Pillow does it, for a batch of packed uint8 images:
+
+        res = Image.fromarray(rgb_i).resize((w, h)); m = Image.fromarray(mask_i).resize((w, h)); base_i.paste(res, (0, 0), m)
+
+    Image i's result [h',w',3] is at byte ``rgb_offsets[i]`` of ``rgb`` and its mask [h',w'] at ``mask_offsets[i]`` of ``mask``,
+    with ``src_sizes[i] = (h', w')``; both are resized to ``dst_sizes[i] = (h, w)`` and the result is blended over the [h,w,3]
+    bytes at ``base_offsets[i]`` of ``base``. ``swap_rb`` reverses the result's channel order first (the forward writes BGR).
+    The pasted image goes to ``dst_offsets[i]`` of ``out``, which may be ``base`` with ``dst_offsets == base_offsets`` (in
+    place); without ``out`` it is packed into a new tensor at 16-byte aligned offsets. All tensors are contiguous CUDA uint8 on
+    one device. Returns ``(out, dst_offsets)``. Only enqueues work on the current stream, except that the first resize between
+    a pair of lengths uploads its coefficient table."""
+    n = len(src_sizes)
+    if not (len(rgb_offsets) == len(mask_offsets) == len(base_offsets) == len(dst_sizes) == n):
+        raise _lib.SketchEditB200Error("rgb_offsets, mask_offsets, src_sizes, base_offsets and dst_sizes must have the same length")
+    for t, nm in ((rgb, "rgb"), (mask, "mask"), (base, "base"), (out, "out")):
+        if t is not None and not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
+            raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % nm)
+    src_sizes = [(int(h), int(w)) for h, w in src_sizes]
+    dst_sizes = [(int(h), int(w)) for h, w in dst_sizes]
+    if out is None:
+        if dst_offsets is not None:
+            raise _lib.SketchEditB200Error("dst_offsets needs out")
+        dst_offsets, total = [], 0
+        for h, w in dst_sizes:
+            dst_offsets.append(total)
+            total += (h * w * 3 + 15) // 16 * 16
+        out = torch.empty(max(total, 1), device=rgb.device, dtype=torch.uint8)
+    elif dst_offsets is None or len(dst_offsets) != n:
+        raise _lib.SketchEditB200Error("out needs one dst_offsets entry per image")
+    for t, nm in ((mask, "mask"), (base, "base"), (out, "out")):
+        if t.device != rgb.device:
+            raise _lib.SketchEditB200Error("rgb on %s but %s on %s" % (rgb.device, nm, t.device))
+    dst_offsets = [int(o) for o in dst_offsets]
+    for buf, offs, sizes, c, nm in ((rgb, rgb_offsets, src_sizes, 3, "rgb"), (mask, mask_offsets, src_sizes, 1, "mask"),
+                                    (base, base_offsets, dst_sizes, 3, "base"), (out, dst_offsets, dst_sizes, 3, "out")):
+        for o, (h, w) in zip(offs, sizes):
+            if o < 0 or o + h * w * c > buf.numel():
+                raise _lib.SketchEditB200Error("%s slice [%d, %d) outside the %d-byte buffer" % (nm, o, o + h * w * c, buf.numel()))
+    lib = _lib.load()
+    L, I = ctypes.c_longlong, ctypes.c_int
+    with torch.cuda.device(rgb.device):
+        chunks = []
+        for c0 in range(0, n, RESIZE_MAX_BATCH):
+            sl = slice(c0, c0 + RESIZE_MAX_BATCH)
+            k = len(src_sizes[sl])
+            offs = lambda v: (L * k)(*[int(o) for o in v[sl]])
+            args = (offs(rgb_offsets), offs(mask_offsets), (I * (2 * k))(*[v for hw in src_sizes[sl] for v in hw]), offs(base_offsets),
+                    offs(dst_offsets), (I * (2 * k))(*[v for hw in dst_sizes[sl] for v in hw]), k)
+            need = L(0)
+            _lib.check(lib.se_resize_paste_u8(None, args[0], None, args[1], args[2], None, args[3], None, args[4], args[5], k,
+                                              int(bool(swap_rb)), None, ctypes.byref(need), None))
+            chunks.append((args, need.value))
+        scratch = torch.empty(max([1] + [b for _, b in chunks]), device=rgb.device, dtype=torch.uint8)
+        for a, _ in chunks:
+            size = L(scratch.numel())
+            _lib.check(lib.se_resize_paste_u8(_ptr(rgb), a[0], _ptr(mask), a[1], a[2], _ptr(base), a[3], _ptr(out), a[4], a[5], a[6],
+                                              int(bool(swap_rb)), _ptr(scratch), ctypes.byref(size), _stream()))
+    return out, dst_offsets
+
+
 def set_resize_table_cache_limit(nbytes):
     """Bytes of coefficient tables the resize keeps per device (process-wide; 0 = the default of 256 MiB). Past the limit the
     device's tables are dropped, after a device synchronise, before the next call that needs a new one."""
