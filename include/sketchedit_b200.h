@@ -163,6 +163,21 @@ int se_resize_paste_u8(const unsigned char* rgb, const long long* rgb_off, const
                        const int* src_hw, const unsigned char* base, const long long* base_off, unsigned char* dst,
                        const long long* dst_off, const int* dst_hw, int n, int swap_rb, void* scratch, long long* scratch_bytes,
                        void* stream);
+/* Resize back and paste n >= 0 boxes in order into canvases, bit for bit as sequential Pillow pastes (a region edit with
+ * several boxes whose boxes may overlap, nest or repeat):
+ *     for i in 0 .. n-1:  res = Image.fromarray(rgb_i).resize((w, h));  m = Image.fromarray(mask_i).resize((w, h));
+ *                         canvas_i.paste(res, (x, y), m)
+ * Box i's result and mask are read as in se_resize_paste_u8 (src_hw[2i] x src_hw[2i+1], at rgb + rgb_off[i] and mask +
+ * mask_off[i]) and resized to h x w = dst_hw[2i] x dst_hw[2i+1]; its canvas is the image whose row 0 starts at canvas +
+ * canvas_off[i], canvas_pitch[i] bytes per row (>= 3 (x + w)), and (y, x) = (box_yx[2i], box_yx[2i+1]) is the box's top-left
+ * pixel in it. Boxes with the same canvas_off share a canvas and must give the same pitch; different canvases must not
+ * overlap in memory, and no canvas may overlap rgb or mask. A later box blends over what an earlier one wrote. Only the pixels
+ * of the boxes are read and written. swap_rb, the size limits, the scratch query and the coefficient-table cache are those of
+ * se_resize_paste_u8 (box i needs the scratch image i of se_resize_paste_u8 needs). */
+int se_resize_composite_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask, const long long* mask_off,
+                           const int* src_hw, unsigned char* canvas, const long long* canvas_off, const long long* canvas_pitch,
+                           const int* box_yx, const int* dst_hw, int n, int swap_rb, void* scratch, long long* scratch_bytes,
+                           void* stream);
 /* Bytes of coefficient tables se_resize_u8 keeps per device (process-wide; 0 restores the default of 256 MiB; negative is an
  * error). When a call's new tables would pass the limit, the device's cache is emptied (after a device synchronise) before the
  * call looks up any table; one call's own tables may exceed it. */

@@ -8,7 +8,9 @@
 // built here on the host in the same order, so the integer weights and therefore every output byte are Pillow's.
 // Pillow computes only the intermediate rows the vertical pass reads; computing all of them gives the same values.
 // se_resize_paste_u8 resizes a result and its mask the same way and pastes the result over a base image with Pillow's
-// Image.paste(im, box, mask) blend, fused into the vertical pass (paste_v_kernel).
+// Image.paste(im, box, mask) blend, fused into the vertical pass (paste_v_kernel); se_resize_composite_u8 pastes boxes that
+// may overlap into shared canvases in order, as sequential Image.paste calls do, with the same kernel.
+#include <limits.h>
 #include <math.h>
 #include <string.h>
 
@@ -169,8 +171,8 @@ __device__ __forceinline__ int clip8(int acc) {
   return v < 0 ? 0 : (v > 255 ? 255 : v);
 }
 
-template <typename P>
-__device__ __forceinline__ int find_image(const PassList<P>& L) {
+template <typename List>
+__device__ __forceinline__ int find_image(const List& L) {
   int i = 0;
   while (i + 1 < L.n && (int)blockIdx.x >= L.p[i + 1].tile0) ++i;
   return i;
@@ -220,10 +222,11 @@ __device__ __forceinline__ void stage_v_taps(int* sk, int* sb, const int* bounds
   for (int j = tid; j < 2 * nrow; j += V_TX * V_TY) sb[j] = bounds ? bounds[2 * y0 + j] : ((j & 1) ? 1 : y0 + j / 2);
 }
 
-// v[j] = clip8(2^21 + sum_x s[x * stride + j] * k[x]) for the first nb of NB bytes: 32-bit loads when vec (then nb == NB and
-// s, stride are 4-byte aligned), byte loads otherwise
+// v[j] = clip8(2^21 + sum_x s[x * stride + j] * k[x]) for the bytes lo <= j < nb of NB: 32-bit loads when vec (then lo == 0,
+// nb == NB and s, stride are 4-byte aligned), byte loads otherwise
 template <int NB>
-__device__ __forceinline__ void v_taps(const unsigned char* s, int stride, const int* k, int n, int nb, bool vec, int (&v)[NB]) {
+__device__ __forceinline__ void v_taps(const unsigned char* s, int stride, const int* k, int n, int lo, int nb, bool vec,
+                                       int (&v)[NB]) {
 #pragma unroll
   for (int j = 0; j < NB; ++j) v[j] = 1 << (RESIZE_PREC_BITS - 1);
   if (vec) {
@@ -242,7 +245,7 @@ __device__ __forceinline__ void v_taps(const unsigned char* s, int stride, const
       const int w = k[x];
 #pragma unroll
       for (int j = 0; j < NB; ++j)
-        if (j < nb) v[j] += (int)r[j] * w;
+        if (j >= lo && j < nb) v[j] += (int)r[j] * w;
     }
   }
 #pragma unroll
@@ -287,66 +290,109 @@ __global__ void __launch_bounds__(V_TX * V_TY) resize_v_kernel(const __grid_cons
   const int nb = min(V_GROUP, d.row_bytes - (int)p);
   const bool vec = d.vec && nb == V_GROUP;
   int v[V_GROUP];
-  v_taps(d.src + (size_t)ymin * d.row_bytes + p, d.row_bytes, sk + threadIdx.y * d.ksize, n, nb, vec, v);
+  v_taps(d.src + (size_t)ymin * d.row_bytes + p, d.row_bytes, sk + threadIdx.y * d.ksize, n, 0, nb, vec, v);
   if (d.swap) swap_rb12(v);
   store12(d.dst + (size_t)(y0 + threadIdx.y) * d.row_bytes + p, v, nb, vec);
 }
 
-// The paste of se_resize_paste_u8: the vertical pass of a result (3 channels) and of its mask, both in_h x out_w, to out_h,
-// then Pillow's Image.paste blend of the result over base with that mask, per channel:
+// The paste of se_resize_paste_u8 and se_resize_composite_u8: boxes pasted in order into canvases (row pitch in bytes). For a
+// box, the vertical pass of its result (3 channels) and of its mask, both in_h x out_w, to out_h, then Pillow's Image.paste
+// blend of the result over the canvas with that mask, per channel:
 //     dst = DIV255(base * (255 - m) + res * m),   DIV255(a) = ((t >> 8) + t) >> 8 with t = a + 128 (libImaging/Paste.c).
-// A thread owns 4 pixels of one output row: 12 result, 4 mask, 12 base and 12 dst bytes. It reads its base bytes before it
-// writes the same dst bytes, so dst may be base.
-struct PPass {
+// A thread owns 4 pixels of one canvas row (x a multiple of 4). It reads the canvas bytes that some box of the launch covers,
+// blends every covering box over them in the launch's order and writes them once; uncovered bytes are never touched. It reads
+// before it writes the same bytes, so dst may be base. The 12 canvas bytes move as 32-bit words when every box that covers
+// one of the 4 pixels covers all 4 and the canvas rows are 4-byte aligned, and a box's result and mask rows likewise.
+struct PBox {   // a box at (oy, ox) of its canvas; rgb and mask are in_h x out_w (after the horizontal passes)
   const unsigned char* rgb;
   const unsigned char* mask;
+  const int* bounds;   // the vertical table; nullptr: the height does not change (one tap of weight 1 at the same row)
+  const int* coeffs;
+  int ksize, out_h, out_w, oy, ox, vec;
+};
+struct PCanvas {   // boxes box0 .. box0 + nbox - 1 of the launch, in order; tiles cover rows y0 .. y0 + h - 1 from column x0
   const unsigned char* base;
   unsigned char* dst;
-  const int* bounds;
-  const int* coeffs;
-  int ksize, in_h, out_h, out_w, groups, swap, vec, tile0, tiles_x;
+  long long pitch;
+  int y0, x0, h, groups, vec, box0, nbox, tile0, tiles_x;
 };
+struct PasteList {
+  PBox b[RESIZE_MAX_BATCH];
+  PCanvas p[RESIZE_MAX_BATCH];
+  int n;   // canvases
+};
+static_assert(sizeof(PasteList) <= 4096, "paste descriptors must fit the kernel parameter space");
 constexpr int P_PIX = V_GROUP / 3;
+static __device__ int g_unit_tap[1] = {1 << RESIZE_PREC_BITS};
 
-__global__ void __launch_bounds__(V_TX * V_TY) paste_v_kernel(const __grid_constant__ PassList<PPass> L) {
-  extern __shared__ int smem[];   // coeffs [V_TY][ksize], bounds [V_TY][2]
-  const PPass& d = L.p[find_image(L)];
+// the pixels [lo, hi) of the 4 at canvas (y, x) that box b covers (lo >= hi: none)
+__device__ __forceinline__ void box_span(const PBox& b, int y, int x, int& lo, int& hi) {
+  const bool row = y >= b.oy && y < b.oy + b.out_h;
+  lo = max(b.ox - x, 0);
+  hi = row ? min(b.ox + b.out_w - x, P_PIX) : 0;
+}
+
+__global__ void __launch_bounds__(V_TX * V_TY) paste_v_kernel(const __grid_constant__ PasteList L, int swap) {
+  const PCanvas& d = L.p[find_image(L)];
   const int t = blockIdx.x - d.tile0;
-  const int g = (t % d.tiles_x) * V_TX + threadIdx.x, y0 = (t / d.tiles_x) * V_TY;
-  const int nrow = min(V_TY, d.out_h - y0);
-  int* sk = smem;
-  int* sb = smem + V_TY * d.ksize;
-  stage_v_taps(sk, sb, d.bounds, d.coeffs, d.ksize, y0, nrow);
-  __syncthreads();
-  if ((int)threadIdx.y >= nrow || g >= d.groups) return;
-  const int ymin = sb[2 * threadIdx.y], n = sb[2 * threadIdx.y + 1];
-  const int* k = sk + threadIdx.y * d.ksize;
-  const int x0 = g * P_PIX, np = min(P_PIX, d.out_w - x0);
-  const bool vec = d.vec && np == P_PIX;
-  int c[V_GROUP], m[P_PIX];
-  v_taps(d.rgb + ((size_t)ymin * d.out_w + x0) * 3, d.out_w * 3, k, n, np * 3, vec, c);
-  v_taps(d.mask + (size_t)ymin * d.out_w + x0, d.out_w, k, n, np, vec, m);
-  if (d.swap) swap_rb12(c);
-  const size_t o = ((size_t)(y0 + threadIdx.y) * d.out_w + x0) * 3;
-  int b[V_GROUP];
+  const int g = (t % d.tiles_x) * V_TX + threadIdx.x, y = d.y0 + (t / d.tiles_x) * V_TY + threadIdx.y;
+  if (g >= d.groups || y >= d.y0 + d.h) return;
+  const int x = d.x0 + g * P_PIX;
+  unsigned covered = 0;   // bit p: some box covers pixel x + p
+  bool same = true;
+  for (int i = d.box0; i < d.box0 + d.nbox; ++i) {
+    int lo, hi;
+    box_span(L.b[i], y, x, lo, hi);
+    if (lo >= hi) continue;
+    covered |= (1u << hi) - (1u << lo);
+    same = same && lo == 0 && hi == P_PIX;
+  }
+  if (!covered) return;
+  const bool vec = d.vec && same;
+  const size_t at = (size_t)y * d.pitch + (size_t)x * 3;
+  const unsigned char* ob = d.base + at;
+  int c[V_GROUP];
   if (vec) {   // plain loads: base may be dst
-    const uint32_t* q = reinterpret_cast<const uint32_t*>(d.base + o);
+    const uint32_t* q = reinterpret_cast<const uint32_t*>(ob);
 #pragma unroll
     for (int w = 0; w < 3; ++w) {
       const uint32_t u = q[w];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) b[4 * w + j] = (int)((u >> (8 * j)) & 0xffu);
+      for (int j = 0; j < 4; ++j) c[4 * w + j] = (int)((u >> (8 * j)) & 0xffu);
     }
   } else {
 #pragma unroll
-    for (int j = 0; j < V_GROUP; ++j) b[j] = j < np * 3 ? (int)d.base[o + j] : 0;
+    for (int j = 0; j < V_GROUP; ++j) c[j] = (covered >> (j / 3)) & 1u ? (int)ob[j] : 0;
   }
+  for (int i = d.box0; i < d.box0 + d.nbox; ++i) {
+    const PBox& b = L.b[i];
+    int lo, hi;
+    box_span(b, y, x, lo, hi);
+    if (lo >= hi) continue;
+    const int r = y - b.oy;
+    const int ymin = b.bounds ? __ldg(b.bounds + 2 * r) : r, n = b.bounds ? __ldg(b.bounds + 2 * r + 1) : 1;
+    const int* k = b.bounds ? b.coeffs + (size_t)r * b.ksize : g_unit_tap;
+    const bool bv = b.vec && lo == 0 && hi == P_PIX;
+    const ptrdiff_t col = (ptrdiff_t)ymin * b.out_w + (x - b.ox);   // pixel 0 of the thread in the box's rows (may be < 0)
+    int v[V_GROUP], m[P_PIX];
+    v_taps(b.rgb + col * 3, b.out_w * 3, k, n, lo * 3, hi * 3, bv, v);
+    v_taps(b.mask + col, b.out_w, k, n, lo, hi, bv, m);
+    if (swap) swap_rb12(v);
 #pragma unroll
-  for (int j = 0; j < V_GROUP; ++j) {
-    const int a = b[j] * (255 - m[j / 3]) + c[j] * m[j / 3] + 128;
-    c[j] = ((a >> 8) + a) >> 8;
+    for (int j = 0; j < V_GROUP; ++j) {
+      if (j / 3 < lo || j / 3 >= hi) continue;
+      const int a = c[j] * (255 - m[j / 3]) + v[j] * m[j / 3] + 128;
+      c[j] = ((a >> 8) + a) >> 8;
+    }
   }
-  store12(d.dst + o, c, np * 3, vec);
+  unsigned char* o = d.dst + at;
+  if (vec) {
+    store12(o, c, V_GROUP, true);
+  } else {
+#pragma unroll
+    for (int j = 0; j < V_GROUP; ++j)
+      if ((covered >> (j / 3)) & 1u) o[j] = (unsigned char)c[j];
+  }
 }
 
 static int cdiv_i(long long a, long long b) { return (int)((a + b - 1) / b); }
@@ -409,6 +455,115 @@ static int v_table(int dev, int ih, int oh, const int** bounds, const int** coef
   *bounds = t->bounds;
   *coeffs = t->coeffs;
   *ksize = t->ksize;
+  return 0;
+}
+
+// One box of se_resize_paste_u8 / se_resize_composite_u8: its result and mask (ih x iw), pasted at ow x oh into canvas
+// `canvas` at (oy, ox).
+struct PasteBox {
+  const unsigned char* rgb;
+  const unsigned char* mask;
+  int ih, iw, oh, ow, canvas, oy, ox;
+};
+struct PasteCanvas {
+  const unsigned char* base;
+  unsigned char* dst;
+  long long pitch;
+};
+
+// bytes of scratch box i needs (a width change: the result's and the mask's intermediates, ih x ow x 3 and ih x ow)
+static size_t paste_scratch(int ih, int iw, int ow) {
+  return iw != ow ? scratch_round((size_t)ih * ow * 3) + scratch_round((size_t)ih * ow) : 0;
+}
+
+// The boxes in order, RESIZE_MAX_BATCH per launch: the horizontal passes of a launch's boxes, then one paste_v_kernel in
+// which each canvas's boxes keep their order; a later launch on the same stream continues the order. mid[i]: box i's scratch.
+static int paste_boxes(const std::vector<PasteBox>& boxes, const std::vector<PasteCanvas>& canvases, const std::vector<size_t>& mid,
+                       void* scratch, int swap_rb, cudaStream_t st) {
+  std::lock_guard<std::mutex> lk(g_resize_mu);
+  int dev = 0;
+  SE_CUDA_OK(cudaGetDevice(&dev));
+  {
+    std::vector<std::pair<int, int>> pairs;
+    for (auto& b : boxes) {
+      if (b.iw != b.ow) pairs.emplace_back(b.iw, b.ow);
+      if (b.ih != b.oh) pairs.emplace_back(b.ih, b.oh);
+    }
+    int rc = reserve_tables(dev, pairs);
+    if (rc) return rc;
+  }
+  const int n = (int)boxes.size();
+  for (int c0 = 0; c0 < n; c0 += RESIZE_MAX_BATCH) {
+    const int c1 = std::min(n, c0 + RESIZE_MAX_BATCH);
+    PassList<HPass> h3, h1;
+    PasteList pl;
+    memset(&h3, 0, sizeof(h3));
+    memset(&h1, 0, sizeof(h1));
+    memset(&pl, 0, sizeof(pl));
+    long long t3 = 0, t1 = 0, ptiles = 0;
+    int k3 = 1, k1 = 1;
+    std::vector<int> order;   // the launch's boxes grouped by canvas (canvases in order of first appearance), in order
+    for (int i = c0; i < c1; ++i) {
+      if (std::find_if(order.begin(), order.end(), [&](int j) { return boxes[j].canvas == boxes[i].canvas; }) != order.end()) continue;
+      for (int j = i; j < c1; ++j)
+        if (boxes[j].canvas == boxes[i].canvas) order.push_back(j);
+    }
+    for (int j = 0; j < (int)order.size(); ++j) {
+      const PasteBox& b = boxes[order[j]];
+      PBox& p = pl.b[j];
+      p.rgb = b.rgb;
+      p.mask = b.mask;
+      if (b.iw != b.ow) {   // the paste reads the horizontal passes' output instead of the result itself
+        unsigned char* s3 = (unsigned char*)scratch + mid[order[j]];
+        unsigned char* s1 = s3 + scratch_round((size_t)b.ih * b.ow * 3);
+        int rc = add_h_pass(dev, h3, t3, k3, b.rgb, s3, b.ih, b.iw, b.ow, 0);
+        if (rc) return rc;
+        rc = add_h_pass(dev, h1, t1, k1, b.mask, s1, b.ih, b.iw, b.ow, 0);
+        if (rc) return rc;
+        p.rgb = s3;
+        p.mask = s1;
+      }
+      int rc = v_table(dev, b.ih, b.oh, &p.bounds, &p.coeffs, &p.ksize);
+      if (rc) return rc;
+      p.out_h = b.oh;
+      p.out_w = b.ow;
+      p.oy = b.oy;
+      p.ox = b.ox;
+      p.vec = b.ow % 4 == 0 && b.ox % 4 == 0 && ((uintptr_t)p.rgb | (uintptr_t)p.mask) % 4 == 0;
+      if (j == 0 || boxes[order[j - 1]].canvas != b.canvas) {
+        const PasteCanvas& cv = canvases[b.canvas];
+        PCanvas& c = pl.p[pl.n++];
+        c.base = cv.base;
+        c.dst = cv.dst;
+        c.pitch = cv.pitch;
+        c.vec = cv.pitch % 4 == 0 && ((uintptr_t)cv.base | (uintptr_t)cv.dst) % 4 == 0;
+        c.box0 = j;
+        c.y0 = c.x0 = INT_MAX;
+        c.h = c.groups = 0;   // (y1, x1) until the canvas's last box
+      }
+      PCanvas& c = pl.p[pl.n - 1];
+      ++c.nbox;
+      c.y0 = std::min(c.y0, b.oy);
+      c.x0 = std::min(c.x0, b.ox / P_PIX * P_PIX);
+      c.h = std::max(c.h, b.oy + b.oh);
+      c.groups = std::max(c.groups, b.ox + b.ow);
+    }
+    for (int i = 0; i < pl.n; ++i) {
+      PCanvas& c = pl.p[i];
+      c.h -= c.y0;
+      c.groups = cdiv_i(c.groups - c.x0, P_PIX);
+      c.tile0 = (int)ptiles;
+      c.tiles_x = cdiv_i(c.groups, V_TX);
+      ptiles += (long long)c.tiles_x * cdiv_i(c.h, V_TY);
+    }
+    SE_REQUIRE(t3 < (1LL << 31) && ptiles < (1LL << 31), "batch too large for one launch");
+    int rc = launch_h<3>(h3, t3, k3, st);
+    if (rc) return rc;
+    rc = launch_h<1>(h1, t1, k1, st);
+    if (rc) return rc;
+    paste_v_kernel<<<(unsigned)ptiles, dim3(V_TX, V_TY), 0, st>>>(pl, swap_rb);
+    SE_CUDA_OK(cudaGetLastError());
+  }
   return 0;
 }
 
@@ -544,8 +699,8 @@ int se_resize_paste_u8(const unsigned char* rgb, const long long* rgb_off, const
     int rc = check_image(i, ih, iw, oh, ow);
     if (rc) return rc;
     SE_REQUIRE(rgb_off[i] >= 0 && mask_off[i] >= 0 && base_off[i] >= 0 && dst_off[i] >= 0, "negative offset");
-    mid[i] = need;   // a width change: the result's and the mask's intermediates, ih x ow x 3 and ih x ow
-    if (iw != ow) need += scratch_round((size_t)ih * ow * 3) + scratch_round((size_t)ih * ow);
+    mid[i] = need;
+    need += paste_scratch(ih, iw, ow);
   }
   if (!scratch) {
     *scratch_bytes = (long long)need;
@@ -554,65 +709,50 @@ int se_resize_paste_u8(const unsigned char* rgb, const long long* rgb_off, const
   SE_REQUIRE((size_t)*scratch_bytes >= need, "scratch holds " + std::to_string(*scratch_bytes) + " bytes, needs " + std::to_string(need));
   if (n == 0) return 0;
   SE_REQUIRE(rgb && mask && base && dst, "null rgb / mask / base / dst");
-  cudaStream_t st = (cudaStream_t)stream;
-  std::lock_guard<std::mutex> lk(g_resize_mu);
-  int dev = 0;
-  SE_CUDA_OK(cudaGetDevice(&dev));
-  {
-    std::vector<std::pair<int, int>> pairs;
-    for (int i = 0; i < n; ++i) {
-      if (src_hw[2 * i + 1] != dst_hw[2 * i + 1]) pairs.emplace_back(src_hw[2 * i + 1], dst_hw[2 * i + 1]);
-      if (src_hw[2 * i] != dst_hw[2 * i]) pairs.emplace_back(src_hw[2 * i], dst_hw[2 * i]);
-    }
-    int rc = reserve_tables(dev, pairs);
-    if (rc) return rc;
+  std::vector<PasteBox> boxes(n);   // image i: one box filling canvas i
+  std::vector<PasteCanvas> canvases(n);
+  for (int i = 0; i < n; ++i) {
+    boxes[i] = {rgb + rgb_off[i], mask + mask_off[i], src_hw[2 * i], src_hw[2 * i + 1], dst_hw[2 * i], dst_hw[2 * i + 1], i, 0, 0};
+    canvases[i] = {base + base_off[i], dst + dst_off[i], 3LL * dst_hw[2 * i + 1]};
   }
-  PassList<HPass> h3, h1;
-  PassList<PPass> pl;
-  memset(&h3, 0, sizeof(h3));
-  memset(&h1, 0, sizeof(h1));
-  memset(&pl, 0, sizeof(pl));
-  long long t3 = 0, t1 = 0, ptiles = 0;
-  int k3 = 1, k1 = 1, pk = 1;
+  return paste_boxes(boxes, canvases, mid, scratch, swap_rb, (cudaStream_t)stream);
+}
+
+int se_resize_composite_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask, const long long* mask_off,
+                           const int* src_hw, unsigned char* canvas, const long long* canvas_off, const long long* canvas_pitch,
+                           const int* box_yx, const int* dst_hw, int n, int swap_rb, void* scratch, long long* scratch_bytes,
+                           void* stream) {
+  SE_REQUIRE(n >= 0, "n must be >= 0 boxes");
+  SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
+  SE_REQUIRE(n == 0 || (rgb_off && mask_off && src_hw && canvas_off && canvas_pitch && box_yx && dst_hw), "null size / offset array");
+  size_t need = 0;
+  std::vector<size_t> mid(n);
+  std::map<long long, int> canvas_of;   // canvas offset -> canvas index
+  std::vector<PasteCanvas> canvases;
+  std::vector<PasteBox> boxes(n);
   for (int i = 0; i < n; ++i) {
     const int ih = src_hw[2 * i], iw = src_hw[2 * i + 1], oh = dst_hw[2 * i], ow = dst_hw[2 * i + 1];
-    PPass& p = pl.p[pl.n++];
-    p.rgb = rgb + rgb_off[i];
-    p.mask = mask + mask_off[i];
-    if (iw != ow) {   // the paste reads the horizontal passes' output instead of the result itself
-      unsigned char* s3 = (unsigned char*)scratch + mid[i];
-      unsigned char* s1 = s3 + scratch_round((size_t)ih * ow * 3);
-      int rc = add_h_pass(dev, h3, t3, k3, p.rgb, s3, ih, iw, ow, 0);
-      if (rc) return rc;
-      rc = add_h_pass(dev, h1, t1, k1, p.mask, s1, ih, iw, ow, 0);
-      if (rc) return rc;
-      p.rgb = s3;
-      p.mask = s1;
-    }
-    p.base = base + base_off[i];
-    p.dst = dst + dst_off[i];
-    int rc = v_table(dev, ih, oh, &p.bounds, &p.coeffs, &p.ksize);
+    int rc = check_image(i, ih, iw, oh, ow);
     if (rc) return rc;
-    p.in_h = ih;
-    p.out_h = oh;
-    p.out_w = ow;
-    p.groups = cdiv_i(ow, P_PIX);
-    p.swap = swap_rb;
-    p.vec = ow % 4 == 0 && ((uintptr_t)p.rgb | (uintptr_t)p.mask | (uintptr_t)p.base | (uintptr_t)p.dst) % 4 == 0;
-    p.tile0 = (int)ptiles;
-    p.tiles_x = cdiv_i(p.groups, V_TX);
-    ptiles += (long long)p.tiles_x * cdiv_i(oh, V_TY);
-    pk = std::max(pk, p.ksize);
+    SE_REQUIRE(rgb_off[i] >= 0 && mask_off[i] >= 0 && canvas_off[i] >= 0 && box_yx[2 * i] >= 0 && box_yx[2 * i + 1] >= 0,
+               "negative offset");
+    SE_REQUIRE(canvas_pitch[i] >= 3LL * (box_yx[2 * i + 1] + ow),
+               "box " + std::to_string(i) + ": the canvas pitch of " + std::to_string(canvas_pitch[i]) + " bytes is narrower than the box");
+    auto it = canvas_of.emplace(canvas_off[i], (int)canvases.size()).first;
+    if (it->second == (int)canvases.size()) canvases.push_back({canvas + canvas_off[i], canvas + canvas_off[i], canvas_pitch[i]});
+    SE_REQUIRE(canvases[it->second].pitch == canvas_pitch[i], "box " + std::to_string(i) + ": boxes of one canvas must have one pitch");
+    boxes[i] = {rgb + rgb_off[i], mask + mask_off[i], ih, iw, oh, ow, it->second, box_yx[2 * i], box_yx[2 * i + 1]};
+    mid[i] = need;
+    need += paste_scratch(ih, iw, ow);
   }
-  SE_REQUIRE(t3 < (1LL << 31) && ptiles < (1LL << 31), "batch too large for one launch");
-  int rc = launch_h<3>(h3, t3, k3, st);
-  if (rc) return rc;
-  rc = launch_h<1>(h1, t1, k1, st);
-  if (rc) return rc;
-  SE_CUDA_OK(cudaFuncSetAttribute(paste_v_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
-  paste_v_kernel<<<(unsigned)ptiles, dim3(V_TX, V_TY), (V_TY * pk + 2 * V_TY) * 4, st>>>(pl);
-  SE_CUDA_OK(cudaGetLastError());
-  return 0;
+  if (!scratch) {
+    *scratch_bytes = (long long)need;
+    return 0;
+  }
+  SE_REQUIRE((size_t)*scratch_bytes >= need, "scratch holds " + std::to_string(*scratch_bytes) + " bytes, needs " + std::to_string(need));
+  if (n == 0) return 0;
+  SE_REQUIRE(rgb && mask && canvas, "null rgb / mask / canvas");
+  return paste_boxes(boxes, canvases, mid, scratch, swap_rb, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -393,6 +393,60 @@ def resize_paste_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, base
     return out, dst_offsets
 
 
+def resize_composite_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, canvas, canvas_offsets, canvas_pitches,
+                               box_offsets, box_sizes, swap_rb=False):
+    """Resize back and paste boxes in order into canvases (``se_resize_composite_u8``), bit for bit as sequential Pillow
+    pastes, in place:
+
+        for each box i in order:  canvas_i.paste(Image.fromarray(rgb_i).resize((w, h)), (x, y), Image.fromarray(mask_i).resize((w, h)))
+
+    Box i's result [h',w',3] and mask [h',w'] are read as in ``resize_paste_u8_packed`` (``src_sizes[i] = (h', w')``). Its
+    canvas starts at byte ``canvas_offsets[i]`` of ``canvas`` with ``canvas_pitches[i]`` bytes per row; ``box_offsets[i] =
+    (y, x)`` is its top-left pixel there and ``box_sizes[i] = (h, w)`` its size. Boxes with the same canvas offset share
+    that canvas, so a later box blends over an earlier one where they overlap. ``swap_rb`` reverses the result's channel
+    order first. All tensors are contiguous CUDA uint8 on one device; only the boxes' canvas pixels are read and written.
+    Returns ``canvas``. Only enqueues work on the current stream, except that the first resize between a pair of lengths
+    uploads its coefficient table."""
+    n = len(src_sizes)
+    if not (len(rgb_offsets) == len(mask_offsets) == len(canvas_offsets) == len(canvas_pitches) == len(box_offsets)
+            == len(box_sizes) == n):
+        raise _lib.SketchEditB200Error("rgb_offsets, mask_offsets, src_sizes, canvas_offsets, canvas_pitches, box_offsets and "
+                                       "box_sizes must have the same length")
+    for t, nm in ((rgb, "rgb"), (mask, "mask"), (canvas, "canvas")):
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
+            raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % nm)
+    for t, nm in ((mask, "mask"), (canvas, "canvas")):
+        if t.device != rgb.device:
+            raise _lib.SketchEditB200Error("rgb on %s but %s on %s" % (rgb.device, nm, t.device))
+    src_sizes = [(int(h), int(w)) for h, w in src_sizes]
+    box_sizes = [(int(h), int(w)) for h, w in box_sizes]
+    box_offsets = [(int(y), int(x)) for y, x in box_offsets]
+    canvas_offsets, canvas_pitches = [int(o) for o in canvas_offsets], [int(p) for p in canvas_pitches]
+    for buf, offs, c, nm in ((rgb, rgb_offsets, 3, "rgb"), (mask, mask_offsets, 1, "mask")):
+        for o, (h, w) in zip(offs, src_sizes):
+            if o < 0 or o + h * w * c > buf.numel():
+                raise _lib.SketchEditB200Error("%s slice [%d, %d) outside the %d-byte buffer" % (nm, o, o + h * w * c, buf.numel()))
+    for o, p, (y, x), (h, w) in zip(canvas_offsets, canvas_pitches, box_offsets, box_sizes):
+        end = o + (y + h - 1) * p + (x + w) * 3
+        if o < 0 or y < 0 or x < 0 or p < (x + w) * 3 or end > canvas.numel():
+            raise _lib.SketchEditB200Error("box (%d, %d) of %dx%d in the canvas at %d (pitch %d) is outside the %d-byte canvas"
+                                           % (y, x, h, w, o, p, canvas.numel()))
+    lib = _lib.load()
+    L, I = ctypes.c_longlong, ctypes.c_int
+    pairs = lambda v: (I * (2 * n))(*[a for hw in v for a in hw])
+    args = ((L * n)(*[int(o) for o in rgb_offsets]), (L * n)(*[int(o) for o in mask_offsets]), pairs(src_sizes),
+            (L * n)(*canvas_offsets), (L * n)(*canvas_pitches), pairs(box_offsets), pairs(box_sizes), n)
+    with torch.cuda.device(rgb.device):
+        need = L(0)
+        _lib.check(lib.se_resize_composite_u8(None, args[0], None, args[1], args[2], None, args[3], args[4], args[5], args[6], n,
+                                              int(bool(swap_rb)), None, ctypes.byref(need), None))
+        scratch = torch.empty(max(1, need.value), device=rgb.device, dtype=torch.uint8)
+        size = L(scratch.numel())
+        _lib.check(lib.se_resize_composite_u8(_ptr(rgb), args[0], _ptr(mask), args[1], args[2], _ptr(canvas), args[3], args[4],
+                                              args[5], args[6], n, int(bool(swap_rb)), _ptr(scratch), ctypes.byref(size), _stream()))
+    return canvas
+
+
 def set_resize_table_cache_limit(nbytes):
     """Bytes of coefficient tables the resize keeps per device (process-wide; 0 = the default of 256 MiB). Past the limit the
     device's tables are dropped, after a device synchronise, before the next call that needs a new one."""

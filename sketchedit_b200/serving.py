@@ -12,11 +12,12 @@ too (``engine.resize_u8_packed``, bit-identical to Pillow), so a batch is one up
     result_pil, mask = proc.process_image(image_pil, mask_pil, return_mask=True)       # ... and the predicted edit mask
     result_pil = proc.process_image(image_pil, mask_pil, edit_mask=corrected_mask)      # run on a revised edit mask
     result_pil = proc.process_image(image_pil, mask_pil, region="auto")                 # edit a crop around the strokes only
+    result_pil = proc.process_image(image_pil, mask_pil, region="strokes")              # one crop per group of strokes
     proc.close()
 
 A region edit (``region=``) crops a box of the photo, runs the forward on it at ``DemoProcessor(region_size=...)`` and pastes
 the result back with the edit mask: its cost follows the box, not the photo, and region requests on photos of any size
-batch together.
+batch together. A request may carry several boxes (``region="strokes"`` or a list), pasted in order.
 
 Everything except the forward itself (``run_batch``) is plain host logic and is unit-tested on the CPU with a fake forward.
 """
@@ -147,13 +148,132 @@ def region_box(bbox, photo_size, region_size):
     return x, y, x + bw, y + bh
 
 
+GROUP_CELL = 8     # region_groups connects strokes on a grid of 8x8-pixel cells
+
+
+def _intersects(a, b):
+    return a[0] < b[2] and b[0] < a[2] and a[1] < b[3] and b[1] < a[3]
+
+
+def region_groups(mask, edit_mask=None, region_size=(256, 256)):
+    """The stroke groups of a region edit with ``region="strokes"``: a list of ``(bbox, box)`` PIL boxes, one per group,
+    ordered by the (upper, left) corner of ``bbox``. ``mask`` and ``edit_mask`` are PIL images of the photo's size.
+
+    1. The non-zero pixels of ``mask`` and ``edit_mask`` are connected (8-neighbourhood) on a grid of 8x8-pixel cells; a cell is
+       set when any of its pixels is. ``bbox`` is the exact pixel bounding box of a group's non-zero pixels.
+    2. Two groups merge while one's ``bbox`` intersects the other's ``region_box``; the merged ``bbox`` is the union.
+    3. ``box = region_box(bbox, mask.size, region_size)``.
+    So every box holds its own group's strokes and no other group's: ``mask.crop(box)`` is that group's sketch alone. Boxes
+    may still overlap, in stroke-free margins. One group gives the box of ``region="auto"``. No stroke is a ValueError."""
+    w, h = mask.size
+    if edit_mask is not None and edit_mask.size != mask.size:
+        raise ValueError("edit_mask is %dx%d, mask %dx%d: they must have one size" % (edit_mask.size + mask.size))
+    c = GROUP_CELL
+    ims = [m if m.mode == "L" else m.convert("L") for m in (mask, edit_mask) if m is not None]
+    bbs = [b for b in (m.getbbox() for m in ims) if b]
+    if not bbs:
+        raise ValueError("region='strokes' needs a sketch stroke or a non-zero edit mask")
+    # only the cells of the union bbox are examined, from a cell corner of the photo's grid
+    ox, oy = min(b[0] for b in bbs) // c * c, min(b[1] for b in bbs) // c * c
+    crop = (ox, oy, max(b[2] for b in bbs), max(b[3] for b in bbs))
+    ch, cw = crop[3] - oy, crop[2] - ox
+    H8, W8 = -(-ch // c), -(-cw // c)
+    pad = np.zeros((H8 * c, W8 * c), np.uint8)
+    for m in ims:
+        np.maximum(pad[:ch, :cw], np.asarray(m.crop(crop)), out=pad[:ch, :cw])
+    blocks = pad.reshape(H8, c, W8, c)
+    cells = (pad.view(np.uint64).reshape(H8, c, W8) != 0).any(axis=1)     # a cell row's 8 pixels as one word: exact
+    # runs of set cells per cell row, joined by union-find with the overlapping (8-neighbour) runs of the row above
+    d = np.diff(np.pad(cells.astype(np.int8), ((0, 0), (1, 1))), axis=1)
+    starts, ends = np.nonzero(d == 1), np.nonzero(d == -1)[1]   # both in row-major order: run k is [s, e) of row r
+    run_r, run_s, run_e = starts[0], starts[1], ends
+    parent = list(range(len(run_r)))
+
+    def find(a):
+        while parent[a] != a:
+            parent[a] = parent[parent[a]]
+            a = parent[a]
+        return a
+
+    row_first = np.searchsorted(run_r, np.arange(H8 + 1))
+    for r in range(1, H8):
+        i, i1 = row_first[r - 1], row_first[r]
+        for k in range(row_first[r], row_first[r + 1]):
+            while i < i1 and run_e[i] < run_s[k]:                  # runs above that end before this one's diagonal neighbour
+                i += 1
+            j = i
+            while j < i1 and run_s[j] <= run_e[k]:
+                a, b = find(j), find(k)
+                if a != b:
+                    parent[b] = a
+                j += 1
+    roots = np.array([find(k) for k in range(len(run_r))])
+    label = np.full((H8, W8), -1, np.int64)
+    for k in range(len(run_r)):
+        label[run_r[k], run_s[k]:run_e[k]] = roots[k]
+    cy, cx = np.nonzero(cells)
+    lab = label[cy, cx]
+    # exact pixel bounds of each set cell, then their extremes per group
+    px = blocks[cy, :, cx, :] != 0                                # [cells, c, c]
+    rows, cols = px.any(axis=2), px.any(axis=1)
+    y0 = oy + cy * c + rows.argmax(axis=1)
+    y1 = oy + cy * c + c - rows[:, ::-1].argmax(axis=1)
+    x0 = ox + cx * c + cols.argmax(axis=1)
+    x1 = ox + cx * c + c - cols[:, ::-1].argmax(axis=1)
+    ids, inv = np.unique(lab, return_inverse=True)
+    bb = np.empty((len(ids), 4), np.int64)
+    bb[:, :2] = np.iinfo(np.int64).max
+    bb[:, 2:] = -1
+    np.minimum.at(bb[:, 0], inv, x0)
+    np.minimum.at(bb[:, 1], inv, y0)
+    np.maximum.at(bb[:, 2], inv, x1)
+    np.maximum.at(bb[:, 3], inv, y1)
+    groups = [tuple(int(v) for v in b) for b in bb]
+    boxes = [region_box(g, (w, h), region_size) for g in groups]
+    merged = True
+    while merged:
+        merged = False
+        for i in range(len(groups)):
+            for j in range(i + 1, len(groups)):
+                if _intersects(groups[j], boxes[i]) or _intersects(groups[i], boxes[j]):
+                    a, b = groups[i], groups.pop(j)
+                    groups[i] = (min(a[0], b[0]), min(a[1], b[1]), max(a[2], b[2]), max(a[3], b[3]))
+                    boxes.pop(j)
+                    boxes[i] = region_box(groups[i], (w, h), region_size)
+                    merged = True
+                    break
+            if merged:
+                break
+    return sorted(zip(groups, boxes), key=lambda gb: (gb[0][1], gb[0][0]))
+
+
 def _check_box(box, w, h):
     if not (isinstance(box, (tuple, list)) and len(box) == 4 and all(isinstance(v, (int, np.integer)) for v in box)):
-        raise ValueError("region must be None, 'auto' or a PIL box (left, upper, right, lower) of integers, got %r" % (box,))
+        raise ValueError("region must be None, 'auto', 'strokes', a PIL box (left, upper, right, lower) of integers or a list of "
+                         "such boxes, got %r" % (box,))
     left, upper, right, lower = (int(v) for v in box)
     if not (0 <= left < right <= w and 0 <= upper < lower <= h):
         raise ValueError("region %r must satisfy 0 <= left < right <= %d and 0 <= upper < lower <= %d" % (tuple(box), w, h))
     return left, upper, right, lower
+
+
+def _overlap_sets(boxes):
+    """Indices of the boxes, split into connected sets of boxes that overlap (each set in box order)."""
+    parent = list(range(len(boxes)))
+
+    def find(a):
+        while parent[a] != a:
+            a = parent[a]
+        return a
+
+    for i in range(len(boxes)):
+        for j in range(i):
+            if _intersects(boxes[i], boxes[j]):
+                parent[find(i)] = find(j)
+    sets = {}
+    for i in range(len(boxes)):
+        sets.setdefault(find(i), []).append(i)
+    return list(sets.values())
 
 
 def _aligned_offsets(nbytes, align=16):
@@ -263,73 +383,113 @@ class DemoProcessor:
         return [(r, masks_back.get(i)) for i, r in enumerate(results)]
 
     def _run_region_device(self, key, payloads):
-        """payloads: (photo crop [bh,bw,3], sketch crop [bh,bw], edit-mask crop [bh,bw] or None, return_mask) at their box sizes;
-        key: ("region", Hn, Wn), plus True when the batch runs on edit masks. Returns (patch [bh,bw,3]: the crop with the result
-        pasted in, the paste mask resized back to the box [bh,bw] when asked for and predicted, else None)."""
+        """payloads: (photo crops [bh,bw,3], sketch crops [bh,bw], edit-mask crops [bh,bw] or None, return_mask, boxes): one crop
+        per PIL box of the request, at its box size; key: ("region", Hn, Wn), plus True when the batch runs on edit masks.
+        Returns per request one (patch, mask) per box: patch [bh,bw,3] is the box's bytes once all of the request's boxes are
+        pasted in order, mask the box's paste mask resized back to [bh,bw] when asked for and predicted, else None."""
         torch = self._torch
-        from .engine import resize_paste_u8_packed, resize_u8_packed
+        from .engine import resize_composite_u8_packed, resize_u8_packed
         H, W = key[1:3]
         edit = key[-1] is True
-        B = len(payloads)
         dev = self.engine.device
-        photos, masks = [p[0] for p in payloads], [p[1] for p in payloads]
-        edits = [p[2] for p in payloads] if edit else []
+        photos, masks = [a for p in payloads for a in p[0]], [a for p in payloads for a in p[1]]   # one item per box
+        edits = [a for p in payloads for a in p[2]] if edit else []
+        boxes = [b for p in payloads for b in p[4]]
+        B = len(photos)
         sizes = [a.shape[:2] for a in photos]
-        back = [i for i, p in enumerate(payloads) if p[3] and not edit]   # predicted masks to resize back and download
+        back = [i for i, r in enumerate(p[3] for p in payloads for _ in p[0]) if r and not edit]   # predicted masks to return
         offs, total = _aligned_offsets([a.nbytes for a in photos + masks + edits])
-        # the patches are pasted in place over the uploaded photo crops, which come first; a predicted mask is resized back into
-        # the slot of its sketch crop. One download covers both.
-        n_down = offs[B + back[-1]] + masks[back[-1]].nbytes if back else offs[B - 1] + photos[-1].nbytes
+        # A box that overlaps no other box of its request is pasted in place over its uploaded photo crop (the first B slots).
+        # A set of overlapping boxes is pasted into a canvas, their bounding rectangle, assembled after the uploads from the
+        # crops; its boxes are then copied back into their crop slots. A predicted mask is resized back into the slot of its
+        # sketch crop. One download covers both.
+        canvas = {}                                   # item -> (canvas offset, pitch, y, x) for boxes in a set of several
+        canvas_end, first = total, 0
+        for p in payloads:
+            rb = p[4]
+            for s in _overlap_sets(rb):
+                if len(s) < 2:
+                    continue
+                L, U = min(rb[i][0] for i in s), min(rb[i][1] for i in s)
+                R, D = max(rb[i][2] for i in s), max(rb[i][3] for i in s)
+                for i in s:
+                    canvas[first + i] = (canvas_end, (R - L) * 3, rb[i][1] - U, rb[i][0] - L)
+                canvas_end += ((D - U) * (R - L) * 3 + 15) // 16 * 16
+            first += len(rb)
+        n_down = max([offs[i] + photos[i].nbytes for i in range(B)] + [offs[B + i] + masks[i].nbytes for i in back])
         stage = self._staging("in", total)          # free: every batch, failed ones included, ends with a stream synchronise
         host = stage.numpy()
         for a, o in zip(photos + masks + edits, offs):
             host[o:o + a.nbytes] = a.reshape(-1)
         down = self._staging("out", n_down)
         net3, net1 = [i * H * W * 3 for i in range(B)], [i * H * W for i in range(B)]
+
+        def in_canvas(work, i):                       # item i's box in its canvas, and its crop slot, as [bh,bw,3] views
+            co, pitch, y, x = canvas[i]
+            bh, bw = sizes[i]
+            rows = work[co:co + (y + bh) * pitch].view(y + bh, pitch)
+            return rows[y:, x * 3:(x + bw) * 3].view(bh, bw, 3), work[offs[i]:offs[i] + photos[i].nbytes].view(bh, bw, 3)
+
         with torch.cuda.device(dev):
             try:
-                src = stage[:total].to(dev, non_blocking=True)
+                work = torch.empty(canvas_end, device=dev, dtype=torch.uint8)
+                work[:total].copy_(stage[:total], non_blocking=True)
+                for i in canvas:                      # 2-D copies; overlapping crops hold the same photo bytes
+                    dst, crop = in_canvas(work, i)
+                    dst.copy_(crop)
                 img = torch.empty(B, H, W, 3, device=dev, dtype=torch.uint8)
                 msk = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
-                resize_u8_packed(src, offs[:B], sizes, [(H, W)] * B, 3, out=img, dst_offsets=net3)
-                resize_u8_packed(src, offs[B:2 * B], sizes, [(H, W)] * B, 1, out=msk, dst_offsets=net1)
+                resize_u8_packed(work, offs[:B], sizes, [(H, W)] * B, 3, out=img, dst_offsets=net3)
+                resize_u8_packed(work, offs[B:2 * B], sizes, [(H, W)] * B, 1, out=msk, dst_offsets=net1)
                 with torch.no_grad():
                     if edit:
                         pm = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
-                        resize_u8_packed(src, offs[2 * B:], sizes, [(H, W)] * B, 1, out=pm, dst_offsets=net1)
+                        resize_u8_packed(work, offs[2 * B:], sizes, [(H, W)] * B, 1, out=pm, dst_offsets=net1)
                         bgr = self.engine.inference_with_mask_u8(img, msk, pm, precision=self.precision)
                     else:
                         bgr, pm = self.engine.inference_u8(img, msk, precision=self.precision)
-                resize_paste_u8_packed(bgr, net3, pm, net1, [(H, W)] * B, src, offs[:B], sizes, swap_rb=True, out=src,
-                                       dst_offsets=offs[:B])
+                place = [canvas.get(i, (offs[i], sizes[i][1] * 3, 0, 0)) for i in range(B)]
+                resize_composite_u8_packed(bgr, net3, pm, net1, [(H, W)] * B, work, [c[0] for c in place], [c[1] for c in place],
+                                           [c[2:] for c in place], sizes, swap_rb=True)
+                for i in canvas:
+                    src, crop = in_canvas(work, i)
+                    crop.copy_(src)
                 if back:
-                    resize_u8_packed(pm, [net1[i] for i in back], [(H, W)] * len(back), [sizes[i] for i in back], 1, out=src,
+                    resize_u8_packed(pm, [net1[i] for i in back], [(H, W)] * len(back), [sizes[i] for i in back], 1, out=work,
                                      dst_offsets=[offs[B + i] for i in back])
-                down[:n_down].copy_(src[:n_down], non_blocking=True)
+                down[:n_down].copy_(work[:n_down], non_blocking=True)
             finally:
                 torch.cuda.current_stream().synchronize()
         host = down.numpy()
-        out = []
+        items = []
         for i, (a, o) in enumerate(zip(photos, offs)):
             m = host[offs[B + i]:offs[B + i] + masks[i].nbytes].reshape(sizes[i]).copy() if i in back else None
-            out.append((host[o:o + a.nbytes].reshape(a.shape).copy(), m))
-        return out
+            items.append((host[o:o + a.nbytes].reshape(a.shape).copy(), m))
+        ends = np.cumsum([len(p[4]) for p in payloads])
+        return [items[e - len(p[4]):e] for e, p in zip(ends, payloads)]
 
     def _run_batch(self, key, payloads):
         """payloads: (photo [H,W,3], mask [H,W], edit mask [H,W] or None, return_mask) at the network size of ``key`` (the
-        floored size, or a region's working size); True as the key's last element: the batch runs on edit masks."""
+        floored size), or for a region key (photos [k,H,W,3], masks [k,H,W], edit masks [k,H,W] or None, return_mask) with one
+        item per box at the working size, and then each result is (rgb [k,H,W,3], mask [k,H,W] or None); True as the key's
+        last element: the batch runs on edit masks."""
         torch = self._torch
-        img = torch.from_numpy(np.stack([p[0] for p in payloads])).cuda(non_blocking=True)     # [B,H,W,3] RGB uint8
-        msk = torch.from_numpy(np.stack([p[1] for p in payloads])).cuda(non_blocking=True)     # [B,H,W] uint8 (> 0 = stroke)
+        join = np.concatenate if key[0] == "region" else np.stack
+        img = torch.from_numpy(join([p[0] for p in payloads])).cuda(non_blocking=True)         # [B,H,W,3] RGB uint8
+        msk = torch.from_numpy(join([p[1] for p in payloads])).cuda(non_blocking=True)         # [B,H,W] uint8 (> 0 = stroke)
         mk = None
         with torch.no_grad():
             if key[-1] is True:
-                edt = torch.from_numpy(np.stack([p[2] for p in payloads])).cuda(non_blocking=True)
+                edt = torch.from_numpy(join([p[2] for p in payloads])).cuda(non_blocking=True)
                 bgr = self.engine.inference_with_mask_u8(img, msk, edt, precision=self.precision)
             else:
                 bgr, mk = self.engine.inference_u8(img, msk, precision=self.precision)
         rgb = bgr.cpu().numpy()[..., ::-1]                                                     # demo.py keeps RGB (test.py swaps to BGR)
         mk = mk.cpu().numpy() if mk is not None else None
+        if key[0] == "region":
+            ends = np.cumsum([len(p[0]) for p in payloads])
+            return [(np.ascontiguousarray(rgb[e - len(p[0]):e]), mk[e - len(p[0]):e] if mk is not None and p[3] else None)
+                    for e, p in zip(ends, payloads)]
         return [(np.ascontiguousarray(rgb[i]), mk[i] if mk is not None and p[3] else None) for i, p in enumerate(payloads)]
 
     def process_image(self, img, mask, edit_mask=None, return_mask=False, region=None):
@@ -346,7 +506,12 @@ class DemoProcessor:
         to ``region_size``, edited, resized back and pasted with the edit mask (predicted or given) resized back to the box,
         exactly as Pillow's ``out = img.copy(); out.paste(res, box, m)``. Pixels outside the box are the photo's own; strokes
         outside it are ignored. mask and edit_mask must then have the photo's size. Region requests on photos of any size
-        share forwards. With return_mask=True a predicted mask comes back at the photo's size, zero outside the box."""
+        share forwards. With return_mask=True a predicted mask comes back at the photo's size, zero outside the box.
+
+        A list of PIL boxes, or 'strokes' for one box per stroke group (``region_groups``), edits several regions in one
+        forward. Every crop is taken from the photo itself and the results are pasted in the list's order, exactly as
+        ``out = img.copy()`` followed by the single-box paste of each box into ``out``; a later box blends over an earlier one
+        where they overlap. The returned predicted mask is then the largest of the boxes' paste masks at each pixel."""
         from PIL import Image
         img = img.convert("RGB")
         if region is not None:
@@ -377,6 +542,24 @@ class DemoProcessor:
             return res
         return res, (edit_mask if edit_mask is not None else mk)
 
+    def _region_boxes(self, img, mask, edit_mask, region):
+        w, h = img.size
+        if isinstance(region, str):
+            if region == "strokes":
+                return [box for _, box in region_groups(mask, edit_mask, self.region_size)]
+            if region != "auto":
+                raise ValueError("region must be None, 'auto', 'strokes', a PIL box or a list of PIL boxes, got %r" % region)
+            bbs = [b for b in (mask.getbbox(), edit_mask.getbbox() if edit_mask is not None else None) if b]
+            if not bbs:
+                raise ValueError("region='auto' needs a sketch stroke or a non-zero edit mask")
+            return [region_box((min(b[0] for b in bbs), min(b[1] for b in bbs), max(b[2] for b in bbs), max(b[3] for b in bbs)),
+                               img.size, self.region_size)]
+        if isinstance(region, list) and not region:
+            raise ValueError("region=[] is empty: give at least one PIL box")
+        if isinstance(region, (list, tuple)) and all(isinstance(b, (list, tuple)) for b in region):   # a list of boxes
+            return [_check_box(b, w, h) for b in region]
+        return [_check_box(region, w, h)]
+
     def _process_region(self, img, mask, edit_mask, return_mask, region):
         from PIL import Image
         w, h = img.size
@@ -385,38 +568,35 @@ class DemoProcessor:
                 raise ValueError("a region edit needs the %s at the photo's size %dx%d (got %dx%d)" % ((nm, w, h) + m.size))
             if self.resize == "device" and m is not None and m.mode != "L":
                 raise ValueError("resize='device' takes an 'L' %s (got mode %r); resize='host' resizes it with Pillow" % (nm, m.mode))
-        if isinstance(region, str):
-            if region != "auto":
-                raise ValueError("region must be None, 'auto' or a PIL box, got %r" % region)
-            bbs = [b for b in (mask.getbbox(), edit_mask.getbbox() if edit_mask is not None else None) if b]
-            if not bbs:
-                raise ValueError("region='auto' needs a sketch stroke or a non-zero edit mask")
-            box = region_box((min(b[0] for b in bbs), min(b[1] for b in bbs), max(b[2] for b in bbs), max(b[3] for b in bbs)),
-                             img.size, self.region_size)
-        else:
-            box = _check_box(region, w, h)
+        boxes = self._region_boxes(img, mask, edit_mask, region)
         Hn, Wn = self.region_size
-        box_size = (box[2] - box[0], box[3] - box[1])
+        sizes = [(b[2] - b[0], b[3] - b[1]) for b in boxes]
         # region requests on edit masks run their own forward, and region requests never share one with whole-photo requests
         key = ("region", Hn, Wn) if edit_mask is None else ("region", Hn, Wn, True)
         out = img.copy()
         if self.resize == "device":
-            edit_raw = np.asarray(edit_mask.crop(box)) if edit_mask is not None else None
-            patch, mk = self.batcher.submit(key, (np.asarray(img.crop(box)), np.asarray(mask.crop(box)), edit_raw, return_mask))
-            out.paste(Image.fromarray(patch), box[:2])
-            mk = Image.fromarray(mk) if mk is not None else None
+            crops = [np.asarray(img.crop(b)) for b in boxes]
+            sketches = [np.asarray(mask.crop(b)) for b in boxes]
+            edits = [np.asarray(edit_mask.crop(b)) for b in boxes] if edit_mask is not None else None
+            got = self.batcher.submit(key, (crops, sketches, edits, return_mask, boxes))
+            for b, (patch, _) in zip(boxes, got):        # in order: a later patch holds the final bytes where boxes overlap
+                out.paste(Image.fromarray(patch), b[:2])
+            mks = [Image.fromarray(mk) if mk is not None else None for _, mk in got]
         else:
-            img_t = np.ascontiguousarray(np.array(img.crop(box).resize((Wn, Hn))), dtype=np.uint8)
-            mask_t = np.ascontiguousarray((np.array(mask.crop(box).resize((Wn, Hn))) > 0).astype(np.uint8) * 255)
-            edit_t = np.ascontiguousarray(np.array(edit_mask.convert("L").crop(box).resize((Wn, Hn))), dtype=np.uint8) \
+            img_t = np.stack([np.array(img.crop(b).resize((Wn, Hn))) for b in boxes]).astype(np.uint8)
+            mask_t = np.stack([(np.array(mask.crop(b).resize((Wn, Hn))) > 0).astype(np.uint8) * 255 for b in boxes])
+            edit_t = np.stack([np.array(edit_mask.convert("L").crop(b).resize((Wn, Hn))) for b in boxes]).astype(np.uint8) \
                 if edit_mask is not None else None
             res, mk = self.batcher.submit(key, (img_t, mask_t, edit_t, True))
-            mk = Image.fromarray(edit_t if edit_t is not None else mk).resize(box_size)
-            out.paste(Image.fromarray(res).resize(box_size), box, mk)
+            mks = [Image.fromarray(edit_t[i] if edit_t is not None else mk[i]).resize(s) for i, s in enumerate(sizes)]
+            for i, (b, s) in enumerate(zip(boxes, sizes)):   # every crop above came from the photo, not from `out`
+                out.paste(Image.fromarray(res[i]).resize(s), b, mks[i])
         if not return_mask:
             return out
         if edit_mask is not None:
             return out, edit_mask
-        full = Image.new("L", img.size, 0)
-        full.paste(mk, box[:2])
-        return out, full
+        full = np.zeros((h, w), np.uint8)            # the largest paste mask over the boxes, 0 outside every box
+        for b, mk in zip(boxes, mks):
+            sub = full[b[1]:b[3], b[0]:b[2]]
+            np.maximum(sub, np.asarray(mk), out=sub)
+        return out, Image.fromarray(full)
