@@ -148,6 +148,14 @@ int se_outputs_to_uint8(const float* composed, const float* mask, int B, int H, 
  * synchronous copy); later calls only enqueue the kernels on `stream`. */
 int se_resize_u8(const unsigned char* src, const long long* src_off, const int* src_hw, unsigned char* dst, const long long* dst_off,
                  const int* dst_hw, int n, int channels, int swap_rb, void* scratch, long long* scratch_bytes, void* stream);
+/* se_resize_u8 of windows of larger images: image i is src_hw[2i] rows of src_hw[2i+1] pixels, its row r at
+ * src[i] + r * src_pitch[i] (bytes, >= src_hw[2i+1] * channels). src is a host array of n device pointers. With src[i] at the
+ * top-left pixel of a box of an h x w x C image and src_pitch[i] = w * C, image i is Image.crop(box).resize(size), bit for bit.
+ * Windows may overlap each other; dst must not overlap any window. dst_off, dst_hw, the limits, the scratch query (src may be
+ * NULL in it) and the coefficient-table cache are those of se_resize_u8. */
+int se_resize_window_u8(const unsigned char* const* src, const long long* src_pitch, const int* src_hw, unsigned char* dst,
+                        const long long* dst_off, const int* dst_hw, int n, int channels, int swap_rb, void* scratch,
+                        long long* scratch_bytes, void* stream);
 /* Resize back and paste, bit for bit as Pillow does it, for a batch of n <= 32 images of their own sizes (a region edit: the
  * forward's result on a crop of the photo, pasted back into the crop):
  *     res = Image.fromarray(rgb_i).resize((w, h));  m = Image.fromarray(mask_i).resize((w, h));  base_i.paste(res, (0, 0), m)

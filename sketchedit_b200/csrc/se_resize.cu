@@ -9,7 +9,9 @@
 // Pillow computes only the intermediate rows the vertical pass reads; computing all of them gives the same values.
 // se_resize_paste_u8 resizes a result and its mask the same way and pastes the result over a base image with Pillow's
 // Image.paste(im, box, mask) blend, fused into the vertical pass (paste_v_kernel); se_resize_composite_u8 pastes boxes that
-// may overlap into shared canvases in order, as sequential Image.paste calls do, with the same kernel.
+// may overlap into shared canvases in order, as sequential Image.paste calls do, with the same kernel. se_resize_window_u8
+// resizes windows of larger images (rows a pitch apart, such as boxes of a photo kept on the device) with the kernels of
+// se_resize_u8: Image.crop(box).resize(size) without the crop.
 #include <limits.h>
 #include <math.h>
 #include <string.h>
@@ -142,18 +144,21 @@ static int axis_table(int dev, int in, int out, const AxisTable** t) {
 // ------------------------------------------------------------------------------------------ kernels
 // Per-image descriptors travel as kernel parameters (RESIZE_MAX_BATCH of them, < 4 KB). A launch covers the tiles of all its
 // images; tile0 is the first tile of an image, so a block finds its image by scanning the (at most 32) descriptors.
-struct HPass {   // rows x in_w -> rows x out_w
+struct HPass {   // rows x in_w -> rows x out_w; source rows src_pitch bytes apart, destination rows packed
   const unsigned char* src;
   unsigned char* dst;
   const int* bounds;
   const int* coeffs;
+  long long src_pitch;
   int ksize, rows, in_w, out_w, swap, tile0, tiles_x;
 };
-struct VPass {   // in_h x row_bytes -> out_h x row_bytes; coeffs == nullptr: copy (one tap of weight 1 at the same row)
+struct VPass {   // in_h x row_bytes -> out_h x row_bytes; source rows src_pitch bytes apart, destination rows packed;
+                 // coeffs == nullptr: copy (one tap of weight 1 at the same row)
   const unsigned char* src;
   unsigned char* dst;
   const int* bounds;
   const int* coeffs;
+  long long src_pitch;
   int ksize, in_h, out_h, row_bytes, groups, swap, vec, tile0, tiles_x;
 };
 template <typename P>
@@ -194,7 +199,7 @@ __global__ void __launch_bounds__(H_TX * H_TY) resize_h_kernel(const __grid_cons
   if ((int)threadIdx.x >= ncol || y >= d.rows) return;
   const int xmin = sb[2 * threadIdx.x], n = sb[2 * threadIdx.x + 1];
   const int* k = sk + threadIdx.x * d.ksize;   // ksize is odd: the 32 lanes hit 32 different banks
-  const unsigned char* s = d.src + ((size_t)y * d.in_w + xmin) * C;
+  const unsigned char* s = d.src + (size_t)y * d.src_pitch + (size_t)xmin * C;
   int acc[C];
 #pragma unroll
   for (int c = 0; c < C; ++c) acc[c] = 1 << (RESIZE_PREC_BITS - 1);
@@ -225,7 +230,7 @@ __device__ __forceinline__ void stage_v_taps(int* sk, int* sb, const int* bounds
 // v[j] = clip8(2^21 + sum_x s[x * stride + j] * k[x]) for the bytes lo <= j < nb of NB: 32-bit loads when vec (then lo == 0,
 // nb == NB and s, stride are 4-byte aligned), byte loads otherwise
 template <int NB>
-__device__ __forceinline__ void v_taps(const unsigned char* s, int stride, const int* k, int n, int lo, int nb, bool vec,
+__device__ __forceinline__ void v_taps(const unsigned char* s, long long stride, const int* k, int n, int lo, int nb, bool vec,
                                        int (&v)[NB]) {
 #pragma unroll
   for (int j = 0; j < NB; ++j) v[j] = 1 << (RESIZE_PREC_BITS - 1);
@@ -290,7 +295,7 @@ __global__ void __launch_bounds__(V_TX * V_TY) resize_v_kernel(const __grid_cons
   const int nb = min(V_GROUP, d.row_bytes - (int)p);
   const bool vec = d.vec && nb == V_GROUP;
   int v[V_GROUP];
-  v_taps(d.src + (size_t)ymin * d.row_bytes + p, d.row_bytes, sk + threadIdx.y * d.ksize, n, 0, nb, vec, v);
+  v_taps(d.src + (size_t)ymin * d.src_pitch + p, d.src_pitch, sk + threadIdx.y * d.ksize, n, 0, nb, vec, v);
   if (d.swap) swap_rb12(v);
   store12(d.dst + (size_t)(y0 + threadIdx.y) * d.row_bytes + p, v, nb, vec);
 }
@@ -412,9 +417,9 @@ static int check_image(int i, int ih, int iw, int oh, int ow) {
   return 0;
 }
 
-// appends the horizontal pass rows x iw -> rows x ow of src into dst (the table of iw -> ow must be cached) to hl
-static int add_h_pass(int dev, PassList<HPass>& hl, long long& tiles, int& kmax, const unsigned char* src, unsigned char* dst,
-                      int rows, int iw, int ow, int swap) {
+// appends the horizontal pass rows x iw -> rows x ow of src (rows src_pitch bytes apart) into dst (packed rows) to hl
+static int add_h_pass(int dev, PassList<HPass>& hl, long long& tiles, int& kmax, const unsigned char* src, long long src_pitch,
+                      unsigned char* dst, int rows, int iw, int ow, int swap) {
   const AxisTable* t = nullptr;
   int rc = axis_table(dev, iw, ow, &t);
   if (rc) return rc;
@@ -423,6 +428,7 @@ static int add_h_pass(int dev, PassList<HPass>& hl, long long& tiles, int& kmax,
   h.dst = dst;
   h.bounds = t->bounds;
   h.coeffs = t->coeffs;
+  h.src_pitch = src_pitch;
   h.ksize = t->ksize;
   h.rows = rows;
   h.in_w = iw;
@@ -455,6 +461,84 @@ static int v_table(int dev, int ih, int oh, const int** bounds, const int** coef
   *bounds = t->bounds;
   *coeffs = t->coeffs;
   *ksize = t->ksize;
+  return 0;
+}
+
+// The scratch query and the launches of se_resize_u8 and se_resize_window_u8, after their checks: image i is read from
+// src[i] (nullptr in the query form), its rows pitch[i] bytes apart, and written packed at dst + dst_off[i].
+static int resize_images(const std::vector<const unsigned char*>& src, const std::vector<long long>& pitch, const int* src_hw,
+                         unsigned char* dst, const long long* dst_off, const int* dst_hw, int n, int C, int swap_rb, void* scratch,
+                         long long* scratch_bytes, cudaStream_t st) {
+  size_t need = 0;
+  std::vector<size_t> mid(n);
+  for (int i = 0; i < n; ++i) {
+    mid[i] = need;
+    if (src_hw[2 * i + 1] != dst_hw[2 * i + 1] && src_hw[2 * i] != dst_hw[2 * i]) need += scratch_round((size_t)src_hw[2 * i] * dst_hw[2 * i + 1] * C);
+  }
+  if (!scratch) {
+    *scratch_bytes = (long long)need;
+    return 0;
+  }
+  SE_REQUIRE((size_t)*scratch_bytes >= need, "scratch holds " + std::to_string(*scratch_bytes) + " bytes, needs " + std::to_string(need));
+  if (n == 0) return 0;
+  SE_REQUIRE(dst && std::find(src.begin(), src.end(), nullptr) == src.end(), "null src / dst");
+  std::lock_guard<std::mutex> lk(g_resize_mu);
+  int dev = 0;
+  SE_CUDA_OK(cudaGetDevice(&dev));
+  {
+    std::vector<std::pair<int, int>> pairs;
+    for (int i = 0; i < n; ++i) {
+      if (src_hw[2 * i + 1] != dst_hw[2 * i + 1]) pairs.emplace_back(src_hw[2 * i + 1], dst_hw[2 * i + 1]);
+      if (src_hw[2 * i] != dst_hw[2 * i]) pairs.emplace_back(src_hw[2 * i], dst_hw[2 * i]);
+    }
+    int rc = reserve_tables(dev, pairs);
+    if (rc) return rc;
+  }
+  PassList<HPass> hl;
+  PassList<VPass> vl;
+  memset(&hl, 0, sizeof(hl));
+  memset(&vl, 0, sizeof(vl));
+  long long htiles = 0, vtiles = 0;
+  int hk = 1, vk = 1;
+  for (int i = 0; i < n; ++i) {
+    const int ih = src_hw[2 * i], iw = src_hw[2 * i + 1], oh = dst_hw[2 * i], ow = dst_hw[2 * i + 1];
+    const unsigned char* s = src[i];
+    long long sp = pitch[i];
+    unsigned char* o = dst + dst_off[i];
+    if (iw != ow) {
+      unsigned char* h_dst = ih != oh ? (unsigned char*)scratch + mid[i] : o;
+      int rc = add_h_pass(dev, hl, htiles, hk, s, sp, h_dst, ih, iw, ow, ih == oh && swap_rb);
+      if (rc) return rc;
+      if (ih == oh) continue;
+      s = h_dst;
+      sp = (long long)ow * C;
+    }
+    VPass& v = vl.p[vl.n++];   // the vertical pass, or the copy of an image whose size does not change
+    v.src = s;
+    v.dst = o;
+    v.src_pitch = sp;
+    int rc = v_table(dev, ih, oh, &v.bounds, &v.coeffs, &v.ksize);
+    if (rc) return rc;
+    v.in_h = ih;
+    v.out_h = oh;
+    v.row_bytes = ow * C;
+    v.groups = cdiv_i(v.row_bytes, V_GROUP);
+    v.swap = swap_rb;
+    v.vec = ((uintptr_t)v.src % 4 == 0) && ((uintptr_t)v.dst % 4 == 0) && v.row_bytes % 4 == 0 && sp % 4 == 0;
+    v.tile0 = (int)vtiles;
+    v.tiles_x = cdiv_i(v.groups, V_TX);
+    vtiles += (long long)v.tiles_x * cdiv_i(oh, V_TY);
+    vk = std::max(vk, v.ksize);
+  }
+  SE_REQUIRE(htiles < (1LL << 31) && vtiles < (1LL << 31), "batch too large for one launch");
+  int rc = C == 3 ? launch_h<3>(hl, htiles, hk, st) : launch_h<1>(hl, htiles, hk, st);
+  if (rc) return rc;
+  if (vl.n) {
+    const int smem = (V_TY * vk + 2 * V_TY) * 4;
+    SE_CUDA_OK(cudaFuncSetAttribute(resize_v_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+    resize_v_kernel<<<(unsigned)vtiles, dim3(V_TX, V_TY), smem, st>>>(vl);
+    SE_CUDA_OK(cudaGetLastError());
+  }
   return 0;
 }
 
@@ -516,9 +600,9 @@ static int paste_boxes(const std::vector<PasteBox>& boxes, const std::vector<Pas
       if (b.iw != b.ow) {   // the paste reads the horizontal passes' output instead of the result itself
         unsigned char* s3 = (unsigned char*)scratch + mid[order[j]];
         unsigned char* s1 = s3 + scratch_round((size_t)b.ih * b.ow * 3);
-        int rc = add_h_pass(dev, h3, t3, k3, b.rgb, s3, b.ih, b.iw, b.ow, 0);
+        int rc = add_h_pass(dev, h3, t3, k3, b.rgb, 3LL * b.iw, s3, b.ih, b.iw, b.ow, 0);
         if (rc) return rc;
-        rc = add_h_pass(dev, h1, t1, k1, b.mask, s1, b.ih, b.iw, b.ow, 0);
+        rc = add_h_pass(dev, h1, t1, k1, b.mask, b.iw, s1, b.ih, b.iw, b.ow, 0);
         if (rc) return rc;
         p.rgb = s3;
         p.mask = s1;
@@ -609,80 +693,39 @@ int se_resize_u8(const unsigned char* src, const long long* src_off, const int* 
   SE_REQUIRE(!swap_rb || channels == 3, "swap_rb needs 3 channels");
   SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
   SE_REQUIRE(n == 0 || (src_off && src_hw && dst_off && dst_hw), "null size / offset array");
-  const int C = channels;
-  size_t need = 0;
-  std::vector<size_t> mid(n);
+  std::vector<const unsigned char*> srcs(n, nullptr);
+  std::vector<long long> pitch(n);
   for (int i = 0; i < n; ++i) {
-    const int ih = src_hw[2 * i], iw = src_hw[2 * i + 1], oh = dst_hw[2 * i], ow = dst_hw[2 * i + 1];
-    int rc = check_image(i, ih, iw, oh, ow);
+    int rc = check_image(i, src_hw[2 * i], src_hw[2 * i + 1], dst_hw[2 * i], dst_hw[2 * i + 1]);
     if (rc) return rc;
     SE_REQUIRE(src_off[i] >= 0 && dst_off[i] >= 0, "negative offset");
-    mid[i] = need;
-    if (iw != ow && ih != oh) need += scratch_round((size_t)ih * ow * C);
+    if (src) srcs[i] = src + src_off[i];
+    pitch[i] = (long long)src_hw[2 * i + 1] * channels;
   }
-  if (!scratch) {
-    *scratch_bytes = (long long)need;
-    return 0;
-  }
-  SE_REQUIRE((size_t)*scratch_bytes >= need, "scratch holds " + std::to_string(*scratch_bytes) + " bytes, needs " + std::to_string(need));
-  if (n == 0) return 0;
-  SE_REQUIRE(src && dst, "null src / dst");
-  cudaStream_t st = (cudaStream_t)stream;
-  std::lock_guard<std::mutex> lk(g_resize_mu);
-  int dev = 0;
-  SE_CUDA_OK(cudaGetDevice(&dev));
-  {
-    std::vector<std::pair<int, int>> pairs;
-    for (int i = 0; i < n; ++i) {
-      if (src_hw[2 * i + 1] != dst_hw[2 * i + 1]) pairs.emplace_back(src_hw[2 * i + 1], dst_hw[2 * i + 1]);
-      if (src_hw[2 * i] != dst_hw[2 * i]) pairs.emplace_back(src_hw[2 * i], dst_hw[2 * i]);
-    }
-    int rc = reserve_tables(dev, pairs);
-    if (rc) return rc;
-  }
-  PassList<HPass> hl;
-  PassList<VPass> vl;
-  memset(&hl, 0, sizeof(hl));
-  memset(&vl, 0, sizeof(vl));
-  long long htiles = 0, vtiles = 0;
-  int hk = 1, vk = 1;
+  return resize_images(srcs, pitch, src_hw, dst, dst_off, dst_hw, n, channels, swap_rb, scratch, scratch_bytes, (cudaStream_t)stream);
+}
+
+int se_resize_window_u8(const unsigned char* const* src, const long long* src_pitch, const int* src_hw, unsigned char* dst,
+                        const long long* dst_off, const int* dst_hw, int n, int channels, int swap_rb, void* scratch,
+                        long long* scratch_bytes, void* stream) {
+  SE_REQUIRE(n >= 0 && n <= RESIZE_MAX_BATCH, "n must be in [0, " + std::to_string(RESIZE_MAX_BATCH) + "] images per call");
+  SE_REQUIRE(channels == 1 || channels == 3, "channels must be 1 or 3");
+  SE_REQUIRE(!swap_rb || channels == 3, "swap_rb needs 3 channels");
+  SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
+  SE_REQUIRE(n == 0 || (src_pitch && src_hw && dst_off && dst_hw), "null size / offset array");
+  std::vector<const unsigned char*> srcs(n, nullptr);
+  std::vector<long long> pitch(n);
   for (int i = 0; i < n; ++i) {
-    const int ih = src_hw[2 * i], iw = src_hw[2 * i + 1], oh = dst_hw[2 * i], ow = dst_hw[2 * i + 1];
-    const unsigned char* s = src + src_off[i];
-    unsigned char* o = dst + dst_off[i];
-    if (iw != ow) {
-      unsigned char* h_dst = ih != oh ? (unsigned char*)scratch + mid[i] : o;
-      int rc = add_h_pass(dev, hl, htiles, hk, s, h_dst, ih, iw, ow, ih == oh && swap_rb);
-      if (rc) return rc;
-      if (ih == oh) continue;
-      s = h_dst;
-    }
-    VPass& v = vl.p[vl.n++];   // the vertical pass, or the copy of an image whose size does not change
-    v.src = s;
-    v.dst = o;
-    int rc = v_table(dev, ih, oh, &v.bounds, &v.coeffs, &v.ksize);
+    int rc = check_image(i, src_hw[2 * i], src_hw[2 * i + 1], dst_hw[2 * i], dst_hw[2 * i + 1]);
     if (rc) return rc;
-    v.in_h = ih;
-    v.out_h = oh;
-    v.row_bytes = ow * C;
-    v.groups = cdiv_i(v.row_bytes, V_GROUP);
-    v.swap = swap_rb;
-    v.vec = ((uintptr_t)v.src % 4 == 0) && ((uintptr_t)v.dst % 4 == 0) && v.row_bytes % 4 == 0;
-    v.tile0 = (int)vtiles;
-    v.tiles_x = cdiv_i(v.groups, V_TX);
-    vtiles += (long long)v.tiles_x * cdiv_i(oh, V_TY);
-    vk = std::max(vk, v.ksize);
+    SE_REQUIRE(dst_off[i] >= 0, "negative offset");
+    const long long row = (long long)src_hw[2 * i + 1] * channels;
+    SE_REQUIRE(src_pitch[i] >= row, "image " + std::to_string(i) + ": the source pitch of " + std::to_string(src_pitch[i]) +
+                                        " bytes is narrower than its row of " + std::to_string(row) + " bytes");
+    if (src) srcs[i] = src[i];
+    pitch[i] = src_pitch[i];
   }
-  SE_REQUIRE(htiles < (1LL << 31) && vtiles < (1LL << 31), "batch too large for one launch");
-  int rc = C == 3 ? launch_h<3>(hl, htiles, hk, st) : launch_h<1>(hl, htiles, hk, st);
-  if (rc) return rc;
-  if (vl.n) {
-    const int smem = (V_TY * vk + 2 * V_TY) * 4;
-    SE_CUDA_OK(cudaFuncSetAttribute(resize_v_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
-    resize_v_kernel<<<(unsigned)vtiles, dim3(V_TX, V_TY), smem, st>>>(vl);
-    SE_CUDA_OK(cudaGetLastError());
-  }
-  return 0;
+  return resize_images(srcs, pitch, src_hw, dst, dst_off, dst_hw, n, channels, swap_rb, scratch, scratch_bytes, (cudaStream_t)stream);
 }
 
 int se_resize_paste_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask, const long long* mask_off,

@@ -331,6 +331,73 @@ def resize_u8_packed(src, src_offsets, src_sizes, dst_sizes, channels, swap_rb=F
     return out, dst_offsets
 
 
+def resize_window_u8_packed(src, src_offsets, src_pitches, src_sizes, dst_sizes, channels, swap_rb=False, out=None,
+                            dst_offsets=None):
+    """``resize_u8_packed`` of windows of larger images (``se_resize_window_u8``): image i is the ``src_sizes[i] = (h, w)``
+    window whose row r starts at byte ``src_offsets[i] + r * src_pitches[i]`` of its source, with ``src_pitches[i] >= w *
+    channels``. ``src`` is one contiguous CUDA uint8 tensor, or a list of them with one per image. With the offset of a box's
+    top-left pixel in an [H,W,C] photo and the pitch ``W * C`` the window is ``Image.crop(box)``, so the result is
+    ``Image.crop(box).resize(size)`` bit for bit, without the crop. Windows may overlap; ``out`` must not overlap any of them.
+    ``out``, ``dst_offsets``, ``swap_rb`` and the return value are those of ``resize_u8_packed``."""
+    n = len(src_sizes)
+    srcs = list(src) if isinstance(src, (list, tuple)) else [src] * n
+    if not (len(srcs) == len(src_offsets) == len(src_pitches) == len(dst_sizes) == n):
+        raise _lib.SketchEditB200Error("src (as a list), src_offsets, src_pitches, src_sizes and dst_sizes must have the same length")
+    for t in srcs + [out]:
+        if t is not None and not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
+            raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % ("out" if t is out else "src"))
+    if n == 0:
+        return out, dst_offsets
+    dev = srcs[0].device
+    if any(t.device != dev for t in srcs):
+        raise _lib.SketchEditB200Error("every src must be on one device")
+    src_sizes = [(int(h), int(w)) for h, w in src_sizes]
+    dst_sizes = [(int(h), int(w)) for h, w in dst_sizes]
+    src_offsets, src_pitches = [int(o) for o in src_offsets], [int(p) for p in src_pitches]
+    for i, (t, o, p, (h, w)) in enumerate(zip(srcs, src_offsets, src_pitches, src_sizes)):
+        if p < w * channels:
+            raise _lib.SketchEditB200Error("window %d: the pitch of %d bytes is narrower than its row of %d bytes" % (i, p, w * channels))
+        if o < 0 or h < 1 or o + (h - 1) * p + w * channels > t.numel():
+            raise _lib.SketchEditB200Error("window %d (%dx%d at %d, pitch %d) is outside the %d-byte src" % (i, h, w, o, p, t.numel()))
+    nbytes = lambda hw: hw[0] * hw[1] * channels
+    if out is None:
+        if dst_offsets is not None:
+            raise _lib.SketchEditB200Error("dst_offsets needs out")
+        dst_offsets, total = [], 0
+        for hw in dst_sizes:
+            dst_offsets.append(total)
+            total += (nbytes(hw) + 15) // 16 * 16
+        out = torch.empty(total, device=dev, dtype=torch.uint8)
+    elif dst_offsets is None or len(dst_offsets) != n:
+        raise _lib.SketchEditB200Error("out needs one dst_offsets entry per image")
+    if out.device != dev:
+        raise _lib.SketchEditB200Error("src on %s but out on %s" % (dev, out.device))
+    dst_offsets = [int(o) for o in dst_offsets]
+    for o, hw in zip(dst_offsets, dst_sizes):
+        if o < 0 or o + nbytes(hw) > out.numel():
+            raise _lib.SketchEditB200Error("out slice [%d, %d) outside the %d-byte buffer" % (o, o + nbytes(hw), out.numel()))
+    lib = _lib.load()
+    L, I, P = ctypes.c_longlong, ctypes.c_int, ctypes.c_void_p
+    with torch.cuda.device(dev):
+        chunks = []
+        for c0 in range(0, n, RESIZE_MAX_BATCH):
+            sl = slice(c0, c0 + RESIZE_MAX_BATCH)
+            k = len(src_sizes[sl])
+            args = ((P * k)(*[t.data_ptr() + o for t, o in zip(srcs[sl], src_offsets[sl])]), (L * k)(*src_pitches[sl]),
+                    (I * (2 * k))(*[v for hw in src_sizes[sl] for v in hw]), (L * k)(*dst_offsets[sl]),
+                    (I * (2 * k))(*[v for hw in dst_sizes[sl] for v in hw]), k)
+            need = L(0)
+            _lib.check(lib.se_resize_window_u8(None, args[1], args[2], None, args[3], args[4], k, channels, int(bool(swap_rb)), None,
+                                               ctypes.byref(need), None))
+            chunks.append((args, need.value))
+        scratch = torch.empty(max([1] + [b for _, b in chunks]), device=dev, dtype=torch.uint8)
+        for a, _ in chunks:
+            size = L(scratch.numel())
+            _lib.check(lib.se_resize_window_u8(a[0], a[1], a[2], _ptr(out), a[3], a[4], a[5], channels, int(bool(swap_rb)),
+                                               _ptr(scratch), ctypes.byref(size), _stream()))
+    return out, dst_offsets
+
+
 def resize_paste_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, base, base_offsets, dst_sizes, swap_rb=False, out=None,
                            dst_offsets=None):
     """Resize back and paste (``se_resize_paste_u8``), bit for bit as Pillow does it, for a batch of packed uint8 images:

@@ -13,17 +13,20 @@ too (``engine.resize_u8_packed``, bit-identical to Pillow), so a batch is one up
     result_pil = proc.process_image(image_pil, mask_pil, edit_mask=corrected_mask)      # run on a revised edit mask
     result_pil = proc.process_image(image_pil, mask_pil, region="auto")                 # edit a crop around the strokes only
     result_pil = proc.process_image(image_pil, mask_pil, region="strokes")              # one crop per group of strokes
+    s = proc.open_session(image_pil)                  # the photo stays on the device across edits
+    r = s.edit(mask_pil, region="strokes")            # r.boxes, r.patches: what changed; s.undo() restores it
     proc.close()
 
 A region edit (``region=``) crops a box of the photo, runs the forward on it at ``DemoProcessor(region_size=...)`` and pastes
 the result back with the edit mask: its cost follows the box, not the photo, and region requests on photos of any size
-batch together. A request may carry several boxes (``region="strokes"`` or a list), pasted in order.
+batch together. A request may carry several boxes (``region="strokes"`` or a list), pasted in order. An ``EditSession`` keeps one photo on
+the device for a chain of edits, each drawn on the previous result, with undo.
 
 Everything except the forward itself (``run_batch``) is plain host logic and is unit-tested on the CPU with a fake forward.
 """
 import threading
 import time
-from collections import OrderedDict, deque
+from collections import OrderedDict, deque, namedtuple
 
 import numpy as np
 
@@ -155,9 +158,11 @@ def _intersects(a, b):
     return a[0] < b[2] and b[0] < a[2] and a[1] < b[3] and b[1] < a[3]
 
 
-def region_groups(mask, edit_mask=None, region_size=(256, 256)):
+def region_groups(mask, edit_mask=None, region_size=(256, 256), photo_size=None, offset=(0, 0)):
     """The stroke groups of a region edit with ``region="strokes"``: a list of ``(bbox, box)`` PIL boxes, one per group,
-    ordered by the (upper, left) corner of ``bbox``. ``mask`` and ``edit_mask`` are PIL images of the photo's size.
+    ordered by the (upper, left) corner of ``bbox``. ``mask`` and ``edit_mask`` are PIL images of the photo's size, or of one
+    smaller size placed at ``offset = (x, y)`` in a photo of PIL size ``photo_size`` (zero elsewhere); the boxes are then those
+    of the zero-padded photo-sized masks, in photo coordinates.
 
     1. The non-zero pixels of ``mask`` and ``edit_mask`` are connected (8-neighbourhood) on a grid of 8x8-pixel cells; a cell is
        set when any of its pixels is. ``bbox`` is the exact pixel bounding box of a group's non-zero pixels.
@@ -165,12 +170,13 @@ def region_groups(mask, edit_mask=None, region_size=(256, 256)):
     3. ``box = region_box(bbox, mask.size, region_size)``.
     So every box holds its own group's strokes and no other group's: ``mask.crop(box)`` is that group's sketch alone. Boxes
     may still overlap, in stroke-free margins. One group gives the box of ``region="auto"``. No stroke is a ValueError."""
-    w, h = mask.size
+    w, h = photo_size or mask.size
+    dx, dy = (int(v) for v in offset)
     if edit_mask is not None and edit_mask.size != mask.size:
         raise ValueError("edit_mask is %dx%d, mask %dx%d: they must have one size" % (edit_mask.size + mask.size))
     c = GROUP_CELL
     ims = [m if m.mode == "L" else m.convert("L") for m in (mask, edit_mask) if m is not None]
-    bbs = [b for b in (m.getbbox() for m in ims) if b]
+    bbs = [(b[0] + dx, b[1] + dy, b[2] + dx, b[3] + dy) for b in (m.getbbox() for m in ims) if b]
     if not bbs:
         raise ValueError("region='strokes' needs a sketch stroke or a non-zero edit mask")
     # only the cells of the union bbox are examined, from a cell corner of the photo's grid
@@ -179,8 +185,8 @@ def region_groups(mask, edit_mask=None, region_size=(256, 256)):
     ch, cw = crop[3] - oy, crop[2] - ox
     H8, W8 = -(-ch // c), -(-cw // c)
     pad = np.zeros((H8 * c, W8 * c), np.uint8)
-    for m in ims:
-        np.maximum(pad[:ch, :cw], np.asarray(m.crop(crop)), out=pad[:ch, :cw])
+    for m in ims:                                               # PIL pads a crop reaching past the mask with zeros
+        np.maximum(pad[:ch, :cw], np.asarray(m.crop((crop[0] - dx, crop[1] - dy, crop[2] - dx, crop[3] - dy))), out=pad[:ch, :cw])
     blocks = pad.reshape(H8, c, W8, c)
     cells = (pad.view(np.uint64).reshape(H8, c, W8) != 0).any(axis=1)     # a cell row's 8 pixels as one word: exact
     # runs of set cells per cell row, joined by union-find with the overlapping (8-neighbour) runs of the row above
@@ -314,12 +320,33 @@ class DemoProcessor:
         self.region_size = region_size
         self.engine = model.engine()
         self._pinned = {}              # name -> reused pinned host staging buffer (grown on demand)
+        self._sessions = set()         # open EditSessions, closed by close()
+        self._sessions_mu = threading.Lock()
+        self._closed = False
         self.batcher = RequestBatcher(self._run_batch if resize == "host" else self._run_batch_device, max_batch=max_batch,
                                       max_wait_ms=max_wait_ms)
 
     def close(self):
+        with self._sessions_mu:
+            self._closed = True
+            sessions = list(self._sessions)
+        for sess in sessions:
+            sess.close()
         self.batcher.close()
         self._pinned.clear()
+
+    def open_session(self, img, history_bytes=256 << 20):
+        """An ``EditSession`` on ``img`` (converted to RGB): with ``resize='device'`` the photo is uploaded once to the engine's
+        device and stays there until ``close()``. ``history_bytes`` bounds the bytes its undo snapshots hold."""
+        sess = EditSession(self, img, history_bytes)
+        with self._sessions_mu:
+            closed = self._closed
+            if not closed:
+                self._sessions.add(sess)
+        if closed:
+            sess.close()
+            raise RuntimeError("DemoProcessor is closed")
+        return sess
 
     def _staging(self, name, nbytes):
         buf = self._pinned.get(name)
@@ -328,86 +355,112 @@ class DemoProcessor:
         return buf
 
     def _run_batch_device(self, key, payloads):
-        """payloads: (raw RGB photo [h,w,3], raw 'L' mask [hm,wm], raw 'L' edit mask [he,we] or None, return_mask) at their own
-        sizes; key: the floored network size, plus True when the batch runs on edit masks."""
+        """payloads: (raw RGB photo [h,w,3] or None, raw 'L' mask [hm,wm], raw 'L' edit mask [he,we] or None, return_mask,
+        session photo or None) at their own sizes; key: the floored network size, plus True when the batch runs on edit masks.
+        A session's photo ([h,w,3] on the device, with the raw photo None) is resized from where it lies, and the result is
+        resized back into it after a snapshot of its previous bytes; its result is then (photo, mask, [snapshot])."""
         if key[0] == "region":
             return self._run_region_device(key, payloads)
         torch = self._torch
-        from .engine import resize_u8_packed
+        from .engine import resize_u8_packed, resize_window_u8_packed
         H, W = key[:2]
         edit = len(key) > 2
         B = len(payloads)
         dev = self.engine.device
-        photos, masks = [p[0] for p in payloads], [p[1] for p in payloads]
+        sess = [p[4] for p in payloads]
+        sizes = [tuple(p[4].shape[:2]) if p[4] is not None else p[0].shape[:2] for p in payloads]
+        photos, masks = [p[0] for p in payloads if p[4] is None], [p[1] for p in payloads]
         edits = [p[2] for p in payloads] if edit else []
         back = [i for i, p in enumerate(payloads) if p[3] and not edit]   # predicted masks to resize back and download
         offs, total = _aligned_offsets([a.nbytes for a in photos + masks + edits])
-        out_offs, out_total = _aligned_offsets([a.nbytes for a in photos] + [photos[i].shape[0] * photos[i].shape[1] for i in back])
+        photo_at = iter(offs)                       # upload offset of each raw photo, in order
+        srcs = [sess[i].view(-1) if sess[i] is not None else None for i in range(B)]
+        src_offs = [0 if sess[i] is not None else next(photo_at) for i in range(B)]
+        np_ = len(photos)
+        out_offs, out_total = _aligned_offsets([h * w * 3 for h, w in sizes] + [sizes[i][0] * sizes[i][1] for i in back])
         stage = self._staging("in", total)          # free: every batch, failed ones included, ends with a stream synchronise
         host = stage.numpy()
         for a, o in zip(photos + masks + edits, offs):
             host[o:o + a.nbytes] = a.reshape(-1)
         down = self._staging("out", out_total)
+        snaps = {}
         with torch.cuda.device(dev):
             try:
                 src = stage[:total].to(dev, non_blocking=True)
+                srcs = [t if t is not None else src for t in srcs]
                 img = torch.empty(B, H, W, 3, device=dev, dtype=torch.uint8)
                 msk = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
-                resize_u8_packed(src, offs[:B], [a.shape[:2] for a in photos], [(H, W)] * B, 3, out=img,
-                                 dst_offsets=[i * H * W * 3 for i in range(B)])
+                resize_window_u8_packed(srcs, src_offs, [w * 3 for _, w in sizes], sizes, [(H, W)] * B, 3, out=img,
+                                        dst_offsets=[i * H * W * 3 for i in range(B)])
                 # the resized mask goes to the forward as it is: its input codec applies > 0 (demo.py:52)
-                resize_u8_packed(src, offs[B:2 * B], [a.shape[:2] for a in masks], [(H, W)] * B, 1, out=msk,
+                resize_u8_packed(src, offs[np_:np_ + B], [a.shape[:2] for a in masks], [(H, W)] * B, 1, out=msk,
                                  dst_offsets=[i * H * W for i in range(B)])
                 with torch.no_grad():
                     if edit:
                         edt = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
-                        resize_u8_packed(src, offs[2 * B:], [a.shape[:2] for a in edits], [(H, W)] * B, 1, out=edt,
+                        resize_u8_packed(src, offs[np_ + B:], [a.shape[:2] for a in edits], [(H, W)] * B, 1, out=edt,
                                          dst_offsets=[i * H * W for i in range(B)])
                         bgr = self.engine.inference_with_mask_u8(img, msk, edt, precision=self.precision)
                     else:
                         bgr, mk = self.engine.inference_u8(img, msk, precision=self.precision)
                 # back to each photo's own size; the forward writes BGR, the demo keeps RGB
                 res = torch.empty(max(out_total, 1), device=dev, dtype=torch.uint8)
-                resize_u8_packed(bgr, [i * H * W * 3 for i in range(B)], [(H, W)] * B, [a.shape[:2] for a in photos], 3,
+                resize_u8_packed(bgr, [i * H * W * 3 for i in range(B)], [(H, W)] * B, sizes, 3,
                                  swap_rb=True, out=res, dst_offsets=out_offs[:B])
+                for i, t in enumerate(sess):
+                    if t is not None:
+                        snaps[i] = t.clone()
+                        t.view(-1).copy_(res[out_offs[i]:out_offs[i] + t.numel()])
                 if back:
-                    resize_u8_packed(mk, [i * H * W for i in back], [(H, W)] * len(back), [photos[i].shape[:2] for i in back], 1,
+                    resize_u8_packed(mk, [i * H * W for i in back], [(H, W)] * len(back), [sizes[i] for i in back], 1,
                                      out=res, dst_offsets=out_offs[B:])
                 down[:out_total].copy_(res[:out_total], non_blocking=True)
             finally:
                 torch.cuda.current_stream().synchronize()
         host = down.numpy()
-        results = [host[o:o + a.nbytes].reshape(a.shape).copy() for a, o in zip(photos, out_offs)]
-        masks_back = dict(zip(back, [host[o:o + photos[i].shape[0] * photos[i].shape[1]].reshape(photos[i].shape[:2]).copy()
+        results = [host[o:o + h * w * 3].reshape(h, w, 3).copy() for (h, w), o in zip(sizes, out_offs)]
+        masks_back = dict(zip(back, [host[o:o + sizes[i][0] * sizes[i][1]].reshape(sizes[i]).copy()
                                      for i, o in zip(back, out_offs[B:])]))
-        return [(r, masks_back.get(i)) for i, r in enumerate(results)]
+        return [(r, masks_back.get(i), [snaps[i]]) if i in snaps else (r, masks_back.get(i)) for i, r in enumerate(results)]
 
     def _run_region_device(self, key, payloads):
-        """payloads: (photo crops [bh,bw,3], sketch crops [bh,bw], edit-mask crops [bh,bw] or None, return_mask, boxes): one crop
-        per PIL box of the request, at its box size; key: ("region", Hn, Wn), plus True when the batch runs on edit masks.
-        Returns per request one (patch, mask) per box: patch [bh,bw,3] is the box's bytes once all of the request's boxes are
-        pasted in order, mask the box's paste mask resized back to [bh,bw] when asked for and predicted, else None."""
+        """payloads: (photo crops [bh,bw,3] or None, sketch crops [bh,bw], edit-mask crops [bh,bw] or None, return_mask, boxes,
+        session photo or None): one crop per PIL box of the request, at its box size; key: ("region", Hn, Wn), plus True when
+        the batch runs on edit masks. Returns per request one (patch, mask) per box: patch [bh,bw,3] is the box's bytes once all
+        of the request's boxes are pasted in order, mask the box's paste mask resized back to [bh,bw] when asked for and
+        predicted, else None. A session's request has no photo crops: its boxes are resized from its photo ([h,w,3] on the
+        device), snapshotted and pasted into it, and its result is (that list, [previous bytes of each box])."""
         torch = self._torch
-        from .engine import resize_composite_u8_packed, resize_u8_packed
+        from .engine import resize_composite_u8_packed, resize_u8_packed, resize_window_u8_packed
         H, W = key[1:3]
         edit = key[-1] is True
         dev = self.engine.device
-        photos, masks = [a for p in payloads for a in p[0]], [a for p in payloads for a in p[1]]   # one item per box
-        edits = [a for p in payloads for a in p[2]] if edit else []
-        boxes = [b for p in payloads for b in p[4]]
-        B = len(photos)
-        sizes = [a.shape[:2] for a in photos]
-        back = [i for i, r in enumerate(p[3] for p in payloads for _ in p[0]) if r and not edit]   # predicted masks to return
-        offs, total = _aligned_offsets([a.nbytes for a in photos + masks + edits])
-        # A box that overlaps no other box of its request is pasted in place over its uploaded photo crop (the first B slots).
-        # A set of overlapping boxes is pasted into a canvas, their bounding rectangle, assembled after the uploads from the
-        # crops; its boxes are then copied back into their crop slots. A predicted mask is resized back into the slot of its
-        # sketch crop. One download covers both.
+        items = [(r, j) for r, p in enumerate(payloads) for j in range(len(p[4]))]   # (request, box) per box
+        B = len(items)
+        boxes = [payloads[r][4][j] for r, j in items]
+        sizes = [(b[3] - b[1], b[2] - b[0]) for b in boxes]
+        sess = [payloads[r][5] for r, _ in items]
+        plain = [i for i in range(B) if sess[i] is None]
+        photos = {i: payloads[r][0][j] for i, (r, j) in enumerate(items) if sess[i] is None}
+        masks = [payloads[r][1][j] for r, j in items]
+        edits = [payloads[r][2][j] for r, j in items] if edit else []
+        back = [i for i, (r, _) in enumerate(items) if payloads[r][3] and not edit]   # predicted masks to return
+        # The work buffer: the plain requests' photo crops (uploaded; a box that overlaps no other box of its request is pasted
+        # in place over its crop), the session boxes' patches, the predicted masks resized back (these three are the one
+        # download), then the sketch and edit-mask crops (uploaded), then the canvases. A set of overlapping boxes of a plain
+        # request is pasted into a canvas, their bounding rectangle, assembled from the crops after the upload; its boxes are
+        # then copied back into their crop slots. A session's boxes are pasted into its photo and copied out to their slots.
+        slots = plain + [i for i in range(B) if sess[i] is not None] + back
+        so, n_down = _aligned_offsets([sizes[i][0] * sizes[i][1] * (3 if k < B else 1) for k, i in enumerate(slots)])
+        rgb_at, mask_at = dict(zip(slots[:B], so[:B])), dict(zip(back, so[B:]))
+        n_plain = so[len(plain)] if len(plain) < len(slots) else n_down   # the end of the plain crops: the first upload
+        mo, m_total = _aligned_offsets([a.nbytes for a in masks + edits])
+        sk_at, total = [n_down + o for o in mo], n_down + m_total
         canvas = {}                                   # item -> (canvas offset, pitch, y, x) for boxes in a set of several
         canvas_end, first = total, 0
         for p in payloads:
             rb = p[4]
-            for s in _overlap_sets(rb):
+            for s in (_overlap_sets(rb) if p[5] is None else []):
                 if len(s) < 2:
                     continue
                 L, U = min(rb[i][0] for i in s), min(rb[i][1] for i in s)
@@ -416,57 +469,87 @@ class DemoProcessor:
                     canvas[first + i] = (canvas_end, (R - L) * 3, rb[i][1] - U, rb[i][0] - L)
                 canvas_end += ((D - U) * (R - L) * 3 + 15) // 16 * 16
             first += len(rb)
-        n_down = max([offs[i] + photos[i].nbytes for i in range(B)] + [offs[B + i] + masks[i].nbytes for i in back])
         stage = self._staging("in", total)          # free: every batch, failed ones included, ends with a stream synchronise
         host = stage.numpy()
-        for a, o in zip(photos + masks + edits, offs):
+        for i, a in photos.items():
+            host[rgb_at[i]:rgb_at[i] + a.nbytes] = a.reshape(-1)
+        for a, o in zip(masks + edits, sk_at):
             host[o:o + a.nbytes] = a.reshape(-1)
         down = self._staging("out", n_down)
         net3, net1 = [i * H * W * 3 for i in range(B)], [i * H * W for i in range(B)]
+
+        def crop_slot(work, i):
+            return work[rgb_at[i]:rgb_at[i] + sizes[i][0] * sizes[i][1] * 3].view(*sizes[i], 3)
 
         def in_canvas(work, i):                       # item i's box in its canvas, and its crop slot, as [bh,bw,3] views
             co, pitch, y, x = canvas[i]
             bh, bw = sizes[i]
             rows = work[co:co + (y + bh) * pitch].view(y + bh, pitch)
-            return rows[y:, x * 3:(x + bw) * 3].view(bh, bw, 3), work[offs[i]:offs[i] + photos[i].nbytes].view(bh, bw, 3)
+            return rows[y:, x * 3:(x + bw) * 3].view(bh, bw, 3), crop_slot(work, i)
 
+        def in_photo(i):                              # a session item's box in its photo, as a [bh,bw,3] view
+            left, upper, right, lower = boxes[i]
+            return sess[i][upper:lower, left:right]
+
+        snaps = {}
         with torch.cuda.device(dev):
             try:
                 work = torch.empty(canvas_end, device=dev, dtype=torch.uint8)
-                work[:total].copy_(stage[:total], non_blocking=True)
+                if n_plain:
+                    work[:n_plain].copy_(stage[:n_plain], non_blocking=True)
+                work[n_down:total].copy_(stage[n_down:total], non_blocking=True)
                 for i in canvas:                      # 2-D copies; overlapping crops hold the same photo bytes
                     dst, crop = in_canvas(work, i)
                     dst.copy_(crop)
                 img = torch.empty(B, H, W, 3, device=dev, dtype=torch.uint8)
                 msk = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
-                resize_u8_packed(work, offs[:B], sizes, [(H, W)] * B, 3, out=img, dst_offsets=net3)
-                resize_u8_packed(work, offs[B:2 * B], sizes, [(H, W)] * B, 1, out=msk, dst_offsets=net1)
+                # the photo crops: plain ones from their upload slots, a session's as windows of its photo
+                srcs = [work if sess[i] is None else sess[i].view(-1) for i in range(B)]
+                src_offs = [rgb_at[i] if sess[i] is None else (boxes[i][1] * sess[i].shape[1] + boxes[i][0]) * 3 for i in range(B)]
+                pitches = [sizes[i][1] * 3 if sess[i] is None else sess[i].shape[1] * 3 for i in range(B)]
+                resize_window_u8_packed(srcs, src_offs, pitches, sizes, [(H, W)] * B, 3, out=img, dst_offsets=net3)
+                resize_u8_packed(work, sk_at[:B], sizes, [(H, W)] * B, 1, out=msk, dst_offsets=net1)
                 with torch.no_grad():
                     if edit:
                         pm = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
-                        resize_u8_packed(work, offs[2 * B:], sizes, [(H, W)] * B, 1, out=pm, dst_offsets=net1)
+                        resize_u8_packed(work, sk_at[B:], sizes, [(H, W)] * B, 1, out=pm, dst_offsets=net1)
                         bgr = self.engine.inference_with_mask_u8(img, msk, pm, precision=self.precision)
                     else:
                         bgr, pm = self.engine.inference_u8(img, msk, precision=self.precision)
-                place = [canvas.get(i, (offs[i], sizes[i][1] * 3, 0, 0)) for i in range(B)]
-                resize_composite_u8_packed(bgr, net3, pm, net1, [(H, W)] * B, work, [c[0] for c in place], [c[1] for c in place],
-                                           [c[2:] for c in place], sizes, swap_rb=True)
+                for i in range(B):
+                    if sess[i] is not None:
+                        snaps[i] = in_photo(i).clone()
+                groups = [plain] if plain else []     # one composite for the plain boxes, one per session
+                groups += [[i for i in range(B) if items[i][0] == r] for r, p in enumerate(payloads) if p[5] is not None]
+                for g in groups:
+                    if sess[g[0]] is None:
+                        place = [canvas.get(i, (rgb_at[i], sizes[i][1] * 3, 0, 0)) for i in g]
+                        target = work
+                    else:
+                        place = [(0, sess[i].shape[1] * 3, boxes[i][1], boxes[i][0]) for i in g]
+                        target = sess[g[0]].view(-1)
+                    resize_composite_u8_packed(bgr, [net3[i] for i in g], pm, [net1[i] for i in g], [(H, W)] * len(g), target,
+                                               [c[0] for c in place], [c[1] for c in place], [c[2:] for c in place],
+                                               [sizes[i] for i in g], swap_rb=True)
                 for i in canvas:
                     src, crop = in_canvas(work, i)
                     crop.copy_(src)
+                for i in snaps:
+                    crop_slot(work, i).copy_(in_photo(i))
                 if back:
                     resize_u8_packed(pm, [net1[i] for i in back], [(H, W)] * len(back), [sizes[i] for i in back], 1, out=work,
-                                     dst_offsets=[offs[B + i] for i in back])
+                                     dst_offsets=[mask_at[i] for i in back])
                 down[:n_down].copy_(work[:n_down], non_blocking=True)
             finally:
                 torch.cuda.current_stream().synchronize()
         host = down.numpy()
-        items = []
-        for i, (a, o) in enumerate(zip(photos, offs)):
-            m = host[offs[B + i]:offs[B + i] + masks[i].nbytes].reshape(sizes[i]).copy() if i in back else None
-            items.append((host[o:o + a.nbytes].reshape(a.shape).copy(), m))
-        ends = np.cumsum([len(p[4]) for p in payloads])
-        return [items[e - len(p[4]):e] for e, p in zip(ends, payloads)]
+        out = [[] for _ in payloads]
+        for i, (r, _) in enumerate(items):
+            (h, w), o = sizes[i], rgb_at[i]
+            m = host[mask_at[i]:mask_at[i] + h * w].reshape(h, w).copy() if i in mask_at else None
+            out[r].append((host[o:o + h * w * 3].reshape(h, w, 3).copy(), m))
+        return [(o, [snaps[i] for i in range(B) if items[i][0] == r]) if p[5] is not None else o
+                for r, (o, p) in enumerate(zip(out, payloads))]
 
     def _run_batch(self, key, payloads):
         """payloads: (photo [H,W,3], mask [H,W], edit mask [H,W] or None, return_mask) at the network size of ``key`` (the
@@ -527,7 +610,7 @@ class DemoProcessor:
                 if m is not None and m.mode != "L":
                     raise ValueError("resize='device' takes an 'L' %s (got mode %r); resize='host' resizes it with Pillow" % (nm, m.mode))
             edit_raw = np.asarray(edit_mask) if edit_mask is not None else None
-            out, mk = self.batcher.submit(key, (np.asarray(img), np.asarray(mask), edit_raw, return_mask))
+            out, mk = self.batcher.submit(key, (np.asarray(img), np.asarray(mask), edit_raw, return_mask, None))
             res = Image.fromarray(out)
             mk = Image.fromarray(mk) if mk is not None else None
         else:
@@ -542,18 +625,20 @@ class DemoProcessor:
             return res
         return res, (edit_mask if edit_mask is not None else mk)
 
-    def _region_boxes(self, img, mask, edit_mask, region):
-        w, h = img.size
+    def _region_boxes(self, size, mask, edit_mask, region, offset=(0, 0)):
+        """The PIL boxes of a region edit of a photo of PIL size ``size``; the masks lie at ``offset`` in it."""
+        w, h = size
+        dx, dy = offset
         if isinstance(region, str):
             if region == "strokes":
-                return [box for _, box in region_groups(mask, edit_mask, self.region_size)]
+                return [box for _, box in region_groups(mask, edit_mask, self.region_size, size, offset)]
             if region != "auto":
                 raise ValueError("region must be None, 'auto', 'strokes', a PIL box or a list of PIL boxes, got %r" % region)
             bbs = [b for b in (mask.getbbox(), edit_mask.getbbox() if edit_mask is not None else None) if b]
             if not bbs:
                 raise ValueError("region='auto' needs a sketch stroke or a non-zero edit mask")
-            return [region_box((min(b[0] for b in bbs), min(b[1] for b in bbs), max(b[2] for b in bbs), max(b[3] for b in bbs)),
-                               img.size, self.region_size)]
+            return [region_box((min(b[0] for b in bbs) + dx, min(b[1] for b in bbs) + dy, max(b[2] for b in bbs) + dx,
+                                max(b[3] for b in bbs) + dy), size, self.region_size)]
         if isinstance(region, list) and not region:
             raise ValueError("region=[] is empty: give at least one PIL box")
         if isinstance(region, (list, tuple)) and all(isinstance(b, (list, tuple)) for b in region):   # a list of boxes
@@ -568,29 +653,18 @@ class DemoProcessor:
                 raise ValueError("a region edit needs the %s at the photo's size %dx%d (got %dx%d)" % ((nm, w, h) + m.size))
             if self.resize == "device" and m is not None and m.mode != "L":
                 raise ValueError("resize='device' takes an 'L' %s (got mode %r); resize='host' resizes it with Pillow" % (nm, m.mode))
-        boxes = self._region_boxes(img, mask, edit_mask, region)
-        Hn, Wn = self.region_size
-        sizes = [(b[2] - b[0], b[3] - b[1]) for b in boxes]
-        # region requests on edit masks run their own forward, and region requests never share one with whole-photo requests
-        key = ("region", Hn, Wn) if edit_mask is None else ("region", Hn, Wn, True)
-        out = img.copy()
+        boxes = self._region_boxes(img.size, mask, edit_mask, region)
         if self.resize == "device":
+            out = img.copy()
             crops = [np.asarray(img.crop(b)) for b in boxes]
             sketches = [np.asarray(mask.crop(b)) for b in boxes]
             edits = [np.asarray(edit_mask.crop(b)) for b in boxes] if edit_mask is not None else None
-            got = self.batcher.submit(key, (crops, sketches, edits, return_mask, boxes))
+            got = self.batcher.submit(self._region_key(edit_mask), (crops, sketches, edits, return_mask, boxes, None))
             for b, (patch, _) in zip(boxes, got):        # in order: a later patch holds the final bytes where boxes overlap
                 out.paste(Image.fromarray(patch), b[:2])
             mks = [Image.fromarray(mk) if mk is not None else None for _, mk in got]
         else:
-            img_t = np.stack([np.array(img.crop(b).resize((Wn, Hn))) for b in boxes]).astype(np.uint8)
-            mask_t = np.stack([(np.array(mask.crop(b).resize((Wn, Hn))) > 0).astype(np.uint8) * 255 for b in boxes])
-            edit_t = np.stack([np.array(edit_mask.convert("L").crop(b).resize((Wn, Hn))) for b in boxes]).astype(np.uint8) \
-                if edit_mask is not None else None
-            res, mk = self.batcher.submit(key, (img_t, mask_t, edit_t, True))
-            mks = [Image.fromarray(edit_t[i] if edit_t is not None else mk[i]).resize(s) for i, s in enumerate(sizes)]
-            for i, (b, s) in enumerate(zip(boxes, sizes)):   # every crop above came from the photo, not from `out`
-                out.paste(Image.fromarray(res[i]).resize(s), b, mks[i])
+            out, mks = self._region_host(img, mask, edit_mask, boxes)
         if not return_mask:
             return out
         if edit_mask is not None:
@@ -600,3 +674,191 @@ class DemoProcessor:
             sub = full[b[1]:b[3], b[0]:b[2]]
             np.maximum(sub, np.asarray(mk), out=sub)
         return out, Image.fromarray(full)
+
+    def _region_key(self, edit_mask):
+        # region requests on edit masks run their own forward, and region requests never share one with whole-photo requests
+        Hn, Wn = self.region_size
+        return ("region", Hn, Wn) if edit_mask is None else ("region", Hn, Wn, True)
+
+    def _region_host(self, img, mask, edit_mask, boxes):
+        """The Pillow flow of a region edit: ``(out, paste masks)``, one 'L' paste mask per box at the box's size."""
+        from PIL import Image
+        Hn, Wn = self.region_size
+        sizes = [(b[2] - b[0], b[3] - b[1]) for b in boxes]
+        out = img.copy()
+        img_t = np.stack([np.array(img.crop(b).resize((Wn, Hn))) for b in boxes]).astype(np.uint8)
+        mask_t = np.stack([(np.array(mask.crop(b).resize((Wn, Hn))) > 0).astype(np.uint8) * 255 for b in boxes])
+        edit_t = np.stack([np.array(edit_mask.convert("L").crop(b).resize((Wn, Hn))) for b in boxes]).astype(np.uint8) \
+            if edit_mask is not None else None
+        res, mk = self.batcher.submit(self._region_key(edit_mask), (img_t, mask_t, edit_t, True))
+        mks = [Image.fromarray(edit_t[i] if edit_t is not None else mk[i]).resize(s) for i, s in enumerate(sizes)]
+        for i, (b, s) in enumerate(zip(boxes, sizes)):   # every crop above came from the photo, not from `out`
+            out.paste(Image.fromarray(res[i]).resize(s), b, mks[i])
+        return out, mks
+
+
+EditResult = namedtuple("EditResult", ["boxes", "patches", "masks"])
+
+
+def _placed(m, size, offset):
+    """m as a PIL 'L' image of PIL size ``size``: placed at ``offset`` and zero elsewhere."""
+    if m is None or (m.size == tuple(size) and tuple(offset) == (0, 0)):
+        return m
+    from PIL import Image
+    full = Image.new("L", tuple(size), 0)
+    full.paste(m, tuple(offset))
+    return full
+
+
+class EditSession:
+    """A photo kept across a chain of edits, each drawn on the result of the one before, with undo
+    (``DemoProcessor.open_session``). ``edit(...)`` is
+
+        cur = proc.process_image(cur, mask, edit_mask, region=region)
+
+    with ``cur`` starting as the photo in RGB, and returns ``EditResult(boxes, patches, masks)``: the edit's PIL boxes in
+    paste order (``region=None``: the whole photo), ``patches[i] = cur.crop(boxes[i])`` after the edit, and ``masks[i]`` the
+    box's paste mask as an 'L' image when ``return_mask`` is set and the mask was predicted, else None. Outside the union of
+    the boxes ``cur`` keeps the previous photo's bytes.
+
+    ``mask`` and ``edit_mask`` are 'L' images of one size, placed at ``offset = (x, y)`` in the photo and zero elsewhere: the
+    boxes and bytes are those of the zero-padded photo-sized masks, without building them (``region=None`` takes photo-sized
+    masks at (0, 0)). ``undo()`` restores the photo from before the last edit not yet undone, exactly; its snapshots hold the
+    previous bytes of each edit's boxes and are dropped oldest first to keep within ``history_bytes``. Edits of one session run
+    one at a time; edits of several sessions share forwards with each other and with ``process_image`` requests of their
+    batch key.
+
+    With ``resize='device'`` the photo lives on the engine's device: an edit uploads only the masks' box crops, resizes the
+    photo's boxes where they lie (``engine.resize_window_u8_packed``), pastes the results into the photo and downloads only the
+    patches; undo snapshots stay on the device. With ``resize='host'`` the session holds a PIL image and runs the Pillow flow."""
+
+    def __init__(self, proc, img, history_bytes):
+        if int(history_bytes) < 0:
+            raise ValueError("history_bytes must be >= 0")
+        self._proc = proc
+        self._mu = threading.Lock()
+        self._history = deque()         # (boxes, previous bytes of each box, bytes held), oldest first
+        self._held = 0
+        self.history_bytes = int(history_bytes)
+        img = img.convert("RGB")
+        self.size = img.size
+        self._img = self._photo = None
+        if proc.resize == "host":
+            self._img = img
+        else:
+            torch = proc._torch
+            w, h = img.size
+            self._photo = torch.empty(h, w, 3, device=proc.engine.device, dtype=torch.uint8)
+            self._photo.copy_(torch.from_numpy(np.array(img)))
+        self._closed = False
+
+    def _check_open(self):
+        if self._closed:
+            raise RuntimeError("EditSession is closed")
+
+    def close(self):
+        """Releases the photo and the snapshots (idempotent); also run by ``DemoProcessor.close()``."""
+        with self._mu:
+            self._closed = True
+            self._img = self._photo = None
+            self._history.clear()
+            self._held = 0
+        with self._proc._sessions_mu:
+            self._proc._sessions.discard(self)
+
+    def image(self):
+        """The current photo as a PIL RGB image."""
+        from PIL import Image
+        with self._mu:
+            self._check_open()
+            if self._img is not None:
+                return self._img.copy()
+            with self._proc._torch.cuda.device(self._photo.device):
+                return Image.fromarray(self._photo.cpu().numpy())
+
+    def _boxes(self, mask, edit_mask, region, offset):
+        w, h = self.size
+        for m, nm in ((mask, "mask"), (edit_mask, "edit_mask")):
+            if m is not None and m.mode != "L":
+                raise ValueError("an EditSession takes an 'L' %s (got mode %r)" % (nm, m.mode))
+        if edit_mask is not None and edit_mask.size != mask.size:
+            raise ValueError("edit_mask is %dx%d, mask %dx%d: they must have one size" % (edit_mask.size + mask.size))
+        if not (isinstance(offset, (tuple, list)) and len(offset) == 2 and all(isinstance(v, (int, np.integer)) for v in offset)):
+            raise ValueError("offset must be (x, y) of integers, got %r" % (offset,))
+        ox, oy = (int(v) for v in offset)
+        if region is None:
+            if (ox, oy) != (0, 0) or mask.size != (w, h):
+                raise ValueError("region=None needs the mask at the photo's size %dx%d and offset (0, 0)" % (w, h))
+            if floor8(h) < 16 or floor8(w) < 16:
+                raise ValueError("image smaller than 16x16 (two stride-2 convolutions, 4x4 mask pool, stride-2 patch grid)")
+            return [(0, 0, w, h)]
+        mw, mh = mask.size
+        if not (0 <= ox and 0 <= oy and ox + mw <= w and oy + mh <= h):
+            raise ValueError("a %dx%d mask at offset (%d, %d) does not fit the %dx%d photo" % (mw, mh, ox, oy, w, h))
+        return self._proc._region_boxes(self.size, mask, edit_mask, region, (ox, oy))
+
+    def edit(self, mask, edit_mask=None, region="auto", return_mask=False, offset=(0, 0)):
+        """One edit of the current photo; see the class. Returns ``EditResult(boxes, patches, masks)``."""
+        from PIL import Image
+        with self._mu:
+            self._check_open()
+            boxes = self._boxes(mask, edit_mask, region, offset)
+            proc, off = self._proc, tuple(int(v) for v in offset)
+            if self._img is not None:
+                fm, fe = _placed(mask, self.size, off), _placed(edit_mask, self.size, off)
+                prev = [self._img.crop(b) for b in boxes]
+                if region is None:
+                    out, mk = proc.process_image(self._img, fm, fe, return_mask=True)
+                    mks = [mk]
+                else:
+                    out, mks = proc._region_host(self._img, fm, fe, boxes)
+                self._img = out
+                patches = [out.crop(b) for b in boxes]
+            else:
+                if region is None:
+                    w, h = self.size
+                    key = (floor8(h), floor8(w)) if edit_mask is None else (floor8(h), floor8(w), True)
+                    edit_raw = np.asarray(edit_mask) if edit_mask is not None else None
+                    patch, mk, prev = proc.batcher.submit(key, (None, np.asarray(mask), edit_raw, return_mask, self._photo))
+                    got = [(patch, mk)]
+                else:
+                    at = [(b[0] - off[0], b[1] - off[1], b[2] - off[0], b[3] - off[1]) for b in boxes]   # mask coordinates
+                    sketches = [np.asarray(mask.crop(b)) for b in at]
+                    edits = [np.asarray(edit_mask.crop(b)) for b in at] if edit_mask is not None else None
+                    got, prev = proc.batcher.submit(proc._region_key(edit_mask),
+                                                    (None, sketches, edits, return_mask, boxes, self._photo))
+                patches = [Image.fromarray(p) for p, _ in got]
+                mks = [Image.fromarray(m) if m is not None else None for _, m in got]
+            masks = [m if return_mask and edit_mask is None else None for m in mks]
+            nbytes = sum((b[2] - b[0]) * (b[3] - b[1]) * 3 for b in boxes)
+            self._history.append((boxes, prev, nbytes))
+            self._held += nbytes
+            while self._history and self._held > self.history_bytes:
+                self._held -= self._history.popleft()[2]
+            return EditResult(boxes, patches, masks)
+
+    def undo(self):
+        """Restores the photo from before the last edit not yet undone. Returns ``(boxes, patches)``: that edit's boxes and the
+        restored photo's bytes in them. Raises RuntimeError when no snapshot is left."""
+        from PIL import Image
+        with self._mu:
+            self._check_open()
+            if not self._history:
+                raise RuntimeError("nothing to undo: no snapshot is left")
+            boxes, prev, nbytes = self._history.pop()
+            self._held -= nbytes
+            if self._img is not None:
+                for b, crop in reversed(list(zip(boxes, prev))):
+                    self._img.paste(crop, b[:2])
+                return boxes, [self._img.crop(b) for b in boxes]
+            torch, photo = self._proc._torch, self._photo
+            with torch.cuda.device(photo.device):
+                for (left, upper, right, lower), t in reversed(list(zip(boxes, prev))):
+                    photo[upper:lower, left:right].copy_(t.view(lower - upper, right - left, 3))
+                down = torch.cat([photo[b[1]:b[3], b[0]:b[2]].reshape(-1) for b in boxes]).cpu().numpy()
+            patches, pos = [], 0
+            for left, upper, right, lower in boxes:
+                n = (lower - upper) * (right - left) * 3
+                patches.append(Image.fromarray(down[pos:pos + n].reshape(lower - upper, right - left, 3)))
+                pos += n
+            return boxes, patches
