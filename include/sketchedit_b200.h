@@ -186,6 +186,25 @@ int se_resize_composite_u8(const unsigned char* rgb, const long long* rgb_off, c
                            const int* src_hw, unsigned char* canvas, const long long* canvas_off, const long long* canvas_pitch,
                            const int* box_yx, const int* dst_hw, int n, int swap_rb, void* scratch, long long* scratch_bytes,
                            void* stream);
+/* se_resize_composite_u8 with each box's paste mask faded to 0 along chosen sides (a region edit's box edges inside the photo,
+ * so the paste shows no seam there). feather holds 4n ints, box i's widths (left, top, right, bottom) in box pixels, each in
+ * [0, the side's length: w for left and right, h for top and bottom]. Box i's resized mask m (h x w) becomes, before the blend,
+ *     m' = DIV255(m * r(y, x)),   r = min(ramp(x, left), ramp(w - 1 - x, right), ramp(y, top), ramp(h - 1 - y, bottom)),
+ *     ramp(d, f) = d >= f ? 255 : (255 * (d + 1)) / (f + 1)   (integer division; d = 0 on the side's edge pixel),
+ * with (y, x) the pixel's place in the box and DIV255 the blend's. A side of width 0 keeps m; DIV255(255 * m) == m, so widths
+ * of 0 give se_resize_composite_u8's bytes, and a box whose four widths are 0 runs its arithmetic unchanged. feather == NULL:
+ * no feathering (se_resize_composite_u8 is this call with NULL). Everything else, the checks, the scratch query and the
+ * coefficient-table cache included, is se_resize_composite_u8's. */
+int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask,
+                                   const long long* mask_off, const int* src_hw, unsigned char* canvas, const long long* canvas_off,
+                                   const long long* canvas_pitch, const int* box_yx, const int* dst_hw, const int* feather, int n,
+                                   int swap_rb, void* scratch, long long* scratch_bytes, void* stream);
+/* The feather of se_resize_composite_feather_u8 on masks alone, in place: image i is the hw[2i] x hw[2i+1] 'L' bytes (rows
+ * packed) at img + off[i], and each of its bytes m becomes DIV255(m * r(y, x)) with the ramp r of its widths feather[4i .. 4i+3]
+ * (left, top, right, bottom; each in [0, the side's length]). Sizes are in [1, 65535]; an image with four widths of 0 is not
+ * touched. For a predicted mask resized back to its box this gives the mask the feathered paste used. Only enqueues the
+ * kernel on `stream`. */
+int se_feather_u8(unsigned char* img, const long long* off, const int* hw, const int* feather, int n, void* stream);
 /* Bytes of coefficient tables se_resize_u8 keeps per device (process-wide; 0 restores the default of 256 MiB; negative is an
  * error). When a call's new tables would pass the limit, the device's cache is emptied (after a device synchronise) before the
  * call looks up any table; one call's own tables may exceed it. */

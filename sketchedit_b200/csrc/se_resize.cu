@@ -9,7 +9,8 @@
 // Pillow computes only the intermediate rows the vertical pass reads; computing all of them gives the same values.
 // se_resize_paste_u8 resizes a result and its mask the same way and pastes the result over a base image with Pillow's
 // Image.paste(im, box, mask) blend, fused into the vertical pass (paste_v_kernel); se_resize_composite_u8 pastes boxes that
-// may overlap into shared canvases in order, as sequential Image.paste calls do, with the same kernel. se_resize_window_u8
+// may overlap into shared canvases in order, as sequential Image.paste calls do, with the same kernel, and
+// se_resize_composite_feather_u8 fades each box's mask to 0 along the box edges it is given widths for. se_resize_window_u8
 // resizes windows of larger images (rows a pitch apart, such as boxes of a photo kept on the device) with the kernels of
 // se_resize_u8: Image.crop(box).resize(size) without the crop.
 #include <limits.h>
@@ -304,6 +305,8 @@ __global__ void __launch_bounds__(V_TX * V_TY) resize_v_kernel(const __grid_cons
 // box, the vertical pass of its result (3 channels) and of its mask, both in_h x out_w, to out_h, then Pillow's Image.paste
 // blend of the result over the canvas with that mask, per channel:
 //     dst = DIV255(base * (255 - m) + res * m),   DIV255(a) = ((t >> 8) + t) >> 8 with t = a + 128 (libImaging/Paste.c).
+// A box with feather widths (se_resize_composite_feather_u8) first takes m = DIV255(m * ramp) with the ramp of feather_pair
+// at the pixel's place in the box; a box without them skips that step.
 // A thread owns 4 pixels of one canvas row (x a multiple of 4). It reads the canvas bytes that some box of the launch covers,
 // blends every covering box over them in the launch's order and writes them once; uncovered bytes are never touched. It reads
 // before it writes the same bytes, so dst may be base. The 12 canvas bytes move as 32-bit words when every box that covers
@@ -313,8 +316,11 @@ struct PBox {   // a box at (oy, ox) of its canvas; rgb and mask are in_h x out_
   const unsigned char* mask;
   const int* bounds;   // the vertical table; nullptr: the height does not change (one tap of weight 1 at the same row)
   const int* coeffs;
-  int ksize, out_h, out_w, oy, ox, vec;
+  int oy, ox;
+  unsigned short out_h, out_w, ksize, vec;   // sizes <= 65535 (check_image); ksize <= 9685 (its shared-memory check)
+  unsigned short feather[4];                 // ramp widths of the left, top, right, bottom sides; all 0: no ramp
 };
+static_assert(sizeof(PBox) == 56, "the feather widths fit PBox's former padding");
 struct PCanvas {   // boxes box0 .. box0 + nbox - 1 of the launch, in order; tiles cover rows y0 .. y0 + h - 1 from column x0
   const unsigned char* base;
   unsigned char* dst;
@@ -382,6 +388,16 @@ __global__ void __launch_bounds__(V_TX * V_TY) paste_v_kernel(const __grid_const
     int v[V_GROUP], m[P_PIX];
     v_taps(b.rgb + col * 3, b.out_w * 3, k, n, lo * 3, hi * 3, bv, v);
     v_taps(b.mask + col, b.out_w, k, n, lo, hi, bv, m);
+    if (b.feather[0] | b.feather[1] | b.feather[2] | b.feather[3]) {
+      const int rv = feather_pair(r, b.out_h - 1 - r, b.feather[1], b.feather[3]);
+#pragma unroll
+      for (int p = 0; p < P_PIX; ++p) {
+        if (p < lo || p >= hi) continue;
+        const int xb = x + p - b.ox;
+        const int ramp = min(rv, feather_pair(xb, b.out_w - 1 - xb, b.feather[0], b.feather[2]));
+        if (ramp < 255) m[p] = div255(m[p] * ramp);
+      }
+    }
     if (swap) swap_rb12(v);
 #pragma unroll
     for (int j = 0; j < V_GROUP; ++j) {
@@ -548,6 +564,7 @@ struct PasteBox {
   const unsigned char* rgb;
   const unsigned char* mask;
   int ih, iw, oh, ow, canvas, oy, ox;
+  int feather[4];   // left, top, right, bottom; zero unless se_resize_composite_feather_u8 gives them
 };
 struct PasteCanvas {
   const unsigned char* base;
@@ -607,13 +624,16 @@ static int paste_boxes(const std::vector<PasteBox>& boxes, const std::vector<Pas
         p.rgb = s3;
         p.mask = s1;
       }
-      int rc = v_table(dev, b.ih, b.oh, &p.bounds, &p.coeffs, &p.ksize);
+      int ksize = 1;
+      int rc = v_table(dev, b.ih, b.oh, &p.bounds, &p.coeffs, &ksize);
       if (rc) return rc;
-      p.out_h = b.oh;
-      p.out_w = b.ow;
+      p.ksize = (unsigned short)ksize;
+      p.out_h = (unsigned short)b.oh;
+      p.out_w = (unsigned short)b.ow;
       p.oy = b.oy;
       p.ox = b.ox;
       p.vec = b.ow % 4 == 0 && b.ox % 4 == 0 && ((uintptr_t)p.rgb | (uintptr_t)p.mask) % 4 == 0;
+      for (int s = 0; s < 4; ++s) p.feather[s] = (unsigned short)b.feather[s];
       if (j == 0 || boxes[order[j - 1]].canvas != b.canvas) {
         const PasteCanvas& cv = canvases[b.canvas];
         PCanvas& c = pl.p[pl.n++];
@@ -755,16 +775,16 @@ int se_resize_paste_u8(const unsigned char* rgb, const long long* rgb_off, const
   std::vector<PasteBox> boxes(n);   // image i: one box filling canvas i
   std::vector<PasteCanvas> canvases(n);
   for (int i = 0; i < n; ++i) {
-    boxes[i] = {rgb + rgb_off[i], mask + mask_off[i], src_hw[2 * i], src_hw[2 * i + 1], dst_hw[2 * i], dst_hw[2 * i + 1], i, 0, 0};
+    boxes[i] = {rgb + rgb_off[i], mask + mask_off[i], src_hw[2 * i], src_hw[2 * i + 1], dst_hw[2 * i], dst_hw[2 * i + 1], i, 0, 0, {}};
     canvases[i] = {base + base_off[i], dst + dst_off[i], 3LL * dst_hw[2 * i + 1]};
   }
   return paste_boxes(boxes, canvases, mid, scratch, swap_rb, (cudaStream_t)stream);
 }
 
-int se_resize_composite_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask, const long long* mask_off,
-                           const int* src_hw, unsigned char* canvas, const long long* canvas_off, const long long* canvas_pitch,
-                           const int* box_yx, const int* dst_hw, int n, int swap_rb, void* scratch, long long* scratch_bytes,
-                           void* stream) {
+int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask,
+                                   const long long* mask_off, const int* src_hw, unsigned char* canvas, const long long* canvas_off,
+                                   const long long* canvas_pitch, const int* box_yx, const int* dst_hw, const int* feather, int n,
+                                   int swap_rb, void* scratch, long long* scratch_bytes, void* stream) {
   SE_REQUIRE(n >= 0, "n must be >= 0 boxes");
   SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
   SE_REQUIRE(n == 0 || (rgb_off && mask_off && src_hw && canvas_off && canvas_pitch && box_yx && dst_hw), "null size / offset array");
@@ -784,7 +804,14 @@ int se_resize_composite_u8(const unsigned char* rgb, const long long* rgb_off, c
     auto it = canvas_of.emplace(canvas_off[i], (int)canvases.size()).first;
     if (it->second == (int)canvases.size()) canvases.push_back({canvas + canvas_off[i], canvas + canvas_off[i], canvas_pitch[i]});
     SE_REQUIRE(canvases[it->second].pitch == canvas_pitch[i], "box " + std::to_string(i) + ": boxes of one canvas must have one pitch");
-    boxes[i] = {rgb + rgb_off[i], mask + mask_off[i], ih, iw, oh, ow, it->second, box_yx[2 * i], box_yx[2 * i + 1]};
+    boxes[i] = {rgb + rgb_off[i], mask + mask_off[i], ih, iw, oh, ow, it->second, box_yx[2 * i], box_yx[2 * i + 1], {}};
+    if (feather) {
+      const int* f = feather + 4 * (size_t)i;
+      SE_REQUIRE(f[0] >= 0 && f[0] <= ow && f[2] >= 0 && f[2] <= ow && f[1] >= 0 && f[1] <= oh && f[3] >= 0 && f[3] <= oh,
+                 "box " + std::to_string(i) + ": feather widths (" + std::to_string(f[0]) + ", " + std::to_string(f[1]) + ", " +
+                     std::to_string(f[2]) + ", " + std::to_string(f[3]) + ") must be in [0, the side's length]");
+      for (int s = 0; s < 4; ++s) boxes[i].feather[s] = f[s];
+    }
     mid[i] = need;
     need += paste_scratch(ih, iw, ow);
   }
@@ -796,6 +823,14 @@ int se_resize_composite_u8(const unsigned char* rgb, const long long* rgb_off, c
   if (n == 0) return 0;
   SE_REQUIRE(rgb && mask && canvas, "null rgb / mask / canvas");
   return paste_boxes(boxes, canvases, mid, scratch, swap_rb, (cudaStream_t)stream);
+}
+
+int se_resize_composite_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask, const long long* mask_off,
+                           const int* src_hw, unsigned char* canvas, const long long* canvas_off, const long long* canvas_pitch,
+                           const int* box_yx, const int* dst_hw, int n, int swap_rb, void* scratch, long long* scratch_bytes,
+                           void* stream) {
+  return se_resize_composite_feather_u8(rgb, rgb_off, mask, mask_off, src_hw, canvas, canvas_off, canvas_pitch, box_yx, dst_hw,
+                                        nullptr, n, swap_rb, scratch, scratch_bytes, stream);
 }
 
 }  // extern "C"

@@ -461,7 +461,7 @@ def resize_paste_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, base
 
 
 def resize_composite_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, canvas, canvas_offsets, canvas_pitches,
-                               box_offsets, box_sizes, swap_rb=False):
+                               box_offsets, box_sizes, swap_rb=False, feather=None):
     """Resize back and paste boxes in order into canvases (``se_resize_composite_u8``), bit for bit as sequential Pillow
     pastes, in place:
 
@@ -472,13 +472,19 @@ def resize_composite_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, 
     (y, x)`` is its top-left pixel there and ``box_sizes[i] = (h, w)`` its size. Boxes with the same canvas offset share
     that canvas, so a later box blends over an earlier one where they overlap. ``swap_rb`` reverses the result's channel
     order first. All tensors are contiguous CUDA uint8 on one device; only the boxes' canvas pixels are read and written.
-    Returns ``canvas``. Only enqueues work on the current stream, except that the first resize between a pair of lengths
-    uploads its coefficient table."""
+    ``feather``: None, or per box its ramp widths ``(left, top, right, bottom)`` in box pixels
+    (``se_resize_composite_feather_u8``): the box's resized mask becomes ``DIV255(m * ramp)`` before the blend, with the ramp
+    of ``serving.feather_ramp``. Returns ``canvas``. Only enqueues work on the current stream, except that the first resize
+    between a pair of lengths uploads its coefficient table."""
     n = len(src_sizes)
     if not (len(rgb_offsets) == len(mask_offsets) == len(canvas_offsets) == len(canvas_pitches) == len(box_offsets)
             == len(box_sizes) == n):
         raise _lib.SketchEditB200Error("rgb_offsets, mask_offsets, src_sizes, canvas_offsets, canvas_pitches, box_offsets and "
                                        "box_sizes must have the same length")
+    if feather is not None:
+        feather = [tuple(int(v) for v in f) for f in feather]
+        if len(feather) != n or any(len(f) != 4 for f in feather):
+            raise _lib.SketchEditB200Error("feather needs 4 widths (left, top, right, bottom) per box")
     for t, nm in ((rgb, "rgb"), (mask, "mask"), (canvas, "canvas")):
         if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
             raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % nm)
@@ -502,16 +508,43 @@ def resize_composite_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, 
     L, I = ctypes.c_longlong, ctypes.c_int
     pairs = lambda v: (I * (2 * n))(*[a for hw in v for a in hw])
     args = ((L * n)(*[int(o) for o in rgb_offsets]), (L * n)(*[int(o) for o in mask_offsets]), pairs(src_sizes),
-            (L * n)(*canvas_offsets), (L * n)(*canvas_pitches), pairs(box_offsets), pairs(box_sizes), n)
+            (L * n)(*canvas_offsets), (L * n)(*canvas_pitches), pairs(box_offsets), pairs(box_sizes),
+            (I * (4 * n))(*[v for f in feather for v in f]) if feather is not None else None, n)
     with torch.cuda.device(rgb.device):
         need = L(0)
-        _lib.check(lib.se_resize_composite_u8(None, args[0], None, args[1], args[2], None, args[3], args[4], args[5], args[6], n,
-                                              int(bool(swap_rb)), None, ctypes.byref(need), None))
+        _lib.check(lib.se_resize_composite_feather_u8(None, args[0], None, args[1], args[2], None, args[3], args[4], args[5],
+                                                      args[6], args[7], n, int(bool(swap_rb)), None, ctypes.byref(need), None))
         scratch = torch.empty(max(1, need.value), device=rgb.device, dtype=torch.uint8)
         size = L(scratch.numel())
-        _lib.check(lib.se_resize_composite_u8(_ptr(rgb), args[0], _ptr(mask), args[1], args[2], _ptr(canvas), args[3], args[4],
-                                              args[5], args[6], n, int(bool(swap_rb)), _ptr(scratch), ctypes.byref(size), _stream()))
+        _lib.check(lib.se_resize_composite_feather_u8(_ptr(rgb), args[0], _ptr(mask), args[1], args[2], _ptr(canvas), args[3],
+                                                      args[4], args[5], args[6], args[7], n, int(bool(swap_rb)), _ptr(scratch),
+                                                      ctypes.byref(size), _stream()))
     return canvas
+
+
+def feather_u8_packed(buf, offsets, sizes, feather):
+    """The feather of ``resize_composite_u8_packed(..., feather=...)`` on 'L' images alone, in place (``se_feather_u8``):
+    image i is the ``sizes[i] = (h, w)`` bytes at byte ``offsets[i]`` of the contiguous CUDA uint8 tensor ``buf``, and each
+    byte m becomes ``DIV255(m * ramp)`` with the ramp of ``feather[i] = (left, top, right, bottom)``. Images whose four widths
+    are 0 are not touched. Returns ``buf``; only enqueues work on the current stream."""
+    n = len(sizes)
+    if len(offsets) != n or len(feather) != n:
+        raise _lib.SketchEditB200Error("offsets, sizes and feather must have the same length")
+    if not (isinstance(buf, torch.Tensor) and buf.is_cuda and buf.dtype == torch.uint8 and buf.is_contiguous()):
+        raise _lib.SketchEditB200Error("buf must be a contiguous CUDA uint8 tensor")
+    sizes = [(int(h), int(w)) for h, w in sizes]
+    offsets = [int(o) for o in offsets]
+    feather = [tuple(int(v) for v in f) for f in feather]
+    if any(len(f) != 4 for f in feather):
+        raise _lib.SketchEditB200Error("feather needs 4 widths (left, top, right, bottom) per image")
+    for o, (h, w) in zip(offsets, sizes):
+        if o < 0 or o + h * w > buf.numel():
+            raise _lib.SketchEditB200Error("image slice [%d, %d) outside the %d-byte buffer" % (o, o + h * w, buf.numel()))
+    L, I = ctypes.c_longlong, ctypes.c_int
+    with torch.cuda.device(buf.device):
+        _lib.check(_lib.load().se_feather_u8(_ptr(buf), (L * max(n, 1))(*offsets), (I * max(2 * n, 1))(*[v for hw in sizes for v in hw]),
+                                             (I * max(4 * n, 1))(*[v for f in feather for v in f]), n, _stream()))
+    return buf
 
 
 def set_resize_table_cache_limit(nbytes):

@@ -13,14 +13,16 @@ too (``engine.resize_u8_packed``, bit-identical to Pillow), so a batch is one up
     result_pil = proc.process_image(image_pil, mask_pil, edit_mask=corrected_mask)      # run on a revised edit mask
     result_pil = proc.process_image(image_pil, mask_pil, region="auto")                 # edit a crop around the strokes only
     result_pil = proc.process_image(image_pil, mask_pil, region="strokes")              # one crop per group of strokes
+    result_pil = proc.process_image(image_pil, mask_pil, region="auto", feather=16)     # paste fading over 16 px at inner edges
     s = proc.open_session(image_pil)                  # the photo stays on the device across edits
     r = s.edit(mask_pil, region="strokes")            # r.boxes, r.patches: what changed; s.undo() restores it
     proc.close()
 
 A region edit (``region=``) crops a box of the photo, runs the forward on it at ``DemoProcessor(region_size=...)`` and pastes
 the result back with the edit mask: its cost follows the box, not the photo, and region requests on photos of any size
-batch together. A request may carry several boxes (``region="strokes"`` or a list), pasted in order. An ``EditSession`` keeps one photo on
-the device for a chain of edits, each drawn on the previous result, with undo.
+batch together. A request may carry several boxes (``region="strokes"`` or a list), pasted in order. ``feather=F`` fades each
+box's paste mask to 0 along the box edges that lie inside the photo (``feather_widths``, ``feather_ramp``), so the paste shows no
+seam there. An ``EditSession`` keeps one photo on the device for a chain of edits, each drawn on the previous result, with undo.
 
 Everything except the forward itself (``run_batch``) is plain host logic and is unit-tested on the CPU with a fake forward.
 """
@@ -253,6 +255,48 @@ def region_groups(mask, edit_mask=None, region_size=(256, 256), photo_size=None,
     return sorted(zip(groups, boxes), key=lambda gb: (gb[0][1], gb[0][0]))
 
 
+def _check_feather(feather):
+    if isinstance(feather, bool) or not isinstance(feather, (int, np.integer)) or feather < 0:
+        raise ValueError("feather must be an int >= 0 (photo pixels), got %r" % (feather,))
+    return int(feather)
+
+
+def feather_widths(box, photo_size, feather):
+    """The feather widths ``(left, top, right, bottom)`` of a region edit's PIL box ``(left, upper, right, lower)`` in a photo
+    of PIL size ``(w, h)``: a side on the photo's border gets 0 (it stays hard), any other ``min(feather, bw // 4)`` (left,
+    right) or ``min(feather, bh // 4)`` (top, bottom) for a ``bw x bh`` box. The quarter cap keeps the band off the strokes of
+    an 'auto' or 'strokes' box: ``region_box`` centres strokes that span at most half of each side, and it only shifts a box
+    towards a photo border, whose side is not feathered."""
+    left, upper, right, lower = (int(v) for v in box)
+    w, h = (int(v) for v in photo_size)
+    fx, fy = min(int(feather), (right - left) // 4), min(int(feather), (lower - upper) // 4)
+    return (0 if left == 0 else fx, 0 if upper == 0 else fy, 0 if right == w else fx, 0 if lower == h else fy)
+
+
+def feather_ramp(size, widths):
+    """The feather ramp [h, w] uint8 of a box of PIL size ``(w, h)`` with ``widths = (left, top, right, bottom)``: a side of
+    width f gives the pixel at distance d from its edge pixel (d = 0 on it) ``255 if d >= f else (255 * (d + 1)) // (f + 1)``,
+    and a pixel takes the least over the four sides. The pasted mask is ``feather_mask(m, widths) = DIV255(m * ramp)``, with
+    Pillow's blend rounding ``DIV255(a) = (((a + 128) >> 8) + a + 128) >> 8``; widths of 0 leave m unchanged."""
+    w, h = (int(v) for v in size)
+    fl, ft, fr, fb = (int(v) for v in widths)
+
+    def side(d, f):
+        return np.where(d >= f, 255, (255 * (d + 1)) // (f + 1))
+
+    x, y = np.arange(w), np.arange(h)
+    rx = np.minimum(side(x, fl), side(w - 1 - x, fr))
+    ry = np.minimum(side(y, ft), side(h - 1 - y, fb))
+    return np.minimum(ry[:, None], rx[None, :]).astype(np.uint8)
+
+
+def feather_mask(m, widths):
+    """``DIV255(m * feather_ramp)`` of an [h, w] uint8 mask (see ``feather_ramp``)."""
+    m = np.asarray(m)
+    a = m.astype(np.int32) * feather_ramp(m.shape[::-1], widths) + 128
+    return (((a >> 8) + a) >> 8).astype(np.uint8)
+
+
 def _check_box(box, w, h):
     if not (isinstance(box, (tuple, list)) and len(box) == 4 and all(isinstance(v, (int, np.integer)) for v in box)):
         raise ValueError("region must be None, 'auto', 'strokes', a PIL box (left, upper, right, lower) of integers or a list of "
@@ -425,13 +469,15 @@ class DemoProcessor:
 
     def _run_region_device(self, key, payloads):
         """payloads: (photo crops [bh,bw,3] or None, sketch crops [bh,bw], edit-mask crops [bh,bw] or None, return_mask, boxes,
-        session photo or None): one crop per PIL box of the request, at its box size; key: ("region", Hn, Wn), plus True when
-        the batch runs on edit masks. Returns per request one (patch, mask) per box: patch [bh,bw,3] is the box's bytes once all
-        of the request's boxes are pasted in order, mask the box's paste mask resized back to [bh,bw] when asked for and
-        predicted, else None. A session's request has no photo crops: its boxes are resized from its photo ([h,w,3] on the
-        device), snapshotted and pasted into it, and its result is (that list, [previous bytes of each box])."""
+        session photo or None, feather, photo PIL size): one crop per PIL box of the request, at its box size; key: ("region",
+        Hn, Wn), plus True when the batch runs on edit masks. Returns per request one (patch, mask) per box: patch [bh,bw,3] is
+        the box's bytes once all of the request's boxes are pasted in order, mask the box's paste mask resized back to [bh,bw]
+        (feathered as pasted) when asked for and predicted, else None. A box's feather widths follow from its place in the
+        photo (``feather_widths``), wherever it is pasted. A session's request has no photo crops: its boxes are resized from
+        its photo ([h,w,3] on the device), snapshotted and pasted into it, and its result is (that list, [previous bytes of
+        each box])."""
         torch = self._torch
-        from .engine import resize_composite_u8_packed, resize_u8_packed, resize_window_u8_packed
+        from .engine import feather_u8_packed, resize_composite_u8_packed, resize_u8_packed, resize_window_u8_packed
         H, W = key[1:3]
         edit = key[-1] is True
         dev = self.engine.device
@@ -445,6 +491,7 @@ class DemoProcessor:
         masks = [payloads[r][1][j] for r, j in items]
         edits = [payloads[r][2][j] for r, j in items] if edit else []
         back = [i for i, (r, _) in enumerate(items) if payloads[r][3] and not edit]   # predicted masks to return
+        fw = [feather_widths(boxes[i], payloads[r][7], payloads[r][6]) for i, (r, _) in enumerate(items)]
         # The work buffer: the plain requests' photo crops (uploaded; a box that overlaps no other box of its request is pasted
         # in place over its crop), the session boxes' patches, the predicted masks resized back (these three are the one
         # download), then the sketch and edit-mask crops (uploaded), then the canvases. A set of overlapping boxes of a plain
@@ -530,7 +577,8 @@ class DemoProcessor:
                         target = sess[g[0]].view(-1)
                     resize_composite_u8_packed(bgr, [net3[i] for i in g], pm, [net1[i] for i in g], [(H, W)] * len(g), target,
                                                [c[0] for c in place], [c[1] for c in place], [c[2:] for c in place],
-                                               [sizes[i] for i in g], swap_rb=True)
+                                               [sizes[i] for i in g], swap_rb=True,
+                                               feather=[fw[i] for i in g] if any(any(fw[i]) for i in g) else None)
                 for i in canvas:
                     src, crop = in_canvas(work, i)
                     crop.copy_(src)
@@ -539,6 +587,9 @@ class DemoProcessor:
                 if back:
                     resize_u8_packed(pm, [net1[i] for i in back], [(H, W)] * len(back), [sizes[i] for i in back], 1, out=work,
                                      dst_offsets=[mask_at[i] for i in back])
+                    fb = [i for i in back if any(fw[i])]
+                    if fb:                            # the masks as pasted
+                        feather_u8_packed(work, [mask_at[i] for i in fb], [sizes[i] for i in fb], [fw[i] for i in fb])
                 down[:n_down].copy_(work[:n_down], non_blocking=True)
             finally:
                 torch.cuda.current_stream().synchronize()
@@ -575,7 +626,7 @@ class DemoProcessor:
                     for e, p in zip(ends, payloads)]
         return [(np.ascontiguousarray(rgb[i]), mk[i] if mk is not None and p[3] else None) for i, p in enumerate(payloads)]
 
-    def process_image(self, img, mask, edit_mask=None, return_mask=False, region=None):
+    def process_image(self, img, mask, edit_mask=None, return_mask=False, region=None, feather=0):
         """img: PIL image; mask: PIL 'L' image, usually of the same size (non-zero = sketch stroke). Returns the edited PIL
         image at the input's size. Sizes are floored to a multiple of 8 for the network exactly like demo.py:43.
 
@@ -594,11 +645,18 @@ class DemoProcessor:
         A list of PIL boxes, or 'strokes' for one box per stroke group (``region_groups``), edits several regions in one
         forward. Every crop is taken from the photo itself and the results are pasted in the list's order, exactly as
         ``out = img.copy()`` followed by the single-box paste of each box into ``out``; a later box blends over an earlier one
-        where they overlap. The returned predicted mask is then the largest of the boxes' paste masks at each pixel."""
+        where they overlap. The returned predicted mask is then the largest of the boxes' paste masks at each pixel.
+
+        feather: an int >= 0 (photo pixels, default 0). A region edit pastes each box with ``feather_mask(m, widths)`` in place
+        of its paste mask m, ``widths = feather_widths(box, img.size, feather)``: the mask fades to 0 over a band along the box
+        edges inside the photo, while edges on the photo's border stay hard. A predicted mask is returned as pasted (feathered);
+        a given edit_mask is returned as given. 0 pastes exactly as without it. It does not change the forward, so requests
+        with different values share forwards. region=None has no inner edges: feather is checked and has no effect."""
         from PIL import Image
+        feather = _check_feather(feather)
         img = img.convert("RGB")
         if region is not None:
-            return self._process_region(img, mask, edit_mask, return_mask, region)
+            return self._process_region(img, mask, edit_mask, return_mask, region, feather)
         w_raw, h_raw = img.size
         h_t, w_t = floor8(h_raw), floor8(w_raw)
         if h_t < 16 or w_t < 16:
@@ -645,7 +703,7 @@ class DemoProcessor:
             return [_check_box(b, w, h) for b in region]
         return [_check_box(region, w, h)]
 
-    def _process_region(self, img, mask, edit_mask, return_mask, region):
+    def _process_region(self, img, mask, edit_mask, return_mask, region, feather=0):
         from PIL import Image
         w, h = img.size
         for m, nm in ((mask, "mask"), (edit_mask, "edit_mask")):
@@ -659,12 +717,13 @@ class DemoProcessor:
             crops = [np.asarray(img.crop(b)) for b in boxes]
             sketches = [np.asarray(mask.crop(b)) for b in boxes]
             edits = [np.asarray(edit_mask.crop(b)) for b in boxes] if edit_mask is not None else None
-            got = self.batcher.submit(self._region_key(edit_mask), (crops, sketches, edits, return_mask, boxes, None))
+            got = self.batcher.submit(self._region_key(edit_mask),
+                                      (crops, sketches, edits, return_mask, boxes, None, feather, img.size))
             for b, (patch, _) in zip(boxes, got):        # in order: a later patch holds the final bytes where boxes overlap
                 out.paste(Image.fromarray(patch), b[:2])
             mks = [Image.fromarray(mk) if mk is not None else None for _, mk in got]
         else:
-            out, mks = self._region_host(img, mask, edit_mask, boxes)
+            out, mks = self._region_host(img, mask, edit_mask, boxes, feather)
         if not return_mask:
             return out
         if edit_mask is not None:
@@ -680,8 +739,9 @@ class DemoProcessor:
         Hn, Wn = self.region_size
         return ("region", Hn, Wn) if edit_mask is None else ("region", Hn, Wn, True)
 
-    def _region_host(self, img, mask, edit_mask, boxes):
-        """The Pillow flow of a region edit: ``(out, paste masks)``, one 'L' paste mask per box at the box's size."""
+    def _region_host(self, img, mask, edit_mask, boxes, feather=0):
+        """The Pillow flow of a region edit: ``(out, paste masks)``, one 'L' paste mask per box at the box's size (feathered
+        with ``feather_widths(box, img.size, feather)``)."""
         from PIL import Image
         Hn, Wn = self.region_size
         sizes = [(b[2] - b[0], b[3] - b[1]) for b in boxes]
@@ -692,6 +752,8 @@ class DemoProcessor:
             if edit_mask is not None else None
         res, mk = self.batcher.submit(self._region_key(edit_mask), (img_t, mask_t, edit_t, True))
         mks = [Image.fromarray(edit_t[i] if edit_t is not None else mk[i]).resize(s) for i, s in enumerate(sizes)]
+        if feather:
+            mks = [Image.fromarray(feather_mask(m, feather_widths(b, img.size, feather))) for m, b in zip(mks, boxes)]
         for i, (b, s) in enumerate(zip(boxes, sizes)):   # every crop above came from the photo, not from `out`
             out.paste(Image.fromarray(res[i]).resize(s), b, mks[i])
         return out, mks
@@ -714,11 +776,11 @@ class EditSession:
     """A photo kept across a chain of edits, each drawn on the result of the one before, with undo
     (``DemoProcessor.open_session``). ``edit(...)`` is
 
-        cur = proc.process_image(cur, mask, edit_mask, region=region)
+        cur = proc.process_image(cur, mask, edit_mask, region=region, feather=feather)
 
     with ``cur`` starting as the photo in RGB, and returns ``EditResult(boxes, patches, masks)``: the edit's PIL boxes in
     paste order (``region=None``: the whole photo), ``patches[i] = cur.crop(boxes[i])`` after the edit, and ``masks[i]`` the
-    box's paste mask as an 'L' image when ``return_mask`` is set and the mask was predicted, else None. Outside the union of
+    box's paste mask (feathered as pasted) as an 'L' image when ``return_mask`` is set and the mask was predicted, else None. Outside the union of
     the boxes ``cur`` keeps the previous photo's bytes.
 
     ``mask`` and ``edit_mask`` are 'L' images of one size, placed at ``offset = (x, y)`` in the photo and zero elsewhere: the
@@ -797,9 +859,10 @@ class EditSession:
             raise ValueError("a %dx%d mask at offset (%d, %d) does not fit the %dx%d photo" % (mw, mh, ox, oy, w, h))
         return self._proc._region_boxes(self.size, mask, edit_mask, region, (ox, oy))
 
-    def edit(self, mask, edit_mask=None, region="auto", return_mask=False, offset=(0, 0)):
+    def edit(self, mask, edit_mask=None, region="auto", return_mask=False, offset=(0, 0), feather=0):
         """One edit of the current photo; see the class. Returns ``EditResult(boxes, patches, masks)``."""
         from PIL import Image
+        feather = _check_feather(feather)
         with self._mu:
             self._check_open()
             boxes = self._boxes(mask, edit_mask, region, offset)
@@ -811,7 +874,7 @@ class EditSession:
                     out, mk = proc.process_image(self._img, fm, fe, return_mask=True)
                     mks = [mk]
                 else:
-                    out, mks = proc._region_host(self._img, fm, fe, boxes)
+                    out, mks = proc._region_host(self._img, fm, fe, boxes, feather)
                 self._img = out
                 patches = [out.crop(b) for b in boxes]
             else:
@@ -826,7 +889,7 @@ class EditSession:
                     sketches = [np.asarray(mask.crop(b)) for b in at]
                     edits = [np.asarray(edit_mask.crop(b)) for b in at] if edit_mask is not None else None
                     got, prev = proc.batcher.submit(proc._region_key(edit_mask),
-                                                    (None, sketches, edits, return_mask, boxes, self._photo))
+                                                    (None, sketches, edits, return_mask, boxes, self._photo, feather, self.size))
                 patches = [Image.fromarray(p) for p, _ in got]
                 mks = [Image.fromarray(m) if m is not None else None for _, m in got]
             masks = [m if return_mask and edit_mask is None else None for m in mks]
