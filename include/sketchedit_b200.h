@@ -205,6 +205,22 @@ int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rg
  * touched. For a predicted mask resized back to its box this gives the mask the feathered paste used. Only enqueues the
  * kernel on `stream`. */
 int se_feather_u8(unsigned char* img, const long long* off, const int* hw, const int* feather, int n, void* stream);
+/* Baseline JPEG of n in [0, 32] RGB windows, byte for byte what Pillow writes for an RGB image without info:
+ *     buf = io.BytesIO();  Image.fromarray(img_i).save(buf, "JPEG", quality=quality, subsampling=subsampling)
+ * quality in [1, 100]; subsampling 0 (4:4:4) or 2 (4:2:0, Pillow's default with quality 75). Image i is hw[2i] rows of
+ * hw[2i+1] RGB pixels (sizes in [1, 65535]), its row r at src[i] + r * src_pitch[i] (bytes, >= 3 * hw[2i+1]); src is a host
+ * array of n device pointers, and windows may overlap each other. The file (SOI, JFIF APP0, two DQT, SOF0, four DHT with the
+ * Annex K tables, SOS, the entropy-coded data, EOI) goes to out + out_off[i], which must hold se_jpeg_max_bytes(h, w,
+ * subsampling) bytes; only its first out_bytes_dev[i] bytes are written, and that count is stored in the device array
+ * out_bytes_dev[i]. No out slice may overlap another or a window. scratch == NULL stores the scratch bytes the call needs in
+ * *scratch_bytes (src, out and out_bytes_dev may be NULL then). Every argument is checked before anything is enqueued on
+ * `stream`; the call only enqueues. */
+int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality, int subsampling,
+                      unsigned char* out, const long long* out_off, long long* out_bytes_dev, void* scratch, long long* scratch_bytes,
+                      void* stream);
+/* Host only: a true upper bound of the file se_jpeg_encode_u8 writes for an h x w image: the 623-byte header, 208 bytes per
+ * 8x8 block (64 codes of at most 26 bits) doubled for the 0x00 after each 0xFF, and EOI. -1 on bad arguments. */
+long long se_jpeg_max_bytes(int h, int w, int subsampling);
 /* Bytes of coefficient tables se_resize_u8 keeps per device (process-wide; 0 restores the default of 256 MiB; negative is an
  * error). When a call's new tables would pass the limit, the device's cache is emptied (after a device synchronise) before the
  * call looks up any table; one call's own tables may exceed it. */

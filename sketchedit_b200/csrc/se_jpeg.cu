@@ -1,0 +1,742 @@
+// Baseline JPEG encoding of uint8 RGB windows, byte for byte what PIL.Image.save(buf, "JPEG", quality=q, subsampling=s) writes
+// for an RGB image without info, s = 0 (4:4:4) or 2 (4:2:0), with libjpeg-turbo's defaults (islow DCT, no smoothing, Annex K
+// Huffman tables, no restart markers). The encoder is integer arithmetic from start to finish, so every byte is libjpeg-turbo's.
+// tests/util_jpeg.py restates each stage in numpy; the comments below name the libjpeg-turbo source a stage follows.
+//
+// One call encodes up to JPEG_MAX_BATCH windows (rows a pitch apart) in these launches on one stream:
+//   dct:    one thread per 8x8 block: the window's samples with the last row and column repeated, RGB -> YCbCr (jccolor.c),
+//           h2v2 downsampling (jcsample.c), level shift, islow FDCT (jfdctint.c), quantisation by libjpeg-turbo's reciprocals
+//           (jcdctmgr.c); writes the zigzag coefficients, the quantised DC and the block's AC bit count.
+//   bits:   one thread per block: the DC difference and the block's total bit count (a dummy luma block of a 4:2:0 MCU, wholly
+//           outside the image, codes DC difference 0 and EOB, as jccoefct.c makes it).
+//   scan:   exclusive scan of the bit counts (three launches, scan_tiles / scan_sums / scan_add).
+//   pack:   one thread per block writes its Huffman codes at its bit offset into a zeroed 32-bit word stream, merging the words
+//           it shares with its neighbours by atomicOr.
+//   stuff:  per 64-byte chunk of the stream: count its 0xFF bytes, scan the counts, then write the chunk after the header with
+//           0x00 after each 0xFF (the last byte padded with 1-bits); the last chunk writes EOI and the image's byte count.
+//   header: one block per image writes the header, a function of (h, w, quality, subsampling) built on the host.
+#include <string.h>
+
+#include <algorithm>
+#include <mutex>
+#include <type_traits>
+#include <utility>
+#include <vector>
+
+#include "../../include/sketchedit_b200.h"
+#include "se_jpeg.h"
+
+namespace se {
+
+// ------------------------------------------------------------------------------------------ tables (ITU T.81 Annex K)
+static const unsigned char kLumaQ[64] = {16, 11, 10, 16, 24,  40,  51,  61,  12, 12, 14, 19, 26,  58,  60,  55,
+                                         14, 13, 16, 24, 40,  57,  69,  56,  14, 17, 22, 29, 51,  87,  80,  62,
+                                         18, 22, 37, 56, 68,  109, 103, 77,  24, 35, 55, 64, 81,  104, 113, 92,
+                                         49, 64, 78, 87, 103, 121, 120, 101, 72, 92, 95, 98, 112, 100, 103, 99};
+static const unsigned char kChromaQ[64] = {17, 18, 24, 47, 99, 99, 99, 99, 18, 21, 26, 66, 99, 99, 99, 99, 24, 26, 56, 99, 99, 99,
+                                           99, 99, 47, 66, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99,
+                                           99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99};
+constexpr unsigned char kZigzag[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
+                                       41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
+                                       30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+
+struct HuffSpec {   // code counts per length 1..16, then the symbols
+  unsigned char counts[16];
+  unsigned char syms[162];
+  int nsym;
+};
+constexpr HuffSpec kDcLuma = {{0, 1, 5, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0}, {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11}, 12};
+constexpr HuffSpec kDcChroma = {{0, 3, 1, 1, 1, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0}, {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11}, 12};
+constexpr HuffSpec kAcLuma = {
+    {0, 2, 1, 3, 3, 2, 4, 3, 5, 5, 4, 4, 0, 0, 1, 0x7d},
+    {0x01, 0x02, 0x03, 0x00, 0x04, 0x11, 0x05, 0x12, 0x21, 0x31, 0x41, 0x06, 0x13, 0x51, 0x61, 0x07, 0x22, 0x71, 0x14, 0x32, 0x81,
+     0x91, 0xa1, 0x08, 0x23, 0x42, 0xb1, 0xc1, 0x15, 0x52, 0xd1, 0xf0, 0x24, 0x33, 0x62, 0x72, 0x82, 0x09, 0x0a, 0x16, 0x17, 0x18,
+     0x19, 0x1a, 0x25, 0x26, 0x27, 0x28, 0x29, 0x2a, 0x34, 0x35, 0x36, 0x37, 0x38, 0x39, 0x3a, 0x43, 0x44, 0x45, 0x46, 0x47, 0x48,
+     0x49, 0x4a, 0x53, 0x54, 0x55, 0x56, 0x57, 0x58, 0x59, 0x5a, 0x63, 0x64, 0x65, 0x66, 0x67, 0x68, 0x69, 0x6a, 0x73, 0x74, 0x75,
+     0x76, 0x77, 0x78, 0x79, 0x7a, 0x83, 0x84, 0x85, 0x86, 0x87, 0x88, 0x89, 0x8a, 0x92, 0x93, 0x94, 0x95, 0x96, 0x97, 0x98, 0x99,
+     0x9a, 0xa2, 0xa3, 0xa4, 0xa5, 0xa6, 0xa7, 0xa8, 0xa9, 0xaa, 0xb2, 0xb3, 0xb4, 0xb5, 0xb6, 0xb7, 0xb8, 0xb9, 0xba, 0xc2, 0xc3,
+     0xc4, 0xc5, 0xc6, 0xc7, 0xc8, 0xc9, 0xca, 0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda, 0xe1, 0xe2, 0xe3, 0xe4, 0xe5,
+     0xe6, 0xe7, 0xe8, 0xe9, 0xea, 0xf1, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa},
+    162};
+constexpr HuffSpec kAcChroma = {
+    {0, 2, 1, 2, 4, 4, 3, 4, 7, 5, 4, 4, 0, 1, 2, 0x77},
+    {0x00, 0x01, 0x02, 0x03, 0x11, 0x04, 0x05, 0x21, 0x31, 0x06, 0x12, 0x41, 0x51, 0x07, 0x61, 0x71, 0x13, 0x22, 0x32, 0x81, 0x08,
+     0x14, 0x42, 0x91, 0xa1, 0xb1, 0xc1, 0x09, 0x23, 0x33, 0x52, 0xf0, 0x15, 0x62, 0x72, 0xd1, 0x0a, 0x16, 0x24, 0x34, 0xe1, 0x25,
+     0xf1, 0x17, 0x18, 0x19, 0x1a, 0x26, 0x27, 0x28, 0x29, 0x2a, 0x35, 0x36, 0x37, 0x38, 0x39, 0x3a, 0x43, 0x44, 0x45, 0x46, 0x47,
+     0x48, 0x49, 0x4a, 0x53, 0x54, 0x55, 0x56, 0x57, 0x58, 0x59, 0x5a, 0x63, 0x64, 0x65, 0x66, 0x67, 0x68, 0x69, 0x6a, 0x73, 0x74,
+     0x75, 0x76, 0x77, 0x78, 0x79, 0x7a, 0x82, 0x83, 0x84, 0x85, 0x86, 0x87, 0x88, 0x89, 0x8a, 0x92, 0x93, 0x94, 0x95, 0x96, 0x97,
+     0x98, 0x99, 0x9a, 0xa2, 0xa3, 0xa4, 0xa5, 0xa6, 0xa7, 0xa8, 0xa9, 0xaa, 0xb2, 0xb3, 0xb4, 0xb5, 0xb6, 0xb7, 0xb8, 0xb9, 0xba,
+     0xc2, 0xc3, 0xc4, 0xc5, 0xc6, 0xc7, 0xc8, 0xc9, 0xca, 0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda, 0xe2, 0xe3, 0xe4,
+     0xe5, 0xe6, 0xe7, 0xe8, 0xe9, 0xea, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa},
+    162};
+
+struct HuffCodes {   // symbol -> canonical code and its length (0: not in the table)
+  unsigned short code[256];
+  unsigned char size[256];
+};
+constexpr HuffCodes huff_codes(const HuffSpec& s) {   // Annex C
+  HuffCodes h{};
+  int code = 0, k = 0;
+  for (int len = 1; len <= 16; ++len) {
+    for (int i = 0; i < s.counts[len - 1]; ++i, ++k, ++code) {
+      h.code[s.syms[k]] = (unsigned short)code;
+      h.size[s.syms[k]] = (unsigned char)len;
+    }
+    code <<= 1;
+  }
+  return h;
+}
+// [0] DC luma, [1] DC chroma, [2] AC luma, [3] AC chroma
+__constant__ HuffCodes c_huff[4] = {huff_codes(kDcLuma), huff_codes(kDcChroma), huff_codes(kAcLuma), huff_codes(kAcChroma)};
+
+// ------------------------------------------------------------------------------------------ quantisation (host)
+struct QuantTab {   // per natural index: q = ((|x| + corr) * recip) >> shift, the sign restored (jcdctmgr.c, 16-bit DCTELEM)
+  unsigned short recip[64], corr[64];
+  unsigned char shift[64];
+  unsigned char q[64];   // the quantiser itself, for the DQT segment
+};
+
+static int quality_scale(int quality) { return quality < 50 ? 5000 / quality : 200 - 2 * quality; }   // jpeg_quality_scaling
+
+static QuantTab quant_tab(const unsigned char* base, int quality) {
+  QuantTab t{};
+  const int scale = quality_scale(quality);
+  for (int i = 0; i < 64; ++i) {
+    const int q = std::min(255, std::max(1, (base[i] * scale + 50) / 100));   // jpeg_add_quant_table, force_baseline
+    const unsigned divisor = 8u * q;                                         // the FDCT output is scaled by 8
+    int b = 31 - __builtin_clz(divisor);
+    int r = 16 + b;
+    unsigned fq = (1u << r) / divisor, fr = (1u << r) % divisor, c = divisor / 2;
+    if (fr == 0) {
+      fq >>= 1;
+      --r;
+    } else if (fr <= divisor / 2) {
+      ++c;
+    } else {
+      ++fq;
+    }
+    t.q[i] = (unsigned char)q;
+    t.recip[i] = (unsigned short)fq;
+    t.corr[i] = (unsigned short)c;
+    t.shift[i] = (unsigned char)r;
+  }
+  return t;
+}
+
+// the luma and chroma tables of one quality, built once per quality
+static const QuantTab* quant_tabs(int quality) {
+  static std::mutex mu;
+  static QuantTab tabs[101][2];
+  static bool built[101] = {};
+  std::lock_guard<std::mutex> lk(mu);
+  if (!built[quality]) {
+    tabs[quality][0] = quant_tab(kLumaQ, quality);
+    tabs[quality][1] = quant_tab(kChromaQ, quality);
+    built[quality] = true;
+  }
+  return tabs[quality];
+}
+
+static void put16(std::vector<unsigned char>& v, int x) {
+  v.push_back((unsigned char)(x >> 8));
+  v.push_back((unsigned char)x);
+}
+
+static void put_dht(std::vector<unsigned char>& v, int cls_id, const HuffSpec& s) {
+  v.insert(v.end(), {0xFF, 0xC4});
+  put16(v, 2 + 1 + 16 + s.nsym);
+  v.push_back((unsigned char)cls_id);
+  v.insert(v.end(), s.counts, s.counts + 16);
+  v.insert(v.end(), s.syms, s.syms + s.nsym);
+}
+
+constexpr int kSofHeightAt = 163;   // byte offsets of SOF0's height and width in the header
+
+// SOI, JFIF APP0 1.01 (density 1:1, units 0), DQT 0 and 1 (zigzag order), SOF0, DHT DC0 AC0 DC1 AC1, SOS (jcmarker.c)
+static std::vector<unsigned char> jpeg_header(int h, int w, const QuantTab* qt, int subsampling) {
+  std::vector<unsigned char> v = {0xFF, 0xD8, 0xFF, 0xE0, 0, 16, 'J', 'F', 'I', 'F', 0, 1, 1, 0, 0, 1, 0, 1, 0, 0};
+  for (int t = 0; t < 2; ++t) {
+    v.insert(v.end(), {0xFF, 0xDB, 0, 67, (unsigned char)t});
+    for (int k = 0; k < 64; ++k) v.push_back(qt[t].q[kZigzag[k]]);
+  }
+  v.insert(v.end(), {0xFF, 0xC0, 0, 17, 8});
+  put16(v, h);
+  put16(v, w);
+  v.insert(v.end(), {3, 1, (unsigned char)(subsampling == 2 ? 0x22 : 0x11), 0, 2, 0x11, 1, 3, 0x11, 1});
+  put_dht(v, 0x00, kDcLuma);
+  put_dht(v, 0x10, kAcLuma);
+  put_dht(v, 0x01, kDcChroma);
+  put_dht(v, 0x11, kAcChroma);
+  v.insert(v.end(), {0xFF, 0xDA, 0, 12, 3, 1, 0x00, 2, 0x11, 3, 0x11, 0, 63, 0});
+  return v;
+}
+
+long long jpeg_max_bytes(int h, int w, int subsampling) {
+  const long long m = subsampling == 2 ? 16 : 8;
+  const long long blocks = ((h + m - 1) / m) * ((w + m - 1) / m) * (subsampling == 2 ? 6 : 3);
+  return JPEG_HEADER_BYTES + 2 * (blocks * (JPEG_MAX_BLOCK_BITS / 8)) + 2;
+}
+
+// ------------------------------------------------------------------------------------------ kernels
+constexpr int kWordsPerBlock = JPEG_MAX_BLOCK_BITS / 32;
+constexpr int kChunkBytes = 64;   // bytes of the stream per stuffing thread
+constexpr int kThreads = 128;
+constexpr int SCAN_T = 256, SCAN_V = 8, SCAN_TILE = SCAN_T * SCAN_V;
+
+struct JImg {   // one image of a call; block, word and chunk indices are the call's (all images' arrays concatenated)
+  const unsigned char* src;
+  unsigned char* out;
+  long long* out_bytes;
+  long long pitch;
+  long long blk0, word0, chunk0;   // its first block, word and stuffing chunk
+  int h, w, mcu_x;                 // image size; MCUs per row
+};
+struct JpegList {
+  JImg im[JPEG_MAX_BATCH];
+  int n, sub;   // images; subsampling (0 or 2)
+  long long blocks, chunks;
+};
+struct JpegQuant {
+  unsigned short recip[2][64], corr[2][64];
+  unsigned char shift[2][64];
+};
+static_assert(sizeof(JpegList) + sizeof(JpegQuant) <= 4096, "descriptors must fit the kernel parameter space");
+
+struct JpegScratch {   // the call's scratch arrays
+  short* coef;                 // [64][blocks], zigzag order; [0] the quantised DC
+  unsigned* bits;              // [blocks]: AC bits (dct), then all bits of the block (bits)
+  int* dcdiff;                 // [blocks]
+  unsigned long long* bitoff;  // [blocks], exclusive scan of bits over the call
+  unsigned* words;             // the bit streams, word0 of each image on
+  unsigned* ffcnt;             // [chunks]
+  unsigned long long* ffoff;   // [chunks], exclusive scan of ffcnt over the call
+  unsigned long long* sums;    // scan tile sums
+};
+
+__device__ __forceinline__ int find_img(const JpegList& L, long long g, bool by_chunk) {
+  int i = 0;
+  while (i + 1 < L.n && g >= (by_chunk ? L.im[i + 1].chunk0 : L.im[i + 1].blk0)) ++i;
+  return i;
+}
+
+// Block e of an image in scan order: its component (0 Y, 1 Cb, 2 Cr) and block column / row in that component's plane.
+// A 4:2:0 MCU holds luma blocks (0,0), (0,1), (1,0), (1,1), then Cb and Cr; a 4:4:4 MCU holds Y, Cb, Cr.
+struct BlockAt {
+  int comp, bx, by;
+  bool dummy;   // a 4:2:0 luma block wholly outside the image
+};
+__device__ __forceinline__ BlockAt block_at(const JImg& d, int sub, long long e) {
+  const int per = sub == 2 ? 6 : 3;
+  const long long mcu = e / per;
+  const int k = (int)(e - mcu * per), mx = (int)(mcu % d.mcu_x), my = (int)(mcu / d.mcu_x);
+  BlockAt b;
+  if (sub == 2 && k < 4) {
+    b.comp = 0;
+    b.bx = 2 * mx + (k & 1);
+    b.by = 2 * my + (k >> 1);
+    b.dummy = b.bx * 8 >= d.w || b.by * 8 >= d.h;
+  } else {
+    b.comp = sub == 2 ? k - 3 : k;
+    b.bx = mx;
+    b.by = my;
+    b.dummy = false;
+  }
+  return b;
+}
+
+__device__ __forceinline__ int nbits(int v) { return v ? 32 - __clz(v < 0 ? -v : v) : 0; }
+
+__device__ __forceinline__ int color(int comp, int r, int g, int b) {   // jccolor.c, 16-bit fixed point
+  if (comp == 0) return (19595 * r + 38470 * g + 7471 * b + 32768) >> 16;
+  if (comp == 1) return (-11059 * r - 21709 * g + 32768 * b + (128 << 16) + 32767) >> 16;
+  return (32768 * r - 27439 * g - 5329 * b + (128 << 16) + 32767) >> 16;
+}
+
+__device__ __forceinline__ int descale(int x, int n) { return (x + (1 << (n - 1))) >> n; }
+
+// one pass of jfdctint.c over the 8 values d[o], d[o + s], ..., d[o + 7 s]
+__device__ __forceinline__ void fdct8(int (&d)[64], int o, int s, bool first) {
+  constexpr int C = 13, P = 2;
+  const int sh = first ? C - P : C + P;
+  int t0 = d[o] + d[o + 7 * s], t7 = d[o] - d[o + 7 * s];
+  int t1 = d[o + s] + d[o + 6 * s], t6 = d[o + s] - d[o + 6 * s];
+  int t2 = d[o + 2 * s] + d[o + 5 * s], t5 = d[o + 2 * s] - d[o + 5 * s];
+  int t3 = d[o + 3 * s] + d[o + 4 * s], t4 = d[o + 3 * s] - d[o + 4 * s];
+  const int t10 = t0 + t3, t13 = t0 - t3, t11 = t1 + t2, t12 = t1 - t2;
+  d[o] = first ? (t10 + t11) * (1 << P) : descale(t10 + t11, P);
+  d[o + 4 * s] = first ? (t10 - t11) * (1 << P) : descale(t10 - t11, P);
+  int z1 = (t12 + t13) * 4433;
+  d[o + 2 * s] = descale(z1 + t13 * 6270, sh);
+  d[o + 6 * s] = descale(z1 - t12 * 15137, sh);
+  z1 = t4 + t7;
+  int z2 = t5 + t6, z3 = t4 + t6, z4 = t5 + t7;
+  const int z5 = (z3 + z4) * 9633;
+  t4 *= 2446;
+  t5 *= 16819;
+  t6 *= 25172;
+  t7 *= 12299;
+  z1 *= -7373;
+  z2 *= -20995;
+  z3 = z3 * -16069 + z5;
+  z4 = z4 * -3196 + z5;
+  d[o + 7 * s] = descale(t4 + z1 + z3, sh);
+  d[o + 5 * s] = descale(t5 + z2 + z4, sh);
+  d[o + 3 * s] = descale(t6 + z2 + z3, sh);
+  d[o + s] = descale(t7 + z1 + z4, sh);
+}
+
+// the code tables in shared memory: a warp's blocks look up different symbols, which constant memory would serialise
+__device__ __forceinline__ void stage_huff(HuffCodes* sh, int first, int count) {
+  const unsigned* s = reinterpret_cast<const unsigned*>(c_huff + first);
+  unsigned* d = reinterpret_cast<unsigned*>(sh);
+  for (int j = threadIdx.x; j < count * (int)(sizeof(HuffCodes) / 4); j += blockDim.x) d[j] = s[j];
+  __syncthreads();
+}
+
+// f(std::integral_constant<int, k>) for k = 0 .. 63 in order: zigzag(k) is then a constant and v[zigzag(k)] a register
+__host__ __device__ constexpr int zigzag(int k) { return kZigzag[k]; }
+template <class F, int... K>
+__device__ __forceinline__ void for_each_zigzag(F&& f, std::integer_sequence<int, K...>) {
+  (f(std::integral_constant<int, K>{}), ...);
+}
+
+__global__ void __launch_bounds__(kThreads) jpeg_dct_kernel(const __grid_constant__ JpegList L, const __grid_constant__ JpegQuant Q,
+                                                            JpegScratch S) {
+  __shared__ HuffCodes sh_ac[2];
+  stage_huff(sh_ac, 2, 2);
+  const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
+  if (g >= L.blocks) return;
+  const JImg& d = L.im[find_img(L, g, false)];
+  const BlockAt b = block_at(d, L.sub, g - d.blk0);
+  if (b.dummy) return;   // its DC and bits come from the block before it (jpeg_bits_kernel, jpeg_pack_kernel)
+  int v[64];
+  if (L.sub == 2 && b.comp) {   // h2v2: rows repeated to an even count, columns to the MCU width, chroma rows to the block grid
+    const int ch = (d.h + 1) / 2;
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+      const int cy = min(b.by * 8 + r, ch - 1);
+      const unsigned char* r0 = d.src + (size_t)min(2 * cy, d.h - 1) * d.pitch;
+      const unsigned char* r1 = d.src + (size_t)min(2 * cy + 1, d.h - 1) * d.pitch;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        const int x0 = min(b.bx * 16 + 2 * c, d.w - 1) * 3, x1 = min(b.bx * 16 + 2 * c + 1, d.w - 1) * 3;
+        const int s = color(b.comp, r0[x0], r0[x0 + 1], r0[x0 + 2]) + color(b.comp, r0[x1], r0[x1 + 1], r0[x1 + 2]) +
+                      color(b.comp, r1[x0], r1[x0 + 1], r1[x0 + 2]) + color(b.comp, r1[x1], r1[x1 + 1], r1[x1 + 2]);
+        v[r * 8 + c] = ((s + 1 + (c & 1)) >> 2) - 128;
+      }
+    }
+  } else {
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+      const unsigned char* row = d.src + (size_t)min(b.by * 8 + r, d.h - 1) * d.pitch;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        const int x = min(b.bx * 8 + c, d.w - 1) * 3;
+        v[r * 8 + c] = color(b.comp, row[x], row[x + 1], row[x + 2]) - 128;
+      }
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < 8; ++r) fdct8(v, r * 8, 1, true);
+#pragma unroll
+  for (int c = 0; c < 8; ++c) fdct8(v, c, 8, false);
+  const int t = b.comp ? 1 : 0;
+  const HuffCodes& ac = sh_ac[t];
+  unsigned bits = 0;
+  int run = 0;
+  for_each_zigzag(
+      [&](auto kc) {
+        constexpr int k = decltype(kc)::value, n = zigzag(k);
+        const int x = v[n], a = x < 0 ? -x : x;
+        const int q = (int)(((unsigned)(a + Q.corr[t][n]) * Q.recip[t][n]) >> Q.shift[t][n]);
+        const int y = x < 0 ? -q : q;
+        S.coef[(size_t)k * L.blocks + g] = (short)y;
+        if (k == 0) return;
+        if (y == 0) {
+          ++run;
+          return;
+        }
+        const int nb = nbits(y);
+        bits += (run >> 4) * ac.size[0xF0] + ac.size[((run & 15) << 4) | nb] + nb;
+        run = 0;
+      },
+      std::make_integer_sequence<int, 64>{});
+  if (run) bits += ac.size[0x00];
+  S.bits[g] = bits;
+}
+
+// the quantised DC of block e's component that block e + 1 of that component codes its difference against: a dummy takes
+// the DC of the block before it in the MCU (block 0 of an MCU is never a dummy)
+__device__ __forceinline__ int dc_of(const JImg& d, int sub, const short* dc, long long e) {
+  while (block_at(d, sub, e).dummy) --e;
+  return dc[d.blk0 + e];
+}
+
+__device__ __forceinline__ long long prev_same_comp(int sub, long long e) {   // -1: the component's first block
+  const int per = sub == 2 ? 6 : 3;
+  const int k = (int)(e % per);
+  if (sub == 2 && k > 0 && k < 4) return e - 1;
+  return e - (sub == 2 && k == 0 ? 3 : per);
+}
+
+__global__ void __launch_bounds__(kThreads) jpeg_bits_kernel(const __grid_constant__ JpegList L, JpegScratch S) {
+  const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
+  if (g >= L.blocks) return;
+  const JImg& d = L.im[find_img(L, g, false)];
+  const long long e = g - d.blk0;
+  const BlockAt b = block_at(d, L.sub, e);
+  const HuffCodes& dch = c_huff[b.comp ? 1 : 0];
+  if (b.dummy) {
+    S.bits[g] = dch.size[0] + c_huff[2].size[0x00];
+    S.dcdiff[g] = 0;
+    return;
+  }
+  const long long p = prev_same_comp(L.sub, e);
+  const int diff = S.coef[g] - (p < 0 ? 0 : dc_of(d, L.sub, S.coef, p));
+  const int nb = nbits(diff);
+  S.bits[g] += dch.size[nb] + nb;
+  S.dcdiff[g] = diff;
+}
+
+// appends len <= 27 bits to a 64-bit accumulator holding n < 32 bits; full words go to w[*wi] by atomicOr
+__device__ __forceinline__ void put_bits(unsigned long long& acc, int& n, unsigned* w, long long& wi, unsigned code, int len) {
+  acc = (acc << len) | code;
+  n += len;
+  if (n >= 32) {
+    n -= 32;
+    atomicOr(w + wi++, (unsigned)(acc >> n));
+  }
+}
+
+__device__ __forceinline__ void put_value(unsigned long long& acc, int& n, unsigned* w, long long& wi, const HuffCodes& h,
+                                          int sym, int v, int nb) {
+  const unsigned bits = (unsigned)(v < 0 ? v - 1 : v) & ((1u << nb) - 1);
+  put_bits(acc, n, w, wi, ((unsigned)h.code[sym] << nb) | bits, h.size[sym] + nb);
+}
+
+__global__ void __launch_bounds__(kThreads) jpeg_pack_kernel(const __grid_constant__ JpegList L, JpegScratch S) {
+  __shared__ HuffCodes sh[4];
+  stage_huff(sh, 0, 4);
+  const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
+  if (g >= L.blocks) return;
+  const JImg& d = L.im[find_img(L, g, false)];
+  const BlockAt b = block_at(d, L.sub, g - d.blk0);
+  const unsigned long long at = S.bitoff[g] - S.bitoff[d.blk0];
+  unsigned* w = S.words + d.word0;
+  long long wi = (long long)(at >> 5);
+  int n = (int)(at & 31);
+  unsigned long long acc = 0;
+  const HuffCodes& dch = sh[b.comp ? 1 : 0];
+  const HuffCodes& ach = sh[b.comp ? 3 : 2];
+  const int diff = S.dcdiff[g];
+  put_value(acc, n, w, wi, dch, nbits(diff), diff, nbits(diff));
+  int run = 0;
+  if (!b.dummy) {
+    for (int k = 1; k < 64; ++k) {
+      const int y = S.coef[(size_t)k * L.blocks + g];
+      if (y == 0) {
+        ++run;
+        continue;
+      }
+      for (; run > 15; run -= 16) put_bits(acc, n, w, wi, ach.code[0xF0], ach.size[0xF0]);
+      const int nb = nbits(y);
+      put_value(acc, n, w, wi, ach, (run << 4) | nb, y, nb);
+      run = 0;
+    }
+  }
+  if (run || b.dummy) put_bits(acc, n, w, wi, ach.code[0x00], ach.size[0x00]);
+  if (n) atomicOr(w + wi, (unsigned)(acc << (32 - n)));
+}
+
+// ---- exclusive scan of unsigned counts into 64-bit offsets, over the whole array (tiles of SCAN_TILE)
+template <int NT>
+__device__ __forceinline__ unsigned long long block_exclusive_scan(unsigned long long v, unsigned long long* total) {
+  __shared__ unsigned long long warp_sum[NT / 32];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  unsigned long long x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) warp_sum[wid] = x;
+  __syncthreads();
+  if (wid == 0) {
+    unsigned long long s = lane < NT / 32 ? warp_sum[lane] : 0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long y = __shfl_up_sync(0xffffffffu, s, o);
+      if (lane >= o) s += y;
+    }
+    if (lane < NT / 32) warp_sum[lane] = s;
+  }
+  __syncthreads();
+  const unsigned long long before = (wid ? warp_sum[wid - 1] : 0) + x - v;
+  *total = warp_sum[NT / 32 - 1];
+  __syncthreads();   // warp_sum is reused by the next call
+  return before;
+}
+
+__global__ void __launch_bounds__(SCAN_T) scan_tiles(const unsigned* in, unsigned long long* out, unsigned long long* sums,
+                                                      long long n) {
+  const long long base = (long long)blockIdx.x * SCAN_TILE + (long long)threadIdx.x * SCAN_V;
+  unsigned v[SCAN_V];
+  unsigned long long s = 0;
+#pragma unroll
+  for (int j = 0; j < SCAN_V; ++j) {
+    v[j] = base + j < n ? in[base + j] : 0u;
+    s += v[j];
+  }
+  unsigned long long total;
+  unsigned long long run = block_exclusive_scan<SCAN_T>(s, &total);
+#pragma unroll
+  for (int j = 0; j < SCAN_V; ++j) {
+    if (base + j < n) out[base + j] = run;
+    run += v[j];
+  }
+  if (threadIdx.x == 0) sums[blockIdx.x] = total;
+}
+
+__global__ void __launch_bounds__(1024) scan_sums(unsigned long long* sums, long long n) {
+  unsigned long long carry = 0;
+  for (long long c = 0; c < n; c += 1024) {
+    const long long i = c + threadIdx.x;
+    const unsigned long long v = i < n ? sums[i] : 0;
+    unsigned long long total;
+    const unsigned long long before = block_exclusive_scan<1024>(v, &total);
+    if (i < n) sums[i] = carry + before;
+    carry += total;
+  }
+}
+
+__global__ void __launch_bounds__(SCAN_T) scan_add(unsigned long long* out, const unsigned long long* sums, long long n) {
+  const long long i = (long long)blockIdx.x * SCAN_T + threadIdx.x;
+  if (i < n) out[i] += sums[i / SCAN_TILE];
+}
+
+static int exclusive_scan(const unsigned* in, unsigned long long* out, unsigned long long* sums, long long n, cudaStream_t st) {
+  const long long tiles = (n + SCAN_TILE - 1) / SCAN_TILE;
+  scan_tiles<<<(unsigned)tiles, SCAN_T, 0, st>>>(in, out, sums, n);
+  scan_sums<<<1, 1024, 0, st>>>(sums, tiles);
+  scan_add<<<(unsigned)((n + SCAN_T - 1) / SCAN_T), SCAN_T, 0, st>>>(out, sums, n);
+  SE_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ---- stuffing
+__device__ __forceinline__ unsigned long long image_bits(const JImg& d, const JImg* next, const JpegList& L, const JpegScratch& S) {
+  const long long last = (next ? next->blk0 : L.blocks) - 1;
+  return S.bitoff[last] + S.bits[last] - S.bitoff[d.blk0];
+}
+
+// byte j of the image's stream, the last one padded with 1-bits
+__device__ __forceinline__ unsigned stream_byte(const unsigned* w, long long j, unsigned long long nbits) {
+  unsigned v = (w[j >> 2] >> (24 - 8 * (j & 3))) & 0xFFu;
+  if (j == (long long)((nbits - 1) >> 3) && (nbits & 7)) v |= 0xFFu >> (nbits & 7);
+  return v;
+}
+
+template <bool WRITE>
+__global__ void __launch_bounds__(kThreads) jpeg_stuff_kernel(const __grid_constant__ JpegList L, JpegScratch S) {
+  const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
+  if (g >= L.chunks) return;
+  const int i = find_img(L, g, true);
+  const JImg& d = L.im[i];
+  const unsigned long long nbits = image_bits(d, i + 1 < L.n ? &L.im[i + 1] : nullptr, L, S);
+  const long long nbytes = (long long)((nbits + 7) >> 3);
+  const long long c = g - d.chunk0, j0 = c * kChunkBytes, j1 = min(j0 + kChunkBytes, nbytes);
+  const unsigned* w = S.words + d.word0;
+  if (!WRITE) {
+    unsigned ff = 0;
+    for (long long j = j0; j < j1; ++j) ff += stream_byte(w, j, nbits) == 0xFFu;
+    S.ffcnt[g] = ff;
+    return;
+  }
+  if (j0 >= nbytes) return;
+  unsigned char* o = d.out + JPEG_HEADER_BYTES + j0 + (S.ffoff[g] - S.ffoff[d.chunk0]);
+  for (long long j = j0; j < j1; ++j) {
+    const unsigned v = stream_byte(w, j, nbits);
+    *o++ = (unsigned char)v;
+    if (v == 0xFFu) *o++ = 0;
+  }
+  if (j1 == nbytes) {   // the image's last chunk
+    o[0] = 0xFF;
+    o[1] = 0xD9;
+    *d.out_bytes = (long long)(o + 2 - d.out);
+  }
+}
+
+struct HeaderList {
+  unsigned char bytes[JPEG_HEADER_BYTES];
+  unsigned char* out[JPEG_MAX_BATCH];
+  unsigned short hw[JPEG_MAX_BATCH][2];
+};
+static_assert(sizeof(HeaderList) <= 4096, "header descriptors must fit the kernel parameter space");
+
+__global__ void __launch_bounds__(kThreads) jpeg_header_kernel(const __grid_constant__ HeaderList H) {
+  unsigned char* o = H.out[blockIdx.x];
+  for (int j = threadIdx.x; j < JPEG_HEADER_BYTES; j += kThreads) {
+    unsigned char v = H.bytes[j];
+    if (j >= kSofHeightAt && j < kSofHeightAt + 4) {
+      const int x = H.hw[blockIdx.x][(j - kSofHeightAt) >> 1];
+      v = (unsigned char)((j - kSofHeightAt) & 1 ? x : x >> 8);
+    }
+    o[j] = v;
+  }
+}
+
+// ------------------------------------------------------------------------------------------ host
+constexpr int kMaxDim = 65535;
+constexpr size_t kScratchAlign = 256;
+static size_t scratch_round(size_t bytes) { return (bytes + kScratchAlign - 1) / kScratchAlign * kScratchAlign; }
+
+struct JpegLayout {   // the call's block, word and chunk counts and where its arrays lie in scratch
+  long long blocks = 0, words = 0, chunks = 0;
+  size_t coef, bits, dcdiff, bitoff, words_at, ffcnt, ffoff, sums, total;
+};
+
+static long long image_blocks(int h, int w, int sub) {
+  const int m = sub == 2 ? 16 : 8;
+  return (long long)((h + m - 1) / m) * ((w + m - 1) / m) * (sub == 2 ? 6 : 3);
+}
+static long long chunks_of(long long blocks) { return (blocks * kWordsPerBlock * 4 + kChunkBytes - 1) / kChunkBytes; }
+
+static JpegLayout jpeg_layout(const int* hw, int n, int sub) {
+  JpegLayout l;
+  for (int i = 0; i < n; ++i) {
+    const long long b = image_blocks(hw[2 * i], hw[2 * i + 1], sub);
+    l.blocks += b;
+    l.words += b * kWordsPerBlock;
+    l.chunks += chunks_of(b);
+  }
+  const long long tiles = (std::max(l.blocks, l.chunks) + SCAN_TILE - 1) / SCAN_TILE;
+  size_t at = 0;
+  auto take = [&](size_t bytes) {
+    const size_t p = at;
+    at += scratch_round(bytes);
+    return p;
+  };
+  l.coef = take((size_t)l.blocks * 64 * sizeof(short));
+  l.bits = take((size_t)l.blocks * sizeof(unsigned));
+  l.dcdiff = take((size_t)l.blocks * sizeof(int));
+  l.bitoff = take((size_t)l.blocks * sizeof(unsigned long long));
+  l.words_at = take((size_t)l.words * sizeof(unsigned));
+  l.ffcnt = take((size_t)l.chunks * sizeof(unsigned));
+  l.ffoff = take((size_t)l.chunks * sizeof(unsigned long long));
+  l.sums = take((size_t)std::max(tiles, 1LL) * sizeof(unsigned long long));
+  l.total = at;
+  return l;
+}
+
+static unsigned grid_of(long long threads, int per_block) { return (unsigned)((threads + per_block - 1) / per_block); }
+
+}  // namespace se
+
+using namespace se;
+
+extern "C" {
+
+long long se_jpeg_max_bytes(int h, int w, int subsampling) {
+  if (h < 1 || w < 1 || h > kMaxDim || w > kMaxDim || (subsampling != 0 && subsampling != 2)) {
+    set_error("se_jpeg_max_bytes: sizes must be in [1, 65535] and subsampling 0 (4:4:4) or 2 (4:2:0)");
+    return -1;
+  }
+  return jpeg_max_bytes(h, w, subsampling);
+}
+
+int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality, int subsampling,
+                      unsigned char* out, const long long* out_off, long long* out_bytes_dev, void* scratch, long long* scratch_bytes,
+                      void* stream) {
+  SE_REQUIRE(n >= 0 && n <= JPEG_MAX_BATCH, "n must be in [0, " + std::to_string(JPEG_MAX_BATCH) + "] images per call");
+  SE_REQUIRE(quality >= 1 && quality <= 100, "quality must be in [1, 100]");
+  SE_REQUIRE(subsampling == 0 || subsampling == 2, "subsampling must be 0 (4:4:4) or 2 (4:2:0)");
+  SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
+  SE_REQUIRE(n == 0 || (src_pitch && hw && out_off), "null size / offset array");
+  for (int i = 0; i < n; ++i) {
+    const int h = hw[2 * i], w = hw[2 * i + 1];
+    SE_REQUIRE(h >= 1 && w >= 1 && h <= kMaxDim && w <= kMaxDim, "image " + std::to_string(i) + ": sizes must be in [1, 65535]");
+    SE_REQUIRE(out_off[i] >= 0, "negative offset");
+    SE_REQUIRE(src_pitch[i] >= 3LL * w, "image " + std::to_string(i) + ": the source pitch of " + std::to_string(src_pitch[i]) +
+                                            " bytes is narrower than its row of " + std::to_string(3LL * w) + " bytes");
+  }
+  const JpegLayout lay = jpeg_layout(hw, n, subsampling);
+  if (!scratch) {
+    *scratch_bytes = (long long)lay.total;
+    return 0;
+  }
+  SE_REQUIRE((size_t)*scratch_bytes >= lay.total,
+             "scratch holds " + std::to_string(*scratch_bytes) + " bytes, needs " + std::to_string(lay.total));
+  if (n == 0) return 0;
+  SE_REQUIRE(src && out && out_bytes_dev, "null src / out / out_bytes");
+  for (int i = 0; i < n; ++i) SE_REQUIRE(src[i] != nullptr, "null src");
+  SE_REQUIRE(lay.blocks < (1LL << 31) * kThreads && lay.chunks < (1LL << 31) * kThreads, "batch too large for one launch");
+  cudaStream_t st = (cudaStream_t)stream;
+
+  const QuantTab* qt = quant_tabs(quality);
+  JpegQuant Q;
+  for (int t = 0; t < 2; ++t) {
+    memcpy(Q.recip[t], qt[t].recip, sizeof(Q.recip[t]));
+    memcpy(Q.corr[t], qt[t].corr, sizeof(Q.corr[t]));
+    memcpy(Q.shift[t], qt[t].shift, sizeof(Q.shift[t]));
+  }
+  JpegList L;
+  HeaderList H;
+  memset(&L, 0, sizeof(L));
+  memset(&H, 0, sizeof(H));
+  const std::vector<unsigned char> hdr = jpeg_header(1, 1, qt, subsampling);
+  memcpy(H.bytes, hdr.data(), JPEG_HEADER_BYTES);
+  L.n = n;
+  L.sub = subsampling;
+  long long blk = 0, word = 0, chunk = 0;
+  for (int i = 0; i < n; ++i) {
+    const int h = hw[2 * i], w = hw[2 * i + 1], m = subsampling == 2 ? 16 : 8;
+    JImg& d = L.im[i];
+    d.src = src[i];
+    d.out = out + out_off[i];
+    d.out_bytes = out_bytes_dev + i;
+    d.pitch = src_pitch[i];
+    d.h = h;
+    d.w = w;
+    d.mcu_x = (w + m - 1) / m;
+    d.blk0 = blk;
+    d.word0 = word;
+    d.chunk0 = chunk;
+    const long long b = image_blocks(h, w, subsampling);
+    blk += b;
+    word += b * kWordsPerBlock;
+    chunk += chunks_of(b);
+    H.out[i] = d.out;
+    H.hw[i][0] = (unsigned short)h;
+    H.hw[i][1] = (unsigned short)w;
+  }
+  L.blocks = blk;
+  L.chunks = chunk;
+  unsigned char* s = (unsigned char*)scratch;
+  JpegScratch S;
+  S.coef = (short*)(s + lay.coef);
+  S.bits = (unsigned*)(s + lay.bits);
+  S.dcdiff = (int*)(s + lay.dcdiff);
+  S.bitoff = (unsigned long long*)(s + lay.bitoff);
+  S.words = (unsigned*)(s + lay.words_at);
+  S.ffcnt = (unsigned*)(s + lay.ffcnt);
+  S.ffoff = (unsigned long long*)(s + lay.ffoff);
+  S.sums = (unsigned long long*)(s + lay.sums);
+
+  SE_CUDA_OK(cudaMemsetAsync(S.words, 0, (size_t)lay.words * sizeof(unsigned), st));
+  jpeg_header_kernel<<<n, kThreads, 0, st>>>(H);
+  jpeg_dct_kernel<<<grid_of(L.blocks, kThreads), kThreads, 0, st>>>(L, Q, S);
+  jpeg_bits_kernel<<<grid_of(L.blocks, kThreads), kThreads, 0, st>>>(L, S);
+  SE_CUDA_OK(cudaGetLastError());
+  int rc = exclusive_scan(S.bits, S.bitoff, S.sums, L.blocks, st);
+  if (rc) return rc;
+  jpeg_pack_kernel<<<grid_of(L.blocks, kThreads), kThreads, 0, st>>>(L, S);
+  jpeg_stuff_kernel<false><<<grid_of(L.chunks, kThreads), kThreads, 0, st>>>(L, S);
+  SE_CUDA_OK(cudaGetLastError());
+  rc = exclusive_scan(S.ffcnt, S.ffoff, S.sums, L.chunks, st);
+  if (rc) return rc;
+  jpeg_stuff_kernel<true><<<grid_of(L.chunks, kThreads), kThreads, 0, st>>>(L, S);
+  SE_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+}  // extern "C"

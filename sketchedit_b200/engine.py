@@ -7,6 +7,7 @@ exposes the reference's call surface for the generator forward pass with CUDA te
 PyTorch is plumbing here (device memory + current stream); all compute is in libsketchedit_b200.so.
 """
 import ctypes
+import numbers
 
 import torch
 
@@ -578,6 +579,158 @@ def resize_u8(images, sizes, swap_rb=False):
     out, dst_offs = resize_u8_packed(src, offs, [tuple(t.shape[:2]) for t in images], sizes, C, swap_rb=swap_rb)
     shape = (lambda h, w: (h, w)) if images[0].dim() == 2 else (lambda h, w: (h, w, C))
     return [out[o:o + h * w * C].view(*shape(int(h), int(w))) for o, (h, w) in zip(dst_offs, sizes)]
+
+
+JPEG_MAX_BATCH = 32      # images per se_jpeg_encode_u8 call; the wrappers split longer lists into calls of this size
+JPEG_SUBSAMPLING = (0, 2)   # Pillow's subsampling values the encoder takes: 4:4:4 and 4:2:0
+
+
+def jpeg_max_bytes(h, w, subsampling=2):
+    """A true upper bound of the JPEG file of an h x w image (``se_jpeg_max_bytes``)."""
+    n = int(_lib.load().se_jpeg_max_bytes(int(h), int(w), int(subsampling)))
+    if n < 0:
+        raise ValueError(_lib.load().se_last_error().decode())
+    return n
+
+
+def _is_int(v):
+    """An integer argument of the JPEG calls: a Python or numpy integer, not a bool."""
+    return isinstance(v, numbers.Integral) and not isinstance(v, bool)
+
+
+def _check_jpeg_args(quality, subsampling):
+    """(quality, subsampling) as Python ints, or ValueError."""
+    if not _is_int(quality) or not 1 <= quality <= 100:
+        raise ValueError("quality must be an integer in [1, 100], got %r" % (quality,))
+    if not _is_int(subsampling) or subsampling not in JPEG_SUBSAMPLING:
+        raise ValueError("subsampling must be 0 (4:4:4) or 2 (4:2:0), got %r" % (subsampling,))
+    return int(quality), int(subsampling)
+
+
+def _jpeg_launch(ptrs, pitches, sizes, quality, subsampling, out, out_offsets, out_bytes):
+    """se_jpeg_encode_u8 over windows already checked, JPEG_MAX_BATCH per call, on the current stream of out's device."""
+    lib = _lib.load()
+    L, I, P = ctypes.c_longlong, ctypes.c_int, ctypes.c_void_p
+    n = len(sizes)
+    with torch.cuda.device(out.device):
+        chunks = []
+        for c0 in range(0, n, JPEG_MAX_BATCH):
+            sl = slice(c0, c0 + JPEG_MAX_BATCH)
+            k = len(sizes[sl])
+            args = ((P * k)(*ptrs[sl]), (L * k)(*pitches[sl]), (I * (2 * k))(*[v for hw in sizes[sl] for v in hw]), k,
+                    (L * k)(*out_offsets[sl]), c0)
+            need = L(0)
+            _lib.check(lib.se_jpeg_encode_u8(None, args[1], args[2], k, quality, subsampling, None, args[4], None, None,
+                                             ctypes.byref(need), None))
+            chunks.append((args, need.value))
+        scratch = torch.empty(max([1] + [b for _, b in chunks]), device=out.device, dtype=torch.uint8)
+        for a, _ in chunks:
+            size = L(scratch.numel())
+            _lib.check(lib.se_jpeg_encode_u8(a[0], a[1], a[2], a[3], quality, subsampling, _ptr(out), a[4],
+                                             ctypes.c_void_p(out_bytes.data_ptr() + 8 * a[5]), _ptr(scratch), ctypes.byref(size),
+                                             _stream()))
+
+
+def jpeg_encode_u8_packed(src, src_offsets, src_pitches, sizes, quality=75, subsampling=2, out=None, out_offsets=None):
+    """Baseline JPEG of RGB windows (``se_jpeg_encode_u8``), byte for byte ``Image.save(buf, "JPEG", quality=quality,
+    subsampling=subsampling)`` of each: image i is the ``sizes[i] = (h, w)`` window whose row r starts at byte ``src_offsets[i] +
+    r * src_pitches[i]`` of its source, with ``src_pitches[i] >= 3 w``. ``src`` is one contiguous CUDA uint8 tensor, or a list
+    of them with one per image; windows may overlap. ``out`` (optional, contiguous CUDA uint8) receives file i at
+    ``out_offsets[i]`` and must hold ``jpeg_max_bytes(h, w, subsampling)`` bytes there. Returns ``(out, out_offsets,
+    out_bytes)``: ``out_bytes`` is a CUDA int64 tensor of the files' lengths. Only enqueues work on the current stream."""
+    quality, subsampling = _check_jpeg_args(quality, subsampling)
+    n = len(sizes)
+    srcs = list(src) if isinstance(src, (list, tuple)) else [src] * n
+    if not (len(srcs) == len(src_offsets) == len(src_pitches) == n):
+        raise _lib.SketchEditB200Error("src (as a list), src_offsets, src_pitches and sizes must have the same length")
+    for t in srcs + [out]:
+        if t is not None and not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
+            raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % ("out" if t is out else "src"))
+    if n == 0:
+        return out, out_offsets, None
+    dev = srcs[0].device
+    if any(t.device != dev for t in srcs):
+        raise _lib.SketchEditB200Error("every src must be on one device")
+    sizes = [(int(h), int(w)) for h, w in sizes]
+    src_offsets, src_pitches = [int(o) for o in src_offsets], [int(p) for p in src_pitches]
+    for i, (t, o, p, (h, w)) in enumerate(zip(srcs, src_offsets, src_pitches, sizes)):
+        if not (1 <= h <= 65535 and 1 <= w <= 65535):
+            raise _lib.SketchEditB200Error("window %d: sizes must be in [1, 65535], got %dx%d" % (i, h, w))
+        if p < 3 * w:
+            raise _lib.SketchEditB200Error("window %d: the pitch of %d bytes is narrower than its row of %d bytes" % (i, p, 3 * w))
+        if o < 0 or o + (h - 1) * p + 3 * w > t.numel():
+            raise _lib.SketchEditB200Error("window %d (%dx%d at %d, pitch %d) is outside the %d-byte src" % (i, h, w, o, p, t.numel()))
+    bound = [jpeg_max_bytes(h, w, subsampling) for h, w in sizes]
+    if out is None:
+        if out_offsets is not None:
+            raise _lib.SketchEditB200Error("out_offsets needs out")
+        out_offsets, total = [], 0
+        for b in bound:
+            out_offsets.append(total)
+            total += (b + 15) // 16 * 16
+        out = torch.empty(total, device=dev, dtype=torch.uint8)
+    elif out_offsets is None or len(out_offsets) != n:
+        raise _lib.SketchEditB200Error("out needs one out_offsets entry per image")
+    if out.device != dev:
+        raise _lib.SketchEditB200Error("src on %s but out on %s" % (dev, out.device))
+    out_offsets = [int(o) for o in out_offsets]
+    for o, b in zip(out_offsets, bound):
+        if o < 0 or o + b > out.numel():
+            raise _lib.SketchEditB200Error("out slice [%d, %d) outside the %d-byte buffer" % (o, o + b, out.numel()))
+    out_bytes = torch.empty(n, device=dev, dtype=torch.int64)
+    _jpeg_launch([t.data_ptr() + o for t, o in zip(srcs, src_offsets)], src_pitches, sizes, quality, subsampling, out,
+                 out_offsets, out_bytes)
+    return out, out_offsets, out_bytes
+
+
+def jpeg_encode_u8(images, quality=75, subsampling=2):
+    """JPEG files of CUDA uint8 [h, w, 3] RGB images, as ``bytes``: each is what ``Image.fromarray(img).save(buf, "JPEG",
+    quality=quality, subsampling=subsampling)`` writes. An image may be a strided view (a box of a larger photo: pixels packed
+    along a row, rows ``stride(0)`` bytes apart); it is encoded where it lies. One download of the lengths, then one of the
+    bytes into pinned staging. quality and subsampling are Python or numpy integers, not bools.
+
+    Device memory: the call allocates, through torch's caching allocator, ``out`` at ``jpeg_max_bytes`` per image and the
+    scratch of ``se_jpeg_encode_u8``, both sized for the worst-case file (26 bits per coefficient, every byte stuffed), and
+    frees them on return. That is about 6.6 + 6.2 MB for a 1000x667 image at 4:2:0 and 104 + 98 MB for 4000x2667 (twice that
+    at 4:4:4), some 50 times a typical file; concurrent calls hold their sum. Each call also zeroes the word stream in
+    scratch (52 MB at 4000x2667, 4:2:0)."""
+    quality, subsampling = _check_jpeg_args(quality, subsampling)
+    images = list(images)
+    if not images:
+        return []
+    for t in images:
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.dim() == 3 and t.shape[2] == 3):
+            raise _lib.SketchEditB200Error("images must be CUDA uint8 [h, w, 3] tensors")
+        if t.stride(2) != 1 or (t.stride(1) != 3 and t.shape[1] > 1) or t.stride(0) < 3 * t.shape[1]:
+            raise _lib.SketchEditB200Error("an image's pixels must be packed along its rows (strides (>= 3 w, 3, 1), got %r)"
+                                           % (t.stride(),))
+        if not (1 <= t.shape[0] <= 65535 and 1 <= t.shape[1] <= 65535):
+            raise _lib.SketchEditB200Error("image sizes must be in [1, 65535], got %dx%d" % tuple(t.shape[:2]))
+    dev = images[0].device
+    if any(t.device != dev for t in images):
+        raise _lib.SketchEditB200Error("every image must be on one device")
+    sizes = [(int(t.shape[0]), int(t.shape[1])) for t in images]
+    offs, total = [], 0
+    for h, w in sizes:
+        offs.append(total)
+        total += (jpeg_max_bytes(h, w, subsampling) + 15) // 16 * 16
+    out = torch.empty(total, device=dev, dtype=torch.uint8)
+    out_bytes = torch.empty(len(images), device=dev, dtype=torch.int64)
+    _jpeg_launch([t.data_ptr() for t in images], [t.stride(0) for t in images], sizes, quality, subsampling, out, offs, out_bytes)
+    with torch.cuda.device(dev):
+        lens = out_bytes.cpu().tolist()
+        staging = torch.empty(max(1, sum(lens)), dtype=torch.uint8, pin_memory=True)
+        at = 0
+        for o, k in zip(offs, lens):
+            staging[at:at + k].copy_(out[o:o + k], non_blocking=True)
+            at += k
+        torch.cuda.current_stream().synchronize()
+    host = staging.numpy()
+    res, at = [], 0
+    for k in lens:
+        res.append(host[at:at + k].tobytes())
+        at += k
+    return res
 
 
 def outputs_to_uint8(composed, mask):
