@@ -15,6 +15,8 @@
 //     stride-1 read of one parity group, selected by a per-tap channel-block offset (C8Layer::tap_cb).
 // 288 threads: warps 0-7 are two consumer warpgroups (rows 0-63 / 64-127 of every 128-position tile: wgmma M = 64 each,
 // accumulators in registers, fused epilogue straight from the fragments, se_tc_device.cuh), warp 8 is the TMA producer.
+// Two-team launches (TEAMS = 2, resident weights): 544 threads, a second pair of consumer warpgroups in warps 8-15 runs
+// every other tile of the CTA from the same weight image and halo ring; the producer is warp 16.
 #include "se_conv_c8.h"
 
 #include <stdlib.h>
@@ -27,8 +29,8 @@
 namespace se {
 
 constexpr int C8_TH = 16, C8_TW = 8;   // output tile: 16 rows x 8 columns = 128 positions
-constexpr int C8_CONSUMER_WARPS = 8;
-constexpr int C8_THREADS = 32 * C8_CONSUMER_WARPS + 32;
+constexpr int C8_CONSUMER_WARPS = 8;   // of one team: two warpgroups
+__host__ __device__ constexpr int c8_threads(int teams) { return 32 * C8_CONSUMER_WARPS * teams + 32; }   // the producer is the last warp
 constexpr int C8_MAX_STAGES = 8;
 
 // slot / phase parity of iteration i in a ring of n slots (shift = log2 n, or < 0: n is not a power of two)
@@ -45,19 +47,26 @@ __device__ __forceinline__ void ring_of(int i, int n, int shift, int& slot, uint
 // the producer loads one (union) halo per real tile, a class selects its resident weight image (cls_bytes apart), its
 // A-offset row aoff[class * C8_CLS_UNITS + unit] and its output sub-pixel offset; the halo buffer is released after the
 // tile's last class.
-template <int NT, bool kF16, int R64, int M64, int R32>
-__global__ void __launch_bounds__(C8_THREADS, 1)
+// TEAMS: teams of two consumer warpgroups (warps 8t .. 8t + 7). Team t runs the CTA's tiles riter = t, t + TEAMS, ...: the
+// tile sequence, the producer and the ring slot of a tile are those of one team, and a halo buffer is read by one team only
+// (a_empty counts that team's 8 warps). The teams share the resident weights, the constants and aoff, and are not ordered
+// against each other: each ping-pongs on its own pair of named barriers. Two teams need resident weights and one k-step.
+template <int NT, bool kF16, int R64, int M64, int R32, int TEAMS>
+__global__ void __launch_bounds__(c8_threads(TEAMS), 1)
 conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   // carve: [halo A buffers][resident weights][stages: (tap A box) + (B image)] [barriers][bias]
-  const bool halo = (p.mode == C8_HALO);
+  // the two-team form runs ping-pong launches only (c8_launch): resident weights, one halo per tile, one k-step, no cluster;
+  // what serves the streamed and per-tap plans compiles away in it
+  constexpr bool kTeams = TEAMS > 1;
+  const bool halo = kTeams || p.mode == C8_HALO;
   constexpr int b64_bytes = NT * 128, b32_bytes = NT * 64;
   constexpr int b_bytes = R64 * b64_bytes + R32 * b32_bytes;
   const int stage_a = halo ? 0 : p.a_bytes;
   const int stage_b = p.resident ? 0 : b_bytes;
   const int stage_bytes = stage_a + stage_b;
-  const bool staged = stage_bytes > 0;
+  const bool staged = !kTeams && stage_bytes > 0;
   uint8_t* sHalo = smem;
   uint8_t* sWres = sHalo + (halo ? p.a_bufs * p.a_bytes : 0);
   uint8_t* sStages = sWres + (p.resident ? p.wres_bytes : 0);
@@ -73,7 +82,7 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
   const int lane = threadIdx.x & 31;
   // 2-CTA cluster (streamed weights): both CTAs run the same number of tiles in lockstep and share every B stage, rank r
   // multicasting part r of it; a stage slot is free when the consumers of BOTH CTAs have released it
-  const bool clustered = p.cluster > 1;
+  const bool clustered = !kTeams && p.cluster > 1;
   const uint32_t rank = clustered ? cluster_ctarank() : 0u;
   if (threadIdx.x == 0) {
     for (int i = 0; i < C8_MAX_STAGES; ++i) {
@@ -88,19 +97,19 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   const int cst_n = NT + 32;
-  epi_fill_constants(bias_s, cst_n, p.bias, p.e, threadIdx.x, C8_THREADS);
+  epi_fill_constants(bias_s, cst_n, p.bias, p.e, threadIdx.x, c8_threads(TEAMS));
   // a cluster's barriers are initialised before any multicast or remote arrive reaches them
   if (clustered) cluster_sync();
   else __syncthreads();
 
   const int total_tiles = p.N * p.tiles_x * p.tiles_y;
-  const int ksteps = p.ksteps;
+  const int ksteps = kTeams ? 1 : p.ksteps;
   // CTA b runs tiles b, b + gridDim.x, ... (gridDim.x = 2 x clusters: rank r of cluster q runs tiles 2 (q + k G) + r) for as
   // long as its cluster's rank-0 tile exists; when that one is the last tile, rank 1 is a PHANTOM for the pair: it loads no
   // A, issues its B parts and releases the stages unread, so that its partner's stages complete
   const int first_tile = (int)blockIdx.x - (int)rank;
 
-  if (warp == C8_CONSUMER_WARPS) {
+  if (warp == C8_CONSUMER_WARPS * TEAMS) {
     // ==================================================================== producer
     if (lane == 0) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
     if (p.resident && elect_one()) {
@@ -164,14 +173,14 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
     }
   } else {
     // ==================================================================== consumers: MMA + epilogue
-    const int wg = warp >> 2, wq = warp & 3;
+    const int team = TEAMS > 1 ? warp / C8_CONSUMER_WARPS : 0;
+    const int wg = (warp >> 2) & 1, wq = warp & 3;
     const uint32_t smem_base = smem_u32(smem);
     const uint32_t off_wres = halo ? (uint32_t)(p.a_bufs * p.a_bytes) : 0u;
     const uint32_t off_stages = off_wres + (p.resident ? (uint32_t)p.wres_bytes : 0u);
     const uint32_t a_m = (uint32_t)wg * 8u * (uint32_t)p.sbo_bytes;   // rows 64..127 of the tile = tile rows 8..15
     const uint32_t n_u64 = p.ntaps * p.n64;
     const int ncls = p.ncls;
-    const uint32_t tpi = (uint32_t)(p.tiles_x * p.tiles_y);
     const uint32_t cst_s = smem_u32(bias_s);
     const bool elu = p.e.epi == EPI_GATE_ELU, paired = p.e.paired != 0;
     if (p.resident) mbar_wait(wres_bar, 0, 6);
@@ -193,9 +202,9 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
     int stage = 0;
     uint32_t phase = 0;
     const int my_tiles = (first_tile < total_tiles) ? (total_tiles - first_tile + (int)gridDim.x - 1) / (int)gridDim.x : 0;
-    const int nv = my_tiles * ncls;
+    const int nv = (my_tiles > team ? (my_tiles - team + TEAMS - 1) / TEAMS : 0) * ncls;   // this team's virtual tiles
     // Ping-pong (resident weights, one k-step per tile: plain layers, stems, stem pairs, fused classes): the two warpgroups'
-    // MMA phases alternate on named barriers 1 and 2 (the 256 consumer threads). Warpgroup 1 issues its MMAs of virtual
+    // MMA phases alternate on named barriers 1 + 2 team and 2 + 2 team (the team's 256 threads). Warpgroup 1 issues its MMAs of virtual
     // tile v after warpgroup 0 has issued its own of v, warpgroup 0 those of v + 1 after warpgroup 1 has issued its own of v.
     // The tensor cores run them in issue order, so each warpgroup's epilogue overlaps the other's MMAs: a tile takes
     // max(2m, m + E) instead of 2m + E (m: one half tile's MMAs, E: its epilogue).
@@ -203,11 +212,27 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
     //    warpgroup 1 still reads tile v;
     //  * every bar.arrive meets its bar.sync: warpgroup 0 arrives on 1 for every v, where warpgroup 1 syncs; warpgroup 1
     //    arrives on 2 for every v but the last, warpgroup 0 syncs on it for every v but the first. No barrier is left
-    //    half-arrived at exit, whatever the tile count (0 and 1 included).
+    //    half-arrived at exit, whatever the team's tile count (0 and 1 included).
     // Streamed launches keep both warpgroups in lockstep: their stage ring cannot cover one that lags a whole MMA phase.
-    const bool pingpong = p.resident && ksteps == 1;
+    const bool pingpong = kTeams || (p.resident && ksteps == 1);
+    const int bar_wg0 = 2 + 2 * team, bar_wg1 = 1 + 2 * team;   // where warpgroup 0 / 1 waits for the other's issue
+    // the team's tile coordinates advance by TEAMS x gridDim.x tiles (mixed radix step, as the producer's by gridDim.x)
+    int riter = team, cls = 0;
+    int tx, ty, img;
+    {
+      const int t0 = (int)blockIdx.x + team * (int)gridDim.x;
+      tx = t0 % p.tiles_x; ty = (t0 / p.tiles_x) % p.tiles_y; img = t0 / (p.tiles_x * p.tiles_y);
+    }
     for (int v = 0; v < nv; ++v) {
-      const int riter = ncls == 1 ? v : v / ncls, cls = v - riter * ncls;
+      if (v > 0 && ++cls == ncls) {
+        cls = 0;
+        riter += TEAMS;
+        tx += p.cstep_x;
+        if (tx >= p.tiles_x) { tx -= p.tiles_x; ++ty; }
+        ty += p.cstep_y;
+        if (ty >= p.tiles_y) { ty -= p.tiles_y; ++img; }
+        img += p.cstep_img;
+      }
       const int tile = (int)blockIdx.x + riter * (int)gridDim.x;
       if (tile >= total_tiles) {   // phantom (clusters stream their weights: ncls == 1)
         for (int ks = 0; ks < ksteps; ++ks) {
@@ -217,16 +242,13 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
         }
         continue;
       }
-      const uint32_t img_u = (uint32_t)tile / tpi, rem = (uint32_t)tile - img_u * tpi;
-      const uint32_t ty_u = rem / (uint32_t)p.tiles_x;
-      const int img = (int)img_u, ty = (int)ty_u, tx = (int)(rem - ty_u * (uint32_t)p.tiles_x);
       int ab = 0;
       if (halo) {
         uint32_t aph;
         ring_of(riter, p.a_bufs, p.a_shift, ab, aph);
         mbar_wait(&a_full[ab], aph, 7);
       }
-      if (pingpong && (wg == 1 || v > 0)) named_bar_sync(wg == 0 ? 2 : 1, 256);
+      if (pingpong && (wg == 1 || v > 0)) named_bar_sync(wg == 0 ? bar_wg0 : bar_wg1, 256);
       int prev = -1;
       for (int ks = 0; ks < ksteps; ++ks) {
         if (staged) mbar_wait(&full_bar[stage], phase, 3);
@@ -267,7 +289,7 @@ conv_c8_kernel(const __grid_constant__ CUtensorMap tmA, const C8Params p) {
           if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
         }
       }
-      if (pingpong && (wg == 0 || v + 1 < nv)) named_bar_arrive(wg == 0 ? 1 : 2, 256);
+      if (pingpong && (wg == 0 || v + 1 < nv)) named_bar_arrive(wg == 0 ? bar_wg1 : bar_wg0, 256);
       wg_wait<0>();
       wg_fence_acc(acc);
       if (prev >= 0) release_stage(prev);
@@ -406,29 +428,32 @@ int c8_configure(C8Layer* L, int ntaps, const int8_t* dy, const int8_t* dx, int 
 // class group or stem pair of the two generators, in both precisions (split-half layers count three product taps per tap).
 // This one table selects the kernel of a launch, gets the shared-memory opt-in and keys the cluster-occupancy cache;
 // se_model_finalize checks every packed layer against it (c8_instantiated).
+// teams = 2: the instantiation also has a two-team form (fn2), which c8_launch runs where its plan allows (c8_teams).
 typedef void (*C8Kernel)(CUtensorMap, C8Params);
-struct C8Inst { int nt; bool f16; int r64, m64, r32; C8Kernel fn; };
-#define C8_INST(nt, f16, r64, m64, r32) {nt, f16, r64, m64, r32, conv_c8_kernel<nt, f16, r64, m64, r32>}
+struct C8Inst { int nt; bool f16; int r64, m64, r32, teams; C8Kernel fn, fn2; };
+#define C8_INST(nt, f16, r64, m64, r32) {nt, f16, r64, m64, r32, 1, conv_c8_kernel<nt, f16, r64, m64, r32, 1>, nullptr}
+#define C8_INST2(nt, f16, r64, m64, r32) \
+  {nt, f16, r64, m64, r32, 2, conv_c8_kernel<nt, f16, r64, m64, r32, 1>, conv_c8_kernel<nt, f16, r64, m64, r32, 2>}
 static const C8Inst kC8Insts[] = {
     // bf16 (resident weights: the whole tile is one k-step)
-    C8_INST(32, false, 0, 0, 9),    // 24->24
-    C8_INST(48, false, 0, 0, 9),    // 24->48 stride 2
-    C8_INST(48, false, 4, 3, 0),    // deconv 48->48 class
-    C8_INST(48, false, 5, 3, 0),    // 5x5 stem
-    C8_INST(96, false, 0, 0, 9),    // 24->96 stride 1 and 2
+    C8_INST2(32, false, 0, 0, 9),   // 24->24
+    C8_INST2(48, false, 0, 0, 9),   // 24->48 stride 2
+    C8_INST2(48, false, 4, 3, 0),   // deconv 48->48 class
+    C8_INST2(48, false, 5, 3, 0),   // 5x5 stem
+    C8_INST2(96, false, 0, 0, 9),   // 24->96 stride 1 and 2
     C8_INST(96, false, 4, 4, 4),    // deconv 96->96 class
-    C8_INST(96, false, 5, 3, 0),    // stem pair
-    C8_INST(96, false, 9, 3, 0),    // 48->96
+    C8_INST2(96, false, 5, 3, 0),   // stem pair
+    C8_INST2(96, false, 9, 3, 0),   // 48->96
     // bf16, streamed weights
     C8_INST(96, false, 3, 3, 0),    // 48->96 stride 2
     C8_INST(192, false, 1, 3, 0),   // 48->192 (stride 1 and 2)
     C8_INST(192, false, 1, 4, 0),   // 192->192
     C8_INST(192, false, 1, 4, 1),   // 96->192 (all rates)
     // split-half
-    C8_INST(32, true, 0, 0, 27),    // 24->24 (resident)
+    C8_INST2(32, true, 0, 0, 27),   // 24->24 (resident)
     C8_INST(48, true, 0, 0, 3),     // 24->48 stride 2
-    C8_INST(48, true, 12, 3, 0),    // deconv 48->48 class (resident)
-    C8_INST(48, true, 15, 3, 0),    // 5x5 stem (resident)
+    C8_INST(48, true, 12, 3, 0),    // deconv 48->48 class (resident; split-half halos leave a ring of two)
+    C8_INST2(48, true, 15, 3, 0),   // 5x5 stem (resident)
     C8_INST(96, true, 0, 0, 3),     // 24->96 stride 1 and 2
     C8_INST(96, true, 1, 3, 0),     // 48->96 stride 2 (one box per tap)
     C8_INST(96, true, 1, 4, 1),     // deconv 96->96 class
@@ -438,29 +463,33 @@ static const C8Inst kC8Insts[] = {
     C8_INST(192, true, 1, 4, 1),    // 96->192 (all rates)
 };
 #undef C8_INST
-static C8Kernel c8_kernel(const C8Layer& L, bool f16) {
+#undef C8_INST2
+static const C8Inst* c8_inst(const C8Layer& L, bool f16) {
   const TcWeights& w = L.w;
   const int r64 = w.n64 ? w.r64 : 0, r32 = w.n32 ? w.r32 : 0, m64 = r64 ? L.mmas64 : 0;
   for (const C8Inst& k : kC8Insts)
-    if (k.nt == w.NT && k.f16 == f16 && k.r64 == r64 && k.m64 == m64 && k.r32 == r32) return k.fn;
+    if (k.nt == w.NT && k.f16 == f16 && k.r64 == r64 && k.m64 == m64 && k.r32 == r32) return &k;
   return nullptr;
 }
 static int c8_set_smem_attr(int bytes) {
-  for (const C8Inst& k : kC8Insts) SE_CUDA_OK(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  for (const C8Inst& k : kC8Insts) {
+    SE_CUDA_OK(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    if (k.fn2) SE_CUDA_OK(cudaFuncSetAttribute(k.fn2, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  }
   return 0;
 }
 int c8_instantiated(const C8Layer& L, bool f16, const std::string& name) {
   const TcWeights& w = L.w;
-  SE_REQUIRE(c8_kernel(L, f16) != nullptr,
+  SE_REQUIRE(c8_inst(L, f16) != nullptr,
              "layer " + name + (f16 ? " (split-half)" : "") + ": no conv_c8_kernel instantiation for N = " + std::to_string(w.NT) +
                  ", k-step of " + std::to_string(w.n64 ? w.r64 : 0) + " x " + std::to_string(L.mmas64) + " + " +
                  std::to_string(w.n32 ? w.r32 : 0) + " x 2 MMAs (se_conv_c8.cu: kC8Insts)");
   return 0;
 }
-static void c8_launch_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, int grid, int smem_bytes, int cluster, cudaStream_t stream) {
+static void c8_launch_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, int grid, int teams, int smem_bytes, int cluster, cudaStream_t stream) {
   *cfg = cudaLaunchConfig_t();
   cfg->gridDim = dim3(grid);
-  cfg->blockDim = dim3(C8_THREADS);
+  cfg->blockDim = dim3(c8_threads(teams));
   cfg->dynamicSmemBytes = smem_bytes;
   cfg->stream = stream;
   if (cluster > 1) {
@@ -482,7 +511,7 @@ static int c8_max_clusters(C8Kernel k, int smem_bytes, int* out) {
   if (it == cache.end()) {
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute attr;
-    c8_launch_config(&cfg, &attr, 2 * g_sms, smem_bytes, 2, 0);
+    c8_launch_config(&cfg, &attr, 2 * g_sms, 1, smem_bytes, 2, 0);
     int n = 0;
     SE_CUDA_OK(cudaOccupancyMaxActiveClusters(&n, k, &cfg));
     SE_REQUIRE(n > 0, "no 2-CTA cluster of conv_c8_kernel fits on the device");
@@ -651,11 +680,15 @@ int c8_launch(const ConvParams& c, const C8Layer& L_in, cudaStream_t stream, con
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     SE_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(C8) failed, CUresult=" + std::to_string((int)r));
   }
-  const C8Kernel kernel = c8_kernel(L, p.f16 != 0);
-  SE_REQUIRE(kernel != nullptr, "no conv_c8_kernel instantiation for the layer's plan (N = " + std::to_string(p.NT) + ")");
+  const C8Inst* inst = c8_inst(L, p.f16 != 0);
+  SE_REQUIRE(inst != nullptr, "no conv_c8_kernel instantiation for the layer's plan (N = " + std::to_string(p.NT) + ")");
   // streamed weights: 2-CTA clusters read each weight stage from L2 once per pair of neighbouring tiles (TMA multicast)
   p.cluster = L.resident ? 1 : 2;
   int grid = total_tiles < g_sms ? total_tiles : g_sms;
+  // Two teams: a ping-pong launch (resident weights, one k-step) whose instantiation has the two-team form, whose CTAs run
+  // at least two tiles, and whose halo ring holds a buffer per team and two more to load ahead into
+  const int teams = (inst->teams == 2 && L.resident && p.ksteps == 1 && p.a_bufs >= 4 && total_tiles > grid) ? 2 : 1;
+  const C8Kernel kernel = teams == 2 ? inst->fn2 : inst->fn;
   if (p.cluster > 1) {
     int max_clusters = 0;
     { int rc_occ = c8_max_clusters(kernel, smem_bytes, &max_clusters); if (rc_occ) return rc_occ; }
@@ -665,9 +698,12 @@ int c8_launch(const ConvParams& c, const C8Layer& L_in, cudaStream_t stream, con
   p.step_x = grid % p.tiles_x;
   p.step_y = (grid / p.tiles_x) % p.tiles_y;
   p.step_img = grid / (p.tiles_x * p.tiles_y);
+  p.cstep_x = (teams * grid) % p.tiles_x;
+  p.cstep_y = (teams * grid / p.tiles_x) % p.tiles_y;
+  p.cstep_img = teams * grid / (p.tiles_x * p.tiles_y);
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr;
-  c8_launch_config(&cfg, &attr, grid, smem_bytes, p.cluster, stream);
+  c8_launch_config(&cfg, &attr, grid, teams, smem_bytes, p.cluster, stream);
   SE_CUDA_OK(cudaLaunchKernelEx(&cfg, kernel, tmA, p));
   return 0;
 }

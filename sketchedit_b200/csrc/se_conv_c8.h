@@ -44,6 +44,7 @@ struct C8Params {
   int N, Ho, Wo;
   int tiles_x, tiles_y;
   int step_x, step_y, step_img;   // gridDim.x decomposed in (tiles_x, tiles_y, images): incremental tile decode
+  int cstep_x, cstep_y, cstep_img;   // the same for a consumer team's step of TEAMS x gridDim.x tiles
   int ntaps;
   int8_t dy[MAX_TAPS], dx[MAX_TAPS];
   int n64, n32, NT, ksteps;   // (the k-step shape r64 / mmas64 / r32 is the instantiation's)
