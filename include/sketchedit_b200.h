@@ -271,6 +271,43 @@ int se_tap_info(se_model* m, int i, char* name, int name_cap, int* desc, long lo
 /* enqueues a copy of tap i's bytes to the device pointer dst on stream */
 int se_tap_copy(se_model* m, int i, void* dst, void* stream);
 
+/* ---- launch record of the channel-blocked wgmma convolution (tests; process-wide, off by default, one host branch per
+ * launch when off). While it is on, every forward and operator call runs eagerly (no CUDA graph is captured or replayed), and
+ * each conv_c8_kernel launch appends one record: the label of the layer that launched it ("<net>.<layer>", e.g. "G.conv11",
+ * "G.conv1+wconv1") and rec[SE_C8_REC_LEN], the plan and tile geometry the launch ran (DESIGN.md 5.1). se_c8_log_enable
+ * clears the record, whether it turns it on or off. */
+enum {
+  SE_C8_INST = 0,          /* index of the kernel instantiation (se_c8_inst_info) */
+  SE_C8_TEAMS = 1,         /* consumer teams per CTA: 1 or 2 */
+  SE_C8_CLUSTER = 2,       /* CTAs per cluster: 2 (streamed weights) or 1 */
+  SE_C8_GRID = 3,          /* CTAs launched */
+  SE_C8_TOTAL_TILES = 4,   /* N x TILES_X x TILES_Y tiles of 16 rows x 8 columns */
+  SE_C8_N = 5, SE_C8_TILES_X = 6, SE_C8_TILES_Y = 7, SE_C8_HO = 8, SE_C8_WO = 9,   /* the position grid of the launch */
+  SE_C8_STEP_X = 10, SE_C8_STEP_Y = 11, SE_C8_STEP_IMG = 12,      /* the grid in mixed radix (tiles_x, tiles_y, images) */
+  SE_C8_CSTEP_X = 13, SE_C8_CSTEP_Y = 14, SE_C8_CSTEP_IMG = 15,   /* teams x the grid, the same way */
+  SE_C8_MODE = 16,         /* 0: one halo per tile, 1: one box per tap */
+  SE_C8_CPT = 17,          /* k-steps per tap (one box per tap: > 1 when a stage holds one 64-channel chunk) */
+  SE_C8_NCLS = 18,         /* fused sub-pixel classes per tile (1: none) */
+  SE_C8_A_BUFS = 19, SE_C8_NUM_STAGES = 20,   /* halo ring depth, weight / tap stage ring depth */
+  SE_C8_OUT_C8 = 21,       /* output layout: 0 NHWC, 1 channel-blocked, 2 space-to-depth channel-blocked */
+  SE_C8_CHOFF = 22, SE_C8_LDO = 23,   /* output channel offset and pitch (channels, or channel blocks x 8) */
+  SE_C8_PHANTOM = 24,      /* 1: clustered with an odd tile count (the last pair's rank 1 computes nothing) */
+  SE_C8_BLK_SPLIT = 25,    /* stem pair: output blocks sent to the first tensor (0: one output tensor) */
+  SE_C8_REC_LEN = 26
+};
+int se_c8_log_enable(int on);
+/* records appended since the last se_c8_log_enable */
+int se_c8_log_count(void);
+/* record i: its label (NUL-terminated, truncated to name_cap bytes) and rec[SE_C8_REC_LEN] (each may be NULL) */
+int se_c8_log_get(int i, char* name, int name_cap, int* rec);
+/* instantiations of conv_c8_kernel (host only) */
+int se_c8_inst_count(void);
+enum { SE_C8_INST_NT = 0, SE_C8_INST_F16 = 1, SE_C8_INST_R64 = 2, SE_C8_INST_M64 = 3, SE_C8_INST_R32 = 4, SE_C8_INST_TEAMS = 5,
+       SE_C8_INST_LEN = 6 };
+/* instantiation i: info[SE_C8_INST_LEN] = GEMM N, split-half operands (1) or bf16 (0), the k-step shape (R64 units of M64
+ * MMAs, R32 units of 2), and TEAMS = 2 when it also has a two-team form (1 otherwise) */
+int se_c8_inst_info(int i, int* info);
+
 #ifdef __cplusplus
 }
 #endif

@@ -69,7 +69,18 @@ SIGNATURES = {
     "se_taps_count": (_c_int, [_c_void_p]),
     "se_tap_info": (_c_int, [_c_void_p, _c_int, _c_char_p, _c_int, ctypes.POINTER(_c_int), ctypes.POINTER(ctypes.c_longlong)]),
     "se_tap_copy": (_c_int, [_c_void_p, _c_int, _c_void_p, _c_void_p]),
+    "se_c8_log_enable": (_c_int, [_c_int]),
+    "se_c8_log_count": (_c_int, []),
+    "se_c8_log_get": (_c_int, [_c_int, _c_char_p, _c_int, ctypes.POINTER(_c_int)]),
+    "se_c8_inst_count": (_c_int, []),
+    "se_c8_inst_info": (_c_int, [_c_int, ctypes.POINTER(_c_int)]),
 }
+
+# fields of a conv_c8 launch record (se_c8_log_get) and of an instantiation (se_c8_inst_info), in header order
+C8_REC = ("inst", "teams", "cluster", "grid", "total_tiles", "N", "tiles_x", "tiles_y", "Ho", "Wo", "step_x", "step_y",
+          "step_img", "cstep_x", "cstep_y", "cstep_img", "mode", "cpt", "ncls", "a_bufs", "num_stages", "out_c8", "choff",
+          "ldo", "phantom", "blk_split")
+C8_INST = ("nt", "f16", "r64", "m64", "r32", "teams")
 
 _lib = None
 

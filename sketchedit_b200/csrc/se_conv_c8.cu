@@ -21,9 +21,12 @@
 
 #include <stdlib.h>
 
+#include <atomic>
 #include <map>
 #include <mutex>
+#include <vector>
 
+#include "../../include/sketchedit_b200.h"
 #include "se_tc_device.cuh"
 
 namespace se {
@@ -521,6 +524,35 @@ static int c8_max_clusters(C8Kernel k, int smem_bytes, int* out) {
   return 0;
 }
 
+// launch record (se_c8_log_enable): one branch per launch while it is off
+struct C8LogEntry { std::string name; int rec[SE_C8_REC_LEN]; };
+static std::atomic<bool> g_c8_log{false};
+static std::mutex g_c8_log_mu;
+static std::vector<C8LogEntry> g_c8_log_recs;
+static std::string g_c8_log_label;
+bool c8_log_on() { return g_c8_log.load(std::memory_order_relaxed); }
+void c8_log_label(const std::string& name) {
+  std::lock_guard<std::mutex> lk(g_c8_log_mu);
+  g_c8_log_label = name;
+}
+static void c8_log_append(const C8Params& p, const ConvParams& c, int inst, int teams, int grid, int total_tiles) {
+  C8LogEntry e;
+  int* r = e.rec;
+  r[SE_C8_INST] = inst; r[SE_C8_TEAMS] = teams; r[SE_C8_CLUSTER] = p.cluster; r[SE_C8_GRID] = grid;
+  r[SE_C8_TOTAL_TILES] = total_tiles; r[SE_C8_N] = p.N; r[SE_C8_TILES_X] = p.tiles_x; r[SE_C8_TILES_Y] = p.tiles_y;
+  r[SE_C8_HO] = p.Ho; r[SE_C8_WO] = p.Wo;
+  r[SE_C8_STEP_X] = p.step_x; r[SE_C8_STEP_Y] = p.step_y; r[SE_C8_STEP_IMG] = p.step_img;
+  r[SE_C8_CSTEP_X] = p.cstep_x; r[SE_C8_CSTEP_Y] = p.cstep_y; r[SE_C8_CSTEP_IMG] = p.cstep_img;
+  r[SE_C8_MODE] = p.mode; r[SE_C8_CPT] = p.cpt; r[SE_C8_NCLS] = p.ncls; r[SE_C8_A_BUFS] = p.a_bufs;
+  r[SE_C8_NUM_STAGES] = p.num_stages;
+  r[SE_C8_OUT_C8] = c.out_c8; r[SE_C8_CHOFF] = c.choff; r[SE_C8_LDO] = c.ldo;
+  r[SE_C8_PHANTOM] = p.cluster > 1 && total_tiles % 2 == 1;
+  r[SE_C8_BLK_SPLIT] = c.out_blk_split > 0 ? c.out_blk_split : 0;
+  std::lock_guard<std::mutex> lk(g_c8_log_mu);
+  e.name = g_c8_log_label;
+  g_c8_log_recs.push_back(e);
+}
+
 static const int kGroupSmemMax = 222 * 1024;   // fused classes may use (almost) the whole opt-in window: weights of all classes + 2 halos
 
 int c8_configure_group(C8Group* G, int ncls, int ntaps, const int8_t (*dy)[8], const int8_t (*dx)[8], const int* ooy, const int* oox, int Ci, int Cout) {
@@ -705,7 +737,50 @@ int c8_launch(const ConvParams& c, const C8Layer& L_in, cudaStream_t stream, con
   cudaLaunchAttribute attr;
   c8_launch_config(&cfg, &attr, grid, teams, smem_bytes, p.cluster, stream);
   SE_CUDA_OK(cudaLaunchKernelEx(&cfg, kernel, tmA, p));
+  if (c8_log_on()) c8_log_append(p, c, (int)(inst - kC8Insts), teams, grid, total_tiles);
   return 0;
 }
 
 }  // namespace se
+
+// ============================================================================================ C ABI: launch record
+extern "C" {
+
+int se_c8_log_enable(int on) {
+  std::lock_guard<std::mutex> lk(se::g_c8_log_mu);
+  se::g_c8_log = on != 0;
+  se::g_c8_log_recs.clear();
+  se::g_c8_log_label.clear();
+  return 0;
+}
+
+int se_c8_log_count(void) {
+  std::lock_guard<std::mutex> lk(se::g_c8_log_mu);
+  return (int)se::g_c8_log_recs.size();
+}
+
+int se_c8_log_get(int i, char* name, int name_cap, int* rec) {
+  std::lock_guard<std::mutex> lk(se::g_c8_log_mu);
+  SE_REQUIRE(i >= 0 && i < (int)se::g_c8_log_recs.size(),
+             "launch record index " + std::to_string(i) + " of " + std::to_string(se::g_c8_log_recs.size()));
+  const se::C8LogEntry& e = se::g_c8_log_recs[i];
+  if (name && name_cap > 0) {
+    const size_t n = std::min(e.name.size(), (size_t)name_cap - 1);
+    memcpy(name, e.name.data(), n);
+    name[n] = 0;
+  }
+  if (rec) memcpy(rec, e.rec, sizeof(e.rec));
+  return 0;
+}
+
+int se_c8_inst_count(void) { return (int)(sizeof(se::kC8Insts) / sizeof(se::kC8Insts[0])); }
+
+int se_c8_inst_info(int i, int* info) {
+  SE_REQUIRE(i >= 0 && i < se_c8_inst_count() && info, "instantiation index " + std::to_string(i) + " of " + std::to_string(se_c8_inst_count()));
+  const se::C8Inst& k = se::kC8Insts[i];
+  info[SE_C8_INST_NT] = k.nt; info[SE_C8_INST_F16] = k.f16 ? 1 : 0; info[SE_C8_INST_R64] = k.r64;
+  info[SE_C8_INST_M64] = k.m64; info[SE_C8_INST_R32] = k.r32; info[SE_C8_INST_TEAMS] = k.teams;
+  return 0;
+}
+
+}  // extern "C"

@@ -71,4 +71,9 @@ int c8_instantiated(const C8Layer& L, bool f16, const std::string& name);
 // geometry of a fused-class launch; returns non-zero (no error text) when the classes do not fit in shared memory
 int c8_configure_group(C8Group* G, int ncls, int ntaps, const int8_t (*dy)[8], const int8_t (*dx)[8], const int* ooy, const int* oox, int Ci, int Cout);
 
+// launch record (se_c8_log_enable, include/sketchedit_b200.h; tests only, off by default): while it is on, every c8_launch
+// appends its plan and geometry under the label of the layer that launched it
+bool c8_log_on();
+void c8_log_label(const std::string& name);   // label of the following launches (run_layer)
+
 }  // namespace se

@@ -664,6 +664,7 @@ static int run_layer(Ctx& c, Layer& L, const View& in, void* out, int ldo, int c
   const bool fused = c.prec == SE_PREC_BF16_TC && !L.groups.empty() && in.c8 == 1;
   const bool split = c.split();
   const int n_launch = fused ? (int)L.groups.size() : (int)L.cls.size();
+  if (c8_log_on() && !c.dry) c8_log_label(std::string(1, L.net) + "." + L.name);
   for (int li = 0; li < n_launch; ++li) {
     const C8Group* grp = fused ? &L.groups[li] : nullptr;
     ClassW& cw = L.cls[fused ? li * grp->ncls : li];
@@ -1263,8 +1264,8 @@ static int with_arena(se_model* m, int prec, int B, cudaStream_t stream, F fn, s
     m->used = true;
   }
   drop_taps(m);
-  // ---- replay a captured forward (a forward with taps on runs eagerly)
-  const bool graphable = g_graphs_on && !g_timing && !m->taps_on && !key.empty();
+  // ---- replay a captured forward (a forward with taps or the launch record on runs eagerly)
+  const bool graphable = g_graphs_on && !g_timing && !m->taps_on && !c8_log_on() && !key.empty();
   const bool legacy = (stream == nullptr || stream == cudaStreamLegacy);
   cudaStream_t gs = stream;   // stream the graph is captured on / launched into
   if (graphable && legacy) {

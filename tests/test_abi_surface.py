@@ -69,6 +69,28 @@ def test_taps_without_gpu(lib_path):
     assert lib.se_taps_count(None) == -1
 
 
+def test_c8_launch_record_without_gpu(lib_path):
+    """the conv_c8 launch record and the instantiation table are host-side: empty with the record on or off, an index past
+    the end is an error, and the table lists its 23 instantiations, nine with a two-team form, in both precisions."""
+    lib = _lib.load()
+    assert len(_lib.C8_REC) == 26 and len(_lib.C8_INST) == 6
+    for on in (1, 0):
+        assert lib.se_c8_log_enable(on) == 0
+        assert lib.se_c8_log_count() == 0
+        assert lib.se_c8_log_get(0, None, 0, None) != 0
+        assert b"launch record index" in lib.se_last_error()
+    info = (ctypes.c_int * len(_lib.C8_INST))()
+    insts = []
+    for i in range(lib.se_c8_inst_count()):
+        assert lib.se_c8_inst_info(i, info) == 0
+        insts.append(dict(zip(_lib.C8_INST, list(info))))
+    assert lib.se_c8_inst_info(len(insts), info) != 0
+    assert len(insts) == 23
+    assert sum(k["teams"] == 2 for k in insts) == 9
+    assert {k["f16"] for k in insts} == {0, 1} and all(k["teams"] in (1, 2) for k in insts)
+    assert len({(k["nt"], k["f16"], k["r64"], k["m64"], k["r32"]) for k in insts}) == 23
+
+
 def test_no_cpu_fallback(lib_path):
     """Without a CUDA device finalize must fail loudly, never fall back."""
     import torch

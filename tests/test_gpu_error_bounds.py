@@ -48,7 +48,7 @@ def _conv_ratio(net, name, x, prec):
 def test_gated_conv_within_bound(net, name, prec):
     worst = (0.0, None)
     for label, B, H, W in UB.conv_sizes(net, name):
-        for regime in UB.conv_regimes(prec):
+        for regime in UB.conv_regimes(prec, label, UB.layer(net, name)[0]):
             x = UB.conv_input(net, name, B, H, W, regime, UB.stable_seed(net, name, label, regime))
             worst = max(worst, (_conv_ratio(net, name, x, prec), (label, H, W, regime)))
     print("bound %s %s.%s: max ratio %.3g at %s" % (prec, net, name, worst[0], worst[1]))
