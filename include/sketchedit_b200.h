@@ -137,64 +137,45 @@ int se_outputs_to_uint8(const float* composed, const float* mask, int B, int H, 
                         unsigned char* mask_u8, void* stream);
 
 /* ---- Pillow-exact resize of uint8 HWC images: PIL.Image.resize(size) with its default filter (BICUBIC, no box, no
- * reducing_gap), bit for bit, for a batch of n <= 32 images of their own sizes (the resize-to-a-multiple-of-8 before the
- * forward and back after it of the reference demo, demo.py:39-73). Image i is read from src + src_off[i] (bytes) with size
- * src_hw[2i] x src_hw[2i+1] x channels and written to dst + dst_off[i] at dst_hw[2i] x dst_hw[2i+1] x channels; channels is 1
- * or 3, sizes are in [1, 65535]. Only the destination slices are written. swap_rb (channels 3) reverses the channel order of
- * the output (BGR <-> RGB). An axis whose length does not change is not resampled; an image of unchanged size is copied.
- * scratch holds the intermediate of images resized along both axes. Query form: scratch == NULL stores the bytes it needs in
- * *scratch_bytes and enqueues nothing; otherwise *scratch_bytes is the size of scratch. The coefficient tables are built on
- * the host and cached on the device per (in, out) pair: the first call with a new length pair uploads its table (a
- * synchronous copy); later calls only enqueue the kernels on `stream`. */
-int se_resize_u8(const unsigned char* src, const long long* src_off, const int* src_hw, unsigned char* dst, const long long* dst_off,
-                 const int* dst_hw, int n, int channels, int swap_rb, void* scratch, long long* scratch_bytes, void* stream);
-/* se_resize_u8 of windows of larger images: image i is src_hw[2i] rows of src_hw[2i+1] pixels, its row r at
- * src[i] + r * src_pitch[i] (bytes, >= src_hw[2i+1] * channels). src is a host array of n device pointers. With src[i] at the
- * top-left pixel of a box of an h x w x C image and src_pitch[i] = w * C, image i is Image.crop(box).resize(size), bit for bit.
- * Windows may overlap each other; dst must not overlap any window. dst_off, dst_hw, the limits, the scratch query (src may be
- * NULL in it) and the coefficient-table cache are those of se_resize_u8. */
+ * reducing_gap), bit for bit, for a batch of n in [0, 32] windows of their own sizes (the resize-to-a-multiple-of-8 before the
+ * forward and back after it of the reference demo, demo.py:39-73, and the crops of a region edit). Image i is src_hw[2i] rows
+ * of src_hw[2i+1] pixels of `channels` bytes (1 or 3), its row r at src[i] + r * src_pitch[i] (bytes, >= src_hw[2i+1] *
+ * channels); src is a host array of n device pointers. It is resized to dst_hw[2i] x dst_hw[2i+1] and written with packed rows
+ * at dst + dst_off[i]. Sizes are in [1, 65535]; only the destination slices are written. With src[i] at the top-left pixel
+ * of a box of an h x w x C image and src_pitch[i] = w * C, image i is Image.crop(box).resize(size). Windows may overlap each
+ * other; dst must not overlap any window. swap_rb (channels 3) reverses the channel order of the output (BGR <-> RGB). An axis
+ * whose length does not change is not resampled; an image of unchanged size is copied. scratch holds the intermediate of
+ * images resized along both axes: src_hw[2i] x dst_hw[2i+1] x channels bytes each, rounded up to 256. Query form: scratch ==
+ * NULL stores the bytes it needs in *scratch_bytes and enqueues nothing (src and dst may be NULL then); otherwise
+ * *scratch_bytes is the size of scratch. The coefficient tables are built on the host and cached on the device per (in, out)
+ * pair: the first call with a new length pair uploads its table (a synchronous copy); later calls only enqueue the kernels on
+ * `stream`. */
 int se_resize_window_u8(const unsigned char* const* src, const long long* src_pitch, const int* src_hw, unsigned char* dst,
                         const long long* dst_off, const int* dst_hw, int n, int channels, int swap_rb, void* scratch,
                         long long* scratch_bytes, void* stream);
-/* Resize back and paste, bit for bit as Pillow does it, for a batch of n <= 32 images of their own sizes (a region edit: the
- * forward's result on a crop of the photo, pasted back into the crop):
- *     res = Image.fromarray(rgb_i).resize((w, h));  m = Image.fromarray(mask_i).resize((w, h));  base_i.paste(res, (0, 0), m)
- * Image i's result is the src_hw[2i] x src_hw[2i+1] x 3 bytes at rgb + rgb_off[i] and its mask the src_hw[2i] x src_hw[2i+1]
- * bytes at mask + mask_off[i]; both are resized to h x w = dst_hw[2i] x dst_hw[2i+1] (each rounded to uint8, as se_resize_u8
- * writes them) and blended per channel over the h x w x 3 bytes at base + base_off[i]:
- * dst = DIV255(base * (255 - m) + res * m) with DIV255(a) = (((a + 128) >> 8) + a + 128) >> 8, Pillow's paste blend. The
- * h x w x 3 output goes to dst + dst_off[i]; dst may be base (in place), but neither may overlap rgb or mask. swap_rb reverses
- * the result's channel order first (the forward writes BGR). Sizes, the scratch query (scratch == NULL stores the bytes needed
- * in *scratch_bytes; scratch holds the intermediates of images whose width changes) and the coefficient-table cache are those
- * of se_resize_u8. */
-int se_resize_paste_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask, const long long* mask_off,
-                       const int* src_hw, const unsigned char* base, const long long* base_off, unsigned char* dst,
-                       const long long* dst_off, const int* dst_hw, int n, int swap_rb, void* scratch, long long* scratch_bytes,
-                       void* stream);
-/* Resize back and paste n >= 0 boxes in order into canvases, bit for bit as sequential Pillow pastes (a region edit with
- * several boxes whose boxes may overlap, nest or repeat):
+/* Resize back and paste n >= 0 boxes in order into canvases, bit for bit as sequential Pillow pastes (a region edit: the
+ * forward's results on crops of the photo, pasted back into their boxes, which may overlap, nest or repeat):
  *     for i in 0 .. n-1:  res = Image.fromarray(rgb_i).resize((w, h));  m = Image.fromarray(mask_i).resize((w, h));
  *                         canvas_i.paste(res, (x, y), m)
- * Box i's result and mask are read as in se_resize_paste_u8 (src_hw[2i] x src_hw[2i+1], at rgb + rgb_off[i] and mask +
- * mask_off[i]) and resized to h x w = dst_hw[2i] x dst_hw[2i+1]; its canvas is the image whose row 0 starts at canvas +
- * canvas_off[i], canvas_pitch[i] bytes per row (>= 3 (x + w)), and (y, x) = (box_yx[2i], box_yx[2i+1]) is the box's top-left
- * pixel in it. Boxes with the same canvas_off share a canvas and must give the same pitch; different canvases must not
- * overlap in memory, and no canvas may overlap rgb or mask. A later box blends over what an earlier one wrote. Only the pixels
- * of the boxes are read and written. swap_rb, the size limits, the scratch query and the coefficient-table cache are those of
- * se_resize_paste_u8 (box i needs the scratch image i of se_resize_paste_u8 needs). */
-int se_resize_composite_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask, const long long* mask_off,
-                           const int* src_hw, unsigned char* canvas, const long long* canvas_off, const long long* canvas_pitch,
-                           const int* box_yx, const int* dst_hw, int n, int swap_rb, void* scratch, long long* scratch_bytes,
-                           void* stream);
-/* se_resize_composite_u8 with each box's paste mask faded to 0 along chosen sides (a region edit's box edges inside the photo,
- * so the paste shows no seam there). feather holds 4n ints, box i's widths (left, top, right, bottom) in box pixels, each in
- * [0, the side's length: w for left and right, h for top and bottom]. Box i's resized mask m (h x w) becomes, before the blend,
+ * Box i's result is the src_hw[2i] x src_hw[2i+1] x 3 bytes at rgb + rgb_off[i] and its mask the src_hw[2i] x src_hw[2i+1]
+ * bytes at mask + mask_off[i]; both are resized to h x w = dst_hw[2i] x dst_hw[2i+1] (each rounded to uint8, as
+ * se_resize_window_u8 writes them; sizes in [1, 65535]). Its canvas is the image whose row 0 starts at canvas + canvas_off[i],
+ * canvas_pitch[i] bytes per row (>= 3 (x + w)), and (y, x) = (box_yx[2i], box_yx[2i+1]) is the box's top-left pixel in it.
+ * Boxes with the same canvas_off share a canvas and must give the same pitch; different canvases must not overlap in memory,
+ * and no canvas may overlap rgb or mask. The blend is Pillow's, per channel:
+ *     canvas = DIV255(canvas * (255 - m) + res * m),   DIV255(a) = (((a + 128) >> 8) + a + 128) >> 8,
+ * so a later box blends over what an earlier one wrote. Only the pixels of the boxes are read and written. swap_rb reverses
+ * the result's channel order first (the forward writes BGR).
+ * feather (may be NULL: no feathering) fades each box's paste mask to 0 along chosen sides (a region edit's box edges inside
+ * the photo, so the paste shows no seam there). It holds 4n ints, box i's widths (left, top, right, bottom) in box pixels,
+ * each in [0, the side's length: w for left and right, h for top and bottom]. Box i's resized mask m becomes, before the blend,
  *     m' = DIV255(m * r(y, x)),   r = min(ramp(x, left), ramp(w - 1 - x, right), ramp(y, top), ramp(h - 1 - y, bottom)),
  *     ramp(d, f) = d >= f ? 255 : (255 * (d + 1)) / (f + 1)   (integer division; d = 0 on the side's edge pixel),
- * with (y, x) the pixel's place in the box and DIV255 the blend's. A side of width 0 keeps m; DIV255(255 * m) == m, so widths
- * of 0 give se_resize_composite_u8's bytes, and a box whose four widths are 0 runs its arithmetic unchanged. feather == NULL:
- * no feathering (se_resize_composite_u8 is this call with NULL). Everything else, the checks, the scratch query and the
- * coefficient-table cache included, is se_resize_composite_u8's. */
+ * with (y, x) the pixel's place in the box. A side of width 0 keeps m; DIV255(255 * m) == m, so widths of 0 give the bytes of
+ * feather == NULL, and a box whose four widths are 0 runs its arithmetic unchanged.
+ * scratch holds the intermediates of boxes whose width changes: r256(src_hw[2i] * w * 3) + r256(src_hw[2i] * w) bytes for
+ * box i, r256 rounding up to 256. The scratch query (scratch == NULL; rgb, mask and canvas may be NULL then) and the
+ * coefficient-table cache are those of se_resize_window_u8. */
 int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask,
                                    const long long* mask_off, const int* src_hw, unsigned char* canvas, const long long* canvas_off,
                                    const long long* canvas_pitch, const int* box_yx, const int* dst_hw, const int* feather, int n,
@@ -205,6 +186,14 @@ int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rg
  * touched. For a predicted mask resized back to its box this gives the mask the feathered paste used. Only enqueues the
  * kernel on `stream`. */
 int se_feather_u8(unsigned char* img, const long long* off, const int* hw, const int* feather, int n, void* stream);
+/* ABI version 2 retired three resize entries of version 1. Each is a call of the entries above:
+ *   se_resize_u8(src, src_off, src_hw, dst, dst_off, dst_hw, n, channels, ...)
+ *       = se_resize_window_u8 with src[i] = src + src_off[i] and src_pitch[i] = src_hw[2i+1] * channels.
+ *   se_resize_paste_u8(rgb, rgb_off, mask, mask_off, src_hw, base, base_off, dst, dst_off, dst_hw, n, ...)
+ *       = se_resize_composite_feather_u8 with one box per canvas: canvas_off[i] = base_off[i] of canvas = base, box_yx[i] =
+ *         (0, 0), canvas_pitch[i] = 3 * dst_hw[2i+1], feather = NULL, pasting in place. For a separate dst, first copy each
+ *         base image to its dst slice and composite into dst.
+ *   se_resize_composite_u8(...) = se_resize_composite_feather_u8(...) with feather = NULL. */
 /* Baseline JPEG of n in [0, 32] RGB windows, byte for byte what Pillow writes for an RGB image without info:
  *     buf = io.BytesIO();  Image.fromarray(img_i).save(buf, "JPEG", quality=quality, subsampling=subsampling)
  * quality in [1, 100]; subsampling 0 (4:4:4) or 2 (4:2:0, Pillow's default with quality 75). Image i is hw[2i] rows of
@@ -221,13 +210,13 @@ int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitc
 /* Host only: a true upper bound of the file se_jpeg_encode_u8 writes for an h x w image: the 623-byte header, 208 bytes per
  * 8x8 block (64 codes of at most 26 bits) doubled for the 0x00 after each 0xFF, and EOI. -1 on bad arguments. */
 long long se_jpeg_max_bytes(int h, int w, int subsampling);
-/* Bytes of coefficient tables se_resize_u8 keeps per device (process-wide; 0 restores the default of 256 MiB; negative is an
+/* Bytes of coefficient tables the resize entries keep per device (process-wide; 0 restores the default of 256 MiB; negative is an
  * error). When a call's new tables would pass the limit, the device's cache is emptied (after a device synchronise) before the
  * call looks up any table; one call's own tables may exceed it. */
 int se_resize_set_table_cache_limit(long long bytes);
 /* bytes of coefficient tables currently cached for the current device */
 long long se_resize_table_cache_bytes(void);
-/* Host only (no device needed): the coefficient table se_resize_u8 uses for one axis of length in -> out. Returns ksize;
+/* Host only (no device needed): the coefficient table the resize entries use for one axis of length in -> out. Returns ksize;
  * bounds [out][2] = (first input sample, number of taps), coeffs [out][ksize] = weights with 22 fractional bits, zero beyond
  * the taps. cap = ints coeffs holds (>= out * ksize). bounds == coeffs == NULL: returns ksize only. Returns -1 on error. */
 int se_resize_coeffs(int in, int out, int* bounds, int* coeffs, long long cap);

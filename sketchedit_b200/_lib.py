@@ -43,14 +43,8 @@ SIGNATURES = {
                                                  _c_void_p, _c_void_p]),
     "se_set_attention_workspace_limit": (_c_int, [ctypes.c_longlong]),
     "se_outputs_to_uint8": (_c_int, [_c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_void_p, _c_void_p, _c_void_p]),
-    "se_resize_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_void_p,
-                              ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
     "se_resize_window_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int,
                                      _c_void_p, ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
-    "se_resize_paste_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
-                                    _c_void_p, _c_int, _c_int, _c_void_p, ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
-    "se_resize_composite_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
-                                        _c_void_p, _c_void_p, _c_int, _c_int, _c_void_p, ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
     "se_resize_composite_feather_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                                                 _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_void_p,
                                                 ctypes.POINTER(ctypes.c_longlong), _c_void_p]),

@@ -1,16 +1,10 @@
 // Glue kernels of the generator forward: input packing, heads (12->3 / 12->1 conv + tanh/sigmoid + blends), global pooling,
 // mask pooling, the fp32 attention operands and softmax, layout conversion. The kernels that touch activations are written once
-// over the activation storage (F32 / Bf16 / Split below). Also se_feather_u8, the feather ramp of region pastes applied to
-// box-sized masks on their own.
-#include <string.h>
-
-#include <string>
+// over the activation storage (F32 / Bf16 / Split below).
 #include <type_traits>
 
-#include "../../include/sketchedit_b200.h"
 #include "se_common.cuh"
 #include "se_misc.h"
-#include "se_resize.h"
 
 namespace se {
 
@@ -663,78 +657,4 @@ int fill_zero(void* p, size_t bytes, cudaStream_t s) {
   return 0;
 }
 
-// se_feather_u8: m = DIV255(m * ramp) in place over box-sized 'L' images, with the ramp paste_v_kernel gives a feathered box
-// (feather_pair, se_resize.h). One thread per pixel; only the pixels inside a band are read and written.
-struct FeatherImage {
-  unsigned char* p;
-  int h, w, tile0, tiles_x;
-  unsigned short f[4];   // left, top, right, bottom
-};
-struct FeatherList {
-  FeatherImage im[RESIZE_MAX_BATCH];
-  int n;
-};
-constexpr int F_TX = 64, F_TY = 4;
-
-__global__ void __launch_bounds__(F_TX * F_TY) feather_kernel(const __grid_constant__ FeatherList L) {
-  int i = 0;
-  while (i + 1 < L.n && (int)blockIdx.x >= L.im[i + 1].tile0) ++i;
-  const FeatherImage& d = L.im[i];
-  const int t = blockIdx.x - d.tile0;
-  const int x = (t % d.tiles_x) * F_TX + threadIdx.x, y = (t / d.tiles_x) * F_TY + threadIdx.y;
-  if (x >= d.w || y >= d.h) return;
-  const int ramp = min(feather_pair(y, d.h - 1 - y, d.f[1], d.f[3]), feather_pair(x, d.w - 1 - x, d.f[0], d.f[2]));
-  if (ramp == 255) return;
-  unsigned char* q = d.p + (size_t)y * d.w + x;
-  *q = (unsigned char)div255(*q * ramp);
-}
-
 }  // namespace se
-
-using namespace se;
-
-extern "C" int se_feather_u8(unsigned char* img, const long long* off, const int* hw, const int* feather, int n, void* stream) {
-  SE_REQUIRE(n >= 0, "n must be >= 0 images");
-  SE_REQUIRE(n == 0 || (off && hw && feather), "null offset / size / feather array");
-  for (int i = 0; i < n; ++i) {
-    const int h = hw[2 * i], w = hw[2 * i + 1];
-    const int* f = feather + 4 * (size_t)i;
-    SE_REQUIRE(h >= 1 && w >= 1 && h <= 65535 && w <= 65535, "image " + std::to_string(i) + ": sizes must be in [1, 65535]");
-    SE_REQUIRE(off[i] >= 0, "negative offset");
-    SE_REQUIRE(f[0] >= 0 && f[0] <= w && f[2] >= 0 && f[2] <= w && f[1] >= 0 && f[1] <= h && f[3] >= 0 && f[3] <= h,
-               "image " + std::to_string(i) + ": feather widths (" + std::to_string(f[0]) + ", " + std::to_string(f[1]) + ", " +
-                   std::to_string(f[2]) + ", " + std::to_string(f[3]) + ") must be in [0, the side's length]");
-  }
-  if (n == 0) return 0;
-  SE_REQUIRE(img, "null img");
-  FeatherList fl;
-  memset(&fl, 0, sizeof(fl));
-  long long tiles = 0;
-  auto launch = [&]() -> int {
-    if (fl.n) {
-      SE_REQUIRE(tiles < (1LL << 31), "batch too large for one launch");
-      feather_kernel<<<(unsigned)tiles, dim3(F_TX, F_TY), 0, (cudaStream_t)stream>>>(fl);
-      SE_CUDA_OK(cudaGetLastError());
-    }
-    memset(&fl, 0, sizeof(fl));
-    tiles = 0;
-    return 0;
-  };
-  for (int i = 0; i < n; ++i) {
-    const int* f = feather + 4 * (size_t)i;
-    if (!(f[0] | f[1] | f[2] | f[3])) continue;   // no band: the image is left as it is
-    FeatherImage& d = fl.im[fl.n++];
-    d.p = img + off[i];
-    d.h = hw[2 * i];
-    d.w = hw[2 * i + 1];
-    for (int s = 0; s < 4; ++s) d.f[s] = (unsigned short)f[s];
-    d.tile0 = (int)tiles;
-    d.tiles_x = cdiv(d.w, F_TX);
-    tiles += (long long)d.tiles_x * cdiv(d.h, F_TY);
-    if (fl.n == RESIZE_MAX_BATCH) {
-      int rc = launch();
-      if (rc) return rc;
-    }
-  }
-  return launch();
-}

@@ -7,12 +7,11 @@
 // with the coefficients Pillow builds in double (precompute_coeffs + normalize_coeffs_8bpc of libImaging/Resample.c). They are
 // built here on the host in the same order, so the integer weights and therefore every output byte are Pillow's.
 // Pillow computes only the intermediate rows the vertical pass reads; computing all of them gives the same values.
-// se_resize_paste_u8 resizes a result and its mask the same way and pastes the result over a base image with Pillow's
-// Image.paste(im, box, mask) blend, fused into the vertical pass (paste_v_kernel); se_resize_composite_u8 pastes boxes that
-// may overlap into shared canvases in order, as sequential Image.paste calls do, with the same kernel, and
-// se_resize_composite_feather_u8 fades each box's mask to 0 along the box edges it is given widths for. se_resize_window_u8
-// resizes windows of larger images (rows a pitch apart, such as boxes of a photo kept on the device) with the kernels of
-// se_resize_u8: Image.crop(box).resize(size) without the crop.
+// se_resize_window_u8 resizes windows of larger images (rows a pitch apart, such as boxes of a photo kept on the device):
+// Image.crop(box).resize(size) without the crop. se_resize_composite_feather_u8 resizes results and their masks the same way
+// and pastes boxes that may overlap into shared canvases in order, as sequential Image.paste(im, box, mask) calls do, with
+// the blend fused into the vertical pass (paste_v_kernel); it fades each box's mask to 0 along the box edges it is given
+// widths for. se_feather_u8 applies that fade to masks alone (feather_kernel).
 #include <limits.h>
 #include <math.h>
 #include <string.h>
@@ -24,9 +23,12 @@
 #include <vector>
 
 #include "../../include/sketchedit_b200.h"
-#include "se_resize.h"
+#include "se_common.cuh"
 
 namespace se {
+
+constexpr int RESIZE_MAX_BATCH = 32;   // images per launch: their descriptors travel as kernel parameters
+constexpr int RESIZE_PREC_BITS = 22;   // fractional bits of the fixed-point coefficients (Pillow's PRECISION_BITS for 8 bpc)
 
 // ------------------------------------------------------------------------------------------ coefficients (host, double)
 static double bicubic_filter(double x) {   // Keys cubic, a = -0.5, support 2
@@ -39,13 +41,15 @@ static double bicubic_filter(double x) {   // Keys cubic, a = -0.5, support 2
 
 static double axis_scale(int in, int out) { return (double)(float)in / out; }   // Pillow: (in1 - in0) / outSize, box in float
 
-int resize_ksize(int in, int out) {
+static int resize_ksize(int in, int out) {
   const double scale = axis_scale(in, out);
   const double fs = scale < 1.0 ? 1.0 : scale;
   return (int)ceil(2.0 * fs) * 2 + 1;
 }
 
-int resize_coeff_table(int in, int out, int* bounds, int* coeffs) {
+// Pillow's coefficient table for one axis (in -> out samples): bounds[2*i] = first input sample of output i, bounds[2*i+1] =
+// number of taps; coeffs[i*ksize + k] the fixed-point weights (zero beyond the taps). Returns ksize.
+static int resize_coeff_table(int in, int out, int* bounds, int* coeffs) {
   const double scale = axis_scale(in, out);
   const double fs = scale < 1.0 ? 1.0 : scale;
   const double support = 2.0 * fs, ss = 1.0 / fs;
@@ -86,7 +90,7 @@ struct AxisTable {
   int ksize = 0;
   size_t bytes = 0;
 };
-static std::mutex g_resize_mu;   // guards the cache and its limit; held for a whole se_resize_u8 call
+static std::mutex g_resize_mu;   // guards the cache and its limit; held for the whole launch part of a call
 static std::map<std::tuple<int, int, int>, AxisTable> g_tables;
 constexpr size_t kDefaultTableCap = 256u << 20;
 static size_t g_table_cap = kDefaultTableCap;
@@ -301,12 +305,28 @@ __global__ void __launch_bounds__(V_TX * V_TY) resize_v_kernel(const __grid_cons
   store12(d.dst + (size_t)(y0 + threadIdx.y) * d.row_bytes + p, v, nb, vec);
 }
 
-// The paste of se_resize_paste_u8 and se_resize_composite_u8: boxes pasted in order into canvases (row pitch in bytes). For a
-// box, the vertical pass of its result (3 channels) and of its mask, both in_h x out_w, to out_h, then Pillow's Image.paste
-// blend of the result over the canvas with that mask, per channel:
+// The feather ramp of a box's paste mask (paste_v_kernel, feather_kernel), over one pair of opposite sides: a side of width f
+// gives the pixel at distance d from its edge pixel (d = 0 on it) 255 * (d + 1) / (f + 1) when d < f and 255 otherwise; the
+// ramp of a pixel is the least over its row's pair (top, bottom) and its column's pair (left, right). The division runs only
+// inside a band and is exact integer division.
+__device__ __forceinline__ int feather_pair(int d0, int d1, int f0, int f1) {
+  int r = 255;
+  if (d0 < f0) r = 255 * (d0 + 1) / (f0 + 1);
+  if (d1 < f1) r = min(r, 255 * (d1 + 1) / (f1 + 1));
+  return r;
+}
+// Pillow's paste rounding: DIV255(a) = (((a + 128) >> 8) + a + 128) >> 8; DIV255(255 * m) == m for every byte m
+__device__ __forceinline__ int div255(int a) {
+  const int t = a + 128;
+  return ((t >> 8) + t) >> 8;
+}
+
+// The paste of se_resize_composite_feather_u8: boxes pasted in order into canvases (row pitch in bytes). For a box, the
+// vertical pass of its result (3 channels) and of its mask, both in_h x out_w, to out_h, then Pillow's Image.paste blend of
+// the result over the canvas with that mask, per channel:
 //     dst = DIV255(base * (255 - m) + res * m),   DIV255(a) = ((t >> 8) + t) >> 8 with t = a + 128 (libImaging/Paste.c).
-// A box with feather widths (se_resize_composite_feather_u8) first takes m = DIV255(m * ramp) with the ramp of feather_pair
-// at the pixel's place in the box; a box without them skips that step.
+// A box with feather widths first takes m = DIV255(m * ramp) with the ramp of feather_pair at the pixel's place in the box;
+// a box without them skips that step.
 // A thread owns 4 pixels of one canvas row (x a multiple of 4). It reads the canvas bytes that some box of the launch covers,
 // blends every covering box over them in the launch's order and writes them once; uncovered bytes are never touched. It reads
 // before it writes the same bytes, so dst may be base. The 12 canvas bytes move as 32-bit words when every box that covers
@@ -416,6 +436,32 @@ __global__ void __launch_bounds__(V_TX * V_TY) paste_v_kernel(const __grid_const
   }
 }
 
+// se_feather_u8: m = DIV255(m * ramp) in place over box-sized 'L' images, with the ramp paste_v_kernel gives a feathered box.
+// One thread per pixel; only the pixels inside a band are read and written.
+struct FeatherImage {
+  unsigned char* p;
+  int h, w, tile0, tiles_x;
+  unsigned short f[4];   // left, top, right, bottom
+};
+struct FeatherList {
+  FeatherImage im[RESIZE_MAX_BATCH];
+  int n;
+};
+constexpr int F_TX = 64, F_TY = 4;
+
+__global__ void __launch_bounds__(F_TX * F_TY) feather_kernel(const __grid_constant__ FeatherList L) {
+  int i = 0;
+  while (i + 1 < L.n && (int)blockIdx.x >= L.im[i + 1].tile0) ++i;
+  const FeatherImage& d = L.im[i];
+  const int t = blockIdx.x - d.tile0;
+  const int x = (t % d.tiles_x) * F_TX + threadIdx.x, y = (t / d.tiles_x) * F_TY + threadIdx.y;
+  if (x >= d.w || y >= d.h) return;
+  const int ramp = min(feather_pair(y, d.h - 1 - y, d.f[1], d.f[3]), feather_pair(x, d.w - 1 - x, d.f[0], d.f[2]));
+  if (ramp == 255) return;
+  unsigned char* q = d.p + (size_t)y * d.w + x;
+  *q = (unsigned char)div255(*q * ramp);
+}
+
 static int cdiv_i(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 constexpr int kMaxDim = 65535;
@@ -424,7 +470,7 @@ constexpr int kMaxSmem = 227 * 1024;
 
 static size_t scratch_round(size_t bytes) { return (bytes + kScratchAlign - 1) / kScratchAlign * kScratchAlign; }
 
-// the checks of image i that se_resize_u8 and se_resize_paste_u8 share
+// the checks of image i that se_resize_window_u8 and se_resize_composite_feather_u8 share
 static int check_image(int i, int ih, int iw, int oh, int ow) {
   SE_REQUIRE(ih >= 1 && iw >= 1 && oh >= 1 && ow >= 1 && ih <= kMaxDim && iw <= kMaxDim && oh <= kMaxDim && ow <= kMaxDim,
              "image " + std::to_string(i) + ": sizes must be in [1, 65535]");
@@ -480,10 +526,10 @@ static int v_table(int dev, int ih, int oh, const int** bounds, const int** coef
   return 0;
 }
 
-// The scratch query and the launches of se_resize_u8 and se_resize_window_u8, after their checks: image i is read from
-// src[i] (nullptr in the query form), its rows pitch[i] bytes apart, and written packed at dst + dst_off[i].
-static int resize_images(const std::vector<const unsigned char*>& src, const std::vector<long long>& pitch, const int* src_hw,
-                         unsigned char* dst, const long long* dst_off, const int* dst_hw, int n, int C, int swap_rb, void* scratch,
+// The scratch query and the launches of se_resize_window_u8, after its checks: image i is read from src[i] (src may be
+// nullptr in the query form), its rows pitch[i] bytes apart, and written packed at dst + dst_off[i].
+static int resize_images(const unsigned char* const* src, const long long* pitch, const int* src_hw, unsigned char* dst,
+                         const long long* dst_off, const int* dst_hw, int n, int C, int swap_rb, void* scratch,
                          long long* scratch_bytes, cudaStream_t st) {
   size_t need = 0;
   std::vector<size_t> mid(n);
@@ -497,7 +543,7 @@ static int resize_images(const std::vector<const unsigned char*>& src, const std
   }
   SE_REQUIRE((size_t)*scratch_bytes >= need, "scratch holds " + std::to_string(*scratch_bytes) + " bytes, needs " + std::to_string(need));
   if (n == 0) return 0;
-  SE_REQUIRE(dst && std::find(src.begin(), src.end(), nullptr) == src.end(), "null src / dst");
+  SE_REQUIRE(dst && src && std::find(src, src + n, nullptr) == src + n, "null src / dst");
   std::lock_guard<std::mutex> lk(g_resize_mu);
   int dev = 0;
   SE_CUDA_OK(cudaGetDevice(&dev));
@@ -558,13 +604,12 @@ static int resize_images(const std::vector<const unsigned char*>& src, const std
   return 0;
 }
 
-// One box of se_resize_paste_u8 / se_resize_composite_u8: its result and mask (ih x iw), pasted at ow x oh into canvas
-// `canvas` at (oy, ox).
+// One box of se_resize_composite_feather_u8: its result and mask (ih x iw), pasted at ow x oh into canvas `canvas` at (oy, ox).
 struct PasteBox {
   const unsigned char* rgb;
   const unsigned char* mask;
   int ih, iw, oh, ow, canvas, oy, ox;
-  int feather[4];   // left, top, right, bottom; zero unless se_resize_composite_feather_u8 gives them
+  int feather[4];   // left, top, right, bottom; zero when the call gives no widths
 };
 struct PasteCanvas {
   const unsigned char* base;
@@ -706,25 +751,6 @@ long long se_resize_table_cache_bytes(void) {
   return (long long)held_bytes(dev);
 }
 
-int se_resize_u8(const unsigned char* src, const long long* src_off, const int* src_hw, unsigned char* dst, const long long* dst_off,
-                 const int* dst_hw, int n, int channels, int swap_rb, void* scratch, long long* scratch_bytes, void* stream) {
-  SE_REQUIRE(n >= 0 && n <= RESIZE_MAX_BATCH, "n must be in [0, " + std::to_string(RESIZE_MAX_BATCH) + "] images per call");
-  SE_REQUIRE(channels == 1 || channels == 3, "channels must be 1 or 3");
-  SE_REQUIRE(!swap_rb || channels == 3, "swap_rb needs 3 channels");
-  SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
-  SE_REQUIRE(n == 0 || (src_off && src_hw && dst_off && dst_hw), "null size / offset array");
-  std::vector<const unsigned char*> srcs(n, nullptr);
-  std::vector<long long> pitch(n);
-  for (int i = 0; i < n; ++i) {
-    int rc = check_image(i, src_hw[2 * i], src_hw[2 * i + 1], dst_hw[2 * i], dst_hw[2 * i + 1]);
-    if (rc) return rc;
-    SE_REQUIRE(src_off[i] >= 0 && dst_off[i] >= 0, "negative offset");
-    if (src) srcs[i] = src + src_off[i];
-    pitch[i] = (long long)src_hw[2 * i + 1] * channels;
-  }
-  return resize_images(srcs, pitch, src_hw, dst, dst_off, dst_hw, n, channels, swap_rb, scratch, scratch_bytes, (cudaStream_t)stream);
-}
-
 int se_resize_window_u8(const unsigned char* const* src, const long long* src_pitch, const int* src_hw, unsigned char* dst,
                         const long long* dst_off, const int* dst_hw, int n, int channels, int swap_rb, void* scratch,
                         long long* scratch_bytes, void* stream) {
@@ -733,8 +759,6 @@ int se_resize_window_u8(const unsigned char* const* src, const long long* src_pi
   SE_REQUIRE(!swap_rb || channels == 3, "swap_rb needs 3 channels");
   SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
   SE_REQUIRE(n == 0 || (src_pitch && src_hw && dst_off && dst_hw), "null size / offset array");
-  std::vector<const unsigned char*> srcs(n, nullptr);
-  std::vector<long long> pitch(n);
   for (int i = 0; i < n; ++i) {
     int rc = check_image(i, src_hw[2 * i], src_hw[2 * i + 1], dst_hw[2 * i], dst_hw[2 * i + 1]);
     if (rc) return rc;
@@ -742,43 +766,9 @@ int se_resize_window_u8(const unsigned char* const* src, const long long* src_pi
     const long long row = (long long)src_hw[2 * i + 1] * channels;
     SE_REQUIRE(src_pitch[i] >= row, "image " + std::to_string(i) + ": the source pitch of " + std::to_string(src_pitch[i]) +
                                         " bytes is narrower than its row of " + std::to_string(row) + " bytes");
-    if (src) srcs[i] = src[i];
-    pitch[i] = src_pitch[i];
   }
-  return resize_images(srcs, pitch, src_hw, dst, dst_off, dst_hw, n, channels, swap_rb, scratch, scratch_bytes, (cudaStream_t)stream);
-}
-
-int se_resize_paste_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask, const long long* mask_off,
-                       const int* src_hw, const unsigned char* base, const long long* base_off, unsigned char* dst,
-                       const long long* dst_off, const int* dst_hw, int n, int swap_rb, void* scratch, long long* scratch_bytes,
-                       void* stream) {
-  SE_REQUIRE(n >= 0 && n <= RESIZE_MAX_BATCH, "n must be in [0, " + std::to_string(RESIZE_MAX_BATCH) + "] images per call");
-  SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
-  SE_REQUIRE(n == 0 || (rgb_off && mask_off && src_hw && base_off && dst_off && dst_hw), "null size / offset array");
-  size_t need = 0;
-  std::vector<size_t> mid(n);
-  for (int i = 0; i < n; ++i) {
-    const int ih = src_hw[2 * i], iw = src_hw[2 * i + 1], oh = dst_hw[2 * i], ow = dst_hw[2 * i + 1];
-    int rc = check_image(i, ih, iw, oh, ow);
-    if (rc) return rc;
-    SE_REQUIRE(rgb_off[i] >= 0 && mask_off[i] >= 0 && base_off[i] >= 0 && dst_off[i] >= 0, "negative offset");
-    mid[i] = need;
-    need += paste_scratch(ih, iw, ow);
-  }
-  if (!scratch) {
-    *scratch_bytes = (long long)need;
-    return 0;
-  }
-  SE_REQUIRE((size_t)*scratch_bytes >= need, "scratch holds " + std::to_string(*scratch_bytes) + " bytes, needs " + std::to_string(need));
-  if (n == 0) return 0;
-  SE_REQUIRE(rgb && mask && base && dst, "null rgb / mask / base / dst");
-  std::vector<PasteBox> boxes(n);   // image i: one box filling canvas i
-  std::vector<PasteCanvas> canvases(n);
-  for (int i = 0; i < n; ++i) {
-    boxes[i] = {rgb + rgb_off[i], mask + mask_off[i], src_hw[2 * i], src_hw[2 * i + 1], dst_hw[2 * i], dst_hw[2 * i + 1], i, 0, 0, {}};
-    canvases[i] = {base + base_off[i], dst + dst_off[i], 3LL * dst_hw[2 * i + 1]};
-  }
-  return paste_boxes(boxes, canvases, mid, scratch, swap_rb, (cudaStream_t)stream);
+  return resize_images(src, src_pitch, src_hw, dst, dst_off, dst_hw, n, channels, swap_rb, scratch, scratch_bytes,
+                       (cudaStream_t)stream);
 }
 
 int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask,
@@ -825,12 +815,50 @@ int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rg
   return paste_boxes(boxes, canvases, mid, scratch, swap_rb, (cudaStream_t)stream);
 }
 
-int se_resize_composite_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask, const long long* mask_off,
-                           const int* src_hw, unsigned char* canvas, const long long* canvas_off, const long long* canvas_pitch,
-                           const int* box_yx, const int* dst_hw, int n, int swap_rb, void* scratch, long long* scratch_bytes,
-                           void* stream) {
-  return se_resize_composite_feather_u8(rgb, rgb_off, mask, mask_off, src_hw, canvas, canvas_off, canvas_pitch, box_yx, dst_hw,
-                                        nullptr, n, swap_rb, scratch, scratch_bytes, stream);
+int se_feather_u8(unsigned char* img, const long long* off, const int* hw, const int* feather, int n, void* stream) {
+  SE_REQUIRE(n >= 0, "n must be >= 0 images");
+  SE_REQUIRE(n == 0 || (off && hw && feather), "null offset / size / feather array");
+  for (int i = 0; i < n; ++i) {
+    const int h = hw[2 * i], w = hw[2 * i + 1];
+    const int* f = feather + 4 * (size_t)i;
+    SE_REQUIRE(h >= 1 && w >= 1 && h <= kMaxDim && w <= kMaxDim, "image " + std::to_string(i) + ": sizes must be in [1, 65535]");
+    SE_REQUIRE(off[i] >= 0, "negative offset");
+    SE_REQUIRE(f[0] >= 0 && f[0] <= w && f[2] >= 0 && f[2] <= w && f[1] >= 0 && f[1] <= h && f[3] >= 0 && f[3] <= h,
+               "image " + std::to_string(i) + ": feather widths (" + std::to_string(f[0]) + ", " + std::to_string(f[1]) + ", " +
+                   std::to_string(f[2]) + ", " + std::to_string(f[3]) + ") must be in [0, the side's length]");
+  }
+  if (n == 0) return 0;
+  SE_REQUIRE(img, "null img");
+  FeatherList fl;
+  memset(&fl, 0, sizeof(fl));
+  long long tiles = 0;
+  auto launch = [&]() -> int {
+    if (fl.n) {
+      SE_REQUIRE(tiles < (1LL << 31), "batch too large for one launch");
+      feather_kernel<<<(unsigned)tiles, dim3(F_TX, F_TY), 0, (cudaStream_t)stream>>>(fl);
+      SE_CUDA_OK(cudaGetLastError());
+    }
+    memset(&fl, 0, sizeof(fl));
+    tiles = 0;
+    return 0;
+  };
+  for (int i = 0; i < n; ++i) {
+    const int* f = feather + 4 * (size_t)i;
+    if (!(f[0] | f[1] | f[2] | f[3])) continue;   // no band: the image is left as it is
+    FeatherImage& d = fl.im[fl.n++];
+    d.p = img + off[i];
+    d.h = hw[2 * i];
+    d.w = hw[2 * i + 1];
+    for (int s = 0; s < 4; ++s) d.f[s] = (unsigned short)f[s];
+    d.tile0 = (int)tiles;
+    d.tiles_x = cdiv_i(d.w, F_TX);
+    tiles += (long long)d.tiles_x * cdiv_i(d.h, F_TY);
+    if (fl.n == RESIZE_MAX_BATCH) {
+      int rc = launch();
+      if (rc) return rc;
+    }
+  }
+  return launch();
 }
 
 }  // extern "C"

@@ -274,7 +274,90 @@ def set_attention_workspace_limit(nbytes):
     _lib.check(_lib.load().se_set_attention_workspace_limit(int(nbytes)))
 
 
-RESIZE_MAX_BATCH = 32    # images per se_resize_u8 call; resize_u8_packed splits longer lists into calls of this size
+RESIZE_MAX_BATCH = 32    # images per se_resize_window_u8 call; the wrappers split longer lists into calls of this size
+
+
+# ---- plumbing shared by the uint8 image wrappers below
+def _chk_u8(*named):
+    """(tensor, name) pairs: contiguous CUDA uint8 tensors, whose pointers the kernels use as they are."""
+    for t, name in named:
+        _chk_out(t, None, name, torch.uint8)
+
+
+def _device(*named):
+    """The one device of the (tensor, name) pairs."""
+    devs = {t.device for t, _ in named}
+    if len(devs) > 1:
+        names = ", ".join(dict.fromkeys(nm for _, nm in named))
+        raise _lib.SketchEditB200Error("%s must be on one device (got %s)" % (names, ", ".join(sorted(map(str, devs)))))
+    return named[0][0].device
+
+
+def _check_windows(what, bufs, offsets, pitches, sizes, bpp):
+    """Window i is sizes[i] = (h, w) rows of w * bpp bytes, row r at byte offsets[i] + r * pitches[i] of bufs[i] (of bufs
+    itself when it is one tensor): its pitch must hold its row and the window must lie inside its buffer. Sizes below 1 are
+    left to the C entry, which names them."""
+    nbytes = [bufs.numel()] * len(sizes) if isinstance(bufs, torch.Tensor) else [t.numel() for t in bufs]
+    for i, (n, o, p, (h, w)) in enumerate(zip(nbytes, offsets, pitches, sizes)):
+        if p < w * bpp:
+            raise _lib.SketchEditB200Error("%s %d: the pitch of %d bytes is narrower than its row of %d bytes" % (what, i, p, w * bpp))
+        if o < 0 or (h >= 1 and w >= 1 and o + (h - 1) * p + w * bpp > n):
+            raise _lib.SketchEditB200Error("%s %d (%dx%d at %d, pitch %d) is outside the %d-byte buffer" % (what, i, h, w, o, p, n))
+
+
+def _aligned_offsets(nbytes, align=16):
+    """Offsets of blocks of nbytes[i] bytes packed at align-byte aligned offsets, and the bytes they span."""
+    offs, total = [], 0
+    for n in nbytes:
+        offs.append(total)
+        total += (n + align - 1) // align * align
+    return offs, total
+
+
+def _out(out, offsets, nbytes, device, name):
+    """(out, offsets) of a wrapper's output slices of nbytes[i] bytes: the caller's, checked, or without ``out`` a new tensor
+    holding them at 16-byte aligned offsets. ``name`` is the offsets argument's name."""
+    if out is None:
+        if offsets is not None:
+            raise _lib.SketchEditB200Error("%s needs out" % name)
+        offsets, total = _aligned_offsets(nbytes)
+        return torch.empty(total, device=device, dtype=torch.uint8), offsets
+    if offsets is None or len(offsets) != len(nbytes):
+        raise _lib.SketchEditB200Error("out needs one %s entry per image" % name)
+    offsets = [int(o) for o in offsets]
+    _check_windows("out", out, offsets, nbytes, [(1, b) for b in nbytes], 1)
+    return out, offsets
+
+
+def _hw(pairs):
+    return [(int(a), int(b)) for a, b in pairs]
+
+
+def _longs(values):
+    return (ctypes.c_longlong * len(values))(*values)
+
+
+def _ints(rows):
+    """The int tuples ``rows`` flattened into one C array."""
+    flat = [v for r in rows for v in r]
+    return (ctypes.c_int * len(flat))(*flat)
+
+
+def _run_chunks(n, per_call, device, chunk):
+    """Calls a scratch-taking C entry over n images, per_call images per call, on the current stream of ``device``.
+    ``chunk(sl)`` returns for the images of slice sl a function f(scratch, scratch_bytes, stream) that makes the call;
+    f(None, ...) is its scratch query. One scratch allocation, the largest query, serves every call."""
+    with torch.cuda.device(device):
+        calls, need = [], 0
+        for c0 in range(0, n, per_call):
+            f = chunk(slice(c0, c0 + per_call))
+            size = ctypes.c_longlong(0)
+            _lib.check(f(None, ctypes.byref(size), None))
+            calls.append(f)
+            need = max(need, size.value)
+        scratch = torch.empty(max(need, 1), device=device, dtype=torch.uint8)
+        for f in calls:
+            _lib.check(f(_ptr(scratch), ctypes.byref(ctypes.c_longlong(scratch.numel())), _stream()))
 
 
 def resize_u8_packed(src, src_offsets, src_sizes, dst_sizes, channels, swap_rb=False, out=None, dst_offsets=None):
@@ -284,52 +367,9 @@ def resize_u8_packed(src, src_offsets, src_sizes, dst_sizes, channels, swap_rb=F
     ``src``; it is resized to ``dst_sizes[i]`` and written at ``dst_offsets[i]`` of ``out``. Without ``out`` the results are
     packed into a new tensor at 16-byte aligned offsets. ``swap_rb`` reverses the channel order of the output (channels 3).
     Returns ``(out, dst_offsets)``. Only enqueues work on the current stream, except that the first resize between a pair of
-    lengths uploads its coefficient table."""
-    n = len(src_sizes)
-    if len(src_offsets) != n or len(dst_sizes) != n:
-        raise _lib.SketchEditB200Error("src_offsets, src_sizes and dst_sizes must have the same length")
-    for t, nm in ((src, "src"), (out, "out")):
-        if t is not None and not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
-            raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % nm)
-    src_sizes = [(int(h), int(w)) for h, w in src_sizes]
-    dst_sizes = [(int(h), int(w)) for h, w in dst_sizes]
-    nbytes = lambda hw: hw[0] * hw[1] * channels
-    if out is None:
-        if dst_offsets is not None:
-            raise _lib.SketchEditB200Error("dst_offsets needs out")
-        dst_offsets, total = [], 0
-        for hw in dst_sizes:
-            dst_offsets.append(total)
-            total += (nbytes(hw) + 15) // 16 * 16
-        out = torch.empty(total, device=src.device, dtype=torch.uint8)
-    elif dst_offsets is None or len(dst_offsets) != n:
-        raise _lib.SketchEditB200Error("out needs one dst_offsets entry per image")
-    if out.device != src.device:
-        raise _lib.SketchEditB200Error("src on %s but out on %s" % (src.device, out.device))
-    dst_offsets = [int(o) for o in dst_offsets]
-    for buf, offs, sizes, nm in ((src, src_offsets, src_sizes, "src"), (out, dst_offsets, dst_sizes, "out")):
-        for o, hw in zip(offs, sizes):
-            if o < 0 or o + nbytes(hw) > buf.numel():
-                raise _lib.SketchEditB200Error("%s slice [%d, %d) outside the %d-byte buffer" % (nm, o, o + nbytes(hw), buf.numel()))
-    lib = _lib.load()
-    with torch.cuda.device(src.device):
-        chunks = []
-        for c0 in range(0, n, RESIZE_MAX_BATCH):
-            sl = slice(c0, c0 + RESIZE_MAX_BATCH)
-            k = len(src_sizes[sl])
-            arr = (ctypes.c_longlong * k, ctypes.c_int * (2 * k))
-            args = (arr[0](*[int(o) for o in src_offsets[sl]]), arr[1](*[v for hw in src_sizes[sl] for v in hw]),
-                    arr[0](*dst_offsets[sl]), arr[1](*[v for hw in dst_sizes[sl] for v in hw]), k)
-            need = ctypes.c_longlong(0)
-            _lib.check(lib.se_resize_u8(None, args[0], args[1], None, args[2], args[3], k, channels, int(bool(swap_rb)), None,
-                                        ctypes.byref(need), None))
-            chunks.append((args, need.value))
-        scratch = torch.empty(max([1] + [b for _, b in chunks]), device=src.device, dtype=torch.uint8)
-        for (a, _) in chunks:
-            size = ctypes.c_longlong(scratch.numel())
-            _lib.check(lib.se_resize_u8(_ptr(src), a[0], a[1], _ptr(out), a[2], a[3], a[4], channels, int(bool(swap_rb)), _ptr(scratch),
-                                        ctypes.byref(size), _stream()))
-    return out, dst_offsets
+    lengths uploads its coefficient table. This is ``resize_window_u8_packed`` with packed rows (pitch ``w * channels``)."""
+    return resize_window_u8_packed(src, src_offsets, [int(w) * channels for _, w in src_sizes], src_sizes, dst_sizes, channels,
+                                   swap_rb=swap_rb, out=out, dst_offsets=dst_offsets)
 
 
 def resize_window_u8_packed(src, src_offsets, src_pitches, src_sizes, dst_sizes, channels, swap_rb=False, out=None,
@@ -341,142 +381,49 @@ def resize_window_u8_packed(src, src_offsets, src_pitches, src_sizes, dst_sizes,
     ``Image.crop(box).resize(size)`` bit for bit, without the crop. Windows may overlap; ``out`` must not overlap any of them.
     ``out``, ``dst_offsets``, ``swap_rb`` and the return value are those of ``resize_u8_packed``."""
     n = len(src_sizes)
-    srcs = list(src) if isinstance(src, (list, tuple)) else [src] * n
+    listed = isinstance(src, (list, tuple))
+    srcs = list(src) if listed else [src] * n
     if not (len(srcs) == len(src_offsets) == len(src_pitches) == len(dst_sizes) == n):
         raise _lib.SketchEditB200Error("src (as a list), src_offsets, src_pitches, src_sizes and dst_sizes must have the same length")
-    for t in srcs + [out]:
-        if t is not None and not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
-            raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % ("out" if t is out else "src"))
-    if n == 0:
+    named = [(t, "src") for t in (srcs if listed else [src])] + ([(out, "out")] if out is not None else [])
+    _chk_u8(*named)
+    if not named:
         return out, dst_offsets
-    dev = srcs[0].device
-    if any(t.device != dev for t in srcs):
-        raise _lib.SketchEditB200Error("every src must be on one device")
-    src_sizes = [(int(h), int(w)) for h, w in src_sizes]
-    dst_sizes = [(int(h), int(w)) for h, w in dst_sizes]
+    dev = _device(*named)
+    src_sizes, dst_sizes = _hw(src_sizes), _hw(dst_sizes)
     src_offsets, src_pitches = [int(o) for o in src_offsets], [int(p) for p in src_pitches]
-    for i, (t, o, p, (h, w)) in enumerate(zip(srcs, src_offsets, src_pitches, src_sizes)):
-        if p < w * channels:
-            raise _lib.SketchEditB200Error("window %d: the pitch of %d bytes is narrower than its row of %d bytes" % (i, p, w * channels))
-        if o < 0 or h < 1 or o + (h - 1) * p + w * channels > t.numel():
-            raise _lib.SketchEditB200Error("window %d (%dx%d at %d, pitch %d) is outside the %d-byte src" % (i, h, w, o, p, t.numel()))
-    nbytes = lambda hw: hw[0] * hw[1] * channels
-    if out is None:
-        if dst_offsets is not None:
-            raise _lib.SketchEditB200Error("dst_offsets needs out")
-        dst_offsets, total = [], 0
-        for hw in dst_sizes:
-            dst_offsets.append(total)
-            total += (nbytes(hw) + 15) // 16 * 16
-        out = torch.empty(total, device=dev, dtype=torch.uint8)
-    elif dst_offsets is None or len(dst_offsets) != n:
-        raise _lib.SketchEditB200Error("out needs one dst_offsets entry per image")
-    if out.device != dev:
-        raise _lib.SketchEditB200Error("src on %s but out on %s" % (dev, out.device))
-    dst_offsets = [int(o) for o in dst_offsets]
-    for o, hw in zip(dst_offsets, dst_sizes):
-        if o < 0 or o + nbytes(hw) > out.numel():
-            raise _lib.SketchEditB200Error("out slice [%d, %d) outside the %d-byte buffer" % (o, o + nbytes(hw), out.numel()))
+    _check_windows("window", srcs if listed else src, src_offsets, src_pitches, src_sizes, channels)
+    out, dst_offsets = _out(out, dst_offsets, [h * w * channels for h, w in dst_sizes], dev, "dst_offsets")
+    ptrs = [t.data_ptr() + o for t, o in zip(srcs, src_offsets)] if listed else [src.data_ptr() + o for o in src_offsets]
     lib = _lib.load()
-    L, I, P = ctypes.c_longlong, ctypes.c_int, ctypes.c_void_p
-    with torch.cuda.device(dev):
-        chunks = []
-        for c0 in range(0, n, RESIZE_MAX_BATCH):
-            sl = slice(c0, c0 + RESIZE_MAX_BATCH)
-            k = len(src_sizes[sl])
-            args = ((P * k)(*[t.data_ptr() + o for t, o in zip(srcs[sl], src_offsets[sl])]), (L * k)(*src_pitches[sl]),
-                    (I * (2 * k))(*[v for hw in src_sizes[sl] for v in hw]), (L * k)(*dst_offsets[sl]),
-                    (I * (2 * k))(*[v for hw in dst_sizes[sl] for v in hw]), k)
-            need = L(0)
-            _lib.check(lib.se_resize_window_u8(None, args[1], args[2], None, args[3], args[4], k, channels, int(bool(swap_rb)), None,
-                                               ctypes.byref(need), None))
-            chunks.append((args, need.value))
-        scratch = torch.empty(max([1] + [b for _, b in chunks]), device=dev, dtype=torch.uint8)
-        for a, _ in chunks:
-            size = L(scratch.numel())
-            _lib.check(lib.se_resize_window_u8(a[0], a[1], a[2], _ptr(out), a[3], a[4], a[5], channels, int(bool(swap_rb)),
-                                               _ptr(scratch), ctypes.byref(size), _stream()))
-    return out, dst_offsets
 
+    def chunk(sl):
+        k = len(ptrs[sl])
+        a = ((ctypes.c_void_p * k)(*ptrs[sl]), _longs(src_pitches[sl]), _ints(src_sizes[sl]), _ptr(out), _longs(dst_offsets[sl]),
+             _ints(dst_sizes[sl]), k, channels, int(bool(swap_rb)))
+        return lambda scratch, size, stream: lib.se_resize_window_u8(*a, scratch, size, stream)
 
-def resize_paste_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, base, base_offsets, dst_sizes, swap_rb=False, out=None,
-                           dst_offsets=None):
-    """Resize back and paste (``se_resize_paste_u8``), bit for bit as Pillow does it, for a batch of packed uint8 images:
-
-        res = Image.fromarray(rgb_i).resize((w, h)); m = Image.fromarray(mask_i).resize((w, h)); base_i.paste(res, (0, 0), m)
-
-    Image i's result [h',w',3] is at byte ``rgb_offsets[i]`` of ``rgb`` and its mask [h',w'] at ``mask_offsets[i]`` of ``mask``,
-    with ``src_sizes[i] = (h', w')``; both are resized to ``dst_sizes[i] = (h, w)`` and the result is blended over the [h,w,3]
-    bytes at ``base_offsets[i]`` of ``base``. ``swap_rb`` reverses the result's channel order first (the forward writes BGR).
-    The pasted image goes to ``dst_offsets[i]`` of ``out``, which may be ``base`` with ``dst_offsets == base_offsets`` (in
-    place); without ``out`` it is packed into a new tensor at 16-byte aligned offsets. All tensors are contiguous CUDA uint8 on
-    one device. Returns ``(out, dst_offsets)``. Only enqueues work on the current stream, except that the first resize between
-    a pair of lengths uploads its coefficient table."""
-    n = len(src_sizes)
-    if not (len(rgb_offsets) == len(mask_offsets) == len(base_offsets) == len(dst_sizes) == n):
-        raise _lib.SketchEditB200Error("rgb_offsets, mask_offsets, src_sizes, base_offsets and dst_sizes must have the same length")
-    for t, nm in ((rgb, "rgb"), (mask, "mask"), (base, "base"), (out, "out")):
-        if t is not None and not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
-            raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % nm)
-    src_sizes = [(int(h), int(w)) for h, w in src_sizes]
-    dst_sizes = [(int(h), int(w)) for h, w in dst_sizes]
-    if out is None:
-        if dst_offsets is not None:
-            raise _lib.SketchEditB200Error("dst_offsets needs out")
-        dst_offsets, total = [], 0
-        for h, w in dst_sizes:
-            dst_offsets.append(total)
-            total += (h * w * 3 + 15) // 16 * 16
-        out = torch.empty(max(total, 1), device=rgb.device, dtype=torch.uint8)
-    elif dst_offsets is None or len(dst_offsets) != n:
-        raise _lib.SketchEditB200Error("out needs one dst_offsets entry per image")
-    for t, nm in ((mask, "mask"), (base, "base"), (out, "out")):
-        if t.device != rgb.device:
-            raise _lib.SketchEditB200Error("rgb on %s but %s on %s" % (rgb.device, nm, t.device))
-    dst_offsets = [int(o) for o in dst_offsets]
-    for buf, offs, sizes, c, nm in ((rgb, rgb_offsets, src_sizes, 3, "rgb"), (mask, mask_offsets, src_sizes, 1, "mask"),
-                                    (base, base_offsets, dst_sizes, 3, "base"), (out, dst_offsets, dst_sizes, 3, "out")):
-        for o, (h, w) in zip(offs, sizes):
-            if o < 0 or o + h * w * c > buf.numel():
-                raise _lib.SketchEditB200Error("%s slice [%d, %d) outside the %d-byte buffer" % (nm, o, o + h * w * c, buf.numel()))
-    lib = _lib.load()
-    L, I = ctypes.c_longlong, ctypes.c_int
-    with torch.cuda.device(rgb.device):
-        chunks = []
-        for c0 in range(0, n, RESIZE_MAX_BATCH):
-            sl = slice(c0, c0 + RESIZE_MAX_BATCH)
-            k = len(src_sizes[sl])
-            offs = lambda v: (L * k)(*[int(o) for o in v[sl]])
-            args = (offs(rgb_offsets), offs(mask_offsets), (I * (2 * k))(*[v for hw in src_sizes[sl] for v in hw]), offs(base_offsets),
-                    offs(dst_offsets), (I * (2 * k))(*[v for hw in dst_sizes[sl] for v in hw]), k)
-            need = L(0)
-            _lib.check(lib.se_resize_paste_u8(None, args[0], None, args[1], args[2], None, args[3], None, args[4], args[5], k,
-                                              int(bool(swap_rb)), None, ctypes.byref(need), None))
-            chunks.append((args, need.value))
-        scratch = torch.empty(max([1] + [b for _, b in chunks]), device=rgb.device, dtype=torch.uint8)
-        for a, _ in chunks:
-            size = L(scratch.numel())
-            _lib.check(lib.se_resize_paste_u8(_ptr(rgb), a[0], _ptr(mask), a[1], a[2], _ptr(base), a[3], _ptr(out), a[4], a[5], a[6],
-                                              int(bool(swap_rb)), _ptr(scratch), ctypes.byref(size), _stream()))
+    _run_chunks(n, RESIZE_MAX_BATCH, dev, chunk)
     return out, dst_offsets
 
 
 def resize_composite_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, canvas, canvas_offsets, canvas_pitches,
                                box_offsets, box_sizes, swap_rb=False, feather=None):
-    """Resize back and paste boxes in order into canvases (``se_resize_composite_u8``), bit for bit as sequential Pillow
-    pastes, in place:
+    """Resize back and paste boxes in order into canvases (``se_resize_composite_feather_u8``), bit for bit as sequential
+    Pillow pastes, in place:
 
         for each box i in order:  canvas_i.paste(Image.fromarray(rgb_i).resize((w, h)), (x, y), Image.fromarray(mask_i).resize((w, h)))
 
-    Box i's result [h',w',3] and mask [h',w'] are read as in ``resize_paste_u8_packed`` (``src_sizes[i] = (h', w')``). Its
-    canvas starts at byte ``canvas_offsets[i]`` of ``canvas`` with ``canvas_pitches[i]`` bytes per row; ``box_offsets[i] =
-    (y, x)`` is its top-left pixel there and ``box_sizes[i] = (h, w)`` its size. Boxes with the same canvas offset share
-    that canvas, so a later box blends over an earlier one where they overlap. ``swap_rb`` reverses the result's channel
-    order first. All tensors are contiguous CUDA uint8 on one device; only the boxes' canvas pixels are read and written.
-    ``feather``: None, or per box its ramp widths ``(left, top, right, bottom)`` in box pixels
-    (``se_resize_composite_feather_u8``): the box's resized mask becomes ``DIV255(m * ramp)`` before the blend, with the ramp
-    of ``serving.feather_ramp``. Returns ``canvas``. Only enqueues work on the current stream, except that the first resize
-    between a pair of lengths uploads its coefficient table."""
+    Box i's result [h',w',3] is at byte ``rgb_offsets[i]`` of ``rgb`` and its mask [h',w'] at ``mask_offsets[i]`` of
+    ``mask``, with ``src_sizes[i] = (h', w')``. Its canvas starts at byte ``canvas_offsets[i]`` of ``canvas`` with
+    ``canvas_pitches[i]`` bytes per row; ``box_offsets[i] = (y, x)`` is its top-left pixel there and ``box_sizes[i] = (h, w)``
+    its size. Boxes with the same canvas offset share that canvas, so a later box blends over an earlier one where they
+    overlap. ``swap_rb`` reverses the result's channel order first (the forward writes BGR). All tensors are contiguous CUDA
+    uint8 on one device; only the boxes' canvas pixels are read and written. To paste into a copy instead, copy the canvas
+    first. ``feather``: None, or per box its ramp widths ``(left, top, right, bottom)`` in box pixels: the box's resized mask
+    becomes ``DIV255(m * ramp)`` before the blend, with the ramp of ``serving.feather_ramp``. Returns ``canvas``. Only
+    enqueues work on the current stream, except that the first resize between a pair of lengths uploads its coefficient
+    table."""
     n = len(src_sizes)
     if not (len(rgb_offsets) == len(mask_offsets) == len(canvas_offsets) == len(canvas_pitches) == len(box_offsets)
             == len(box_sizes) == n):
@@ -486,40 +433,26 @@ def resize_composite_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, 
         feather = [tuple(int(v) for v in f) for f in feather]
         if len(feather) != n or any(len(f) != 4 for f in feather):
             raise _lib.SketchEditB200Error("feather needs 4 widths (left, top, right, bottom) per box")
-    for t, nm in ((rgb, "rgb"), (mask, "mask"), (canvas, "canvas")):
-        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
-            raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % nm)
-    for t, nm in ((mask, "mask"), (canvas, "canvas")):
-        if t.device != rgb.device:
-            raise _lib.SketchEditB200Error("rgb on %s but %s on %s" % (rgb.device, nm, t.device))
-    src_sizes = [(int(h), int(w)) for h, w in src_sizes]
-    box_sizes = [(int(h), int(w)) for h, w in box_sizes]
-    box_offsets = [(int(y), int(x)) for y, x in box_offsets]
+    named = [(rgb, "rgb"), (mask, "mask"), (canvas, "canvas")]
+    _chk_u8(*named)
+    dev = _device(*named)
+    src_sizes, box_sizes, box_offsets = _hw(src_sizes), _hw(box_sizes), _hw(box_offsets)
+    rgb_offsets, mask_offsets = [int(o) for o in rgb_offsets], [int(o) for o in mask_offsets]
     canvas_offsets, canvas_pitches = [int(o) for o in canvas_offsets], [int(p) for p in canvas_pitches]
-    for buf, offs, c, nm in ((rgb, rgb_offsets, 3, "rgb"), (mask, mask_offsets, 1, "mask")):
-        for o, (h, w) in zip(offs, src_sizes):
-            if o < 0 or o + h * w * c > buf.numel():
-                raise _lib.SketchEditB200Error("%s slice [%d, %d) outside the %d-byte buffer" % (nm, o, o + h * w * c, buf.numel()))
-    for o, p, (y, x), (h, w) in zip(canvas_offsets, canvas_pitches, box_offsets, box_sizes):
-        end = o + (y + h - 1) * p + (x + w) * 3
-        if o < 0 or y < 0 or x < 0 or p < (x + w) * 3 or end > canvas.numel():
-            raise _lib.SketchEditB200Error("box (%d, %d) of %dx%d in the canvas at %d (pitch %d) is outside the %d-byte canvas"
-                                           % (y, x, h, w, o, p, canvas.numel()))
+    _check_windows("rgb", rgb, rgb_offsets, [3 * w for _, w in src_sizes], src_sizes, 3)
+    _check_windows("mask", mask, mask_offsets, [w for _, w in src_sizes], src_sizes, 1)
+    for i, (y, x) in enumerate(box_offsets):
+        if y < 0 or x < 0:
+            raise _lib.SketchEditB200Error("box %d at (%d, %d) is outside the canvas" % (i, y, x))
+    # box i lies inside the window of its canvas's first y + h rows and first x + w pixels
+    _check_windows("box", canvas, canvas_offsets, canvas_pitches,
+                   [(y + h, x + w) for (y, x), (h, w) in zip(box_offsets, box_sizes)], 3)
     lib = _lib.load()
-    L, I = ctypes.c_longlong, ctypes.c_int
-    pairs = lambda v: (I * (2 * n))(*[a for hw in v for a in hw])
-    args = ((L * n)(*[int(o) for o in rgb_offsets]), (L * n)(*[int(o) for o in mask_offsets]), pairs(src_sizes),
-            (L * n)(*canvas_offsets), (L * n)(*canvas_pitches), pairs(box_offsets), pairs(box_sizes),
-            (I * (4 * n))(*[v for f in feather for v in f]) if feather is not None else None, n)
-    with torch.cuda.device(rgb.device):
-        need = L(0)
-        _lib.check(lib.se_resize_composite_feather_u8(None, args[0], None, args[1], args[2], None, args[3], args[4], args[5],
-                                                      args[6], args[7], n, int(bool(swap_rb)), None, ctypes.byref(need), None))
-        scratch = torch.empty(max(1, need.value), device=rgb.device, dtype=torch.uint8)
-        size = L(scratch.numel())
-        _lib.check(lib.se_resize_composite_feather_u8(_ptr(rgb), args[0], _ptr(mask), args[1], args[2], _ptr(canvas), args[3],
-                                                      args[4], args[5], args[6], args[7], n, int(bool(swap_rb)), _ptr(scratch),
-                                                      ctypes.byref(size), _stream()))
+    a = (_ptr(rgb), _longs(rgb_offsets), _ptr(mask), _longs(mask_offsets), _ints(src_sizes), _ptr(canvas), _longs(canvas_offsets),
+         _longs(canvas_pitches), _ints(box_offsets), _ints(box_sizes), _ints(feather) if feather is not None else None, n,
+         int(bool(swap_rb)))
+    # one call: the entry keeps the boxes' order across its launches
+    _run_chunks(n, max(n, 1), dev, lambda sl: lambda scratch, size, stream: lib.se_resize_composite_feather_u8(*a, scratch, size, stream))
     return canvas
 
 
@@ -531,20 +464,14 @@ def feather_u8_packed(buf, offsets, sizes, feather):
     n = len(sizes)
     if len(offsets) != n or len(feather) != n:
         raise _lib.SketchEditB200Error("offsets, sizes and feather must have the same length")
-    if not (isinstance(buf, torch.Tensor) and buf.is_cuda and buf.dtype == torch.uint8 and buf.is_contiguous()):
-        raise _lib.SketchEditB200Error("buf must be a contiguous CUDA uint8 tensor")
-    sizes = [(int(h), int(w)) for h, w in sizes]
-    offsets = [int(o) for o in offsets]
+    _chk_u8((buf, "buf"))
+    sizes, offsets = _hw(sizes), [int(o) for o in offsets]
     feather = [tuple(int(v) for v in f) for f in feather]
     if any(len(f) != 4 for f in feather):
         raise _lib.SketchEditB200Error("feather needs 4 widths (left, top, right, bottom) per image")
-    for o, (h, w) in zip(offsets, sizes):
-        if o < 0 or o + h * w > buf.numel():
-            raise _lib.SketchEditB200Error("image slice [%d, %d) outside the %d-byte buffer" % (o, o + h * w, buf.numel()))
-    L, I = ctypes.c_longlong, ctypes.c_int
+    _check_windows("image", buf, offsets, [w for _, w in sizes], sizes, 1)
     with torch.cuda.device(buf.device):
-        _lib.check(_lib.load().se_feather_u8(_ptr(buf), (L * max(n, 1))(*offsets), (I * max(2 * n, 1))(*[v for hw in sizes for v in hw]),
-                                             (I * max(4 * n, 1))(*[v for f in feather for v in f]), n, _stream()))
+        _lib.check(_lib.load().se_feather_u8(_ptr(buf), _longs(offsets), _ints(sizes), _ints(feather), n, _stream()))
     return buf
 
 
@@ -610,25 +537,14 @@ def _check_jpeg_args(quality, subsampling):
 def _jpeg_launch(ptrs, pitches, sizes, quality, subsampling, out, out_offsets, out_bytes):
     """se_jpeg_encode_u8 over windows already checked, JPEG_MAX_BATCH per call, on the current stream of out's device."""
     lib = _lib.load()
-    L, I, P = ctypes.c_longlong, ctypes.c_int, ctypes.c_void_p
-    n = len(sizes)
-    with torch.cuda.device(out.device):
-        chunks = []
-        for c0 in range(0, n, JPEG_MAX_BATCH):
-            sl = slice(c0, c0 + JPEG_MAX_BATCH)
-            k = len(sizes[sl])
-            args = ((P * k)(*ptrs[sl]), (L * k)(*pitches[sl]), (I * (2 * k))(*[v for hw in sizes[sl] for v in hw]), k,
-                    (L * k)(*out_offsets[sl]), c0)
-            need = L(0)
-            _lib.check(lib.se_jpeg_encode_u8(None, args[1], args[2], k, quality, subsampling, None, args[4], None, None,
-                                             ctypes.byref(need), None))
-            chunks.append((args, need.value))
-        scratch = torch.empty(max([1] + [b for _, b in chunks]), device=out.device, dtype=torch.uint8)
-        for a, _ in chunks:
-            size = L(scratch.numel())
-            _lib.check(lib.se_jpeg_encode_u8(a[0], a[1], a[2], a[3], quality, subsampling, _ptr(out), a[4],
-                                             ctypes.c_void_p(out_bytes.data_ptr() + 8 * a[5]), _ptr(scratch), ctypes.byref(size),
-                                             _stream()))
+
+    def chunk(sl):
+        k = len(ptrs[sl])
+        a = ((ctypes.c_void_p * k)(*ptrs[sl]), _longs(pitches[sl]), _ints(sizes[sl]), k, quality, subsampling, _ptr(out),
+             _longs(out_offsets[sl]), ctypes.c_void_p(out_bytes.data_ptr() + 8 * sl.start))
+        return lambda scratch, size, stream: lib.se_jpeg_encode_u8(*a, scratch, size, stream)
+
+    _run_chunks(len(sizes), JPEG_MAX_BATCH, out.device, chunk)
 
 
 def jpeg_encode_u8_packed(src, src_offsets, src_pitches, sizes, quality=75, subsampling=2, out=None, out_offsets=None):
@@ -643,40 +559,18 @@ def jpeg_encode_u8_packed(src, src_offsets, src_pitches, sizes, quality=75, subs
     srcs = list(src) if isinstance(src, (list, tuple)) else [src] * n
     if not (len(srcs) == len(src_offsets) == len(src_pitches) == n):
         raise _lib.SketchEditB200Error("src (as a list), src_offsets, src_pitches and sizes must have the same length")
-    for t in srcs + [out]:
-        if t is not None and not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
-            raise _lib.SketchEditB200Error("%s must be a contiguous CUDA uint8 tensor" % ("out" if t is out else "src"))
+    named = [(t, "src") for t in srcs] + ([(out, "out")] if out is not None else [])
+    _chk_u8(*named)
     if n == 0:
         return out, out_offsets, None
-    dev = srcs[0].device
-    if any(t.device != dev for t in srcs):
-        raise _lib.SketchEditB200Error("every src must be on one device")
-    sizes = [(int(h), int(w)) for h, w in sizes]
+    dev = _device(*named)
+    sizes = _hw(sizes)
     src_offsets, src_pitches = [int(o) for o in src_offsets], [int(p) for p in src_pitches]
-    for i, (t, o, p, (h, w)) in enumerate(zip(srcs, src_offsets, src_pitches, sizes)):
+    for i, (h, w) in enumerate(sizes):
         if not (1 <= h <= 65535 and 1 <= w <= 65535):
             raise _lib.SketchEditB200Error("window %d: sizes must be in [1, 65535], got %dx%d" % (i, h, w))
-        if p < 3 * w:
-            raise _lib.SketchEditB200Error("window %d: the pitch of %d bytes is narrower than its row of %d bytes" % (i, p, 3 * w))
-        if o < 0 or o + (h - 1) * p + 3 * w > t.numel():
-            raise _lib.SketchEditB200Error("window %d (%dx%d at %d, pitch %d) is outside the %d-byte src" % (i, h, w, o, p, t.numel()))
-    bound = [jpeg_max_bytes(h, w, subsampling) for h, w in sizes]
-    if out is None:
-        if out_offsets is not None:
-            raise _lib.SketchEditB200Error("out_offsets needs out")
-        out_offsets, total = [], 0
-        for b in bound:
-            out_offsets.append(total)
-            total += (b + 15) // 16 * 16
-        out = torch.empty(total, device=dev, dtype=torch.uint8)
-    elif out_offsets is None or len(out_offsets) != n:
-        raise _lib.SketchEditB200Error("out needs one out_offsets entry per image")
-    if out.device != dev:
-        raise _lib.SketchEditB200Error("src on %s but out on %s" % (dev, out.device))
-    out_offsets = [int(o) for o in out_offsets]
-    for o, b in zip(out_offsets, bound):
-        if o < 0 or o + b > out.numel():
-            raise _lib.SketchEditB200Error("out slice [%d, %d) outside the %d-byte buffer" % (o, o + b, out.numel()))
+    _check_windows("window", srcs, src_offsets, src_pitches, sizes, 3)
+    out, out_offsets = _out(out, out_offsets, [jpeg_max_bytes(h, w, subsampling) for h, w in sizes], dev, "out_offsets")
     out_bytes = torch.empty(n, device=dev, dtype=torch.int64)
     _jpeg_launch([t.data_ptr() + o for t, o in zip(srcs, src_offsets)], src_pitches, sizes, quality, subsampling, out,
                  out_offsets, out_bytes)
@@ -706,15 +600,9 @@ def jpeg_encode_u8(images, quality=75, subsampling=2):
                                            % (t.stride(),))
         if not (1 <= t.shape[0] <= 65535 and 1 <= t.shape[1] <= 65535):
             raise _lib.SketchEditB200Error("image sizes must be in [1, 65535], got %dx%d" % tuple(t.shape[:2]))
-    dev = images[0].device
-    if any(t.device != dev for t in images):
-        raise _lib.SketchEditB200Error("every image must be on one device")
+    dev = _device(*[(t, "image") for t in images])
     sizes = [(int(t.shape[0]), int(t.shape[1])) for t in images]
-    offs, total = [], 0
-    for h, w in sizes:
-        offs.append(total)
-        total += (jpeg_max_bytes(h, w, subsampling) + 15) // 16 * 16
-    out = torch.empty(total, device=dev, dtype=torch.uint8)
+    out, offs = _out(None, None, [jpeg_max_bytes(h, w, subsampling) for h, w in sizes], dev, "out_offsets")
     out_bytes = torch.empty(len(images), device=dev, dtype=torch.int64)
     _jpeg_launch([t.data_ptr() for t in images], [t.stride(0) for t in images], sizes, quality, subsampling, out, offs, out_bytes)
     with torch.cuda.device(dev):

@@ -326,14 +326,6 @@ def _overlap_sets(boxes):
     return list(sets.values())
 
 
-def _aligned_offsets(nbytes, align=16):
-    offs, total = [], 0
-    for n in nbytes:
-        offs.append(total)
-        total += (n + align - 1) // align * align
-    return offs, total
-
-
 class DemoProcessor:
     """``process_image`` of the reference demo (demo.py:39-73) on the batched uint8 forward.
 
@@ -406,7 +398,7 @@ class DemoProcessor:
         if key[0] == "region":
             return self._run_region_device(key, payloads)
         torch = self._torch
-        from .engine import resize_u8_packed, resize_window_u8_packed
+        from .engine import _aligned_offsets, resize_u8_packed, resize_window_u8_packed
         H, W = key[:2]
         edit = len(key) > 2
         B = len(payloads)
@@ -477,7 +469,8 @@ class DemoProcessor:
         its photo ([h,w,3] on the device), snapshotted and pasted into it, and its result is (that list, [previous bytes of
         each box])."""
         torch = self._torch
-        from .engine import feather_u8_packed, resize_composite_u8_packed, resize_u8_packed, resize_window_u8_packed
+        from .engine import (_aligned_offsets, feather_u8_packed, resize_composite_u8_packed, resize_u8_packed,
+                             resize_window_u8_packed)
         H, W = key[1:3]
         edit = key[-1] is True
         dev = self.engine.device

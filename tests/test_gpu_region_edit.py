@@ -1,5 +1,5 @@
-"""Region edits on the GPU: se_resize_paste_u8 (engine.resize_paste_u8_packed) reproduces Pillow's resize-and-paste bit for
-bit in ragged batches and writes nothing outside its destination slices, and the device flow of
+"""Region edits on the GPU: the composite with one box per canvas (engine.resize_composite_u8_packed) reproduces Pillow's
+resize-and-paste bit for bit in ragged batches and writes nothing outside its destination slices, and the device flow of
 DemoProcessor.process_image(..., region=...) returns exactly the Pillow flow's bytes."""
 import threading
 
@@ -66,7 +66,7 @@ def _pack(arrays, align, start, fill):
 def test_paste_matches_pillow_and_keeps_to_its_slices(lib, swap_rb, in_place, aligned):
     import torch
 
-    from sketchedit_b200.engine import resize_paste_u8_packed
+    from sketchedit_b200.engine import resize_composite_u8_packed
     data = [_inputs(s, d, seed=400 + i) for i, (s, d) in enumerate(CASES)]
     rgb, rgb_offs = _pack([x[0] for x in data], aligned, 0 if aligned else 3, 0)
     msk, msk_offs = _pack([x[1] for x in data], aligned, 0 if aligned else 1, 0)
@@ -74,11 +74,14 @@ def test_paste_matches_pillow_and_keeps_to_its_slices(lib, swap_rb, in_place, al
     dev = {k: torch.from_numpy(v).cuda() for k, v in (("rgb", rgb), ("mask", msk), ("base", base))}
     if in_place:
         out, dst_offs = dev["base"], base_offs
-    else:
+    else:                                   # a separate destination: each base copied to its slice, then pasted over there
         _, dst_offs = _pack([x[2] for x in data], aligned, 32 if aligned else 9, 0x5A)
         out = torch.full((dst_offs[-1] + data[-1][2].nbytes + 77,), 0x5A, dtype=torch.uint8, device="cuda")
-    resize_paste_u8_packed(dev["rgb"], rgb_offs, dev["mask"], msk_offs, [s for s, _ in CASES], dev["base"], base_offs,
-                           [d for _, d in CASES], swap_rb=swap_rb, out=out, dst_offsets=dst_offs)
+        for (_, _, b), bo, do in zip(data, base_offs, dst_offs):
+            out[do:do + b.nbytes].copy_(dev["base"][bo:bo + b.nbytes])
+    dst = [d for _, d in CASES]             # one box per canvas, filling it: at (0, 0), pitch 3 w
+    resize_composite_u8_packed(dev["rgb"], rgb_offs, dev["mask"], msk_offs, [s for s, _ in CASES], out, dst_offs,
+                               [3 * w for _, w in dst], [(0, 0)] * len(dst), dst, swap_rb=swap_rb)
     o = out.cpu().numpy()
     inside = np.zeros(o.size, bool)
     for (s, d), (r, m, b), off in zip(CASES, data, dst_offs):
@@ -95,19 +98,20 @@ def test_paste_matches_pillow_and_keeps_to_its_slices(lib, swap_rb, in_place, al
 
 @pytest.mark.gpu
 def test_paste_splits_long_batches(lib):
-    """More than RESIZE_MAX_BATCH images: the wrapper runs them in chunks with one scratch allocation."""
+    """More than 32 canvases of one box each: the composite runs them in several launches with one scratch allocation."""
     import torch
 
-    from sketchedit_b200.engine import resize_paste_u8_packed
+    from sketchedit_b200.engine import resize_composite_u8_packed
     cases = [((32, 40), (50 + i, 29 + 2 * i)) for i in range(37)]
     data = [_inputs(s, d, seed=700 + i) for i, (s, d) in enumerate(cases)]
     rgb, ro = _pack([x[0] for x in data], True, 0, 0)
     msk, mo = _pack([x[1] for x in data], True, 0, 0)
     base, bo = _pack([x[2] for x in data], True, 0, 0)
-    out, offs = resize_paste_u8_packed(torch.from_numpy(rgb).cuda(), ro, torch.from_numpy(msk).cuda(), mo, [s for s, _ in cases],
-                                       torch.from_numpy(base).cuda(), bo, [d for _, d in cases], swap_rb=True)
+    out = torch.from_numpy(base).cuda()
+    resize_composite_u8_packed(torch.from_numpy(rgb).cuda(), ro, torch.from_numpy(msk).cuda(), mo, [s for s, _ in cases], out, bo,
+                               [3 * d[1] for _, d in cases], [(0, 0)] * len(cases), [d for _, d in cases], swap_rb=True)
     o = out.cpu().numpy()
-    for (r, m, b), off in zip(data, offs):
+    for (r, m, b), off in zip(data, bo):
         assert np.array_equal(o[off:off + b.nbytes], _pillow(r, m, b, True).reshape(-1))
 
 

@@ -1,7 +1,6 @@
 """Feathered region pastes on the GPU: se_resize_composite_feather_u8 and se_feather_u8 against the numpy statement bit for bit
-(with guard bytes), zero widths and NULL against se_resize_composite_u8, and the device flows of DemoProcessor.process_image
+(with guard bytes), zero widths against NULL widths, and the device flows of DemoProcessor.process_image
 and EditSession.edit with feather > 0 against the Pillow flows."""
-import ctypes
 import gc
 import threading
 
@@ -66,35 +65,20 @@ def _canvas_buffer(canvases, aligned, seed):
     return imgs, offs, pitches, buf
 
 
-def _composite(canvases, boxes, feather, swap, aligned, seed, entry="feather"):
-    """Runs one composite over canvases packed with guard bytes between rows and around them. entry: 'feather'
-    (engine.resize_composite_u8_packed with feather), or 'plain' (se_resize_composite_u8 called directly). Returns
-    (device bytes, canvases, offsets, pitches, results)."""
+def _composite(canvases, boxes, feather, swap, aligned, seed):
+    """Runs one composite (engine.resize_composite_u8_packed) over canvases packed with guard bytes between rows and around
+    them. Returns (device bytes, canvases, offsets, pitches, results)."""
     import torch
 
-    from sketchedit_b200.engine import _ptr, _stream, resize_composite_u8_packed
+    from sketchedit_b200.engine import resize_composite_u8_packed
     imgs, offs, pitches, buf = _canvas_buffer(canvases, aligned, seed)
     results = [_result(src, seed + 1 + i) for i, (_, _, _, src) in enumerate(boxes)]
     rgb, ro = _pack([r for r, _ in results], aligned, 0 if aligned else 3)
     msk, mo = _pack([m for _, m in results], aligned, 0 if aligned else 1)
     dev, rgb_d, msk_d = torch.from_numpy(buf).cuda(), torch.from_numpy(rgb).cuda(), torch.from_numpy(msk).cuda()
-    args = ([b[3] for b in boxes], [offs[b[0]] for b in boxes], [pitches[b[0]] for b in boxes], [b[1] for b in boxes],
-            [b[2] for b in boxes])
-    if entry == "feather":
-        resize_composite_u8_packed(rgb_d, ro, msk_d, mo, args[0], dev, *args[1:], swap_rb=swap, feather=feather)
-    else:
-        lib = _lib.load()
-        n = len(boxes)
-        L, I = ctypes.c_longlong, ctypes.c_int
-        pairs = lambda v: (I * (2 * n))(*[a for hw in v for a in hw])
-        a = ((L * n)(*ro), (L * n)(*mo), pairs(args[0]), (L * n)(*args[1]), (L * n)(*args[2]), pairs(args[3]), pairs(args[4]))
-        need = L(0)
-        assert lib.se_resize_composite_u8(None, a[0], None, a[1], a[2], None, a[3], a[4], a[5], a[6], n, int(swap), None,
-                                          ctypes.byref(need), None) == 0
-        scratch = torch.empty(max(1, need.value), device="cuda", dtype=torch.uint8)
-        size = L(scratch.numel())
-        _lib.check(lib.se_resize_composite_u8(_ptr(rgb_d), a[0], _ptr(msk_d), a[1], a[2], _ptr(dev), a[3], a[4], a[5], a[6], n,
-                                              int(swap), _ptr(scratch), ctypes.byref(size), _stream()))
+    resize_composite_u8_packed(rgb_d, ro, msk_d, mo, [b[3] for b in boxes], dev, [offs[b[0]] for b in boxes],
+                               [pitches[b[0]] for b in boxes], [b[1] for b in boxes], [b[2] for b in boxes], swap_rb=swap,
+                               feather=feather)
     return dev.cpu().numpy(), imgs, offs, pitches, results
 
 
@@ -147,12 +131,10 @@ def test_feathered_composite_past_one_launch(lib):
 @pytest.mark.gpu
 @pytest.mark.parametrize("aligned", [True, False])
 def test_zero_widths_and_null_are_the_plain_composite(lib, aligned):
-    zeros = [(0, 0, 0, 0)] * len(BOXES)
-    plain = _composite(CANVASES, BOXES, None, True, aligned, seed=41, entry="plain")
+    plain = _composite(CANVASES, BOXES, None, True, aligned, seed=41)              # feather == NULL
     _check_statement(plain[0], *plain[1:4], BOXES, plain[4], None, True)
-    for f in (None, zeros):
-        got = _composite(CANVASES, BOXES, f, True, aligned, seed=41)[0]
-        assert np.array_equal(got, plain[0])
+    got = _composite(CANVASES, BOXES, [(0, 0, 0, 0)] * len(BOXES), True, aligned, seed=41)[0]
+    assert np.array_equal(got, plain[0])
 
 
 @pytest.mark.gpu

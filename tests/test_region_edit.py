@@ -1,11 +1,7 @@
-"""Region edits (DemoProcessor.process_image(..., region=...), se_resize_paste_u8) on the CPU: the box rule of
-serving.region_box, the validation of region requests, the paste blend against Image.paste on every byte triple, and the host
-checks of se_resize_paste_u8."""
+"""Region edits (DemoProcessor.process_image(..., region=...)) on the CPU: the box rule of serving.region_box, the validation
+of region requests, the paste blend against Image.paste on every byte triple, and the host checks of the one-box-per-canvas
+paste of se_resize_composite_feather_u8."""
 import ctypes
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -141,7 +137,7 @@ def test_div255_blend_equals_image_paste_on_every_byte_triple():
         assert np.array_equal(got, want), (b0, int((got != want).any(axis=-1).sum()))
 
 
-# ------------------------------------------------------------------------------------------ se_resize_paste_u8 on the host
+# ------------------------------------------------------------------------------------------ one box per canvas on the host
 @pytest.fixture(scope="module")
 def lib():
     build.build(verbose=False)
@@ -149,11 +145,15 @@ def lib():
 
 
 def _query(lib, src, dst, n=1, scratch=None, scratch_bytes=0, off=0):
+    """se_resize_composite_feather_u8 with n boxes, each filling its own canvas (at (0, 0), pitch 3 w), no feather."""
     k = max(n, 1)
-    offs = (ctypes.c_longlong * k)(*([off] * k))
-    shw, dhw = (ctypes.c_int * (2 * k))(*(src * k)), (ctypes.c_int * (2 * k))(*(dst * k))
-    need = ctypes.c_longlong(scratch_bytes)
-    rc = lib.se_resize_paste_u8(None, offs, None, offs, shw, None, offs, None, offs, dhw, n, 1, scratch, ctypes.byref(need), None)
+    L, I = ctypes.c_longlong, ctypes.c_int
+    offs = (L * k)(*([off] * k))
+    coff, pitches = (L * k)(*range(off, off + 10 ** 6 * k, 10 ** 6)), (L * k)(*([3 * dst[1]] * k))
+    shw, dhw, yx = (I * (2 * k))(*(src * k)), (I * (2 * k))(*(dst * k)), (I * (2 * k))(*([0, 0] * k))
+    need = L(scratch_bytes)
+    rc = lib.se_resize_composite_feather_u8(None, offs, None, offs, shw, None, coff, pitches, yx, dhw, None, n, 1, scratch,
+                                            ctypes.byref(need), None)
     return rc, need.value, lib.se_last_error().decode()
 
 
@@ -163,13 +163,13 @@ def test_paste_scratch_query(lib):
     assert _query(lib, (256, 256), (608, 256))[:2] == (0, 0)           # width unchanged: the paste reads the result itself
     assert _query(lib, (256, 256), (256, 256))[:2] == (0, 0)
     assert _query(lib, (256, 256), (100, 77), n=3)[:2] == (0, 3 * (r256(256 * 77 * 3) + r256(256 * 77)))
+    assert _query(lib, (256, 256), (100, 77), n=33)[:2] == (0, 33 * (r256(256 * 77 * 3) + r256(256 * 77)))   # no batch bound
     assert _query(lib, (256, 256), (100, 77), n=0)[:2] == (0, 0)
 
 
 def test_paste_validates_on_the_host_with_the_resize_messages(lib):
     cases = [
-        (dict(src=(256, 256), dst=(64, 64), n=33), "images per call"),
-        (dict(src=(256, 256), dst=(64, 64), n=-1), "images per call"),
+        (dict(src=(256, 256), dst=(64, 64), n=-1), "n must be >= 0 boxes"),
         (dict(src=(0, 256), dst=(64, 64)), "sizes must be in [1, 65535]"),
         (dict(src=(256, 256), dst=(64, 65536)), "sizes must be in [1, 65535]"),
         (dict(src=(8, 60000), dst=(8, 1)), "downscale factor too large"),
@@ -179,42 +179,16 @@ def test_paste_validates_on_the_host_with_the_resize_messages(lib):
     for kw, msg in cases:
         rc, _, err = _query(lib, **kw)
         assert rc != 0 and msg in err, (kw, err)
-    # the shared checks say what se_resize_u8 says
+    # the shared checks say what the window resize says
     need = ctypes.c_longlong(0)
     off, hw = (ctypes.c_longlong * 1)(0), (ctypes.c_int * 2)(0, 256)
-    assert lib.se_resize_u8(None, off, hw, None, off, (ctypes.c_int * 2)(64, 64), 1, 3, 0, None, ctypes.byref(need), None) != 0
+    assert lib.se_resize_window_u8(None, (ctypes.c_longlong * 1)(768), hw, None, off, (ctypes.c_int * 2)(64, 64), 1, 3, 0, None,
+                                   ctypes.byref(need), None) != 0
     assert _query(lib, (0, 256), (64, 64))[2].split(" : ")[-1].split(" at ")[0] == \
         lib.se_last_error().decode().split(" : ")[-1].split(" at ")[0]
     hw = (ctypes.c_int * 2)(64, 64)
-    assert lib.se_resize_paste_u8(None, None, None, None, hw, None, None, None, None, hw, 1, 0, None, ctypes.byref(need), None) != 0
+    assert lib.se_resize_composite_feather_u8(None, None, None, None, hw, None, None, None, None, hw, None, 1, 0, None,
+                                              ctypes.byref(need), None) != 0
     assert "null size / offset array" in lib.se_last_error().decode()
-    assert lib.se_resize_paste_u8(None, None, None, None, None, None, None, None, None, None, 0, 0, None, None, None) != 0
-
-
-def _nvcc():
-    try:
-        nvcc = build._nvcc()
-    except RuntimeError:
-        return None
-    return nvcc if os.path.isabs(nvcc) or shutil.which(nvcc) else None
-
-
-@pytest.mark.skipif(_nvcc() is None, reason="nvcc not available")
-def test_resize_kernels_do_not_spill(tmp_path):
-    """se_resize.cu for sm_90a with the library's flags: paste_v_kernel and the resize passes keep everything in registers."""
-    flags = [f for f in build.NVCC_FLAGS if not f.startswith("--use_fast_math")]   # as build.build() compiles
-    cmd = [_nvcc()] + flags + ["-Xptxas", "-v", "-c", os.path.join(build.CSRC, "se_resize.cu"), "-o", str(tmp_path / "r.o")]
-    out = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert out.returncode == 0, out.stdout
-    spills, fn = {}, None
-    for line in out.stdout.splitlines():
-        m = re.search(r"Compiling entry function '(\w+)'", line)
-        if m:
-            fn = m.group(1)
-            continue
-        m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and fn:
-            spills[fn] = int(m.group(1)) + int(m.group(2))
-            fn = None
-    assert any("paste_v_kernel" in k for k in spills) and len(spills) == 4, out.stdout[-2000:]
-    assert not [k for k, n in spills.items() if n], spills
+    assert lib.se_resize_composite_feather_u8(None, None, None, None, None, None, None, None, None, None, None, 0, 0, None, None,
+                                              None) != 0

@@ -1,10 +1,7 @@
 """Several regions per request on the CPU: the grouping rule of serving.region_groups (region="strokes"), the validation of box
 lists, the host flow of DemoProcessor against the Pillow statement with a fake forward, and the host checks of
-se_resize_composite_u8."""
+se_resize_composite_feather_u8 without feather widths."""
 import ctypes
-import os
-import re
-import subprocess
 from collections import deque
 
 import numpy as np
@@ -271,7 +268,7 @@ def test_host_flow_strokes_uses_the_groups(fake):
     assert fake.batcher.batches[-1] == (("region", 64, 48), 1)         # a request's boxes run in one forward
 
 
-# ------------------------------------------------------------------------------------------ se_resize_composite_u8 on the host
+# ------------------------------------------------------------------------------------------ the composite on the host
 @pytest.fixture(scope="module")
 def lib():
     build.build(verbose=False)
@@ -286,7 +283,8 @@ def _query(lib, src, dst, n=1, yx=(0, 0), pitch=None, canvas_off=None, scratch=N
     pitches = (L * k)(*(pitch if isinstance(pitch, list) else [pitch if pitch is not None else 3 * (yx[1] + dst[1])] * k))
     shw, dhw, byx = (I * (2 * k))(*(src * k)), (I * (2 * k))(*(dst * k)), (I * (2 * k))(*(yx * k))
     need = L(scratch_bytes)
-    rc = lib.se_resize_composite_u8(None, offs, None, offs, shw, None, coff, pitches, byx, dhw, n, 1, scratch, ctypes.byref(need), None)
+    rc = lib.se_resize_composite_feather_u8(None, offs, None, offs, shw, None, coff, pitches, byx, dhw, None, n, 1, scratch,
+                                            ctypes.byref(need), None)
     return rc, need.value, lib.se_last_error().decode()
 
 
@@ -316,31 +314,11 @@ def test_composite_validates_on_the_host(lib):
         assert rc != 0 and msg in err, (kw, err)
     need = ctypes.c_longlong(0)
     off, hw = (ctypes.c_longlong * 1)(0), (ctypes.c_int * 2)(0, 256)
-    assert lib.se_resize_u8(None, off, hw, None, off, (ctypes.c_int * 2)(64, 64), 1, 3, 0, None, ctypes.byref(need), None) != 0
+    assert lib.se_resize_window_u8(None, (ctypes.c_longlong * 1)(768), hw, None, off, (ctypes.c_int * 2)(64, 64), 1, 3, 0, None,
+                                   ctypes.byref(need), None) != 0
     assert _query(lib, (0, 256), (64, 64))[2].split(" : ")[-1].split(" at ")[0] == \
-        lib.se_last_error().decode().split(" : ")[-1].split(" at ")[0]        # the shared checks say what se_resize_u8 says
+        lib.se_last_error().decode().split(" : ")[-1].split(" at ")[0]        # the shared checks say what the window resize says
     hw = (ctypes.c_int * 2)(64, 64)
-    assert lib.se_resize_composite_u8(None, None, None, None, hw, None, None, None, None, hw, 1, 0, None, ctypes.byref(need),
-                                      None) != 0
+    assert lib.se_resize_composite_feather_u8(None, None, None, None, hw, None, None, None, None, hw, None, 1, 0, None,
+                                              ctypes.byref(need), None) != 0
     assert "null size / offset array" in lib.se_last_error().decode()
-
-
-def test_paste_kernel_is_the_composite_kernel_and_does_not_spill(tmp_path):
-    """One paste kernel serves both entry points; compiled for sm_90a with the library's flags it keeps everything in
-    registers."""
-    try:
-        nvcc = build._nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc not available")
-    if not os.path.exists(nvcc) and not any(os.access(os.path.join(p, nvcc), os.X_OK) for p in os.environ["PATH"].split(":")):
-        pytest.skip("nvcc not available")
-    flags = [f for f in build.NVCC_FLAGS if not f.startswith("--use_fast_math")]
-    cmd = [nvcc] + flags + ["-Xptxas", "-v", "-c", os.path.join(build.CSRC, "se_resize.cu"), "-o", str(tmp_path / "r.o")]
-    out = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert out.returncode == 0, out.stdout
-    lines = out.stdout.splitlines()
-    paste = [i for i, ln in enumerate(lines) if re.search(r"Compiling entry function '\w*paste_v_kernel\w*'", ln)]
-    assert len(paste) == 1 and "PasteList" in lines[paste[0]], out.stdout[-2000:]
-    stats = [re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", ln) for ln in lines[paste[0]:]]
-    m = next(s for s in stats if s)
-    assert m.groups() == ("0", "0", "0"), lines[paste[0]:paste[0] + 4]

@@ -4,6 +4,10 @@ CPU: the coefficient tables of se_resize_coeffs, run through the fixed-point pas
 for bit. GPU: the kernels reproduce Pillow in ragged batches, write nothing outside their destination slices, and the device
 resize flow of the demo returns exactly what the Pillow flow returns."""
 import ctypes
+import os
+import re
+import shutil
+import subprocess
 import threading
 
 import numpy as np
@@ -99,17 +103,52 @@ def test_coefficient_table_shape_and_errors(lib):
 
 def test_resize_call_validates_on_the_host(lib):
     need = ctypes.c_longlong(0)
-    hw = (ctypes.c_int * 2)(10, 10)
-    off = (ctypes.c_longlong * 1)(0)
-    assert lib.se_resize_u8(None, off, hw, None, off, hw, 1, 2, 0, None, ctypes.byref(need), None) != 0      # channels
-    assert lib.se_resize_u8(None, off, hw, None, off, hw, 1, 1, 1, None, ctypes.byref(need), None) != 0      # swap_rb on 1 channel
-    assert lib.se_resize_u8(None, off, hw, None, off, hw, 33, 3, 0, None, ctypes.byref(need), None) != 0     # batch bound
+    L = ctypes.c_longlong
+    hw = (ctypes.c_int * 66)(*([10] * 66))
+    off, pitch = (L * 33)(*([0] * 33)), lambda c: (L * 33)(*([10 * c] * 33))       # packed rows: pitch w * channels
+    assert lib.se_resize_window_u8(None, pitch(2), hw, None, off, hw, 1, 2, 0, None, ctypes.byref(need), None) != 0      # channels
+    assert lib.se_resize_window_u8(None, pitch(1), hw, None, off, hw, 1, 1, 1, None, ctypes.byref(need), None) != 0      # swap_rb, 1 ch
+    assert lib.se_resize_window_u8(None, pitch(3), hw, None, off, hw, 33, 3, 0, None, ctypes.byref(need), None) != 0     # batch bound
     src_hw, dst_hw = (ctypes.c_int * 2)(75, 100), (ctypes.c_int * 2)(72, 96)
-    assert lib.se_resize_u8(None, off, src_hw, None, off, dst_hw, 1, 3, 0, None, ctypes.byref(need), None) == 0
+    src_pitch = (L * 1)(300)
+    assert lib.se_resize_window_u8(None, src_pitch, src_hw, None, off, dst_hw, 1, 3, 0, None, ctypes.byref(need), None) == 0
     assert need.value >= 75 * 96 * 3                                                                          # the intermediate
-    assert lib.se_resize_u8(None, off, src_hw, None, off, (ctypes.c_int * 2)(75, 96), 1, 3, 0, None, ctypes.byref(need), None) == 0
+    assert lib.se_resize_window_u8(None, src_pitch, src_hw, None, off, (ctypes.c_int * 2)(75, 96), 1, 3, 0, None, ctypes.byref(need),
+                                   None) == 0
     assert need.value == 0                                                                                    # one axis: no scratch
     assert lib.se_resize_set_table_cache_limit(-1) != 0 and lib.se_resize_set_table_cache_limit(0) == 0
+
+
+def test_resize_kernels_do_not_spill(tmp_path):
+    """Every kernel of se_resize.cu, compiled for sm_90a with the library's flags, keeps everything in registers: the two
+    horizontal passes, the vertical pass, feather_kernel, and one paste_v_kernel taking PasteList that runs every paste,
+    feathered or not."""
+    try:
+        nvcc = build._nvcc()
+    except RuntimeError:
+        pytest.skip("nvcc not available")
+    if not (os.path.isabs(nvcc) and os.path.exists(nvcc)) and not shutil.which(nvcc):
+        pytest.skip("nvcc not available")
+    flags = [f for f in build.NVCC_FLAGS if not f.startswith("--use_fast_math")]   # as build.build() compiles
+    cmd = [nvcc] + flags + ["-Xptxas", "-v", "-c", os.path.join(build.CSRC, "se_resize.cu"), "-o", str(tmp_path / "r.o")]
+    out = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    assert out.returncode == 0, out.stdout[-3000:]
+    lines = out.stdout.splitlines()
+    entries = [i for i, ln in enumerate(lines) if re.search(r"Compiling entry function '\w+'", ln)]
+    names = [re.search(r"'(\w+)'", lines[i]).group(1) for i in entries]
+    count = lambda k: sum(k in n for n in names)
+    assert len(names) == 5 and count("resize_h_kernel") == 2 and count("resize_v_kernel") == 1, names
+    assert count("feather_kernel") == 1 and count("paste_v_kernel") == 1, names
+    regs = {}
+    for i, name in zip(entries, names):
+        m = next(s for s in (re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", ln)
+                             for ln in lines[i:]) if s)
+        assert m.groups() == ("0", "0", "0"), lines[i:i + 4]
+        regs[name] = int(next(s for s in (re.search(r"Used (\d+) registers", ln) for ln in lines[i:]) if s).group(1))
+    paste = next(n for n in names if "paste_v_kernel" in n)
+    assert "PasteList" in paste, names
+    # 256 threads per block: up to 80 registers keeps paste_v_kernel at 3 blocks per SM, as with the 77 it used before feathering
+    assert regs[paste] <= 80, regs
 
 
 # ---------------------------------------------------------------------------------------------------------------- GPU

@@ -6,7 +6,8 @@ For 1000x667 and 4000x2667 photos with the local sketch of tools/serving_bench.p
 reports three cases, alternated in one process: the whole photo, region='auto' at 256x256 and region='auto' at 512x512:
   - latency: median wall time of process_image from one thread (includes the batcher's max_wait_ms window);
   - throughput: requests/s of 16 threads submitting together (16 requests per thread, or 1 for whole 4000x2667 photos);
-  - the paste kernel alone (paste_v_kernel of se_resize_paste_u8) for a batch of 16 region results pasted into their boxes:
+  - the paste kernel alone (paste_v_kernel of se_resize_composite_feather_u8, one box per canvas) for a batch of 16 region
+    results pasted into their boxes:
     its device time from a separate torch.profiler run, the bytes it moves (the result and mask rows it reads once, the base
     it reads and the patch it writes) and that rate over the H100 SXM data-sheet 3.35 TB/s.
 Prints the card's name and power limit with the numbers and one JSON line. Needs an H100; nothing is written to the tree.
@@ -46,7 +47,7 @@ def main():
 
     import torch
 
-    from sketchedit_b200.engine import resize_paste_u8_packed
+    from sketchedit_b200.engine import resize_composite_u8_packed
     from sketchedit_b200.serving import DemoProcessor, region_box
     assert torch.cuda.is_available(), "region_bench.py needs a GPU"
     name, power = card()
@@ -108,8 +109,8 @@ def main():
                 [i * bh * bw * 3 for i in range(B)]
 
             def paste():
-                resize_paste_u8_packed(res, ro, res, mo, [(Hn, Wn)] * B, base, bo, [(bh, bw)] * B, swap_rb=True, out=base,
-                                       dst_offsets=bo)
+                resize_composite_u8_packed(res, ro, res, mo, [(Hn, Wn)] * B, base, bo, [bw * 3] * B, [(0, 0)] * B, [(bh, bw)] * B,
+                                           swap_rb=True)
 
             iters = 50
             paste()
