@@ -103,6 +103,21 @@ int se_forward_with_mask_u8(se_model* m, const unsigned char* image_u8, const un
                             const unsigned char* edit_mask_u8, int B, int H, int W, int precision, unsigned char* bgr_u8,
                             void* stream);
 
+/* ---- previewing the edit mask (mask revising in two steps): netM's mask alone, then the forward on it.
+ * se_predict_mask_u8: se_forward_inference_u8's input codec, then netM's trunk and mask branch only (no image decoder, no
+ * netG): mask [B,1,H,W] receives netM's fp32 soft mask and mask_u8 [B,H,W] its bytes exactly as se_forward_inference_u8
+ * writes them. Either output may be NULL, not both. The soft mask is bit for bit the one netM computes inside
+ * se_forward_inference_u8 on the same bytes, in every precision and whatever the batch. */
+int se_predict_mask_u8(se_model* m, const unsigned char* image_u8, const unsigned char* sketch_u8, int B, int H, int W,
+                       int precision, float* mask, unsigned char* mask_u8, void* stream);
+/* se_forward_u8_with_soft_mask: se_forward_with_mask's forward on se_forward_inference_u8's codecs: uint8 image and sketch,
+ * an fp32 edit_mask [B,1,H,W] used as given (netG inpaints edit_mask > 0.5, the result is blended with edit_mask), bgr_u8
+ * [B,H,W,3]. netM does not run. Given the mask of se_predict_mask_u8, bgr_u8 is se_forward_inference_u8's bit for bit;
+ * unlike the mask_u8 bytes, which se_forward_with_mask_u8 decodes to a mask up to 1/255 off. NULL pointers are errors. */
+int se_forward_u8_with_soft_mask(se_model* m, const unsigned char* image_u8, const unsigned char* sketch_u8,
+                                 const float* edit_mask, int B, int H, int W, int precision, unsigned char* bgr_u8,
+                                 void* stream);
+
 /* ---- netM: replaces MDGenerator.forward(x, guide) -> (mask1, x_stage1)  (editline2_g.py:59-94) */
 int se_netM_forward(se_model* m, const float* x, const float* guide, int B, int H, int W, int precision, float* mask1,
                     float* x_stage1 /* may be NULL */, void* stream);

@@ -33,6 +33,9 @@ SIGNATURES = {
     "se_forward_with_mask": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_int, _c_void_p, _c_void_p,
                                       _c_void_p, _c_void_p, _c_void_p, _c_void_p]),
     "se_forward_with_mask_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_int, _c_void_p, _c_void_p]),
+    "se_predict_mask_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_int, _c_void_p, _c_void_p, _c_void_p]),
+    "se_forward_u8_with_soft_mask": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_int, _c_void_p,
+                                              _c_void_p]),
     "se_netM_forward": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_int, _c_void_p, _c_void_p,
                                  _c_void_p]),
     "se_netG_forward": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int,

@@ -1204,7 +1204,8 @@ static int run_generate(Ctx& c, int H, int W, const Request& r) {
   if (r.image_u8) {
     // input codec (reference data/testimage_dataset.py:89-103); the output codec is fused into the two heads (test.py:25-35):
     // the float image and masks live only in the workspace
-    img = c.get(3 * plane); sk = c.get(plane); soft = c.get(plane); mb = c.get(plane);
+    img = c.get(3 * plane); sk = c.get(plane); mb = c.get(plane);
+    if (!r.edit_mask) soft = c.get(plane);   // a caller's fp32 edit mask is blended as given: no soft plane to decode
     image = (const float*)img.p, sketch = (const float*)sk.p;
     c.tag(r.edit_mask_u8 ? "u8_to_inputs_kernel|input codec + edit mask" : "u8_to_inputs_kernel|input codec", 0, 0, 0,
           (double)c.B * H * W * (r.edit_mask_u8 ? 5 + 24 : 4 + 16));
@@ -1235,6 +1236,30 @@ static int run_generate(Ctx& c, int H, int W, const Request& r) {
   int rc = run_netG(c, H, W, g);
   if (rc) return rc;
   c.put(mb); c.put(soft); c.put(sk); c.put(img);
+  return 0;
+}
+
+// netM's mask alone on the input codec's bytes: the soft mask (caller's, or a workspace plane) and its bytes where set, from the
+// trunk and the mask branch; netM's image decoder and netG do not run. The same launches as netM's inside run_generate on a u8
+// request, so the mask is that forward's bit for bit. All fields are 8 bytes wide: they form the graph key.
+struct MaskRequest {
+  const unsigned char *image_u8 = nullptr, *sketch_u8 = nullptr;
+  float* mask = nullptr;
+  unsigned char* mask_u8 = nullptr;
+};
+
+static int run_predict_mask(Ctx& c, int H, int W, const MaskRequest& r) {
+  const size_t plane = (size_t)c.B * H * W * 4;
+  Buf img = c.get(3 * plane), sk = c.get(plane), soft;
+  if (!r.mask) soft = c.get(plane);
+  c.tag("u8_to_inputs_kernel|input codec", 0, 0, 0, (double)c.B * H * W * (4 + 16));
+  CK(u8_to_inputs(r.image_u8, r.sketch_u8, nullptr, (float*)img.p, (float*)sk.p, nullptr, nullptr, c.B, H, W, c.stream));
+  NetMIO nm{(const float*)img.p, (const float*)sk.p};
+  nm.mask = r.mask ? r.mask : (float*)soft.p;
+  nm.mask_u8 = r.mask_u8;
+  int rc = run_netM(c, H, W, nm);
+  if (rc) return rc;
+  c.put(soft); c.put(sk); c.put(img);
   return 0;
 }
 
@@ -1565,6 +1590,23 @@ int se_forward_with_mask_u8(se_model* m, const unsigned char* image_u8, const un
   SE_REQUIRE(image_u8 && sketch_u8 && edit_mask_u8 && bgr_u8, "null tensor");
   Request r;
   r.image_u8 = image_u8; r.sketch_u8 = sketch_u8; r.edit_mask_u8 = edit_mask_u8; r.bgr_u8 = bgr_u8;
+  return keyed_forward(m, precision, B, H, W, stream, 1, r, run_generate);
+}
+
+int se_predict_mask_u8(se_model* m, const unsigned char* image_u8, const unsigned char* sketch_u8, int B, int H, int W, int precision,
+                       float* mask, unsigned char* mask_u8, void* stream) {
+  SE_REQUIRE(image_u8 && sketch_u8, "null tensor");
+  SE_REQUIRE(mask || mask_u8, "se_predict_mask_u8 needs mask or mask_u8");
+  MaskRequest r;
+  r.image_u8 = image_u8; r.sketch_u8 = sketch_u8; r.mask = mask; r.mask_u8 = mask_u8;
+  return keyed_forward(m, precision, B, H, W, stream, 4, r, run_predict_mask);
+}
+
+int se_forward_u8_with_soft_mask(se_model* m, const unsigned char* image_u8, const unsigned char* sketch_u8, const float* edit_mask, int B,
+                                 int H, int W, int precision, unsigned char* bgr_u8, void* stream) {
+  SE_REQUIRE(image_u8 && sketch_u8 && edit_mask && bgr_u8, "null tensor");
+  Request r;
+  r.image_u8 = image_u8; r.sketch_u8 = sketch_u8; r.edit_mask = edit_mask; r.bgr_u8 = bgr_u8;
   return keyed_forward(m, precision, B, H, W, stream, 1, r, run_generate);
 }
 

@@ -194,6 +194,32 @@ class Engine:
                                                     _lib.PREC[precision], _ptr(bgr), _stream()))
         return bgr
 
+    def predict_mask_u8(self, image_u8, sketch_u8, precision="bf16", out=None):
+        """netM's edit mask alone, on ``inference_u8``'s input codec (``se_predict_mask_u8``; netG does not run): returns
+        (mask_f32 [B,1,H,W], mask_u8 [B,H,W]), the soft mask bit for bit as netM computes it inside ``inference_u8`` on the
+        same bytes, and its bytes as that call writes them. ``out=(mask_f32, mask_u8)`` writes into caller-owned CUDA
+        tensors (float32 and uint8)."""
+        B, H, W, (image_u8, sketch_u8), (mk,), _ = self._forward_tensors(
+            torch.uint8, (("image_u8", image_u8), ("sketch_u8", sketch_u8)), (1,), out[1] if out is not None else None)
+        soft = _f32(B, 1, H, W, like=mk) if out is None else _chk_out(out[0], (B, 1, H, W), "out[0]")
+        self._on_device(soft)
+        _lib.check(self.lib.se_predict_mask_u8(self.h, _ptr(image_u8), _ptr(sketch_u8), B, H, W, _lib.PREC[precision], _ptr(soft),
+                                               _ptr(mk), _stream()))
+        return soft, mk
+
+    def inference_u8_with_soft_mask(self, image_u8, sketch_u8, edit_mask, precision="bf16", out=None):
+        """``inference_u8`` on a caller's fp32 edit mask [B,1,H,W] (``se_forward_u8_with_soft_mask``; netM does not run):
+        netG inpaints edit_mask > 0.5 and the result is blended with edit_mask as given. Given the mask_f32 of
+        ``predict_mask_u8``, the returned bgr_u8 [B,H,W,3] is ``inference_u8``'s bit for bit. ``out``: a caller-owned
+        contiguous CUDA uint8 tensor of that shape."""
+        B, H, W, (image_u8, sketch_u8), (bgr,), _ = self._forward_tensors(
+            torch.uint8, (("image_u8", image_u8), ("sketch_u8", sketch_u8)), (3,), out)
+        _chk_out(edit_mask, (B, 1, H, W), "edit_mask")
+        self._on_device(edit_mask)
+        _lib.check(self.lib.se_forward_u8_with_soft_mask(self.h, _ptr(image_u8), _ptr(sketch_u8), _ptr(edit_mask), B, H, W,
+                                                         _lib.PREC[precision], _ptr(bgr), _stream()))
+        return bgr
+
     def netM(self, x, guide, precision="bf16", want_image=True):
         B, H, W, (x, guide), (mask1,), ex = self._forward_tensors(torch.float32, (("tensor", x), ("tensor", guide)), (1,), None,
                                                                   ("x_stage1",) if want_image else ())

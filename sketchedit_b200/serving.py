@@ -16,6 +16,9 @@ too (``engine.resize_u8_packed``, bit-identical to Pillow), so a batch is one up
     result_pil = proc.process_image(image_pil, mask_pil, region="auto", feather=16)     # paste fading over 16 px at inner edges
     s = proc.open_session(image_pil)                  # the photo stays on the device across edits
     r = s.edit(mask_pil, region="strokes")            # r.boxes, r.patches: what changed; s.undo() restores it
+    p = s.propose(mask_pil, region="strokes")         # p.boxes, p.masks: the edit's region, from netM alone
+    r = s.accept(p)                                   # that edit, byte for byte (or accept(p, edit_masks=corrections))
+    mask = proc.predict_mask(image_pil, mask_pil)     # process_image's returned mask, without the image
     proc.close()
 
 A region edit (``region=``) crops a box of the photo, runs the forward on it at ``DemoProcessor(region_size=...)`` and pastes
@@ -110,19 +113,23 @@ class RequestBatcher:
                         return
                     self._cv.wait(timeout=wait)
                     reqs, wait = self._take()
-            key = reqs[0].key
-            try:
-                results = self.run_batch(key, [r.payload for r in reqs])
-                if len(results) != len(reqs):
-                    raise RuntimeError("run_batch returned %d results for %d requests" % (len(results), len(reqs)))
-                for r, res in zip(reqs, results):
-                    r.result = res
-            except BaseException as e:      # noqa: BLE001 - delivered to every requester of this batch
-                for r in reqs:
-                    r.error = e
-            self.batches.append((key, len(reqs)))
+            self._dispatch(reqs)
+            reqs = None                     # the results belong to their requesters: device memory in them is not kept here
+
+    def _dispatch(self, reqs):
+        key = reqs[0].key
+        try:
+            results = self.run_batch(key, [r.payload for r in reqs])
+            if len(results) != len(reqs):
+                raise RuntimeError("run_batch returned %d results for %d requests" % (len(results), len(reqs)))
+            for r, res in zip(reqs, results):
+                r.result = res
+        except BaseException as e:      # noqa: BLE001 - delivered to every requester of this batch
             for r in reqs:
-                r.event.set()
+                r.error = e
+        self.batches.append((key, len(reqs)))
+        for r in reqs:
+            r.event.set()
 
 
 def floor8(n):
@@ -393,14 +400,18 @@ class DemoProcessor:
     def _run_batch_device(self, key, payloads):
         """payloads: (raw RGB photo [h,w,3] or None, raw 'L' mask [hm,wm], raw 'L' edit mask [he,we] or None, return_mask,
         session photo or None) at their own sizes; key: the floored network size, plus True when the batch runs on edit masks.
+        With SOFT in place of True (``EditSession.accept``) each payload ends with a proposal's fp32 soft masks [1,1,H,W] on
+        the device, which the batch runs on, and none returns a mask. A PREDICT key is ``_run_predict_device``'s.
         A session's photo ([h,w,3] on the device, with the raw photo None) is resized from where it lies, and the result is
         resized back into it after a snapshot of its previous bytes; its result is then (photo, mask, [snapshot])."""
+        if key[-1] == PREDICT:
+            return self._run_predict_device(key, payloads)
         if key[0] == "region":
             return self._run_region_device(key, payloads)
         torch = self._torch
         from .engine import _aligned_offsets, resize_u8_packed, resize_window_u8_packed
         H, W = key[:2]
-        edit = len(key) > 2
+        edit, soft = key[-1] is True, key[-1] == SOFT
         B = len(payloads)
         dev = self.engine.device
         sess = [p[4] for p in payloads]
@@ -437,6 +448,9 @@ class DemoProcessor:
                         resize_u8_packed(src, offs[np_ + B:], [a.shape[:2] for a in edits], [(H, W)] * B, 1, out=edt,
                                          dst_offsets=[i * H * W for i in range(B)])
                         bgr = self.engine.inference_with_mask_u8(img, msk, edt, precision=self.precision)
+                    elif soft:
+                        slab = self._soft_slab([p[5] for p in payloads], H, W)
+                        bgr = self.engine.inference_u8_with_soft_mask(img, msk, slab, precision=self.precision)
                     else:
                         bgr, mk = self.engine.inference_u8(img, msk, precision=self.precision)
                 # back to each photo's own size; the forward writes BGR, the demo keeps RGB
@@ -467,12 +481,14 @@ class DemoProcessor:
         (feathered as pasted) when asked for and predicted, else None. A box's feather widths follow from its place in the
         photo (``feather_widths``), wherever it is pasted. A session's request has no photo crops: its boxes are resized from
         its photo ([h,w,3] on the device), snapshotted and pasted into it, and its result is (that list, [previous bytes of
-        each box])."""
+        each box]). With SOFT in place of True (``EditSession.accept``) the edit-mask crops are a proposal's paste masks at
+        the working size [H,W], and the payload ends with its fp32 soft masks [k,1,H,W] on the device, which the forward runs
+        on; no mask is returned."""
         torch = self._torch
         from .engine import (_aligned_offsets, feather_u8_packed, resize_composite_u8_packed, resize_u8_packed,
                              resize_window_u8_packed)
         H, W = key[1:3]
-        edit = key[-1] is True
+        edit, soft = key[-1] is True, key[-1] == SOFT
         dev = self.engine.device
         items = [(r, j) for r, p in enumerate(payloads) for j in range(len(p[4]))]   # (request, box) per box
         B = len(items)
@@ -482,8 +498,8 @@ class DemoProcessor:
         plain = [i for i in range(B) if sess[i] is None]
         photos = {i: payloads[r][0][j] for i, (r, j) in enumerate(items) if sess[i] is None}
         masks = [payloads[r][1][j] for r, j in items]
-        edits = [payloads[r][2][j] for r, j in items] if edit else []
-        back = [i for i, (r, _) in enumerate(items) if payloads[r][3] and not edit]   # predicted masks to return
+        edits = [payloads[r][2][j] for r, j in items] if edit or soft else []
+        back = [i for i, (r, _) in enumerate(items) if payloads[r][3] and not edit and not soft]   # predicted masks to return
         fw = [feather_widths(boxes[i], payloads[r][7], payloads[r][6]) for i, (r, _) in enumerate(items)]
         # The work buffer: the plain requests' photo crops (uploaded; a box that overlaps no other box of its request is pasted
         # in place over its crop), the session boxes' patches, the predicted masks resized back (these three are the one
@@ -549,11 +565,16 @@ class DemoProcessor:
                 pitches = [sizes[i][1] * 3 if sess[i] is None else sess[i].shape[1] * 3 for i in range(B)]
                 resize_window_u8_packed(srcs, src_offs, pitches, sizes, [(H, W)] * B, 3, out=img, dst_offsets=net3)
                 resize_u8_packed(work, sk_at[:B], sizes, [(H, W)] * B, 1, out=msk, dst_offsets=net1)
+                pm_at = net1                          # the paste masks: pm at pm_at[i]
                 with torch.no_grad():
                     if edit:
                         pm = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
                         resize_u8_packed(work, sk_at[B:], sizes, [(H, W)] * B, 1, out=pm, dst_offsets=net1)
                         bgr = self.engine.inference_with_mask_u8(img, msk, pm, precision=self.precision)
+                    elif soft:                        # the proposal's mask bytes were uploaded at the working size
+                        pm, pm_at = work, sk_at[B:]
+                        slab = self._soft_slab([p[8] for p in payloads], H, W)
+                        bgr = self.engine.inference_u8_with_soft_mask(img, msk, slab, precision=self.precision)
                     else:
                         bgr, pm = self.engine.inference_u8(img, msk, precision=self.precision)
                 for i in range(B):
@@ -568,7 +589,7 @@ class DemoProcessor:
                     else:
                         place = [(0, sess[i].shape[1] * 3, boxes[i][1], boxes[i][0]) for i in g]
                         target = sess[g[0]].view(-1)
-                    resize_composite_u8_packed(bgr, [net3[i] for i in g], pm, [net1[i] for i in g], [(H, W)] * len(g), target,
+                    resize_composite_u8_packed(bgr, [net3[i] for i in g], pm, [pm_at[i] for i in g], [(H, W)] * len(g), target,
                                                [c[0] for c in place], [c[1] for c in place], [c[2:] for c in place],
                                                [sizes[i] for i in g], swap_rb=True,
                                                feather=[fw[i] for i in g] if any(any(fw[i]) for i in g) else None)
@@ -595,11 +616,101 @@ class DemoProcessor:
         return [(o, [snaps[i] for i in range(B) if items[i][0] == r]) if p[5] is not None else o
                 for r, (o, p) in enumerate(zip(out, payloads))]
 
+    def _run_predict_device(self, key, payloads):
+        """The mask-only forward of ``predict_mask`` and ``EditSession.propose``. payloads: (photo crops [bh,bw,3] or None,
+        sketch crops, boxes, session photo or None, feather, photo PIL size); key: the working size (the floored photo size, or
+        ("region", Hn, Wn)) and PREDICT. A whole-photo request is the one box (0, 0, w, h) with its sketch at its own size.
+        Each crop is resized to the working size like the edit's (a session's from its photo), and each box's predicted mask
+        is resized back to the box and feathered as the edit pastes it. Returns per request (fp32 soft masks [k,1,H,W] on the
+        device, mask bytes [k,H,W], [the box's paste mask [bh,bw] per box])."""
+        torch = self._torch
+        from .engine import _aligned_offsets, feather_u8_packed, resize_u8_packed, resize_window_u8_packed
+        H, W = key[-3:-1]
+        dev = self.engine.device
+        items = [(r, j) for r, p in enumerate(payloads) for j in range(len(p[2]))]
+        B = len(items)
+        boxes = [payloads[r][2][j] for r, j in items]
+        sizes = [(b[3] - b[1], b[2] - b[0]) for b in boxes]
+        sess = [payloads[r][3] for r, _ in items]
+        photos = [payloads[r][0][j] for r, j in items if payloads[r][3] is None]
+        sketches = [payloads[r][1][j] for r, j in items]
+        fw = [feather_widths(boxes[i], payloads[r][5], payloads[r][4]) for i, (r, _) in enumerate(items)]
+        offs, total = _aligned_offsets([a.nbytes for a in photos + sketches])
+        photo_at = iter(offs)
+        net3, net1 = [i * H * W * 3 for i in range(B)], [i * H * W for i in range(B)]
+        back, n_down = _aligned_offsets([B * H * W] + [h * w for h, w in sizes])   # the working-size bytes, then the masks
+        back = back[1:]
+        stage = self._staging("in", total)          # free: every batch, failed ones included, ends with a stream synchronise
+        host = stage.numpy()
+        for a, o in zip(photos + sketches, offs):
+            host[o:o + a.nbytes] = a.reshape(-1)
+        down = self._staging("out", n_down)
+        with torch.cuda.device(dev):
+            try:
+                src = stage[:total].to(dev, non_blocking=True)
+                img = torch.empty(B, H, W, 3, device=dev, dtype=torch.uint8)
+                msk = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
+                srcs = [src if t is None else t.view(-1) for t in sess]
+                src_offs = [next(photo_at) if t is None else (b[1] * t.shape[1] + b[0]) * 3 for t, b in zip(sess, boxes)]
+                pitches = [w * 3 if t is None else t.shape[1] * 3 for t, (_, w) in zip(sess, sizes)]
+                resize_window_u8_packed(srcs, src_offs, pitches, sizes, [(H, W)] * B, 3, out=img, dst_offsets=net3)
+                resize_u8_packed(src, offs[len(photos):], [a.shape[:2] for a in sketches], [(H, W)] * B, 1, out=msk,
+                                 dst_offsets=net1)
+                with torch.no_grad():
+                    soft, mk = self.engine.predict_mask_u8(img, msk, precision=self.precision)
+                res = torch.empty(n_down, device=dev, dtype=torch.uint8)
+                res[:B * H * W].copy_(mk.view(-1))
+                resize_u8_packed(mk, net1, [(H, W)] * B, sizes, 1, out=res, dst_offsets=back)
+                fb = [i for i in range(B) if any(fw[i])]
+                if fb:                                # the masks as pasted
+                    feather_u8_packed(res, [back[i] for i in fb], [sizes[i] for i in fb], [fw[i] for i in fb])
+                down[:n_down].copy_(res, non_blocking=True)
+                ends = np.cumsum([len(p[2]) for p in payloads]).tolist()
+                kept = [soft[e - len(p[2]):e].clone() for e, p in zip(ends, payloads)]   # each proposal holds its own
+            finally:
+                torch.cuda.current_stream().synchronize()
+        host = down.numpy()
+        work = host[:B * H * W].reshape(B, H, W)
+        masks = [host[o:o + h * w].reshape(h, w).copy() for o, (h, w) in zip(back, sizes)]
+        return [(k, work[e - len(p[2]):e].copy(), masks[e - len(p[2]):e]) for k, e, p in zip(kept, ends, payloads)]
+
+    def _soft_slab(self, softs, H, W):
+        """The requests' fp32 soft masks [k,1,H,W], in order, gathered into one [B,1,H,W] tensor by device copies."""
+        torch = self._torch
+        slab = torch.empty(sum(len(t) for t in softs), 1, H, W, device=self.engine.device, dtype=torch.float32)
+        at = 0
+        for t in softs:
+            slab[at:at + len(t)].copy_(t)
+            at += len(t)
+        return slab
+
+    def _run_masks_host(self, key, payloads):
+        """The host flow's PREDICT and SOFT batches. payloads: (photos [k,H,W,3], masks [k,H,W]), plus for SOFT the fp32 soft
+        masks [k,1,H,W] on the device. Results: PREDICT (soft masks [k,1,H,W] on the device, mask bytes [k,H,W]), SOFT
+        rgb [k,H,W,3]."""
+        torch = self._torch
+        dev = self.engine.device
+        ends = np.cumsum([len(p[0]) for p in payloads]).tolist()
+        with torch.cuda.device(dev):
+            img = torch.from_numpy(np.concatenate([p[0] for p in payloads])).to(dev, non_blocking=True)
+            msk = torch.from_numpy(np.concatenate([p[1] for p in payloads])).to(dev, non_blocking=True)
+            with torch.no_grad():
+                if key[-1] == PREDICT:
+                    soft, mk = self.engine.predict_mask_u8(img, msk, precision=self.precision)
+                    mk = mk.cpu().numpy()
+                    return [(soft[e - len(p[0]):e].clone(), mk[e - len(p[0]):e]) for e, p in zip(ends, payloads)]
+                bgr = self.engine.inference_u8_with_soft_mask(img, msk, self._soft_slab([p[2] for p in payloads], *msk.shape[1:]),
+                                                              precision=self.precision)
+            rgb = bgr.cpu().numpy()[..., ::-1]
+        return [np.ascontiguousarray(rgb[e - len(p[0]):e]) for e, p in zip(ends, payloads)]
+
     def _run_batch(self, key, payloads):
         """payloads: (photo [H,W,3], mask [H,W], edit mask [H,W] or None, return_mask) at the network size of ``key`` (the
         floored size), or for a region key (photos [k,H,W,3], masks [k,H,W], edit masks [k,H,W] or None, return_mask) with one
         item per box at the working size, and then each result is (rgb [k,H,W,3], mask [k,H,W] or None); True as the key's
-        last element: the batch runs on edit masks."""
+        last element: the batch runs on edit masks. PREDICT or SOFT there: ``_run_masks_host``."""
+        if key[-1] in (PREDICT, SOFT):
+            return self._run_masks_host(key, payloads)
         torch = self._torch
         join = np.concatenate if key[0] == "region" else np.stack
         img = torch.from_numpy(join([p[0] for p in payloads])).cuda(non_blocking=True)         # [B,H,W,3] RGB uint8
@@ -696,14 +807,68 @@ class DemoProcessor:
             return [_check_box(b, w, h) for b in region]
         return [_check_box(region, w, h)]
 
-    def _process_region(self, img, mask, edit_mask, return_mask, region, feather=0):
+    def predict_mask(self, img, mask, region=None, feather=0):
+        """The edit mask ``process_image(img, mask, region=region, return_mask=True, feather=feather)[1]`` returns, bit for
+        bit, from netM alone (``Engine.predict_mask_u8``): netG does not run and no image is made, for about a quarter of the
+        forward's arithmetic. Takes the arguments, and raises the errors, of ``process_image`` without an edit mask. Requests
+        share mask-only forwards with each other and with ``EditSession.propose``, never with edits."""
         from PIL import Image
+        feather = _check_feather(feather)
+        img = img.convert("RGB")
         w, h = img.size
+        if region is None:
+            if floor8(h) < 16 or floor8(w) < 16:
+                raise ValueError("image smaller than 16x16 (two stride-2 convolutions, 4x4 mask pool, stride-2 patch grid)")
+            if self.resize == "device" and mask.mode != "L":
+                raise ValueError("resize='device' takes an 'L' mask (got mode %r); resize='host' resizes it with Pillow" % mask.mode)
+            return self._predict(img, None, mask, [(0, 0, w, h)], True, 0, img.size, (0, 0))[2][0]
+        self._check_region_masks(img.size, mask, None)
+        boxes = self._region_boxes(img.size, mask, None, region)
+        return Image.fromarray(_union_mask(img.size, boxes, self._predict(img, None, mask, boxes, False, feather, img.size, (0, 0))[2]))
+
+    def _predict(self, img, photo, mask, boxes, whole, feather, size, offset):
+        """The mask-only forward of a request: ``(soft, work, masks, inputs)``. ``soft``: the fp32 soft masks [k,1,H,W] on the
+        engine's device, one per box at the working size; ``work``: their bytes [k,H,W] (the device flow's paste masks at
+        the working size); ``masks``: the 'L' paste mask per box at the box's size (feathered) or, ``whole``, at the photo's;
+        ``inputs``: what ``EditSession.accept`` submits again (the device flow: the sketch crops; the host flow: the resized
+        photo and sketch). The photo is the PIL ``img`` or, with the device flow of a session, ``photo`` on the device; the
+        mask lies at ``offset`` in a photo of PIL size ``size``."""
+        from PIL import Image
+        w, h = size
+        key = (floor8(h), floor8(w), PREDICT) if whole else ("region",) + self.region_size + (PREDICT,)
+        if self.resize == "device":
+            at = [(b[0] - offset[0], b[1] - offset[1], b[2] - offset[0], b[3] - offset[1]) for b in boxes]   # mask coordinates
+            sketches = [np.asarray(mask)] if whole else [np.asarray(mask.crop(b)) for b in at]
+            crops = None if photo is not None else [np.asarray(img)] if whole else [np.asarray(img.crop(b)) for b in boxes]
+            soft, work, mks = self.batcher.submit(key, (crops, sketches, boxes, photo, feather, size))
+            return soft, work, [Image.fromarray(m) for m in mks], sketches
+        if whole:
+            h_t, w_t = key[:2]
+            img_t = np.ascontiguousarray(np.array(img.resize((w_t, h_t))), dtype=np.uint8)[None]
+            mask_t = np.ascontiguousarray((np.array(mask.resize((w_t, h_t))) > 0).astype(np.uint8) * 255)[None]
+            soft, mk = self.batcher.submit(key, (img_t, mask_t))
+            return soft, mk, [Image.fromarray(mk[0]).resize(size)], (img_t, mask_t)
+        Hn, Wn = self.region_size
+        fm = _placed(mask, size, offset)
+        img_t = np.stack([np.array(img.crop(b).resize((Wn, Hn))) for b in boxes]).astype(np.uint8)
+        mask_t = np.stack([(np.array(fm.crop(b).resize((Wn, Hn))) > 0).astype(np.uint8) * 255 for b in boxes])
+        soft, mk = self.batcher.submit(key, (img_t, mask_t))
+        mks = [Image.fromarray(mk[i]).resize((b[2] - b[0], b[3] - b[1])) for i, b in enumerate(boxes)]
+        if feather:
+            mks = [Image.fromarray(feather_mask(m, feather_widths(b, size, feather))) for m, b in zip(mks, boxes)]
+        return soft, mk, mks, (img_t, mask_t)
+
+    def _check_region_masks(self, size, mask, edit_mask):
+        w, h = size
         for m, nm in ((mask, "mask"), (edit_mask, "edit_mask")):
-            if m is not None and m.size != img.size:
+            if m is not None and m.size != size:
                 raise ValueError("a region edit needs the %s at the photo's size %dx%d (got %dx%d)" % ((nm, w, h) + m.size))
             if self.resize == "device" and m is not None and m.mode != "L":
                 raise ValueError("resize='device' takes an 'L' %s (got mode %r); resize='host' resizes it with Pillow" % (nm, m.mode))
+
+    def _process_region(self, img, mask, edit_mask, return_mask, region, feather=0):
+        from PIL import Image
+        self._check_region_masks(img.size, mask, edit_mask)
         boxes = self._region_boxes(img.size, mask, edit_mask, region)
         if self.resize == "device":
             out = img.copy()
@@ -721,11 +886,7 @@ class DemoProcessor:
             return out
         if edit_mask is not None:
             return out, edit_mask
-        full = np.zeros((h, w), np.uint8)            # the largest paste mask over the boxes, 0 outside every box
-        for b, mk in zip(boxes, mks):
-            sub = full[b[1]:b[3], b[0]:b[2]]
-            np.maximum(sub, np.asarray(mk), out=sub)
-        return out, Image.fromarray(full)
+        return out, Image.fromarray(_union_mask(img.size, boxes, mks))
 
     def _region_key(self, edit_mask):
         # region requests on edit masks run their own forward, and region requests never share one with whole-photo requests
@@ -734,14 +895,16 @@ class DemoProcessor:
 
     def _region_host(self, img, mask, edit_mask, boxes, feather=0):
         """The Pillow flow of a region edit: ``(out, paste masks)``, one 'L' paste mask per box at the box's size (feathered
-        with ``feather_widths(box, img.size, feather)``)."""
+        with ``feather_widths(box, img.size, feather)``). ``edit_mask`` may also be a list of each box's edit mask."""
         from PIL import Image
         Hn, Wn = self.region_size
         sizes = [(b[2] - b[0], b[3] - b[1]) for b in boxes]
         out = img.copy()
         img_t = np.stack([np.array(img.crop(b).resize((Wn, Hn))) for b in boxes]).astype(np.uint8)
         mask_t = np.stack([(np.array(mask.crop(b).resize((Wn, Hn))) > 0).astype(np.uint8) * 255 for b in boxes])
-        edit_t = np.stack([np.array(edit_mask.convert("L").crop(b).resize((Wn, Hn))) for b in boxes]).astype(np.uint8) \
+        if edit_mask is not None:
+            ems = edit_mask if isinstance(edit_mask, list) else [edit_mask.convert("L").crop(b) for b in boxes]
+        edit_t = np.stack([np.array(e.convert("L").resize((Wn, Hn))) for e in ems]).astype(np.uint8) \
             if edit_mask is not None else None
         res, mk = self.batcher.submit(self._region_key(edit_mask), (img_t, mask_t, edit_t, True))
         mks = [Image.fromarray(edit_t[i] if edit_t is not None else mk[i]).resize(s) for i, s in enumerate(sizes)]
@@ -753,6 +916,20 @@ class DemoProcessor:
 
 
 EditResult = namedtuple("EditResult", ["boxes", "patches", "masks"])
+
+# last element of the batch keys of mask-only forwards (``predict_mask``, ``EditSession.propose``) and of forwards on a
+# proposal's fp32 soft masks (``EditSession.accept``): neither shares a forward with an edit
+PREDICT, SOFT = "predict", "soft"
+
+
+def _union_mask(size, boxes, mks):
+    """The largest of the boxes' paste masks at each pixel of a photo of PIL size ``size``, 0 outside every box, [h,w]."""
+    w, h = size
+    full = np.zeros((h, w), np.uint8)
+    for b, mk in zip(boxes, mks):
+        sub = full[b[1]:b[3], b[0]:b[2]]
+        np.maximum(sub, np.asarray(mk), out=sub)
+    return full
 
 
 def _placed(m, size, offset):
@@ -785,7 +962,11 @@ class EditSession:
 
     With ``resize='device'`` the photo lives on the engine's device: an edit uploads only the masks' box crops, resizes the
     photo's boxes where they lie (``engine.resize_window_u8_packed``), pastes the results into the photo and downloads only the
-    patches; undo snapshots stay on the device. With ``resize='host'`` the session holds a PIL image and runs the Pillow flow."""
+    patches; undo snapshots stay on the device. With ``resize='host'`` the session holds a PIL image and runs the Pillow flow.
+
+    ``propose(mask, ...)`` previews an edit: the boxes and paste masks ``edit`` would use, from netM alone. ``accept(p)`` then
+    runs that edit on netM's exact fp32 masks (the same bytes as ``edit``), or ``accept(p, edit_masks=...)`` on the user's
+    corrections. Any ``edit``, ``undo``, ``accept`` or ``close`` of the session invalidates its open proposals."""
 
     def __init__(self, proc, img, history_bytes):
         if int(history_bytes) < 0:
@@ -798,6 +979,7 @@ class EditSession:
         img = img.convert("RGB")
         self.size = img.size
         self._img = self._photo = None
+        self._proposals = set()         # open proposals, computed on the current photo
         if proc.resize == "host":
             self._img = img
         else:
@@ -815,6 +997,7 @@ class EditSession:
         """Releases the photo and the snapshots (idempotent); also run by ``DemoProcessor.close()``."""
         with self._mu:
             self._closed = True
+            self._drop_proposals()
             self._img = self._photo = None
             self._history.clear()
             self._held = 0
@@ -883,46 +1066,140 @@ class EditSession:
             raise ValueError("a %dx%d mask at offset (%d, %d) does not fit the %dx%d photo" % (mw, mh, ox, oy, w, h))
         return self._proc._region_boxes(self.size, mask, edit_mask, region, (ox, oy))
 
+    def _drop_proposals(self):
+        for p in self._proposals:
+            p._drop()
+        self._proposals.clear()
+
+    def propose(self, mask, region="auto", offset=(0, 0), feather=0):
+        """The edit ``edit(mask, region=region, offset=offset, feather=feather)`` would make, before it is made: returns a
+        ``Proposal`` whose ``boxes`` are that edit's boxes and whose ``masks`` are its paste masks (feathered as pasted),
+        bit for bit ``edit(..., return_mask=True).masks``, from netM alone (``Engine.predict_mask_u8``; netG does not run,
+        about a quarter of an edit's arithmetic). The photo does not change. The proposal holds each box's fp32 soft mask at
+        the working size on the engine's device (4 bytes per working pixel) until it is accepted, closed or invalidated.
+        Proposals share mask-only forwards with each other and with ``DemoProcessor.predict_mask``."""
+        feather = _check_feather(feather)
+        with self._mu:
+            self._check_open()
+            boxes = self._boxes(mask, None, region, offset)
+            off = tuple(int(v) for v in offset)
+            soft, work, masks, inputs = self._proc._predict(self._img, self._photo, mask, boxes, region is None, feather,
+                                                            self.size, off)
+            p = Proposal(self, boxes, masks, region is None, mask, off, feather, soft, work, inputs)
+            self._proposals.add(p)
+            return p
+
+    def accept(self, p, edit_masks=None, return_mask=False):
+        """Makes the edit of the open proposal ``p`` of this session and returns its ``EditResult``, like ``edit``.
+
+        ``edit_masks=None`` runs the forward on the proposal's fp32 soft masks (``Engine.inference_u8_with_soft_mask``; netM
+        does not run again): the photo, the result, ``undo`` and ``jpeg`` afterwards are bit for bit those of
+        ``edit(mask, region=p.boxes, offset=offset, feather=feather)``, which is the ``edit`` of the ``region`` given to
+        ``propose``; ``return_mask`` returns ``p.masks``. A list of one 'L' image per box, of the box's size, runs the edit
+        on those corrected masks: it is ``edit(mask, edit_mask=M, region=p.boxes, ...)`` whenever ``edit_masks[i]`` is
+        ``M``'s crop of box i. ``p.masks`` given back unchanged is not "no change": those bytes are feathered and truncated
+        (up to 1/255 off netM's mask, and pixels of soft mask in (0.5, 128/255) are no longer inpainted). No change is
+        ``edit_masks=None``.
+
+        The photo is not uploaded again: the device flow resizes the boxes again from the photo on the device, as ``edit``
+        does, which keeps a proposal at its soft masks alone; the host flow keeps the Pillow-resized inputs it uploaded.
+        The proposal is then closed, and so are the session's other proposals."""
+        from PIL import Image
+        if not isinstance(p, Proposal):
+            raise TypeError("accept takes a Proposal of this session, got %r" % (type(p).__name__,))
+        with self._mu:
+            self._check_open()
+            if p._session is not self:
+                raise ValueError("the proposal belongs to another session")
+            if p._soft is None:
+                raise RuntimeError("the proposal is closed: it was accepted or closed, or the photo changed since it was made")
+            if edit_masks is not None:
+                if not isinstance(edit_masks, (list, tuple)) or len(edit_masks) != len(p.boxes):
+                    raise ValueError("edit_masks must be None or a list of %d 'L' images, one per box" % len(p.boxes))
+                for i, (m, b) in enumerate(zip(edit_masks, p.boxes)):
+                    if getattr(m, "mode", None) != "L" or m.size != (b[2] - b[0], b[3] - b[1]):
+                        raise ValueError("edit_masks[%d] must be an 'L' image of its box's size %dx%d" % ((i, b[2] - b[0], b[3] - b[1])))
+            soft, work, inputs = p._soft, p._work, p._inputs
+            self._drop_proposals()
+            if edit_masks is not None:
+                return self._edit(p._mask, list(edit_masks), p.boxes, p._whole, return_mask, p._offset, p._feather)
+            proc, boxes = self._proc, p.boxes
+            if self._img is not None:
+                prev = [self._img.crop(b) for b in boxes]
+                key = inputs[0].shape[1:3] + (SOFT,) if p._whole else ("region",) + proc.region_size + (SOFT,)
+                res = proc.batcher.submit(key, inputs + (soft,))
+                if p._whole:
+                    out = Image.fromarray(res[0]).resize(self.size)
+                else:
+                    out = self._img.copy()
+                    for i, b in enumerate(boxes):    # the edit's paste, with its paste masks
+                        out.paste(Image.fromarray(res[i]).resize((b[2] - b[0], b[3] - b[1])), b, p.masks[i])
+                self._img = out
+                patches = [out.crop(b) for b in boxes]
+            else:
+                if p._whole:
+                    w, h = self.size
+                    patch, _, prev = proc.batcher.submit((floor8(h), floor8(w), SOFT),
+                                                         (None, inputs[0], None, False, self._photo, soft))
+                    got = [(patch, None)]
+                else:
+                    got, prev = proc.batcher.submit(("region",) + proc.region_size + (SOFT,),
+                                                    (None, inputs, list(work), False, boxes, self._photo, p._feather, self.size,
+                                                     soft))
+                patches = [Image.fromarray(q) for q, _ in got]
+            return self._record(boxes, prev, patches, list(p.masks) if return_mask else [None] * len(boxes))
+
+    def _record(self, boxes, prev, patches, masks):
+        nbytes = sum((b[2] - b[0]) * (b[3] - b[1]) * 3 for b in boxes)
+        self._history.append((boxes, prev, nbytes))
+        self._held += nbytes
+        while self._history and self._held > self.history_bytes:
+            self._held -= self._history.popleft()[2]
+        return EditResult(boxes, patches, masks)
+
     def edit(self, mask, edit_mask=None, region="auto", return_mask=False, offset=(0, 0), feather=0):
         """One edit of the current photo; see the class. Returns ``EditResult(boxes, patches, masks)``."""
-        from PIL import Image
         feather = _check_feather(feather)
         with self._mu:
             self._check_open()
             boxes = self._boxes(mask, edit_mask, region, offset)
-            proc, off = self._proc, tuple(int(v) for v in offset)
-            if self._img is not None:
-                fm, fe = _placed(mask, self.size, off), _placed(edit_mask, self.size, off)
-                prev = [self._img.crop(b) for b in boxes]
-                if region is None:
-                    out, mk = proc.process_image(self._img, fm, fe, return_mask=True)
-                    mks = [mk]
-                else:
-                    out, mks = proc._region_host(self._img, fm, fe, boxes, feather)
-                self._img = out
-                patches = [out.crop(b) for b in boxes]
+            self._drop_proposals()
+            return self._edit(mask, edit_mask, boxes, region is None, return_mask, tuple(int(v) for v in offset), feather)
+
+    def _edit(self, mask, edit_mask, boxes, whole, return_mask, off, feather):
+        """``edit`` under the lock, on checked arguments; ``edit_mask`` may also be a list of each box's edit mask."""
+        from PIL import Image
+        if whole and isinstance(edit_mask, list):
+            edit_mask = edit_mask[0]
+        proc = self._proc
+        if self._img is not None:
+            fm = _placed(mask, self.size, off)
+            fe = edit_mask if isinstance(edit_mask, list) else _placed(edit_mask, self.size, off)
+            prev = [self._img.crop(b) for b in boxes]
+            if whole:
+                out, mk = proc.process_image(self._img, fm, fe, return_mask=True)
+                mks = [mk]
             else:
-                if region is None:
-                    w, h = self.size
-                    key = (floor8(h), floor8(w)) if edit_mask is None else (floor8(h), floor8(w), True)
-                    edit_raw = np.asarray(edit_mask) if edit_mask is not None else None
-                    patch, mk, prev = proc.batcher.submit(key, (None, np.asarray(mask), edit_raw, return_mask, self._photo))
-                    got = [(patch, mk)]
-                else:
-                    at = [(b[0] - off[0], b[1] - off[1], b[2] - off[0], b[3] - off[1]) for b in boxes]   # mask coordinates
-                    sketches = [np.asarray(mask.crop(b)) for b in at]
-                    edits = [np.asarray(edit_mask.crop(b)) for b in at] if edit_mask is not None else None
-                    got, prev = proc.batcher.submit(proc._region_key(edit_mask),
-                                                    (None, sketches, edits, return_mask, boxes, self._photo, feather, self.size))
-                patches = [Image.fromarray(p) for p, _ in got]
-                mks = [Image.fromarray(m) if m is not None else None for _, m in got]
-            masks = [m if return_mask and edit_mask is None else None for m in mks]
-            nbytes = sum((b[2] - b[0]) * (b[3] - b[1]) * 3 for b in boxes)
-            self._history.append((boxes, prev, nbytes))
-            self._held += nbytes
-            while self._history and self._held > self.history_bytes:
-                self._held -= self._history.popleft()[2]
-            return EditResult(boxes, patches, masks)
+                out, mks = proc._region_host(self._img, fm, fe, boxes, feather)
+            self._img = out
+            patches = [out.crop(b) for b in boxes]
+        else:
+            if whole:
+                w, h = self.size
+                key = (floor8(h), floor8(w)) if edit_mask is None else (floor8(h), floor8(w), True)
+                edit_raw = np.asarray(edit_mask) if edit_mask is not None else None
+                patch, mk, prev = proc.batcher.submit(key, (None, np.asarray(mask), edit_raw, return_mask, self._photo))
+                got = [(patch, mk)]
+            else:
+                at = [(b[0] - off[0], b[1] - off[1], b[2] - off[0], b[3] - off[1]) for b in boxes]   # mask coordinates
+                sketches = [np.asarray(mask.crop(b)) for b in at]
+                edits = None if edit_mask is None else [np.asarray(e) for e in edit_mask] if isinstance(edit_mask, list) \
+                    else [np.asarray(edit_mask.crop(b)) for b in at]
+                got, prev = proc.batcher.submit(proc._region_key(edit_mask),
+                                                (None, sketches, edits, return_mask, boxes, self._photo, feather, self.size))
+            patches = [Image.fromarray(p) for p, _ in got]
+            mks = [Image.fromarray(m) if m is not None else None for _, m in got]
+        return self._record(boxes, prev, patches, [m if return_mask and edit_mask is None else None for m in mks])
 
     def undo(self):
         """Restores the photo from before the last edit not yet undone. Returns ``(boxes, patches)``: that edit's boxes and the
@@ -932,6 +1209,7 @@ class EditSession:
             self._check_open()
             if not self._history:
                 raise RuntimeError("nothing to undo: no snapshot is left")
+            self._drop_proposals()
             boxes, prev, nbytes = self._history.pop()
             self._held -= nbytes
             if self._img is not None:
@@ -949,3 +1227,29 @@ class EditSession:
                 patches.append(Image.fromarray(down[pos:pos + n].reshape(lower - upper, right - left, 3)))
                 pos += n
             return boxes, patches
+
+
+class Proposal:
+    """A previewed edit of an ``EditSession`` (``EditSession.propose``): ``boxes``, the PIL boxes the edit would use, and
+    ``masks``, each box's 'L' paste mask as the edit would paste it. It holds each box's fp32 soft mask on the engine's
+    device until ``EditSession.accept`` takes it, ``close()`` releases it, or an ``edit``, ``undo``, ``accept`` or ``close``
+    of its session invalidates it (the photo it was computed on has changed). It is accepted at most once."""
+
+    def __init__(self, session, boxes, masks, whole, mask, offset, feather, soft, work, inputs):
+        self.boxes, self.masks = boxes, masks
+        self._session, self._whole, self._mask, self._offset, self._feather = session, whole, mask, offset, feather
+        self._soft, self._work, self._inputs = soft, work, inputs
+
+    @property
+    def open(self):
+        """True until the proposal is accepted, closed or invalidated."""
+        return self._soft is not None
+
+    def _drop(self):
+        self._soft = self._work = self._inputs = None
+
+    def close(self):
+        """Releases the proposal's device memory (idempotent); ``accept`` then raises."""
+        with self._session._mu:
+            self._drop()
+            self._session._proposals.discard(self)
