@@ -225,6 +225,23 @@ int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitc
 /* Host only: a true upper bound of the file se_jpeg_encode_u8 writes for an h x w image: the 623-byte header, 208 bytes per
  * 8x8 block (64 codes of at most 26 bits) doubled for the 0x00 after each 0xFF, and EOI. -1 on bad arguments. */
 long long se_jpeg_max_bytes(int h, int w, int subsampling);
+/* PNG of n in [0, 32] windows, byte for byte what OpenCV writes with no parameters (OpenCV 4.13, libpng 1.6, zlib 1.3):
+ *     cv2.imencode(".png", img_i)[1]
+ * where img_i is the window as BGR (channels 3) or grey (channels 1). Image i is hw[2i] rows of hw[2i+1] pixels of `channels`
+ * bytes (sizes in [1, 65535]), its row r at src[i] + r * src_pitch[i] (bytes, >= channels * hw[2i+1]); src is a host array of n
+ * device pointers, and windows may overlap each other. swap_rb = 1 reads BGR pixels (the forward's output, what cv2.imwrite
+ * is given), 0 reads RGB; it does not affect one channel. The file (signature, IHDR, the zlib stream in IDAT chunks of 8192
+ * bytes, IEND) goes to out + out_off[i], which must hold se_png_max_bytes(h, w, channels) bytes; only its first
+ * out_bytes_dev[i] bytes are written, and that count is stored in the device array out_bytes_dev[i]. No out slice may overlap
+ * another or a window. scratch == NULL stores the scratch bytes the call needs in *scratch_bytes (src, out and out_bytes_dev
+ * may be NULL then). Every argument is checked before anything is enqueued on `stream`; the call only enqueues. */
+int se_png_encode_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int channels, int swap_rb,
+                     unsigned char* out, const long long* out_off, long long* out_bytes_dev, void* scratch, long long* scratch_bytes,
+                     void* stream);
+/* Host only: a true upper bound of the file se_png_encode_u8 writes for an h x w image of `channels` (1 or 3) bytes per pixel:
+ * the filtered data h (1 + w c) stored, 8 bytes per possible deflate block, the zlib header and Adler-32, 12 bytes per IDAT
+ * chunk, the signature, IHDR and IEND. -1 on bad arguments. */
+long long se_png_max_bytes(int h, int w, int channels);
 /* Bytes of coefficient tables the resize entries keep per device (process-wide; 0 restores the default of 256 MiB; negative is an
  * error). When a call's new tables would pass the limit, the device's cache is emptied (after a device synchronise) before the
  * call looks up any table; one call's own tables may exceed it. */

@@ -84,7 +84,7 @@ class EditLine2Model(torch.nn.Module):
         return {"mask": ex["mask_bin"], "maskim": ex["mask_image"], "coarse": ex["coarse"], "fine": ex["fine"],
                 "composed": composed}
 
-    def inference_stream(self, loader, depth=2, pinned_ring=True, gather=None, uint8=False, with_data=False):
+    def inference_stream(self, loader, depth=2, pinned_ring=True, gather=None, uint8=False, with_data=False, png=None):
         """Pipelined form of ``for data in loader: model(data, mode='inference')`` for throughput serving.
 
         Yields ``(composed, mask)`` per batch, in order, as PINNED CPU tensors (views of one packed [B,4,H,W] host
@@ -102,6 +102,12 @@ class EditLine2Model(torch.nn.Module):
 
         with_data=True: yield ``(out0, out1, data)`` (test.py needs the batch's output paths).
 
+        png=("image",) or ("image", "mask") (uint8 mode): each batch's BGR results (and masks) are encoded on the device after
+        the forward, on the compute stream (``engine.png_encode_u8_packed``), and only the files are downloaded: each result is
+        a list of ``bytes`` per image, ``cv2.imencode(".png", x)[1]`` of the array uint8 mode yields, and the mask result is
+        None without "mask". The lengths leave the device with the batch; the bytes are downloaded when the batch is drawn,
+        while later batches compute.
+
         pinned_ring=True (default): results are views of a ring of ``depth + 2`` pinned buffers handed out round robin. The
         copy of batch i + depth - 1 is already in flight when result i is drawn, so a result stays intact while at most
         ``depth`` further results are drawn (you may hold the newest ``depth + 1``; consume or ``.clone()`` older ones);
@@ -112,12 +118,19 @@ class EditLine2Model(torch.nn.Module):
         batch's packed outputs are written into this rank's slice of the gather buffer and all-gathered over NCCL (async, in
         place) before this rank's shard is copied to the host; all ranks must feed equal batch sizes."""
         import collections
+
+        from sketchedit_b200 import engine as E
         eng = self.engine()
+        if png is not None:
+            png = tuple(png)
+            if not uint8 or png not in (("image",), ("image", "mask")):
+                raise ValueError('png= needs uint8=True and is ("image",) or ("image", "mask") (got %r)' % (png,))
         if gather is not None and (gather.depth != depth or uint8):
             raise ValueError("gather= needs float mode and a ring depth equal to the stream depth (%d)" % depth)
         dev = torch.device("cuda")
         cur = torch.cuda.current_stream()
         s_in, s_out = torch.cuda.Stream(), torch.cuda.Stream()
+        s_files = torch.cuda.Stream() if png else None   # file downloads: behind nothing but the batch's own encode
         slots = [None] * depth
         pending = collections.deque()
         ring = {}        # (B, H, W) -> [buffers, results handed out so far]
@@ -141,7 +154,13 @@ class EditLine2Model(torch.nn.Module):
         def drain_one():
             host, ev, data = pending.popleft()
             ev.synchronize()
-            res = (host[0], host[1]) if uint8 else (host[0][:, :3], host[0][:, 3:4])
+            if png:   # host: (files buffer, offsets, pinned lengths, images)
+                out, offs, lens, B = host
+                with torch.cuda.stream(s_files):
+                    files = E.download_files(out, offs, lens.tolist())
+                res = (files[:B], files[B:] if len(png) == 2 else None)
+            else:
+                res = (host[0], host[1]) if uint8 else (host[0][:, :3], host[0][:, 3:4])
             return res + (data,) if with_data else res
 
         in_keys = ("image_u8", "mask_u8") if uint8 else ("image", "mask")
@@ -152,6 +171,7 @@ class EditLine2Model(torch.nn.Module):
                 raise ValueError("inference_stream runs batches with an edit mask in uint8 mode only (uint8=True, data['edit_mask_u8'])")
             B, H, W = (img_h.shape[0], img_h.shape[1], img_h.shape[2]) if uint8 else (img_h.shape[0], img_h.shape[2], img_h.shape[3])
             slot = slots[i % depth]
+            fresh = slot is None or slot["shape"] != (B, H, W) or (edit_h is not None and "edit" not in slot)
             if slot is None or slot["shape"] != (B, H, W):
                 if slot is not None:   # shape change (ragged last batch): let the old buffers' users finish first
                     slot["ev_comp"].synchronize()
@@ -159,6 +179,9 @@ class EditLine2Model(torch.nn.Module):
                 if uint8:
                     u8 = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.uint8)
                     bufs = {"img": u8(B, H, W, 3), "line": u8(B, H, W), "out": (u8(B, H, W, 3), u8(B, H, W))}
+                    if png:   # the files of the batch: images, then masks
+                        offs, total = E._aligned_offsets([E.png_max_bytes(H, W, 3)] * B + [E.png_max_bytes(H, W, 1)] * B * (len(png) - 1))
+                        bufs["png"] = (u8(total), offs)
                 else:
                     f32 = lambda c: torch.empty(B, c, H, W, device=dev, dtype=torch.float32)
                     bufs = {"img": f32(3), "line": f32(1), "out": None if gather is not None else (f32(4),)}
@@ -166,6 +189,10 @@ class EditLine2Model(torch.nn.Module):
                 slots[i % depth] = slot
             if edit_h is not None and "edit" not in slot:
                 slot["edit"] = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
+            if fresh:
+                # new buffers come from the compute stream's pool, so queued compute-stream work may still use their memory
+                # (the PNG encode's freed scratch, for one): the copies into them wait for it
+                s_in.wait_stream(cur)
             s_in.wait_event(slot["ev_comp"])           # the previous user of these input buffers has been computed
             if edit_h is not None:
                 s_in.wait_event(slot["ev_out"])        # ... and the edit mask, which is also an output, has left the device
@@ -196,12 +223,26 @@ class EditLine2Model(torch.nn.Module):
                     eng.inference_u8(slot["img"], slot["line"], precision=self.precision, out=slot["out"])
                 else:
                     eng.inference_packed(slot["img"], slot["line"], precision=self.precision, out=slot["out"][0])
+                if png:
+                    # the drain of the batch that last used this files buffer has already downloaded it
+                    files, offs = slot["png"]
+                    lens = [E.png_encode_u8_packed(t, [b * t[0].numel() for b in range(B)], [W * c] * B, [(H, W)] * B, c,
+                                                   swap_rb=True, out=files, out_offsets=offs[k * B:(k + 1) * B])[2]
+                            for k, (t, c) in enumerate(zip(src[:len(png)], (3, 1)))]
                 slot["ev_comp"].record(cur)
                 s_out.wait_event(slot["ev_comp"])
             with torch.cuda.stream(s_out):
-                host = host_out(B, H, W)
-                for h_t, d_t in zip(host, src):
-                    h_t.copy_(d_t, non_blocking=True)
+                if png:
+                    n_files = B * len(png)
+                    lens_h = torch.empty(n_files, dtype=torch.int64, pin_memory=True)
+                    for k, l in enumerate(lens):
+                        lens_h[k * B:(k + 1) * B].copy_(l, non_blocking=True)
+                        l.record_stream(s_out)
+                    host = (slot["png"][0], slot["png"][1][:n_files], lens_h, B)
+                else:
+                    host = host_out(B, H, W)
+                    for h_t, d_t in zip(host, src):
+                        h_t.copy_(d_t, non_blocking=True)
                 slot["ev_out"].record(s_out)
                 done = torch.cuda.Event()
                 done.record(s_out)

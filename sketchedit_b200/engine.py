@@ -631,20 +631,114 @@ def jpeg_encode_u8(images, quality=75, subsampling=2):
     out, offs = _out(None, None, [jpeg_max_bytes(h, w, subsampling) for h, w in sizes], dev, "out_offsets")
     out_bytes = torch.empty(len(images), device=dev, dtype=torch.int64)
     _jpeg_launch([t.data_ptr() for t in images], [t.stride(0) for t in images], sizes, quality, subsampling, out, offs, out_bytes)
-    with torch.cuda.device(dev):
-        lens = out_bytes.cpu().tolist()
-        staging = torch.empty(max(1, sum(lens)), dtype=torch.uint8, pin_memory=True)
+    return download_files(out, offs, out_bytes.cpu().tolist())
+
+
+def download_files(out, offsets, lengths):
+    """The files at ``offsets`` of the CUDA uint8 tensor ``out``, ``lengths[i]`` bytes each, as ``bytes``: one copy into
+    pinned staging on the current stream of out's device, then a synchronise of that stream."""
+    with torch.cuda.device(out.device):
+        staging = torch.empty(max(1, sum(lengths)), dtype=torch.uint8, pin_memory=True)
         at = 0
-        for o, k in zip(offs, lens):
+        for o, k in zip(offsets, lengths):
             staging[at:at + k].copy_(out[o:o + k], non_blocking=True)
             at += k
         torch.cuda.current_stream().synchronize()
     host = staging.numpy()
     res, at = [], 0
-    for k in lens:
+    for k in lengths:
         res.append(host[at:at + k].tobytes())
         at += k
     return res
+
+
+PNG_MAX_BATCH = 32       # images per se_png_encode_u8 call; the wrappers split longer lists into calls of this size
+
+
+def png_max_bytes(h, w, channels=3):
+    """A true upper bound of the PNG file of an h x w image of ``channels`` (1 or 3) bytes per pixel (``se_png_max_bytes``)."""
+    n = int(_lib.load().se_png_max_bytes(int(h), int(w), int(channels)))
+    if n < 0:
+        raise ValueError(_lib.load().se_last_error().decode())
+    return n
+
+
+def _png_launch(ptrs, pitches, sizes, channels, swap_rb, out, out_offsets, out_bytes):
+    """se_png_encode_u8 over windows already checked, PNG_MAX_BATCH per call, on the current stream of out's device."""
+    lib = _lib.load()
+
+    def chunk(sl):
+        k = len(ptrs[sl])
+        a = ((ctypes.c_void_p * k)(*ptrs[sl]), _longs(pitches[sl]), _ints(sizes[sl]), k, channels, int(bool(swap_rb)), _ptr(out),
+             _longs(out_offsets[sl]), ctypes.c_void_p(out_bytes.data_ptr() + 8 * sl.start))
+        return lambda scratch, size, stream: lib.se_png_encode_u8(*a, scratch, size, stream)
+
+    _run_chunks(len(sizes), PNG_MAX_BATCH, out.device, chunk)
+
+
+def png_encode_u8_packed(src, src_offsets, src_pitches, sizes, channels, swap_rb=False, out=None, out_offsets=None):
+    """PNG files of windows (``se_png_encode_u8``), byte for byte ``cv2.imencode(".png", img)[1]`` of each with img the window
+    as BGR (``channels`` 3) or grey (1): image i is the ``sizes[i] = (h, w)`` window whose row r starts at byte ``src_offsets[i] +
+    r * src_pitches[i]`` of its source, with ``src_pitches[i] >= channels * w``. ``swap_rb`` says the pixels are BGR (the
+    forward's output); otherwise they are RGB. ``src`` is one contiguous CUDA uint8 tensor, or a list of them with one per image;
+    windows may overlap. ``out`` (optional, contiguous CUDA uint8) receives file i at ``out_offsets[i]`` and must hold
+    ``png_max_bytes(h, w, channels)`` bytes there. Returns ``(out, out_offsets, out_bytes)``: ``out_bytes`` is a CUDA int64
+    tensor of the files' lengths. Only enqueues work on the current stream."""
+    if channels not in (1, 3) or isinstance(channels, bool):
+        raise ValueError("channels must be 1 or 3, got %r" % (channels,))
+    n = len(sizes)
+    srcs = list(src) if isinstance(src, (list, tuple)) else [src] * n
+    if not (len(srcs) == len(src_offsets) == len(src_pitches) == n):
+        raise _lib.SketchEditB200Error("src (as a list), src_offsets, src_pitches and sizes must have the same length")
+    named = [(t, "src") for t in srcs] + ([(out, "out")] if out is not None else [])
+    _chk_u8(*named)
+    if n == 0:
+        return out, out_offsets, None
+    dev = _device(*named)
+    sizes = _hw(sizes)
+    src_offsets, src_pitches = [int(o) for o in src_offsets], [int(p) for p in src_pitches]
+    for i, (h, w) in enumerate(sizes):
+        if not (1 <= h <= 65535 and 1 <= w <= 65535):
+            raise _lib.SketchEditB200Error("window %d: sizes must be in [1, 65535], got %dx%d" % (i, h, w))
+    _check_windows("window", srcs, src_offsets, src_pitches, sizes, channels)
+    out, out_offsets = _out(out, out_offsets, [png_max_bytes(h, w, channels) for h, w in sizes], dev, "out_offsets")
+    out_bytes = torch.empty(n, device=dev, dtype=torch.int64)
+    _png_launch([t.data_ptr() + o for t, o in zip(srcs, src_offsets)], src_pitches, sizes, channels, swap_rb, out, out_offsets,
+                out_bytes)
+    return out, out_offsets, out_bytes
+
+
+def png_encode_u8(images, swap_rb=False):
+    """PNG files of CUDA uint8 images, as ``bytes``: [h, w, 3] RGB (``swap_rb``: BGR) or [h, w] grey, one channel count for the
+    list. Each is ``cv2.imencode(".png", img)[1]`` of the image as BGR or grey. An image may be a strided view (a box of a larger
+    photo: pixels packed along a row, rows ``stride(0)`` bytes apart); it is encoded where it lies. One download of the lengths,
+    then one of the bytes into pinned staging.
+
+    Device memory: the call allocates, through torch's caching allocator, ``out`` at ``png_max_bytes`` per image (the
+    filtered data, h (1 + w c) bytes, stored) and the scratch of ``se_png_encode_u8`` (about 1.2 bytes per filtered byte, the
+    word stream included), and frees them on return: about 2 + 2.4 MB for a 1000x667 RGB image and 32 + 38 MB for 4000x2667;
+    concurrent calls hold their sum. Each call also zeroes the word stream in scratch (32 MB at 4000x2667)."""
+    images = list(images)
+    if not images:
+        return []
+    chans = {1 if isinstance(t, torch.Tensor) and t.dim() == 2 else 3 for t in images}
+    if len(chans) > 1:
+        raise _lib.SketchEditB200Error("images must all be [h, w] or all be [h, w, 3]")
+    C = chans.pop()
+    for t in images:
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and
+                (t.dim() == 2 if C == 1 else t.dim() == 3 and t.shape[2] == 3)):
+            raise _lib.SketchEditB200Error("images must be CUDA uint8 [h, w, 3] or [h, w] tensors")
+        if (C == 3 and t.stride(2) != 1) or (t.stride(1) != C and t.shape[1] > 1) or t.stride(0) < C * t.shape[1]:
+            raise _lib.SketchEditB200Error("an image's pixels must be packed along its rows (got strides %r)" % (t.stride(),))
+        if not (1 <= t.shape[0] <= 65535 and 1 <= t.shape[1] <= 65535):
+            raise _lib.SketchEditB200Error("image sizes must be in [1, 65535], got %dx%d" % tuple(t.shape[:2]))
+    dev = _device(*[(t, "image") for t in images])
+    sizes = [(int(t.shape[0]), int(t.shape[1])) for t in images]
+    out, offs = _out(None, None, [png_max_bytes(h, w, C) for h, w in sizes], dev, "out_offsets")
+    out_bytes = torch.empty(len(images), device=dev, dtype=torch.int64)
+    _png_launch([t.data_ptr() for t in images], [t.stride(0) for t in images], sizes, C, swap_rb, out, offs, out_bytes)
+    return download_files(out, offs, out_bytes.cpu().tolist())
 
 
 def outputs_to_uint8(composed, mask):

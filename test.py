@@ -1,7 +1,8 @@
 """Batch inference entry point -- same command line as the reference's test.py (reference test.py:12-37,
 test_celeb.sh, test_places.sh): build the dataloader and the model from the flags, run
 ``model(data, mode='inference')`` per batch on the CUDA kernels, convert to uint8 (truncating, like
-``astype(np.uint8)``), RGB->BGR, and write PNGs to --output_dir (masks to --output_mask_dir).
+``astype(np.uint8)``), RGB->BGR, and write PNGs to --output_dir (masks to --output_mask_dir). PNG files are encoded on the
+device, byte for byte as cv2.imwrite writes them.
 
 ``--edit_mask_dir D`` runs every entry on the mask ``D/<output name>`` instead of netM's prediction: write the masks with
 --output_mask_dir, correct the wrong ones by hand, and rerun with --edit_mask_dir pointing at them."""
@@ -30,14 +31,32 @@ def main(argv=None):
     # the reference loop (test.py:20-37: model(data_i, mode='inference') -> uint8 -> BGR -> imwrite), pipelined: copies of the
     # neighbouring batches overlap the forward, and both codecs (normalise / binarise in, (x+1)/2*255 -> uint8 HWC BGR out) run
     # on the device, so 4 bytes per pixel cross PCIe in each direction instead of 16
+    # When every output is a PNG, the files are encoded on the device too (byte for byte what cv2.imwrite writes) and only
+    # they are downloaded; cv2 picks its encoder by the extension, case-insensitively, and stays the writer of other formats.
+    mask_dir = getattr(opt, "output_mask_dir", None)
+    png = None
+    if all(out.lower().endswith(".png") for _, _, out in getattr(dataloader.dataset, "items", [("", "", "")])):
+        png = ("image", "mask") if mask_dir is not None else ("image",)
     with torch.no_grad():
-        for bgr, mk, batch in model.inference_stream(batches(), uint8=True, with_data=True):
-            bgr, mk = bgr.numpy(), mk.numpy()
+        for res, mk, batch in model.inference_stream(batches(), uint8=True, with_data=True, png=png):
+            if png is None:
+                res, mk = res.numpy(), mk.numpy()
             for b, path in enumerate(batch["path"]):
                 print("process image... %s" % path)
-                assert cv2.imwrite(os.path.join(opt.output_dir, path), bgr[b])
-                if getattr(opt, "output_mask_dir", None) is not None:
-                    assert cv2.imwrite(os.path.join(opt.output_mask_dir, path), mk[b])
+                if png is None:
+                    assert cv2.imwrite(os.path.join(opt.output_dir, path), res[b])
+                else:
+                    _write(os.path.join(opt.output_dir, path), res[b])
+                if mask_dir is not None:
+                    if png is None:
+                        assert cv2.imwrite(os.path.join(mask_dir, path), mk[b])
+                    else:
+                        _write(os.path.join(mask_dir, path), mk[b])
+
+
+def _write(path, data):
+    with open(path, "wb") as f:
+        f.write(data)
 
 
 if __name__ == "__main__":
