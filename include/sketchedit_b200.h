@@ -118,6 +118,22 @@ int se_forward_u8_with_soft_mask(se_model* m, const unsigned char* image_u8, con
                                  const float* edit_mask, int B, int H, int W, int precision, unsigned char* bgr_u8,
                                  void* stream);
 
+/* se_forward_u8_export: one of the three uint8 region forwards above, with the attention exported for region-edit detail
+ * (se_detail_u8). The mask argument chooses it: neither edit mask is se_forward_inference_u8 (mask_u8 [B,H,W] receives its
+ * mask bytes, so it must not be NULL), edit_mask_u8 is se_forward_with_mask_u8 and the fp32 edit_mask [B,1,H,W] is
+ * se_forward_u8_with_soft_mask; giving both is an error, and mask_u8 is ignored with either. bgr_u8 (and mask_u8) are that
+ * call's bytes bit for bit, in every precision. Two more outputs:
+ *   attn [B, L, L] fp32: the softmax weights of netG's contextual attention exactly as the forward used them (bf16: the
+ *        stored bf16 probabilities; fp32 tensor-core mode: the fp32 weights before their split into fp16 halves), in
+ *        se_contextual_attention_forward's layout [key][query], L = (H/8 - 1) (W/8 - 1); 4 L^2 bytes per image, computed in
+ *        one band of query rows: the attention's L x L workspace (bf16: 2 L^2 bytes per image, fp32_direct: 8 L^2) is then
+ *        not held to se_set_attention_workspace_limit, as for every call that returns the attention map.
+ *   hole_u8 [B,H,W]: the mask netG inpaints (mask_inpaint) as 0 / 1 bytes.
+ * A model without the attention (SE_OPT_USE_CAM = 0) has no weights to export: the call fails. */
+int se_forward_u8_export(se_model* m, const unsigned char* image_u8, const unsigned char* sketch_u8, const unsigned char* edit_mask_u8,
+                         const float* edit_mask, int B, int H, int W, int precision, unsigned char* bgr_u8, unsigned char* mask_u8,
+                         float* attn, unsigned char* hole_u8, void* stream);
+
 /* ---- netM: replaces MDGenerator.forward(x, guide) -> (mask1, x_stage1)  (editline2_g.py:59-94) */
 int se_netM_forward(se_model* m, const float* x, const float* guide, int B, int H, int W, int precision, float* mask1,
                     float* x_stage1 /* may be NULL */, void* stream);
@@ -195,6 +211,36 @@ int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rg
                                    const long long* mask_off, const int* src_hw, unsigned char* canvas, const long long* canvas_off,
                                    const long long* canvas_pitch, const int* box_yx, const int* dst_hw, const int* feather, int n,
                                    int swap_rb, void* scratch, long long* scratch_bytes, void* stream);
+/* se_resize_composite_feather_u8 with a detail plane per box (region-edit detail): detail (may be NULL: none) holds at byte
+ * detail_off[i] (even; a negative offset: box i has none) box i's int16 plane [h][w][3] in RGB order, as se_detail_u8 writes
+ * it. Box i's resized result, after the vertical pass's rounding and the channel swap, becomes clamp(res + D, 0, 255) before
+ * the blend; everything else is se_resize_composite_feather_u8's, which is this call with detail = NULL. */
+int se_resize_composite_feather_detail_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask,
+                                          const long long* mask_off, const int* src_hw, unsigned char* canvas, const long long* canvas_off,
+                                          const long long* canvas_pitch, const int* box_yx, const int* dst_hw, const int* feather,
+                                          const short* detail, const long long* detail_off, int n, int swap_rb, void* scratch,
+                                          long long* scratch_bytes, void* stream);
+/* Region-edit detail (contextual residual aggregation on netG's attention weights; DESIGN.md section 7b): for n >= 0 boxes of a
+ * region edit at the working size Hn x Wn (multiples of 8, >= 16), box i of box_hw[2i] x box_hw[2i+1] = bh x bw pixels:
+ *   photo[i], photo_pitch[i]  the photo's box, RGB bytes, row r at photo[i] + r * photo_pitch[i] (a host array of n device pointers)
+ *   low + low_off[i]          resize(resize(box, (Wn, Hn)), (bw, bh)), [bh][bw][3] (se_resize_window_u8 both ways)
+ *   hole + hole_off[i]        the forward's hole_u8 [Hn][Wn] for the box
+ *   attn + attn_off[i]        the forward's attn [L][L] for the box (byte offset, a multiple of 4)
+ * writes the int16 plane D [bh][bw][3] at byte D + d_off[i] (even), and where agg is not NULL the fp32 aggregate A [bh][bw][3]
+ * at byte agg + agg_off[i] (0 outside the hole), with u(x) = ((2x + 1) Wn) / (2 bw), v(y) likewise, the patch grid ws x hs =
+ * (Wn/8 - 1) x (Hn/8 - 1), patch (py, px) covering working pixels [8py, 8py + 16) x [8px, 8px + 16), ax(px) = min{x : u(x) >= 8px}:
+ *   R(x, y) = hole(v(y), u(x)) ? 0 : photo - low
+ *   A(x, y) = (1/nq) sum over the nq patches q covering (v(y), u(x)) of sum_k attn[k][q] R(min(ax(k) + x - ax(q), bw - 1), likewise y)
+ *   D(x, y) = hole(v(y), u(x)) ? round half away from zero (A) : 0
+ * Every patch position must have an anchor, u(bw - 1) >= Wn - 16 and v(bh - 1) >= Hn - 16 (true from bw >= Wn / 32 and
+ * bh >= Hn / 32): a smaller box is an error. The GEMM runs over all L query rows (M = Mp), not only those that touch the hole.
+ * A is an fp32 computation within 255 (L + 8) 2^-22 of its float64 value. Boxes run in order through one scratch of the
+ * largest box's need (256 B aligned): 4 Mp^2 + 12 Mp Np bytes, Mp = L rounded up to 256, Np = 3 fw fh rounded up to 256,
+ * fw = ceil(16 bw / Wn) + 2, fh likewise. Query form (scratch == NULL) as se_resize_window_u8's. Only enqueues work on `stream`. */
+int se_detail_u8(const unsigned char* const* photo, const long long* photo_pitch, const int* box_hw, int n, int Hn, int Wn,
+                 const unsigned char* low, const long long* low_off, const unsigned char* hole, const long long* hole_off, const float* attn,
+                 const long long* attn_off, short* D, const long long* d_off, float* agg, const long long* agg_off, void* scratch,
+                 long long* scratch_bytes, void* stream);
 /* The feather of se_resize_composite_feather_u8 on masks alone, in place: image i is the hw[2i] x hw[2i+1] 'L' bytes (rows
  * packed) at img + off[i], and each of its bytes m becomes DIV255(m * r(y, x)) with the ramp r of its widths feather[4i .. 4i+3]
  * (left, top, right, bottom; each in [0, the side's length]). Sizes are in [1, 65535]; an image with four widths of 0 is not

@@ -51,6 +51,14 @@ SIGNATURES = {
     "se_resize_composite_feather_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                                                 _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_void_p,
                                                 ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
+    "se_forward_u8_export": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_int, _c_void_p,
+                                      _c_void_p, _c_void_p, _c_void_p, _c_void_p]),
+    "se_resize_composite_feather_detail_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                                                       _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int,
+                                                       _c_int, _c_void_p, ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
+    "se_detail_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                              _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                              ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
     "se_feather_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_void_p]),
     "se_jpeg_encode_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                                    ctypes.POINTER(ctypes.c_longlong), _c_void_p]),

@@ -26,6 +26,7 @@
 #include "se_gemm_split.h"
 #include "se_conv_tc.h"
 #include "se_misc.h"
+#include "se_detail.h"
 
 namespace se {
 
@@ -832,7 +833,7 @@ static int run_cam_tc(Ctx& c, const View& f, const float* mask_s, void* out, flo
           (double)c.B * f.H * f.W * 96 * 2 * 2 + 2.0 * (double)c.B * pl.KB * pl.hs * pl.ws * 16);   // P of all bands
   }
   CK(cam_forward_tc(f.p, mask_s, out, pl, fn.p, (float*)cs.p, P.p, attn_out, c.stream));
-  if (!c.dry) g_launches += 1 + 2 * pl.n_bands;   // norm, colscale and an S + PV pair per band behind one call
+  if (!c.dry) g_launches += 1 + 2 * pl.n_bands + (attn_out ? 1 : 0);   // norm, colscale and an S + PV pair per band behind one call
   c.put(P); c.put(cs); c.put(fn);
   return 0;
 }
@@ -943,7 +944,7 @@ static int run_cam(Ctx& c, const View& f, const float* mask_s, void* out, int ou
 }
 
 // Attention of the fp32-on-tensor-cores mode: f fp32 NHWC [B][h][w][96] -> out fp32 NHWC, split-half fp16 wgmma GEMMs (se_gemm_split.cu)
-static int run_cam_split(Ctx& c, const float* f, int h, int w, int C, const float* mask_s, float* out) {
+static int run_cam_split(Ctx& c, const float* f, int h, int w, int C, const float* mask_s, float* out, float* attn_out = nullptr) {
   CamSplitPlan pl;
   {
     int rc = cam_split_plan(c.B, h, w, C, c.attn_limit, &pl);
@@ -958,7 +959,7 @@ static int run_cam_split(Ctx& c, const float* f, int h, int w, int C, const floa
   const double fl = 2.0 * c.B * (double)pl.L * pl.L * pl.KQ * 2.0;   // S and PV, algorithmic (one product each)
   c.tag("gemm_split_kernel x2 (split-half fp16 x3) + pack / softmax / fold|contextual attention", 1, fl, 3.0 * 2.0 * c.B * (double)pl.Mp * pl.Mp * pl.KQ * 2.0,
         (double)c.B * h * w * C * 4 * 2 + 2.0 * pl.q_bytes * 2 + 2.0 * c.B * (double)pl.Mp * pl.Mp * 8 /* S + P of all bands */ + 2.0 * pl.o_bytes);
-  CK(cam_forward_split(f, (const float*)rnorm.p, (const float*)colm.p, out, pl, q.p, kn.p, (float*)sb.p, pb.p, (float*)ob.p, c.stream));
+  CK(cam_forward_split(f, (const float*)rnorm.p, (const float*)colm.p, out, pl, q.p, kn.p, (float*)sb.p, pb.p, (float*)ob.p, attn_out, c.stream));
   if (!c.dry) g_launches += 1 + 3 * pl.n_bands;   // pack, S GEMM + softmax + PV GEMM per band, fold behind one call
   c.put(ob); c.put(pb); c.put(sb); c.put(kn); c.put(q); c.put(colm); c.put(rnorm);
   return 0;
@@ -1066,6 +1067,7 @@ struct NetGIO {
   unsigned char* composed_u8 = nullptr;
   const float* mask_soft = nullptr;
   long long msoft_bs = 0;
+  float* attn = nullptr;   // the attention's softmax weights [B][L][L] (cam_1's layout), one band
 };
 
 static int run_netG(Ctx& c, int H, int W, const NetGIO& io) {
@@ -1148,13 +1150,13 @@ static int run_netG(Ctx& c, int H, int W, const NetGIO& io) {
       const Layout pml{LAYOUT_C8, h, w, pm.v.ld};
       CK(act_to_f32(pm.v.p, DT_F16X2, pml, (float*)f32.p, 1, c.B, 96, c.stream));
       TAP("in:G.cam.f32", nhwc(f32.p, h, w, 96, 96), 0, 0);
-      rc = run_cam_split(c, (const float*)f32.p, h, w, 96, (const float*)ms.p, (float*)o32.p);
+      rc = run_cam_split(c, (const float*)f32.p, h, w, 96, (const float*)ms.p, (float*)o32.p, io.attn);
       if (rc) return rc;
       TAP("out:G.cam.f32", nhwc(o32.p, h, w, 96, 96), 0, 0);
       CK(f32_to_act((const float*)o32.p, 1, camo.p, DT_F16X2, pml, c.B, 96, c.stream));
       c.put(o32); c.put(f32);
     } else {
-      rc = tc ? run_cam_tc(c, pm.v, (const float*)ms.p, camo.p, nullptr) : run_cam(c, pm.v, (const float*)ms.p, camo.p, 96, nullptr, 0);
+      rc = tc ? run_cam_tc(c, pm.v, (const float*)ms.p, camo.p, io.attn) : run_cam(c, pm.v, (const float*)ms.p, camo.p, 96, io.attn, 0);
       if (rc) return rc;
     }
     c.put(ms);
@@ -1192,6 +1194,8 @@ struct Request {
   float *coarse = nullptr, *fine = nullptr, *mask_image = nullptr;
   const float* mask_bin_in = nullptr;
   float* mask_bin_out = nullptr;
+  float* attn = nullptr;                 // netG's attention weights (NetGIO::attn)
+  unsigned char* hole_u8 = nullptr;      // the mask netG inpaints as 0 / 1 bytes [B,H,W]
 };
 
 // input codec, mask source, netM (only its trunk and image decoder, for mask_image, on a caller's mask), then
@@ -1228,8 +1232,12 @@ static int run_generate(Ctx& c, int H, int W, const Request& r) {
   }
   if (from_netM && r.mask_bin_in) mbin = r.mask_bin_in;
   if (from_netM && r.mask_bin_out && !c.dry) SE_CUDA_OK(cudaMemcpyAsync(r.mask_bin_out, mbin, plane, cudaMemcpyDeviceToDevice, c.stream));
+  if (r.hole_u8) {
+    c.tag("detail_hole_kernel|mask_inpaint bytes", 0, 0, 0, (double)c.B * H * W * 5);
+    CK(detail_hole_u8(mbin, r.hole_u8, (long long)c.B * H * W, c.stream));
+  }
   NetGIO g{image, image, mbin, mbin, sketch};
-  g.x_stage1 = r.coarse; g.x_stage2 = r.fine;
+  g.x_stage1 = r.coarse; g.x_stage2 = r.fine; g.attn = r.attn;
   g.composed = r.composed; g.composed_bs = r.composed_bs; g.composed_u8 = r.bgr_u8;
   g.mask_soft = r.edit_mask ? r.edit_mask : msoft;
   g.msoft_bs = r.edit_mask ? 0 : r.mask_bs;
@@ -1607,6 +1615,21 @@ int se_forward_u8_with_soft_mask(se_model* m, const unsigned char* image_u8, con
   SE_REQUIRE(image_u8 && sketch_u8 && edit_mask && bgr_u8, "null tensor");
   Request r;
   r.image_u8 = image_u8; r.sketch_u8 = sketch_u8; r.edit_mask = edit_mask; r.bgr_u8 = bgr_u8;
+  return keyed_forward(m, precision, B, H, W, stream, 1, r, run_generate);
+}
+
+int se_forward_u8_export(se_model* m, const unsigned char* image_u8, const unsigned char* sketch_u8, const unsigned char* edit_mask_u8,
+                         const float* edit_mask, int B, int H, int W, int precision, unsigned char* bgr_u8, unsigned char* mask_u8, float* attn,
+                         unsigned char* hole_u8, void* stream) {
+  SE_REQUIRE(image_u8 && sketch_u8 && bgr_u8 && attn && hole_u8, "null tensor");
+  SE_REQUIRE(!(edit_mask_u8 && edit_mask), "se_forward_u8_export takes at most one of edit_mask_u8 and edit_mask");
+  SE_REQUIRE(edit_mask_u8 || edit_mask || mask_u8, "se_forward_u8_export without an edit mask writes mask_u8: it must not be NULL");
+  SE_REQUIRE(m && m->opt[SE_OPT_USE_CAM], "se_forward_u8_export returns the contextual attention's weights: the model runs without it "
+                                          "(use_cam = 0)");
+  Request r;
+  r.image_u8 = image_u8; r.sketch_u8 = sketch_u8; r.edit_mask_u8 = edit_mask_u8; r.edit_mask = edit_mask; r.bgr_u8 = bgr_u8;
+  r.mask_u8 = edit_mask_u8 || edit_mask ? nullptr : mask_u8;
+  r.attn = attn; r.hole_u8 = hole_u8;
   return keyed_forward(m, precision, B, H, W, stream, 1, r, run_generate);
 }
 

@@ -192,7 +192,9 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 // ------------------------------------------------------------------------------------------ softmax -> P (split-half, K-blocked)
 // S: fp32 [B][rows][Np] (query rows n_base + r); P: fp16 [B][2][Np / 8][rows][8] (times kScaleP). Rows of any length, read
 // from global memory. Block = 8 rows (one warp each computes its row's statistics); query rows >= L and keys >= L are 0.
-__global__ void __launch_bounds__(256) cam_split_softmax_kernel(const float* __restrict__ S, uint4* __restrict__ P, int L, int rows, int n_base, int Np) {
+// attn (optional): the fp32 weights before the split, [B][L keys][L queries] (the layout of cam_1's return value).
+__global__ void __launch_bounds__(256) cam_split_softmax_kernel(const float* __restrict__ S, uint4* __restrict__ P, int L, int rows, int n_base, int Np,
+                                                                float* __restrict__ attn) {
   __shared__ float s_inv[8], s_max[8];
   const int b = blockIdx.y, r0 = blockIdx.x * 8, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float* src = S + ((size_t)b * rows + r0) * Np;
@@ -223,6 +225,10 @@ __global__ void __launch_bounds__(256) cam_split_softmax_kernel(const float* __r
       for (int k = 0; k < 8; k += 2) {
         const float p0 = (lb * 8 + k < L) ? expf(row[k] - mx) * inv : 0.0f;
         const float p1 = (lb * 8 + k + 1 < L) ? expf(row[k + 1] - mx) * inv : 0.0f;
+        if (attn) {
+          if (lb * 8 + k < L) attn[((size_t)b * L + lb * 8 + k) * L + n] = p0;
+          if (lb * 8 + k + 1 < L) attn[((size_t)b * L + lb * 8 + k + 1) * L + n] = p1;
+        }
         __half h0, l0, h1, l1;
         split_half(p0, kScaleP, h0, l0);
         split_half(p1, kScaleP, h1, l1);
@@ -329,7 +335,7 @@ static int gs_launch(bool bmn, const CUtensorMap& tmA, const CUtensorMap& tmB, c
 }
 
 int cam_forward_split(const float* f, const float* rnorm, const float* colmask, float* out, const CamSplitPlan& pl, void* Q, void* Kn, float* S, void* P,
-                      float* O, cudaStream_t stream) {
+                      float* O, float* attn, cudaStream_t stream) {
   const int B = pl.B, C = pl.C, CB = C / 8, L = pl.L, Mp = pl.Mp;
   SE_REQUIRE(((reinterpret_cast<uintptr_t>(Q) | reinterpret_cast<uintptr_t>(Kn) | reinterpret_cast<uintptr_t>(P)) & 127) == 0 &&
                  ((reinterpret_cast<uintptr_t>(S) | reinterpret_cast<uintptr_t>(O) | reinterpret_cast<uintptr_t>(f) | reinterpret_cast<uintptr_t>(out)) & 15) == 0,
@@ -355,7 +361,7 @@ int cam_forward_split(const float* f, const float* rnorm, const float* colmask, 
       rc = gs_launch(false, tmQ, tmK, p, Mp / GS_BN, rows / GS_BM, B, stream);
       if (rc) return rc;
     }
-    cam_split_softmax_kernel<<<dim3(rows / 8, B), 256, 0, stream>>>(S, (uint4*)P, L, rows, n0, Mp);
+    cam_split_softmax_kernel<<<dim3(rows / 8, B), 256, 0, stream>>>(S, (uint4*)P, L, rows, n0, Mp, attn);
     SE_CUDA_OK(cudaGetLastError());
     {   // O[n0 + r] = P Q  (B operand = the query patches again, read MN-major)
       CUtensorMap tmP;
@@ -374,6 +380,21 @@ int cam_forward_split(const float* f, const float* rnorm, const float* colmask, 
     SE_CUDA_OK(cudaGetLastError());
   }
   return 0;
+}
+
+int gemm_split_mn(const void* A, const void* B, float* C, int M, int K, int N, float scale, cudaStream_t stream) {
+  SE_REQUIRE(M % GS_BM == 0 && K % GS_BK == 0 && N % GS_BN == 0 && M > 0 && K > 0 && N > 0, "split GEMM: M, K, N multiples of 128, 32, 256");
+  SE_REQUIRE(((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B)) & 127) == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0,
+             "split GEMM operands must be 128 B aligned");
+  CUtensorMap tmA, tmB;
+  int rc = gs_map(&tmA, A, M, K / 8, 2, GS_BM, GS_BK / 8);
+  if (rc) return rc;
+  rc = gs_map(&tmB, B, K, N / 8, 2, GS_BK, GS_BN / 8);
+  if (rc) return rc;
+  GemmSplitParams p;
+  p.K = K; p.a_row0 = 0; p.C = C; p.c_img_stride = (long long)M * N; p.ldc = N;
+  p.scale = scale; p.colscale = nullptr; p.ncs = 0;
+  return gs_launch(true, tmA, tmB, p, N / GS_BN, M / GS_BM, 1, stream);
 }
 
 }  // namespace se

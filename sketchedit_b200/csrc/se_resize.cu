@@ -353,6 +353,11 @@ struct PasteList {
   int n;   // canvases
 };
 static_assert(sizeof(PasteList) <= 4096, "paste descriptors must fit the kernel parameter space");
+// se_resize_composite_feather_detail_u8: per box of the launch its int16 detail plane [out_h][out_w][3] (RGB) or nullptr.
+// A separate parameter: PasteList fills the classic 4 KB of kernel parameters (sm_90 takes up to 32 KB).
+struct PasteDetail {
+  const short* d[RESIZE_MAX_BATCH];
+};
 constexpr int P_PIX = V_GROUP / 3;
 static __device__ int g_unit_tap[1] = {1 << RESIZE_PREC_BITS};
 
@@ -363,7 +368,10 @@ __device__ __forceinline__ void box_span(const PBox& b, int y, int x, int& lo, i
   hi = row ? min(b.ox + b.out_w - x, P_PIX) : 0;
 }
 
-__global__ void __launch_bounds__(V_TX * V_TY) paste_v_kernel(const __grid_constant__ PasteList L, int swap) {
+// A box with a detail plane adds it to the result after the vertical pass's clip8 and the channel swap, clamped to [0, 255]
+// (one test per box and thread; a box without one runs the plain paste).
+__global__ void __launch_bounds__(V_TX * V_TY) paste_v_kernel(const __grid_constant__ PasteList L, int swap,
+                                                              const __grid_constant__ PasteDetail D) {
   const PCanvas& d = L.p[find_image(L)];
   const int t = blockIdx.x - d.tile0;
   const int g = (t % d.tiles_x) * V_TX + threadIdx.x, y = d.y0 + (t / d.tiles_x) * V_TY + threadIdx.y;
@@ -419,6 +427,12 @@ __global__ void __launch_bounds__(V_TX * V_TY) paste_v_kernel(const __grid_const
       }
     }
     if (swap) swap_rb12(v);
+    if (const short* dp = D.d[i]) {
+      const short* dr = dp + ((ptrdiff_t)r * b.out_w + (x - b.ox)) * 3;   // pixel 0 of the thread (may lie left of the box)
+#pragma unroll
+      for (int j = 0; j < V_GROUP; ++j)
+        if (j / 3 >= lo && j / 3 < hi) v[j] = min(max(v[j] + (int)dr[j], 0), 255);
+    }
 #pragma unroll
     for (int j = 0; j < V_GROUP; ++j) {
       if (j / 3 < lo || j / 3 >= hi) continue;
@@ -610,6 +624,7 @@ struct PasteBox {
   const unsigned char* mask;
   int ih, iw, oh, ow, canvas, oy, ox;
   int feather[4];   // left, top, right, bottom; zero when the call gives no widths
+  const short* detail;   // int16 [oh][ow][3] added after the vertical pass, or nullptr
 };
 struct PasteCanvas {
   const unsigned char* base;
@@ -643,9 +658,11 @@ static int paste_boxes(const std::vector<PasteBox>& boxes, const std::vector<Pas
     const int c1 = std::min(n, c0 + RESIZE_MAX_BATCH);
     PassList<HPass> h3, h1;
     PasteList pl;
+    PasteDetail dl;
     memset(&h3, 0, sizeof(h3));
     memset(&h1, 0, sizeof(h1));
     memset(&pl, 0, sizeof(pl));
+    memset(&dl, 0, sizeof(dl));
     long long t3 = 0, t1 = 0, ptiles = 0;
     int k3 = 1, k1 = 1;
     std::vector<int> order;   // the launch's boxes grouped by canvas (canvases in order of first appearance), in order
@@ -659,6 +676,7 @@ static int paste_boxes(const std::vector<PasteBox>& boxes, const std::vector<Pas
       PBox& p = pl.b[j];
       p.rgb = b.rgb;
       p.mask = b.mask;
+      dl.d[j] = b.detail;
       if (b.iw != b.ow) {   // the paste reads the horizontal passes' output instead of the result itself
         unsigned char* s3 = (unsigned char*)scratch + mid[order[j]];
         unsigned char* s1 = s3 + scratch_round((size_t)b.ih * b.ow * 3);
@@ -710,7 +728,7 @@ static int paste_boxes(const std::vector<PasteBox>& boxes, const std::vector<Pas
     if (rc) return rc;
     rc = launch_h<1>(h1, t1, k1, st);
     if (rc) return rc;
-    paste_v_kernel<<<(unsigned)ptiles, dim3(V_TX, V_TY), 0, st>>>(pl, swap_rb);
+    paste_v_kernel<<<(unsigned)ptiles, dim3(V_TX, V_TY), 0, st>>>(pl, swap_rb, dl);
     SE_CUDA_OK(cudaGetLastError());
   }
   return 0;
@@ -771,10 +789,12 @@ int se_resize_window_u8(const unsigned char* const* src, const long long* src_pi
                        (cudaStream_t)stream);
 }
 
-int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask,
-                                   const long long* mask_off, const int* src_hw, unsigned char* canvas, const long long* canvas_off,
-                                   const long long* canvas_pitch, const int* box_yx, const int* dst_hw, const int* feather, int n,
-                                   int swap_rb, void* scratch, long long* scratch_bytes, void* stream) {
+int se_resize_composite_feather_detail_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask,
+                                          const long long* mask_off, const int* src_hw, unsigned char* canvas, const long long* canvas_off,
+                                          const long long* canvas_pitch, const int* box_yx, const int* dst_hw, const int* feather,
+                                          const short* detail, const long long* detail_off, int n, int swap_rb, void* scratch,
+                                          long long* scratch_bytes, void* stream) {
+  SE_REQUIRE(!detail || detail_off, "detail needs detail_off");
   SE_REQUIRE(n >= 0, "n must be >= 0 boxes");
   SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
   SE_REQUIRE(n == 0 || (rgb_off && mask_off && src_hw && canvas_off && canvas_pitch && box_yx && dst_hw), "null size / offset array");
@@ -794,7 +814,11 @@ int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rg
     auto it = canvas_of.emplace(canvas_off[i], (int)canvases.size()).first;
     if (it->second == (int)canvases.size()) canvases.push_back({canvas + canvas_off[i], canvas + canvas_off[i], canvas_pitch[i]});
     SE_REQUIRE(canvases[it->second].pitch == canvas_pitch[i], "box " + std::to_string(i) + ": boxes of one canvas must have one pitch");
-    boxes[i] = {rgb + rgb_off[i], mask + mask_off[i], ih, iw, oh, ow, it->second, box_yx[2 * i], box_yx[2 * i + 1], {}};
+    boxes[i] = {rgb + rgb_off[i], mask + mask_off[i], ih, iw, oh, ow, it->second, box_yx[2 * i], box_yx[2 * i + 1], {}, nullptr};
+    if (detail && detail_off[i] >= 0) {
+      SE_REQUIRE(detail_off[i] % 2 == 0, "box " + std::to_string(i) + ": detail_off must be a multiple of 2 bytes");
+      boxes[i].detail = (const short*)((const char*)detail + detail_off[i]);
+    }
     if (feather) {
       const int* f = feather + 4 * (size_t)i;
       SE_REQUIRE(f[0] >= 0 && f[0] <= ow && f[2] >= 0 && f[2] <= ow && f[1] >= 0 && f[1] <= oh && f[3] >= 0 && f[3] <= oh,
@@ -813,6 +837,14 @@ int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rg
   if (n == 0) return 0;
   SE_REQUIRE(rgb && mask && canvas, "null rgb / mask / canvas");
   return paste_boxes(boxes, canvases, mid, scratch, swap_rb, (cudaStream_t)stream);
+}
+
+int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask,
+                                   const long long* mask_off, const int* src_hw, unsigned char* canvas, const long long* canvas_off,
+                                   const long long* canvas_pitch, const int* box_yx, const int* dst_hw, const int* feather, int n,
+                                   int swap_rb, void* scratch, long long* scratch_bytes, void* stream) {
+  return se_resize_composite_feather_detail_u8(rgb, rgb_off, mask, mask_off, src_hw, canvas, canvas_off, canvas_pitch, box_yx, dst_hw, feather,
+                                               nullptr, nullptr, n, swap_rb, scratch, scratch_bytes, stream);
 }
 
 int se_feather_u8(unsigned char* img, const long long* off, const int* hw, const int* feather, int n, void* stream) {

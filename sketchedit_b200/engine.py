@@ -53,6 +53,7 @@ class Engine:
         _lib.check(self.lib.se_model_create(ctypes.byref(h)))
         self.h = h
         self.finalized = False
+        self.use_cam = True              # the library's default options run the contextual attention
 
     def __del__(self):
         try:
@@ -91,6 +92,7 @@ class Engine:
         for key, val in (("use_cam", use_cam), ("pool_avg", pool_type == "avg"), ("no_mask_cc", no_mask_cc),
                          ("no_mask_coarse", no_mask_coarse), ("joint_train_inp", joint_train_inp)):
             _lib.check(self.lib.se_model_set_option(self.h, _lib.OPT[key], int(bool(val))))
+        self.use_cam = bool(use_cam)     # whether the forward has attention weights to export (inference_u8_export)
 
     def finalize(self):
         if not torch.cuda.is_available():
@@ -219,6 +221,33 @@ class Engine:
         _lib.check(self.lib.se_forward_u8_with_soft_mask(self.h, _ptr(image_u8), _ptr(sketch_u8), _ptr(edit_mask), B, H, W,
                                                          _lib.PREC[precision], _ptr(bgr), _stream()))
         return bgr
+
+    def inference_u8_export(self, image_u8, sketch_u8, edit_mask_u8=None, edit_mask=None, precision="bf16"):
+        """One of ``inference_u8`` (no edit mask), ``inference_with_mask_u8`` (``edit_mask_u8``) or
+        ``inference_u8_with_soft_mask`` (``edit_mask``, fp32 [B,1,H,W]), with netG's attention exported for region-edit detail
+        (``se_forward_u8_export``). Returns (bgr_u8 [B,H,W,3], mask_u8 [B,H,W] or None with an edit mask, attn fp32 [B,L,L],
+        hole_u8 [B,H,W]): bgr_u8 and mask_u8 are the chosen call's bit for bit; attn holds the attention's softmax weights as
+        the forward used them, [key][query] like ``contextual_attention(..., want_attn=True)``, L = (H/8 - 1)(W/8 - 1); hole_u8
+        is the mask netG inpaints as 0 / 1. attn takes 4 L^2 bytes per image: 3.7 MB at 256 x 256, 63 MB at 512 x 512. To return
+        it whole, the attention runs in one band of query rows: its L x L workspace (bf16: P at 2 L^2 bytes per image;
+        fp32_direct: S and P at 8 L^2) is then not held to ``set_attention_workspace_limit``. A model without the attention
+        (``use_cam=False``) has no weights to export: the call raises."""
+        if edit_mask_u8 is not None and edit_mask is not None:
+            raise _lib.SketchEditB200Error("give at most one of edit_mask_u8 and edit_mask")
+        ins = (("image_u8", image_u8), ("sketch_u8", sketch_u8)) + ((("edit_mask_u8", edit_mask_u8),) if edit_mask_u8 is not None else ())
+        B, H, W, ins, (bgr,), _ = self._forward_tensors(torch.uint8, ins, (3,), None)
+        predicted = edit_mask_u8 is None and edit_mask is None
+        mk = torch.empty(B, H, W, device=bgr.device, dtype=torch.uint8) if predicted else None
+        if edit_mask is not None:
+            _chk_out(edit_mask, (B, 1, H, W), "edit_mask")
+            self._on_device(edit_mask)
+        L = (H // 8 - 1) * (W // 8 - 1)
+        attn = _f32(B, L, L, like=bgr)
+        hole = torch.empty(B, H, W, device=bgr.device, dtype=torch.uint8)
+        _lib.check(self.lib.se_forward_u8_export(self.h, _ptr(ins[0]), _ptr(ins[1]), _ptr(ins[2]) if len(ins) > 2 else None,
+                                                 _ptr(edit_mask), B, H, W, _lib.PREC[precision], _ptr(bgr), _ptr(mk), _ptr(attn),
+                                                 _ptr(hole), _stream()))
+        return bgr, mk, attn, hole
 
     def netM(self, x, guide, precision="bf16", want_image=True):
         B, H, W, (x, guide), (mask1,), ex = self._forward_tensors(torch.float32, (("tensor", x), ("tensor", guide)), (1,), None,
@@ -434,7 +463,7 @@ def resize_window_u8_packed(src, src_offsets, src_pitches, src_sizes, dst_sizes,
 
 
 def resize_composite_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, canvas, canvas_offsets, canvas_pitches,
-                               box_offsets, box_sizes, swap_rb=False, feather=None):
+                               box_offsets, box_sizes, swap_rb=False, feather=None, detail=None, detail_offsets=None):
     """Resize back and paste boxes in order into canvases (``se_resize_composite_feather_u8``), bit for bit as sequential
     Pillow pastes, in place:
 
@@ -447,9 +476,11 @@ def resize_composite_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, 
     overlap. ``swap_rb`` reverses the result's channel order first (the forward writes BGR). All tensors are contiguous CUDA
     uint8 on one device; only the boxes' canvas pixels are read and written. To paste into a copy instead, copy the canvas
     first. ``feather``: None, or per box its ramp widths ``(left, top, right, bottom)`` in box pixels: the box's resized mask
-    becomes ``DIV255(m * ramp)`` before the blend, with the ramp of ``serving.feather_ramp``. Returns ``canvas``. Only
-    enqueues work on the current stream, except that the first resize between a pair of lengths uploads its coefficient
-    table."""
+    becomes ``DIV255(m * ramp)`` before the blend, with the ramp of ``serving.feather_ramp``. ``detail``: None, or a contiguous
+    CUDA int16 tensor holding at byte ``detail_offsets[i]`` box i's detail plane [h,w,3] (RGB, from ``detail_u8_packed``; an
+    offset < 0: none), added to the resized result with a clamp to [0, 255] before the blend
+    (``se_resize_composite_feather_detail_u8``). Returns ``canvas``. Only enqueues work on the current stream, except that the
+    first resize between a pair of lengths uploads its coefficient table."""
     n = len(src_sizes)
     if not (len(rgb_offsets) == len(mask_offsets) == len(canvas_offsets) == len(canvas_pitches) == len(box_offsets)
             == len(box_sizes) == n):
@@ -462,6 +493,16 @@ def resize_composite_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, 
     named = [(rgb, "rgb"), (mask, "mask"), (canvas, "canvas")]
     _chk_u8(*named)
     dev = _device(*named)
+    if detail is not None:
+        _chk_out(detail, None, "detail", torch.int16)
+        _device(*named, (detail, "detail"))
+        if detail_offsets is None or len(detail_offsets) != n:
+            raise _lib.SketchEditB200Error("detail needs one detail_offsets entry per box")
+        detail_offsets = [int(o) for o in detail_offsets]
+        for i, o in enumerate(detail_offsets):
+            h, w = int(box_sizes[i][0]), int(box_sizes[i][1])
+            if o >= 0 and (o % 2 or o + h * w * 6 > detail.numel() * 2):
+                raise _lib.SketchEditB200Error("detail %d at byte %d is outside the detail tensor or not 2-byte aligned" % (i, o))
     src_sizes, box_sizes, box_offsets = _hw(src_sizes), _hw(box_sizes), _hw(box_offsets)
     rgb_offsets, mask_offsets = [int(o) for o in rgb_offsets], [int(o) for o in mask_offsets]
     canvas_offsets, canvas_pitches = [int(o) for o in canvas_offsets], [int(p) for p in canvas_pitches]
@@ -475,11 +516,61 @@ def resize_composite_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, 
                    [(y + h, x + w) for (y, x), (h, w) in zip(box_offsets, box_sizes)], 3)
     lib = _lib.load()
     a = (_ptr(rgb), _longs(rgb_offsets), _ptr(mask), _longs(mask_offsets), _ints(src_sizes), _ptr(canvas), _longs(canvas_offsets),
-         _longs(canvas_pitches), _ints(box_offsets), _ints(box_sizes), _ints(feather) if feather is not None else None, n,
-         int(bool(swap_rb)))
+         _longs(canvas_pitches), _ints(box_offsets), _ints(box_sizes), _ints(feather) if feather is not None else None)
+    if detail is None:
+        call = lambda scratch, size, stream: lib.se_resize_composite_feather_u8(*a, n, int(bool(swap_rb)), scratch, size, stream)
+    else:
+        d = (_ptr(detail), _longs(detail_offsets), n, int(bool(swap_rb)))
+        call = lambda scratch, size, stream: lib.se_resize_composite_feather_detail_u8(*a, *d, scratch, size, stream)
     # one call: the entry keeps the boxes' order across its launches
-    _run_chunks(n, max(n, 1), dev, lambda sl: lambda scratch, size, stream: lib.se_resize_composite_feather_u8(*a, scratch, size, stream))
+    _run_chunks(n, max(n, 1), dev, lambda sl: call)
     return canvas
+
+
+def detail_u8_packed(photo, photo_offsets, photo_pitches, box_sizes, region_size, low, low_offsets, hole, hole_offsets, attn,
+                     attn_offsets, want_agg=False):
+    """Region-edit detail planes (``se_detail_u8``; DESIGN.md section 7b): for box i of ``box_sizes[i] = (bh, bw)`` edited at
+    ``region_size = (Hn, Wn)``, the RGB window of the photo whose row r starts at byte ``photo_offsets[i] + r * photo_pitches[i]``
+    of ``photo`` (one contiguous CUDA uint8 tensor, or a list with one per box), ``low``'s [bh,bw,3] at byte ``low_offsets[i]``
+    (the window resized to the working size and back), the forward's hole_u8 [Hn,Wn] at byte ``hole_offsets[i]`` of ``hole`` and
+    its attn [L,L] at element ``attn_offsets[i]`` of the fp32 tensor ``attn``. Returns ``(D, d_offsets, agg)``: D a CUDA int16
+    tensor holding box i's plane [bh,bw,3] at byte ``d_offsets[i]``, for ``resize_composite_u8_packed(..., detail=D,
+    detail_offsets=d_offsets)``; agg (``want_agg``) a CUDA float32 tensor holding box i's aggregate A [bh,bw,3] at element
+    ``d_offsets[i] // 2``, else None. Only enqueues work on the current stream. Transient device memory: one box's scratch at
+    a time, 4 Mp^2 + 12 Mp Np bytes (Mp = L rounded up to 256; Np = 3 fw fh rounded up to 256, fw = ceil(16 bw / Wn) + 2):
+    about 64 MB for a 608 x 608 box at 256 x 256."""
+    n = len(box_sizes)
+    listed = isinstance(photo, (list, tuple))
+    srcs = list(photo) if listed else [photo] * n
+    if not (len(srcs) == len(photo_offsets) == len(photo_pitches) == len(low_offsets) == len(hole_offsets) == len(attn_offsets) == n):
+        raise _lib.SketchEditB200Error("photo (as a list), photo_offsets, photo_pitches, box_sizes, low_offsets, hole_offsets and "
+                                       "attn_offsets must have the same length")
+    Hn, Wn = (int(v) for v in region_size)
+    L = (Hn // 8 - 1) * (Wn // 8 - 1)
+    named = [(t, "photo") for t in (srcs if listed else [photo])] + [(low, "low"), (hole, "hole")]
+    _chk_u8(*named)
+    _chk_out(attn, None, "attn")
+    dev = _device(*named, (attn, "attn"))
+    sizes = _hw(box_sizes)
+    photo_offsets, photo_pitches = [int(o) for o in photo_offsets], [int(p) for p in photo_pitches]
+    low_offsets, hole_offsets, attn_offsets = [int(o) for o in low_offsets], [int(o) for o in hole_offsets], [int(o) for o in attn_offsets]
+    _check_windows("window", srcs if listed else photo, photo_offsets, photo_pitches, sizes, 3)
+    _check_windows("low", low, low_offsets, [3 * w for _, w in sizes], sizes, 3)
+    _check_windows("hole", hole, hole_offsets, [Wn] * n, [(Hn, Wn)] * n, 1)
+    for i, o in enumerate(attn_offsets):
+        if o < 0 or o + L * L > attn.numel():
+            raise _lib.SketchEditB200Error("attn %d at element %d is outside the attn tensor" % (i, o))
+    d_offs, total = _aligned_offsets([h * w * 3 * 4 for h, w in sizes])   # room for A (fp32) at the same element index as D
+    D = torch.empty(max(total // 4, 1), device=dev, dtype=torch.int16)     # plane i at byte d_offs[i] // 2, 6 bh bw bytes
+    agg = torch.empty(max(total // 4, 1), device=dev, dtype=torch.float32) if want_agg else None
+    d_offs = [o // 2 for o in d_offs]
+    ptrs = [t.data_ptr() + o for t, o in zip(srcs, photo_offsets)]
+    lib = _lib.load()
+    a = ((ctypes.c_void_p * n)(*ptrs), _longs(photo_pitches), _ints(sizes), n, Hn, Wn, _ptr(low), _longs(low_offsets), _ptr(hole),
+         _longs(hole_offsets), _ptr(attn), _longs([4 * o for o in attn_offsets]), _ptr(D), _longs(d_offs), _ptr(agg),
+         _longs([2 * o for o in d_offs]) if want_agg else None)
+    _run_chunks(n, max(n, 1), dev, lambda sl: lambda scratch, size, stream: lib.se_detail_u8(*a, scratch, size, stream))
+    return D, d_offs, agg
 
 
 def feather_u8_packed(buf, offsets, sizes, feather):

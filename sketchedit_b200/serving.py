@@ -14,6 +14,7 @@ too (``engine.resize_u8_packed``, bit-identical to Pillow), so a batch is one up
     result_pil = proc.process_image(image_pil, mask_pil, region="auto")                 # edit a crop around the strokes only
     result_pil = proc.process_image(image_pil, mask_pil, region="strokes")              # one crop per group of strokes
     result_pil = proc.process_image(image_pil, mask_pil, region="auto", feather=16)     # paste fading over 16 px at inner edges
+    result_pil = proc.process_image(image_pil, mask_pil, region="auto", detail=True)    # restore the photo's fine detail in the hole
     s = proc.open_session(image_pil)                  # the photo stays on the device across edits
     r = s.edit(mask_pil, region="strokes")            # r.boxes, r.patches: what changed; s.undo() restores it
     p = s.propose(mask_pil, region="strokes")         # p.boxes, p.masks: the edit's region, from netM alone
@@ -25,7 +26,8 @@ A region edit (``region=``) crops a box of the photo, runs the forward on it at 
 the result back with the edit mask: its cost follows the box, not the photo, and region requests on photos of any size
 batch together. A request may carry several boxes (``region="strokes"`` or a list), pasted in order. ``feather=F`` fades each
 box's paste mask to 0 along the box edges that lie inside the photo (``feather_widths``, ``feather_ramp``), so the paste shows no
-seam there. An ``EditSession`` keeps one photo on the device for a chain of edits, each drawn on the previous result, with undo.
+seam there. ``detail=True`` adds back, inside the hole, the photo's high frequencies that the box's resize round trip lost,
+gathered with netG's own attention weights (``process_image``). An ``EditSession`` keeps one photo on the device for a chain of edits, each drawn on the previous result, with undo.
 
 Everything except the forward itself (``run_batch``) is plain host logic and is unit-tested on the CPU with a fake forward.
 """
@@ -262,6 +264,38 @@ def region_groups(mask, edit_mask=None, region_size=(256, 256), photo_size=None,
     return sorted(zip(groups, boxes), key=lambda gb: (gb[0][1], gb[0][0]))
 
 
+def detail_box_ok(size, region_size):
+    """Whether a box of PIL size ``(w, h)`` can take detail at the working size ``(Hn, Wn)``: every patch position of the
+    working grid must have a box-pixel anchor, ``u(w - 1) >= Wn - 16`` with ``u(x) = ((2x + 1) Wn) // (2 w)`` (and likewise
+    rows), which holds from ``w >= Wn / 32``. A narrower box has patches no box column maps into (DESIGN.md section 7b)."""
+    w, h = (int(v) for v in size)
+    Hn, Wn = (int(v) for v in region_size)
+    return (2 * w - 1) * Wn // (2 * w) >= Wn - 16 and (2 * h - 1) * Hn // (2 * h) >= Hn - 16
+
+
+def _check_detail(detail, region_none, host, has_attention=True):
+    """``detail`` checked against the request: a bool, and only for a region edit of the device flow on a model with the
+    contextual attention (whose weights it uses). Checked before the request is queued, so a detail request never makes a
+    batch it shares with other requests fail."""
+    if not isinstance(detail, bool):
+        raise ValueError("detail must be True or False, got %r" % (detail,))
+    if detail and not has_attention:
+        raise ValueError("detail=True needs the model's contextual attention (use_cam): it aggregates with its weights")
+    if detail and region_none:
+        raise ValueError("detail=True needs a region edit: the whole-photo flow only floors the photo to a multiple of 8, so no "
+                         "detail is lost to restore")
+    if detail and host:
+        raise ValueError("detail=True needs resize='device': the host flow has no GPU forward export to take it from")
+    return detail
+
+
+def _check_detail_boxes(boxes, region_size):
+    for b in boxes:
+        if not detail_box_ok((b[2] - b[0], b[3] - b[1]), region_size):
+            raise ValueError("detail=True needs boxes of at least 1/32 of the working size %dx%d per side, got box %r"
+                             % (region_size[1], region_size[0], tuple(b)))
+
+
 def _check_feather(feather):
     if isinstance(feather, bool) or not isinstance(feather, (int, np.integer)) or feather < 0:
         raise ValueError("feather must be an int >= 0 (photo pixels), got %r" % (feather,))
@@ -475,7 +509,7 @@ class DemoProcessor:
 
     def _run_region_device(self, key, payloads):
         """payloads: (photo crops [bh,bw,3] or None, sketch crops [bh,bw], edit-mask crops [bh,bw] or None, return_mask, boxes,
-        session photo or None, feather, photo PIL size): one crop per PIL box of the request, at its box size; key: ("region",
+        session photo or None, feather, photo PIL size, detail): one crop per PIL box of the request, at its box size; key: ("region",
         Hn, Wn), plus True when the batch runs on edit masks. Returns per request one (patch, mask) per box: patch [bh,bw,3] is
         the box's bytes once all of the request's boxes are pasted in order, mask the box's paste mask resized back to [bh,bw]
         (feathered as pasted) when asked for and predicted, else None. A box's feather widths follow from its place in the
@@ -483,9 +517,11 @@ class DemoProcessor:
         its photo ([h,w,3] on the device), snapshotted and pasted into it, and its result is (that list, [previous bytes of
         each box]). With SOFT in place of True (``EditSession.accept``) the edit-mask crops are a proposal's paste masks at
         the working size [H,W], and the payload ends with its fp32 soft masks [k,1,H,W] on the device, which the forward runs
-        on; no mask is returned."""
+        on; no mask is returned. When a request asks for detail the batch's forward also exports netG's attention and hole
+        (``Engine.inference_u8_export``; the same bytes), and that request's boxes are pasted with their detail planes
+        (``detail_u8_packed``), computed from the photo before any box of the batch is pasted."""
         torch = self._torch
-        from .engine import (_aligned_offsets, feather_u8_packed, resize_composite_u8_packed, resize_u8_packed,
+        from .engine import (_aligned_offsets, detail_u8_packed, feather_u8_packed, resize_composite_u8_packed, resize_u8_packed,
                              resize_window_u8_packed)
         H, W = key[1:3]
         edit, soft = key[-1] is True, key[-1] == SOFT
@@ -501,6 +537,7 @@ class DemoProcessor:
         edits = [payloads[r][2][j] for r, j in items] if edit or soft else []
         back = [i for i, (r, _) in enumerate(items) if payloads[r][3] and not edit and not soft]   # predicted masks to return
         fw = [feather_widths(boxes[i], payloads[r][7], payloads[r][6]) for i, (r, _) in enumerate(items)]
+        det = [i for i, (r, _) in enumerate(items) if payloads[r][8]]   # boxes pasted with detail
         # The work buffer: the plain requests' photo crops (uploaded; a box that overlaps no other box of its request is pasted
         # in place over its crop), the session boxes' patches, the predicted masks resized back (these three are the one
         # download), then the sketch and edit-mask crops (uploaded), then the canvases. A set of overlapping boxes of a plain
@@ -570,13 +607,29 @@ class DemoProcessor:
                     if edit:
                         pm = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
                         resize_u8_packed(work, sk_at[B:], sizes, [(H, W)] * B, 1, out=pm, dst_offsets=net1)
-                        bgr = self.engine.inference_with_mask_u8(img, msk, pm, precision=self.precision)
+                        if det:
+                            bgr, _, attn, hole = self.engine.inference_u8_export(img, msk, edit_mask_u8=pm, precision=self.precision)
+                        else:
+                            bgr = self.engine.inference_with_mask_u8(img, msk, pm, precision=self.precision)
                     elif soft:                        # the proposal's mask bytes were uploaded at the working size
                         pm, pm_at = work, sk_at[B:]
-                        slab = self._soft_slab([p[8] for p in payloads], H, W)
-                        bgr = self.engine.inference_u8_with_soft_mask(img, msk, slab, precision=self.precision)
+                        slab = self._soft_slab([p[9] for p in payloads], H, W)
+                        if det:
+                            bgr, _, attn, hole = self.engine.inference_u8_export(img, msk, edit_mask=slab, precision=self.precision)
+                        else:
+                            bgr = self.engine.inference_u8_with_soft_mask(img, msk, slab, precision=self.precision)
+                    elif det:
+                        bgr, pm, attn, hole = self.engine.inference_u8_export(img, msk, precision=self.precision)
                     else:
                         bgr, pm = self.engine.inference_u8(img, msk, precision=self.precision)
+                D = d_at = None
+                if det:                               # from the photo's bytes, before any box is pasted
+                    low, low_at = resize_u8_packed(img, [net3[i] for i in det], [(H, W)] * len(det), [sizes[i] for i in det], 3)
+                    L = attn.shape[1]
+                    D, d_offs, _ = detail_u8_packed([srcs[i] for i in det], [src_offs[i] for i in det], [pitches[i] for i in det],
+                                                    [sizes[i] for i in det], (H, W), low, low_at, hole, [net1[i] for i in det],
+                                                    attn, [i * L * L for i in det])
+                    d_at = dict(zip(det, d_offs))
                 for i in range(B):
                     if sess[i] is not None:
                         snaps[i] = in_photo(i).clone()
@@ -589,10 +642,12 @@ class DemoProcessor:
                     else:
                         place = [(0, sess[i].shape[1] * 3, boxes[i][1], boxes[i][0]) for i in g]
                         target = sess[g[0]].view(-1)
+                    gd = D is not None and any(i in d_at for i in g)
                     resize_composite_u8_packed(bgr, [net3[i] for i in g], pm, [pm_at[i] for i in g], [(H, W)] * len(g), target,
                                                [c[0] for c in place], [c[1] for c in place], [c[2:] for c in place],
                                                [sizes[i] for i in g], swap_rb=True,
-                                               feather=[fw[i] for i in g] if any(any(fw[i]) for i in g) else None)
+                                               feather=[fw[i] for i in g] if any(any(fw[i]) for i in g) else None,
+                                               detail=D if gd else None, detail_offsets=[d_at.get(i, -1) for i in g] if gd else None)
                 for i in canvas:
                     src, crop = in_canvas(work, i)
                     crop.copy_(src)
@@ -730,7 +785,7 @@ class DemoProcessor:
                     for e, p in zip(ends, payloads)]
         return [(np.ascontiguousarray(rgb[i]), mk[i] if mk is not None and p[3] else None) for i, p in enumerate(payloads)]
 
-    def process_image(self, img, mask, edit_mask=None, return_mask=False, region=None, feather=0):
+    def process_image(self, img, mask, edit_mask=None, return_mask=False, region=None, feather=0, detail=False):
         """img: PIL image; mask: PIL 'L' image, usually of the same size (non-zero = sketch stroke). Returns the edited PIL
         image at the input's size. Sizes are floored to a multiple of 8 for the network exactly like demo.py:43.
 
@@ -755,12 +810,26 @@ class DemoProcessor:
         of its paste mask m, ``widths = feather_widths(box, img.size, feather)``: the mask fades to 0 over a band along the box
         edges inside the photo, while edges on the photo's border stay hard. A predicted mask is returned as pasted (feathered);
         a given edit_mask is returned as given. 0 pastes exactly as without it. It does not change the forward, so requests
-        with different values share forwards. region=None has no inner edges: feather is checked and has no effect."""
+        with different values share forwards. region=None has no inner edges: feather is checked and has no effect.
+
+        detail: False (default) or True, for region edits with resize='device'. The network sees each box resampled to the
+        working size, so the pasted result is an upsample without the photo's fine detail. True adds it back inside the hole
+        (contextual residual aggregation): the detail the resize round trip removes from the photo, zero in the hole, is
+        gathered into each hole patch with the softmax weights netG's contextual attention computed, and added to the
+        resized result before the paste (DESIGN.md section 7b). False pastes exactly as without it. It needs a model with the
+        contextual attention (use_cam) and boxes of at least 1/32 of the working size per side (``detail_box_ok``); requests
+        that do not meet this raise ValueError before they are queued. It changes no forward
+        output, so requests with and without it share forwards; a batch with any detail request runs the forward that also
+        returns the attention weights, 4 L^2 bytes per box (L = (Hn/8 - 1)(Wn/8 - 1): 3.7 MB at 256 x 256, 63 MB at
+        512 x 512), held until the batch ends, and runs the attention in one band, so its L x L workspace is not held to
+        ``engine.set_attention_workspace_limit``; each detail box takes transient scratch (``engine.detail_u8_packed``).
+        Whether it looks better needs trained weights to judge. With region=None or resize='host' it is a ValueError."""
         from PIL import Image
         feather = _check_feather(feather)
+        detail = self._check_detail(detail, region is None)
         img = img.convert("RGB")
         if region is not None:
-            return self._process_region(img, mask, edit_mask, return_mask, region, feather)
+            return self._process_region(img, mask, edit_mask, return_mask, region, feather, detail)
         w_raw, h_raw = img.size
         h_t, w_t = floor8(h_raw), floor8(w_raw)
         if h_t < 16 or w_t < 16:
@@ -866,17 +935,19 @@ class DemoProcessor:
             if self.resize == "device" and m is not None and m.mode != "L":
                 raise ValueError("resize='device' takes an 'L' %s (got mode %r); resize='host' resizes it with Pillow" % (nm, m.mode))
 
-    def _process_region(self, img, mask, edit_mask, return_mask, region, feather=0):
+    def _process_region(self, img, mask, edit_mask, return_mask, region, feather=0, detail=False):
         from PIL import Image
         self._check_region_masks(img.size, mask, edit_mask)
         boxes = self._region_boxes(img.size, mask, edit_mask, region)
+        if detail:
+            _check_detail_boxes(boxes, self.region_size)
         if self.resize == "device":
             out = img.copy()
             crops = [np.asarray(img.crop(b)) for b in boxes]
             sketches = [np.asarray(mask.crop(b)) for b in boxes]
             edits = [np.asarray(edit_mask.crop(b)) for b in boxes] if edit_mask is not None else None
             got = self.batcher.submit(self._region_key(edit_mask),
-                                      (crops, sketches, edits, return_mask, boxes, None, feather, img.size))
+                                      (crops, sketches, edits, return_mask, boxes, None, feather, img.size, detail))
             for b, (patch, _) in zip(boxes, got):        # in order: a later patch holds the final bytes where boxes overlap
                 out.paste(Image.fromarray(patch), b[:2])
             mks = [Image.fromarray(mk) if mk is not None else None for _, mk in got]
@@ -887,6 +958,9 @@ class DemoProcessor:
         if edit_mask is not None:
             return out, edit_mask
         return out, Image.fromarray(_union_mask(img.size, boxes, mks))
+
+    def _check_detail(self, detail, region_none):
+        return _check_detail(detail, region_none, self.resize == "host", getattr(self.engine, "use_cam", True))
 
     def _region_key(self, edit_mask):
         # region requests on edit masks run their own forward, and region requests never share one with whole-photo requests
@@ -1121,7 +1195,7 @@ class EditSession:
             self._proposals.add(p)
             return p
 
-    def accept(self, p, edit_masks=None, return_mask=False):
+    def accept(self, p, edit_masks=None, return_mask=False, detail=False):
         """Makes the edit of the open proposal ``p`` of this session and returns its ``EditResult``, like ``edit``.
 
         ``edit_masks=None`` runs the forward on the proposal's fp32 soft masks (``Engine.inference_u8_with_soft_mask``; netM
@@ -1135,10 +1209,14 @@ class EditSession:
 
         The photo is not uploaded again: the device flow resizes the boxes again from the photo on the device, as ``edit``
         does, which keeps a proposal at its soft masks alone; the host flow keeps the Pillow-resized inputs it uploaded.
-        The proposal is then closed, and so are the session's other proposals."""
+        The proposal is then closed, and so are the session's other proposals. ``detail`` is ``edit``'s: ``accept(p,
+        detail=True)`` is ``edit(..., detail=True)`` byte for byte."""
         from PIL import Image
         if not isinstance(p, Proposal):
             raise TypeError("accept takes a Proposal of this session, got %r" % (type(p).__name__,))
+        detail = self._proc._check_detail(detail, p._whole)
+        if detail:
+            _check_detail_boxes(p.boxes, self._proc.region_size)
         with self._mu:
             self._check_open()
             if p._session is not self:
@@ -1154,7 +1232,7 @@ class EditSession:
             soft, work, inputs = p._soft, p._work, p._inputs
             self._drop_proposals()
             if edit_masks is not None:
-                return self._edit(p._mask, list(edit_masks), p.boxes, p._whole, return_mask, p._offset, p._feather)
+                return self._edit(p._mask, list(edit_masks), p.boxes, p._whole, return_mask, p._offset, p._feather, detail)
             proc, boxes = self._proc, p.boxes
             if self._img is not None:
                 prev = [self._img.crop(b) for b in boxes]
@@ -1177,7 +1255,7 @@ class EditSession:
                 else:
                     got, prev = proc.batcher.submit(("region",) + proc.region_size + (SOFT,),
                                                     (None, inputs, list(work), False, boxes, self._photo, p._feather, self.size,
-                                                     soft))
+                                                     detail, soft))
                 patches = [Image.fromarray(q) for q, _ in got]
             return self._record(boxes, prev, patches, list(p.masks) if return_mask else [None] * len(boxes))
 
@@ -1189,16 +1267,20 @@ class EditSession:
             self._held -= self._history.popleft()[2]
         return EditResult(boxes, patches, masks)
 
-    def edit(self, mask, edit_mask=None, region="auto", return_mask=False, offset=(0, 0), feather=0):
-        """One edit of the current photo; see the class. Returns ``EditResult(boxes, patches, masks)``."""
+    def edit(self, mask, edit_mask=None, region="auto", return_mask=False, offset=(0, 0), feather=0, detail=False):
+        """One edit of the current photo; see the class. Returns ``EditResult(boxes, patches, masks)``. ``detail`` is
+        ``DemoProcessor.process_image``'s (region edits of the device flow); undo restores the photo exactly either way."""
         feather = _check_feather(feather)
+        detail = self._proc._check_detail(detail, region is None)
         with self._mu:
             self._check_open()
             boxes = self._boxes(mask, edit_mask, region, offset)
+            if detail:
+                _check_detail_boxes(boxes, self._proc.region_size)
             self._drop_proposals()
-            return self._edit(mask, edit_mask, boxes, region is None, return_mask, tuple(int(v) for v in offset), feather)
+            return self._edit(mask, edit_mask, boxes, region is None, return_mask, tuple(int(v) for v in offset), feather, detail)
 
-    def _edit(self, mask, edit_mask, boxes, whole, return_mask, off, feather):
+    def _edit(self, mask, edit_mask, boxes, whole, return_mask, off, feather, detail=False):
         """``edit`` under the lock, on checked arguments; ``edit_mask`` may also be a list of each box's edit mask."""
         from PIL import Image
         if whole and isinstance(edit_mask, list):
@@ -1228,7 +1310,7 @@ class EditSession:
                 edits = None if edit_mask is None else [np.asarray(e) for e in edit_mask] if isinstance(edit_mask, list) \
                     else [np.asarray(edit_mask.crop(b)) for b in at]
                 got, prev = proc.batcher.submit(proc._region_key(edit_mask),
-                                                (None, sketches, edits, return_mask, boxes, self._photo, feather, self.size))
+                                                (None, sketches, edits, return_mask, boxes, self._photo, feather, self.size, detail))
             patches = [Image.fromarray(p) for p, _ in got]
             mks = [Image.fromarray(m) if m is not None else None for _, m in got]
         return self._record(boxes, prev, patches, [m if return_mask and edit_mask is None else None for m in mks])
