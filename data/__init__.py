@@ -22,6 +22,16 @@ def create_dataloader(opt):
     dataset = find_dataset_using_name(opt.dataset_mode)()
     dataset.initialize(opt)
     print("dataset [%s] of size %d was created" % (type(dataset).__name__, len(dataset)))
+    return loader_of(dataset, opt)
+
+
+def loader_of(dataset, opt, files=False):
+    """The DataLoader of ``dataset`` under opt's settings. files=True puts a TestImageDataset in its files mode (items carry
+    the PNG files, batches come from ``collate_files``), for the device decoder of ``inference_stream(uint8=True)``."""
+    collate = None
+    if files:
+        from data.testimage_dataset import collate_files
+        dataset.files, collate = True, collate_files
     return torch.utils.data.DataLoader(dataset, batch_size=opt.batchSize, shuffle=not opt.serial_batches,
                                        num_workers=int(opt.nThreads), drop_last=opt.isTrain,
-                                       pin_memory=True)
+                                       pin_memory=True, collate_fn=collate)

@@ -2,8 +2,13 @@
 an image under ``--image_dirs`` and a sketch under ``--mask_dirs``. The image becomes a [-1,1] RGB tensor,
 the sketch an 'L' image resized to the image size and binarised with ``> 0``. Several ';'-separated
 dir/list triples may be given. With ``--edit_mask_dir`` each item also carries the edit mask stored there under its
-output name ('edit_mask_u8' [H,W] uint8, 'edit_mask' [1,H,W] = v/255), resized to the image like the sketch."""
+output name ('edit_mask_u8' [H,W] uint8, 'edit_mask' [1,H,W] = v/255), resized to the image like the sketch.
+
+``files = True`` (test.py, when every input is a PNG) makes items carry the files instead of pixels, for the device
+decoder of ``EditLine2Model.inference_stream(uint8=True)``; ``collate_files`` packs them into batches."""
+import io
 import os
+from collections import namedtuple
 
 import numpy as np
 import torch
@@ -12,6 +17,8 @@ from PIL import Image
 
 
 class TestImageDataset(torch.utils.data.Dataset):
+    files = False   # items carry the photo, sketch and edit-mask files (bytes) and their sizes, not pixels
+
     @staticmethod
     def modify_commandline_options(parser, is_train):
         # same required flags and defaults as the reference (data/testimage_dataset.py:16-32)
@@ -46,8 +53,19 @@ class TestImageDataset(torch.utils.data.Dataset):
     def __len__(self):
         return len(self.items)
 
+    def edit_path(self, out):
+        epath = os.path.join(self.opt.edit_mask_dir, out)
+        if not os.path.isfile(epath):
+            raise FileNotFoundError("edit mask %s not found (--edit_mask_dir expects one file per output name)" % epath)
+        return epath
+
     def __getitem__(self, index):
         ipath, mpath, out = self.items[index]
+        if self.files:
+            item = {"path": out, "photo": _file(ipath), "sketch": _file(mpath)}
+            if getattr(self.opt, "edit_mask_dir", None) is not None:
+                item["edit"] = _file(self.edit_path(out))
+            return item
         img = Image.open(ipath).convert("RGB")
         w, h = img.size
         image_u8 = torch.from_numpy(np.asarray(img, dtype=np.uint8).copy())
@@ -62,12 +80,54 @@ class TestImageDataset(torch.utils.data.Dataset):
         edir = getattr(self.opt, "edit_mask_dir", None)
         if edir is not None:
             # the mask a previous run wrote under --output_mask_dir (possibly corrected by hand) replaces netM's prediction
-            epath = os.path.join(edir, out)
-            if not os.path.isfile(epath):
-                raise FileNotFoundError("edit mask %s not found (--edit_mask_dir expects one file per output name)" % epath)
-            em = Image.open(epath).convert("L")
+            em = Image.open(self.edit_path(out)).convert("L")
             if em.size != (w, h):
                 em = em.resize((w, h))
             item["edit_mask_u8"] = torch.from_numpy(np.asarray(em, dtype=np.uint8).copy())
             item["edit_mask"] = item["edit_mask_u8"].float().div(255)[None]
         return item
+
+
+def _file(path):
+    """(bytes, (h, w)) of an image file: the size from a PNG's IHDR, else from Pillow's header read."""
+    with open(path, "rb") as f:
+        data = f.read()
+    from sketchedit_b200 import pngfile
+    hw = pngfile.size(data)
+    if hw is None:
+        w, h = Image.open(io.BytesIO(data)).size
+        hw = (h, w)
+    return data, hw
+
+
+PngFile = namedtuple("PngFile", "target index head offset length size data")
+PngFile.__doc__ = """One file of a files-mode batch: target 'img', 'line' or 'edit'; index, its item in the batch; head, the
+``pngfile.PngHead`` without its stream (None when the parser sends the file to Pillow); offset and length of its stream in
+the batch's png_streams (its palette follows the stream); size, its (h, w); data, the file's bytes, which Pillow decodes
+when the parser or the device decoder refuses the file."""
+
+
+def collate_files(items):
+    """A batch of files-mode items for ``inference_stream(uint8=True)``: 'path' as usual; 'png_size', the photos' (H, W);
+    'png_streams', the joined IDAT payloads (and palette) of every file ``pngfile.parse`` sends to the device, packed in one
+    uint8 tensor (the DataLoader pins it); 'png', a ``PngFile`` per file: photos, then sketches, then edit masks."""
+    from sketchedit_b200 import pngfile
+    sizes = {it["photo"][1] for it in items}
+    if len(sizes) != 1:
+        raise RuntimeError("the photos of a batch must have one size, got %s" % sorted(sizes))
+    files, streams, at = [], [], 0
+    for target, key in (("img", "photo"), ("line", "sketch"), ("edit", "edit")):
+        for b, it in enumerate(items):
+            if key not in it:
+                continue
+            data, hw = it[key]
+            try:
+                hd = pngfile.parse(data)
+            except pngfile.Host:
+                files.append(PngFile(target, b, None, 0, 0, hw, data))
+                continue
+            files.append(PngFile(target, b, hd._replace(stream=b""), at, len(hd.stream), hw, data))
+            streams.append(hd.stream + hd.palette)   # engine.png_stage's layout: each stream followed by its palette
+            at += len(streams[-1])
+    packed = torch.frombuffer(bytearray(b"".join(streams)) or bytearray(1), dtype=torch.uint8)
+    return {"path": [it["path"] for it in items], "png_size": sizes.pop(), "png_streams": packed, "png": files}

@@ -288,6 +288,22 @@ int se_png_encode_u8(const unsigned char* const* src, const long long* src_pitch
  * the filtered data h (1 + w c) stored, 8 bytes per possible deflate block, the zlib header and Adler-32, 12 bytes per IDAT
  * chunk, the signature, IHDR and IEND. -1 on bad arguments. */
 long long se_png_max_bytes(int h, int w, int channels);
+/* Pixels of n in [0, 256] non-interlaced PNG files, pixel for pixel np.asarray(Image.open(f).convert(mode)) (Pillow 12) with
+ * mode "RGB" (HWC, 3 bytes) or "L". The host parses each file's container and passes its IDAT payloads concatenated into one
+ * zlib stream: file i's stream is the src_len[i] bytes at device address src + src_off[i]. info[6i..6i+5] are its height and
+ * width (in [1, 65535]), bit depth, colour type (0 at depth 1/2/4/8, 2 at 8, 3 at 1/2/4/8, 4 at 8, 6 at 8), palette entries
+ * (1 to 256 for colour type 3, else 0) and output bytes per pixel (3 "RGB", 1 "L"); a colour type 3 file's palette (RGB
+ * triples) is at src + plte_off[i] (plte_off may be NULL when no file has one). Its pixels go to the device address out[i]
+ * (h w mode bytes; out is a host array of n pointers, so one call fills several buffers), and its status to the device int
+ * status_dev[i]: 0 when the pixels are Pillow's, nonzero for anything doubtful (a bad zlib header or FDICT, a bad block or
+ * code, an over-subscribed table, a distance reaching before the start, too few or too many bytes, a wrong Adler-32, a
+ * filter type past 4, a palette index past the palette), when the pixels are undefined and the file must go to Pillow. Bytes after the Adler-32 are ignored. Every read is checked against src_len[i] and every
+ * write against the file's raw size. scratch holds each file's raw filtered scanlines, h (1 + ceil(w bits / 8)) bytes
+ * rounded up to 16; scratch == NULL stores the bytes the call needs in *scratch_bytes (src, out and status_dev may be NULL
+ * then). Every argument is checked before anything is enqueued on `stream`; the call only enqueues. */
+int se_png_decode_u8(const unsigned char* src, const long long* src_off, const long long* src_len, const int* info,
+                     const long long* plte_off, int n, unsigned char* const* out, int* status_dev,
+                     void* scratch, long long* scratch_bytes, void* stream);
 /* Bytes of coefficient tables the resize entries keep per device (process-wide; 0 restores the default of 256 MiB; negative is an
  * error). When a call's new tables would pass the limit, the device's cache is emptied (after a device synchronise) before the
  * call looks up any table; one call's own tables may exceed it. */

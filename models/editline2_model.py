@@ -100,6 +100,13 @@ class EditLine2Model(torch.nn.Module):
         (``Engine.inference_with_mask_u8``) and its mask result is a copy of the supplied bytes; batches with and without
         one may be mixed. Float mode rejects batches that carry an edit mask.
 
+        uint8 mode also takes batches of PNG files (``data.testimage_dataset.collate_files``: 'png_streams', 'png', 'png_size'
+        in place of the pixels): their compressed streams are uploaded from pinned memory and decoded on the input stream
+        into the batch's input buffers (``engine.png_decode_u8_packed``), sketches and edit masks of another size than their
+        photo resized to it as Pillow's ``.resize`` does. The host reads the decoder's per-file status once the decode is
+        done (the previous batch's forward is already queued by then) and uploads Pillow's pixels of the files the parser or
+        the decoder sent to it before the batch's forward.
+
         with_data=True: yield ``(out0, out1, data)`` (test.py needs the batch's output paths).
 
         png=("image",) or ("image", "mask") (uint8 mode): each batch's BGR results (and masks) are encoded on the device after
@@ -165,11 +172,18 @@ class EditLine2Model(torch.nn.Module):
 
         in_keys = ("image_u8", "mask_u8") if uint8 else ("image", "mask")
         for i, data in enumerate(loader):
-            img_h, line_h = data[in_keys[0]], data[in_keys[1]]
-            edit_h = data.get("edit_mask_u8") if uint8 else None
+            files = data.get("png") if uint8 else None
+            if files is not None:
+                B, (H, W) = len(data["path"]), data["png_size"]
+                edit_h = True if any(f.target == "edit" for f in files) else None
+            else:
+                img_h, line_h = data[in_keys[0]], data[in_keys[1]]
+                edit_h = data.get("edit_mask_u8") if uint8 else None
+                B, H, W = (img_h.shape[0], img_h.shape[1], img_h.shape[2]) if uint8 else (img_h.shape[0], img_h.shape[2], img_h.shape[3])
             if not uint8 and (data.get("edit_mask") is not None or data.get("edit_mask_u8") is not None):
                 raise ValueError("inference_stream runs batches with an edit mask in uint8 mode only (uint8=True, data['edit_mask_u8'])")
-            B, H, W = (img_h.shape[0], img_h.shape[1], img_h.shape[2]) if uint8 else (img_h.shape[0], img_h.shape[2], img_h.shape[3])
+            if not uint8 and data.get("png") is not None:
+                raise ValueError("inference_stream runs batches of PNG files in uint8 mode only (uint8=True)")
             slot = slots[i % depth]
             fresh = slot is None or slot["shape"] != (B, H, W) or (edit_h is not None and "edit" not in slot)
             if slot is None or slot["shape"] != (B, H, W):
@@ -197,10 +211,13 @@ class EditLine2Model(torch.nn.Module):
             if edit_h is not None:
                 s_in.wait_event(slot["ev_out"])        # ... and the edit mask, which is also an output, has left the device
             with torch.cuda.stream(s_in):
-                slot["img"].copy_(img_h, non_blocking=True)
-                slot["line"].copy_(line_h, non_blocking=True)
-                if edit_h is not None:
-                    slot["edit"].copy_(edit_h, non_blocking=True)
+                if files is not None:
+                    _decode_png_batch(data, slot, B, H, W, dev)
+                else:
+                    slot["img"].copy_(img_h, non_blocking=True)
+                    slot["line"].copy_(line_h, non_blocking=True)
+                    if edit_h is not None:
+                        slot["edit"].copy_(edit_h, non_blocking=True)
                 slot["ev_in"].record(s_in)
             cur.wait_event(slot["ev_in"])
             cur.wait_event(slot["ev_out"])             # ... and its outputs have left the device buffers
@@ -251,3 +268,49 @@ class EditLine2Model(torch.nn.Module):
                 yield drain_one()
         while pending:
             yield drain_one()
+
+
+def _decode_png_batch(data, slot, B, H, W, dev):
+    """Enqueues on the current stream the decode of a batch of PNG files (``collate_files``) into slot['img'], ['line'] and
+    ['edit']: one upload of the streams and one decode launch straight into the slot's buffers (files of another size than
+    the photo go to a staging buffer and are resized into them, as Pillow's ``.resize`` does); the host waits for the status
+    words and puts Pillow's pixels in place of the files the parser or the decoder sent to Pillow."""
+    import numpy as np
+
+    from sketchedit_b200 import engine as E
+    from sketchedit_b200 import pngfile
+    files = data["png"]
+    chans = {"img": 3, "line": 1, "edit": 1}
+    mode = {"img": "RGB", "line": "L", "edit": "L"}
+    sized = [k for k, f in enumerate(files) if tuple(f.size) != (H, W)]   # sketches / edit masks to resize (photos set H, W)
+    aux_offs, aux_total = E._aligned_offsets([files[k].size[0] * files[k].size[1] for k in sized])
+    aux = torch.empty(max(aux_total, 1), device=dev, dtype=torch.uint8)
+    where = {k: (aux, o) for k, o in zip(sized, aux_offs)}   # file -> (buffer, byte offset) of its decoded pixels
+    for k, f in enumerate(files):
+        if k not in where:
+            where[k] = (slot[f.target].view(-1), f.index * H * W * chans[f.target])
+    on_dev = [k for k, f in enumerate(files) if f.head is not None]
+    bad = [k for k, f in enumerate(files) if f.head is None]
+    if on_dev:
+        src = data["png_streams"].to(dev, non_blocking=True)
+        status = E.png_decode_u8_packed(src, [files[k].offset for k in on_dev], [files[k].length for k in on_dev],
+                                        [files[k].head for k in on_dev], [mode[files[k].target] for k in on_dev],
+                                        out=[where[k][0] for k in on_dev], out_offsets=[where[k][1] for k in on_dev])[2]
+        status_h = torch.empty(len(on_dev), dtype=torch.int32, pin_memory=True)
+        status_h.copy_(status, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        ev.synchronize()
+        bad += [k for k, s in zip(on_dev, status_h.tolist()) if s]
+    for k in bad:
+        f = files[k]
+        px = np.ascontiguousarray(pngfile.pillow_decode(f.data, mode[f.target]))
+        if px.shape[:2] != tuple(f.size):
+            raise RuntimeError("%s decodes to %dx%d, its header says %dx%d" % ((data["path"][f.index],) + px.shape[:2] + tuple(f.size)))
+        buf, o = where[k]
+        buf[o:o + px.size].copy_(torch.from_numpy(px).reshape(-1).pin_memory(), non_blocking=True)
+    for target in ("line", "edit"):
+        ks = [k for k in sized if files[k].target == target]
+        if ks:
+            E.resize_u8_packed(aux, [where[k][1] for k in ks], [files[k].size for k in ks], [(H, W)] * len(ks), 1,
+                               out=slot[target].view(-1), dst_offsets=[files[k].index * H * W for k in ks])

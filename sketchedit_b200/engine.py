@@ -11,7 +11,7 @@ import numbers
 
 import torch
 
-from . import _lib
+from . import _lib, pngfile
 from .arch import NET_LAYERS, layer_map, out_channels_after_gate
 
 
@@ -830,6 +830,114 @@ def png_encode_u8(images, swap_rb=False):
     out_bytes = torch.empty(len(images), device=dev, dtype=torch.int64)
     _png_launch([t.data_ptr() for t in images], [t.stride(0) for t in images], sizes, C, swap_rb, out, offs, out_bytes)
     return download_files(out, offs, out_bytes.cpu().tolist())
+
+
+PNG_DECODE_MAX_BATCH = 256   # files per se_png_decode_u8 call; the wrappers split longer lists into calls of this size
+
+
+def png_stage(heads):
+    """The streams of the ``pngfile.PngHead`` list ``heads``, each followed by its palette, packed into one pinned uint8
+    tensor: ``(staging, offsets, lengths)`` of the streams, the layout ``png_decode_u8_packed`` reads."""
+    parts = [hd.stream + hd.palette for hd in heads]
+    staging = torch.empty(max(1, sum(map(len, parts))), dtype=torch.uint8, pin_memory=True)
+    buf, offsets, at = staging.numpy(), [], 0
+    for part in parts:
+        buf[at:at + len(part)] = memoryview(part).cast("B") if part else ()
+        offsets.append(at)
+        at += len(part)
+    return staging, offsets, [len(hd.stream) for hd in heads]
+
+
+def png_decode_u8_packed(src, src_offsets, src_lengths, heads, modes, out=None, out_offsets=None):
+    """Pixels of PNG files from their zlib streams (``se_png_decode_u8``), one launch per PNG_DECODE_MAX_BATCH files: file
+    i's IDAT payloads, joined, are the ``src_lengths[i]`` bytes at ``src_offsets[i]`` of the contiguous CUDA uint8 tensor
+    ``src``, followed there by its palette when it has one (``png_stage``'s layout); ``heads[i]`` is its
+    ``pngfile.PngHead`` (size, depth, colour type, palette length; its ``stream`` is not read) and ``modes[i]`` (or one
+    ``modes`` for all) is "RGB" or "L". ``out`` (optional) is one contiguous CUDA uint8 tensor or a list of them with one
+    per file; file i's h x w x 3 or h x w bytes go to ``out_offsets[i]`` of its tensor. Returns ``(out, out_offsets,
+    status)``: ``status`` is a CUDA int32 tensor, 0 where the pixels are ``np.asarray(Image.open(f).convert(mode))`` and
+    nonzero where the file must go to Pillow. Only enqueues work on the current stream."""
+    n = len(heads)
+    modes = [modes] * n if isinstance(modes, str) else list(modes)
+    if len(modes) != n or len(src_offsets) != n or len(src_lengths) != n:
+        raise _lib.SketchEditB200Error("src_offsets, src_lengths, heads and modes must have the same length")
+    if any(m not in pngfile.MODES for m in modes):
+        raise ValueError("modes must be 'RGB' or 'L', got %r" % (modes,))
+    outs = list(out) if isinstance(out, (list, tuple)) else None
+    if outs is not None and len(outs) != n:
+        raise _lib.SketchEditB200Error("out (as a list) needs one tensor per file")
+    named = [(src, "src")] + [(t, "out") for t in (outs if outs is not None else [out] if out is not None else [])]
+    _chk_u8(*named)
+    dev = _device(*named)
+    src_offsets, src_lengths = [int(o) for o in src_offsets], [int(k) for k in src_lengths]
+    plens = [len(hd.palette) for hd in heads]
+    _check_windows("stream", src, src_offsets, [k + p for k, p in zip(src_lengths, plens)],
+                   [(1, k + p) for k, p in zip(src_lengths, plens)], 1)
+    plte_offs = [o + k for o, k in zip(src_offsets, src_lengths)]
+    chans = [pngfile.MODES[m] for m in modes]
+    nbytes = [hd.h * hd.w * c for hd, c in zip(heads, chans)]
+    if outs is None:
+        out, out_offsets = _out(out, out_offsets, nbytes, dev, "out_offsets")
+        outs = [out] * n
+    else:
+        if out_offsets is None or len(out_offsets) != n:
+            raise _lib.SketchEditB200Error("out needs one out_offsets entry per file")
+        out_offsets = [int(o) for o in out_offsets]
+        _check_windows("out", outs, out_offsets, nbytes, [(1, b) for b in nbytes], 1)
+    status = torch.empty(n, device=dev, dtype=torch.int32)
+    if n == 0:
+        return out, out_offsets, status
+    info = [(hd.h, hd.w, hd.depth, hd.ctype, len(hd.palette) // 3, c) for hd, c in zip(heads, chans)]
+    dst = [t.data_ptr() + o for t, o in zip(outs, out_offsets)]
+    lib = _lib.load()
+
+    def chunk(sl):
+        k = len(info[sl])
+        a = (_ptr(src), _longs(src_offsets[sl]), _longs(src_lengths[sl]), _ints(info[sl]), _longs(plte_offs[sl]), k,
+             (ctypes.c_void_p * k)(*dst[sl]), ctypes.c_void_p(status.data_ptr() + 4 * sl.start))
+        return lambda scratch, size, stream: lib.se_png_decode_u8(*a, scratch, size, stream)
+
+    _run_chunks(n, PNG_DECODE_MAX_BATCH, dev, chunk)
+    return out, out_offsets, status
+
+
+def png_decode_u8(files, mode="RGB", device=None):
+    """Pixels of PNG files (``bytes``) as CUDA uint8 tensors, [h, w, 3] for ``mode`` "RGB" and [h, w] for "L", each equal to
+    ``np.asarray(Image.open(f).convert(mode))``, Pillow's exception included. Files ``pngfile.parse`` accepts are decoded on
+    the device (one upload of their streams from pinned staging, then one download of the status words); the others, and
+    any the device reports a nonzero status for, are decoded by Pillow and uploaded.
+
+    Device memory: the pixels, the compressed streams and, while the call runs, each file's raw filtered scanlines
+    (h (1 + w bytes per pixel) bytes)."""
+    files = list(files)
+    dev = torch.device("cuda") if device is None else torch.device(device)
+    heads = []
+    for f in files:
+        try:
+            heads.append(pngfile.parse(f))
+        except pngfile.Host:
+            heads.append(None)
+    on_dev = [i for i, hd in enumerate(heads) if hd is not None]
+    res = [None] * len(files)
+    if on_dev:
+        with torch.cuda.device(dev):
+            staging, offs, lens = png_stage([heads[i] for i in on_dev])
+            src = staging.to(dev, non_blocking=True)
+            out, out_offs, status = png_decode_u8_packed(src, offs, lens, [heads[i] for i in on_dev], mode)
+            c = pngfile.MODES[mode]
+            for k, i in enumerate(on_dev):
+                hd = heads[i]
+                if c == 3:
+                    res[i] = out[out_offs[k]:out_offs[k] + hd.h * hd.w * 3].view(hd.h, hd.w, 3)
+                else:
+                    res[i] = out[out_offs[k]:out_offs[k] + hd.h * hd.w].view(hd.h, hd.w)
+            for k, s in enumerate(status.cpu().tolist()):
+                if s:
+                    res[on_dev[k]] = None
+    for i, r in enumerate(res):
+        if r is None:
+            res[i] = torch.from_numpy(pngfile.pillow_decode(files[i], mode).copy()).to(dev)
+    return res
 
 
 def outputs_to_uint8(composed, mask):

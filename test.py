@@ -15,10 +15,37 @@ import data
 import models
 from options.test_options import TestOptions
 
+# PNG inputs are decoded on the device only where tools/png_decode_bench.py measured it faster than the host loader at both
+# 1 and 8 workers (H100 80GB HBM3, 700 W, steady images/s): 256² batch 16 (338 and 332 against 72 and 241), 256² batch 128
+# (1203 and 1493 against 111 and 1381), 512² batch 16 (102 and 96 against 24 and 80). It lost at batch 4 with 8 workers
+# (87 against 105 at 256², 26 against 44 at 512², 8.7 against 19.5 at 1024²) and at batch 1 (23 against 42): one warp
+# decodes each file, so small batches and large photos leave most of the GPU idle while a file decodes serially.
+PNG_DECODE_MIN_BATCH = 16
+PNG_DECODE_MAX_PIXELS = 512 * 512
+
+
+def _png_inputs(dataset, opt):
+    """Whether test.py's loader hands the device decoder the files: every photo, sketch and edit mask is a PNG by its name
+    (any case), batches hold PNG_DECODE_MIN_BATCH images or more, and no photo's IHDR is larger than PNG_DECODE_MAX_PIXELS."""
+    from sketchedit_b200 import pngfile
+    items = getattr(dataset, "items", None)
+    edits = getattr(opt, "edit_mask_dir", None) is not None   # an edit mask is named like its output, items' third entry
+    if not items or opt.batchSize < PNG_DECODE_MIN_BATCH or not all(
+            p.lower().endswith(".png") for it in items for p in (it if edits else it[:2])):
+        return False
+    for ipath, _, _ in items:
+        with open(ipath, "rb") as f:
+            hw = pngfile.size(f.read(24))
+        if hw is None or hw[0] * hw[1] > PNG_DECODE_MAX_PIXELS:
+            return False
+    return True
+
 
 def main(argv=None):
     opt = TestOptions().parse(argv)
     dataloader = data.create_dataloader(opt)
+    if _png_inputs(dataloader.dataset, opt):   # decoded on the device, pixel for pixel as Pillow opens them
+        dataloader = data.loader_of(dataloader.dataset, opt, files=True)
     model = models.create_model(opt)
     model.eval()
 
