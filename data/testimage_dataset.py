@@ -115,7 +115,7 @@ def collate_files(items):
     sizes = {it["photo"][1] for it in items}
     if len(sizes) != 1:
         raise RuntimeError("the photos of a batch must have one size, got %s" % sorted(sizes))
-    files, streams, at = [], [], 0
+    files = []
     for target, key in (("img", "photo"), ("line", "sketch"), ("edit", "edit")):
         for b, it in enumerate(items):
             if key not in it:
@@ -124,10 +124,10 @@ def collate_files(items):
             try:
                 hd = pngfile.parse(data)
             except pngfile.Host:
-                files.append(PngFile(target, b, None, 0, 0, hw, data))
-                continue
-            files.append(PngFile(target, b, hd._replace(stream=b""), at, len(hd.stream), hw, data))
-            streams.append(hd.stream + hd.palette)   # engine.png_stage's layout: each stream followed by its palette
-            at += len(streams[-1])
-    packed = torch.frombuffer(bytearray(b"".join(streams)) or bytearray(1), dtype=torch.uint8)
+                hd = None
+            files.append((target, b, hd, hw, data))
+    packed, offs, lens = pngfile.stage([f[2] for f in files if f[2] is not None], lambda n: torch.empty(n, dtype=torch.uint8))
+    staged = iter(zip(offs, lens))
+    files = [PngFile(t, b, None, 0, 0, hw, data) if hd is None else PngFile(t, b, hd._replace(stream=b""), *next(staged), hw, data)
+             for t, b, hd, hw, data in files]
     return {"path": [it["path"] for it in items], "png_size": sizes.pop(), "png_streams": packed, "png": files}

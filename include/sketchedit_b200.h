@@ -204,17 +204,13 @@ int se_resize_window_u8(const unsigned char* const* src, const long long* src_pi
  *     ramp(d, f) = d >= f ? 255 : (255 * (d + 1)) / (f + 1)   (integer division; d = 0 on the side's edge pixel),
  * with (y, x) the pixel's place in the box. A side of width 0 keeps m; DIV255(255 * m) == m, so widths of 0 give the bytes of
  * feather == NULL, and a box whose four widths are 0 runs its arithmetic unchanged.
+ * detail (may be NULL, and detail_off with it: none) adds a detail plane per box (region-edit detail): it holds at byte
+ * detail_off[i] (even; a negative offset: box i has none) box i's int16 plane [h][w][3] in RGB order, as se_detail_u8 writes
+ * it. Box i's resized result, after the vertical pass's rounding and the channel swap, becomes clamp(res + D, 0, 255) before
+ * the blend.
  * scratch holds the intermediates of boxes whose width changes: r256(src_hw[2i] * w * 3) + r256(src_hw[2i] * w) bytes for
  * box i, r256 rounding up to 256. The scratch query (scratch == NULL; rgb, mask and canvas may be NULL then) and the
  * coefficient-table cache are those of se_resize_window_u8. */
-int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask,
-                                   const long long* mask_off, const int* src_hw, unsigned char* canvas, const long long* canvas_off,
-                                   const long long* canvas_pitch, const int* box_yx, const int* dst_hw, const int* feather, int n,
-                                   int swap_rb, void* scratch, long long* scratch_bytes, void* stream);
-/* se_resize_composite_feather_u8 with a detail plane per box (region-edit detail): detail (may be NULL: none) holds at byte
- * detail_off[i] (even; a negative offset: box i has none) box i's int16 plane [h][w][3] in RGB order, as se_detail_u8 writes
- * it. Box i's resized result, after the vertical pass's rounding and the channel swap, becomes clamp(res + D, 0, 255) before
- * the blend; everything else is se_resize_composite_feather_u8's, which is this call with detail = NULL. */
 int se_resize_composite_feather_detail_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask,
                                           const long long* mask_off, const int* src_hw, unsigned char* canvas, const long long* canvas_off,
                                           const long long* canvas_pitch, const int* box_yx, const int* dst_hw, const int* feather,
@@ -241,20 +237,24 @@ int se_detail_u8(const unsigned char* const* photo, const long long* photo_pitch
                  const unsigned char* low, const long long* low_off, const unsigned char* hole, const long long* hole_off, const float* attn,
                  const long long* attn_off, short* D, const long long* d_off, float* agg, const long long* agg_off, void* scratch,
                  long long* scratch_bytes, void* stream);
-/* The feather of se_resize_composite_feather_u8 on masks alone, in place: image i is the hw[2i] x hw[2i+1] 'L' bytes (rows
+/* The feather of se_resize_composite_feather_detail_u8 on masks alone, in place: image i is the hw[2i] x hw[2i+1] 'L' bytes (rows
  * packed) at img + off[i], and each of its bytes m becomes DIV255(m * r(y, x)) with the ramp r of its widths feather[4i .. 4i+3]
  * (left, top, right, bottom; each in [0, the side's length]). Sizes are in [1, 65535]; an image with four widths of 0 is not
  * touched. For a predicted mask resized back to its box this gives the mask the feathered paste used. Only enqueues the
  * kernel on `stream`. */
 int se_feather_u8(unsigned char* img, const long long* off, const int* hw, const int* feather, int n, void* stream);
-/* ABI version 2 retired three resize entries of version 1. Each is a call of the entries above:
+/* Retired entries. Each is a call of the entries above. ABI version 2 retired three resize entries of version 1:
  *   se_resize_u8(src, src_off, src_hw, dst, dst_off, dst_hw, n, channels, ...)
  *       = se_resize_window_u8 with src[i] = src + src_off[i] and src_pitch[i] = src_hw[2i+1] * channels.
  *   se_resize_paste_u8(rgb, rgb_off, mask, mask_off, src_hw, base, base_off, dst, dst_off, dst_hw, n, ...)
- *       = se_resize_composite_feather_u8 with one box per canvas: canvas_off[i] = base_off[i] of canvas = base, box_yx[i] =
- *         (0, 0), canvas_pitch[i] = 3 * dst_hw[2i+1], feather = NULL, pasting in place. For a separate dst, first copy each
- *         base image to its dst slice and composite into dst.
- *   se_resize_composite_u8(...) = se_resize_composite_feather_u8(...) with feather = NULL. */
+ *       = se_resize_composite_feather_detail_u8 with one box per canvas: canvas_off[i] = base_off[i] of canvas = base,
+ *         box_yx[i] = (0, 0), canvas_pitch[i] = 3 * dst_hw[2i+1], feather = detail = detail_off = NULL, pasting in place. For a
+ *         separate dst, first copy each base image to its dst slice and composite into dst.
+ *   se_resize_composite_u8(...) = se_resize_composite_feather_detail_u8(...) with feather = detail = detail_off = NULL.
+ * ABI version 3 retired one more:
+ *   se_resize_composite_feather_u8(rgb, rgb_off, mask, mask_off, src_hw, canvas, canvas_off, canvas_pitch, box_yx, dst_hw,
+ *                                  feather, n, swap_rb, scratch, scratch_bytes, stream)
+ *       = se_resize_composite_feather_detail_u8 with the same arguments and detail = detail_off = NULL before n. */
 /* Baseline JPEG of n in [0, 32] RGB windows, byte for byte what Pillow writes for an RGB image without info:
  *     buf = io.BytesIO();  Image.fromarray(img_i).save(buf, "JPEG", quality=quality, subsampling=subsampling)
  * quality in [1, 100]; subsampling 0 (4:4:4) or 2 (4:2:0, Pillow's default with quality 75). Image i is hw[2i] rows of

@@ -272,13 +272,9 @@ class EditLine2Model(torch.nn.Module):
 
 def _decode_png_batch(data, slot, B, H, W, dev):
     """Enqueues on the current stream the decode of a batch of PNG files (``collate_files``) into slot['img'], ['line'] and
-    ['edit']: one upload of the streams and one decode launch straight into the slot's buffers (files of another size than
-    the photo go to a staging buffer and are resized into them, as Pillow's ``.resize`` does); the host waits for the status
-    words and puts Pillow's pixels in place of the files the parser or the decoder sent to Pillow."""
-    import numpy as np
-
+    ['edit'] (``engine.png_decode_into``: Pillow's pixels wherever the parser or the decoder refuses a file). Files of another
+    size than the photo go to a staging buffer and are resized into them, as Pillow's ``.resize`` does."""
     from sketchedit_b200 import engine as E
-    from sketchedit_b200 import pngfile
     files = data["png"]
     chans = {"img": 3, "line": 1, "edit": 1}
     mode = {"img": "RGB", "line": "L", "edit": "L"}
@@ -289,26 +285,10 @@ def _decode_png_batch(data, slot, B, H, W, dev):
     for k, f in enumerate(files):
         if k not in where:
             where[k] = (slot[f.target].view(-1), f.index * H * W * chans[f.target])
-    on_dev = [k for k, f in enumerate(files) if f.head is not None]
-    bad = [k for k, f in enumerate(files) if f.head is None]
-    if on_dev:
-        src = data["png_streams"].to(dev, non_blocking=True)
-        status = E.png_decode_u8_packed(src, [files[k].offset for k in on_dev], [files[k].length for k in on_dev],
-                                        [files[k].head for k in on_dev], [mode[files[k].target] for k in on_dev],
-                                        out=[where[k][0] for k in on_dev], out_offsets=[where[k][1] for k in on_dev])[2]
-        status_h = torch.empty(len(on_dev), dtype=torch.int32, pin_memory=True)
-        status_h.copy_(status, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        ev.synchronize()
-        bad += [k for k, s in zip(on_dev, status_h.tolist()) if s]
-    for k in bad:
-        f = files[k]
-        px = np.ascontiguousarray(pngfile.pillow_decode(f.data, mode[f.target]))
-        if px.shape[:2] != tuple(f.size):
-            raise RuntimeError("%s decodes to %dx%d, its header says %dx%d" % ((data["path"][f.index],) + px.shape[:2] + tuple(f.size)))
-        buf, o = where[k]
-        buf[o:o + px.size].copy_(torch.from_numpy(px).reshape(-1).pin_memory(), non_blocking=True)
+    parsed = [f for f in files if f.head is not None]
+    E.png_decode_into((data["png_streams"], [f.offset for f in parsed], [f.length for f in parsed]), [f.head for f in files],
+                      [mode[f.target] for f in files], [f.data for f in files], [where[k] + (f.size,) for k, f in enumerate(files)],
+                      [data["path"][f.index] for f in files], dev)
     for target in ("line", "edit"):
         ks = [k for k in sized if files[k].target == target]
         if ks:

@@ -37,6 +37,55 @@ const char* last_error();
   } while (0)
 
 // ------------------------------------------------------------------------------------------
+// batch entries of the image I/O (resize, composite, detail, JPEG and PNG codecs)
+constexpr int kMaxDim = 65535;   // largest image side they take: the JPEG header's 16-bit size fields
+
+// scratch arrays start at multiples of 256 bytes
+inline size_t scratch_round(size_t bytes) { return (bytes + 255) / 256 * 256; }
+// blocks of per_block threads covering `threads` threads; also tiles of per_block covering a length
+inline unsigned grid_of(long long threads, int per_block) { return (unsigned)((threads + per_block - 1) / per_block); }
+
+// The scratch protocol of a batch entry that takes (void* scratch, long long* scratch_bytes): without scratch the call is a
+// query and stores the bytes it needs; with it, the scratch must hold them. Either way a call of no images ends here.
+#define SE_SCRATCH(scratch, scratch_bytes, need, n)                                                                  \
+  do {                                                                                                               \
+    const long long _need = (long long)(need);                                                                       \
+    if (!(scratch)) {                                                                                                \
+      *(scratch_bytes) = _need;                                                                                      \
+      return 0;                                                                                                      \
+    }                                                                                                                \
+    SE_REQUIRE(*(scratch_bytes) >= _need,                                                                            \
+               "scratch holds " + std::to_string(*(scratch_bytes)) + " bytes, needs " + std::to_string(_need));     \
+    if ((n) == 0) return 0;                                                                                          \
+  } while (0)
+
+// the sides of item i ("image", "box", "file") of a batch
+inline int check_sides(const char* item, int i, int h, int w) {
+  SE_REQUIRE(h >= 1 && w >= 1 && h <= kMaxDim && w <= kMaxDim, std::string(item) + " " + std::to_string(i) + ": sizes must be in [1, 65535]");
+  return 0;
+}
+
+// window i of the encoders and the resize: its sides, its output offset and a source pitch of at least its row of `row` bytes
+inline int check_window(int i, int h, int w, long long pitch, long long row, long long out_off) {
+  if (int rc = check_sides("image", i, h, w)) return rc;
+  SE_REQUIRE(out_off >= 0, "negative offset");
+  SE_REQUIRE(pitch >= row, "image " + std::to_string(i) + ": the source pitch of " + std::to_string(pitch) +
+                               " bytes is narrower than its row of " + std::to_string(row) + " bytes");
+  return 0;
+}
+
+#ifdef __CUDACC__
+// The image of a batch that unit g (a tile, block or chunk of the launch) belongs to: images hold consecutive units from
+// their member `first` on, so it is the last image whose first unit is at or before g.
+template <typename D, typename T>
+__device__ __forceinline__ int image_of(const D* im, int n, T D::*first, T g) {
+  int i = 0;
+  while (i + 1 < n && g >= im[i + 1].*first) ++i;
+  return i;
+}
+#endif
+
+// ------------------------------------------------------------------------------------------
 // tile geometry shared by every convolution kernel: one CTA tile = 8 x 16 output positions
 constexpr int TILE_H = 8;
 constexpr int TILE_W = 16;

@@ -28,7 +28,6 @@
 namespace se {
 
 constexpr float kDetailScaleP = 16384.0f;   // P <= 1 stored times 2^14 (fp16 range); the GEMM's scale undoes it exactly
-constexpr int kDetailMaxDim = 65535;
 
 struct DetailBox {
   int bh, bw, Hn, Wn, hs, ws, L;
@@ -49,11 +48,10 @@ static DetailBox detail_box(int bh, int bw, int Hn, int Wn) {
   return d;
 }
 
-static size_t r256(size_t n) { return (n + 255) / 256 * 256; }
 // scratch of one box: the P operand, the residual operand, the GEMM's output
-static size_t detail_a_bytes(const DetailBox& d) { return r256((size_t)2 * d.Mp * d.Mp * 2); }
-static size_t detail_b_bytes(const DetailBox& d) { return r256((size_t)2 * d.Np * d.Mp * 2); }
-static size_t detail_scratch(const DetailBox& d) { return detail_a_bytes(d) + detail_b_bytes(d) + r256((size_t)d.Mp * d.Np * 4); }
+static size_t detail_a_bytes(const DetailBox& d) { return scratch_round((size_t)2 * d.Mp * d.Mp * 2); }
+static size_t detail_b_bytes(const DetailBox& d) { return scratch_round((size_t)2 * d.Np * d.Mp * 2); }
+static size_t detail_scratch(const DetailBox& d) { return detail_a_bytes(d) + detail_b_bytes(d) + scratch_round((size_t)d.Mp * d.Np * 4); }
 
 __device__ __forceinline__ int work_of(int x, int b, int n) { return (int)(((2LL * x + 1) * n) / (2LL * b)); }
 // min { x >= 0 : work_of(x, b, n) >= 8 p }: (2x + 1) n >= 16 p b
@@ -148,7 +146,7 @@ __global__ void detail_fold_kernel(const float* __restrict__ C, const unsigned c
 
 int detail_hole_u8(const float* mbin, unsigned char* hole, long long n, cudaStream_t stream) {
   if (n <= 0) return 0;
-  detail_hole_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(mbin, hole, n);
+  detail_hole_kernel<<<grid_of(n, 256), 256, 0, stream>>>(mbin, hole, n);
   SE_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -160,18 +158,18 @@ static int detail_one(const unsigned char* photo, long long pitch, const unsigne
   float* C = (float*)((char*)Rp + detail_b_bytes(d));
   {
     const long long n = (long long)d.Mp / 8 * d.Mp;
-    detail_pack_p_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(attn, (uint4*)A, d.L, d.Mp);
+    detail_pack_p_kernel<<<grid_of(n, 256), 256, 0, st>>>(attn, (uint4*)A, d.L, d.Mp);
     SE_CUDA_OK(cudaGetLastError());
   }
   {
     const long long n = (long long)d.Np / 8 * d.Mp;
-    detail_pack_r_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(photo, pitch, low, hole, d, (uint4*)Rp);
+    detail_pack_r_kernel<<<grid_of(n, 256), 256, 0, st>>>(photo, pitch, low, hole, d, (uint4*)Rp);
     SE_CUDA_OK(cudaGetLastError());
   }
   int rc = gemm_split_mn(A, Rp, C, d.Mp, d.Mp, d.Np, 1.0f / kDetailScaleP, st);
   if (rc) return rc;
   const long long n = (long long)d.bh * d.bw;
-  detail_fold_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(C, hole, d, D, agg);
+  detail_fold_kernel<<<grid_of(n, 256), 256, 0, st>>>(C, hole, d, D, agg);
   SE_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -194,7 +192,7 @@ int se_detail_u8(const unsigned char* const* photo, const long long* photo_pitch
   size_t need = 0;
   for (int i = 0; i < n; ++i) {
     const int bh = box_hw[2 * i], bw = box_hw[2 * i + 1];
-    SE_REQUIRE(bh >= 1 && bw >= 1 && bh <= kDetailMaxDim && bw <= kDetailMaxDim, "box " + std::to_string(i) + ": sizes must be in [1, 65535]");
+    if (int rc = check_sides("box", i, bh, bw)) return rc;
     SE_REQUIRE(photo_pitch[i] >= 3LL * bw, "box " + std::to_string(i) + ": the photo pitch is narrower than the box's row");
     // every patch position needs a box-pixel anchor: u(bw - 1) >= Wn - 16 (bw >= Wn / 32), likewise rows
     SE_REQUIRE((2LL * bw - 1) * Wn / (2LL * bw) >= Wn - 16 && (2LL * bh - 1) * Hn / (2LL * bh) >= Hn - 16,
@@ -205,13 +203,8 @@ int se_detail_u8(const unsigned char* const* photo, const long long* photo_pitch
                "box " + std::to_string(i) + ": offsets must be >= 0 and aligned to their element size");
     need = std::max(need, detail_scratch(detail_box(bh, bw, Hn, Wn)));
   }
-  if (!scratch) {
-    *scratch_bytes = (long long)need;
-    return 0;
-  }
-  SE_REQUIRE((size_t)*scratch_bytes >= need, "scratch holds " + std::to_string(*scratch_bytes) + " bytes, needs " + std::to_string(need));
   SE_REQUIRE(((uintptr_t)scratch & 255) == 0, "scratch must be 256 B aligned");
-  if (n == 0) return 0;
+  SE_SCRATCH(scratch, scratch_bytes, need, n);
   SE_REQUIRE(photo && low && hole && attn && D, "null photo / low / hole / attn / D");
   for (int i = 0; i < n; ++i) {   // in order on one stream: every box reuses the scratch
     SE_REQUIRE(photo[i] != nullptr, "null photo window");

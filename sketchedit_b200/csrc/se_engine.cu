@@ -1466,7 +1466,7 @@ static int keyed_forward(se_model* m, int prec, int B, int H, int W, void* strea
 extern "C" {
 
 const char* se_last_error(void) { return se::last_error(); }
-int se_abi_version(void) { return 2; }
+int se_abi_version(void) { return 3; }
 
 int se_model_create(se_model** out) {
   SE_REQUIRE(out != nullptr, "out");

@@ -213,12 +213,6 @@ struct JpegScratch {   // the call's scratch arrays
   unsigned long long* sums;    // scan tile sums
 };
 
-__device__ __forceinline__ int find_img(const JpegList& L, long long g, bool by_chunk) {
-  int i = 0;
-  while (i + 1 < L.n && g >= (by_chunk ? L.im[i + 1].chunk0 : L.im[i + 1].blk0)) ++i;
-  return i;
-}
-
 // Block e of an image in scan order: its component (0 Y, 1 Cb, 2 Cr) and block column / row in that component's plane.
 // A 4:2:0 MCU holds luma blocks (0,0), (0,1), (1,0), (1,1), then Cb and Cr; a 4:4:4 MCU holds Y, Cb, Cr.
 struct BlockAt {
@@ -306,7 +300,7 @@ __global__ void __launch_bounds__(kThreads) jpeg_dct_kernel(const __grid_constan
   stage_huff(sh_ac, 2, 2);
   const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
   if (g >= L.blocks) return;
-  const JImg& d = L.im[find_img(L, g, false)];
+  const JImg& d = L.im[image_of(L.im, L.n, &JImg::blk0, g)];
   const BlockAt b = block_at(d, L.sub, g - d.blk0);
   if (b.dummy) return;   // its DC and bits come from the block before it (jpeg_bits_kernel, jpeg_pack_kernel)
   int v[64];
@@ -382,7 +376,7 @@ __device__ __forceinline__ long long prev_same_comp(int sub, long long e) {   //
 __global__ void __launch_bounds__(kThreads) jpeg_bits_kernel(const __grid_constant__ JpegList L, JpegScratch S) {
   const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
   if (g >= L.blocks) return;
-  const JImg& d = L.im[find_img(L, g, false)];
+  const JImg& d = L.im[image_of(L.im, L.n, &JImg::blk0, g)];
   const long long e = g - d.blk0;
   const BlockAt b = block_at(d, L.sub, e);
   const HuffCodes& dch = c_huff[b.comp ? 1 : 0];
@@ -419,7 +413,7 @@ __global__ void __launch_bounds__(kThreads) jpeg_pack_kernel(const __grid_consta
   stage_huff(sh, 0, 4);
   const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
   if (g >= L.blocks) return;
-  const JImg& d = L.im[find_img(L, g, false)];
+  const JImg& d = L.im[image_of(L.im, L.n, &JImg::blk0, g)];
   const BlockAt b = block_at(d, L.sub, g - d.blk0);
   const unsigned long long at = S.bitoff[g] - S.bitoff[d.blk0];
   unsigned* w = S.words + d.word0;
@@ -465,7 +459,7 @@ template <bool WRITE>
 __global__ void __launch_bounds__(kThreads) jpeg_stuff_kernel(const __grid_constant__ JpegList L, JpegScratch S) {
   const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
   if (g >= L.chunks) return;
-  const int i = find_img(L, g, true);
+  const int i = image_of(L.im, L.n, &JImg::chunk0, g);
   const JImg& d = L.im[i];
   const unsigned long long nbits = image_bits(d, i + 1 < L.n ? &L.im[i + 1] : nullptr, L, S);
   const long long nbytes = (long long)((nbits + 7) >> 3);
@@ -511,10 +505,6 @@ __global__ void __launch_bounds__(kThreads) jpeg_header_kernel(const __grid_cons
 }
 
 // ------------------------------------------------------------------------------------------ host
-constexpr int kMaxDim = 65535;
-constexpr size_t kScratchAlign = 256;
-static size_t scratch_round(size_t bytes) { return (bytes + kScratchAlign - 1) / kScratchAlign * kScratchAlign; }
-
 struct JpegLayout {   // the call's block, word and chunk counts and where its arrays lie in scratch
   long long blocks = 0, words = 0, chunks = 0;
   size_t coef, bits, dcdiff, bitoff, words_at, ffcnt, ffoff, sums, total;
@@ -553,8 +543,6 @@ static JpegLayout jpeg_layout(const int* hw, int n, int sub) {
   return l;
 }
 
-static unsigned grid_of(long long threads, int per_block) { return (unsigned)((threads + per_block - 1) / per_block); }
-
 }  // namespace se
 
 using namespace se;
@@ -577,21 +565,10 @@ int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitc
   SE_REQUIRE(subsampling == 0 || subsampling == 2, "subsampling must be 0 (4:4:4) or 2 (4:2:0)");
   SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
   SE_REQUIRE(n == 0 || (src_pitch && hw && out_off), "null size / offset array");
-  for (int i = 0; i < n; ++i) {
-    const int h = hw[2 * i], w = hw[2 * i + 1];
-    SE_REQUIRE(h >= 1 && w >= 1 && h <= kMaxDim && w <= kMaxDim, "image " + std::to_string(i) + ": sizes must be in [1, 65535]");
-    SE_REQUIRE(out_off[i] >= 0, "negative offset");
-    SE_REQUIRE(src_pitch[i] >= 3LL * w, "image " + std::to_string(i) + ": the source pitch of " + std::to_string(src_pitch[i]) +
-                                            " bytes is narrower than its row of " + std::to_string(3LL * w) + " bytes");
-  }
+  for (int i = 0; i < n; ++i)
+    if (int rc = check_window(i, hw[2 * i], hw[2 * i + 1], src_pitch[i], 3LL * hw[2 * i + 1], out_off[i])) return rc;
   const JpegLayout lay = jpeg_layout(hw, n, subsampling);
-  if (!scratch) {
-    *scratch_bytes = (long long)lay.total;
-    return 0;
-  }
-  SE_REQUIRE((size_t)*scratch_bytes >= lay.total,
-             "scratch holds " + std::to_string(*scratch_bytes) + " bytes, needs " + std::to_string(lay.total));
-  if (n == 0) return 0;
+  SE_SCRATCH(scratch, scratch_bytes, lay.total, n);
   SE_REQUIRE(src && out && out_bytes_dev, "null src / out / out_bytes");
   for (int i = 0; i < n; ++i) SE_REQUIRE(src[i] != nullptr, "null src");
   SE_REQUIRE(lay.blocks < (1LL << 31) * kThreads && lay.chunks < (1LL << 31) * kThreads, "batch too large for one launch");

@@ -40,7 +40,6 @@ constexpr int kMaxMatch = 258;
 constexpr int kChunk = 8192;        // libpng's zbuffer: stream bytes per IDAT chunk
 constexpr int kHead = 8 + 25;       // signature and IHDR
 constexpr int kLCodes = 286, kDCodes = 30, kBLCodes = 19, kHeapSize = 2 * kLCodes + 1, kEndBlock = 256;
-constexpr int kMaxDim = 65535;
 constexpr int kChunkWarps = 4;
 
 // ------------------------------------------------------------------------------------------ tables (trees.c, CRC-32)
@@ -146,22 +145,6 @@ struct PngScratch {
   unsigned* words;
   unsigned long long* sums;
 };
-
-__device__ __forceinline__ int img_of_tile(const PngList& L, long long g) {
-  int i = 0;
-  while (i + 1 < L.n && g >= L.im[i + 1].tile0) ++i;
-  return i;
-}
-__device__ __forceinline__ int img_of_blk(const PngList& L, long long g) {
-  int i = 0;
-  while (i + 1 < L.n && g >= L.im[i + 1].blk0) ++i;
-  return i;
-}
-__device__ __forceinline__ int img_of_chunk(const PngList& L, long long g) {
-  int i = 0;
-  while (i + 1 < L.n && g >= L.im[i + 1].chunk0) ++i;
-  return i;
-}
 
 // ------------------------------------------------------------------------------------------ filtered bytes
 // The thread's kTileV filtered bytes from image position j0 (fewer at the image's end), and the byte before j0 (-1 at 0).
@@ -289,7 +272,7 @@ __device__ __forceinline__ T block_sum(T v) {
 // per tile: its first and last run start (call coordinates) and its Adler-32 sums
 __global__ void __launch_bounds__(kTileT) png_runs_kernel(const __grid_constant__ PngList L, PngScratch S) {
   const long long tile = blockIdx.x;
-  const PImg& d = L.im[img_of_tile(L, tile)];
+  const PImg& d = L.im[image_of(L.im, L.n, &PImg::tile0, tile)];
   __shared__ long long lo[kTileT], hi[kTileT];
   ThreadRuns R;
   thread_runs(L, d, tile, nullptr, R);
@@ -376,7 +359,7 @@ __device__ __forceinline__ void put_byte(unsigned* w, unsigned long long byte_po
 template <int MODE>
 __global__ void __launch_bounds__(kTileT) png_sym_kernel(const __grid_constant__ PngList L, PngScratch S) {
   const long long tile = blockIdx.x;
-  const PImg& d = L.im[img_of_tile(L, tile)];
+  const PImg& d = L.im[image_of(L.im, L.n, &PImg::tile0, tile)];
   ThreadRuns R;
   thread_runs(L, d, tile, &S, R);
   if (MODE == kCount) {
@@ -617,7 +600,7 @@ __device__ __forceinline__ long long image_syms(const PImg& d, const PngScratch&
 __global__ void __launch_bounds__(1) png_tree_kernel(const __grid_constant__ PngList L, PngScratch S) {
   __shared__ TreeWork W;   // about 6.4 KB: in shared memory rather than on a per-thread stack
   const long long g = blockIdx.x;
-  const PImg& d = L.im[img_of_blk(L, g)];
+  const PImg& d = L.im[image_of(L.im, L.n, &PImg::blk0, g)];
   const long long nsym = image_syms(d, S), nblocks = nsym / kBlockSyms + 1, b = g - d.blk0;
   if (b >= nblocks) return;
   PBlk& B = S.blk[g];
@@ -718,7 +701,7 @@ __global__ void __launch_bounds__(32) png_place_kernel(const __grid_constant__ P
 __global__ void __launch_bounds__(32) png_header_kernel(const __grid_constant__ PngList L, PngScratch S) {
   const long long g = (long long)blockIdx.x * 32 + threadIdx.x;
   if (g >= L.blocks) return;
-  const int i = img_of_blk(L, g);
+  const int i = image_of(L.im, L.n, &PImg::blk0, g);
   const PImg& d = L.im[i];
   if (g - d.blk0 >= S.st[i].nblocks) return;
   const PBlk& B = S.blk[g];
@@ -777,7 +760,7 @@ __global__ void __launch_bounds__(32 * kChunkWarps) png_file_kernel(const __grid
   __syncthreads();
   const long long g = (long long)blockIdx.x * kChunkWarps + (threadIdx.x >> 5);
   if (g >= L.chunks) return;
-  const int i = img_of_chunk(L, g), lane = threadIdx.x & 31;
+  const int i = image_of(L.im, L.n, &PImg::chunk0, g), lane = threadIdx.x & 31;
   const PImg& d = L.im[i];
   const PState st = S.st[i];
   const long long c = g - d.chunk0, nch = (st.zlen + kChunk - 1) / kChunk;
@@ -834,9 +817,6 @@ __global__ void __launch_bounds__(32 * kChunkWarps) png_file_kernel(const __grid
 }
 
 // ------------------------------------------------------------------------------------------ host
-constexpr size_t kScratchAlign = 256;
-static size_t scratch_round(size_t bytes) { return (bytes + kScratchAlign - 1) / kScratchAlign * kScratchAlign; }
-
 static long long filtered_bytes(int h, int w, int c) { return (long long)h * (1 + (long long)w * c); }
 static long long deflate_max(long long n) { return n + 8 * (n / kBlockSyms + 2) + 8; }
 static long long max_blocks(long long n) { return n / kBlockSyms + 1; }
@@ -905,8 +885,6 @@ static PngLayout png_layout(const int* hw, int n, int c) {
   return l;
 }
 
-static unsigned grid_of(long long threads, int per_block) { return (unsigned)((threads + per_block - 1) / per_block); }
-
 }  // namespace se
 
 using namespace se;
@@ -929,22 +907,10 @@ int se_png_encode_u8(const unsigned char* const* src, const long long* src_pitch
   SE_REQUIRE(swap_rb == 0 || swap_rb == 1, "swap_rb must be 0 or 1");
   SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
   SE_REQUIRE(n == 0 || (src_pitch && hw && out_off), "null size / offset array");
-  for (int i = 0; i < n; ++i) {
-    const int h = hw[2 * i], w = hw[2 * i + 1];
-    SE_REQUIRE(h >= 1 && w >= 1 && h <= kMaxDim && w <= kMaxDim, "image " + std::to_string(i) + ": sizes must be in [1, 65535]");
-    SE_REQUIRE(out_off[i] >= 0, "negative offset");
-    SE_REQUIRE(src_pitch[i] >= (long long)channels * w, "image " + std::to_string(i) + ": the source pitch of " +
-                                                            std::to_string(src_pitch[i]) + " bytes is narrower than its row of " +
-                                                            std::to_string((long long)channels * w) + " bytes");
-  }
+  for (int i = 0; i < n; ++i)
+    if (int rc = check_window(i, hw[2 * i], hw[2 * i + 1], src_pitch[i], (long long)channels * hw[2 * i + 1], out_off[i])) return rc;
   const PngLayout lay = png_layout(hw, n, channels);
-  if (!scratch) {
-    *scratch_bytes = (long long)lay.total;
-    return 0;
-  }
-  SE_REQUIRE((size_t)*scratch_bytes >= lay.total,
-             "scratch holds " + std::to_string(*scratch_bytes) + " bytes, needs " + std::to_string(lay.total));
-  if (n == 0) return 0;
+  SE_SCRATCH(scratch, scratch_bytes, lay.total, n);
   SE_REQUIRE(src && out && out_bytes_dev, "null src / out / out_bytes");
   for (int i = 0; i < n; ++i) SE_REQUIRE(src[i] != nullptr, "null src");
   SE_REQUIRE(lay.tiles < (1LL << 31) && lay.chunks < (1LL << 31) * kChunkWarps, "batch too large for one launch");

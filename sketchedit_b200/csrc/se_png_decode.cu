@@ -21,7 +21,6 @@
 namespace se {
 
 constexpr int PNG_DECODE_MAX_BATCH = 256;   // files per call: their descriptors travel as kernel parameters
-constexpr int kDecMaxDim = 65535;
 
 struct PDec {
   long long src_off, src_len, plte_off, raw_off;
@@ -171,7 +170,7 @@ int se_png_decode_u8(const unsigned char* src, const long long* src_off, const l
     const int* f = info + 6 * i;
     const int h = f[0], w = f[1], depth = f[2], ctype = f[3], npal = f[4], mode = f[5];
     const std::string at = "file " + std::to_string(i) + ": ";
-    SE_REQUIRE(h >= 1 && w >= 1 && h <= kDecMaxDim && w <= kDecMaxDim, at + "sizes must be in [1, 65535]");
+    if (int rc = check_sides("file", i, h, w)) return rc;
     const bool ok = (ctype == 0 && (depth == 1 || depth == 2 || depth == 4 || depth == 8)) ||
                     (ctype == 3 && (depth == 1 || depth == 2 || depth == 4 || depth == 8)) ||
                     ((ctype == 2 || ctype == 4 || ctype == 6) && depth == 8);
@@ -182,12 +181,7 @@ int se_png_decode_u8(const unsigned char* src, const long long* src_off, const l
     SE_REQUIRE(src_off[i] >= 0 && src_len[i] >= 0, at + "negative offset or length");
     need += (raw_bytes(h, w, depth, ctype) + 15) / 16 * 16;
   }
-  if (!scratch) {
-    *scratch_bytes = need;
-    return 0;
-  }
-  SE_REQUIRE(*scratch_bytes >= need, "scratch holds " + std::to_string(*scratch_bytes) + " bytes, needs " + std::to_string(need));
-  if (n == 0) return 0;
+  SE_SCRATCH(scratch, scratch_bytes, need, n);
   SE_REQUIRE(src && out && status_dev, "null src / out / status");
   for (int i = 0; i < n; ++i) SE_REQUIRE(out[i] != nullptr, "null out");
   PDecList L;

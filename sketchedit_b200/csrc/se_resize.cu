@@ -8,7 +8,7 @@
 // built here on the host in the same order, so the integer weights and therefore every output byte are Pillow's.
 // Pillow computes only the intermediate rows the vertical pass reads; computing all of them gives the same values.
 // se_resize_window_u8 resizes windows of larger images (rows a pitch apart, such as boxes of a photo kept on the device):
-// Image.crop(box).resize(size) without the crop. se_resize_composite_feather_u8 resizes results and their masks the same way
+// Image.crop(box).resize(size) without the crop. se_resize_composite_feather_detail_u8 resizes results and their masks the same way
 // and pastes boxes that may overlap into shared canvases in order, as sequential Image.paste(im, box, mask) calls do, with
 // the blend fused into the vertical pass (paste_v_kernel); it fades each box's mask to 0 along the box edges it is given
 // widths for. se_feather_u8 applies that fade to masks alone (feather_kernel).
@@ -148,7 +148,7 @@ static int axis_table(int dev, int in, int out, const AxisTable** t) {
 
 // ------------------------------------------------------------------------------------------ kernels
 // Per-image descriptors travel as kernel parameters (RESIZE_MAX_BATCH of them, < 4 KB). A launch covers the tiles of all its
-// images; tile0 is the first tile of an image, so a block finds its image by scanning the (at most 32) descriptors.
+// images; tile0 is the first tile of an image, so a block finds its image by scanning the (at most 32) descriptors (image_of).
 struct HPass {   // rows x in_w -> rows x out_w; source rows src_pitch bytes apart, destination rows packed
   const unsigned char* src;
   unsigned char* dst;
@@ -181,17 +181,10 @@ __device__ __forceinline__ int clip8(int acc) {
   return v < 0 ? 0 : (v > 255 ? 255 : v);
 }
 
-template <typename List>
-__device__ __forceinline__ int find_image(const List& L) {
-  int i = 0;
-  while (i + 1 < L.n && (int)blockIdx.x >= L.p[i + 1].tile0) ++i;
-  return i;
-}
-
 template <int C>
 __global__ void __launch_bounds__(H_TX * H_TY) resize_h_kernel(const __grid_constant__ PassList<HPass> L) {
   extern __shared__ int smem[];   // coeffs [H_TX][ksize], bounds [H_TX][2]
-  const HPass& d = L.p[find_image(L)];
+  const HPass& d = L.p[image_of(L.p, L.n, &HPass::tile0, (int)blockIdx.x)];
   const int t = blockIdx.x - d.tile0;
   const int x0 = (t % d.tiles_x) * H_TX, y = (t / d.tiles_x) * H_TY + threadIdx.y;
   const int ncol = min(H_TX, d.out_w - x0);
@@ -286,7 +279,7 @@ __device__ __forceinline__ void store12(unsigned char* o, const int (&v)[V_GROUP
 
 __global__ void __launch_bounds__(V_TX * V_TY) resize_v_kernel(const __grid_constant__ PassList<VPass> L) {
   extern __shared__ int smem[];   // coeffs [V_TY][ksize], bounds [V_TY][2]
-  const VPass& d = L.p[find_image(L)];
+  const VPass& d = L.p[image_of(L.p, L.n, &VPass::tile0, (int)blockIdx.x)];
   const int t = blockIdx.x - d.tile0;
   const int g = (t % d.tiles_x) * V_TX + threadIdx.x, y0 = (t / d.tiles_x) * V_TY;
   const int nrow = min(V_TY, d.out_h - y0);
@@ -321,7 +314,7 @@ __device__ __forceinline__ int div255(int a) {
   return ((t >> 8) + t) >> 8;
 }
 
-// The paste of se_resize_composite_feather_u8: boxes pasted in order into canvases (row pitch in bytes). For a box, the
+// The paste of se_resize_composite_feather_detail_u8: boxes pasted in order into canvases (row pitch in bytes). For a box, the
 // vertical pass of its result (3 channels) and of its mask, both in_h x out_w, to out_h, then Pillow's Image.paste blend of
 // the result over the canvas with that mask, per channel:
 //     dst = DIV255(base * (255 - m) + res * m),   DIV255(a) = ((t >> 8) + t) >> 8 with t = a + 128 (libImaging/Paste.c).
@@ -337,7 +330,7 @@ struct PBox {   // a box at (oy, ox) of its canvas; rgb and mask are in_h x out_
   const int* bounds;   // the vertical table; nullptr: the height does not change (one tap of weight 1 at the same row)
   const int* coeffs;
   int oy, ox;
-  unsigned short out_h, out_w, ksize, vec;   // sizes <= 65535 (check_image); ksize <= 9685 (its shared-memory check)
+  unsigned short out_h, out_w, ksize, vec;   // sizes <= 65535 (check_resize); ksize <= 9685 (its shared-memory check)
   unsigned short feather[4];                 // ramp widths of the left, top, right, bottom sides; all 0: no ramp
 };
 static_assert(sizeof(PBox) == 56, "the feather widths fit PBox's former padding");
@@ -372,7 +365,7 @@ __device__ __forceinline__ void box_span(const PBox& b, int y, int x, int& lo, i
 // (one test per box and thread; a box without one runs the plain paste).
 __global__ void __launch_bounds__(V_TX * V_TY) paste_v_kernel(const __grid_constant__ PasteList L, int swap,
                                                               const __grid_constant__ PasteDetail D) {
-  const PCanvas& d = L.p[find_image(L)];
+  const PCanvas& d = L.p[image_of(L.p, L.n, &PCanvas::tile0, (int)blockIdx.x)];
   const int t = blockIdx.x - d.tile0;
   const int g = (t % d.tiles_x) * V_TX + threadIdx.x, y = d.y0 + (t / d.tiles_x) * V_TY + threadIdx.y;
   if (g >= d.groups || y >= d.y0 + d.h) return;
@@ -464,9 +457,7 @@ struct FeatherList {
 constexpr int F_TX = 64, F_TY = 4;
 
 __global__ void __launch_bounds__(F_TX * F_TY) feather_kernel(const __grid_constant__ FeatherList L) {
-  int i = 0;
-  while (i + 1 < L.n && (int)blockIdx.x >= L.im[i + 1].tile0) ++i;
-  const FeatherImage& d = L.im[i];
+  const FeatherImage& d = L.im[image_of(L.im, L.n, &FeatherImage::tile0, (int)blockIdx.x)];
   const int t = blockIdx.x - d.tile0;
   const int x = (t % d.tiles_x) * F_TX + threadIdx.x, y = (t / d.tiles_x) * F_TY + threadIdx.y;
   if (x >= d.w || y >= d.h) return;
@@ -476,18 +467,12 @@ __global__ void __launch_bounds__(F_TX * F_TY) feather_kernel(const __grid_const
   *q = (unsigned char)div255(*q * ramp);
 }
 
-static int cdiv_i(long long a, long long b) { return (int)((a + b - 1) / b); }
-
-constexpr int kMaxDim = 65535;
-constexpr size_t kScratchAlign = 256;
 constexpr int kMaxSmem = 227 * 1024;
 
-static size_t scratch_round(size_t bytes) { return (bytes + kScratchAlign - 1) / kScratchAlign * kScratchAlign; }
-
-// the checks of image i that se_resize_window_u8 and se_resize_composite_feather_u8 share
-static int check_image(int i, int ih, int iw, int oh, int ow) {
-  SE_REQUIRE(ih >= 1 && iw >= 1 && oh >= 1 && ow >= 1 && ih <= kMaxDim && iw <= kMaxDim && oh <= kMaxDim && ow <= kMaxDim,
-             "image " + std::to_string(i) + ": sizes must be in [1, 65535]");
+// the checks of image i that se_resize_window_u8 and se_resize_composite_feather_detail_u8 share besides its source's: the
+// output's sides, and a filter that fits shared memory
+static int check_resize(int i, int ih, int iw, int oh, int ow) {
+  if (int rc = check_sides("image", i, oh, ow)) return rc;
   SE_REQUIRE(resize_ksize(iw, ow) * (H_TX + 2) * 4 <= kMaxSmem && resize_ksize(ih, oh) * (V_TY + 2) * 4 <= kMaxSmem,
              "image " + std::to_string(i) + ": downscale factor too large");
   return 0;
@@ -511,8 +496,8 @@ static int add_h_pass(int dev, PassList<HPass>& hl, long long& tiles, int& kmax,
   h.out_w = ow;
   h.swap = swap;
   h.tile0 = (int)tiles;
-  h.tiles_x = cdiv_i(ow, H_TX);
-  tiles += (long long)h.tiles_x * cdiv_i(rows, H_TY);
+  h.tiles_x = grid_of(ow, H_TX);
+  tiles += (long long)h.tiles_x * grid_of(rows, H_TY);
   kmax = std::max(kmax, t->ksize);
   return 0;
 }
@@ -551,12 +536,7 @@ static int resize_images(const unsigned char* const* src, const long long* pitch
     mid[i] = need;
     if (src_hw[2 * i + 1] != dst_hw[2 * i + 1] && src_hw[2 * i] != dst_hw[2 * i]) need += scratch_round((size_t)src_hw[2 * i] * dst_hw[2 * i + 1] * C);
   }
-  if (!scratch) {
-    *scratch_bytes = (long long)need;
-    return 0;
-  }
-  SE_REQUIRE((size_t)*scratch_bytes >= need, "scratch holds " + std::to_string(*scratch_bytes) + " bytes, needs " + std::to_string(need));
-  if (n == 0) return 0;
+  SE_SCRATCH(scratch, scratch_bytes, need, n);
   SE_REQUIRE(dst && src && std::find(src, src + n, nullptr) == src + n, "null src / dst");
   std::lock_guard<std::mutex> lk(g_resize_mu);
   int dev = 0;
@@ -598,12 +578,12 @@ static int resize_images(const unsigned char* const* src, const long long* pitch
     v.in_h = ih;
     v.out_h = oh;
     v.row_bytes = ow * C;
-    v.groups = cdiv_i(v.row_bytes, V_GROUP);
+    v.groups = grid_of(v.row_bytes, V_GROUP);
     v.swap = swap_rb;
     v.vec = ((uintptr_t)v.src % 4 == 0) && ((uintptr_t)v.dst % 4 == 0) && v.row_bytes % 4 == 0 && sp % 4 == 0;
     v.tile0 = (int)vtiles;
-    v.tiles_x = cdiv_i(v.groups, V_TX);
-    vtiles += (long long)v.tiles_x * cdiv_i(oh, V_TY);
+    v.tiles_x = grid_of(v.groups, V_TX);
+    vtiles += (long long)v.tiles_x * grid_of(oh, V_TY);
     vk = std::max(vk, v.ksize);
   }
   SE_REQUIRE(htiles < (1LL << 31) && vtiles < (1LL << 31), "batch too large for one launch");
@@ -618,7 +598,7 @@ static int resize_images(const unsigned char* const* src, const long long* pitch
   return 0;
 }
 
-// One box of se_resize_composite_feather_u8: its result and mask (ih x iw), pasted at ow x oh into canvas `canvas` at (oy, ox).
+// One box of se_resize_composite_feather_detail_u8: its result and mask (ih x iw), pasted at ow x oh into canvas `canvas` at (oy, ox).
 struct PasteBox {
   const unsigned char* rgb;
   const unsigned char* mask;
@@ -718,10 +698,10 @@ static int paste_boxes(const std::vector<PasteBox>& boxes, const std::vector<Pas
     for (int i = 0; i < pl.n; ++i) {
       PCanvas& c = pl.p[i];
       c.h -= c.y0;
-      c.groups = cdiv_i(c.groups - c.x0, P_PIX);
+      c.groups = grid_of(c.groups - c.x0, P_PIX);
       c.tile0 = (int)ptiles;
-      c.tiles_x = cdiv_i(c.groups, V_TX);
-      ptiles += (long long)c.tiles_x * cdiv_i(c.h, V_TY);
+      c.tiles_x = grid_of(c.groups, V_TX);
+      ptiles += (long long)c.tiles_x * grid_of(c.h, V_TY);
     }
     SE_REQUIRE(t3 < (1LL << 31) && ptiles < (1LL << 31), "batch too large for one launch");
     int rc = launch_h<3>(h3, t3, k3, st);
@@ -778,12 +758,9 @@ int se_resize_window_u8(const unsigned char* const* src, const long long* src_pi
   SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
   SE_REQUIRE(n == 0 || (src_pitch && src_hw && dst_off && dst_hw), "null size / offset array");
   for (int i = 0; i < n; ++i) {
-    int rc = check_image(i, src_hw[2 * i], src_hw[2 * i + 1], dst_hw[2 * i], dst_hw[2 * i + 1]);
-    if (rc) return rc;
-    SE_REQUIRE(dst_off[i] >= 0, "negative offset");
-    const long long row = (long long)src_hw[2 * i + 1] * channels;
-    SE_REQUIRE(src_pitch[i] >= row, "image " + std::to_string(i) + ": the source pitch of " + std::to_string(src_pitch[i]) +
-                                        " bytes is narrower than its row of " + std::to_string(row) + " bytes");
+    const int ih = src_hw[2 * i], iw = src_hw[2 * i + 1];
+    if (int rc = check_window(i, ih, iw, src_pitch[i], (long long)iw * channels, dst_off[i])) return rc;
+    if (int rc = check_resize(i, ih, iw, dst_hw[2 * i], dst_hw[2 * i + 1])) return rc;
   }
   return resize_images(src, src_pitch, src_hw, dst, dst_off, dst_hw, n, channels, swap_rb, scratch, scratch_bytes,
                        (cudaStream_t)stream);
@@ -805,8 +782,8 @@ int se_resize_composite_feather_detail_u8(const unsigned char* rgb, const long l
   std::vector<PasteBox> boxes(n);
   for (int i = 0; i < n; ++i) {
     const int ih = src_hw[2 * i], iw = src_hw[2 * i + 1], oh = dst_hw[2 * i], ow = dst_hw[2 * i + 1];
-    int rc = check_image(i, ih, iw, oh, ow);
-    if (rc) return rc;
+    if (int rc = check_sides("image", i, ih, iw)) return rc;
+    if (int rc = check_resize(i, ih, iw, oh, ow)) return rc;
     SE_REQUIRE(rgb_off[i] >= 0 && mask_off[i] >= 0 && canvas_off[i] >= 0 && box_yx[2 * i] >= 0 && box_yx[2 * i + 1] >= 0,
                "negative offset");
     SE_REQUIRE(canvas_pitch[i] >= 3LL * (box_yx[2 * i + 1] + ow),
@@ -829,22 +806,9 @@ int se_resize_composite_feather_detail_u8(const unsigned char* rgb, const long l
     mid[i] = need;
     need += paste_scratch(ih, iw, ow);
   }
-  if (!scratch) {
-    *scratch_bytes = (long long)need;
-    return 0;
-  }
-  SE_REQUIRE((size_t)*scratch_bytes >= need, "scratch holds " + std::to_string(*scratch_bytes) + " bytes, needs " + std::to_string(need));
-  if (n == 0) return 0;
+  SE_SCRATCH(scratch, scratch_bytes, need, n);
   SE_REQUIRE(rgb && mask && canvas, "null rgb / mask / canvas");
   return paste_boxes(boxes, canvases, mid, scratch, swap_rb, (cudaStream_t)stream);
-}
-
-int se_resize_composite_feather_u8(const unsigned char* rgb, const long long* rgb_off, const unsigned char* mask,
-                                   const long long* mask_off, const int* src_hw, unsigned char* canvas, const long long* canvas_off,
-                                   const long long* canvas_pitch, const int* box_yx, const int* dst_hw, const int* feather, int n,
-                                   int swap_rb, void* scratch, long long* scratch_bytes, void* stream) {
-  return se_resize_composite_feather_detail_u8(rgb, rgb_off, mask, mask_off, src_hw, canvas, canvas_off, canvas_pitch, box_yx, dst_hw, feather,
-                                               nullptr, nullptr, n, swap_rb, scratch, scratch_bytes, stream);
 }
 
 int se_feather_u8(unsigned char* img, const long long* off, const int* hw, const int* feather, int n, void* stream) {
@@ -853,7 +817,7 @@ int se_feather_u8(unsigned char* img, const long long* off, const int* hw, const
   for (int i = 0; i < n; ++i) {
     const int h = hw[2 * i], w = hw[2 * i + 1];
     const int* f = feather + 4 * (size_t)i;
-    SE_REQUIRE(h >= 1 && w >= 1 && h <= kMaxDim && w <= kMaxDim, "image " + std::to_string(i) + ": sizes must be in [1, 65535]");
+    if (int rc = check_sides("image", i, h, w)) return rc;
     SE_REQUIRE(off[i] >= 0, "negative offset");
     SE_REQUIRE(f[0] >= 0 && f[0] <= w && f[2] >= 0 && f[2] <= w && f[1] >= 0 && f[1] <= h && f[3] >= 0 && f[3] <= h,
                "image " + std::to_string(i) + ": feather widths (" + std::to_string(f[0]) + ", " + std::to_string(f[1]) + ", " +
@@ -883,8 +847,8 @@ int se_feather_u8(unsigned char* img, const long long* off, const int* hw, const
     d.w = hw[2 * i + 1];
     for (int s = 0; s < 4; ++s) d.f[s] = (unsigned short)f[s];
     d.tile0 = (int)tiles;
-    d.tiles_x = cdiv_i(d.w, F_TX);
-    tiles += (long long)d.tiles_x * cdiv_i(d.h, F_TY);
+    d.tiles_x = grid_of(d.w, F_TX);
+    tiles += (long long)d.tiles_x * grid_of(d.h, F_TY);
     if (fl.n == RESIZE_MAX_BATCH) {
       int rc = launch();
       if (rc) return rc;

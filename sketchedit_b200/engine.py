@@ -9,6 +9,7 @@ PyTorch is plumbing here (device memory + current stream); all compute is in lib
 import ctypes
 import numbers
 
+import numpy as np
 import torch
 
 from . import _lib, pngfile
@@ -464,7 +465,7 @@ def resize_window_u8_packed(src, src_offsets, src_pitches, src_sizes, dst_sizes,
 
 def resize_composite_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, canvas, canvas_offsets, canvas_pitches,
                                box_offsets, box_sizes, swap_rb=False, feather=None, detail=None, detail_offsets=None):
-    """Resize back and paste boxes in order into canvases (``se_resize_composite_feather_u8``), bit for bit as sequential
+    """Resize back and paste boxes in order into canvases (``se_resize_composite_feather_detail_u8``), bit for bit as sequential
     Pillow pastes, in place:
 
         for each box i in order:  canvas_i.paste(Image.fromarray(rgb_i).resize((w, h)), (x, y), Image.fromarray(mask_i).resize((w, h)))
@@ -478,8 +479,7 @@ def resize_composite_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, 
     first. ``feather``: None, or per box its ramp widths ``(left, top, right, bottom)`` in box pixels: the box's resized mask
     becomes ``DIV255(m * ramp)`` before the blend, with the ramp of ``serving.feather_ramp``. ``detail``: None, or a contiguous
     CUDA int16 tensor holding at byte ``detail_offsets[i]`` box i's detail plane [h,w,3] (RGB, from ``detail_u8_packed``; an
-    offset < 0: none), added to the resized result with a clamp to [0, 255] before the blend
-    (``se_resize_composite_feather_detail_u8``). Returns ``canvas``. Only enqueues work on the current stream, except that the
+    offset < 0: none), added to the resized result with a clamp to [0, 255] before the blend. Returns ``canvas``. Only enqueues work on the current stream, except that the
     first resize between a pair of lengths uploads its coefficient table."""
     n = len(src_sizes)
     if not (len(rgb_offsets) == len(mask_offsets) == len(canvas_offsets) == len(canvas_pitches) == len(box_offsets)
@@ -516,12 +516,9 @@ def resize_composite_u8_packed(rgb, rgb_offsets, mask, mask_offsets, src_sizes, 
                    [(y + h, x + w) for (y, x), (h, w) in zip(box_offsets, box_sizes)], 3)
     lib = _lib.load()
     a = (_ptr(rgb), _longs(rgb_offsets), _ptr(mask), _longs(mask_offsets), _ints(src_sizes), _ptr(canvas), _longs(canvas_offsets),
-         _longs(canvas_pitches), _ints(box_offsets), _ints(box_sizes), _ints(feather) if feather is not None else None)
-    if detail is None:
-        call = lambda scratch, size, stream: lib.se_resize_composite_feather_u8(*a, n, int(bool(swap_rb)), scratch, size, stream)
-    else:
-        d = (_ptr(detail), _longs(detail_offsets), n, int(bool(swap_rb)))
-        call = lambda scratch, size, stream: lib.se_resize_composite_feather_detail_u8(*a, *d, scratch, size, stream)
+         _longs(canvas_pitches), _ints(box_offsets), _ints(box_sizes), _ints(feather) if feather is not None else None,
+         _ptr(detail), _longs(detail_offsets) if detail is not None else None, n, int(bool(swap_rb)))
+    call = lambda scratch, size, stream: lib.se_resize_composite_feather_detail_u8(*a, scratch, size, stream)
     # one call: the entry keeps the boxes' order across its launches
     _run_chunks(n, max(n, 1), dev, lambda sl: call)
     return canvas
@@ -629,12 +626,17 @@ JPEG_MAX_BATCH = 32      # images per se_jpeg_encode_u8 call; the wrappers split
 JPEG_SUBSAMPLING = (0, 2)   # Pillow's subsampling values the encoder takes: 4:4:4 and 4:2:0
 
 
-def jpeg_max_bytes(h, w, subsampling=2):
-    """A true upper bound of the JPEG file of an h x w image (``se_jpeg_max_bytes``)."""
-    n = int(_lib.load().se_jpeg_max_bytes(int(h), int(w), int(subsampling)))
+def _max_bytes(entry, *args):
+    """The file bound ``entry(*args)`` (se_jpeg_max_bytes, se_png_max_bytes), or ValueError with the library's message."""
+    n = int(entry(*(int(a) for a in args)))
     if n < 0:
         raise ValueError(_lib.load().se_last_error().decode())
     return n
+
+
+def jpeg_max_bytes(h, w, subsampling=2):
+    """A true upper bound of the JPEG file of an h x w image (``se_jpeg_max_bytes``)."""
+    return _max_bytes(_lib.load().se_jpeg_max_bytes, h, w, subsampling)
 
 
 def _is_int(v):
@@ -651,27 +653,28 @@ def _check_jpeg_args(quality, subsampling):
     return int(quality), int(subsampling)
 
 
-def _jpeg_launch(ptrs, pitches, sizes, quality, subsampling, out, out_offsets, out_bytes):
-    """se_jpeg_encode_u8 over windows already checked, JPEG_MAX_BATCH per call, on the current stream of out's device."""
-    lib = _lib.load()
+def _encode(codec, ptrs, pitches, sizes, dev, out=None, out_offsets=None):
+    """The encoder ``codec`` over windows already checked, its batch size per call, on the current stream of ``dev``.
+    ``codec = (entry, per_call, args, max_bytes)``: the C entry's name (se_jpeg_encode_u8, se_png_encode_u8), images per
+    call, its format arguments after n, and the file bound of an h x w window. Returns ``(out, out_offsets, out_bytes)``."""
+    entry, per_call, args, max_bytes = codec
+    entry = getattr(_lib.load(), entry)
+    out, out_offsets = _out(out, out_offsets, [max_bytes(h, w) for h, w in sizes], dev, "out_offsets")
+    out_bytes = torch.empty(len(sizes), device=dev, dtype=torch.int64)
 
     def chunk(sl):
         k = len(ptrs[sl])
-        a = ((ctypes.c_void_p * k)(*ptrs[sl]), _longs(pitches[sl]), _ints(sizes[sl]), k, quality, subsampling, _ptr(out),
-             _longs(out_offsets[sl]), ctypes.c_void_p(out_bytes.data_ptr() + 8 * sl.start))
-        return lambda scratch, size, stream: lib.se_jpeg_encode_u8(*a, scratch, size, stream)
+        a = ((ctypes.c_void_p * k)(*ptrs[sl]), _longs(pitches[sl]), _ints(sizes[sl]), k, *args, _ptr(out), _longs(out_offsets[sl]),
+             ctypes.c_void_p(out_bytes.data_ptr() + 8 * sl.start))
+        return lambda scratch, size, stream: entry(*a, scratch, size, stream)
 
-    _run_chunks(len(sizes), JPEG_MAX_BATCH, out.device, chunk)
+    _run_chunks(len(sizes), per_call, dev, chunk)
+    return out, out_offsets, out_bytes
 
 
-def jpeg_encode_u8_packed(src, src_offsets, src_pitches, sizes, quality=75, subsampling=2, out=None, out_offsets=None):
-    """Baseline JPEG of RGB windows (``se_jpeg_encode_u8``), byte for byte ``Image.save(buf, "JPEG", quality=quality,
-    subsampling=subsampling)`` of each: image i is the ``sizes[i] = (h, w)`` window whose row r starts at byte ``src_offsets[i] +
-    r * src_pitches[i]`` of its source, with ``src_pitches[i] >= 3 w``. ``src`` is one contiguous CUDA uint8 tensor, or a list
-    of them with one per image; windows may overlap. ``out`` (optional, contiguous CUDA uint8) receives file i at
-    ``out_offsets[i]`` and must hold ``jpeg_max_bytes(h, w, subsampling)`` bytes there. Returns ``(out, out_offsets,
-    out_bytes)``: ``out_bytes`` is a CUDA int64 tensor of the files' lengths. Only enqueues work on the current stream."""
-    quality, subsampling = _check_jpeg_args(quality, subsampling)
+def _encode_packed(codec, channels, src, src_offsets, src_pitches, sizes, out, out_offsets):
+    """The body of ``jpeg_encode_u8_packed`` and ``png_encode_u8_packed`` for ``codec`` (``_encode``) on windows of
+    ``channels`` bytes per pixel."""
     n = len(sizes)
     srcs = list(src) if isinstance(src, (list, tuple)) else [src] * n
     if not (len(srcs) == len(src_offsets) == len(src_pitches) == n):
@@ -686,12 +689,42 @@ def jpeg_encode_u8_packed(src, src_offsets, src_pitches, sizes, quality=75, subs
     for i, (h, w) in enumerate(sizes):
         if not (1 <= h <= 65535 and 1 <= w <= 65535):
             raise _lib.SketchEditB200Error("window %d: sizes must be in [1, 65535], got %dx%d" % (i, h, w))
-    _check_windows("window", srcs, src_offsets, src_pitches, sizes, 3)
-    out, out_offsets = _out(out, out_offsets, [jpeg_max_bytes(h, w, subsampling) for h, w in sizes], dev, "out_offsets")
-    out_bytes = torch.empty(n, device=dev, dtype=torch.int64)
-    _jpeg_launch([t.data_ptr() + o for t, o in zip(srcs, src_offsets)], src_pitches, sizes, quality, subsampling, out,
-                 out_offsets, out_bytes)
-    return out, out_offsets, out_bytes
+    _check_windows("window", srcs, src_offsets, src_pitches, sizes, channels)
+    return _encode(codec, [t.data_ptr() + o for t, o in zip(srcs, src_offsets)], src_pitches, sizes, dev, out, out_offsets)
+
+
+def _encode_list(codec, channels, images):
+    """The body of ``jpeg_encode_u8`` and ``png_encode_u8`` for ``codec`` (``_encode``) on a non-empty list of CUDA uint8
+    images of ``channels`` bytes per pixel ([h, w, 3], or [h, w] for 1): their files as ``bytes``."""
+    shape = "[h, w, 3]" if channels == 3 else "[h, w]"
+    for t in images:
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and
+                (t.dim() == 3 and t.shape[2] == 3 if channels == 3 else t.dim() == 2)):
+            raise _lib.SketchEditB200Error("images must be CUDA uint8 %s tensors" % shape)
+        if (channels == 3 and t.stride(2) != 1) or (t.stride(1) != channels and t.shape[1] > 1) or t.stride(0) < channels * t.shape[1]:
+            raise _lib.SketchEditB200Error("an image's pixels must be packed along its rows (got strides %r)" % (t.stride(),))
+        if not (1 <= t.shape[0] <= 65535 and 1 <= t.shape[1] <= 65535):
+            raise _lib.SketchEditB200Error("image sizes must be in [1, 65535], got %dx%d" % tuple(t.shape[:2]))
+    dev = _device(*[(t, "image") for t in images])
+    out, offs, out_bytes = _encode(codec, [t.data_ptr() for t in images], [t.stride(0) for t in images],
+                                   [(int(t.shape[0]), int(t.shape[1])) for t in images], dev)
+    return download_files(out, offs, out_bytes.cpu().tolist())
+
+
+def _jpeg_codec(quality, subsampling):
+    """``_encode``'s codec for JPEG at (quality, subsampling), checked."""
+    quality, subsampling = _check_jpeg_args(quality, subsampling)
+    return "se_jpeg_encode_u8", JPEG_MAX_BATCH, (quality, subsampling), lambda h, w: jpeg_max_bytes(h, w, subsampling)
+
+
+def jpeg_encode_u8_packed(src, src_offsets, src_pitches, sizes, quality=75, subsampling=2, out=None, out_offsets=None):
+    """Baseline JPEG of RGB windows (``se_jpeg_encode_u8``), byte for byte ``Image.save(buf, "JPEG", quality=quality,
+    subsampling=subsampling)`` of each: image i is the ``sizes[i] = (h, w)`` window whose row r starts at byte ``src_offsets[i] +
+    r * src_pitches[i]`` of its source, with ``src_pitches[i] >= 3 w``. ``src`` is one contiguous CUDA uint8 tensor, or a list
+    of them with one per image; windows may overlap. ``out`` (optional, contiguous CUDA uint8) receives file i at
+    ``out_offsets[i]`` and must hold ``jpeg_max_bytes(h, w, subsampling)`` bytes there. Returns ``(out, out_offsets,
+    out_bytes)``: ``out_bytes`` is a CUDA int64 tensor of the files' lengths. Only enqueues work on the current stream."""
+    return _encode_packed(_jpeg_codec(quality, subsampling), 3, src, src_offsets, src_pitches, sizes, out, out_offsets)
 
 
 def jpeg_encode_u8(images, quality=75, subsampling=2):
@@ -705,24 +738,9 @@ def jpeg_encode_u8(images, quality=75, subsampling=2):
     frees them on return. That is about 6.6 + 6.2 MB for a 1000x667 image at 4:2:0 and 104 + 98 MB for 4000x2667 (twice that
     at 4:4:4), some 50 times a typical file; concurrent calls hold their sum. Each call also zeroes the word stream in
     scratch (52 MB at 4000x2667, 4:2:0)."""
-    quality, subsampling = _check_jpeg_args(quality, subsampling)
+    codec = _jpeg_codec(quality, subsampling)
     images = list(images)
-    if not images:
-        return []
-    for t in images:
-        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.dim() == 3 and t.shape[2] == 3):
-            raise _lib.SketchEditB200Error("images must be CUDA uint8 [h, w, 3] tensors")
-        if t.stride(2) != 1 or (t.stride(1) != 3 and t.shape[1] > 1) or t.stride(0) < 3 * t.shape[1]:
-            raise _lib.SketchEditB200Error("an image's pixels must be packed along its rows (strides (>= 3 w, 3, 1), got %r)"
-                                           % (t.stride(),))
-        if not (1 <= t.shape[0] <= 65535 and 1 <= t.shape[1] <= 65535):
-            raise _lib.SketchEditB200Error("image sizes must be in [1, 65535], got %dx%d" % tuple(t.shape[:2]))
-    dev = _device(*[(t, "image") for t in images])
-    sizes = [(int(t.shape[0]), int(t.shape[1])) for t in images]
-    out, offs = _out(None, None, [jpeg_max_bytes(h, w, subsampling) for h, w in sizes], dev, "out_offsets")
-    out_bytes = torch.empty(len(images), device=dev, dtype=torch.int64)
-    _jpeg_launch([t.data_ptr() for t in images], [t.stride(0) for t in images], sizes, quality, subsampling, out, offs, out_bytes)
-    return download_files(out, offs, out_bytes.cpu().tolist())
+    return _encode_list(codec, 3, images) if images else []
 
 
 def download_files(out, offsets, lengths):
@@ -748,23 +766,12 @@ PNG_MAX_BATCH = 32       # images per se_png_encode_u8 call; the wrappers split 
 
 def png_max_bytes(h, w, channels=3):
     """A true upper bound of the PNG file of an h x w image of ``channels`` (1 or 3) bytes per pixel (``se_png_max_bytes``)."""
-    n = int(_lib.load().se_png_max_bytes(int(h), int(w), int(channels)))
-    if n < 0:
-        raise ValueError(_lib.load().se_last_error().decode())
-    return n
+    return _max_bytes(_lib.load().se_png_max_bytes, h, w, channels)
 
 
-def _png_launch(ptrs, pitches, sizes, channels, swap_rb, out, out_offsets, out_bytes):
-    """se_png_encode_u8 over windows already checked, PNG_MAX_BATCH per call, on the current stream of out's device."""
-    lib = _lib.load()
-
-    def chunk(sl):
-        k = len(ptrs[sl])
-        a = ((ctypes.c_void_p * k)(*ptrs[sl]), _longs(pitches[sl]), _ints(sizes[sl]), k, channels, int(bool(swap_rb)), _ptr(out),
-             _longs(out_offsets[sl]), ctypes.c_void_p(out_bytes.data_ptr() + 8 * sl.start))
-        return lambda scratch, size, stream: lib.se_png_encode_u8(*a, scratch, size, stream)
-
-    _run_chunks(len(sizes), PNG_MAX_BATCH, out.device, chunk)
+def _png_codec(channels, swap_rb):
+    """``_encode``'s codec for PNG of ``channels`` bytes per pixel (``swap_rb``: BGR pixels)."""
+    return "se_png_encode_u8", PNG_MAX_BATCH, (channels, int(bool(swap_rb))), lambda h, w: png_max_bytes(h, w, channels)
 
 
 def png_encode_u8_packed(src, src_offsets, src_pitches, sizes, channels, swap_rb=False, out=None, out_offsets=None):
@@ -777,26 +784,7 @@ def png_encode_u8_packed(src, src_offsets, src_pitches, sizes, channels, swap_rb
     tensor of the files' lengths. Only enqueues work on the current stream."""
     if channels not in (1, 3) or isinstance(channels, bool):
         raise ValueError("channels must be 1 or 3, got %r" % (channels,))
-    n = len(sizes)
-    srcs = list(src) if isinstance(src, (list, tuple)) else [src] * n
-    if not (len(srcs) == len(src_offsets) == len(src_pitches) == n):
-        raise _lib.SketchEditB200Error("src (as a list), src_offsets, src_pitches and sizes must have the same length")
-    named = [(t, "src") for t in srcs] + ([(out, "out")] if out is not None else [])
-    _chk_u8(*named)
-    if n == 0:
-        return out, out_offsets, None
-    dev = _device(*named)
-    sizes = _hw(sizes)
-    src_offsets, src_pitches = [int(o) for o in src_offsets], [int(p) for p in src_pitches]
-    for i, (h, w) in enumerate(sizes):
-        if not (1 <= h <= 65535 and 1 <= w <= 65535):
-            raise _lib.SketchEditB200Error("window %d: sizes must be in [1, 65535], got %dx%d" % (i, h, w))
-    _check_windows("window", srcs, src_offsets, src_pitches, sizes, channels)
-    out, out_offsets = _out(out, out_offsets, [png_max_bytes(h, w, channels) for h, w in sizes], dev, "out_offsets")
-    out_bytes = torch.empty(n, device=dev, dtype=torch.int64)
-    _png_launch([t.data_ptr() + o for t, o in zip(srcs, src_offsets)], src_pitches, sizes, channels, swap_rb, out, out_offsets,
-                out_bytes)
-    return out, out_offsets, out_bytes
+    return _encode_packed(_png_codec(channels, swap_rb), channels, src, src_offsets, src_pitches, sizes, out, out_offsets)
 
 
 def png_encode_u8(images, swap_rb=False):
@@ -816,36 +804,16 @@ def png_encode_u8(images, swap_rb=False):
     if len(chans) > 1:
         raise _lib.SketchEditB200Error("images must all be [h, w] or all be [h, w, 3]")
     C = chans.pop()
-    for t in images:
-        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and
-                (t.dim() == 2 if C == 1 else t.dim() == 3 and t.shape[2] == 3)):
-            raise _lib.SketchEditB200Error("images must be CUDA uint8 [h, w, 3] or [h, w] tensors")
-        if (C == 3 and t.stride(2) != 1) or (t.stride(1) != C and t.shape[1] > 1) or t.stride(0) < C * t.shape[1]:
-            raise _lib.SketchEditB200Error("an image's pixels must be packed along its rows (got strides %r)" % (t.stride(),))
-        if not (1 <= t.shape[0] <= 65535 and 1 <= t.shape[1] <= 65535):
-            raise _lib.SketchEditB200Error("image sizes must be in [1, 65535], got %dx%d" % tuple(t.shape[:2]))
-    dev = _device(*[(t, "image") for t in images])
-    sizes = [(int(t.shape[0]), int(t.shape[1])) for t in images]
-    out, offs = _out(None, None, [png_max_bytes(h, w, C) for h, w in sizes], dev, "out_offsets")
-    out_bytes = torch.empty(len(images), device=dev, dtype=torch.int64)
-    _png_launch([t.data_ptr() for t in images], [t.stride(0) for t in images], sizes, C, swap_rb, out, offs, out_bytes)
-    return download_files(out, offs, out_bytes.cpu().tolist())
+    return _encode_list(_png_codec(C, swap_rb), C, images)
 
 
 PNG_DECODE_MAX_BATCH = 256   # files per se_png_decode_u8 call; the wrappers split longer lists into calls of this size
 
 
 def png_stage(heads):
-    """The streams of the ``pngfile.PngHead`` list ``heads``, each followed by its palette, packed into one pinned uint8
-    tensor: ``(staging, offsets, lengths)`` of the streams, the layout ``png_decode_u8_packed`` reads."""
-    parts = [hd.stream + hd.palette for hd in heads]
-    staging = torch.empty(max(1, sum(map(len, parts))), dtype=torch.uint8, pin_memory=True)
-    buf, offsets, at = staging.numpy(), [], 0
-    for part in parts:
-        buf[at:at + len(part)] = memoryview(part).cast("B") if part else ()
-        offsets.append(at)
-        at += len(part)
-    return staging, offsets, [len(hd.stream) for hd in heads]
+    """The streams of the ``pngfile.PngHead`` list ``heads`` packed into one pinned uint8 tensor (``pngfile.stage``, the layout
+    ``png_decode_u8_packed`` reads): ``(staging, offsets, lengths)`` of the streams."""
+    return pngfile.stage(heads, lambda n: torch.empty(n, dtype=torch.uint8, pin_memory=True))
 
 
 def png_decode_u8_packed(src, src_offsets, src_lengths, heads, modes, out=None, out_offsets=None):
@@ -901,6 +869,41 @@ def png_decode_u8_packed(src, src_offsets, src_lengths, heads, modes, out=None, 
     return out, out_offsets, status
 
 
+def png_decode_into(staged, heads, modes, files, dst, names, device):
+    """Pixels of PNG files into place, always Pillow's: file k (``bytes``) is decoded to ``modes[k]`` ("RGB" or "L").
+    ``heads[k]`` is its ``pngfile.PngHead``, or None when the parser sent it to Pillow; ``staged = (staging, offsets,
+    lengths)`` holds the streams of the parsed files in order (``pngfile.stage``'s layout in a host tensor). ``dst[k] =
+    (tensor, byte offset, (h, w))`` is where its pixels go in a CUDA uint8 tensor and the size its header gives, or None for
+    a tensor of its own. The parsed files are decoded on ``device`` straight into place (one upload of the streams), the
+    host waits once for the status words, then Pillow decodes the files the parser or the device refused, each checked
+    against its size (a ``RuntimeError`` naming ``names[k]``) and uploaded. Runs on the current stream; returns
+    ``{k: tensor}`` for the files without a ``dst``."""
+    on_dev = [k for k, hd in enumerate(heads) if hd is not None]
+    bad = [k for k, hd in enumerate(heads) if hd is None]
+    if on_dev:
+        staging, offsets, lengths = staged
+        status = png_decode_u8_packed(staging.to(device, non_blocking=True), offsets, lengths, [heads[k] for k in on_dev],
+                                      [modes[k] for k in on_dev], out=[dst[k][0] for k in on_dev],
+                                      out_offsets=[dst[k][1] for k in on_dev])[2]
+        status_h = torch.empty(len(on_dev), dtype=torch.int32, pin_memory=True)
+        status_h.copy_(status, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        ev.synchronize()
+        bad += [k for k, s in zip(on_dev, status_h.tolist()) if s]
+    own = {}
+    for k in bad:
+        px = np.array(pngfile.pillow_decode(files[k], modes[k]))   # a writable copy for torch
+        if dst[k] is None:
+            own[k] = torch.from_numpy(px).to(device)
+            continue
+        buf, o, hw = dst[k]
+        if px.shape[:2] != tuple(hw):
+            raise RuntimeError("%s decodes to %dx%d, its header says %dx%d" % ((names[k],) + px.shape[:2] + tuple(hw)))
+        buf[o:o + px.size].copy_(torch.from_numpy(px).reshape(-1).pin_memory(), non_blocking=True)
+    return own
+
+
 def png_decode_u8(files, mode="RGB", device=None):
     """Pixels of PNG files (``bytes``) as CUDA uint8 tensors, [h, w, 3] for ``mode`` "RGB" and [h, w] for "L", each equal to
     ``np.asarray(Image.open(f).convert(mode))``, Pillow's exception included. Files ``pngfile.parse`` accepts are decoded on
@@ -917,27 +920,19 @@ def png_decode_u8(files, mode="RGB", device=None):
             heads.append(pngfile.parse(f))
         except pngfile.Host:
             heads.append(None)
-    on_dev = [i for i, hd in enumerate(heads) if hd is not None]
-    res = [None] * len(files)
-    if on_dev:
-        with torch.cuda.device(dev):
-            staging, offs, lens = png_stage([heads[i] for i in on_dev])
-            src = staging.to(dev, non_blocking=True)
-            out, out_offs, status = png_decode_u8_packed(src, offs, lens, [heads[i] for i in on_dev], mode)
-            c = pngfile.MODES[mode]
-            for k, i in enumerate(on_dev):
-                hd = heads[i]
-                if c == 3:
-                    res[i] = out[out_offs[k]:out_offs[k] + hd.h * hd.w * 3].view(hd.h, hd.w, 3)
-                else:
-                    res[i] = out[out_offs[k]:out_offs[k] + hd.h * hd.w].view(hd.h, hd.w)
-            for k, s in enumerate(status.cpu().tolist()):
-                if s:
-                    res[on_dev[k]] = None
-    for i, r in enumerate(res):
-        if r is None:
-            res[i] = torch.from_numpy(pngfile.pillow_decode(files[i], mode).copy()).to(dev)
-    return res
+    parsed = [hd for hd in heads if hd is not None]
+    c = pngfile.MODES[mode]
+    with torch.cuda.device(dev):
+        offs, total = _aligned_offsets([hd.h * hd.w * c for hd in parsed])
+        out = torch.empty(max(total, 1), device=dev, dtype=torch.uint8)
+        at = iter(offs)
+        dst = [None if hd is None else (out, next(at), (hd.h, hd.w)) for hd in heads]
+        res = png_decode_into(png_stage(parsed) if parsed else None, heads, [mode] * len(files), files, dst,
+                              ["file %d" % i for i in range(len(files))], dev)
+    for i, (d, hd) in enumerate(zip(dst, heads)):
+        if d is not None:
+            res[i] = out[d[1]:d[1] + hd.h * hd.w * c].view((hd.h, hd.w, c) if c == 3 else (hd.h, hd.w))
+    return [res[i] for i in range(len(files))]
 
 
 def outputs_to_uint8(composed, mask):

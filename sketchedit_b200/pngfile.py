@@ -103,6 +103,23 @@ def size(data):
     return h, w
 
 
+def stage(heads, alloc):
+    """The device decoder's input for the ``PngHead`` list ``heads``: each file's stream followed by its palette, packed in
+    order, one copy of each into the buffer ``alloc(total)`` returns (total >= 1 bytes; a uint8 numpy array or CPU tensor).
+    Returns ``(buffer, offsets, lengths)`` of the streams."""
+    offsets, at = [], 0
+    for hd in heads:
+        offsets.append(at)
+        at += len(hd.stream) + len(hd.palette)
+    buf = alloc(max(at, 1))
+    view = np.asarray(buf)
+    for hd, o in zip(heads, offsets):
+        n = len(hd.stream)
+        view[o:o + n] = np.frombuffer(hd.stream, np.uint8)
+        view[o + n:o + n + len(hd.palette)] = np.frombuffer(hd.palette, np.uint8)
+    return buf, offsets, [len(hd.stream) for hd in heads]
+
+
 def pillow_decode(data, mode):
     """What the device decoder stands for: np.asarray(Image.open(f).convert(mode)), Pillow's exception included."""
     from PIL import Image

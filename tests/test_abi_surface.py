@@ -32,9 +32,9 @@ def test_library_exports_every_symbol(lib_path):
         assert hasattr(lib, name), name
 
 
-def test_abi_version_and_error_string(lib_path):
+def test_abi_version_3_and_error_string(lib_path):
     lib = _lib.load()
-    assert lib.se_abi_version() == 2
+    assert lib.se_abi_version() == 3
     assert isinstance(lib.se_last_error(), bytes)
 
 

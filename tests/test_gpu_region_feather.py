@@ -1,4 +1,4 @@
-"""Feathered region pastes on the GPU: se_resize_composite_feather_u8 and se_feather_u8 against the numpy statement bit for bit
+"""Feathered region pastes on the GPU: se_resize_composite_feather_detail_u8 and se_feather_u8 against the numpy statement bit for bit
 (with guard bytes), zero widths against NULL widths, and the device flows of DemoProcessor.process_image
 and EditSession.edit with feather > 0 against the Pillow flows."""
 import gc

@@ -1,4 +1,4 @@
-"""Several regions per request on the GPU: se_resize_composite_feather_u8 (engine.resize_composite_u8_packed) reproduces sequential
+"""Several regions per request on the GPU: se_resize_composite_feather_detail_u8 (engine.resize_composite_u8_packed) reproduces sequential
 Pillow pastes bit for bit and writes nothing outside its boxes, and the device flow of DemoProcessor.process_image with
 region="strokes" or a list of boxes returns exactly the Pillow flow's bytes."""
 import threading

@@ -1,6 +1,8 @@
 """tests/util_png.py is cv2's PNG encoder: its files equal ``cv2.imencode(".png", img)`` and ``cv2.imwrite`` over sizes at every
 zlib window step, both channel counts and the contents that reach each of zlib's block forms, plus constructed blocks (an
-empty final block, the 15-bit length repair, static trees, stored data). One test pins the environment the encoder restates."""
+empty final block, the 15-bit length repair, static trees, stored data). One test pins the environment the encoder restates,
+and one that se_png_encode_u8 checks its arguments on the host before anything runs."""
+import ctypes
 import os
 import re
 import zlib
@@ -9,6 +11,7 @@ import cv2
 import numpy as np
 import pytest
 
+from sketchedit_b200 import _lib, build
 from tests import util_png as P
 
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
@@ -187,3 +190,50 @@ def test_max_bytes_bounds_the_files():
         for c in (1, 3):
             a = content("noise", h, w, c, rs)
             assert len(cv2_png(a)) <= P.max_bytes(h, w, c), (h, w, c)
+
+
+@pytest.fixture(scope="module")
+def lib():
+    build.build(verbose=False)
+    return _lib.load()
+
+
+def _call(lib, hw, pitch, n=1, channels=3, swap_rb=0, out_off=0, scratch=None, need=None, src=None, out=None, out_bytes=None):
+    need = need if need is not None else ctypes.c_longlong(0)
+    k = max(n, 1)
+    hw_a = (ctypes.c_int * (2 * k))(*(list(hw) * k))
+    p_a = (ctypes.c_longlong * k)(*([pitch] * k))
+    o_a = (ctypes.c_longlong * k)(*([out_off] * k))
+    rc = lib.se_png_encode_u8(src, p_a, hw_a, n, channels, swap_rb, out, o_a, out_bytes, scratch, ctypes.byref(need), None)
+    return rc, need.value, lib.se_last_error().decode() if rc else ""
+
+
+def test_host_checks_and_scratch_query(lib):
+    rc, need, _ = _call(lib, (10, 10), 30)
+    assert rc == 0 and need > 0
+    rc, need1, _ = _call(lib, (10, 10), 10, channels=1)
+    assert rc == 0 and need1 < need
+    rc, need2, _ = _call(lib, (10, 10), 30, n=2)
+    assert rc == 0 and need2 > need
+    assert _call(lib, (10, 10), 30, n=0)[:2] == (0, 512)          # the per-image state and the scan sums, one slot each
+    for kw, msg in [(dict(channels=2), "channels must be 1 or 3"), (dict(channels=4), "channels must be 1 or 3"),
+                    (dict(swap_rb=2), "swap_rb must be 0 or 1"), (dict(n=33), "n must be in"), (dict(n=-1), "n must be in"),
+                    (dict(out_off=-1), "negative offset")]:
+        rc, _, err = _call(lib, (10, 10), 30, **kw)
+        assert rc != 0 and msg in err, (kw, err)
+    for hw, pitch, channels, msg in [((0, 10), 30, 3, "image 0: sizes must be in [1, 65535]"),
+                                     ((10, 65536), 3 * 65536, 3, "image 0: sizes must be in [1, 65535]"),
+                                     ((10, 10), 29, 3, "image 0: the source pitch of 29 bytes is narrower than its row of 30 bytes"),
+                                     ((10, 10), 9, 1, "image 0: the source pitch of 9 bytes is narrower than its row of 10 bytes")]:
+        rc, _, err = _call(lib, hw, pitch, channels=channels)
+        assert rc != 0 and msg in err, (hw, pitch, channels, err)
+    assert lib.se_png_encode_u8(None, None, None, 1, 3, 0, None, None, None, None, ctypes.byref(ctypes.c_longlong(0)), None) != 0
+    assert "null size / offset array" in lib.se_last_error().decode()
+    # past the query: scratch too small, then null pointers, all refused before anything is enqueued
+    rc, _, err = _call(lib, (10, 10), 30, scratch=ctypes.c_void_p(256), need=ctypes.c_longlong(1))
+    assert rc != 0 and "scratch holds 1 bytes, needs %d" % need in err
+    rc, _, err = _call(lib, (10, 10), 30, scratch=ctypes.c_void_p(256), need=ctypes.c_longlong(need))
+    assert rc != 0 and "null src / out / out_bytes" in err
+    assert _call(lib, (10, 10), 30, n=0, scratch=ctypes.c_void_p(256), need=ctypes.c_longlong(512))[0] == 0
+    assert lib.se_png_max_bytes(0, 5, 3) == -1 and lib.se_png_max_bytes(5, 65536, 1) == -1 and lib.se_png_max_bytes(5, 5, 2) == -1
+    assert lib.se_png_max_bytes(65535, 65535, 3) == P.max_bytes(65535, 65535, 3)

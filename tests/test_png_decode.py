@@ -1,5 +1,7 @@
 """PNG decoding on the host: the numpy restatement (tests/util_png_decode.py) against Pillow, the container parser's routing,
-and the inflate core of se_png_decode.cu built for the host (one lane) against zlib on malformed and mutated streams."""
+the inflate core of se_png_decode.cu built for the host (one lane) against zlib on malformed and mutated streams, and the
+argument checks se_png_decode_u8 makes before anything runs."""
+import ctypes
 import io
 import os
 import random
@@ -12,7 +14,7 @@ import numpy as np
 import pytest
 from PIL import Image
 
-from sketchedit_b200 import pngfile
+from sketchedit_b200 import _lib, build, pngfile
 from tests import util_png_decode as U
 
 CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "sketchedit_b200", "csrc")
@@ -197,3 +199,52 @@ def test_inflate_host_mutated(inflate_host):
             z[k:k] = bytes(rnd.randrange(256) for _ in range(rnd.randint(1, 8)))
         cases.append((bytes(z), n + rnd.choice((0, 0, 0, -1, 1))))
     check(inflate_host, cases)
+
+
+# ------------------------------------------------------------------------------------------------ se_png_decode_u8's host checks
+@pytest.fixture(scope="module")
+def lib():
+    build.build(verbose=False)
+    return _lib.load()
+
+
+def _call(lib, info, n=1, src_off=0, src_len=100, plte_off=0, scratch=None, need=None, src=None, out=None, status=None):
+    need = need if need is not None else ctypes.c_longlong(0)
+    k = max(n, 1)
+    L = ctypes.c_longlong
+    info_a = (ctypes.c_int * (6 * k))(*(list(info) * k))
+    rc = lib.se_png_decode_u8(src, (L * k)(*([src_off] * k)), (L * k)(*([src_len] * k)), info_a, (L * k)(*([plte_off] * k)), n,
+                              out, status, scratch, ctypes.byref(need), None)
+    return rc, need.value, lib.se_last_error().decode() if rc else ""
+
+
+def test_host_checks_and_scratch_query(lib):
+    rgb = (10, 10, 8, 2, 0, 3)                                     # h, w, depth, colour type, palette entries, output channels
+    assert _call(lib, rgb)[:2] == (0, 320)                         # 10 filtered rows of 1 + 30 bytes, rounded up to 16
+    assert _call(lib, rgb, n=3)[:2] == (0, 960)
+    assert _call(lib, (5, 7, 1, 3, 2, 1))[:2] == (0, 5 * (1 + 1) + 6)   # 1-bit palette: 1 byte per row
+    assert _call(lib, rgb, n=0)[:2] == (0, 0)
+    for info, kw, msg in [(rgb, dict(n=257), "n must be in"), (rgb, dict(n=-1), "n must be in"),
+                          ((0, 10, 8, 2, 0, 3), {}, "file 0: sizes must be in [1, 65535]"),
+                          ((10, 65536, 8, 2, 0, 3), {}, "file 0: sizes must be in [1, 65535]"),
+                          ((10, 10, 16, 2, 0, 3), {}, "colour type 2 at depth 16 is not decoded here"),
+                          ((10, 10, 8, 5, 0, 3), {}, "colour type 5 at depth 8 is not decoded here"),
+                          ((10, 10, 8, 3, 0, 3), {}, "a palette of 1 to 256 entries"),
+                          ((10, 10, 8, 3, 257, 3), {}, "a palette of 1 to 256 entries"),
+                          ((10, 10, 8, 3, 4, 3), dict(plte_off=-1), "a palette of 1 to 256 entries"),
+                          ((10, 10, 8, 2, 4, 3), {}, "a palette of 1 to 256 entries"),
+                          ((10, 10, 8, 2, 0, 2), {}, "mode must be 1 (L) or 3 (RGB)"),
+                          (rgb, dict(src_off=-1), "negative offset or length"), (rgb, dict(src_len=-1), "negative offset or length")]:
+        rc, _, err = _call(lib, info, **kw)
+        assert rc != 0 and msg in err, (info, kw, err)
+    assert lib.se_png_decode_u8(None, None, None, None, None, 1, None, None, None, ctypes.byref(ctypes.c_longlong(0)), None) != 0
+    assert "null length / offset / info array" in lib.se_last_error().decode()
+    # past the query: scratch too small, then null pointers, all refused before anything is enqueued
+    rc, _, err = _call(lib, rgb, scratch=ctypes.c_void_p(256), need=ctypes.c_longlong(1))
+    assert rc != 0 and "scratch holds 1 bytes, needs 320" in err
+    rc, _, err = _call(lib, rgb, scratch=ctypes.c_void_p(256), need=ctypes.c_longlong(320))
+    assert rc != 0 and "null src / out / status" in err
+    rc, _, err = _call(lib, rgb, scratch=ctypes.c_void_p(256), need=ctypes.c_longlong(320), src=ctypes.c_void_p(256),
+                       out=(ctypes.c_void_p * 1)(None), status=ctypes.c_void_p(256))
+    assert rc != 0 and "null out" in err
+    assert _call(lib, rgb, n=0, scratch=ctypes.c_void_p(256), need=ctypes.c_longlong(0))[0] == 0

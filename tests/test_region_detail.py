@@ -1,9 +1,12 @@
 """Region-edit detail on the CPU: the geometry of the restatement (tests/util_detail.py), its properties, the argument checks
-of the serving flows, and that detail and plain region requests share batches."""
+of the serving flows and of se_detail_u8, and that detail and plain region requests share batches."""
+import ctypes
+
 import numpy as np
 import pytest
 from PIL import Image
 
+from sketchedit_b200 import _lib, build
 from sketchedit_b200.serving import _check_detail, detail_box_ok
 from tests import util_detail as U
 from tests.test_region_feather import _FakeProcessor, _NoForward, _photo
@@ -174,3 +177,65 @@ def test_no_detail_on_boxes_without_anchors():
         assert [d for _, d in p.keys] == [[True]]
     finally:
         p.batcher.close()
+
+
+# ------------------------------------------------------------------------------------------ se_detail_u8's host checks
+@pytest.fixture(scope="module")
+def lib():
+    build.build(verbose=False)
+    return _lib.load()
+
+
+def _scratch_need(bh, bw, Hn, Wn):
+    """se_detail_u8's scratch for one box: the P operand, the residual operand and the GEMM's output, each rounded to 256 B."""
+    r = lambda v: -(-v // 256) * 256
+    Mp = r((Hn // 8 - 1) * (Wn // 8 - 1))
+    Np = r(U.footprint(bw, Wn) * U.footprint(bh, Hn) * 3)
+    return r(4 * Mp * Mp) + r(4 * Np * Mp) + r(4 * Mp * Np)
+
+
+def _call(lib, hw, pitch, n=1, size=(64, 64), offs=(0, 0, 0, 0), agg=None, agg_off=0, scratch=None, need=None, photo=None):
+    need = need if need is not None else ctypes.c_longlong(0)
+    k = max(n, 1)
+    L = ctypes.c_longlong
+    arr = lambda v: (L * k)(*([v] * k))
+    low_off, hole_off, attn_off, d_off = offs
+    rc = lib.se_detail_u8(photo, arr(pitch), (ctypes.c_int * (2 * k))(*(list(hw) * k)), n, size[0], size[1], None, arr(low_off), None,
+                          arr(hole_off), None, arr(attn_off), None, arr(d_off), agg, arr(agg_off) if agg_off is not None else None,
+                          scratch, ctypes.byref(need), None)
+    return rc, need.value, lib.se_last_error().decode() if rc else ""
+
+
+def test_host_checks_and_scratch_query(lib):
+    assert _call(lib, (64, 64), 192)[:2] == (0, _scratch_need(64, 64, 64, 64))
+    assert _call(lib, (608, 400), 1200, size=(256, 256))[:2] == (0, _scratch_need(608, 400, 256, 256))
+    assert _call(lib, (64, 64), 192, n=3)[:2] == (0, _scratch_need(64, 64, 64, 64))   # the boxes take turns with one scratch
+    assert _call(lib, (64, 64), 192, n=0)[:2] == (0, 0)
+    for hw, pitch, kw, msg in [((64, 64), 192, dict(n=-1), "n must be >= 0"),
+                               ((64, 64), 192, dict(size=(60, 64)), "multiples of 8 and >= 16"),
+                               ((64, 64), 192, dict(size=(8, 64)), "multiples of 8 and >= 16"),
+                               ((64, 64), 192, dict(agg=ctypes.c_void_p(256), agg_off=None), "agg needs agg_off"),
+                               ((0, 64), 192, {}, "box 0: sizes must be in [1, 65535]"),
+                               ((64, 65536), 3 * 65536, {}, "box 0: sizes must be in [1, 65535]"),
+                               ((64, 64), 191, {}, "box 0: the photo pitch is narrower than the box's row"),
+                               ((7, 120), 360, dict(size=(256, 256)), "box 0: 7 x 120 is below 1/32 of the working size"),
+                               ((64, 64), 192, dict(offs=(-1, 0, 0, 0)), "box 0: offsets must be >= 0 and aligned"),
+                               ((64, 64), 192, dict(offs=(0, -1, 0, 0)), "box 0: offsets must be >= 0 and aligned"),
+                               ((64, 64), 192, dict(offs=(0, 0, 2, 0)), "box 0: offsets must be >= 0 and aligned"),
+                               ((64, 64), 192, dict(offs=(0, 0, 0, 1)), "box 0: offsets must be >= 0 and aligned"),
+                               ((64, 64), 192, dict(agg=ctypes.c_void_p(256), agg_off=2), "box 0: offsets must be >= 0 and aligned")]:
+        rc, _, err = _call(lib, hw, pitch, **kw)
+        assert rc != 0 and msg in err, (hw, pitch, kw, err)
+    hw = (ctypes.c_int * 2)(64, 64)
+    assert lib.se_detail_u8(None, None, hw, 1, 64, 64, None, None, None, None, None, None, None, None, None, None, None,
+                            ctypes.byref(ctypes.c_longlong(0)), None) != 0
+    assert "null size / offset array" in lib.se_last_error().decode()
+    # past the query: scratch too small or misaligned, then null pointers, all refused before anything is enqueued
+    need = _scratch_need(64, 64, 64, 64)
+    rc, _, err = _call(lib, (64, 64), 192, scratch=ctypes.c_void_p(256), need=ctypes.c_longlong(1))
+    assert rc != 0 and "scratch holds 1 bytes, needs %d" % need in err
+    rc, _, err = _call(lib, (64, 64), 192, scratch=ctypes.c_void_p(16), need=ctypes.c_longlong(need))
+    assert rc != 0 and "scratch must be 256 B aligned" in err
+    rc, _, err = _call(lib, (64, 64), 192, scratch=ctypes.c_void_p(256), need=ctypes.c_longlong(need))
+    assert rc != 0 and "null photo / low / hole / attn / D" in err
+    assert _call(lib, (64, 64), 192, n=0, scratch=ctypes.c_void_p(256), need=ctypes.c_longlong(0))[0] == 0

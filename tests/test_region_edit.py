@@ -1,6 +1,6 @@
 """Region edits (DemoProcessor.process_image(..., region=...)) on the CPU: the box rule of serving.region_box, the validation
 of region requests, the paste blend against Image.paste on every byte triple, and the host checks of the one-box-per-canvas
-paste of se_resize_composite_feather_u8."""
+paste of se_resize_composite_feather_detail_u8."""
 import ctypes
 
 import numpy as np
@@ -145,19 +145,19 @@ def lib():
 
 
 def _query(lib, src, dst, n=1, scratch=None, scratch_bytes=0, off=0):
-    """se_resize_composite_feather_u8 with n boxes, each filling its own canvas (at (0, 0), pitch 3 w), no feather."""
+    """se_resize_composite_feather_detail_u8 with n boxes, each filling its own canvas (at (0, 0), pitch 3 w), no feather."""
     k = max(n, 1)
     L, I = ctypes.c_longlong, ctypes.c_int
     offs = (L * k)(*([off] * k))
     coff, pitches = (L * k)(*range(off, off + 10 ** 6 * k, 10 ** 6)), (L * k)(*([3 * dst[1]] * k))
     shw, dhw, yx = (I * (2 * k))(*(src * k)), (I * (2 * k))(*(dst * k)), (I * (2 * k))(*([0, 0] * k))
     need = L(scratch_bytes)
-    rc = lib.se_resize_composite_feather_u8(None, offs, None, offs, shw, None, coff, pitches, yx, dhw, None, n, 1, scratch,
-                                            ctypes.byref(need), None)
+    rc = lib.se_resize_composite_feather_detail_u8(None, offs, None, offs, shw, None, coff, pitches, yx, dhw, None, None, None, n, 1,
+                                                   scratch, ctypes.byref(need), None)
     return rc, need.value, lib.se_last_error().decode()
 
 
-def test_paste_scratch_query(lib):
+def test_paste_scratch_query_with_null_detail(lib):
     r256 = lambda b: (b + 255) // 256 * 256
     assert _query(lib, (256, 256), (608, 608))[:2] == (0, r256(256 * 608 * 3) + r256(256 * 608))
     assert _query(lib, (256, 256), (608, 256))[:2] == (0, 0)           # width unchanged: the paste reads the result itself
@@ -167,7 +167,7 @@ def test_paste_scratch_query(lib):
     assert _query(lib, (256, 256), (100, 77), n=0)[:2] == (0, 0)
 
 
-def test_paste_validates_on_the_host_with_the_resize_messages(lib):
+def test_paste_with_null_detail_validates_on_the_host_with_the_resize_messages(lib):
     cases = [
         (dict(src=(256, 256), dst=(64, 64), n=-1), "n must be >= 0 boxes"),
         (dict(src=(0, 256), dst=(64, 64)), "sizes must be in [1, 65535]"),
@@ -187,8 +187,8 @@ def test_paste_validates_on_the_host_with_the_resize_messages(lib):
     assert _query(lib, (0, 256), (64, 64))[2].split(" : ")[-1].split(" at ")[0] == \
         lib.se_last_error().decode().split(" : ")[-1].split(" at ")[0]
     hw = (ctypes.c_int * 2)(64, 64)
-    assert lib.se_resize_composite_feather_u8(None, None, None, None, hw, None, None, None, None, hw, None, 1, 0, None,
-                                              ctypes.byref(need), None) != 0
+    assert lib.se_resize_composite_feather_detail_u8(None, None, None, None, hw, None, None, None, None, hw, None, None, None, 1, 0,
+                                                     None, ctypes.byref(need), None) != 0
     assert "null size / offset array" in lib.se_last_error().decode()
-    assert lib.se_resize_composite_feather_u8(None, None, None, None, None, None, None, None, None, None, None, 0, 0, None, None,
-                                              None) != 0
+    assert lib.se_resize_composite_feather_detail_u8(None, None, None, None, None, None, None, None, None, None, None, None, None, 0,
+                                                     0, None, None, None) != 0

@@ -1,6 +1,6 @@
 """Feathered region pastes on the CPU: the width rule and the ramp of serving.feather_widths / feather_ramp, the host flow of
 DemoProcessor with a fake forward against the Pillow statement, the property that the band never reaches a stroke of an
-'auto' or 'strokes' box, the seam bound, host sessions with feather, and the host checks of se_resize_composite_feather_u8 and
+'auto' or 'strokes' box, the seam bound, host sessions with feather, and the host checks of se_resize_composite_feather_detail_u8 and
 se_feather_u8."""
 import ctypes
 
@@ -347,12 +347,12 @@ def _composite(lib, src, dst, n=1, yx=(0, 0), feather=None, scratch=None, scratc
     shw, dhw, byx = (I * (2 * k))(*(src * k)), (I * (2 * k))(*(dst * k)), (I * (2 * k))(*(yx * k))
     fw = (I * (4 * k))(*(list(feather) * k)) if feather is not None else None
     need = L(scratch_bytes)
-    rc = lib.se_resize_composite_feather_u8(None, offs, None, offs, shw, None, coff, pitches, byx, dhw, fw, n, 1, scratch,
-                                            ctypes.byref(need), None)
+    rc = lib.se_resize_composite_feather_detail_u8(None, offs, None, offs, shw, None, coff, pitches, byx, dhw, fw, None, None, n, 1,
+                                                   scratch, ctypes.byref(need), None)
     return rc, need.value, lib.se_last_error().decode()
 
 
-def test_composite_feather_scratch_query_is_the_composites(lib):
+def test_composite_feather_scratch_query_is_the_composites_with_null_detail(lib):
     for src, dst, n in [((256, 256), (608, 608), 1), ((256, 256), (608, 256), 2), ((256, 256), (100, 77), 3),
                         ((256, 256), (100, 77), 70), ((256, 256), (100, 77), 0)]:
         want = _composite(lib, src, dst, n)                              # feather == NULL
@@ -361,7 +361,7 @@ def test_composite_feather_scratch_query_is_the_composites(lib):
             assert _composite(lib, src, dst, n, feather=f)[:2] == want[:2], (src, dst, n, f)
 
 
-def test_composite_feather_validates_on_the_host(lib):
+def test_composite_feather_with_null_detail_validates_on_the_host(lib):
     for f in [(-1, 0, 0, 0), (0, -1, 0, 0), (0, 0, -3, 0), (0, 0, 0, -1), (78, 0, 0, 0), (0, 101, 0, 0), (0, 0, 78, 0),
               (0, 0, 0, 101)]:
         rc, _, err = _composite(lib, (256, 256), (100, 77), feather=f)
@@ -374,16 +374,16 @@ def test_composite_feather_validates_on_the_host(lib):
     need = ctypes.c_longlong(0)
     hw = (ctypes.c_int * 2)(64, 64)
     fw = (ctypes.c_int * 4)(1, 1, 1, 1)
-    assert lib.se_resize_composite_feather_u8(None, None, None, None, hw, None, None, None, None, hw, fw, 1, 0, None,
-                                              ctypes.byref(need), None) != 0
+    assert lib.se_resize_composite_feather_detail_u8(None, None, None, None, hw, None, None, None, None, hw, fw, None, None, 1, 0,
+                                                     None, ctypes.byref(need), None) != 0
     assert "null size / offset array" in lib.se_last_error().decode()
     rc, need_b, _ = _composite(lib, (256, 256), (64, 64), feather=(1, 1, 1, 1))
     assert rc == 0
     scratch = ctypes.c_longlong(max(need_b, 1))
     offs = (ctypes.c_longlong * 1)(0)
-    assert lib.se_resize_composite_feather_u8(None, offs, None, offs, (ctypes.c_int * 2)(256, 256), None, offs,
-                                              (ctypes.c_longlong * 1)(192), (ctypes.c_int * 2)(0, 0), hw, fw, 1, 0, 1,
-                                              ctypes.byref(scratch), None) != 0
+    assert lib.se_resize_composite_feather_detail_u8(None, offs, None, offs, (ctypes.c_int * 2)(256, 256), None, offs,
+                                                     (ctypes.c_longlong * 1)(192), (ctypes.c_int * 2)(0, 0), hw, fw, None, None, 1, 0, 1,
+                                                     ctypes.byref(scratch), None) != 0
     assert "null rgb / mask / canvas" in lib.se_last_error().decode()
 
 

@@ -1,6 +1,6 @@
 """Several regions per request on the CPU: the grouping rule of serving.region_groups (region="strokes"), the validation of box
 lists, the host flow of DemoProcessor against the Pillow statement with a fake forward, and the host checks of
-se_resize_composite_feather_u8 without feather widths."""
+se_resize_composite_feather_detail_u8 without feather widths."""
 import ctypes
 from collections import deque
 
@@ -283,12 +283,12 @@ def _query(lib, src, dst, n=1, yx=(0, 0), pitch=None, canvas_off=None, scratch=N
     pitches = (L * k)(*(pitch if isinstance(pitch, list) else [pitch if pitch is not None else 3 * (yx[1] + dst[1])] * k))
     shw, dhw, byx = (I * (2 * k))(*(src * k)), (I * (2 * k))(*(dst * k)), (I * (2 * k))(*(yx * k))
     need = L(scratch_bytes)
-    rc = lib.se_resize_composite_feather_u8(None, offs, None, offs, shw, None, coff, pitches, byx, dhw, None, n, 1, scratch,
-                                            ctypes.byref(need), None)
+    rc = lib.se_resize_composite_feather_detail_u8(None, offs, None, offs, shw, None, coff, pitches, byx, dhw, None, None, None, n, 1,
+                                                   scratch, ctypes.byref(need), None)
     return rc, need.value, lib.se_last_error().decode()
 
 
-def test_composite_scratch_query(lib):
+def test_composite_scratch_query_with_null_detail(lib):
     r256 = lambda b: (b + 255) // 256 * 256
     assert _query(lib, (256, 256), (608, 608))[:2] == (0, r256(256 * 608 * 3) + r256(256 * 608))
     assert _query(lib, (256, 256), (608, 256))[:2] == (0, 0)           # width unchanged: the paste reads the result itself
@@ -297,7 +297,7 @@ def test_composite_scratch_query(lib):
     assert _query(lib, (256, 256), (100, 77), n=0)[:2] == (0, 0)
 
 
-def test_composite_validates_on_the_host(lib):
+def test_composite_with_null_detail_validates_on_the_host(lib):
     cases = [
         (dict(src=(256, 256), dst=(64, 64), n=-1), "boxes"),
         (dict(src=(0, 256), dst=(64, 64)), "sizes must be in [1, 65535]"),
@@ -319,6 +319,6 @@ def test_composite_validates_on_the_host(lib):
     assert _query(lib, (0, 256), (64, 64))[2].split(" : ")[-1].split(" at ")[0] == \
         lib.se_last_error().decode().split(" : ")[-1].split(" at ")[0]        # the shared checks say what the window resize says
     hw = (ctypes.c_int * 2)(64, 64)
-    assert lib.se_resize_composite_feather_u8(None, None, None, None, hw, None, None, None, None, hw, None, 1, 0, None,
-                                              ctypes.byref(need), None) != 0
+    assert lib.se_resize_composite_feather_detail_u8(None, None, None, None, hw, None, None, None, None, hw, None, None, None, 1, 0,
+                                                     None, ctypes.byref(need), None) != 0
     assert "null size / offset array" in lib.se_last_error().decode()

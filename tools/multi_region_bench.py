@@ -7,7 +7,7 @@ two distant groups and three groups of which two have overlapping boxes, it comp
 region='strokes' (region_groups), alternated in one process:
   - latency: median wall time of process_image from one thread (includes the batcher's max_wait_ms window);
   - throughput: requests/s of 16 threads submitting 16 requests each;
-  - the composite kernel alone (paste_v_kernel of se_resize_composite_feather_u8) for 16 requests' boxes pasted into their canvases
+  - the composite kernel alone (paste_v_kernel of se_resize_composite_feather_detail_u8) for 16 requests' boxes pasted into their canvases
     as the device flow does it (a canvas per set of overlapping boxes): its device time from a separate torch.profiler run,
     the bytes it moves (the result and mask rows it reads once, each canvas pixel a box covers read and written once) and
     that rate over the H100 SXM data-sheet 3.35 TB/s.

@@ -6,7 +6,7 @@ For 1000x667 and 4000x2667 photos with the local sketch of tools/serving_bench.p
 reports three cases, alternated in one process: the whole photo, region='auto' at 256x256 and region='auto' at 512x512:
   - latency: median wall time of process_image from one thread (includes the batcher's max_wait_ms window);
   - throughput: requests/s of 16 threads submitting together (16 requests per thread, or 1 for whole 4000x2667 photos);
-  - the paste kernel alone (paste_v_kernel of se_resize_composite_feather_u8, one box per canvas) for a batch of 16 region
+  - the paste kernel alone (paste_v_kernel of se_resize_composite_feather_detail_u8, one box per canvas) for a batch of 16 region
     results pasted into their boxes:
     its device time from a separate torch.profiler run, the bytes it moves (the result and mask rows it reads once, the base
     it reads and the patch it writes) and that rate over the H100 SXM data-sheet 3.35 TB/s.
