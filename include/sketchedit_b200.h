@@ -256,20 +256,29 @@ int se_feather_u8(unsigned char* img, const long long* off, const int* hw, const
  *                                  feather, n, swap_rb, scratch, scratch_bytes, stream)
  *       = se_resize_composite_feather_detail_u8 with the same arguments and detail = detail_off = NULL before n. */
 /* Baseline JPEG of n in [0, 32] RGB windows, byte for byte what Pillow writes for an RGB image without info:
- *     buf = io.BytesIO();  Image.fromarray(img_i).save(buf, "JPEG", quality=quality, subsampling=subsampling)
- * quality in [1, 100]; subsampling 0 (4:4:4) or 2 (4:2:0, Pillow's default with quality 75). Image i is hw[2i] rows of
- * hw[2i+1] RGB pixels (sizes in [1, 65535]), its row r at src[i] + r * src_pitch[i] (bytes, >= 3 * hw[2i+1]); src is a host
- * array of n device pointers, and windows may overlap each other. The file (SOI, JFIF APP0, two DQT, SOF0, four DHT with the
- * Annex K tables, SOS, the entropy-coded data, EOI) goes to out + out_off[i], which must hold se_jpeg_max_bytes(h, w,
- * subsampling) bytes; only its first out_bytes_dev[i] bytes are written, and that count is stored in the device array
- * out_bytes_dev[i]. No out slice may overlap another or a window. scratch == NULL stores the scratch bytes the call needs in
- * *scratch_bytes (src, out and out_bytes_dev may be NULL then). Every argument is checked before anything is enqueued on
- * `stream`; the call only enqueues. */
+ *     buf = io.BytesIO();  Image.fromarray(img_i).save(buf, "JPEG", quality=quality, subsampling=subsampling, optimize=optimize)
+ * quality in [1, 100]; subsampling 0 (4:4:4) or 2 (4:2:0, Pillow's default with quality 75); optimize 0 (the Annex K Huffman
+ * tables, Pillow's default) or 1 (Huffman tables built for each image from its symbol counts: a smaller file of the same
+ * pixels). Image i is hw[2i] rows of hw[2i+1] RGB pixels (sizes in [1, 65535]), its row r at src[i] + r * src_pitch[i]
+ * (bytes, >= 3 * hw[2i+1]); src is a host array of n device pointers, and windows may overlap each other. The file (SOI,
+ * JFIF APP0, two DQT, SOF0, four DHT with the Annex K or the image's tables, SOS, the entropy-coded data, EOI) goes to
+ * out + out_off[i], which must hold se_jpeg_max_bytes(h, w, subsampling) bytes with either value of optimize; only its first
+ * out_bytes_dev[i] bytes are written, and that count is stored in the device array out_bytes_dev[i]. No out slice may
+ * overlap another or a window. scratch == NULL stores the scratch bytes the call needs in *scratch_bytes (src, out and
+ * out_bytes_dev may be NULL then); optimize = 1 needs about 12 KB more per image. Every argument is checked before anything
+ * is enqueued on `stream`; the call only enqueues, and never waits on the device. */
+int se_jpeg_encode_opt_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality,
+                          int subsampling, int optimize, unsigned char* out, const long long* out_off, long long* out_bytes_dev,
+                          void* scratch, long long* scratch_bytes, void* stream);
+/* se_jpeg_encode_opt_u8 with optimize = 0: the file of
+ *     buf = io.BytesIO();  Image.fromarray(img_i).save(buf, "JPEG", quality=quality, subsampling=subsampling) */
 int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality, int subsampling,
                       unsigned char* out, const long long* out_off, long long* out_bytes_dev, void* scratch, long long* scratch_bytes,
                       void* stream);
-/* Host only: a true upper bound of the file se_jpeg_encode_u8 writes for an h x w image: the 623-byte header, 208 bytes per
- * 8x8 block (64 codes of at most 26 bits) doubled for the 0x00 after each 0xFF, and EOI. -1 on bad arguments. */
+/* Host only: a true upper bound of the file se_jpeg_encode_opt_u8 writes for an h x w image with either value of optimize:
+ * the 623-byte header, 208 bytes per 8x8 block (64 codes of at most 26 bits) doubled for the 0x00 after each 0xFF, and EOI.
+ * Optimal tables keep codes within 16 bits and list only used symbols, so their header is no longer than the Annex K one,
+ * and a block's bits stay within 208 bytes (DESIGN.md, section 7b). -1 on bad arguments. */
 long long se_jpeg_max_bytes(int h, int w, int subsampling);
 /* PNG of n in [0, 32] windows, byte for byte what OpenCV writes with no parameters (OpenCV 4.13, libpng 1.6, zlib 1.3):
  *     cv2.imencode(".png", img_i)[1]

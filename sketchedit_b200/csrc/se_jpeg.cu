@@ -15,6 +15,9 @@
 //   stuff:  per 64-byte chunk of the stream: count its 0xFF bytes, scan the counts, then write the chunk after the header with
 //           0x00 after each 0xFF (the last byte padded with 1-bits); the last chunk writes EOI and the image's byte count.
 //   header: one block per image writes the header, a function of (h, w, quality, subsampling) built on the host.
+// With optimize = 1 (Pillow's optimize=True) se_jpeg_opt.cu counts each image's symbols after the bits kernel, builds its
+// Huffman tables, writes its header and recounts the block bits; pack then codes with the image's tables from scratch and
+// stuff writes the data after the image's header, whose length is on the device.
 #include <string.h>
 
 #include <algorithm>
@@ -71,10 +74,6 @@ constexpr HuffSpec kAcChroma = {
      0xe5, 0xe6, 0xe7, 0xe8, 0xe9, 0xea, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa},
     162};
 
-struct HuffCodes {   // symbol -> canonical code and its length (0: not in the table)
-  unsigned short code[256];
-  unsigned char size[256];
-};
 constexpr HuffCodes huff_codes(const HuffSpec& s) {   // Annex C
   HuffCodes h{};
   int code = 0, k = 0;
@@ -151,8 +150,6 @@ static void put_dht(std::vector<unsigned char>& v, int cls_id, const HuffSpec& s
   v.insert(v.end(), s.syms, s.syms + s.nsym);
 }
 
-constexpr int kSofHeightAt = 163;   // byte offsets of SOF0's height and width in the header
-
 // SOI, JFIF APP0 1.01 (density 1:1, units 0), DQT 0 and 1 (zigzag order), SOF0, DHT DC0 AC0 DC1 AC1, SOS (jcmarker.c)
 static std::vector<unsigned char> jpeg_header(int h, int w, const QuantTab* qt, int subsampling) {
   std::vector<unsigned char> v = {0xFF, 0xD8, 0xFF, 0xE0, 0, 16, 'J', 'F', 'I', 'F', 0, 1, 1, 0, 0, 1, 0, 1, 0, 0};
@@ -183,62 +180,11 @@ constexpr int kWordsPerBlock = JPEG_MAX_BLOCK_BITS / 32;
 constexpr int kChunkBytes = 64;   // bytes of the stream per stuffing thread
 constexpr int kThreads = 128;
 
-struct JImg {   // one image of a call; block, word and chunk indices are the call's (all images' arrays concatenated)
-  const unsigned char* src;
-  unsigned char* out;
-  long long* out_bytes;
-  long long pitch;
-  long long blk0, word0, chunk0;   // its first block, word and stuffing chunk
-  int h, w, mcu_x;                 // image size; MCUs per row
-};
-struct JpegList {
-  JImg im[JPEG_MAX_BATCH];
-  int n, sub;   // images; subsampling (0 or 2)
-  long long blocks, chunks;
-};
 struct JpegQuant {
   unsigned short recip[2][64], corr[2][64];
   unsigned char shift[2][64];
 };
 static_assert(sizeof(JpegList) + sizeof(JpegQuant) <= 4096, "descriptors must fit the kernel parameter space");
-
-struct JpegScratch {   // the call's scratch arrays
-  short* coef;                 // [64][blocks], zigzag order; [0] the quantised DC
-  unsigned* bits;              // [blocks]: AC bits (dct), then all bits of the block (bits)
-  int* dcdiff;                 // [blocks]
-  unsigned long long* bitoff;  // [blocks], exclusive scan of bits over the call
-  unsigned* words;             // the bit streams, word0 of each image on
-  unsigned* ffcnt;             // [chunks]
-  unsigned long long* ffoff;   // [chunks], exclusive scan of ffcnt over the call
-  unsigned long long* sums;    // scan tile sums
-};
-
-// Block e of an image in scan order: its component (0 Y, 1 Cb, 2 Cr) and block column / row in that component's plane.
-// A 4:2:0 MCU holds luma blocks (0,0), (0,1), (1,0), (1,1), then Cb and Cr; a 4:4:4 MCU holds Y, Cb, Cr.
-struct BlockAt {
-  int comp, bx, by;
-  bool dummy;   // a 4:2:0 luma block wholly outside the image
-};
-__device__ __forceinline__ BlockAt block_at(const JImg& d, int sub, long long e) {
-  const int per = sub == 2 ? 6 : 3;
-  const long long mcu = e / per;
-  const int k = (int)(e - mcu * per), mx = (int)(mcu % d.mcu_x), my = (int)(mcu / d.mcu_x);
-  BlockAt b;
-  if (sub == 2 && k < 4) {
-    b.comp = 0;
-    b.bx = 2 * mx + (k & 1);
-    b.by = 2 * my + (k >> 1);
-    b.dummy = b.bx * 8 >= d.w || b.by * 8 >= d.h;
-  } else {
-    b.comp = sub == 2 ? k - 3 : k;
-    b.bx = mx;
-    b.by = my;
-    b.dummy = false;
-  }
-  return b;
-}
-
-__device__ __forceinline__ int nbits(int v) { return v ? 32 - __clz(v < 0 ? -v : v) : 0; }
 
 __device__ __forceinline__ int color(int comp, int r, int g, int b) {   // jccolor.c, 16-bit fixed point
   if (comp == 0) return (19595 * r + 38470 * g + 7471 * b + 32768) >> 16;
@@ -413,15 +359,17 @@ __global__ void __launch_bounds__(kThreads) jpeg_pack_kernel(const __grid_consta
   stage_huff(sh, 0, 4);
   const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
   if (g >= L.blocks) return;
-  const JImg& d = L.im[image_of(L.im, L.n, &JImg::blk0, g)];
+  const int i = image_of(L.im, L.n, &JImg::blk0, g);
+  const JImg& d = L.im[i];
   const BlockAt b = block_at(d, L.sub, g - d.blk0);
   const unsigned long long at = S.bitoff[g] - S.bitoff[d.blk0];
   unsigned* w = S.words + d.word0;
   long long wi = (long long)(at >> 5);
   int n = (int)(at & 31);
   unsigned long long acc = 0;
-  const HuffCodes& dch = sh[b.comp ? 1 : 0];
-  const HuffCodes& ach = sh[b.comp ? 3 : 2];
+  const HuffCodes* T = S.tabs ? S.tabs[i].codes : sh;   // the image's optimal tables, or Annex K's
+  const HuffCodes& dch = T[b.comp ? 1 : 0];
+  const HuffCodes& ach = T[b.comp ? 3 : 2];
   const int diff = S.dcdiff[g];
   put_value(acc, n, w, wi, dch, nbits(diff), diff, nbits(diff));
   int run = 0;
@@ -472,7 +420,7 @@ __global__ void __launch_bounds__(kThreads) jpeg_stuff_kernel(const __grid_const
     return;
   }
   if (j0 >= nbytes) return;
-  unsigned char* o = d.out + JPEG_HEADER_BYTES + j0 + (S.ffoff[g] - S.ffoff[d.chunk0]);
+  unsigned char* o = d.out + (S.hdr_len ? S.hdr_len[i] : JPEG_HEADER_BYTES) + j0 + (S.ffoff[g] - S.ffoff[d.chunk0]);
   for (long long j = j0; j < j1; ++j) {
     const unsigned v = stream_byte(w, j, nbits);
     *o++ = (unsigned char)v;
@@ -485,29 +433,15 @@ __global__ void __launch_bounds__(kThreads) jpeg_stuff_kernel(const __grid_const
   }
 }
 
-struct HeaderList {
-  unsigned char bytes[JPEG_HEADER_BYTES];
-  unsigned char* out[JPEG_MAX_BATCH];
-  unsigned short hw[JPEG_MAX_BATCH][2];
-};
-static_assert(sizeof(HeaderList) <= 4096, "header descriptors must fit the kernel parameter space");
-
 __global__ void __launch_bounds__(kThreads) jpeg_header_kernel(const __grid_constant__ HeaderList H) {
   unsigned char* o = H.out[blockIdx.x];
-  for (int j = threadIdx.x; j < JPEG_HEADER_BYTES; j += kThreads) {
-    unsigned char v = H.bytes[j];
-    if (j >= kSofHeightAt && j < kSofHeightAt + 4) {
-      const int x = H.hw[blockIdx.x][(j - kSofHeightAt) >> 1];
-      v = (unsigned char)((j - kSofHeightAt) & 1 ? x : x >> 8);
-    }
-    o[j] = v;
-  }
+  for (int j = threadIdx.x; j < JPEG_HEADER_BYTES; j += kThreads) o[j] = header_byte(H, blockIdx.x, j);
 }
 
 // ------------------------------------------------------------------------------------------ host
 struct JpegLayout {   // the call's block, word and chunk counts and where its arrays lie in scratch
   long long blocks = 0, words = 0, chunks = 0;
-  size_t coef, bits, dcdiff, bitoff, words_at, ffcnt, ffoff, sums, total;
+  size_t coef, bits, dcdiff, bitoff, words_at, ffcnt, ffoff, sums, hist, tabs, hdr_len, total;
 };
 
 static long long image_blocks(int h, int w, int sub) {
@@ -516,7 +450,7 @@ static long long image_blocks(int h, int w, int sub) {
 }
 static long long chunks_of(long long blocks) { return (blocks * kWordsPerBlock * 4 + kChunkBytes - 1) / kChunkBytes; }
 
-static JpegLayout jpeg_layout(const int* hw, int n, int sub) {
+static JpegLayout jpeg_layout(const int* hw, int n, int sub, bool optimize) {
   JpegLayout l;
   for (int i = 0; i < n; ++i) {
     const long long b = image_blocks(hw[2 * i], hw[2 * i + 1], sub);
@@ -539,6 +473,9 @@ static JpegLayout jpeg_layout(const int* hw, int n, int sub) {
   l.ffcnt = take((size_t)l.chunks * sizeof(unsigned));
   l.ffoff = take((size_t)l.chunks * sizeof(unsigned long long));
   l.sums = take((size_t)std::max(tiles, 1LL) * sizeof(unsigned long long));
+  l.hist = take(optimize ? (size_t)n * 4 * 256 * sizeof(unsigned long long) : 0);
+  l.tabs = take(optimize ? (size_t)n * sizeof(JpegTables) : 0);
+  l.hdr_len = take(optimize ? (size_t)n * sizeof(int) : 0);
   l.total = at;
   return l;
 }
@@ -557,17 +494,18 @@ long long se_jpeg_max_bytes(int h, int w, int subsampling) {
   return jpeg_max_bytes(h, w, subsampling);
 }
 
-int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality, int subsampling,
-                      unsigned char* out, const long long* out_off, long long* out_bytes_dev, void* scratch, long long* scratch_bytes,
-                      void* stream) {
+int se_jpeg_encode_opt_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality,
+                          int subsampling, int optimize, unsigned char* out, const long long* out_off, long long* out_bytes_dev,
+                          void* scratch, long long* scratch_bytes, void* stream) {
   SE_REQUIRE(n >= 0 && n <= JPEG_MAX_BATCH, "n must be in [0, " + std::to_string(JPEG_MAX_BATCH) + "] images per call");
   SE_REQUIRE(quality >= 1 && quality <= 100, "quality must be in [1, 100]");
   SE_REQUIRE(subsampling == 0 || subsampling == 2, "subsampling must be 0 (4:4:4) or 2 (4:2:0)");
+  SE_REQUIRE(optimize == 0 || optimize == 1, "optimize must be 0 or 1");
   SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
   SE_REQUIRE(n == 0 || (src_pitch && hw && out_off), "null size / offset array");
   for (int i = 0; i < n; ++i)
     if (int rc = check_window(i, hw[2 * i], hw[2 * i + 1], src_pitch[i], 3LL * hw[2 * i + 1], out_off[i])) return rc;
-  const JpegLayout lay = jpeg_layout(hw, n, subsampling);
+  const JpegLayout lay = jpeg_layout(hw, n, subsampling, optimize);
   SE_SCRATCH(scratch, scratch_bytes, lay.total, n);
   SE_REQUIRE(src && out && out_bytes_dev, "null src / out / out_bytes");
   for (int i = 0; i < n; ++i) SE_REQUIRE(src[i] != nullptr, "null src");
@@ -623,13 +561,22 @@ int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitc
   S.ffcnt = (unsigned*)(s + lay.ffcnt);
   S.ffoff = (unsigned long long*)(s + lay.ffoff);
   S.sums = (unsigned long long*)(s + lay.sums);
+  S.hist = optimize ? (unsigned long long*)(s + lay.hist) : nullptr;
+  S.tabs = optimize ? (JpegTables*)(s + lay.tabs) : nullptr;
+  S.hdr_len = optimize ? (int*)(s + lay.hdr_len) : nullptr;
 
   SE_CUDA_OK(cudaMemsetAsync(S.words, 0, (size_t)lay.words * sizeof(unsigned), st));
-  jpeg_header_kernel<<<n, kThreads, 0, st>>>(H);
+  if (!optimize) jpeg_header_kernel<<<n, kThreads, 0, st>>>(H);
   jpeg_dct_kernel<<<grid_of(L.blocks, kThreads), kThreads, 0, st>>>(L, Q, S);
   jpeg_bits_kernel<<<grid_of(L.blocks, kThreads), kThreads, 0, st>>>(L, S);
   SE_CUDA_OK(cudaGetLastError());
-  int rc = exclusive_scan(S.bits, S.bitoff, S.sums, L.blocks, st);
+  int rc;
+  if (optimize) {   // the DC differences are in place; the bit counts so far are Annex K's and are rewritten
+    SE_CUDA_OK(cudaMemsetAsync(S.hist, 0, lay.tabs - lay.hist, st));
+    if ((rc = jpeg_optimize_tables(L, S, st))) return rc;
+    if ((rc = jpeg_optimize_header(L, H, S, st))) return rc;
+  }
+  rc = exclusive_scan(S.bits, S.bitoff, S.sums, L.blocks, st);
   if (rc) return rc;
   jpeg_pack_kernel<<<grid_of(L.blocks, kThreads), kThreads, 0, st>>>(L, S);
   jpeg_stuff_kernel<false><<<grid_of(L.chunks, kThreads), kThreads, 0, st>>>(L, S);
@@ -639,6 +586,13 @@ int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitc
   jpeg_stuff_kernel<true><<<grid_of(L.chunks, kThreads), kThreads, 0, st>>>(L, S);
   SE_CUDA_OK(cudaGetLastError());
   return 0;
+}
+
+int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality, int subsampling,
+                      unsigned char* out, const long long* out_off, long long* out_bytes_dev, void* scratch, long long* scratch_bytes,
+                      void* stream) {
+  return se_jpeg_encode_opt_u8(src, src_pitch, hw, n, quality, subsampling, 0, out, out_off, out_bytes_dev, scratch, scratch_bytes,
+                               stream);
 }
 
 }  // extern "C"

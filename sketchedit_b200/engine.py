@@ -622,7 +622,7 @@ def resize_u8(images, sizes, swap_rb=False):
     return [out[o:o + h * w * C].view(*shape(int(h), int(w))) for o, (h, w) in zip(dst_offs, sizes)]
 
 
-JPEG_MAX_BATCH = 32      # images per se_jpeg_encode_u8 call; the wrappers split longer lists into calls of this size
+JPEG_MAX_BATCH = 32      # images per se_jpeg_encode_opt_u8 call; the wrappers split longer lists into calls of this size
 JPEG_SUBSAMPLING = (0, 2)   # Pillow's subsampling values the encoder takes: 4:4:4 and 4:2:0
 
 
@@ -644,18 +644,20 @@ def _is_int(v):
     return isinstance(v, numbers.Integral) and not isinstance(v, bool)
 
 
-def _check_jpeg_args(quality, subsampling):
-    """(quality, subsampling) as Python ints, or ValueError."""
+def _check_jpeg_args(quality, subsampling, optimize=False):
+    """(quality, subsampling) as Python ints, or ValueError; ``optimize`` must be a bool (Python or numpy)."""
     if not _is_int(quality) or not 1 <= quality <= 100:
         raise ValueError("quality must be an integer in [1, 100], got %r" % (quality,))
     if not _is_int(subsampling) or subsampling not in JPEG_SUBSAMPLING:
         raise ValueError("subsampling must be 0 (4:4:4) or 2 (4:2:0), got %r" % (subsampling,))
+    if not isinstance(optimize, (bool, np.bool_)):
+        raise ValueError("optimize must be a bool, got %r" % (optimize,))
     return int(quality), int(subsampling)
 
 
 def _encode(codec, ptrs, pitches, sizes, dev, out=None, out_offsets=None):
     """The encoder ``codec`` over windows already checked, its batch size per call, on the current stream of ``dev``.
-    ``codec = (entry, per_call, args, max_bytes)``: the C entry's name (se_jpeg_encode_u8, se_png_encode_u8), images per
+    ``codec = (entry, per_call, args, max_bytes)``: the C entry's name (se_jpeg_encode_opt_u8, se_png_encode_u8), images per
     call, its format arguments after n, and the file bound of an h x w window. Returns ``(out, out_offsets, out_bytes)``."""
     entry, per_call, args, max_bytes = codec
     entry = getattr(_lib.load(), entry)
@@ -711,34 +713,40 @@ def _encode_list(codec, channels, images):
     return download_files(out, offs, out_bytes.cpu().tolist())
 
 
-def _jpeg_codec(quality, subsampling):
-    """``_encode``'s codec for JPEG at (quality, subsampling), checked."""
-    quality, subsampling = _check_jpeg_args(quality, subsampling)
-    return "se_jpeg_encode_u8", JPEG_MAX_BATCH, (quality, subsampling), lambda h, w: jpeg_max_bytes(h, w, subsampling)
+def _jpeg_codec(quality, subsampling, optimize):
+    """``_encode``'s codec for JPEG at (quality, subsampling, optimize), checked."""
+    quality, subsampling = _check_jpeg_args(quality, subsampling, optimize)
+    return ("se_jpeg_encode_opt_u8", JPEG_MAX_BATCH, (quality, subsampling, int(bool(optimize))),
+            lambda h, w: jpeg_max_bytes(h, w, subsampling))
 
 
-def jpeg_encode_u8_packed(src, src_offsets, src_pitches, sizes, quality=75, subsampling=2, out=None, out_offsets=None):
-    """Baseline JPEG of RGB windows (``se_jpeg_encode_u8``), byte for byte ``Image.save(buf, "JPEG", quality=quality,
-    subsampling=subsampling)`` of each: image i is the ``sizes[i] = (h, w)`` window whose row r starts at byte ``src_offsets[i] +
+def jpeg_encode_u8_packed(src, src_offsets, src_pitches, sizes, quality=75, subsampling=2, out=None, out_offsets=None,
+                          optimize=False):
+    """Baseline JPEG of RGB windows (``se_jpeg_encode_opt_u8``), byte for byte ``Image.save(buf, "JPEG", quality=quality,
+    subsampling=subsampling, optimize=optimize)`` of each: image i is the ``sizes[i] = (h, w)`` window whose row r starts at byte ``src_offsets[i] +
     r * src_pitches[i]`` of its source, with ``src_pitches[i] >= 3 w``. ``src`` is one contiguous CUDA uint8 tensor, or a list
     of them with one per image; windows may overlap. ``out`` (optional, contiguous CUDA uint8) receives file i at
     ``out_offsets[i]`` and must hold ``jpeg_max_bytes(h, w, subsampling)`` bytes there. Returns ``(out, out_offsets,
     out_bytes)``: ``out_bytes`` is a CUDA int64 tensor of the files' lengths. Only enqueues work on the current stream."""
-    return _encode_packed(_jpeg_codec(quality, subsampling), 3, src, src_offsets, src_pitches, sizes, out, out_offsets)
+    return _encode_packed(_jpeg_codec(quality, subsampling, optimize), 3, src, src_offsets, src_pitches, sizes, out, out_offsets)
 
 
-def jpeg_encode_u8(images, quality=75, subsampling=2):
+def jpeg_encode_u8(images, quality=75, subsampling=2, optimize=False):
     """JPEG files of CUDA uint8 [h, w, 3] RGB images, as ``bytes``: each is what ``Image.fromarray(img).save(buf, "JPEG",
-    quality=quality, subsampling=subsampling)`` writes. An image may be a strided view (a box of a larger photo: pixels packed
-    along a row, rows ``stride(0)`` bytes apart); it is encoded where it lies. One download of the lengths, then one of the
-    bytes into pinned staging. quality and subsampling are Python or numpy integers, not bools.
+    quality=quality, subsampling=subsampling, optimize=optimize)`` writes. An image may be a strided view (a box of a larger
+    photo: pixels packed along a row, rows ``stride(0)`` bytes apart); it is encoded where it lies. One download of the
+    lengths, then one of the bytes into pinned staging. quality and subsampling are Python or numpy integers, not bools;
+    optimize is a bool. ``optimize=True`` builds Huffman tables for each image from its symbol counts, on the device: the
+    pixels are the same and the file smaller. Pillow itself fails (OSError) to write an optimized file larger than its
+    buffer of max(64 KiB, h w) bytes (2 h w from quality 95 on), such as noise; the device writes it.
 
     Device memory: the call allocates, through torch's caching allocator, ``out`` at ``jpeg_max_bytes`` per image and the
-    scratch of ``se_jpeg_encode_u8``, both sized for the worst-case file (26 bits per coefficient, every byte stuffed), and
-    frees them on return. That is about 6.6 + 6.2 MB for a 1000x667 image at 4:2:0 and 104 + 98 MB for 4000x2667 (twice that
-    at 4:4:4), some 50 times a typical file; concurrent calls hold their sum. Each call also zeroes the word stream in
-    scratch (52 MB at 4000x2667, 4:2:0)."""
-    codec = _jpeg_codec(quality, subsampling)
+    scratch of ``se_jpeg_encode_opt_u8``, both sized for the worst-case file (26 bits per coefficient, every byte stuffed),
+    and frees them on return. That is about 6.6 + 6.2 MB for a 1000x667 image at 4:2:0 and 104 + 98 MB for 4000x2667 (twice
+    that at 4:4:4), some 50 times a typical file; concurrent calls hold their sum. ``optimize=True`` adds about 12 KB of
+    scratch per image (its histograms and tables). Each call also zeroes the word stream in scratch (52 MB at 4000x2667,
+    4:2:0)."""
+    codec = _jpeg_codec(quality, subsampling, optimize)
     images = list(images)
     return _encode_list(codec, 3, images) if images else []
 
