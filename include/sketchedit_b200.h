@@ -231,7 +231,7 @@ int se_resize_composite_feather_detail_u8(const unsigned char* rgb, const long l
  * Every patch position must have an anchor, u(bw - 1) >= Wn - 16 and v(bh - 1) >= Hn - 16 (true from bw >= Wn / 32 and
  * bh >= Hn / 32): a smaller box is an error. The GEMM runs over all L query rows (M = Mp), not only those that touch the hole.
  * A is an fp32 computation within 255 (L + 8) 2^-22 of its float64 value. Boxes run in order through one scratch of the
- * largest box's need (256 B aligned): 4 Mp^2 + 12 Mp Np bytes, Mp = L rounded up to 256, Np = 3 fw fh rounded up to 256,
+ * largest box's need (256 B aligned): 4 Mp^2 + 8 Mp Np bytes, Mp = L rounded up to 256, Np = 3 fw fh rounded up to 256,
  * fw = ceil(16 bw / Wn) + 2, fh likewise. Query form (scratch == NULL) as se_resize_window_u8's. Only enqueues work on `stream`. */
 int se_detail_u8(const unsigned char* const* photo, const long long* photo_pitch, const int* box_hw, int n, int Hn, int Wn,
                  const unsigned char* low, const long long* low_off, const unsigned char* hole, const long long* hole_off, const float* attn,

@@ -534,8 +534,8 @@ def detail_u8_packed(photo, photo_offsets, photo_pitches, box_sizes, region_size
     tensor holding box i's plane [bh,bw,3] at byte ``d_offsets[i]``, for ``resize_composite_u8_packed(..., detail=D,
     detail_offsets=d_offsets)``; agg (``want_agg``) a CUDA float32 tensor holding box i's aggregate A [bh,bw,3] at element
     ``d_offsets[i] // 2``, else None. Only enqueues work on the current stream. Transient device memory: one box's scratch at
-    a time, 4 Mp^2 + 12 Mp Np bytes (Mp = L rounded up to 256; Np = 3 fw fh rounded up to 256, fw = ceil(16 bw / Wn) + 2):
-    about 64 MB for a 608 x 608 box at 256 x 256."""
+    a time, 4 Mp^2 + 8 Mp Np bytes (Mp = L rounded up to 256; Np = 3 fw fh rounded up to 256, fw = ceil(16 bw / Wn) + 2):
+    about 44 MB for a 608 x 608 box at 256 x 256."""
     n = len(box_sizes)
     listed = isinstance(photo, (list, tuple))
     srcs = list(photo) if listed else [photo] * n

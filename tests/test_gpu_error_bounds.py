@@ -137,14 +137,7 @@ def test_contextual_attention_within_bound(h, w, B, mkind, fkind, mode):
     assert q <= 1.0, q
     if mode == "fp32_attn":
         # the attention map against fp64: P_l moves by at most P_l (exp(2 delta_n) - 1 + rel)
-        _, A = O.contextual_attention(feat.double(), mask_s.double())
-        fq = F.unfold(feat.double(), 4, stride=2).abs()                                  # |q| [B, d, L]
-        fn = feat.double() / torch.sqrt((feat.double() ** 2).sum((2, 3), keepdim=True) + 1e-8)
-        fk = F.unfold(fn, 4, stride=2).abs()
-        valid = (F.unfold(1 - mask_s.double(), 4, stride=2).mean(1) > 0.1).double()    # [B, L]
-        qk = torch.einsum("bdl,bdn->bln", fk, fq) * valid[:, :, None] * 10.0           # [B, keys, queries]
-        d_n = err["logit_rel"] * qk.max(1).values + err["logit_abs"]                     # [B, N]
-        bA = A * (torch.expm1(2 * d_n)[:, None, :] + err["rel"]) + UB.U32 * A + 2.0 ** -126
+        A, bA = UB.attention_fp32_map(feat, mask_s)
         qa = UB.max_ratio(attn.cpu(), A, bA)
         print("bound attention map %dx%d %s feat %s: max ratio %.3g" % (h, w, mkind, fkind, qa))
         assert qa <= 1.0, qa

@@ -370,14 +370,33 @@ def attention_out_bound(pre, y_ref, mode):
     return pre + U32 * (y_ref.abs() + pre) + 2.0 ** -126
 
 
-def attention_bf16_reference(feat, mask_s):
-    """fp64 reference and per-element bound of contextual_attention(precision="bf16") (se_cam.cu), whole map at once.
+def attention_fp32_map(feat, mask_s):
+    """fp64 softmax weights P [B, L keys, L queries] of the attention on feat and the per-element bound of the fp32 CUDA-core
+    map (contextual_attention(precision="fp32" or "fp32_direct", want_attn=True), and the fp32_direct forward's export):
+    logits off by at most delta_n (attention_err("fp32_direct")) move P_l by at most P_l (exp(2 delta_n) - 1 + rel), and
+    the stored fp32 value adds u. Runs on the device of feat."""
+    f = feat.double()
+    B, C, h, w = f.shape
+    err = attention_err("fp32_direct", C, h, w)
+    Q = F.unfold(f, 4, stride=2)                                                   # [B, d, L]
+    K = F.unfold(f / torch.sqrt((f ** 2).sum((2, 3), keepdim=True) + 1e-8), 4, stride=2)
+    valid = (F.unfold(1 - mask_s.double(), 4, stride=2).mean(1) > 0.1).double()   # [B, L]
+    P = torch.softmax(10.0 * valid[:, :, None] * torch.einsum("bdl,bdn->bln", K, Q), dim=1)
+    qk = torch.einsum("bdl,bdn->bln", K.abs(), Q.abs()) * valid[:, :, None] * 10.0  # [B, keys, queries]
+    d_n = err["logit_rel"] * qk.max(1).values + err["logit_abs"]                     # [B, N]
+    return P, P * (torch.expm1(2 * d_n)[:, None, :] + err["rel"]) + U32 * P + 2.0 ** -126
 
-    The reference runs on what the kernels multiply: queries and values bf16(feat), keys bf16(f * rnorm) and the
-    probabilities rounded to bf16, Y = fold(sum_l bf16(P_l) V_l). The bound covers what can still differ: a key element
-    whose fp32 rnorm moves it across a bf16 rounding boundary (one ulp), the fp32 accumulation of the logits, the softmax
-    statistics, a P_l that lands on the other side of a bf16 rounding boundary, the P V accumulation and the bf16 output.
-    Returns (Y [B, C, h, w], bound [B, C, h, w])."""
+
+def attention_bf16_map(feat, mask_s):
+    """fp64 reference and per-element bound of the bf16 attention's stored probabilities (se_cam.cu; the map that
+    contextual_attention(precision="bf16", want_attn=True) and the bf16 export forward return): Pb = bf16(P) of the exact
+    softmax on the kernels' operands, and Wp, how far the stored value may be from Pb (see attention_bf16_reference).
+    Returns (Pb, Wp), both [B, L keys, L queries]; runs on the device of feat."""
+    return _attention_bf16_probs(feat, mask_s)[:2]
+
+
+def _attention_bf16_probs(feat, mask_s):
+    """(Pb, Wp, Q, h, w) of attention_bf16_reference."""
     f = bf16(feat.float()).double()
     B, C, h, w = f.shape
     hs, ws = (h - 4) // 2 + 1, (w - 4) // 2 + 1
@@ -408,6 +427,20 @@ def attention_bf16_reference(feat, mask_s):
     Pb = bf16(P)
     # (+ 2^-126: ex2.approx.ftz flushes probabilities below fp32's normal range to 0)
     Wp = torch.maximum((bf16(P * torch.exp(E) * (1 + eps_c)) - Pb).abs(), (bf16(P * torch.exp(-E) * (1 - eps_c)) - Pb).abs()) + 2.0 ** -126
+    return Pb, Wp, Q, h, w
+
+
+def attention_bf16_reference(feat, mask_s):
+    """fp64 reference and per-element bound of contextual_attention(precision="bf16") (se_cam.cu), whole map at once.
+
+    The reference runs on what the kernels multiply: queries and values bf16(feat), keys bf16(f * rnorm) and the
+    probabilities rounded to bf16, Y = fold(sum_l bf16(P_l) V_l). The bound covers what can still differ: a key element
+    whose fp32 rnorm moves it across a bf16 rounding boundary (one ulp), the fp32 accumulation of the logits, the softmax
+    statistics, a P_l that lands on the other side of a bf16 rounding boundary, the P V accumulation and the bf16 output.
+    Returns (Y [B, C, h, w], bound [B, C, h, w])."""
+    Pb, Wp, Q, h, w = _attention_bf16_probs(feat, mask_s)
+    L = Pb.shape[1]
+    Qa = Q.abs()
     O = torch.einsum("bln,bdl->bdn", Pb, Q)
     Ow = torch.einsum("bln,bdl->bdn", Wp, Qa)
     Oa = torch.einsum("bln,bdl->bdn", Pb + Wp, Qa)
