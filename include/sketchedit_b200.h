@@ -280,6 +280,20 @@ int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitc
  * Optimal tables keep codes within 16 bits and list only used symbols, so their header is no longer than the Annex K one,
  * and a block's bits stay within 208 bytes (DESIGN.md, section 7b). -1 on bad arguments. */
 long long se_jpeg_max_bytes(int h, int w, int subsampling);
+/* Progressive JPEG of n in [0, 32] RGB windows, byte for byte what Pillow writes for an RGB image without info:
+ *     buf = io.BytesIO();  Image.fromarray(img_i).save(buf, "JPEG", quality=quality, subsampling=subsampling, progressive=True)
+ * with either value of Pillow's optimize (libjpeg-turbo builds optimal tables for every progressive file). The file is SOI,
+ * JFIF APP0, two DQT, SOF2, then the ten scans of jpeg_simple_progression, each after the DHT segments of the tables built
+ * from its own symbol counts and its SOS, then EOI. Arguments are those of se_jpeg_encode_opt_u8 without optimize, and are
+ * checked the same way; out + out_off[i] must hold se_jpeg_progressive_max_bytes(h, w, subsampling) bytes. The scratch is
+ * about 2.2 times that of se_jpeg_encode_opt_u8. The call only enqueues, and never waits on the device. */
+int se_jpeg_encode_progressive_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n,
+                                  int quality, int subsampling, unsigned char* out, const long long* out_off,
+                                  long long* out_bytes_dev, void* scratch, long long* scratch_bytes, void* stream);
+/* Host only: a true upper bound of the file se_jpeg_encode_progressive_u8 writes for an h x w image: the headers of the ten
+ * scans with the largest alphabets, per block the most bits each scan can spend on it (DESIGN.md, section 7b) padded per
+ * scan, doubled for the 0x00 after each 0xFF, and EOI. -1 on bad arguments. */
+long long se_jpeg_progressive_max_bytes(int h, int w, int subsampling);
 /* PNG of n in [0, 32] windows, byte for byte what OpenCV writes with no parameters (OpenCV 4.13, libpng 1.6, zlib 1.3):
  *     cv2.imencode(".png", img_i)[1]
  * where img_i is the window as BGR (channels 3) or grey (channels 1). Image i is hw[2i] rows of hw[2i+1] pixels of `channels`

@@ -305,20 +305,6 @@ __global__ void __launch_bounds__(kThreads) jpeg_dct_kernel(const __grid_constan
   S.bits[g] = bits;
 }
 
-// the quantised DC of block e's component that block e + 1 of that component codes its difference against: a dummy takes
-// the DC of the block before it in the MCU (block 0 of an MCU is never a dummy)
-__device__ __forceinline__ int dc_of(const JImg& d, int sub, const short* dc, long long e) {
-  while (block_at(d, sub, e).dummy) --e;
-  return dc[d.blk0 + e];
-}
-
-__device__ __forceinline__ long long prev_same_comp(int sub, long long e) {   // -1: the component's first block
-  const int per = sub == 2 ? 6 : 3;
-  const int k = (int)(e % per);
-  if (sub == 2 && k > 0 && k < 4) return e - 1;
-  return e - (sub == 2 && k == 0 ? 3 : per);
-}
-
 __global__ void __launch_bounds__(kThreads) jpeg_bits_kernel(const __grid_constant__ JpegList L, JpegScratch S) {
   const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
   if (g >= L.blocks) return;
@@ -336,16 +322,6 @@ __global__ void __launch_bounds__(kThreads) jpeg_bits_kernel(const __grid_consta
   const int nb = nbits(diff);
   S.bits[g] += dch.size[nb] + nb;
   S.dcdiff[g] = diff;
-}
-
-// appends len <= 27 bits to a 64-bit accumulator holding n < 32 bits; full words go to w[*wi] by atomicOr
-__device__ __forceinline__ void put_bits(unsigned long long& acc, int& n, unsigned* w, long long& wi, unsigned code, int len) {
-  acc = (acc << len) | code;
-  n += len;
-  if (n >= 32) {
-    n -= 32;
-    atomicOr(w + wi++, (unsigned)(acc >> n));
-  }
 }
 
 __device__ __forceinline__ void put_value(unsigned long long& acc, int& n, unsigned* w, long long& wi, const HuffCodes& h,
@@ -396,13 +372,6 @@ __device__ __forceinline__ unsigned long long image_bits(const JImg& d, const JI
   return S.bitoff[last] + S.bits[last] - S.bitoff[d.blk0];
 }
 
-// byte j of the image's stream, the last one padded with 1-bits
-__device__ __forceinline__ unsigned stream_byte(const unsigned* w, long long j, unsigned long long nbits) {
-  unsigned v = (w[j >> 2] >> (24 - 8 * (j & 3))) & 0xFFu;
-  if (j == (long long)((nbits - 1) >> 3) && (nbits & 7)) v |= 0xFFu >> (nbits & 7);
-  return v;
-}
-
 template <bool WRITE>
 __global__ void __launch_bounds__(kThreads) jpeg_stuff_kernel(const __grid_constant__ JpegList L, JpegScratch S) {
   const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
@@ -441,7 +410,8 @@ __global__ void __launch_bounds__(kThreads) jpeg_header_kernel(const __grid_cons
 // ------------------------------------------------------------------------------------------ host
 struct JpegLayout {   // the call's block, word and chunk counts and where its arrays lie in scratch
   long long blocks = 0, words = 0, chunks = 0;
-  size_t coef, bits, dcdiff, bitoff, words_at, ffcnt, ffoff, sums, hist, tabs, hdr_len, total;
+  size_t coef = 0, bits = 0, dcdiff = 0, bitoff = 0, words_at = 0, ffcnt = 0, ffoff = 0, sums = 0, hist = 0, tabs = 0,
+         hdr_len = 0, prog = 0, total = 0;
 };
 
 static long long image_blocks(int h, int w, int sub) {
@@ -450,11 +420,13 @@ static long long image_blocks(int h, int w, int sub) {
 }
 static long long chunks_of(long long blocks) { return (blocks * kWordsPerBlock * 4 + kChunkBytes - 1) / kChunkBytes; }
 
-static JpegLayout jpeg_layout(const int* hw, int n, int sub, bool optimize) {
+// progressive: the coefficients and the dct kernel's bit counts, then se_jpeg_prog.cu's arrays of `prog` bytes
+static JpegLayout jpeg_layout(const int* hw, int n, int sub, bool optimize, bool progressive, size_t prog) {
   JpegLayout l;
   for (int i = 0; i < n; ++i) {
     const long long b = image_blocks(hw[2 * i], hw[2 * i + 1], sub);
     l.blocks += b;
+    if (progressive) continue;
     l.words += b * kWordsPerBlock;
     l.chunks += chunks_of(b);
   }
@@ -467,6 +439,11 @@ static JpegLayout jpeg_layout(const int* hw, int n, int sub, bool optimize) {
   };
   l.coef = take((size_t)l.blocks * 64 * sizeof(short));
   l.bits = take((size_t)l.blocks * sizeof(unsigned));
+  if (progressive) {
+    l.prog = take(prog);
+    l.total = at;
+    return l;
+  }
   l.dcdiff = take((size_t)l.blocks * sizeof(int));
   l.bitoff = take((size_t)l.blocks * sizeof(unsigned long long));
   l.words_at = take((size_t)l.words * sizeof(unsigned));
@@ -494,9 +471,22 @@ long long se_jpeg_max_bytes(int h, int w, int subsampling) {
   return jpeg_max_bytes(h, w, subsampling);
 }
 
-int se_jpeg_encode_opt_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality,
-                          int subsampling, int optimize, unsigned char* out, const long long* out_off, long long* out_bytes_dev,
-                          void* scratch, long long* scratch_bytes, void* stream) {
+long long se_jpeg_progressive_max_bytes(int h, int w, int subsampling) {
+  if (h < 1 || w < 1 || h > kMaxDim || w > kMaxDim || (subsampling != 0 && subsampling != 2)) {
+    set_error("se_jpeg_progressive_max_bytes: sizes must be in [1, 65535] and subsampling 0 (4:4:4) or 2 (4:2:0)");
+    return -1;
+  }
+  return jpeg_prog_max_bytes(h, w, subsampling);
+}
+
+}  // extern "C"
+
+namespace se {
+
+// se_jpeg_encode_opt_u8 (progressive = false) and se_jpeg_encode_progressive_u8 (true, optimize = 0)
+static int jpeg_encode(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality,
+                       int subsampling, int optimize, bool progressive, unsigned char* out, const long long* out_off,
+                       long long* out_bytes_dev, void* scratch, long long* scratch_bytes, void* stream) {
   SE_REQUIRE(n >= 0 && n <= JPEG_MAX_BATCH, "n must be in [0, " + std::to_string(JPEG_MAX_BATCH) + "] images per call");
   SE_REQUIRE(quality >= 1 && quality <= 100, "quality must be in [1, 100]");
   SE_REQUIRE(subsampling == 0 || subsampling == 2, "subsampling must be 0 (4:4:4) or 2 (4:2:0)");
@@ -505,11 +495,25 @@ int se_jpeg_encode_opt_u8(const unsigned char* const* src, const long long* src_
   SE_REQUIRE(n == 0 || (src_pitch && hw && out_off), "null size / offset array");
   for (int i = 0; i < n; ++i)
     if (int rc = check_window(i, hw[2 * i], hw[2 * i + 1], src_pitch[i], 3LL * hw[2 * i + 1], out_off[i])) return rc;
-  const JpegLayout lay = jpeg_layout(hw, n, subsampling, optimize);
+  JpegList L;
+  ProgList P;
+  ProgScratch PS;
+  memset(&L, 0, sizeof(L));
+  memset(&P, 0, sizeof(P));
+  memset(&PS, 0, sizeof(PS));
+  L.n = n;
+  L.sub = subsampling;
+  for (int i = 0; i < n; ++i) {
+    L.im[i].h = hw[2 * i];
+    L.im[i].w = hw[2 * i + 1];
+  }
+  const JpegLayout lay = jpeg_layout(hw, n, subsampling, optimize, progressive,
+                                     progressive ? jpeg_prog_layout(L, nullptr, &P, &PS) : 0);
   SE_SCRATCH(scratch, scratch_bytes, lay.total, n);
   SE_REQUIRE(src && out && out_bytes_dev, "null src / out / out_bytes");
   for (int i = 0; i < n; ++i) SE_REQUIRE(src[i] != nullptr, "null src");
   SE_REQUIRE(lay.blocks < (1LL << 31) * kThreads && lay.chunks < (1LL << 31) * kThreads, "batch too large for one launch");
+  SE_REQUIRE(P.slots < (1LL << 31) * kThreads && P.chunks < (1LL << 31) * kThreads, "batch too large for one launch");
   cudaStream_t st = (cudaStream_t)stream;
 
   const QuantTab* qt = quant_tabs(quality);
@@ -519,14 +523,10 @@ int se_jpeg_encode_opt_u8(const unsigned char* const* src, const long long* src_
     memcpy(Q.corr[t], qt[t].corr, sizeof(Q.corr[t]));
     memcpy(Q.shift[t], qt[t].shift, sizeof(Q.shift[t]));
   }
-  JpegList L;
   HeaderList H;
-  memset(&L, 0, sizeof(L));
   memset(&H, 0, sizeof(H));
   const std::vector<unsigned char> hdr = jpeg_header(1, 1, qt, subsampling);
   memcpy(H.bytes, hdr.data(), JPEG_HEADER_BYTES);
-  L.n = n;
-  L.sub = subsampling;
   long long blk = 0, word = 0, chunk = 0;
   for (int i = 0; i < n; ++i) {
     const int h = hw[2 * i], w = hw[2 * i + 1], m = subsampling == 2 ? 16 : 8;
@@ -565,6 +565,13 @@ int se_jpeg_encode_opt_u8(const unsigned char* const* src, const long long* src_
   S.tabs = optimize ? (JpegTables*)(s + lay.tabs) : nullptr;
   S.hdr_len = optimize ? (int*)(s + lay.hdr_len) : nullptr;
 
+  if (progressive) {
+    jpeg_prog_layout(L, s + lay.prog, &P, &PS);
+    PS.coef = S.coef;
+    jpeg_dct_kernel<<<grid_of(L.blocks, kThreads), kThreads, 0, st>>>(L, Q, S);
+    SE_CUDA_OK(cudaGetLastError());
+    return jpeg_progressive(L, H, P, PS, st);
+  }
   SE_CUDA_OK(cudaMemsetAsync(S.words, 0, (size_t)lay.words * sizeof(unsigned), st));
   if (!optimize) jpeg_header_kernel<<<n, kThreads, 0, st>>>(H);
   jpeg_dct_kernel<<<grid_of(L.blocks, kThreads), kThreads, 0, st>>>(L, Q, S);
@@ -586,6 +593,24 @@ int se_jpeg_encode_opt_u8(const unsigned char* const* src, const long long* src_
   jpeg_stuff_kernel<true><<<grid_of(L.chunks, kThreads), kThreads, 0, st>>>(L, S);
   SE_CUDA_OK(cudaGetLastError());
   return 0;
+}
+
+}  // namespace se
+
+extern "C" {
+
+int se_jpeg_encode_opt_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality,
+                          int subsampling, int optimize, unsigned char* out, const long long* out_off, long long* out_bytes_dev,
+                          void* scratch, long long* scratch_bytes, void* stream) {
+  return jpeg_encode(src, src_pitch, hw, n, quality, subsampling, optimize, false, out, out_off, out_bytes_dev, scratch,
+                     scratch_bytes, stream);
+}
+
+int se_jpeg_encode_progressive_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n,
+                                  int quality, int subsampling, unsigned char* out, const long long* out_off,
+                                  long long* out_bytes_dev, void* scratch, long long* scratch_bytes, void* stream) {
+  return jpeg_encode(src, src_pitch, hw, n, quality, subsampling, 0, true, out, out_off, out_bytes_dev, scratch, scratch_bytes,
+                     stream);
 }
 
 int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality, int subsampling,

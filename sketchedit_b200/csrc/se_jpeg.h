@@ -102,6 +102,37 @@ __device__ __forceinline__ BlockAt block_at(const JImg& d, int sub, long long e)
 }
 
 __device__ __forceinline__ int nbits(int v) { return v ? 32 - __clz(v < 0 ? -v : v) : 0; }
+
+// the quantised DC of block e's component that block e + 1 of that component codes its difference against: a dummy takes
+// the DC of the block before it in the MCU (block 0 of an MCU is never a dummy)
+__device__ __forceinline__ int dc_of(const JImg& d, int sub, const short* dc, long long e) {
+  while (block_at(d, sub, e).dummy) --e;
+  return dc[d.blk0 + e];
+}
+
+__device__ __forceinline__ long long prev_same_comp(int sub, long long e) {   // -1: the component's first block
+  const int per = sub == 2 ? 6 : 3;
+  const int k = (int)(e % per);
+  if (sub == 2 && k > 0 && k < 4) return e - 1;
+  return e - (sub == 2 && k == 0 ? 3 : per);
+}
+
+// appends len <= 32 bits to a 64-bit accumulator holding n < 32 bits; full words go to w[*wi] by atomicOr
+__device__ __forceinline__ void put_bits(unsigned long long& acc, int& n, unsigned* w, long long& wi, unsigned code, int len) {
+  acc = (acc << len) | code;
+  n += len;
+  if (n >= 32) {
+    n -= 32;
+    atomicOr(w + wi++, (unsigned)(acc >> n));
+  }
+}
+
+// byte j of a stream, the last one padded with 1-bits
+__device__ __forceinline__ unsigned stream_byte(const unsigned* w, long long j, unsigned long long nbits) {
+  unsigned v = (w[j >> 2] >> (24 - 8 * (j & 3))) & 0xFFu;
+  if (j == (long long)((nbits - 1) >> 3) && (nbits & 7)) v |= 0xFFu >> (nbits & 7);
+  return v;
+}
 #endif
 
 // se_jpeg_opt.cu, each only enqueues on `st`. jpeg_optimize_tables: from the coefficients and DC differences in S, count
@@ -110,5 +141,52 @@ __device__ __forceinline__ int nbits(int v) { return v ? 32 - __clz(v < 0 ? -v :
 // to S.bits.
 int jpeg_optimize_tables(const JpegList& L, const JpegScratch& S, cudaStream_t st);
 int jpeg_optimize_header(const JpegList& L, const HeaderList& H, const JpegScratch& S, cudaStream_t st);
+// the optimal tables of `slots` histogram sets hist[slot][ntab][256] (ntab <= 4) into tabs[slot].codes[0 .. ntab)
+int jpeg_build_tables(const unsigned long long* hist, JpegTables* tabs, int slots, int ntab, cudaStream_t st);
+
+// ---- progressive (se_jpeg_prog.cu): the ten scans of jpeg_simple_progression, each coded with its own optimal tables.
+// A slot is one block of one scan; an image's slots run scan by scan, and each (image, scan) has its own bit stream.
+constexpr int JPEG_SCANS = 10;
+
+struct PImg {   // one image of a progressive call: its first slot, stream word and stuffing chunk, and its file
+  long long slot0, word0, chunk0;
+  unsigned char* out;
+  long long* out_bytes;
+};
+struct ProgList {
+  PImg im[JPEG_MAX_BATCH];
+  long long slots, chunks;
+  int sub;
+};
+
+struct ProgRun {   // the EOB runs a slot emits before its first coded symbol (pre) and after its last (post)
+  unsigned short pre_run, pre_be, post_run, post_be;   // run length (0: none) and the correction bits that go with it
+  unsigned pre_from, post_from;                         // the stream's first slot holding those bits
+};
+
+struct ProgScratch {
+  const short* coef;             // se_jpeg.cu's [64][blocks] zigzag coefficients
+  unsigned char* flags;          // [slots] AC scans: bit 7 the block ends in an EOB run, bit 6 it codes a symbol, bits 0-5
+                                 // its trailing correction bits
+  unsigned long long* corr;      // [slots] those bits, the first in the highest place
+  ProgRun* runs;                 // [slots]
+  unsigned* bits;                // [slots] bit count
+  unsigned long long* bitoff;    // [slots] exclusive scan of bits over the call
+  unsigned* words;               // the bit streams
+  unsigned* ffcnt;               // [chunks]
+  unsigned long long* ffoff;     // [chunks]
+  unsigned long long* sums;      // scan tile sums
+  unsigned long long* hist;      // [n][JPEG_SCANS][2][256]
+  JpegTables* tabs;              // [n][JPEG_SCANS], tables 0 (luma) and 1 (chroma)
+  long long* data_at;            // [n][JPEG_SCANS] where each scan's data starts in the file
+};
+
+// The call's slot, word and chunk layout into P (images' sizes from L) and, with base != null, S's arrays at base; returns
+// the scratch bytes. S.coef is the caller's.
+size_t jpeg_prog_layout(const JpegList& L, unsigned char* base, ProgList* P, ProgScratch* S);
+// a true bound of the progressive file of an h x w image (DESIGN §7b)
+long long jpeg_prog_max_bytes(int h, int w, int subsampling);
+// Enqueues the progressive coder on `st` after se_jpeg.cu's dct kernel: writes each image's file and byte count.
+int jpeg_progressive(const JpegList& L, const HeaderList& H, const ProgList& P, const ProgScratch& S, cudaStream_t st);
 
 }  // namespace se

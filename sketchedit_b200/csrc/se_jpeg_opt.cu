@@ -5,8 +5,9 @@
 //   hist:   one thread per 8x8 block counts the symbols the block codes (DC category, AC run/size, ZRL, EOB; a dummy luma
 //           block of a 4:2:0 MCU codes DC 0 and EOB) into its image's four 256-bin histograms: a CTA counts its first image's
 //           blocks in shared memory and adds them to global memory once, and any other image's straight to global memory.
-//   tables: one warp per (image, table) runs ITU T.81 Annex K.2 with libjpeg's tie rule, limits the lengths to 16 bits
-//           (Annex K.3), drops the reserved code and lists the symbols; writes the codes and the DHT contents.
+//   tables: one warp per (image, table), or per (image, scan, table) for se_jpeg_prog.cu, runs ITU T.81 Annex K.2 with
+//           libjpeg's tie rule, limits the lengths to 16 bits (Annex K.3), drops the reserved code and lists the symbols;
+//           writes the codes and the DHT contents.
 //   header: one CTA per image writes SOI..SOF0, the four DHT segments of its tables and SOS, and the header's length.
 //   bits:   one thread per block, its bit count with the image's tables (replacing the Annex K count).
 // se_jpeg.cu's scan, pack and stuff kernels then read the tables and the header length from scratch. The counts are
@@ -81,13 +82,14 @@ struct TableShared {
   int at[kMaxLen + 1];           // the first list position of each unlimited length
 };
 
-// One warp per table: blockIdx.x is the image, warp t its table t.
-__global__ void __launch_bounds__(kThreads) jpeg_table_kernel(JpegScratch S) {
+// One warp per table: blockIdx.x is the slot (an image, or one scan of an image), warp t its table t of ntab, counted in
+// hist[slot][t][256].
+__global__ void __launch_bounds__(kThreads) jpeg_table_kernel(const unsigned long long* hist_all, JpegTables* tabs, int ntab) {
   __shared__ TableShared shared[4];
   const int t = threadIdx.x >> 5, lane = threadIdx.x & 31;
   TableShared& W = shared[t];
-  const unsigned long long* hist = S.hist + ((size_t)blockIdx.x * 4 + t) * 256;
-  JpegTables& out = S.tabs[blockIdx.x];
+  const unsigned long long* hist = hist_all + ((size_t)blockIdx.x * ntab + t) * 256;
+  JpegTables& out = tabs[blockIdx.x];
   HuffCodes& hc = out.codes[t];
 
   // Annex K.2: merge the least frequent entry c1 with the next least frequent c2; among equal counts the higher symbol
@@ -220,7 +222,11 @@ __global__ void __launch_bounds__(kThreads) jpeg_opt_bits_kernel(const __grid_co
 
 int jpeg_optimize_tables(const JpegList& L, const JpegScratch& S, cudaStream_t st) {
   jpeg_hist_kernel<<<grid_of(L.blocks, kThreads), kThreads, 0, st>>>(L, S);
-  jpeg_table_kernel<<<L.n, kThreads, 0, st>>>(S);
+  return jpeg_build_tables(S.hist, S.tabs, L.n, 4, st);
+}
+
+int jpeg_build_tables(const unsigned long long* hist, JpegTables* tabs, int slots, int ntab, cudaStream_t st) {
+  jpeg_table_kernel<<<slots, 32 * ntab, 0, st>>>(hist, tabs, ntab);
   SE_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -634,9 +634,11 @@ def _max_bytes(entry, *args):
     return n
 
 
-def jpeg_max_bytes(h, w, subsampling=2):
-    """A true upper bound of the JPEG file of an h x w image (``se_jpeg_max_bytes``)."""
-    return _max_bytes(_lib.load().se_jpeg_max_bytes, h, w, subsampling)
+def jpeg_max_bytes(h, w, subsampling=2, progressive=False):
+    """A true upper bound of the JPEG file of an h x w image (``se_jpeg_max_bytes``, or ``se_jpeg_progressive_max_bytes``
+    with ``progressive=True``, about 2.2 times as large)."""
+    lib = _lib.load()
+    return _max_bytes(lib.se_jpeg_progressive_max_bytes if progressive else lib.se_jpeg_max_bytes, h, w, subsampling)
 
 
 def _is_int(v):
@@ -644,14 +646,17 @@ def _is_int(v):
     return isinstance(v, numbers.Integral) and not isinstance(v, bool)
 
 
-def _check_jpeg_args(quality, subsampling, optimize=False):
-    """(quality, subsampling) as Python ints, or ValueError; ``optimize`` must be a bool (Python or numpy)."""
+def _check_jpeg_args(quality, subsampling, optimize=False, progressive=False):
+    """(quality, subsampling) as Python ints, or ValueError; ``optimize`` and ``progressive`` must be bools (Python or
+    numpy)."""
     if not _is_int(quality) or not 1 <= quality <= 100:
         raise ValueError("quality must be an integer in [1, 100], got %r" % (quality,))
     if not _is_int(subsampling) or subsampling not in JPEG_SUBSAMPLING:
         raise ValueError("subsampling must be 0 (4:4:4) or 2 (4:2:0), got %r" % (subsampling,))
     if not isinstance(optimize, (bool, np.bool_)):
         raise ValueError("optimize must be a bool, got %r" % (optimize,))
+    if not isinstance(progressive, (bool, np.bool_)):
+        raise ValueError("progressive must be a bool, got %r" % (progressive,))
     return int(quality), int(subsampling)
 
 
@@ -713,25 +718,32 @@ def _encode_list(codec, channels, images):
     return download_files(out, offs, out_bytes.cpu().tolist())
 
 
-def _jpeg_codec(quality, subsampling, optimize):
-    """``_encode``'s codec for JPEG at (quality, subsampling, optimize), checked."""
-    quality, subsampling = _check_jpeg_args(quality, subsampling, optimize)
+def _jpeg_codec(quality, subsampling, optimize, progressive=False):
+    """``_encode``'s codec for JPEG at (quality, subsampling, optimize, progressive), checked. A progressive file has
+    optimal tables whatever ``optimize`` is, as in libjpeg-turbo."""
+    quality, subsampling = _check_jpeg_args(quality, subsampling, optimize, progressive)
+    if progressive:
+        return ("se_jpeg_encode_progressive_u8", JPEG_MAX_BATCH, (quality, subsampling),
+                lambda h, w: jpeg_max_bytes(h, w, subsampling, progressive=True))
     return ("se_jpeg_encode_opt_u8", JPEG_MAX_BATCH, (quality, subsampling, int(bool(optimize))),
             lambda h, w: jpeg_max_bytes(h, w, subsampling))
 
 
 def jpeg_encode_u8_packed(src, src_offsets, src_pitches, sizes, quality=75, subsampling=2, out=None, out_offsets=None,
-                          optimize=False):
+                          optimize=False, progressive=False):
     """Baseline JPEG of RGB windows (``se_jpeg_encode_opt_u8``), byte for byte ``Image.save(buf, "JPEG", quality=quality,
     subsampling=subsampling, optimize=optimize)`` of each: image i is the ``sizes[i] = (h, w)`` window whose row r starts at byte ``src_offsets[i] +
     r * src_pitches[i]`` of its source, with ``src_pitches[i] >= 3 w``. ``src`` is one contiguous CUDA uint8 tensor, or a list
     of them with one per image; windows may overlap. ``out`` (optional, contiguous CUDA uint8) receives file i at
-    ``out_offsets[i]`` and must hold ``jpeg_max_bytes(h, w, subsampling)`` bytes there. Returns ``(out, out_offsets,
-    out_bytes)``: ``out_bytes`` is a CUDA int64 tensor of the files' lengths. Only enqueues work on the current stream."""
-    return _encode_packed(_jpeg_codec(quality, subsampling, optimize), 3, src, src_offsets, src_pitches, sizes, out, out_offsets)
+    ``out_offsets[i]`` and must hold ``jpeg_max_bytes(h, w, subsampling, progressive)`` bytes there. Returns ``(out,
+    out_offsets, out_bytes)``: ``out_bytes`` is a CUDA int64 tensor of the files' lengths. Only enqueues work on the current
+    stream. ``progressive=True`` writes ``save(..., progressive=True)``'s file instead (``se_jpeg_encode_progressive_u8``),
+    the same whatever ``optimize`` is."""
+    return _encode_packed(_jpeg_codec(quality, subsampling, optimize, progressive), 3, src, src_offsets, src_pitches, sizes,
+                          out, out_offsets)
 
 
-def jpeg_encode_u8(images, quality=75, subsampling=2, optimize=False):
+def jpeg_encode_u8(images, quality=75, subsampling=2, optimize=False, progressive=False):
     """JPEG files of CUDA uint8 [h, w, 3] RGB images, as ``bytes``: each is what ``Image.fromarray(img).save(buf, "JPEG",
     quality=quality, subsampling=subsampling, optimize=optimize)`` writes. An image may be a strided view (a box of a larger
     photo: pixels packed along a row, rows ``stride(0)`` bytes apart); it is encoded where it lies. One download of the
@@ -745,8 +757,14 @@ def jpeg_encode_u8(images, quality=75, subsampling=2, optimize=False):
     and frees them on return. That is about 6.6 + 6.2 MB for a 1000x667 image at 4:2:0 and 104 + 98 MB for 4000x2667 (twice
     that at 4:4:4), some 50 times a typical file; concurrent calls hold their sum. ``optimize=True`` adds about 12 KB of
     scratch per image (its histograms and tables). Each call also zeroes the word stream in scratch (52 MB at 4000x2667,
-    4:2:0)."""
-    codec = _jpeg_codec(quality, subsampling, optimize)
+    4:2:0).
+
+    ``progressive=True`` (a bool) writes what ``save(..., progressive=True)`` writes, with either value of ``optimize``: the
+    ten scans of libjpeg-turbo's jpeg_simple_progression, each with optimal tables from its own counts, coded on the device
+    (``se_jpeg_encode_progressive_u8``). A page shows such a file coarse first and sharpens it as the rest arrives. Its
+    ``out`` is ``jpeg_max_bytes(..., progressive=True)`` per image and its scratch about 2.2 times the baseline one: some
+    229 + 219 MB at 4000x2667 with 4:2:0 (408 + 395 MB at 4:4:4), freed on return."""
+    codec = _jpeg_codec(quality, subsampling, optimize, progressive)
     images = list(images)
     return _encode_list(codec, 3, images) if images else []
 

@@ -1088,34 +1088,38 @@ class EditSession:
             with self._proc._torch.cuda.device(self._photo.device):
                 return Image.fromarray(self._photo.cpu().numpy())
 
-    def jpeg(self, quality=75, subsampling=2, box=None, optimize=False):
+    def jpeg(self, quality=75, subsampling=2, box=None, optimize=False, progressive=False):
         """The current photo, or its PIL box ``(left, upper, right, lower)``, as a JPEG file: the bytes of
 
             buf = io.BytesIO();  s.image().crop(box).save(buf, "JPEG", quality=quality, subsampling=subsampling,
-                                                          optimize=optimize)
+                                                          optimize=optimize, progressive=progressive)
 
         (no crop when ``box`` is None). ``quality`` in [1, 100]; ``subsampling`` 0 (4:4:4) or 2 (4:2:0, Pillow's default);
         ``optimize`` a bool: True builds Huffman tables for the image, a smaller file of the same pixels. Pillow fails
         (OSError) to write an optimized file larger than its buffer of max(64 KiB, w h) bytes (2 w h from quality 95 on),
         as a noisy photo at quality 90, 4:4:4 can be; the device encode still writes the file, the one Pillow writes
-        with a larger buffer.
+        with a larger buffer. ``progressive`` a bool: True writes a progressive file (ten scans, each with its own optimal
+        tables, whatever ``optimize`` is), which a page shows coarse at once and sharpens as the rest arrives; Pillow
+        refuses the same large files there.
         With ``resize='device'`` the photo is encoded on its device where it lies (``engine.jpeg_encode_u8``) and only the
         file is downloaded; with ``resize='host'`` Pillow encodes it. quality, subsampling and the box's entries are Python or
         numpy integers, not bools. The device encode holds transient device memory sized for the worst-case file (about
-        200 MB for a 4000x2667 photo at 4:2:0, 400 MB at 4:4:4, with or without optimize; ``engine.jpeg_encode_u8``)."""
+        200 MB for a 4000x2667 photo at 4:2:0, 400 MB at 4:4:4, with or without optimize, and about 450 MB at 4:2:0 for a
+        progressive file; ``engine.jpeg_encode_u8``)."""
         import io
 
         from . import engine
-        quality, subsampling = engine._check_jpeg_args(quality, subsampling, optimize)
+        quality, subsampling = engine._check_jpeg_args(quality, subsampling, optimize, progressive)
         with self._mu:
             self._check_open()
             box = self._box(box)
             if self._img is not None:
                 img = self._img if box is None else self._img.crop(box)
                 buf = io.BytesIO()
-                img.save(buf, "JPEG", quality=quality, subsampling=subsampling, optimize=bool(optimize))
+                img.save(buf, "JPEG", quality=quality, subsampling=subsampling, optimize=bool(optimize),
+                         progressive=bool(progressive))
                 return buf.getvalue()
-            return engine.jpeg_encode_u8([self._window(box)], quality, subsampling, optimize)[0]
+            return engine.jpeg_encode_u8([self._window(box)], quality, subsampling, optimize, progressive)[0]
 
     def png(self, box=None):
         """The current photo, or its PIL box ``(left, upper, right, lower)``, as a PNG file: the bytes of
