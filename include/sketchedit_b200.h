@@ -184,6 +184,23 @@ int se_outputs_to_uint8(const float* composed, const float* mask, int B, int H, 
 int se_resize_window_u8(const unsigned char* const* src, const long long* src_pitch, const int* src_hw, unsigned char* dst,
                         const long long* dst_off, const int* dst_hw, int n, int channels, int swap_rb, void* scratch,
                         long long* scratch_bytes, void* stream);
+/* Pillow's reducing resize of n in [0, 32] RGB windows, bit for bit (Pillow 12.2), the resize of Image.thumbnail(size):
+ *     Image.crop(box).resize((w, h), Image.BICUBIC, reducing_gap=2.0)
+ * The windows, their pitches, dst, dst_off and the sizes are those of se_resize_window_u8 with 3 channels and no swap;
+ * the caller applies thumbnail's size rule. For a window of iw x ih resized to w x h, fx = int(iw / w / 2) or 1, fy
+ * likewise. If either is > 1 the window is first reduced to ceil(iw / fx) x ceil(ih / fy) cells, each the average of the
+ * pixels it covers (right and bottom cells may be partial), per channel ((s + n / 2) * m mod 2^32) >> 24 with s the cell's
+ * byte sum, n its pixel count and m = uint32(float(2^32) / float(256 n)) (Image.reduce). The reduced image is then resampled
+ * bicubically over the box (0, 0, iw / fx, ih / fy), box ends in C floats; an axis is resampled when its length changes or
+ * its box end is not its length, vertically first when the reduced image is more than 100 times taller than wide and its
+ * height shrinks, horizontally first otherwise. A window whose size does not change is copied. fx fy must stay below 2^24.
+ * scratch holds per window its reduced image (when fx or fy > 1) and the intermediate of a resample along both axes, each
+ * rounded up to 256 bytes; the query form (scratch == NULL) is se_resize_window_u8's. The coefficient tables share
+ * se_resize_window_u8's cache and limit, keyed by (in, box end, out): the first call with a new key uploads its table (a
+ * synchronous copy); otherwise the call only enqueues work on `stream`. */
+int se_resize_reducing_u8(const unsigned char* const* src, const long long* src_pitch, const int* src_hw, unsigned char* dst,
+                          const long long* dst_off, const int* dst_hw, int n, void* scratch, long long* scratch_bytes,
+                          void* stream);
 /* Resize back and paste n >= 0 boxes in order into canvases, bit for bit as sequential Pillow pastes (a region edit: the
  * forward's results on crops of the photo, pasted back into their boxes, which may overlap, nest or repeat):
  *     for i in 0 .. n-1:  res = Image.fromarray(rgb_i).resize((w, h));  m = Image.fromarray(mask_i).resize((w, h));

@@ -48,6 +48,8 @@ SIGNATURES = {
     "se_outputs_to_uint8": (_c_int, [_c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_void_p, _c_void_p, _c_void_p]),
     "se_resize_window_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int,
                                      _c_void_p, ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
+    "se_resize_reducing_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_void_p,
+                                       ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
     "se_forward_u8_export": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_int, _c_void_p,
                                       _c_void_p, _c_void_p, _c_void_p, _c_void_p]),
     "se_resize_composite_feather_detail_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p,

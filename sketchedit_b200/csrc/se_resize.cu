@@ -11,7 +11,8 @@
 // Image.crop(box).resize(size) without the crop. se_resize_composite_feather_detail_u8 resizes results and their masks the same way
 // and pastes boxes that may overlap into shared canvases in order, as sequential Image.paste(im, box, mask) calls do, with
 // the blend fused into the vertical pass (paste_v_kernel); it fades each box's mask to 0 along the box edges it is given
-// widths for. se_feather_u8 applies that fade to masks alone (feather_kernel).
+// widths for. se_feather_u8 applies that fade to masks alone (feather_kernel). resize_box_rgb (se_resize.h) runs the same two
+// passes with the fractional box of Image.resize(..., reducing_gap=...), in either order, for se_thumbnail.cu.
 #include <limits.h>
 #include <math.h>
 #include <string.h>
@@ -24,10 +25,10 @@
 
 #include "../../include/sketchedit_b200.h"
 #include "se_common.cuh"
+#include "se_resize.h"
 
 namespace se {
 
-constexpr int RESIZE_MAX_BATCH = 32;   // images per launch: their descriptors travel as kernel parameters
 constexpr int RESIZE_PREC_BITS = 22;   // fractional bits of the fixed-point coefficients (Pillow's PRECISION_BITS for 8 bpc)
 
 // ------------------------------------------------------------------------------------------ coefficients (host, double)
@@ -39,18 +40,20 @@ static double bicubic_filter(double x) {   // Keys cubic, a = -0.5, support 2
   return 0.0;
 }
 
-static double axis_scale(int in, int out) { return (double)(float)in / out; }   // Pillow: (in1 - in0) / outSize, box in float
+// Pillow: (in1 - in0) / outSize with the box in floats; in0 = 0 and, without a box, in1 = in
+static double axis_scale(float in1, int out) { return (double)in1 / out; }
 
-static int resize_ksize(int in, int out) {
-  const double scale = axis_scale(in, out);
+static int resize_ksize(float in1, int out) {
+  const double scale = axis_scale(in1, out);
   const double fs = scale < 1.0 ? 1.0 : scale;
   return (int)ceil(2.0 * fs) * 2 + 1;
 }
 
-// Pillow's coefficient table for one axis (in -> out samples): bounds[2*i] = first input sample of output i, bounds[2*i+1] =
-// number of taps; coeffs[i*ksize + k] the fixed-point weights (zero beyond the taps). Returns ksize.
-static int resize_coeff_table(int in, int out, int* bounds, int* coeffs) {
-  const double scale = axis_scale(in, out);
+// Pillow's coefficient table for one axis (in -> out samples over the box (0, in1); in1 = in without a box): bounds[2*i] =
+// first input sample of output i, bounds[2*i+1] = number of taps; coeffs[i*ksize + k] the fixed-point weights (zero beyond
+// the taps). Returns ksize.
+static int resize_coeff_table(int in, float in1, int out, int* bounds, int* coeffs) {
+  const double scale = axis_scale(in1, out);
   const double fs = scale < 1.0 ? 1.0 : scale;
   const double support = 2.0 * fs, ss = 1.0 / fs;
   const int ksize = (int)ceil(support) * 2 + 1;
@@ -80,7 +83,8 @@ static int resize_coeff_table(int in, int out, int* bounds, int* coeffs) {
 }
 
 // ------------------------------------------------------------------------------------------ device cache of the tables
-// One table per (device, in, out): a size seen before costs no host work and no copy. A new table is built and uploaded
+// One table per (device, in, in1, out), in1 the box end's float bits (in itself without a box): a size seen before costs no
+// host work and no copy. A new table is built and uploaded
 // synchronously. Each device's tables are limited to g_table_cap bytes (se_resize_set_table_cache_limit). When a call's new
 // tables would pass the limit, the device's cache is emptied after a device synchronise BEFORE the call looks up any table, so
 // every table a call launches with stays allocated until its kernels have run. (A single call's own tables may exceed the limit.)
@@ -91,11 +95,24 @@ struct AxisTable {
   size_t bytes = 0;
 };
 static std::mutex g_resize_mu;   // guards the cache and its limit; held for the whole launch part of a call
-static std::map<std::tuple<int, int, int>, AxisTable> g_tables;
+struct TableKey {   // one axis: in samples, the box end in1 (in without a box), out samples
+  int in;
+  float in1;
+  int out;
+  bool operator==(const TableKey& o) const { return in == o.in && out == o.out && in1_bits() == o.in1_bits(); }
+  uint32_t in1_bits() const {
+    uint32_t u;
+    memcpy(&u, &in1, 4);
+    return u;
+  }
+};
+static std::map<std::tuple<int, int, uint32_t, int>, AxisTable> g_tables;
 constexpr size_t kDefaultTableCap = 256u << 20;
 static size_t g_table_cap = kDefaultTableCap;
 
-static size_t table_bytes(int in, int out) { return (size_t)out * (2 + resize_ksize(in, out)) * sizeof(int); }
+static std::tuple<int, int, uint32_t, int> cache_key(int dev, const TableKey& k) { return std::make_tuple(dev, k.in, k.in1_bits(), k.out); }
+static TableKey plain_key(int in, int out) { return {in, (float)in, out}; }
+static size_t table_bytes(const TableKey& k) { return (size_t)k.out * (2 + resize_ksize(k.in1, k.out)) * sizeof(int); }
 
 static size_t held_bytes(int dev) {
   size_t held = 0;
@@ -104,14 +121,14 @@ static size_t held_bytes(int dev) {
   return held;
 }
 
-// (in, out) pairs of one call: empties the device's cache first when the call's missing tables would pass the limit
-static int reserve_tables(int dev, const std::vector<std::pair<int, int>>& pairs) {
-  std::vector<std::pair<int, int>> missing;
+// the tables of one call: empties the device's cache first when the call's missing tables would pass the limit
+static int reserve_tables(int dev, const std::vector<TableKey>& keys) {
+  std::vector<TableKey> missing;
   size_t need = 0;
-  for (auto& p : pairs) {
-    if (g_tables.count(std::make_tuple(dev, p.first, p.second)) || std::find(missing.begin(), missing.end(), p) != missing.end()) continue;
-    missing.push_back(p);
-    need += table_bytes(p.first, p.second);
+  for (auto& k : keys) {
+    if (g_tables.count(cache_key(dev, k)) || std::find(missing.begin(), missing.end(), k) != missing.end()) continue;
+    missing.push_back(k);
+    need += table_bytes(k);
   }
   if (need == 0 || held_bytes(dev) + need <= g_table_cap) return 0;
   SE_CUDA_OK(cudaDeviceSynchronize());   // launches already enqueued may still read the tables
@@ -126,22 +143,22 @@ static int reserve_tables(int dev, const std::vector<std::pair<int, int>>& pairs
   return 0;
 }
 
-// the cached table of (in, out), built and uploaded on a miss; never frees a table (reserve_tables does, before any lookup)
-static int axis_table(int dev, int in, int out, const AxisTable** t) {
-  const auto key = std::make_tuple(dev, in, out);
+// the cached table of k, built and uploaded on a miss; never frees a table (reserve_tables does, before any lookup)
+static int axis_table(int dev, const TableKey& k, const AxisTable** t) {
+  const auto key = cache_key(dev, k);
   auto it = g_tables.find(key);
   if (it != g_tables.end()) {
     *t = &it->second;
     return 0;
   }
   AxisTable a;
-  a.ksize = resize_ksize(in, out);
-  std::vector<int> host((size_t)out * (2 + a.ksize));
-  resize_coeff_table(in, out, host.data(), host.data() + 2 * (size_t)out);
+  a.ksize = resize_ksize(k.in1, k.out);
+  std::vector<int> host((size_t)k.out * (2 + a.ksize));
+  resize_coeff_table(k.in, k.in1, k.out, host.data(), host.data() + 2 * (size_t)k.out);
   a.bytes = host.size() * sizeof(int);
   SE_CUDA_OK(cudaMalloc(&a.bounds, a.bytes));
   SE_CUDA_OK(cudaMemcpy(a.bounds, host.data(), a.bytes, cudaMemcpyHostToDevice));
-  a.coeffs = a.bounds + 2 * (size_t)out;
+  a.coeffs = a.bounds + 2 * (size_t)k.out;
   *t = &(g_tables[key] = a);
   return 0;
 }
@@ -478,11 +495,12 @@ static int check_resize(int i, int ih, int iw, int oh, int ow) {
   return 0;
 }
 
-// appends the horizontal pass rows x iw -> rows x ow of src (rows src_pitch bytes apart) into dst (packed rows) to hl
+// appends the horizontal pass rows x iw -> rows x ow of src (rows src_pitch bytes apart) into dst (packed rows) to hl, over
+// the box (0, in1) of the rows (in1 = iw: no box)
 static int add_h_pass(int dev, PassList<HPass>& hl, long long& tiles, int& kmax, const unsigned char* src, long long src_pitch,
-                      unsigned char* dst, int rows, int iw, int ow, int swap) {
+                      unsigned char* dst, int rows, int iw, float in1, int ow, int swap) {
   const AxisTable* t = nullptr;
-  int rc = axis_table(dev, iw, ow, &t);
+  int rc = axis_table(dev, {iw, in1, ow}, &t);
   if (rc) return rc;
   HPass& h = hl.p[hl.n++];
   h.src = src;
@@ -511,17 +529,50 @@ static int launch_h(const PassList<HPass>& hl, long long tiles, int kmax, cudaSt
   return 0;
 }
 
-// the vertical table of ih -> oh, or none (a copy) when the height does not change
-static int v_table(int dev, int ih, int oh, const int** bounds, const int** coeffs, int* ksize) {
+// the vertical table of ih -> oh over the box (0, in1) of the columns (in1 = ih: no box), or none (a copy) when the height
+// does not change and there is no box
+static int v_table(int dev, int ih, float in1, int oh, const int** bounds, const int** coeffs, int* ksize) {
   *bounds = *coeffs = nullptr;
   *ksize = 1;
-  if (ih == oh) return 0;
+  if (ih == oh && in1 == (float)ih) return 0;
   const AxisTable* t = nullptr;
-  int rc = axis_table(dev, ih, oh, &t);
+  int rc = axis_table(dev, {ih, in1, oh}, &t);
   if (rc) return rc;
   *bounds = t->bounds;
   *coeffs = t->coeffs;
   *ksize = t->ksize;
+  return 0;
+}
+
+// appends the vertical pass in_h x row_bytes -> oh x row_bytes of src (rows src_pitch bytes apart) into dst (packed rows) to
+// vl, over the box (0, in1) of the columns (in1 = in_h: no box); without a box and a height change it copies
+static int add_v_pass(int dev, PassList<VPass>& vl, long long& tiles, int& kmax, const unsigned char* src, long long src_pitch,
+                      unsigned char* dst, int in_h, float in1, int oh, int row_bytes, int swap) {
+  VPass& v = vl.p[vl.n++];
+  v.src = src;
+  v.dst = dst;
+  v.src_pitch = src_pitch;
+  int rc = v_table(dev, in_h, in1, oh, &v.bounds, &v.coeffs, &v.ksize);
+  if (rc) return rc;
+  v.in_h = in_h;
+  v.out_h = oh;
+  v.row_bytes = row_bytes;
+  v.groups = grid_of(v.row_bytes, V_GROUP);
+  v.swap = swap;
+  v.vec = ((uintptr_t)v.src % 4 == 0) && ((uintptr_t)v.dst % 4 == 0) && v.row_bytes % 4 == 0 && src_pitch % 4 == 0;
+  v.tile0 = (int)tiles;
+  v.tiles_x = grid_of(v.groups, V_TX);
+  tiles += (long long)v.tiles_x * grid_of(oh, V_TY);
+  kmax = std::max(kmax, v.ksize);
+  return 0;
+}
+
+static int launch_v(const PassList<VPass>& vl, long long tiles, int kmax, cudaStream_t st) {
+  if (!vl.n) return 0;
+  const int smem = (V_TY * kmax + 2 * V_TY) * 4;
+  SE_CUDA_OK(cudaFuncSetAttribute(resize_v_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+  resize_v_kernel<<<(unsigned)tiles, dim3(V_TX, V_TY), smem, st>>>(vl);
+  SE_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
@@ -542,12 +593,12 @@ static int resize_images(const unsigned char* const* src, const long long* pitch
   int dev = 0;
   SE_CUDA_OK(cudaGetDevice(&dev));
   {
-    std::vector<std::pair<int, int>> pairs;
+    std::vector<TableKey> keys;
     for (int i = 0; i < n; ++i) {
-      if (src_hw[2 * i + 1] != dst_hw[2 * i + 1]) pairs.emplace_back(src_hw[2 * i + 1], dst_hw[2 * i + 1]);
-      if (src_hw[2 * i] != dst_hw[2 * i]) pairs.emplace_back(src_hw[2 * i], dst_hw[2 * i]);
+      if (src_hw[2 * i + 1] != dst_hw[2 * i + 1]) keys.push_back(plain_key(src_hw[2 * i + 1], dst_hw[2 * i + 1]));
+      if (src_hw[2 * i] != dst_hw[2 * i]) keys.push_back(plain_key(src_hw[2 * i], dst_hw[2 * i]));
     }
-    int rc = reserve_tables(dev, pairs);
+    int rc = reserve_tables(dev, keys);
     if (rc) return rc;
   }
   PassList<HPass> hl;
@@ -563,39 +614,73 @@ static int resize_images(const unsigned char* const* src, const long long* pitch
     unsigned char* o = dst + dst_off[i];
     if (iw != ow) {
       unsigned char* h_dst = ih != oh ? (unsigned char*)scratch + mid[i] : o;
-      int rc = add_h_pass(dev, hl, htiles, hk, s, sp, h_dst, ih, iw, ow, ih == oh && swap_rb);
+      int rc = add_h_pass(dev, hl, htiles, hk, s, sp, h_dst, ih, iw, (float)iw, ow, ih == oh && swap_rb);
       if (rc) return rc;
       if (ih == oh) continue;
       s = h_dst;
       sp = (long long)ow * C;
     }
-    VPass& v = vl.p[vl.n++];   // the vertical pass, or the copy of an image whose size does not change
-    v.src = s;
-    v.dst = o;
-    v.src_pitch = sp;
-    int rc = v_table(dev, ih, oh, &v.bounds, &v.coeffs, &v.ksize);
+    // the vertical pass, or the copy of an image whose size does not change
+    int rc = add_v_pass(dev, vl, vtiles, vk, s, sp, o, ih, (float)ih, oh, ow * C, swap_rb);
     if (rc) return rc;
-    v.in_h = ih;
-    v.out_h = oh;
-    v.row_bytes = ow * C;
-    v.groups = grid_of(v.row_bytes, V_GROUP);
-    v.swap = swap_rb;
-    v.vec = ((uintptr_t)v.src % 4 == 0) && ((uintptr_t)v.dst % 4 == 0) && v.row_bytes % 4 == 0 && sp % 4 == 0;
-    v.tile0 = (int)vtiles;
-    v.tiles_x = grid_of(v.groups, V_TX);
-    vtiles += (long long)v.tiles_x * grid_of(oh, V_TY);
-    vk = std::max(vk, v.ksize);
   }
   SE_REQUIRE(htiles < (1LL << 31) && vtiles < (1LL << 31), "batch too large for one launch");
   int rc = C == 3 ? launch_h<3>(hl, htiles, hk, st) : launch_h<1>(hl, htiles, hk, st);
   if (rc) return rc;
-  if (vl.n) {
-    const int smem = (V_TY * vk + 2 * V_TY) * 4;
-    SE_CUDA_OK(cudaFuncSetAttribute(resize_v_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
-    resize_v_kernel<<<(unsigned)vtiles, dim3(V_TX, V_TY), smem, st>>>(vl);
-    SE_CUDA_OK(cudaGetLastError());
+  return launch_v(vl, vtiles, vk, st);
+}
+
+int resize_box_rgb(const BoxResize* im, int n, cudaStream_t st) {
+  std::lock_guard<std::mutex> lk(g_resize_mu);
+  int dev = 0;
+  SE_CUDA_OK(cudaGetDevice(&dev));
+  {
+    std::vector<TableKey> keys;
+    for (int i = 0; i < n; ++i) {
+      if (box_needs_h(im[i])) keys.push_back({im[i].iw, im[i].in1_w, im[i].ow});
+      if (box_needs_v(im[i])) keys.push_back({im[i].ih, im[i].in1_h, im[i].oh});
+    }
+    int rc = reserve_tables(dev, keys);
+    if (rc) return rc;
   }
-  return 0;
+  // three launches: the horizontal passes that come first, every vertical pass (or copy), the horizontal passes that come
+  // after a vertical one
+  PassList<HPass> h0, h1;
+  PassList<VPass> vl;
+  memset(&h0, 0, sizeof(h0));
+  memset(&h1, 0, sizeof(h1));
+  memset(&vl, 0, sizeof(vl));
+  long long t0 = 0, t1 = 0, vt = 0;
+  int k0 = 1, k1 = 1, vk = 1;
+  for (int i = 0; i < n; ++i) {
+    const BoxResize& b = im[i];
+    const bool nh = box_needs_h(b), nv = box_needs_v(b);
+    if (b.v_first && nh && nv) {
+      int rc = add_v_pass(dev, vl, vt, vk, b.src, b.pitch, b.mid, b.ih, b.in1_h, b.oh, b.iw * 3, 0);
+      if (rc) return rc;
+      rc = add_h_pass(dev, h1, t1, k1, b.mid, 3LL * b.iw, b.dst, b.oh, b.iw, b.in1_w, b.ow, 0);
+      if (rc) return rc;
+      continue;
+    }
+    const unsigned char* s = b.src;
+    long long sp = b.pitch;
+    if (nh) {
+      unsigned char* h_dst = nv ? b.mid : b.dst;
+      int rc = add_h_pass(dev, h0, t0, k0, s, sp, h_dst, b.ih, b.iw, b.in1_w, b.ow, 0);
+      if (rc) return rc;
+      if (!nv) continue;
+      s = h_dst;
+      sp = 3LL * b.ow;
+    }
+    int rc = add_v_pass(dev, vl, vt, vk, s, sp, b.dst, b.ih, b.in1_h, b.oh, b.ow * 3, 0);
+    if (rc) return rc;
+  }
+  SE_REQUIRE(t0 < (1LL << 31) && t1 < (1LL << 31) && vt < (1LL << 31), "batch too large for one launch");
+  int rc = launch_h<3>(h0, t0, k0, st);
+  if (rc) return rc;
+  rc = launch_v(vl, vt, vk, st);
+  if (rc) return rc;
+  return launch_h<3>(h1, t1, k1, st);
 }
 
 // One box of se_resize_composite_feather_detail_u8: its result and mask (ih x iw), pasted at ow x oh into canvas `canvas` at (oy, ox).
@@ -625,12 +710,12 @@ static int paste_boxes(const std::vector<PasteBox>& boxes, const std::vector<Pas
   int dev = 0;
   SE_CUDA_OK(cudaGetDevice(&dev));
   {
-    std::vector<std::pair<int, int>> pairs;
+    std::vector<TableKey> keys;
     for (auto& b : boxes) {
-      if (b.iw != b.ow) pairs.emplace_back(b.iw, b.ow);
-      if (b.ih != b.oh) pairs.emplace_back(b.ih, b.oh);
+      if (b.iw != b.ow) keys.push_back(plain_key(b.iw, b.ow));
+      if (b.ih != b.oh) keys.push_back(plain_key(b.ih, b.oh));
     }
-    int rc = reserve_tables(dev, pairs);
+    int rc = reserve_tables(dev, keys);
     if (rc) return rc;
   }
   const int n = (int)boxes.size();
@@ -660,15 +745,15 @@ static int paste_boxes(const std::vector<PasteBox>& boxes, const std::vector<Pas
       if (b.iw != b.ow) {   // the paste reads the horizontal passes' output instead of the result itself
         unsigned char* s3 = (unsigned char*)scratch + mid[order[j]];
         unsigned char* s1 = s3 + scratch_round((size_t)b.ih * b.ow * 3);
-        int rc = add_h_pass(dev, h3, t3, k3, b.rgb, 3LL * b.iw, s3, b.ih, b.iw, b.ow, 0);
+        int rc = add_h_pass(dev, h3, t3, k3, b.rgb, 3LL * b.iw, s3, b.ih, b.iw, (float)b.iw, b.ow, 0);
         if (rc) return rc;
-        rc = add_h_pass(dev, h1, t1, k1, b.mask, b.iw, s1, b.ih, b.iw, b.ow, 0);
+        rc = add_h_pass(dev, h1, t1, k1, b.mask, b.iw, s1, b.ih, b.iw, (float)b.iw, b.ow, 0);
         if (rc) return rc;
         p.rgb = s3;
         p.mask = s1;
       }
       int ksize = 1;
-      int rc = v_table(dev, b.ih, b.oh, &p.bounds, &p.coeffs, &ksize);
+      int rc = v_table(dev, b.ih, (float)b.ih, b.oh, &p.bounds, &p.coeffs, &ksize);
       if (rc) return rc;
       p.ksize = (unsigned short)ksize;
       p.out_h = (unsigned short)b.oh;
@@ -732,7 +817,7 @@ int se_resize_coeffs(int in, int out, int* bounds, int* coeffs, long long cap) {
               " ints (got cap " + std::to_string(cap) + ")");
     return -1;
   }
-  return resize_coeff_table(in, out, bounds, coeffs);
+  return resize_coeff_table(in, (float)in, out, bounds, coeffs);
 }
 
 int se_resize_set_table_cache_limit(long long bytes) {

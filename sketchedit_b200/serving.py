@@ -19,6 +19,7 @@ too (``engine.resize_u8_packed``, bit-identical to Pillow), so a batch is one up
     r = s.edit(mask_pil, region="strokes")            # r.boxes, r.patches: what changed; s.undo() restores it
     p = s.propose(mask_pil, region="strokes")         # p.boxes, p.masks: the edit's region, from netM alone
     r = s.accept(p)                                   # that edit, byte for byte (or accept(p, edit_masks=corrections))
+    preview = s.jpeg(size=(640, 640))                 # Pillow's thumbnail of the photo, made and encoded on the device
     mask = proc.predict_mask(image_pil, mask_pil)     # process_image's returned mask, without the image
     proc.close()
 
@@ -1078,23 +1079,33 @@ class EditSession:
         with self._proc._sessions_mu:
             self._proc._sessions.discard(self)
 
-    def image(self):
-        """The current photo as a PIL RGB image."""
+    def image(self, size=None):
+        """The current photo as a PIL RGB image. ``size = (width, height)`` gives a preview instead: the photo as
+        ``Image.thumbnail(size)`` leaves a copy of it (Pillow 12.2: BICUBIC, reducing_gap=2.0), at most ``size`` and with its
+        aspect ratio kept; a photo that already fits comes back whole. With ``resize='device'`` the preview is made on the
+        device (``engine.thumbnail_u8``) and only it is downloaded."""
         from PIL import Image
+        size = self._size(size)
         with self._mu:
             self._check_open()
             if self._img is not None:
-                return self._img.copy()
+                img = self._host_image(None, size)
+                return img.copy() if img is self._img else img
             with self._proc._torch.cuda.device(self._photo.device):
-                return Image.fromarray(self._photo.cpu().numpy())
+                return Image.fromarray(self._pixels(None, size).cpu().numpy())
 
-    def jpeg(self, quality=75, subsampling=2, box=None, optimize=False, progressive=False):
+    def jpeg(self, quality=75, subsampling=2, box=None, optimize=False, progressive=False, size=None):
         """The current photo, or its PIL box ``(left, upper, right, lower)``, as a JPEG file: the bytes of
 
-            buf = io.BytesIO();  s.image().crop(box).save(buf, "JPEG", quality=quality, subsampling=subsampling,
-                                                          optimize=optimize, progressive=progressive)
+            img = s.image().crop(box);  img.thumbnail(size)
+        buf = io.BytesIO();  img.save(buf, "JPEG", quality=quality, subsampling=subsampling, optimize=optimize,
+                                      progressive=progressive)
 
-        (no crop when ``box`` is None). ``quality`` in [1, 100]; ``subsampling`` 0 (4:4:4) or 2 (4:2:0, Pillow's default);
+        (no crop when ``box`` is None, no thumbnail when ``size`` is None). ``size = (width, height)`` makes a preview:
+        the photo or box scaled down to fit ``size`` as ``Image.thumbnail`` does (Pillow 12.2: BICUBIC, reducing_gap=2.0);
+        one that already fits is encoded whole. On the device the preview is made from the photo where it lies into a
+        small buffer (``engine.thumbnail_u8``, about 6 MB of transient memory for a 4000x2667 photo to 640x427) and
+        encoded there, so the encode's memory follows the preview's size (about 5 MB at 640x427, 4:2:0). ``quality`` in [1, 100]; ``subsampling`` 0 (4:4:4) or 2 (4:2:0, Pillow's default);
         ``optimize`` a bool: True builds Huffman tables for the image, a smaller file of the same pixels. Pillow fails
         (OSError) to write an optimized file larger than its buffer of max(64 KiB, w h) bytes (2 w h from quality 95 on),
         as a noisy photo at quality 90, 4:4:4 can be; the device encode still writes the file, the one Pillow writes
@@ -1110,36 +1121,64 @@ class EditSession:
 
         from . import engine
         quality, subsampling = engine._check_jpeg_args(quality, subsampling, optimize, progressive)
+        size = self._size(size)
         with self._mu:
             self._check_open()
             box = self._box(box)
             if self._img is not None:
-                img = self._img if box is None else self._img.crop(box)
+                img = self._host_image(box, size)
                 buf = io.BytesIO()
                 img.save(buf, "JPEG", quality=quality, subsampling=subsampling, optimize=bool(optimize),
                          progressive=bool(progressive))
                 return buf.getvalue()
-            return engine.jpeg_encode_u8([self._window(box)], quality, subsampling, optimize, progressive)[0]
+            return engine.jpeg_encode_u8([self._pixels(box, size)], quality, subsampling, optimize, progressive)[0]
 
-    def png(self, box=None):
+    def png(self, box=None, size=None):
         """The current photo, or its PIL box ``(left, upper, right, lower)``, as a PNG file: the bytes of
 
-            cv2.imencode(".png", np.array(s.image().crop(box))[:, :, ::-1])[1]
+            img = s.image().crop(box);  img.thumbnail(size)
+            cv2.imencode(".png", np.array(img)[:, :, ::-1])[1]
 
-        (no crop when ``box`` is None), the file ``cv2.imwrite`` writes for the photo. With ``resize='device'`` the photo is
+        (no crop when ``box`` is None, no thumbnail when ``size`` is None), the file ``cv2.imwrite`` writes for the photo;
+        ``size`` makes a preview as in ``jpeg``. With ``resize='device'`` the photo is
         encoded on its device where it lies (``engine.png_encode_u8``) and only the file is downloaded; with ``resize='host'``
         cv2 encodes it. The box's entries are Python or numpy integers, not bools. The device encode holds transient device
         memory of about 2.2 bytes per photo byte (``engine.png_encode_u8``)."""
         from . import engine
+        size = self._size(size)
         with self._mu:
             self._check_open()
             box = self._box(box)
             if self._img is not None:
                 import cv2
                 import numpy as np
-                img = self._img if box is None else self._img.crop(box)
+                img = self._host_image(box, size)
                 return cv2.imencode(".png", np.ascontiguousarray(np.asarray(img)[:, :, ::-1]))[1].tobytes()
-            return engine.png_encode_u8([self._window(box)])[0]
+            return engine.png_encode_u8([self._pixels(box, size)])[0]
+
+    @staticmethod
+    def _size(size):
+        """A preview bound checked: None, or ``(width, height)`` as Python ints."""
+        from . import engine
+        return None if size is None else engine.check_thumbnail_size(size)
+
+    def _host_image(self, box, size):
+        """The host flow's PIL image of ``box`` (the whole photo for None), thumbnailed to ``size`` unless it is None. The
+        thumbnail is made on a copy (``thumbnail`` works in place), so the session's photo is never touched."""
+        img = self._img if box is None else self._img.crop(box)
+        if size is not None:
+            img = img.copy() if img is self._img else img
+            img.thumbnail(size)
+        return img
+
+    def _pixels(self, box, size):
+        """The device flow's pixels of ``box``: the resident photo's window, or when ``size`` is given and the window does
+        not fit it, the window's thumbnail in a new device buffer."""
+        from . import engine
+        win = self._window(box)
+        if size is not None and engine.thumbnail_size(win.shape[1], win.shape[0], size) is not None:
+            win = engine.thumbnail_u8([win], size)[0]
+        return win
 
     def _box(self, box):
         """``box`` checked against the photo, as a tuple of ints (None stays None)."""
