@@ -311,6 +311,32 @@ int se_jpeg_encode_progressive_u8(const unsigned char* const* src, const long lo
  * scans with the largest alphabets, per block the most bits each scan can spend on it (DESIGN.md, section 7b) padded per
  * scan, doubled for the 0x00 after each 0xFF, and EOI. -1 on bad arguments. */
 long long se_jpeg_progressive_max_bytes(int h, int w, int subsampling);
+/* JPEG of n in [0, 32] RGB windows with the caller's quantisation tables, subsampling and APP1 / APP2 segments, byte for
+ * byte what Pillow writes for an RGB image:
+ *     buf = io.BytesIO();  Image.fromarray(img_i).save(buf, "JPEG", qtables=T, subsampling=subsampling, optimize=optimize,
+ *                                                      progressive=progressive, exif=E, icc_profile=I)
+ * and so also src.save(buf, "JPEG", quality="keep", ...) of a JPEG src with T = src.quantization and subsampling
+ * JpegImagePlugin.get_sampling(src) (-1 there is 2 here). qtables holds ntables in [1, 4] tables of 64 entries in [0, 255],
+ * natural order (as Image.quantization gives them); an entry 0 is taken as 1, as libjpeg does, and an entry above 255 (a
+ * 16-bit table, an extended-sequential file) is refused. Pillow's component -> table assignment: one table serves all three
+ * components and one DQT is written; with two, Y uses table 0 and Cb, Cr table 1; with three or four, component c uses
+ * table c and a fourth table is never written. subsampling 0 (4:4:4), 1 (4:2:2: 16x8 MCUs, h2v1 chroma) or 2 (4:2:0).
+ * segments holds segments_len in [0, 2^30] host bytes of back-to-back APP1 (FF E1) / APP2 (FF E2) segments, each with a
+ * length that matches, written after APP0 as Pillow writes its EXIF block and then its ICC_PROFILE chunks (the Python
+ * engine.jpeg_app_segments builds them). progressive = 1 writes se_jpeg_encode_progressive_u8's ten scans whatever optimize
+ * is. The other arguments are those of se_jpeg_encode_opt_u8 and are checked the same way; out + out_off[i] must hold
+ * se_jpeg_tables_max_bytes(h, w, subsampling, ntables, progressive, segments_len) bytes, and the scratch is that of the
+ * quality entries at the same subsampling. The segments are copied into each file on `stream` (from pageable host memory,
+ * so the copy is done with the host bytes when the call returns). The call only enqueues. */
+int se_jpeg_encode_tables_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n,
+                             const unsigned short* qtables, int ntables, int subsampling, int optimize, int progressive,
+                             const unsigned char* segments, long long segments_len, unsigned char* out, const long long* out_off,
+                             long long* out_bytes_dev, void* scratch, long long* scratch_bytes, void* stream);
+/* Host only: a true upper bound of the file se_jpeg_encode_tables_u8 writes for an h x w image: that of
+ * se_jpeg_max_bytes (progressive = 0) or se_jpeg_progressive_max_bytes (1) with the header's min(ntables, 3) DQT segments and
+ * segments_len bytes of APP1 / APP2 segments, and 4:2:2's 4 blocks per 16x8 MCU. Entries >= 1 keep a block within the
+ * quality-100 bound. -1 on bad arguments. */
+long long se_jpeg_tables_max_bytes(int h, int w, int subsampling, int ntables, int progressive, long long segments_len);
 /* PNG of n in [0, 32] windows, byte for byte what OpenCV writes with no parameters (OpenCV 4.13, libpng 1.6, zlib 1.3):
  *     cv2.imencode(".png", img_i)[1]
  * where img_i is the window as BGR (channels 3) or grey (channels 1). Image i is hw[2i] rows of hw[2i+1] pixels of `channels`

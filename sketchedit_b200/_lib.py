@@ -67,6 +67,10 @@ SIGNATURES = {
     "se_jpeg_encode_progressive_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_void_p, _c_void_p,
                                                _c_void_p, _c_void_p, ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
     "se_jpeg_progressive_max_bytes": (ctypes.c_longlong, [_c_int, _c_int, _c_int]),
+    "se_jpeg_encode_tables_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_int, _c_void_p, _c_int, _c_int, _c_int, _c_int,
+                                          _c_void_p, ctypes.c_longlong, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                                          ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
+    "se_jpeg_tables_max_bytes": (ctypes.c_longlong, [_c_int, _c_int, _c_int, _c_int, _c_int, ctypes.c_longlong]),
     "se_png_encode_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                                   ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
     "se_png_max_bytes": (ctypes.c_longlong, [_c_int, _c_int, _c_int]),

@@ -2,19 +2,22 @@
 // for an RGB image without info, s = 0 (4:4:4) or 2 (4:2:0), with libjpeg-turbo's defaults (islow DCT, no smoothing, Annex K
 // Huffman tables, no restart markers). The encoder is integer arithmetic from start to finish, so every byte is libjpeg-turbo's.
 // tests/util_jpeg.py restates each stage in numpy; the comments below name the libjpeg-turbo source a stage follows.
+// se_jpeg_encode_tables_u8 runs the same kernels with the caller's quantisation tables, 4:2:2 besides (h2v1 downsampling,
+// 16x8 MCUs: tests/util_jpeg_keep.py), and APP1 / APP2 segments after APP0, which the host copies into each file.
 //
 // One call encodes up to JPEG_MAX_BATCH windows (rows a pitch apart) in these launches on one stream:
 //   dct:    one thread per 8x8 block: the window's samples with the last row and column repeated, RGB -> YCbCr (jccolor.c),
-//           h2v2 downsampling (jcsample.c), level shift, islow FDCT (jfdctint.c), quantisation by libjpeg-turbo's reciprocals
+//           h2v2 or h2v1 downsampling (jcsample.c), level shift, islow FDCT (jfdctint.c), quantisation by libjpeg-turbo's reciprocals
 //           (jcdctmgr.c); writes the zigzag coefficients, the quantised DC and the block's AC bit count.
-//   bits:   one thread per block: the DC difference and the block's total bit count (a dummy luma block of a 4:2:0 MCU, wholly
-//           outside the image, codes DC difference 0 and EOB, as jccoefct.c makes it).
+//   bits:   one thread per block: the DC difference and the block's total bit count (a dummy luma block of a 4:2:0 or 4:2:2
+//           MCU, wholly outside the image, codes DC difference 0 and EOB, as jccoefct.c makes it).
 //   scan:   exclusive scan of the bit counts (three launches, scan_tiles / scan_sums / scan_add).
 //   pack:   one thread per block writes its Huffman codes at its bit offset into a zeroed 32-bit word stream, merging the words
 //           it shares with its neighbours by atomicOr.
 //   stuff:  per 64-byte chunk of the stream: count its 0xFF bytes, scan the counts, then write the chunk after the header with
 //           0x00 after each 0xFF (the last byte padded with 1-bits); the last chunk writes EOI and the image's byte count.
-//   header: one block per image writes the header, a function of (h, w, quality, subsampling) built on the host.
+//   header: one block per image writes the header, a function of (h, w, tables, subsampling) built on the host, around the
+//           APP1 / APP2 segments the host has copied after APP0.
 // With optimize = 1 (Pillow's optimize=True) se_jpeg_opt.cu counts each image's symbols after the bits kernel, builds its
 // Huffman tables, writes its header and recounts the block bits; pack then codes with the image's tables from scratch and
 // stuff writes the data after the image's header, whose length is on the device.
@@ -98,12 +101,11 @@ struct QuantTab {   // per natural index: q = ((|x| + corr) * recip) >> shift, t
 
 static int quality_scale(int quality) { return quality < 50 ? 5000 / quality : 200 - 2 * quality; }   // jpeg_quality_scaling
 
-static QuantTab quant_tab(const unsigned char* base, int quality) {
+// the quantiser q[i] (natural order, 1..255) and its reciprocal, correction and shift
+static QuantTab quant_tab(const unsigned short* q) {
   QuantTab t{};
-  const int scale = quality_scale(quality);
   for (int i = 0; i < 64; ++i) {
-    const int q = std::min(255, std::max(1, (base[i] * scale + 50) / 100));   // jpeg_add_quant_table, force_baseline
-    const unsigned divisor = 8u * q;                                         // the FDCT output is scaled by 8
+    const unsigned divisor = 8u * q[i];   // the FDCT output is scaled by 8
     int b = 31 - __builtin_clz(divisor);
     int r = 16 + b;
     unsigned fq = (1u << r) / divisor, fr = (1u << r) % divisor, c = divisor / 2;
@@ -115,12 +117,19 @@ static QuantTab quant_tab(const unsigned char* base, int quality) {
     } else {
       ++fq;
     }
-    t.q[i] = (unsigned char)q;
+    t.q[i] = (unsigned char)q[i];
     t.recip[i] = (unsigned short)fq;
     t.corr[i] = (unsigned short)c;
     t.shift[i] = (unsigned char)r;
   }
   return t;
+}
+
+static QuantTab quant_tab(const unsigned char* base, int quality) {
+  const int scale = quality_scale(quality);
+  unsigned short q[64];
+  for (int i = 0; i < 64; ++i) q[i] = (unsigned short)std::min(255, std::max(1, (base[i] * scale + 50) / 100));   // force_baseline
+  return quant_tab(q);
 }
 
 // the luma and chroma tables of one quality, built once per quality
@@ -150,17 +159,23 @@ static void put_dht(std::vector<unsigned char>& v, int cls_id, const HuffSpec& s
   v.insert(v.end(), s.syms, s.syms + s.nsym);
 }
 
-// SOI, JFIF APP0 1.01 (density 1:1, units 0), DQT 0 and 1 (zigzag order), SOF0, DHT DC0 AC0 DC1 AC1, SOS (jcmarker.c)
-static std::vector<unsigned char> jpeg_header(int h, int w, const QuantTab* qt, int subsampling) {
+// Pillow's table of component c when the call has nq DQT segments (JpegEncode.c): one table serves all, two split luma and
+// chroma, three give each component its own
+static int comp_table(int nq, int c) { return std::min(c, nq - 1); }
+
+// SOI, JFIF APP0 1.01 (density 1:1, units 0), DQT 0 .. nq - 1 (zigzag order), SOF0, DHT DC0 AC0 DC1 AC1, SOS (jcmarker.c)
+static std::vector<unsigned char> jpeg_header(int h, int w, const QuantTab* qt, int nq, int subsampling) {
   std::vector<unsigned char> v = {0xFF, 0xD8, 0xFF, 0xE0, 0, 16, 'J', 'F', 'I', 'F', 0, 1, 1, 0, 0, 1, 0, 1, 0, 0};
-  for (int t = 0; t < 2; ++t) {
+  for (int t = 0; t < nq; ++t) {
     v.insert(v.end(), {0xFF, 0xDB, 0, 67, (unsigned char)t});
     for (int k = 0; k < 64; ++k) v.push_back(qt[t].q[kZigzag[k]]);
   }
   v.insert(v.end(), {0xFF, 0xC0, 0, 17, 8});
   put16(v, h);
   put16(v, w);
-  v.insert(v.end(), {3, 1, (unsigned char)(subsampling == 2 ? 0x22 : 0x11), 0, 2, 0x11, 1, 3, 0x11, 1});
+  const unsigned char y = subsampling == 2 ? 0x22 : subsampling == 1 ? 0x21 : 0x11;
+  v.insert(v.end(), {3, 1, y, (unsigned char)comp_table(nq, 0), 2, 0x11, (unsigned char)comp_table(nq, 1), 3, 0x11,
+                     (unsigned char)comp_table(nq, 2)});
   put_dht(v, 0x00, kDcLuma);
   put_dht(v, 0x10, kAcLuma);
   put_dht(v, 0x01, kDcChroma);
@@ -169,10 +184,13 @@ static std::vector<unsigned char> jpeg_header(int h, int w, const QuantTab* qt, 
   return v;
 }
 
-long long jpeg_max_bytes(int h, int w, int subsampling) {
-  const long long m = subsampling == 2 ? 16 : 8;
-  const long long blocks = ((h + m - 1) / m) * ((w + m - 1) / m) * (subsampling == 2 ? 6 : 3);
-  return JPEG_HEADER_BYTES + 2 * (blocks * (JPEG_MAX_BLOCK_BITS / 8)) + 2;
+static long long image_blocks(int h, int w, int sub) {
+  const int mh = mcu_h(sub), mw = mcu_w(sub);
+  return (long long)((h + mh - 1) / mh) * ((w + mw - 1) / mw) * mcu_blocks(sub);
+}
+
+long long jpeg_max_bytes(int h, int w, int subsampling, long long header_bytes) {
+  return header_bytes + 2 * (image_blocks(h, w, subsampling) * (JPEG_MAX_BLOCK_BITS / 8)) + 2;
 }
 
 // ------------------------------------------------------------------------------------------ kernels
@@ -180,9 +198,10 @@ constexpr int kWordsPerBlock = JPEG_MAX_BLOCK_BITS / 32;
 constexpr int kChunkBytes = 64;   // bytes of the stream per stuffing thread
 constexpr int kThreads = 128;
 
-struct JpegQuant {
-  unsigned short recip[2][64], corr[2][64];
-  unsigned char shift[2][64];
+struct JpegQuant {   // the call's tables, and each component's table: components sharing a table read the same words
+  unsigned short recip[3][64], corr[3][64];
+  unsigned char shift[3][64];
+  unsigned char tq[3];
 };
 static_assert(sizeof(JpegList) + sizeof(JpegQuant) <= 4096, "descriptors must fit the kernel parameter space");
 
@@ -265,6 +284,17 @@ __global__ void __launch_bounds__(kThreads) jpeg_dct_kernel(const __grid_constan
         v[r * 8 + c] = ((s + 1 + (c & 1)) >> 2) - 128;
       }
     }
+  } else if (L.sub == 1 && b.comp) {   // h2v1: columns repeated to the MCU width, rows to the block grid
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+      const unsigned char* row = d.src + (size_t)min(b.by * 8 + r, d.h - 1) * d.pitch;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        const int x0 = min(b.bx * 16 + 2 * c, d.w - 1) * 3, x1 = min(b.bx * 16 + 2 * c + 1, d.w - 1) * 3;
+        const int s = color(b.comp, row[x0], row[x0 + 1], row[x0 + 2]) + color(b.comp, row[x1], row[x1 + 1], row[x1 + 2]);
+        v[r * 8 + c] = ((s + (c & 1)) >> 1) - 128;
+      }
+    }
   } else {
 #pragma unroll
     for (int r = 0; r < 8; ++r) {
@@ -280,8 +310,8 @@ __global__ void __launch_bounds__(kThreads) jpeg_dct_kernel(const __grid_constan
   for (int r = 0; r < 8; ++r) fdct8(v, r * 8, 1, true);
 #pragma unroll
   for (int c = 0; c < 8; ++c) fdct8(v, c, 8, false);
-  const int t = b.comp ? 1 : 0;
-  const HuffCodes& ac = sh_ac[t];
+  const int t = Q.tq[b.comp];
+  const HuffCodes& ac = sh_ac[b.comp ? 1 : 0];
   unsigned bits = 0;
   int run = 0;
   for_each_zigzag(
@@ -389,7 +419,7 @@ __global__ void __launch_bounds__(kThreads) jpeg_stuff_kernel(const __grid_const
     return;
   }
   if (j0 >= nbytes) return;
-  unsigned char* o = d.out + (S.hdr_len ? S.hdr_len[i] : JPEG_HEADER_BYTES) + j0 + (S.ffoff[g] - S.ffoff[d.chunk0]);
+  unsigned char* o = d.out + (S.hdr_len ? S.hdr_len[i] : L.hdr) + j0 + (S.ffoff[g] - S.ffoff[d.chunk0]);
   for (long long j = j0; j < j1; ++j) {
     const unsigned v = stream_byte(w, j, nbits);
     *o++ = (unsigned char)v;
@@ -404,7 +434,7 @@ __global__ void __launch_bounds__(kThreads) jpeg_stuff_kernel(const __grid_const
 
 __global__ void __launch_bounds__(kThreads) jpeg_header_kernel(const __grid_constant__ HeaderList H) {
   unsigned char* o = H.out[blockIdx.x];
-  for (int j = threadIdx.x; j < JPEG_HEADER_BYTES; j += kThreads) o[j] = header_byte(H, blockIdx.x, j);
+  for (int j = threadIdx.x; j < H.len; j += kThreads) o[header_at(H, j)] = header_byte(H, blockIdx.x, j);
 }
 
 // ------------------------------------------------------------------------------------------ host
@@ -414,10 +444,6 @@ struct JpegLayout {   // the call's block, word and chunk counts and where its a
          hdr_len = 0, prog = 0, total = 0;
 };
 
-static long long image_blocks(int h, int w, int sub) {
-  const int m = sub == 2 ? 16 : 8;
-  return (long long)((h + m - 1) / m) * ((w + m - 1) / m) * (sub == 2 ? 6 : 3);
-}
 static long long chunks_of(long long blocks) { return (blocks * kWordsPerBlock * 4 + kChunkBytes - 1) / kChunkBytes; }
 
 // progressive: the coefficients and the dct kernel's bit counts, then se_jpeg_prog.cu's arrays of `prog` bytes
@@ -457,6 +483,49 @@ static JpegLayout jpeg_layout(const int* hw, int n, int sub, bool optimize, bool
   return l;
 }
 
+// What a call writes besides the pixels: its DQT tables, subsampling and APP1 / APP2 segments
+struct JpegFormat {
+  QuantTab qt[3];                        // DQT tables 0 .. nq - 1
+  int nq = 2, sub = 2;
+  const unsigned char* meta = nullptr;   // host bytes of the segments, written after APP0
+  long long meta_len = 0;
+};
+
+// the format of the quality entries: the Annex K tables at `quality`, no segments
+static JpegFormat quality_format(int quality, int subsampling) {
+  JpegFormat F;
+  const QuantTab* qt = quant_tabs(quality);
+  F.qt[0] = qt[0];
+  F.qt[1] = qt[1];
+  F.sub = subsampling;
+  return F;
+}
+
+constexpr long long kMaxMeta = 1LL << 30;   // APP1 / APP2 bytes a call takes
+
+// se_jpeg_encode_tables_u8's check of its segments: each one FF E1 or FF E2 with a length that matches, back to back
+static int check_segments(const unsigned char* seg, long long len) {
+  SE_REQUIRE(len >= 0 && len <= kMaxMeta, "segments_len must be in [0, 2^30]");
+  SE_REQUIRE(len == 0 || seg != nullptr, "null segments");
+  for (long long at = 0; at < len;) {
+    SE_REQUIRE(len - at >= 4, "segment at byte " + std::to_string(at) + " is cut short");
+    SE_REQUIRE(seg[at] == 0xFF && (seg[at + 1] == 0xE1 || seg[at + 1] == 0xE2),
+               "segment at byte " + std::to_string(at) + " is not an APP1 (FF E1) or APP2 (FF E2) marker");
+    const int n = seg[at + 2] << 8 | seg[at + 3];
+    SE_REQUIRE(n >= 2 && n <= len - at - 2, "segment at byte " + std::to_string(at) + " has length " + std::to_string(n) +
+                                                " and " + std::to_string(len - at - 2) + " bytes after its marker");
+    at += 2 + n;
+  }
+  return 0;
+}
+
+// the table count, entries and subsampling of se_jpeg_encode_tables_u8 and its bound
+static int check_tables_format(int ntables, int subsampling) {
+  SE_REQUIRE(ntables >= 1 && ntables <= 4, "ntables must be in [1, 4]");
+  SE_REQUIRE(subsampling >= 0 && subsampling <= 2, "subsampling must be 0 (4:4:4), 1 (4:2:2) or 2 (4:2:0)");
+  return 0;
+}
+
 }  // namespace se
 
 using namespace se;
@@ -479,22 +548,34 @@ long long se_jpeg_progressive_max_bytes(int h, int w, int subsampling) {
   return jpeg_prog_max_bytes(h, w, subsampling);
 }
 
+long long se_jpeg_tables_max_bytes(int h, int w, int subsampling, int ntables, int progressive, long long segments_len) {
+  if (h < 1 || w < 1 || h > kMaxDim || w > kMaxDim || subsampling < 0 || subsampling > 2 || ntables < 1 || ntables > 4 ||
+      (progressive != 0 && progressive != 1) || segments_len < 0 || segments_len > kMaxMeta) {
+    set_error("se_jpeg_tables_max_bytes: sizes must be in [1, 65535], subsampling 0, 1 or 2, ntables in [1, 4], progressive 0 "
+              "or 1 and segments_len in [0, 2^30]");
+    return -1;
+  }
+  const int nq = std::min(ntables, 3);
+  return progressive ? jpeg_prog_max_bytes(h, w, subsampling, jpeg_sof_end(nq, segments_len))
+                     : jpeg_max_bytes(h, w, subsampling, jpeg_header_bytes(nq, segments_len));
+}
+
 }  // extern "C"
 
 namespace se {
 
-// se_jpeg_encode_opt_u8 (progressive = false) and se_jpeg_encode_progressive_u8 (true, optimize = 0)
-static int jpeg_encode(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality,
-                       int subsampling, int optimize, bool progressive, unsigned char* out, const long long* out_off,
-                       long long* out_bytes_dev, void* scratch, long long* scratch_bytes, void* stream) {
+// every entry: the quality entries (progressive = false, or true with optimize = 0) and se_jpeg_encode_tables_u8, whose
+// format F is checked by the caller
+static int jpeg_encode(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, const JpegFormat& F,
+                       int optimize, bool progressive, unsigned char* out, const long long* out_off, long long* out_bytes_dev,
+                       void* scratch, long long* scratch_bytes, void* stream) {
   SE_REQUIRE(n >= 0 && n <= JPEG_MAX_BATCH, "n must be in [0, " + std::to_string(JPEG_MAX_BATCH) + "] images per call");
-  SE_REQUIRE(quality >= 1 && quality <= 100, "quality must be in [1, 100]");
-  SE_REQUIRE(subsampling == 0 || subsampling == 2, "subsampling must be 0 (4:4:4) or 2 (4:2:0)");
   SE_REQUIRE(optimize == 0 || optimize == 1, "optimize must be 0 or 1");
   SE_REQUIRE(scratch_bytes != nullptr, "scratch_bytes");
   SE_REQUIRE(n == 0 || (src_pitch && hw && out_off), "null size / offset array");
   for (int i = 0; i < n; ++i)
     if (int rc = check_window(i, hw[2 * i], hw[2 * i + 1], src_pitch[i], 3LL * hw[2 * i + 1], out_off[i])) return rc;
+  const int subsampling = F.sub;
   JpegList L;
   ProgList P;
   ProgScratch PS;
@@ -516,20 +597,25 @@ static int jpeg_encode(const unsigned char* const* src, const long long* src_pit
   SE_REQUIRE(P.slots < (1LL << 31) * kThreads && P.chunks < (1LL << 31) * kThreads, "batch too large for one launch");
   cudaStream_t st = (cudaStream_t)stream;
 
-  const QuantTab* qt = quant_tabs(quality);
   JpegQuant Q;
-  for (int t = 0; t < 2; ++t) {
-    memcpy(Q.recip[t], qt[t].recip, sizeof(Q.recip[t]));
-    memcpy(Q.corr[t], qt[t].corr, sizeof(Q.corr[t]));
-    memcpy(Q.shift[t], qt[t].shift, sizeof(Q.shift[t]));
+  memset(&Q, 0, sizeof(Q));
+  for (int t = 0; t < F.nq; ++t) {
+    memcpy(Q.recip[t], F.qt[t].recip, sizeof(Q.recip[t]));
+    memcpy(Q.corr[t], F.qt[t].corr, sizeof(Q.corr[t]));
+    memcpy(Q.shift[t], F.qt[t].shift, sizeof(Q.shift[t]));
   }
+  for (int c = 0; c < 3; ++c) Q.tq[c] = (unsigned char)comp_table(F.nq, c);
   HeaderList H;
   memset(&H, 0, sizeof(H));
-  const std::vector<unsigned char> hdr = jpeg_header(1, 1, qt, subsampling);
-  memcpy(H.bytes, hdr.data(), JPEG_HEADER_BYTES);
+  const std::vector<unsigned char> hdr = jpeg_header(1, 1, F.qt, F.nq, subsampling);
+  memcpy(H.bytes, hdr.data(), hdr.size());
+  H.len = (int)hdr.size();
+  H.sof_end = jpeg_sof_end(F.nq, 0);
+  H.meta = (int)F.meta_len;
+  L.hdr = H.len + H.meta;
   long long blk = 0, word = 0, chunk = 0;
   for (int i = 0; i < n; ++i) {
-    const int h = hw[2 * i], w = hw[2 * i + 1], m = subsampling == 2 ? 16 : 8;
+    const int h = hw[2 * i], w = hw[2 * i + 1], m = mcu_w(subsampling);
     JImg& d = L.im[i];
     d.src = src[i];
     d.out = out + out_off[i];
@@ -548,6 +634,9 @@ static int jpeg_encode(const unsigned char* const* src, const long long* src_pit
     H.out[i] = d.out;
     H.hw[i][0] = (unsigned short)h;
     H.hw[i][1] = (unsigned short)w;
+    // the segments go straight into each file after APP0; the header kernels write around them
+    if (F.meta_len)
+      SE_CUDA_OK(cudaMemcpyAsync(d.out + JPEG_APP0_END, F.meta, (size_t)F.meta_len, cudaMemcpyHostToDevice, st));
   }
   L.blocks = blk;
   L.chunks = chunk;
@@ -595,6 +684,13 @@ static int jpeg_encode(const unsigned char* const* src, const long long* src_pit
   return 0;
 }
 
+// the quality entries' checks of quality and subsampling
+static int check_quality(int quality, int subsampling) {
+  SE_REQUIRE(quality >= 1 && quality <= 100, "quality must be in [1, 100]");
+  SE_REQUIRE(subsampling == 0 || subsampling == 2, "subsampling must be 0 (4:4:4) or 2 (4:2:0)");
+  return 0;
+}
+
 }  // namespace se
 
 extern "C" {
@@ -602,15 +698,17 @@ extern "C" {
 int se_jpeg_encode_opt_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality,
                           int subsampling, int optimize, unsigned char* out, const long long* out_off, long long* out_bytes_dev,
                           void* scratch, long long* scratch_bytes, void* stream) {
-  return jpeg_encode(src, src_pitch, hw, n, quality, subsampling, optimize, false, out, out_off, out_bytes_dev, scratch,
-                     scratch_bytes, stream);
+  if (int rc = check_quality(quality, subsampling)) return rc;
+  return jpeg_encode(src, src_pitch, hw, n, quality_format(quality, subsampling), optimize, false, out, out_off, out_bytes_dev,
+                     scratch, scratch_bytes, stream);
 }
 
 int se_jpeg_encode_progressive_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n,
                                   int quality, int subsampling, unsigned char* out, const long long* out_off,
                                   long long* out_bytes_dev, void* scratch, long long* scratch_bytes, void* stream) {
-  return jpeg_encode(src, src_pitch, hw, n, quality, subsampling, 0, true, out, out_off, out_bytes_dev, scratch, scratch_bytes,
-                     stream);
+  if (int rc = check_quality(quality, subsampling)) return rc;
+  return jpeg_encode(src, src_pitch, hw, n, quality_format(quality, subsampling), 0, true, out, out_off, out_bytes_dev,
+                     scratch, scratch_bytes, stream);
 }
 
 int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n, int quality, int subsampling,
@@ -618,6 +716,32 @@ int se_jpeg_encode_u8(const unsigned char* const* src, const long long* src_pitc
                       void* stream) {
   return se_jpeg_encode_opt_u8(src, src_pitch, hw, n, quality, subsampling, 0, out, out_off, out_bytes_dev, scratch, scratch_bytes,
                                stream);
+}
+
+int se_jpeg_encode_tables_u8(const unsigned char* const* src, const long long* src_pitch, const int* hw, int n,
+                             const unsigned short* qtables, int ntables, int subsampling, int optimize, int progressive,
+                             const unsigned char* segments, long long segments_len, unsigned char* out, const long long* out_off,
+                             long long* out_bytes_dev, void* scratch, long long* scratch_bytes, void* stream) {
+  if (int rc = check_tables_format(ntables, subsampling)) return rc;
+  SE_REQUIRE(qtables != nullptr, "null qtables");
+  SE_REQUIRE(progressive == 0 || progressive == 1, "progressive must be 0 or 1");
+  SE_REQUIRE(optimize == 0 || optimize == 1, "optimize must be 0 or 1");
+  for (int k = 0; k < 64 * ntables; ++k)
+    SE_REQUIRE(qtables[k] <= 255, "table " + std::to_string(k / 64) + " entry " + std::to_string(k % 64) + " is " +
+                                      std::to_string(qtables[k]) + ": entries must be in [0, 255] (8-bit baseline tables)");
+  if (int rc = check_segments(segments, segments_len)) return rc;
+  JpegFormat F;
+  F.nq = std::min(ntables, 3);
+  for (int t = 0; t < F.nq; ++t) {
+    unsigned short q[64];
+    for (int k = 0; k < 64; ++k) q[k] = std::max<unsigned short>(1, qtables[64 * t + k]);   // jpeg_add_quant_table at scale 100
+    F.qt[t] = quant_tab(q);
+  }
+  F.sub = subsampling;
+  F.meta = segments;
+  F.meta_len = segments_len;
+  return jpeg_encode(src, src_pitch, hw, n, F, progressive ? 0 : optimize, progressive, out, out_off, out_bytes_dev, scratch,
+                     scratch_bytes, stream);
 }
 
 }  // extern "C"

@@ -1,20 +1,37 @@
 // Baseline JPEG encoding of uint8 RGB windows on the GPU (se_jpeg.cu), byte for byte what PIL.Image.save(buf, "JPEG",
-// quality=q, subsampling=s[, optimize=True]) writes with libjpeg-turbo for s = 0 (4:4:4) and s = 2 (4:2:0). The optimal
-// Huffman tables of optimize=True are built by the kernels of se_jpeg_opt.cu.
+// quality=q, subsampling=s[, optimize=True]) writes with libjpeg-turbo for s = 0 (4:4:4) and s = 2 (4:2:0), and what
+// save(buf, "JPEG", qtables=T, subsampling=s, exif=E, icc_profile=I) writes for 1 to 4 8-bit tables T and s = 0, 1 (4:2:2)
+// or 2 (se_jpeg_encode_tables_u8). The optimal Huffman tables of optimize=True are built by the kernels of se_jpeg_opt.cu.
 #pragma once
 #include "se_common.cuh"
 
 namespace se {
 
 constexpr int JPEG_MAX_BATCH = 32;          // images per call: their descriptors travel as kernel parameters
-constexpr int JPEG_HEADER_BYTES = 623;      // SOI, APP0, 2 DQT, SOF0, 4 DHT, SOS
+constexpr int JPEG_HEADER_BYTES = 623;      // SOI, APP0, 2 DQT, SOF0, 4 DHT, SOS: the header of the quality entries
+constexpr int JPEG_HEADER_MAX = 692;        // ... with 3 DQT, the most a call writes besides its APP1 / APP2 segments
 constexpr int JPEG_MAX_BLOCK_BITS = 1664;   // 64 x (16-bit code + 10 value bits) >= DC (<= 16 + 11) + 63 AC (see DESIGN §7b)
-constexpr int JPEG_SOF_END = 177;           // header bytes before the first DHT: SOI, APP0, 2 DQT, SOF0
+constexpr int JPEG_APP0_END = 20;           // SOI and the JFIF APP0; a call's APP1 / APP2 segments follow
 constexpr int JPEG_SOS_BYTES = 14;          // the SOS segment that ends the header
-constexpr int kSofHeightAt = 163;           // byte offsets of SOF0's height and width in the header
+constexpr int JPEG_DHT_BYTES = 432;         // the four Annex K DHT segments
 
-// se_jpeg_max_bytes without the checks: the header, JPEG_MAX_BLOCK_BITS per block doubled for 0xFF stuffing, and EOI
-long long jpeg_max_bytes(int h, int w, int subsampling);
+// header bytes of a call with nq DQT segments and meta bytes of APP1 / APP2 segments: through SOF0, and in all
+__host__ __device__ constexpr int jpeg_sof_end(int nq, long long meta) { return (int)(JPEG_APP0_END + meta) + 69 * nq + 19; }
+__host__ __device__ constexpr long long jpeg_header_bytes(int nq, long long meta) {
+  return jpeg_sof_end(nq, meta) + JPEG_DHT_BYTES + JPEG_SOS_BYTES;
+}
+static_assert(jpeg_header_bytes(2, 0) == JPEG_HEADER_BYTES && jpeg_header_bytes(3, 0) == JPEG_HEADER_MAX, "header layout");
+
+// MCU geometry of a subsampling 0 (4:4:4, 8x8: Y Cb Cr), 1 (4:2:2, 16x8: Y0 Y1 Cb Cr) or 2 (4:2:0, 16x16: Y0..Y3 Cb Cr)
+__host__ __device__ __forceinline__ int mcu_blocks(int sub) { return sub == 2 ? 6 : sub == 1 ? 4 : 3; }
+__host__ __device__ __forceinline__ int mcu_w(int sub) { return sub ? 16 : 8; }
+__host__ __device__ __forceinline__ int mcu_h(int sub) { return sub == 2 ? 16 : 8; }
+// block e's MCU, e / mcu_blocks(sub), as divisions by constants (a 64-bit division by a variable is a long subroutine)
+__host__ __device__ __forceinline__ long long mcu_of(int sub, long long e) { return sub == 2 ? e / 6 : sub == 1 ? e / 4 : e / 3; }
+
+// se_jpeg_max_bytes without the checks: the header (header_bytes of them), JPEG_MAX_BLOCK_BITS per block doubled for 0xFF
+// stuffing, and EOI
+long long jpeg_max_bytes(int h, int w, int subsampling, long long header_bytes = JPEG_HEADER_BYTES);
 
 struct HuffCodes {   // symbol -> canonical code and its length (0: not in the table)
   unsigned short code[256];
@@ -40,7 +57,8 @@ struct JImg {   // one image of a call; block, word and chunk indices are the ca
 };
 struct JpegList {
   JImg im[JPEG_MAX_BATCH];
-  int n, sub;   // images; subsampling (0 or 2)
+  int n, sub;   // images; subsampling (0, 1 or 2)
+  int hdr;      // header bytes of each file (baseline Annex K tables)
   long long blocks, chunks;
 };
 
@@ -53,47 +71,54 @@ struct JpegScratch {   // the call's scratch arrays
   unsigned* ffcnt;             // [chunks]
   unsigned long long* ffoff;   // [chunks], exclusive scan of ffcnt over the call
   unsigned long long* sums;    // scan tile sums
-  // optimize only, else null: the Annex K tables and the 623-byte header are used
+  // optimize only, else null: the Annex K Huffman tables and the header of L.hdr bytes are used
   unsigned long long* hist;    // [n][4][256] symbol counts per image and table
   JpegTables* tabs;            // [n] optimal tables
   int* hdr_len;                // [n] header bytes, where the entropy-coded data starts
 };
 
+// The call's header without its APP1 / APP2 segments, for a 1x1 image: SOI, APP0, the DQTs, SOF0, the DHTs, SOS. In a file
+// the segments (meta bytes, copied there by the host entry) follow APP0, so byte j >= JPEG_APP0_END lies at j + meta.
 struct HeaderList {
-  unsigned char bytes[JPEG_HEADER_BYTES];   // the Annex K header of a 1x1 image at the call's quality and subsampling
+  unsigned char bytes[JPEG_HEADER_MAX];
+  int len, sof_end, meta;   // bytes used; those through SOF0; the APP1 / APP2 bytes after APP0 in the file
   unsigned char* out[JPEG_MAX_BATCH];
   unsigned short hw[JPEG_MAX_BATCH][2];
 };
 static_assert(sizeof(HeaderList) <= 4096, "header descriptors must fit the kernel parameter space");
 
-// header byte j of image i (j < JPEG_SOF_END, or of SOS) with its height and width in SOF0
+// header byte j of image i (j < H.sof_end, or of SOS) with its height and width in SOF0
 __host__ __device__ __forceinline__ unsigned char header_byte(const HeaderList& H, int i, int j) {
-  if (j >= kSofHeightAt && j < kSofHeightAt + 4) {
-    const int x = H.hw[i][(j - kSofHeightAt) >> 1];
-    return (unsigned char)((j - kSofHeightAt) & 1 ? x : x >> 8);
+  const int at = H.sof_end - 14;   // SOF0's height and width
+  if (j >= at && j < at + 4) {
+    const int x = H.hw[i][(j - at) >> 1];
+    return (unsigned char)((j - at) & 1 ? x : x >> 8);
   }
   return H.bytes[j];
 }
+// where header byte j goes in the file
+__host__ __device__ __forceinline__ long long header_at(const HeaderList& H, int j) { return j < JPEG_APP0_END ? j : j + H.meta; }
 
 #ifdef __CUDACC__
 // Block e of an image in scan order: its component (0 Y, 1 Cb, 2 Cr) and block column / row in that component's plane.
-// A 4:2:0 MCU holds luma blocks (0,0), (0,1), (1,0), (1,1), then Cb and Cr; a 4:4:4 MCU holds Y, Cb, Cr.
+// A 4:2:0 MCU holds luma blocks (0,0), (0,1), (1,0), (1,1), then Cb and Cr; a 4:2:2 MCU luma blocks (0,0), (0,1), then Cb
+// and Cr; a 4:4:4 MCU holds Y, Cb, Cr.
 struct BlockAt {
   int comp, bx, by;
-  bool dummy;   // a 4:2:0 luma block wholly outside the image
+  bool dummy;   // a 4:2:0 or 4:2:2 luma block wholly outside the image
 };
 __device__ __forceinline__ BlockAt block_at(const JImg& d, int sub, long long e) {
-  const int per = sub == 2 ? 6 : 3;
-  const long long mcu = e / per;
+  const int per = mcu_blocks(sub), nl = per - 2;
+  const long long mcu = mcu_of(sub, e);
   const int k = (int)(e - mcu * per), mx = (int)(mcu % d.mcu_x), my = (int)(mcu / d.mcu_x);
   BlockAt b;
-  if (sub == 2 && k < 4) {
+  if (sub && k < nl) {
     b.comp = 0;
     b.bx = 2 * mx + (k & 1);
-    b.by = 2 * my + (k >> 1);
+    b.by = (sub == 2 ? 2 : 1) * my + (k >> 1);
     b.dummy = b.bx * 8 >= d.w || b.by * 8 >= d.h;
   } else {
-    b.comp = sub == 2 ? k - 3 : k;
+    b.comp = k - nl + 1;
     b.bx = mx;
     b.by = my;
     b.dummy = false;
@@ -111,10 +136,10 @@ __device__ __forceinline__ int dc_of(const JImg& d, int sub, const short* dc, lo
 }
 
 __device__ __forceinline__ long long prev_same_comp(int sub, long long e) {   // -1: the component's first block
-  const int per = sub == 2 ? 6 : 3;
-  const int k = (int)(e % per);
-  if (sub == 2 && k > 0 && k < 4) return e - 1;
-  return e - (sub == 2 && k == 0 ? 3 : per);
+  const int per = mcu_blocks(sub), nl = per - 2;
+  const int k = (int)(e - mcu_of(sub, e) * per);
+  if (k > 0 && k < nl) return e - 1;
+  return e - (k == 0 ? per - nl + 1 : per);
 }
 
 // appends len <= 32 bits to a 64-bit accumulator holding n < 32 bits; full words go to w[*wi] by atomicOr
@@ -184,8 +209,8 @@ struct ProgScratch {
 // The call's slot, word and chunk layout into P (images' sizes from L) and, with base != null, S's arrays at base; returns
 // the scratch bytes. S.coef is the caller's.
 size_t jpeg_prog_layout(const JpegList& L, unsigned char* base, ProgList* P, ProgScratch* S);
-// a true bound of the progressive file of an h x w image (DESIGN §7b)
-long long jpeg_prog_max_bytes(int h, int w, int subsampling);
+// a true bound of the progressive file of an h x w image whose header through SOF2 is sof_end bytes (DESIGN §7b)
+long long jpeg_prog_max_bytes(int h, int w, int subsampling, int sof_end = jpeg_sof_end(2, 0));
 // Enqueues the progressive coder on `st` after se_jpeg.cu's dct kernel: writes each image's file and byte count.
 int jpeg_progressive(const JpegList& L, const HeaderList& H, const ProgList& P, const ProgScratch& S, cudaStream_t st);
 

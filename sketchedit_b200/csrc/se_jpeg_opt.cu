@@ -3,12 +3,13 @@
 // each step in numpy. After se_jpeg.cu's dct and bits kernels have left the quantised coefficients and DC differences in
 // scratch, per call:
 //   hist:   one thread per 8x8 block counts the symbols the block codes (DC category, AC run/size, ZRL, EOB; a dummy luma
-//           block of a 4:2:0 MCU codes DC 0 and EOB) into its image's four 256-bin histograms: a CTA counts its first image's
+//           block of a 4:2:0 or 4:2:2 MCU codes DC 0 and EOB) into its image's four 256-bin histograms: a CTA counts its first image's
 //           blocks in shared memory and adds them to global memory once, and any other image's straight to global memory.
 //   tables: one warp per (image, table), or per (image, scan, table) for se_jpeg_prog.cu, runs ITU T.81 Annex K.2 with
 //           libjpeg's tie rule, limits the lengths to 16 bits (Annex K.3), drops the reserved code and lists the symbols;
 //           writes the codes and the DHT contents.
-//   header: one CTA per image writes SOI..SOF0, the four DHT segments of its tables and SOS, and the header's length.
+//   header: one CTA per image writes SOI..SOF0 around the APP1 / APP2 segments the host copied there, the four DHT segments
+//           of its tables and SOS, and the header's length.
 //   bits:   one thread per block, its bit count with the image's tables (replacing the Annex K count).
 // se_jpeg.cu's scan, pack and stuff kernels then read the tables and the header length from scratch. The counts are
 // integers, so every launch order gives the same tables.
@@ -184,17 +185,17 @@ __global__ void __launch_bounds__(kThreads) jpeg_opt_header_kernel(const __grid_
   const int i = blockIdx.x;
   const JpegTables& T = S.tabs[i];
   unsigned char* o = H.out[i];
-  int seg[5];   // where each DHT segment starts, then SOS
-  seg[0] = JPEG_SOF_END;
+  int seg[5];   // where each DHT segment starts, then SOS (header bytes without the APP1 / APP2 segments)
+  seg[0] = H.sof_end;
 #pragma unroll
   for (int k = 0; k < 4; ++k) seg[k + 1] = seg[k] + 2 + 2 + 1 + 16 + T.nsym[dht_table(k)];
   const int len = seg[4] + JPEG_SOS_BYTES;
   for (int j = threadIdx.x; j < len; j += kThreads) {
     unsigned char v;
-    if (j < JPEG_SOF_END) {
+    if (j < H.sof_end) {
       v = header_byte(H, i, j);
     } else if (j >= seg[4]) {
-      v = H.bytes[JPEG_HEADER_BYTES - JPEG_SOS_BYTES + (j - seg[4])];
+      v = H.bytes[H.len - JPEG_SOS_BYTES + (j - seg[4])];
     } else {
       int k = 0;
       while (j >= seg[k + 1]) ++k;
@@ -202,9 +203,9 @@ __global__ void __launch_bounds__(kThreads) jpeg_opt_header_kernel(const __grid_
       v = r == 0 ? 0xFF : r == 1 ? 0xC4 : r == 2 ? n >> 8 : r == 3 ? n & 0xFF : r == 4 ? dht_class_id(k)
         : r < 21 ? T.counts[t][r - 5] : T.syms[t][r - 21];
     }
-    o[j] = v;
+    o[header_at(H, j)] = v;
   }
-  if (threadIdx.x == 0) S.hdr_len[i] = len;
+  if (threadIdx.x == 0) S.hdr_len[i] = len + H.meta;
 }
 
 __global__ void __launch_bounds__(kThreads) jpeg_opt_bits_kernel(const __grid_constant__ JpegList L, JpegScratch S) {

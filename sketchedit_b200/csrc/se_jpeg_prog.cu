@@ -32,7 +32,6 @@ constexpr int kChunkBytes = 64;
 constexpr int kMaxRun = 0x7FFF;                 // jcphuff.c forces an EOB run out at this length
 constexpr int kCorrLimit = 1000 - 64 + 1;       // ... and once more than MAX_CORR_BITS - DCTSIZE2 + 1 correction bits wait
 constexpr unsigned char kT = 0x80, kN = 0x40;   // slot flags
-constexpr int kSofMarkerAt = 159;               // SOF0's marker byte in se_jpeg.cu's header, 0xC2 here
 static_assert(sizeof(JpegList) + sizeof(ProgList) + sizeof(ProgScratch) <= 4096, "descriptors must fit the kernel parameter space");
 static_assert(sizeof(HeaderList) + sizeof(ProgList) + sizeof(ProgScratch) <= 4096, "descriptors must fit the kernel parameter space");
 
@@ -59,10 +58,10 @@ __host__ __device__ __forceinline__ ScanDef scan_def(int s) {
 // the slots of scan s: every block of every MCU for the DC scans, else the component's own blocks
 __host__ __device__ __forceinline__ long long scan_slots(int h, int w, int sub, int s) {
   const int c = scan_def(s).comp;
-  const long long m = sub == 2 ? 16 : 8;
-  const long long mcus = ((h + m - 1) / m) * ((w + m - 1) / m);
-  if (c < 0) return mcus * (sub == 2 ? 6 : 3);
-  if (c > 0) return mcus;
+  const long long mh = mcu_h(sub), mw = mcu_w(sub);
+  const long long mcus = ((h + mh - 1) / mh) * ((w + mw - 1) / mw);
+  if (c < 0) return mcus * mcu_blocks(sub);
+  if (c > 0) return mcus;   // a chroma block per MCU
   return (long long)((h + 7) / 8) * ((w + 7) / 8);
 }
 
@@ -104,10 +103,12 @@ __device__ Stream stream_of(const JpegList& L, const ProgList& P, long long g, b
 // the MCU-order block (se_jpeg.cu's numbering within the image) of slot p of a scan of component c (-1: interleaved)
 __device__ __forceinline__ long long slot_block(const JImg& d, int sub, int c, long long p) {
   if (c < 0) return p;
+  const int per = mcu_blocks(sub);
   if (sub == 0) return p * 3 + c;
-  if (c > 0) return p * 6 + 3 + c;
+  if (c > 0) return p * per + per - 3 + c;
   const int bw = (d.w + 7) / 8;
   const long long bx = p % bw, by = p / bw;
+  if (sub == 1) return (by * d.mcu_x + (bx >> 1)) * 4 + (bx & 1);
   return ((by >> 1) * d.mcu_x + (bx >> 1)) * 6 + (by & 1) * 2 + (bx & 1);
 }
 
@@ -452,7 +453,7 @@ __global__ void __launch_bounds__(kThreads) jpeg_prog_header_kernel(const __grid
   __shared__ long long hdr_at[JPEG_SCANS + 1];
   const int i = blockIdx.x;
   if (threadIdx.x == 0) {
-    long long at = JPEG_SOF_END, slot = P.im[i].slot0, chunk = P.im[i].chunk0;
+    long long at = H.sof_end + H.meta, slot = P.im[i].slot0, chunk = P.im[i].chunk0;
     for (int s = 0; s < JPEG_SCANS; ++s) {
       Stream st;
       st.slot0 = slot;
@@ -476,7 +477,8 @@ __global__ void __launch_bounds__(kThreads) jpeg_prog_header_kernel(const __grid
   }
   __syncthreads();
   unsigned char* o = P.im[i].out;
-  for (int j = threadIdx.x; j < JPEG_SOF_END; j += kThreads) o[j] = j == kSofMarkerAt ? 0xC2 : header_byte(H, i, j);
+  for (int j = threadIdx.x; j < H.sof_end; j += kThreads)   // SOF0's marker byte becomes SOF2's
+    o[header_at(H, j)] = j == H.sof_end - 18 ? 0xC2 : header_byte(H, i, j);
   for (int s = 0; s < JPEG_SCANS; ++s) {
     const JpegTables& T = S.tabs[i * JPEG_SCANS + s];
     const int len = (int)(S.data_at[i * JPEG_SCANS + s] - hdr_at[s]);
@@ -486,10 +488,10 @@ __global__ void __launch_bounds__(kThreads) jpeg_prog_header_kernel(const __grid
 
 }  // namespace
 
-long long jpeg_prog_max_bytes(int h, int w, int subsampling) {
-  // the header through SOF2; scan 1's two DC tables (<= 12 symbols each) and SOS; scan 7's SOS; eight AC scans' table
+long long jpeg_prog_max_bytes(int h, int w, int subsampling, int sof_end) {
+  // the header through SOF2 (sof_end bytes); scan 1's two DC tables (<= 12 symbols each) and SOS; scan 7's SOS; eight AC scans' table
   // (<= 176 symbols: 160 run/size, ZRL and 15 EOB runs) and SOS; EOI
-  const long long headers = JPEG_SOF_END + 2 * (21 + 12) + 14 + 14 + 8 * (21 + 176 + 10) + 2;
+  const long long headers = sof_end + 2 * (21 + 12) + 14 + 14 + 8 * (21 + 176 + 10) + 2;
   long long bits = 0;
   for (int s = 0; s < JPEG_SCANS; ++s) bits += ((scan_slots(h, w, subsampling, s) * slot_max_bits(s) + 7) / 8) * 8;
   return headers + 2 * (bits / 8);   // each scan's bits padded to a byte, every byte possibly followed by 0x00

@@ -6,6 +6,7 @@ exposes the reference's call surface for the generator forward pass with CUDA te
 
 PyTorch is plumbing here (device memory + current stream); all compute is in libsketchedit_b200.so.
 """
+import array
 import ctypes
 import math
 import numbers
@@ -840,6 +841,111 @@ def jpeg_encode_u8(images, quality=75, subsampling=2, optimize=False, progressiv
     codec = _jpeg_codec(quality, subsampling, optimize, progressive)
     images = list(images)
     return _encode_list(codec, 3, images) if images else []
+
+
+# ITU T.81 Annex K.1 quantisation bases, natural order: libjpeg's tables at a quality are these scaled (jpeg_quality_tables)
+JPEG_LUMA_Q = (16, 11, 10, 16, 24, 40, 51, 61, 12, 12, 14, 19, 26, 58, 60, 55, 14, 13, 16, 24, 40, 57, 69, 56, 14, 17, 22, 29, 51,
+               87, 80, 62, 18, 22, 37, 56, 68, 109, 103, 77, 24, 35, 55, 64, 81, 104, 113, 92, 49, 64, 78, 87, 103, 121, 120, 101,
+               72, 92, 95, 98, 112, 100, 103, 99)
+JPEG_CHROMA_Q = (17, 18, 24, 47, 99, 99, 99, 99, 18, 21, 26, 66, 99, 99, 99, 99, 24, 26, 56, 99, 99, 99, 99, 99, 47, 66) + (99,) * 38
+JPEG_MAX_MARKER = 65533       # most bytes after an APP marker's length field: Pillow's bound on its EXIF block and ICC chunks
+JPEG_ICC_CHUNK = JPEG_MAX_MARKER - 14   # profile bytes per APP2 segment, after "ICC_PROFILE\0", its number and the count
+
+
+def jpeg_quality_tables(quality):
+    """The luma and chroma tables (natural order) libjpeg uses at ``quality`` in [1, 100] (jpeg_quality_scaling,
+    jpeg_add_quant_table with force_baseline): ``save(quality=q)`` is byte for byte ``save(qtables=jpeg_quality_tables(q))``."""
+    quality, _ = _check_jpeg_args(quality, 2)
+    scale = 5000 // quality if quality < 50 else 200 - 2 * quality
+    return [[min(255, max(1, (b * scale + 50) // 100)) for b in base] for base in (JPEG_LUMA_Q, JPEG_CHROMA_Q)]
+
+
+def jpeg_app_segments(exif=b"", icc_profile=None):
+    """The APP1 / APP2 segments Pillow 12.2 writes after APP0 for ``save(..., exif=exif, icc_profile=icc_profile)``, as
+    ``bytes``: ``exif`` (bytes or a ``PIL.Image.Exif``, at most 65533 bytes, else ValueError("EXIF data is too long")) as one
+    APP1 segment unless empty, then ``icc_profile`` (bytes or None) in chunks of 65519 bytes, each an APP2 segment
+    ``ICC_PROFILE\\0`` + its number from 1 + the chunk count + the chunk. At most 255 chunks (a profile under 16 MB)."""
+    from PIL import Image
+    if isinstance(exif, Image.Exif):
+        exif = exif.tobytes()
+    if not isinstance(exif, (bytes, bytearray)):
+        raise ValueError("exif must be bytes or a PIL.Image.Exif, got %r" % (type(exif).__name__,))
+    if icc_profile is not None and not isinstance(icc_profile, (bytes, bytearray)):
+        raise ValueError("icc_profile must be bytes or None, got %r" % (type(icc_profile).__name__,))
+    if len(exif) > JPEG_MAX_MARKER:
+        raise ValueError("EXIF data is too long")
+    out = bytearray()
+    if exif:
+        out += b"\xff\xe1" + (2 + len(exif)).to_bytes(2, "big") + exif
+    if icc_profile:
+        chunks = [icc_profile[i:i + JPEG_ICC_CHUNK] for i in range(0, len(icc_profile), JPEG_ICC_CHUNK)]
+        if len(chunks) > 255:
+            raise ValueError("icc_profile is too long: %d bytes make more than 255 APP2 segments" % len(icc_profile))
+        for i, c in enumerate(chunks, 1):
+            out += b"\xff\xe2" + (2 + 14 + len(c)).to_bytes(2, "big") + b"ICC_PROFILE\0" + bytes([i, len(chunks)]) + c
+    return bytes(out)
+
+
+def _check_qtables(qtables):
+    """Quantisation tables as a list of 1 to 4 lists of 64 ints in [0, 255], or ValueError. ``qtables`` is a dict (as
+    ``Image.quantization`` gives it: keys 0, 1, ... taken in order, as Pillow takes them) or a list / tuple of tables in
+    natural order. An entry above 255 would make Pillow write a 16-bit table and an extended-sequential (SOF1) file, which the
+    device encoder does not; such tables are refused."""
+    if isinstance(qtables, dict):
+        qtables = [qtables[k] for k in range(len(qtables)) if k in qtables]
+    if not isinstance(qtables, (list, tuple)) or not 1 <= len(qtables) <= 4:
+        raise ValueError("qtables must be 1 to 4 tables of 64 entries")
+    out = []
+    for t in qtables:
+        t = list(t) if isinstance(t, (list, tuple, np.ndarray, array.array)) else None
+        if t is None or len(t) != 64 or not all(_is_int(v) for v in t):
+            raise ValueError("qtables must be 1 to 4 tables of 64 integers")
+        if not all(0 <= v <= 255 for v in t):
+            raise ValueError("quantisation table entries must be in [0, 255]: larger ones need a 16-bit table (an "
+                             "extended-sequential file), which the encoder does not write")
+        out.append([int(v) for v in t])
+    return out
+
+
+def _check_tables_sampling(subsampling):
+    """Pillow's subsampling for the tables entry: -1 (libjpeg's default, 4:2:0), 0, 1 or 2, as the entry's 0, 1 or 2."""
+    if not _is_int(subsampling) or subsampling not in (-1, 0, 1, 2):
+        raise ValueError("subsampling must be -1, 0 (4:4:4), 1 (4:2:2) or 2 (4:2:0), got %r" % (subsampling,))
+    return 2 if subsampling == -1 else int(subsampling)
+
+
+def jpeg_tables_max_bytes(h, w, subsampling, ntables, progressive=False, segments_len=0):
+    """A true upper bound of the file ``jpeg_encode_tables_u8`` writes for an h x w image with ``ntables`` tables and
+    ``segments_len`` bytes of APP segments (``se_jpeg_tables_max_bytes``)."""
+    return _max_bytes(_lib.load().se_jpeg_tables_max_bytes, h, w, _check_tables_sampling(subsampling), ntables,
+                      int(bool(progressive)), segments_len)
+
+
+def jpeg_encode_tables_u8(images, qtables, subsampling, optimize=False, progressive=False, exif=b"", icc_profile=None):
+    """JPEG files of CUDA uint8 [h, w, 3] RGB images with the given quantisation tables, as ``bytes``: each is what
+
+        Image.fromarray(img).save(buf, "JPEG", qtables=qtables, subsampling=subsampling, optimize=optimize,
+                                  progressive=progressive, exif=exif, icc_profile=icc_profile)
+
+    writes (``se_jpeg_encode_tables_u8``), and so ``src.save(buf, "JPEG", quality="keep", ...)``'s file for
+    ``qtables=src.quantization`` and ``subsampling=JpegImagePlugin.get_sampling(src)`` of a JPEG ``src``. ``qtables``: 1 to
+    4 tables of 64 entries in [0, 255], natural order, as a list or as ``Image.quantization``'s dict (``_check_qtables``);
+    ``subsampling`` -1 (libjpeg's default, 4:2:0), 0 (4:4:4), 1 (4:2:2) or 2 (4:2:0); ``exif`` and ``icc_profile`` as in
+    ``jpeg_app_segments``. ``jpeg_quality_tables(q)`` gives the file of ``save(quality=q)``. Images, strides and device
+    memory are as in ``jpeg_encode_u8``, plus the segments in each ``out`` slot."""
+    qtables = _check_qtables(qtables)
+    sub = _check_tables_sampling(subsampling)
+    _check_jpeg_args(75, 2, optimize, progressive)
+    segments = jpeg_app_segments(exif, icc_profile)
+    images = list(images)
+    if not images:
+        return []
+    tabs = (ctypes.c_ushort * (64 * len(qtables)))(*[v for t in qtables for v in t])
+    seg = (ctypes.c_ubyte * len(segments)).from_buffer_copy(segments) if segments else None
+    codec = ("se_jpeg_encode_tables_u8", JPEG_MAX_BATCH,
+             (tabs, len(qtables), sub, int(bool(optimize)), int(bool(progressive)), seg, len(segments)),
+             lambda h, w: jpeg_tables_max_bytes(h, w, sub, len(qtables), progressive, len(segments)))
+    return _encode_list(codec, 3, images)
 
 
 def download_files(out, offsets, lengths):

@@ -1051,6 +1051,13 @@ class EditSession:
         self._history = deque()         # (boxes, previous bytes of each box, bytes held), oldest first
         self._held = 0
         self.history_bytes = int(history_bytes)
+        # what jpeg(quality="keep", exif=s.exif, icc_profile=s.icc_profile) keeps of the upload, read before the conversion
+        self._keep = None               # a JPEG upload's (quantisation tables, JpegImagePlugin.get_sampling)
+        if getattr(img, "format", None) == "JPEG" and getattr(img, "quantization", None):
+            from PIL import JpegImagePlugin
+            self._keep = (dict(img.quantization), JpegImagePlugin.get_sampling(img))
+        self._exif = img.info.get("exif", b"")
+        self._icc_profile = img.info.get("icc_profile")
         img = img.convert("RGB")
         self.size = img.size
         self._img = self._photo = None
@@ -1067,6 +1074,17 @@ class EditSession:
     def _check_open(self):
         if self._closed:
             raise RuntimeError("EditSession is closed")
+
+    @property
+    def exif(self):
+        """The upload's EXIF block (its ``info["exif"]``), or ``b""``: ``jpeg(exif=s.exif)`` carries it into the file. Its
+        contents are not rewritten, so an IFD1 thumbnail in it still shows the unedited photo."""
+        return self._exif
+
+    @property
+    def icc_profile(self):
+        """The upload's ICC profile (its ``info["icc_profile"]``), or None: ``jpeg(icc_profile=s.icc_profile)`` carries it."""
+        return self._icc_profile
 
     def close(self):
         """Releases the photo and the snapshots (idempotent); also run by ``DemoProcessor.close()``."""
@@ -1094,7 +1112,8 @@ class EditSession:
             with self._proc._torch.cuda.device(self._photo.device):
                 return Image.fromarray(self._pixels(None, size).cpu().numpy())
 
-    def jpeg(self, quality=75, subsampling=2, box=None, optimize=False, progressive=False, size=None):
+    def jpeg(self, quality=75, subsampling=2, box=None, optimize=False, progressive=False, size=None, exif=b"",
+             icc_profile=None):
         """The current photo, or its PIL box ``(left, upper, right, lower)``, as a JPEG file: the bytes of
 
             img = s.image().crop(box);  img.thumbnail(size)
@@ -1116,22 +1135,53 @@ class EditSession:
         file is downloaded; with ``resize='host'`` Pillow encodes it. quality, subsampling and the box's entries are Python or
         numpy integers, not bools. The device encode holds transient device memory sized for the worst-case file (about
         200 MB for a 4000x2667 photo at 4:2:0, 400 MB at 4:4:4, with or without optimize, and about 450 MB at 4:2:0 for a
-        progressive file; ``engine.jpeg_encode_u8``)."""
+        progressive file; ``engine.jpeg_encode_u8``).
+
+        ``quality="keep"`` keeps the format of a JPEG upload (the image given to ``open_session``): its quantisation tables
+        and subsampling, 4:2:2 included, as Pillow's ``upload.save(buf, "JPEG", quality="keep")`` does, so the blocks an edit
+        did not touch come out nearly as they went in; ``subsampling`` is then ignored, as Pillow ignores it. The file is
+
+            img.save(buf, "JPEG", qtables=upload.quantization, subsampling=JpegImagePlugin.get_sampling(upload), ...)
+
+        with the other arguments as above, and ValueError("Cannot use 'keep' when original image is not a JPEG") when the
+        upload is not a JPEG. ``exif`` (bytes or a ``PIL.Image.Exif``, at most 65533 bytes) and ``icc_profile`` (bytes or
+        None) are written as Pillow's ``save(exif=..., icc_profile=...)`` writes them, after APP0; ``s.exif`` and
+        ``s.icc_profile`` are the upload's, so ``s.jpeg(quality="keep", exif=s.exif, icc_profile=s.icc_profile)`` gives back
+        the photo as it was uploaded, edits included. An upload table with an entry above 255 (a 16-bit table; no 8-bit
+        baseline file has one) is refused with ValueError. On the device these calls run ``engine.jpeg_encode_tables_u8``,
+        a numeric quality with the tables of ``engine.jpeg_quality_tables``."""
         import io
 
         from . import engine
-        quality, subsampling = engine._check_jpeg_args(quality, subsampling, optimize, progressive)
+        keep = isinstance(quality, str) and quality == "keep"
+        if keep:
+            engine._check_jpeg_args(75, 2, optimize, progressive)
+        else:
+            quality, subsampling = engine._check_jpeg_args(quality, subsampling, optimize, progressive)
+        segments = engine.jpeg_app_segments(exif, icc_profile)
         size = self._size(size)
         with self._mu:
             self._check_open()
+            if keep and self._keep is None:
+                raise ValueError("Cannot use 'keep' when original image is not a JPEG")
+            qtables, sampling = self._keep if keep else (None, None)
+            if keep:
+                engine._check_qtables(qtables)
             box = self._box(box)
+            kw = dict(optimize=bool(optimize), progressive=bool(progressive))
             if self._img is not None:
                 img = self._host_image(box, size)
                 buf = io.BytesIO()
-                img.save(buf, "JPEG", quality=quality, subsampling=subsampling, optimize=bool(optimize),
-                         progressive=bool(progressive))
+                fmt = dict(qtables=qtables, subsampling=sampling) if keep else dict(quality=quality, subsampling=subsampling)
+                img.save(buf, "JPEG", exif=exif, icc_profile=icc_profile, **fmt, **kw)
                 return buf.getvalue()
-            return engine.jpeg_encode_u8([self._pixels(box, size)], quality, subsampling, optimize, progressive)[0]
+            pixels = self._pixels(box, size)
+            if keep:
+                return engine.jpeg_encode_tables_u8([pixels], qtables, sampling, exif=exif, icc_profile=icc_profile, **kw)[0]
+            if segments:
+                return engine.jpeg_encode_tables_u8([pixels], engine.jpeg_quality_tables(quality), subsampling, exif=exif,
+                                                    icc_profile=icc_profile, **kw)[0]
+            return engine.jpeg_encode_u8([pixels], quality, subsampling, optimize, progressive)[0]
 
     def png(self, box=None, size=None):
         """The current photo, or its PIL box ``(left, upper, right, lower)``, as a PNG file: the bytes of
