@@ -370,6 +370,17 @@ long long se_png_max_bytes(int h, int w, int channels);
 int se_png_decode_u8(const unsigned char* src, const long long* src_off, const long long* src_len, const int* info,
                      const long long* plte_off, int n, unsigned char* const* out, int* status_dev,
                      void* scratch, long long* scratch_bytes, void* stream);
+/* se_png_decode_u8 for large files: the same files, arguments, pixels and status rule, with each file's stream inflated by
+ * many warps at once instead of one. The stream is cut every chunk_bytes (>= 1) compressed bytes; each cut starts at the
+ * first dynamic-Huffman block header after it, and every chunk is decoded on its own. A file is decoded only if its chunks
+ * join end to start into exactly the file's raw size; otherwise (as for a stream with a false block start) its status is
+ * nonzero and it must go to Pillow. A stream with few dynamic blocks decodes correctly but with little parallelism. Each
+ * file's raw size, h (1 + ceil(w bits / 8)), is at most 2^31 - 1. scratch holds per file the raw filtered scanlines and 4
+ * bytes per raw byte of staging (about 32 + 128 MB for a 4000x2667 RGB file), plus 48 bytes per chunk (file i has
+ * src_len[i] / chunk_bytes + 1 chunks); the query works as in se_png_decode_u8. */
+int se_png_split_u8(const unsigned char* src, const long long* src_off, const long long* src_len, const int* info,
+                    const long long* plte_off, int n, unsigned char* const* out, int* status_dev, long long chunk_bytes,
+                    void* scratch, long long* scratch_bytes, void* stream);
 /* Bytes of coefficient tables the resize entries keep per device (process-wide; 0 restores the default of 256 MiB; negative is an
  * error). When a call's new tables would pass the limit, the device's cache is emptied (after a device synchronise) before the
  * call looks up any table; one call's own tables may exceed it. */

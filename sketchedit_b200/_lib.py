@@ -76,6 +76,8 @@ SIGNATURES = {
     "se_png_max_bytes": (ctypes.c_longlong, [_c_int, _c_int, _c_int]),
     "se_png_decode_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_void_p, _c_void_p,
                                   _c_void_p, ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
+    "se_png_split_u8": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_void_p, _c_void_p,
+                                 ctypes.c_longlong, _c_void_p, ctypes.POINTER(ctypes.c_longlong), _c_void_p]),
     "se_resize_coeffs": (_c_int, [_c_int, _c_int, _c_void_p, _c_void_p, ctypes.c_longlong]),
     "se_resize_set_table_cache_limit": (_c_int, [ctypes.c_longlong]),
     "se_resize_table_cache_bytes": (ctypes.c_longlong, []),

@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsketchedit_b200.so")
-SOURCES = ["se_engine.cu", "se_conv_c8.cu", "se_cam.cu", "se_conv_direct.cu", "se_misc.cu", "se_gemm_split.cu", "se_resize.cu", "se_jpeg.cu", "se_jpeg_opt.cu", "se_jpeg_prog.cu", "se_png.cu", "se_png_decode.cu", "se_detail.cu", "se_thumbnail.cu"]
+SOURCES = ["se_engine.cu", "se_conv_c8.cu", "se_cam.cu", "se_conv_direct.cu", "se_misc.cu", "se_gemm_split.cu", "se_resize.cu", "se_jpeg.cu", "se_jpeg_opt.cu", "se_jpeg_prog.cu", "se_png.cu", "se_png_decode.cu", "se_png_split.cu", "se_detail.cu", "se_thumbnail.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 

@@ -37,6 +37,8 @@ enum InflateStatus : int {
   // set by the PNG stages after inflation
   PNG_FILTER = 10,      // a row's filter type is not 0-4
   PNG_PALETTE = 11,     // a palette index at or past the palette's entries
+  // set by the split inflate (se_inflate_split.cuh)
+  INF_LINK = 12,        // a chunk ends elsewhere than where the next one starts, or the last one before the final block
 };
 
 constexpr int kTabBits = 10;   // first-level lookup: codes of at most 10 bits resolve in one shared-memory read
@@ -138,6 +140,16 @@ struct BitIn {
     cnt -= k;
     return v;
   }
+  SE_HD long long bit() const { return pos * 8 - cnt; }   // the offset of the next bit in the stream
+  // moves to bit b of the stream (b >= 0); false when b is past its end
+  SE_HD bool seek(long long b) {
+    pos = b >> 3;
+    buf = 0;
+    cnt = 0;
+    if (pos > n || !need((int)(b & 7))) return false;
+    take((int)(b & 7));
+    return true;
+  }
 };
 
 // One symbol of h; -INF_CODE or -INF_SHORT_INPUT on failure.
@@ -193,6 +205,144 @@ SE_HD inline unsigned adler32_lanes(const unsigned char* raw, long long n, int l
   return (unsigned)(b << 16 | a);
 }
 
+// Reads one block's header at in's position into *last and *type. A stored block leaves in byte-aligned at its LEN bytes of
+// data, LEN in *stored; a Huffman block leaves its tables in t. All lanes call it and get the same result.
+SE_HD inline int inflate_header(BitIn& in, InflateTabs& t, unsigned* last, unsigned* type, unsigned* stored, int lane, int nl) {
+  if (!in.need(3)) return INF_SHORT_INPUT;
+  *last = in.take(1);
+  *type = in.take(2);
+  if (*type == 0) {
+    in.take(in.cnt & 7);
+    if (!in.need(32)) return INF_SHORT_INPUT;
+    const unsigned len = in.take(16), nlen = in.take(16);
+    if (len != (~nlen & 0xFFFF)) return INF_BLOCK;
+    *stored = len;
+    return INF_OK;
+  }
+  if (*type == 3) return INF_BLOCK;
+  if (*type == 1) {
+    SE_LANE_SYNC();   // no lane still reads the previous block's lengths
+    for (int s = lane; s < 288 + 32; s += nl) t.lens[s] = (unsigned char)(s < 144 ? 8 : s < 256 ? 9 : s < 280 ? 7 : s < 288 ? 8 : 5);
+    SE_LANE_SYNC();
+    if (huff_build(t.lit, t.lens, 288, 1, lane, nl) || huff_build(t.dist, t.lens + 288, 32, 2, lane, nl)) return INF_TABLE;
+    return INF_OK;
+  }
+  if (!in.need(14)) return INF_SHORT_INPUT;
+  const int nlit = (int)in.take(5) + 257;
+  const int ndist = (int)in.take(5) + 1;
+  const int ncode = (int)in.take(4) + 4;
+  if (nlit > 286 || ndist > 30) return INF_TABLE;
+  const unsigned char order[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
+  unsigned char cl[19] = {0};
+  for (int k = 0; k < ncode; ++k) {
+    if (!in.need(3)) return INF_SHORT_INPUT;
+    cl[order[k]] = (unsigned char)in.take(3);
+  }
+  if (huff_build(t.lit, cl, 19, 0, lane, nl)) return INF_TABLE;
+  int k = 0;
+  while (k < nlit + ndist) {
+    const int s = huff_decode(t.lit, in);
+    if (s < 0) return -s;
+    if (s < 16) {
+      t.lens[k++] = (unsigned char)s;
+      continue;
+    }
+    int rep, v = 0;
+    if (s == 16) {
+      if (k == 0) return INF_TABLE;
+      if (!in.need(2)) return INF_SHORT_INPUT;
+      v = t.lens[k - 1];
+      rep = 3 + (int)in.take(2);
+    } else if (s == 17) {
+      if (!in.need(3)) return INF_SHORT_INPUT;
+      rep = 3 + (int)in.take(3);
+    } else {
+      if (!in.need(7)) return INF_SHORT_INPUT;
+      rep = 11 + (int)in.take(7);
+    }
+    if (k + rep > nlit + ndist) return INF_TABLE;
+    while (rep--) t.lens[k++] = (unsigned char)v;
+  }
+  if (t.lens[256] == 0) return INF_TABLE;
+  if (huff_build(t.lit, t.lens, nlit, 1, lane, nl) || huff_build(t.dist, t.lens + nlit, ndist, 2, lane, nl)) return INF_TABLE;
+  return INF_OK;
+}
+
+// One block at in's position, its bytes handed to `out`: out.stored(data, len) for a stored block, out.lit(byte) and
+// out.match(len, dist) for a Huffman block's symbols; each returns INF_OK or the status that ends the decode. *last is the
+// block's BFINAL. All lanes call it and get the same result.
+template <class Out>
+SE_HD inline int inflate_block(BitIn& in, InflateTabs& t, Out& out, unsigned* last, int lane, int nl) {
+  unsigned type = 0, stored = 0;
+  if (int st = inflate_header(in, t, last, &type, &stored, lane, nl)) return st;
+  if (type == 0) {
+    const long long at = in.pos - in.cnt / 8;   // the bit buffer holds whole bytes now: rewind it into the stream
+    if (at + stored > in.n) return INF_SHORT_INPUT;
+    if (int st = out.stored(in.p + at, stored)) return st;
+    in.pos = at + stored;
+    in.buf = 0;
+    in.cnt = 0;
+    return INF_OK;
+  }
+  for (;;) {
+    const int s = huff_decode(t.lit, in);
+    if (s < 0) return -s;
+    if (s < 256) {
+      if (int st = out.lit(s)) return st;
+      continue;
+    }
+    if (s == 256) return INF_OK;
+    const int lc = s - 257;
+    if (lc >= 29) return INF_CODE;
+    const int lx = len_extra(lc);
+    if (!in.need(lx)) return INF_SHORT_INPUT;
+    const long long len = len_base(lc) + in.take(lx);
+    const int dc = huff_decode(t.dist, in);
+    if (dc < 0) return -dc;
+    if (dc >= 30) return INF_CODE;
+    const int dx = dist_extra(dc);
+    if (!in.need(dx)) return INF_SHORT_INPUT;
+    const long long d = dist_base(dc) + in.take(dx);
+    if (int st = out.match(len, d)) return st;
+  }
+}
+
+// inflate_block's output into raw[0, raw_n), out bytes written so far; lane 0 writes the literals, all lanes the copies.
+struct ByteOut {
+  unsigned char* raw;
+  long long raw_n, out;
+  int lane, nl;
+  SE_HD int stored(const unsigned char* data, unsigned len) {
+    if (out + len > raw_n) return INF_LONG_OUTPUT;
+    SE_LANE_SYNC();
+    for (unsigned k = lane; k < len; k += nl) raw[out + k] = data[k];
+    SE_LANE_SYNC();
+    out += len;
+    return INF_OK;
+  }
+  SE_HD int lit(int s) {
+    if (out >= raw_n) return INF_LONG_OUTPUT;
+    if (lane == 0) raw[out] = (unsigned char)s;
+    ++out;
+    return INF_OK;
+  }
+  SE_HD int match(long long len, long long d) {
+    if (d > out) return INF_DISTANCE;
+    if (out + len > raw_n) return INF_LONG_OUTPUT;
+    SE_LANE_SYNC();   // the literals lane 0 just wrote are visible to every lane
+    // byte k of the match is byte k mod d of the d bytes before it: no lane reads a byte this copy writes
+    for (long long k = lane; k < len; k += nl) raw[out + k] = raw[out - d + (k < d ? k : k % d)];
+    SE_LANE_SYNC();
+    out += len;
+    return INF_OK;
+  }
+};
+
+// The zlib header's check (RFC 1950): 0 when CMF, FLG name deflate with a window of at most 32 KB, no preset dictionary.
+SE_HD inline int zlib_header(unsigned cmf, unsigned flg) {
+  return (cmf & 15) != 8 || (cmf >> 4) > 7 || (cmf * 256 + flg) % 31 != 0 || (flg & 0x20) ? INF_HEADER : INF_OK;
+}
+
 // Inflates the zlib stream src[0, n) into raw[0, raw_n). Returns INF_OK only when the stream is a complete zlib stream
 // whose last block ends at exactly raw_n bytes and whose Adler-32 matches; bytes after the Adler-32 are ignored.
 // `t` is scratch for the tables (shared memory on the device); all lanes of the group call it and get the same result.
@@ -201,108 +351,12 @@ SE_HD inline int inflate_zlib(const unsigned char* src, long long n, unsigned ch
   BitIn in{src, 0, n, 0ull, 0};
   if (!in.need(16)) return INF_SHORT_INPUT;
   const unsigned cmf = in.take(8), flg = in.take(8);
-  if ((cmf & 15) != 8 || (cmf >> 4) > 7 || (cmf * 256 + flg) % 31 != 0 || (flg & 0x20)) return INF_HEADER;
-  long long out = 0;
-  for (;;) {
-    if (!in.need(3)) return INF_SHORT_INPUT;
-    const unsigned last = in.take(1), type = in.take(2);
-    if (type == 0) {
-      in.take(in.cnt & 7);
-      if (!in.need(32)) return INF_SHORT_INPUT;
-      const unsigned len = in.take(16), nlen = in.take(16);
-      if (len != (~nlen & 0xFFFF)) return INF_BLOCK;
-      const long long at = in.pos - in.cnt / 8;   // the bit buffer holds whole bytes now: rewind it into the stream
-      if (at + len > n) return INF_SHORT_INPUT;
-      if (out + len > raw_n) return INF_LONG_OUTPUT;
-      SE_LANE_SYNC();
-      for (unsigned k = lane; k < len; k += nl) raw[out + k] = src[at + k];
-      SE_LANE_SYNC();
-      out += len;
-      in.pos = at + len;
-      in.buf = 0;
-      in.cnt = 0;
-    } else if (type == 3) {
-      return INF_BLOCK;
-    } else {
-      if (type == 1) {
-        SE_LANE_SYNC();   // no lane still reads the previous block's lengths
-        for (int s = lane; s < 288 + 32; s += nl) t.lens[s] = (unsigned char)(s < 144 ? 8 : s < 256 ? 9 : s < 280 ? 7 : s < 288 ? 8 : 5);
-        SE_LANE_SYNC();
-        if (huff_build(t.lit, t.lens, 288, 1, lane, nl) || huff_build(t.dist, t.lens + 288, 32, 2, lane, nl)) return INF_TABLE;
-      } else {
-        if (!in.need(14)) return INF_SHORT_INPUT;
-        const int nlit = (int)in.take(5) + 257;
-        const int ndist = (int)in.take(5) + 1;
-        const int ncode = (int)in.take(4) + 4;
-        if (nlit > 286 || ndist > 30) return INF_TABLE;
-        const unsigned char order[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
-        unsigned char cl[19] = {0};
-        for (int k = 0; k < ncode; ++k) {
-          if (!in.need(3)) return INF_SHORT_INPUT;
-          cl[order[k]] = (unsigned char)in.take(3);
-        }
-        if (huff_build(t.lit, cl, 19, 0, lane, nl)) return INF_TABLE;
-        int k = 0;
-        while (k < nlit + ndist) {
-          const int s = huff_decode(t.lit, in);
-          if (s < 0) return -s;
-          if (s < 16) {
-            t.lens[k++] = (unsigned char)s;
-            continue;
-          }
-          int rep, v = 0;
-          if (s == 16) {
-            if (k == 0) return INF_TABLE;
-            if (!in.need(2)) return INF_SHORT_INPUT;
-            v = t.lens[k - 1];
-            rep = 3 + (int)in.take(2);
-          } else if (s == 17) {
-            if (!in.need(3)) return INF_SHORT_INPUT;
-            rep = 3 + (int)in.take(3);
-          } else {
-            if (!in.need(7)) return INF_SHORT_INPUT;
-            rep = 11 + (int)in.take(7);
-          }
-          if (k + rep > nlit + ndist) return INF_TABLE;
-          while (rep--) t.lens[k++] = (unsigned char)v;
-        }
-        if (t.lens[256] == 0) return INF_TABLE;
-        if (huff_build(t.lit, t.lens, nlit, 1, lane, nl) || huff_build(t.dist, t.lens + nlit, ndist, 2, lane, nl)) return INF_TABLE;
-      }
-      for (;;) {
-        const int s = huff_decode(t.lit, in);
-        if (s < 0) return -s;
-        if (s < 256) {
-          if (out >= raw_n) return INF_LONG_OUTPUT;
-          if (lane == 0) raw[out] = (unsigned char)s;
-          ++out;
-          continue;
-        }
-        if (s == 256) break;
-        const int lc = s - 257;
-        if (lc >= 29) return INF_CODE;
-        const int lx = len_extra(lc);
-        if (!in.need(lx)) return INF_SHORT_INPUT;
-        const long long len = len_base(lc) + in.take(lx);
-        const int dc = huff_decode(t.dist, in);
-        if (dc < 0) return -dc;
-        if (dc >= 30) return INF_CODE;
-        const int dx = dist_extra(dc);
-        if (!in.need(dx)) return INF_SHORT_INPUT;
-        const long long d = dist_base(dc) + in.take(dx);
-        if (d > out) return INF_DISTANCE;
-        if (out + len > raw_n) return INF_LONG_OUTPUT;
-        SE_LANE_SYNC();   // the literals lane 0 just wrote are visible to every lane
-        // byte k of the match is byte k mod d of the d bytes before it: no lane reads a byte this copy writes
-        for (long long k = lane; k < len; k += nl) raw[out + k] = raw[out - d + (k < d ? k : k % d)];
-        SE_LANE_SYNC();
-        out += len;
-      }
-    }
-    if (last) break;
-  }
+  if (zlib_header(cmf, flg)) return INF_HEADER;
+  ByteOut out{raw, raw_n, 0, lane, nl};
+  for (unsigned last = 0; !last;)
+    if (int st = inflate_block(in, t, out, &last, lane, nl)) return st;
   SE_LANE_SYNC();
-  if (out != raw_n) return INF_SHORT_OUTPUT;
+  if (out.out != raw_n) return INF_SHORT_OUTPUT;
   in.take(in.cnt & 7);
   if (!in.need(32)) return INF_SHORT_INPUT;
   unsigned want = 0;

@@ -405,13 +405,16 @@ def _run_chunks(n, per_call, device, chunk):
     """Calls a scratch-taking C entry over n images, per_call images per call, on the current stream of ``device``.
     ``chunk(sl)`` returns for the images of slice sl a function f(scratch, scratch_bytes, stream) that makes the call;
     f(None, ...) is its scratch query. One scratch allocation, the largest query, serves every call."""
+    _run_calls([chunk(slice(c0, c0 + per_call)) for c0 in range(0, n, per_call)], device)
+
+
+def _run_calls(calls, device):
+    """``_run_chunks`` over the call functions ``calls``, in order."""
     with torch.cuda.device(device):
-        calls, need = [], 0
-        for c0 in range(0, n, per_call):
-            f = chunk(slice(c0, c0 + per_call))
+        need = 0
+        for f in calls:
             size = ctypes.c_longlong(0)
             _lib.check(f(None, ctypes.byref(size), None))
-            calls.append(f)
             need = max(need, size.value)
         scratch = torch.empty(max(need, 1), device=device, dtype=torch.uint8)
         for f in calls:
@@ -1013,6 +1016,22 @@ def png_encode_u8(images, swap_rb=False):
 
 
 PNG_DECODE_MAX_BATCH = 256   # files per se_png_decode_u8 call; the wrappers split longer lists into calls of this size
+# Files of at least this many raw bytes (filtered scanlines, h (1 + row bytes)) go to se_png_split_u8, one file per call,
+# the rest to se_png_decode_u8's one warp per file. tools/png_split_bench.py measured the crossover (DESIGN.md 7b).
+PNG_SPLIT_MIN_RAW = 4 << 20
+PNG_SPLIT_MIN_CHUNK = 16 << 10   # compressed bytes per chunk of the split decoder: about one of zlib's default blocks
+PNG_SPLIT_MAX_CHUNKS = 4096      # chunks per file; longer streams get longer chunks
+
+
+def png_split_chunk_bytes(stream_bytes):
+    """The chunk spacing of se_png_split_u8 for a zlib stream of ``stream_bytes`` bytes."""
+    return max(PNG_SPLIT_MIN_CHUNK, -(-int(stream_bytes) // PNG_SPLIT_MAX_CHUNKS))
+
+
+def png_raw_bytes(hd):
+    """The raw filtered scanlines of the ``pngfile.PngHead`` hd: h (1 + row bytes)."""
+    ch = {0: 1, 2: 3, 3: 1, 4: 2, 6: 4}[hd.ctype]
+    return hd.h * (1 + (hd.w * ch * hd.depth + 7) // 8)
 
 
 def png_stage(heads):
@@ -1029,7 +1048,11 @@ def png_decode_u8_packed(src, src_offsets, src_lengths, heads, modes, out=None, 
     ``modes`` for all) is "RGB" or "L". ``out`` (optional) is one contiguous CUDA uint8 tensor or a list of them with one
     per file; file i's h x w x 3 or h x w bytes go to ``out_offsets[i]`` of its tensor. Returns ``(out, out_offsets,
     status)``: ``status`` is a CUDA int32 tensor, 0 where the pixels are ``np.asarray(Image.open(f).convert(mode))`` and
-    nonzero where the file must go to Pillow. Only enqueues work on the current stream."""
+    nonzero where the file must go to Pillow. Only enqueues work on the current stream.
+
+    A file of ``PNG_SPLIT_MIN_RAW`` raw bytes or more is decoded by ``se_png_split_u8`` across the whole GPU, with chunks of
+    ``png_split_chunk_bytes`` of its stream; the others by one warp each. The split decoder's scratch is the file's raw
+    scanlines plus 4 bytes per raw byte (about 160 MB for a 4000x2667 RGB file), held while the call runs."""
     n = len(heads)
     modes = [modes] * n if isinstance(modes, str) else list(modes)
     if len(modes) != n or len(src_offsets) != n or len(src_lengths) != n:
@@ -1064,13 +1087,25 @@ def png_decode_u8_packed(src, src_offsets, src_lengths, heads, modes, out=None, 
     dst = [t.data_ptr() + o for t, o in zip(outs, out_offsets)]
     lib = _lib.load()
 
-    def chunk(sl):
+    def call(sl, split):
         k = len(info[sl])
         a = (_ptr(src), _longs(src_offsets[sl]), _longs(src_lengths[sl]), _ints(info[sl]), _longs(plte_offs[sl]), k,
              (ctypes.c_void_p * k)(*dst[sl]), ctypes.c_void_p(status.data_ptr() + 4 * sl.start))
+        if split:
+            S = png_split_chunk_bytes(src_lengths[sl.start])
+            return lambda scratch, size, stream: lib.se_png_split_u8(*a, S, scratch, size, stream)
         return lambda scratch, size, stream: lib.se_png_decode_u8(*a, scratch, size, stream)
 
-    _run_chunks(n, PNG_DECODE_MAX_BATCH, dev, chunk)
+    # runs of consecutive files of one decoder: one split file per call, up to PNG_DECODE_MAX_BATCH one-warp files
+    split = [png_raw_bytes(hd) >= PNG_SPLIT_MIN_RAW for hd in heads]
+    calls, k = [], 0
+    while k < n:
+        j = k + 1
+        while j < n and not split[k] and not split[j] and j - k < PNG_DECODE_MAX_BATCH:
+            j += 1
+        calls.append(call(slice(k, j), split[k]))
+        k = j
+    _run_calls(calls, dev)
     return out, out_offsets, status
 
 

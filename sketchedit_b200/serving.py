@@ -415,7 +415,14 @@ class DemoProcessor:
 
     def open_session(self, img, history_bytes=256 << 20):
         """An ``EditSession`` on ``img`` (converted to RGB): with ``resize='device'`` the photo is uploaded once to the engine's
-        device and stays there until ``close()``. ``history_bytes`` bounds the bytes its undo snapshots hold."""
+        device and stays there until ``close()``. ``history_bytes`` bounds the bytes its undo snapshots hold.
+
+        ``img`` is a PIL image or the upload's bytes (``bytes``, ``bytearray`` or ``memoryview``); the session on bytes is
+        the session on ``Image.open(io.BytesIO(img))``, Pillow's exception included for a file it cannot open. With
+        ``resize='device'`` a PNG that ``pngfile.parse`` accepts and that has at least ``engine.PNG_SPLIT_MIN_RAW`` bytes of
+        scanlines (about 1200x1200 RGB and up) is decoded across the whole GPU straight into the session's photo
+        (``engine.png_decode_into``: only the compressed stream is uploaded, no full-size host array); JPEG, smaller PNG
+        files (where Pillow is faster) and every other file go through Pillow."""
         sess = EditSession(self, img, history_bytes)
         with self._sessions_mu:
             closed = self._closed
@@ -1053,27 +1060,61 @@ class EditSession:
         self.history_bytes = int(history_bytes)
         # what jpeg(quality="keep", exif=s.exif, icc_profile=s.icc_profile) keeps of the upload, read before the conversion
         self._keep = None               # a JPEG upload's (quantisation tables, JpegImagePlugin.get_sampling)
-        if getattr(img, "format", None) == "JPEG" and getattr(img, "quantization", None):
-            from PIL import JpegImagePlugin
-            self._keep = (dict(img.quantization), JpegImagePlugin.get_sampling(img))
-        self._exif = img.info.get("exif", b"")
-        self._icc_profile = img.info.get("icc_profile")
-        img = img.convert("RGB")
-        self.size = img.size
+        self._exif, self._icc_profile = b"", None
         self._img = self._photo = None
         self._proposals = set()         # open proposals, computed on the current photo
-        if proc.resize == "host":
-            self._img = img
+        head = None
+        if isinstance(img, (bytes, bytearray, memoryview)):   # the upload's bytes: Image.open(io.BytesIO(img)) below
+            img = bytes(img)
+            if proc.resize == "device":
+                from . import engine, pngfile
+                try:
+                    head = pngfile.parse(img)
+                except pngfile.Host:
+                    pass
+                if head is not None and engine.png_raw_bytes(head) < engine.PNG_SPLIT_MIN_RAW:
+                    head = None   # below the split decoder's size Pillow is faster (DESIGN.md 7b)
+            if head is None:
+                import io
+
+                from PIL import Image
+                img = Image.open(io.BytesIO(img))
+        if head is not None:   # a PNG the device decodes; it has no EXIF or ICC chunk (pngfile sends those to Pillow)
+            self.size = (head.w, head.h)
+            self._photo = self._decode_png(img, head)
         else:
-            torch = proc._torch
-            w, h = img.size
-            self._photo = torch.empty(h, w, 3, device=proc.engine.device, dtype=torch.uint8)
-            self._photo.copy_(torch.from_numpy(np.array(img)))
+            if getattr(img, "format", None) == "JPEG" and getattr(img, "quantization", None):
+                from PIL import JpegImagePlugin
+                self._keep = (dict(img.quantization), JpegImagePlugin.get_sampling(img))
+            self._exif = img.info.get("exif", b"")
+            self._icc_profile = img.info.get("icc_profile")
+            img = img.convert("RGB")
+            self.size = img.size
+            if proc.resize == "host":
+                self._img = img
+            else:
+                torch = proc._torch
+                w, h = img.size
+                self._photo = torch.empty(h, w, 3, device=proc.engine.device, dtype=torch.uint8)
+                self._photo.copy_(torch.from_numpy(np.array(img)))
         self._closed = False
 
     def _check_open(self):
         if self._closed:
             raise RuntimeError("EditSession is closed")
+
+    def _decode_png(self, data, head):
+        """The photo of the PNG upload ``data`` (``pngfile.parse`` gave ``head``) in a new tensor on the engine's device:
+        its stream staged in pinned memory and decoded there (``engine.png_decode_into``), no full-size host array; the host
+        reads the status once, and a file the device refuses is decoded by Pillow (its exception included) into the tensor."""
+        from . import engine
+        torch = self._proc._torch
+        dev = self._proc.engine.device
+        with torch.cuda.device(dev):
+            photo = torch.empty(head.h, head.w, 3, device=dev, dtype=torch.uint8)
+            engine.png_decode_into(engine.png_stage([head]), [head], ["RGB"], [data], [(photo.view(-1), 0, (head.h, head.w))],
+                                   ["the upload"], dev)
+        return photo
 
     @property
     def exif(self):
